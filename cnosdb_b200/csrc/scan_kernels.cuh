@@ -1652,13 +1652,24 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           const uint32_t kb = (kword >> off) & smask;                   // rows the row filter keeps
           n_points += __popc(m);
           if (seg_in) n_inrange += __popc(kb);
-          if (!SEL) {  // one loop for dense and sparse bitmaps: a warp holds pages of both kinds
-            if (accumulate) va.count += __popc(m & kb);
+          if (!SEL) {
+            const uint32_t take = accumulate ? (m & kb) : 0u;  // rows whose value is accumulated
+            va.count += __popc(take);
+            // Dense spans (every row holds a value and is kept: every span of a page without nulls when the query has no
+            // field predicates - C4 generates 5 % nulls on 1 % of its pages, bench.py) decode popc(m) values with no test
+            // per row. The lanes choose together: a lane on the other loop would run it after them. (Both loops give the
+            // same result, so which lanes the vote sees only decides the speed.)
+            if (__all_sync(__activemask(), take == m)) {
 #pragma unroll 1
-            for (uint32_t j = 0; j < span; j++) {
-              if ((m >> j) & 1) {
+              for (uint32_t n = __popc(m); n; n--) {
                 const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
-                if (accumulate && ((kb >> j) & 1)) va.add(v, pt, flip);
+                va.add(v, pt, flip);
+              }
+            } else {  // only the rows holding a value
+#pragma unroll 1
+              for (uint32_t b = m; b; b &= b - 1) {
+                const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
+                if (take & b & (0u - b)) va.add(v, pt, flip);
               }
             }
           } else {  // FIRST / LAST wanted: the run's first and last KEPT rows keep (ts, value, valid)
