@@ -1287,6 +1287,24 @@ __device__ __forceinline__ void reduce_staged(const ScanParams &P, uint64_t *sta
   __syncwarp();
 }
 
+// Every lane parks its partial (identities unless `live`) in staging slot `seq`, the lane `meta_lane` records the slot's
+// (query column << 32) | cell, and every FLUSH_SLOTS slots the warp reduces them. Called by all 32 lanes.
+template <int VK>
+__device__ __forceinline__ void stage_partial(const ScanParams &P, uint64_t *stab, uint64_t *stage, uint32_t &seq, bool live,
+                                              const ValueAcc<VK> &va, bool meta_lane, uint64_t gcell) {
+  uint64_t *q = stage + (size_t)seq * FLUSH_Q * 32 + (threadIdx.x & 31);
+  q[0] = live ? va.count : 0;
+  q[32] = live ? va.sum : 0;  // 0 bits == +0.0
+  if (VK != VK_GOR) q[64] = live ? (uint64_t)va.sum_hi : 0;
+  q[96] = live ? (uint64_t)va.kmin : (uint64_t)INT64_MAX;
+  q[128] = live ? (uint64_t)va.kmax : (uint64_t)INT64_MIN;
+  if (meta_lane) stage[FLUSH_SLOTS * FLUSH_Q * 32 + seq] = gcell;
+  if (++seq == FLUSH_SLOTS) {
+    reduce_staged<VK>(P, stab, stage, seq);
+    seq = 0;
+  }
+}
+
 // Flush of one finished run per flushing lane (no FIRST/LAST). `seq` = staged slots in use (warp-uniform).
 template <int VK>
 __device__ __forceinline__ void flush_runs(const ScanParams &P, uint64_t *stab, uint64_t *stage, uint32_t &seq, bool active,
@@ -1302,18 +1320,7 @@ __device__ __forceinline__ void flush_runs(const ScanParams &P, uint64_t *stab, 
   // atomic per quantity instead of 32 contended ones.
   const bool same = !P.group_by_series && __all_sync(FULL, !active || gcell == lcell);
   if (same) {
-    uint64_t *q = stage + (size_t)seq * FLUSH_Q * 32 + lane;
-    const bool live = active && va.count;
-    q[0] = live ? va.count : 0;
-    q[32] = live ? va.sum : 0;  // 0 bits == +0.0
-    if (VK != VK_GOR) q[64] = live ? (uint64_t)va.sum_hi : 0;
-    q[96] = live ? (uint64_t)va.kmin : (uint64_t)INT64_MAX;
-    q[128] = live ? (uint64_t)va.kmax : (uint64_t)INT64_MIN;
-    if ((int)lane == leader) stage[FLUSH_SLOTS * FLUSH_Q * 32 + seq] = lcell;
-    if (++seq == FLUSH_SLOTS) {
-      reduce_staged<VK>(P, stab, stage, seq);
-      seq = 0;
-    }
+    stage_partial<VK>(P, stab, stage, seq, active && va.count, va, (int)lane == leader, lcell);
   } else if (active && va.count) {  // lanes on different cells (GROUP BY series, unaligned pages): one update each
     table_update(P, stab, P.cols[qcol], cell, mask, VK == VK_GOR || (VK == VK_GEN && pt == TSKV_PT_F64), va.count, va.sum,
                  va.sum_hi, va.kmin, va.kmax);
@@ -1536,6 +1543,104 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
       }
     }
     fast = __all_sync(FULL, elig);
+  }
+
+  // ---- Uniform schedule (RLE timestamps, GROUP BY bucket, no FIRST / LAST). When every lane that holds rows starts at
+  // the same row and time, steps by the same delta, has the same range rows [ra, rb1), the same bucket state and the same
+  // query column (TSBS-aligned pages: 80 % of C4's), the bucket edges fall on the same rows in every lane. The warp then
+  // walks ONE schedule, the leader's: per bitmap word one dense / sparse vote, per bucket its rows and one staged store
+  // per lane - no per-lane segment state, no alignment reduction, no ballot / same-cell vote, since all lanes close the
+  // same cell. The staged partials and their order are the ones the segment loop below makes for such a warp. Lanes
+  // without rows walk along idle; a lane whose values run out stops decoding as there. (Not for the generic value
+  // codecs: their larger cursor leaves no registers for a second loop.)
+  if (TK == TK_RLE && VK != VK_GEN && !SEL && fast && P.width > 0 && !P.group_by_series) {
+    const bool mine = row < n_rows;
+    const uint32_t with_rows = __ballot_sync(FULL, mine);
+    const int src = with_rows ? __ffs(with_rows) - 1 : 0;
+    const uint64_t t_first = rle_t0 + (uint64_t)row * rle_delta;
+    // (`&`, not `&&`: every lane must reach every shuffle)
+    const bool agree = (shfl_u64(rle_delta, src) == rle_delta) & (shfl_u64(t_first, src) == t_first) &
+                       (shfl_u64(e_off, src) == e_off) & (__shfl_sync(FULL, row, src) == row) &
+                       (__shfl_sync(FULL, n_rows, src) == n_rows) & (__shfl_sync(FULL, ra, src) == ra) &
+                       (__shfl_sync(FULL, rb1, src) == rb1) & (__shfl_sync(FULL, bidx, src) == bidx) &
+                       (__shfl_sync(FULL, nb, src) == nb) & (__shfl_sync(FULL, qcol, src) == qcol);
+    if (with_rows && __all_sync(FULL, !mine || agree)) {
+      // the leader's schedule in every lane (lanes without rows may hold other values)
+      rle_delta = shfl_u64(rle_delta, src);
+      e_off = shfl_u64(e_off, src);
+      w_rem = shfl_u64(w_rem, src);
+      q32 = __shfl_sync(FULL, q32, src);
+      row = __shfl_sync(FULL, row, src);
+      ra = __shfl_sync(FULL, ra, src);
+      rb1 = __shfl_sync(FULL, rb1, src);
+      bidx = __shfl_sync(FULL, bidx, src);
+      nb = __shfl_sync(FULL, nb, src);
+      const uint64_t col = (uint64_t)__shfl_sync(FULL, qcol, src) << 32;
+      uint32_t end = __shfl_sync(FULL, n_rows, src);
+      while (row < end) {  // one bitmap word per pass (`row` is a multiple of 32 here)
+        if (n_rows) {      // this lane still decodes: take the prefetched word, prefetch the next
+          vword = vahead;
+          vahead = __ldg(vbm + (row >> 5) + 1);  // reads at most 8 bytes past the bitmap (inside the page)
+          if (keepw) kword = __ldg(keepw + (row >> 5));
+        }
+        const uint32_t wend = min(row + 32, end);
+        const uint32_t m = (n_rows && !allnull) ? vword & (0xffffffffu >> (32 - (wend - row))) : 0u;  // rows holding a value
+        const uint32_t lo = min(max(ra, row), wend) - row, hi = max(min(max(rb1, row), wend) - row, lo);
+        const uint32_t take = m & kword & (uint32_t)((1ull << hi) - (1ull << lo));  // rows whose value is accumulated
+        // Dense words (every row holding a value is kept, on all lanes) decode popc values with no test per row.
+        // The vote only chooses the speed: both loops give the same result.
+        const bool dense = __all_sync(FULL, take == m);
+        uint32_t r = row;
+        while (r < wend) {  // the word's pieces: rows before the range, one per bucket, rows after it
+          const bool in = r >= ra && r < rb1;
+          uint32_t pend = r < ra ? min(ra, wend) : wend;
+          if (in) {
+            if (nb == 0) {  // next bucket (one narrower than the step may hold no row at all)
+              do {
+                bidx++;
+                nb = q32 + (e_off < w_rem ? 1u : 0u);
+                e_off = e_off + (uint64_t)nb * rle_delta - (uint64_t)P.width;
+              } while (nb == 0);
+              if (bidx >= P.n_buckets) {
+                if (n_rows) { report_error(P, TSKV_ERR_BUCKET_RANGE, page); n_rows = r; }
+                end = r;
+                break;
+              }
+            }
+            const uint32_t lim = min(rb1, wend);
+            pend = nb < lim - r ? r + nb : lim;
+            nb -= pend - r;
+          }
+          const uint32_t pmask = (uint32_t)((1ull << (pend - row)) - (1ull << (r - row)));
+          const uint32_t mp = n_rows ? m & pmask : 0u, tp = take & mp;
+          n_points += __popc(mp);
+          if (in && n_rows) n_inrange += __popc(kword & pmask);
+          va.count += __popc(tp);
+          if (dense) {
+#pragma unroll 1
+            for (uint32_t n = __popc(mp); n; n--) {
+              const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
+              va.add(v, pt, flip);
+            }
+          } else {  // only the rows holding a value
+#pragma unroll 1
+            for (uint32_t b = mp; b; b &= b - 1) {
+              const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
+              if (tp & b & (0u - b)) va.add(v, pt, flip);
+            }
+          }
+          r = pend;
+          if (n_rows) check_values();
+          if (in && (nb == 0 || r == rb1)) {  // the bucket's last row: its partial goes to the staging area
+            va.fold(pt);
+            stage_partial<VK>(P, stab, stage, staged, n_rows && va.count, va, lane == 0, col | bidx);
+            va.reset();
+          }
+        }
+        row = r;
+      }
+      row = n_rows;  // nothing is left for the segment loop below
+    }
   }
 
   // The warp walks its 32 pages SEGMENT by segment (a segment = rows of one page sharing (selected, bucket)), and for
