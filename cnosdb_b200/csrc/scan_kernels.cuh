@@ -928,9 +928,14 @@ __device__ __forceinline__ bool locate_bucket(const ScanParams &P, int64_t t, Bu
     return true;
   }
   const int64_t w = P.width;
-  if (b.valid && b.floor_regime && t > b.hi && (uint64_t)t - (uint64_t)b.hi <= (uint64_t)w &&
-      b.idx + 1 < P.n_buckets) {
-    b.lo = b.hi + 1; b.hi = b.hi + w; b.idx += 1;  // next bucket of the floor-aligned regime
+  // the last t whose dividend t - origin_mod + w does not wrap: floor-regime buckets end there, rows past it belong to
+  // the reference's wrapped windows
+  const int64_t cap = (int64_t)((uint64_t)INT64_MAX - ((uint64_t)w - (uint64_t)P.origin_mod));
+  if (b.valid && b.floor_regime && t > b.hi && (uint64_t)t - (uint64_t)b.hi <= (uint64_t)w && t <= cap &&
+      b.idx + 1 < P.n_buckets) {  // next bucket of the floor-aligned regime
+    b.lo = b.hi + 1;
+    b.hi = (int64_t)((uint64_t)b.hi + ((uint64_t)cap - (uint64_t)b.hi < (uint64_t)w ? (uint64_t)cap - (uint64_t)b.hi : (uint64_t)w));
+    b.idx += 1;
     return true;
   }
   int64_t dividend = (int64_t)((uint64_t)t - (uint64_t)P.origin_mod + (uint64_t)w);
@@ -939,8 +944,13 @@ __device__ __forceinline__ bool locate_bucket(const ScanParams &P, int64_t t, Bu
   int64_t diff = (int64_t)((uint64_t)start - (uint64_t)P.first_bucket_start);
   if (diff < 0 || diff % w != 0 || diff / w >= (int64_t)P.n_buckets) return false;
   b.idx = (uint32_t)(diff / w);
-  if (dividend >= 0) { b.lo = start; b.hi = start + (w - 1); }
-  else { b.lo = start - w + 1; b.hi = start; }
+  if (dividend >= 0) {  // [start, start + w), cut at cap (start <= t <= cap)
+    const uint64_t room = (uint64_t)cap - (uint64_t)start;
+    b.lo = start;
+    b.hi = (int64_t)((uint64_t)start + (room < (uint64_t)(w - 1) ? room : (uint64_t)(w - 1)));
+  } else {
+    b.lo = start - w + 1; b.hi = start;
+  }
   b.floor_regime = dividend >= 0;
   b.valid = true;
   return true;
@@ -1513,7 +1523,8 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
       // (the parts of a page may take different paths: both give the same result)
       const uint64_t span_t = (uint64_t)(page_rows - 1) * rle_delta;
       elig = (int64_t)rle_delta > 0 && __umul64hi((uint64_t)(page_rows - 1), rle_delta) == 0 && span_t < (1ull << 62) &&
-             rle_t0 + (1ull << 62) < (1ull << 63) && P.width < ((int64_t)1 << 61);
+             rle_t0 + (1ull << 62) < (1ull << 63) && rle_t0 + span_t + (1ull << 62) < (1ull << 63) &&
+             P.width < ((int64_t)1 << 61);  // (every row < 2^62: no dividend t - origin_mod + width wraps)
       if (elig) {
         const int64_t t0 = (int64_t)rle_t0;
         ra = 0;
