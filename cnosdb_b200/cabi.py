@@ -124,6 +124,7 @@ GPU_SYMBOLS = [
     "tskvgpu_scan_sync", "tskvgpu_scan_partials", "tskvgpu_scan_exchange_view", "tskvgpu_scan_merge_gathered",
     "tskvgpu_scan_snapshot_keys", "tskvgpu_scan_mask_values", "tskvgpu_scan_finalize",
     "tskvgpu_scan_finalize_device", "tskvgpu_scan_destroy", "tskvgpu_version",
+    "tskvgpu_scan_prepare_sliding", "tskvgpu_scan_aggregate_sliding",
 ]
 
 
@@ -185,6 +186,8 @@ def load_gpu_library():
     lib.tskvgpu_query_output_layout.argtypes = [vp, C.POINTER(Query), C.POINTER(OutputLayout)]
     lib.tskvgpu_scan_aggregate.argtypes = [vp, vp, C.POINTER(Query), vp, vp]
     lib.tskvgpu_scan_prepare.argtypes = [vp, vp, C.POINTER(Query), C.POINTER(vp)]
+    lib.tskvgpu_scan_aggregate_sliding.argtypes = [vp, vp, C.POINTER(Query), C.c_int64, vp, vp]
+    lib.tskvgpu_scan_prepare_sliding.argtypes = [vp, vp, C.POINTER(Query), C.c_int64, C.POINTER(vp)]
     lib.tskvgpu_scan_run.argtypes = [vp, vp]
     lib.tskvgpu_scan_enqueue.argtypes = [vp, vp]
     lib.tskvgpu_scan_sync.argtypes = [vp, vp]

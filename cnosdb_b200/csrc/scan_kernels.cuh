@@ -72,7 +72,10 @@ struct ScanParams {
   tskv_time_range ranges[MAX_RANGES];
   uint32_t n_ranges;
   int64_t width;         // <= 0: single bucket
-  int64_t origin_mod;    // origin % width
+  int64_t origin_mod;    // origin % width; a sliding scan's panes: origin % window, which may lie outside (-width, width)
+  // Rows whose dividend t - origin_mod + width does not wrap: [wrap_lo, floor_cap] (set by the host; a tumbling scan has
+  // wrap_lo = INT64_MIN). Floor-regime buckets end at floor_cap; rows below wrap_lo are located one by one.
+  int64_t floor_cap, wrap_lo;
   int64_t first_bucket_start;
   uint32_t n_buckets;
   uint32_t group_by_series;
@@ -930,7 +933,7 @@ __device__ __forceinline__ bool locate_bucket(const ScanParams &P, int64_t t, Bu
   const int64_t w = P.width;
   // the last t whose dividend t - origin_mod + w does not wrap: floor-regime buckets end there, rows past it belong to
   // the reference's wrapped windows
-  const int64_t cap = (int64_t)((uint64_t)INT64_MAX - ((uint64_t)w - (uint64_t)P.origin_mod));
+  const int64_t cap = P.floor_cap;
   if (b.valid && b.floor_regime && t > b.hi && (uint64_t)t - (uint64_t)b.hi <= (uint64_t)w && t <= cap &&
       b.idx + 1 < P.n_buckets) {  // next bucket of the floor-aligned regime
     b.lo = b.hi + 1;
@@ -944,14 +947,18 @@ __device__ __forceinline__ bool locate_bucket(const ScanParams &P, int64_t t, Bu
   int64_t diff = (int64_t)((uint64_t)start - (uint64_t)P.first_bucket_start);
   if (diff < 0 || diff % w != 0 || diff / w >= (int64_t)P.n_buckets) return false;
   b.idx = (uint32_t)(diff / w);
+  // rows below wrap_lo (dividend wrapped downwards, >= 0) share a start up to wrap_lo - 1 at most, and the next bucket is
+  // not start + w: they take no step
+  const bool wrapped = t < P.wrap_lo;
   if (dividend >= 0) {  // [start, start + w), cut at cap (start <= t <= cap)
-    const uint64_t room = (uint64_t)cap - (uint64_t)start;
+    const uint64_t room = (uint64_t)(wrapped ? P.wrap_lo - 1 : cap) - (uint64_t)start;
     b.lo = start;
     b.hi = (int64_t)((uint64_t)start + (room < (uint64_t)(w - 1) ? room : (uint64_t)(w - 1)));
-  } else {
+  } else {  // (start - w, start], cut at wrap_lo
     b.lo = start - w + 1; b.hi = start;
+    if (b.lo < P.wrap_lo) b.lo = P.wrap_lo;
   }
-  b.floor_regime = dividend >= 0;
+  b.floor_regime = dividend >= 0 && !wrapped;
   b.valid = true;
   return true;
 }
@@ -1524,7 +1531,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
       const uint64_t span_t = (uint64_t)(page_rows - 1) * rle_delta;
       elig = (int64_t)rle_delta > 0 && __umul64hi((uint64_t)(page_rows - 1), rle_delta) == 0 && span_t < (1ull << 62) &&
              rle_t0 + (1ull << 62) < (1ull << 63) && rle_t0 + span_t + (1ull << 62) < (1ull << 63) &&
-             P.width < ((int64_t)1 << 61);  // (every row < 2^62: no dividend t - origin_mod + width wraps)
+             P.width < ((int64_t)1 << 61);  // (every row < 2^62 and |origin_mod| < 2^61: no dividend t - origin_mod + width wraps)
       if (elig) {
         const int64_t t0 = (int64_t)rle_t0;
         ra = 0;
@@ -1996,6 +2003,67 @@ __global__ void k_export_pairs(uint64_t *state, StateLayout L, const MeanExport 
   for (uint64_t k = i; k < L.last_cells; k += stride) {
     state[L.last_keys_off + k] = state[L.last_pairs_off + 2 * k];
     state[L.selval_off + L.first_cells + k] = state[L.last_pairs_off + 2 * k + 1];
+  }
+}
+
+// Sliding windows (tskvgpu_scan_prepare_sliding): the fused kernels aggregate into panes one slide wide; window j of a
+// group is the fold of its panes j - k + 1 .. j (those that exist: pane p starts k - 1 slides after window p). One op
+// per state array of the window layout that the kernels fill (counts, sums, min / max keys).
+enum { COMBINE_ADD = 0, COMBINE_INT_SUM = 1, COMBINE_F64_SUM = 2, COMBINE_MIN = 3, COMBINE_MAX = 4 };
+struct CombineOp {
+  uint64_t pane_off, win_off;        // the array in the pane state / in the window state
+  uint64_t pane_hi_off, win_hi_off;  // COMBINE_INT_SUM with has_hi: high words of the exact 128-bit sum (MEAN)
+  uint32_t kind, has_hi;
+};
+
+// One thread per (op = blockIdx.y, group, window). Counts and integer sums add (wrapping low word; with has_hi the
+// carries go to the high word), f64 sums add in pane order, min / max keys take the min / max.
+__global__ void k_window_combine(const uint64_t *pane, uint64_t *win, const CombineOp *ops, uint32_t n_groups,
+                                 uint32_t n_windows, uint32_t n_panes, uint32_t k) {
+  const CombineOp op = ops[blockIdx.y];
+  const uint64_t n = (uint64_t)n_groups * n_windows;
+  for (uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; c < n; c += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t g = c / n_windows;
+    const uint32_t j = (uint32_t)(c - g * n_windows);
+    const uint32_t p0 = j + 1 >= k ? j + 1 - k : 0, p1 = j < n_panes - 1 ? j : n_panes - 1;
+    const uint64_t *src = pane + op.pane_off + g * n_panes;
+    switch (op.kind) {
+      case COMBINE_INT_SUM: {
+        const uint64_t *src_hi = pane + op.pane_hi_off + g * n_panes;
+        uint64_t lo = 0, hi = 0;
+        for (uint32_t p = p0; p <= p1; p++) {
+          const uint64_t v = src[p];
+          lo += v;
+          hi += (lo < v ? 1u : 0u) + (op.has_hi ? src_hi[p] : 0u);
+        }
+        win[op.win_off + c] = lo;
+        if (op.has_hi) win[op.win_hi_off + c] = hi;
+        break;
+      }
+      case COMBINE_F64_SUM: {
+        double acc = 0.0;
+        for (uint32_t p = p0; p <= p1; p++) acc += __longlong_as_double((long long)src[p]);
+        win[op.win_off + c] = (uint64_t)__double_as_longlong(acc);
+        break;
+      }
+      case COMBINE_MIN: {
+        int64_t acc = INT64_MAX;
+        for (uint32_t p = p0; p <= p1; p++) acc = (int64_t)src[p] < acc ? (int64_t)src[p] : acc;
+        win[op.win_off + c] = (uint64_t)acc;
+        break;
+      }
+      case COMBINE_MAX: {
+        int64_t acc = INT64_MIN;
+        for (uint32_t p = p0; p <= p1; p++) acc = (int64_t)src[p] > acc ? (int64_t)src[p] : acc;
+        win[op.win_off + c] = (uint64_t)acc;
+        break;
+      }
+      default: {
+        uint64_t acc = 0;
+        for (uint32_t p = p0; p <= p1; p++) acc += src[p];
+        win[op.win_off + c] = acc;
+      }
+    }
   }
 }
 

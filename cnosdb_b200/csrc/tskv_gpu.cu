@@ -184,6 +184,13 @@ struct tskv_scan {
   uint32_t *d_mvalid = nullptr;
   uint32_t *d_mpage = nullptr;
   uint64_t *d_mrow_off = nullptr, *d_mbm_off = nullptr;
+  // Layout of the state the fused kernels write at params.state: d_state / sl for a tumbling scan. A sliding scan's
+  // kernels fill d_pane_state (panes one slide wide) and k_window_combine folds every run of win_k panes into the
+  // windows of d_state / sl, which export, exchange, partials and finalize see.
+  StateLayout kern_sl{};
+  uint64_t *d_pane_state = nullptr;
+  CombineOp *d_combine = nullptr;
+  uint32_t n_combine = 0, win_k = 1, n_panes = 0, n_windows = 0;
 };
 
 namespace {
@@ -345,6 +352,111 @@ tskv_status compute_layout(const tskv_pages *pages, const tskv_query *q, tskv_ou
   return TSKV_OK;
 }
 
+// Offsets of the partial state of `q` over n_cells cells: the sections tskv_partials_view exposes, in that order, then
+// the scan's own arrays (first / last pairs, key snapshot, high words of exact integer sums).
+struct StatePlan {
+  StateLayout sl{};
+  std::vector<ColState> cols;
+  std::vector<MeanExport> means;
+  std::vector<uint64_t> msum_off;  // per column: the exported f64 exact integer sum of MEAN, or 0
+};
+StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
+  StatePlan plan;
+  plan.cols.resize(q->n_columns);
+  plan.msum_off.assign(q->n_columns, 0);
+  std::vector<ColState> &cols = plan.cols;
+  std::vector<MeanExport> &means = plan.means;
+  std::vector<uint64_t> &msum_off = plan.msum_off;
+  StateLayout &sl = plan.sl;
+  uint64_t off = 0;
+  sl.sum_i64_off = off;
+  for (uint32_t c = 0; c < q->n_columns; c++) {
+    const tskv_agg_column &qc = q->columns[c];
+    cols[c] = ColState{};
+    cols[c].column_id = qc.column_id;
+    cols[c].phys_type = qc.phys_type;
+    cols[c].agg_mask = qc.agg_mask;
+    cols[c].count_off = off;
+    off += n_cells;
+    if ((qc.agg_mask & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) && qc.phys_type != TSKV_PT_F64) {
+      cols[c].sum_off = off;
+      off += n_cells;
+    }
+  }
+  sl.sum_i64_len = off - sl.sum_i64_off;
+  sl.sum_f64_off = off;
+  for (uint32_t c = 0; c < q->n_columns; c++)
+    if ((q->columns[c].agg_mask & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) && q->columns[c].phys_type == TSKV_PT_F64) {
+      cols[c].sum_off = off;
+      off += n_cells;
+    }
+  for (uint32_t c = 0; c < q->n_columns; c++)
+    if ((q->columns[c].agg_mask & TSKV_AGG_MEAN) && q->columns[c].phys_type != TSKV_PT_F64) {
+      msum_off[c] = off;  // exported exact integer sum as f64 (all-reducible)
+      off += n_cells;
+    }
+  sl.sum_f64_len = off - sl.sum_f64_off;
+  uint64_t n_first = 0, n_last = 0;
+  for (uint32_t c = 0; c < q->n_columns; c++) {
+    if (q->columns[c].agg_mask & TSKV_AGG_FIRST) n_first += n_cells;
+    if (q->columns[c].agg_mask & TSKV_AGG_LAST) n_last += n_cells;
+  }
+  sl.first_cells = n_first;
+  sl.last_cells = n_last;
+  sl.min_off = off;
+  for (uint32_t c = 0; c < q->n_columns; c++)
+    if (q->columns[c].agg_mask & TSKV_AGG_MIN) {
+      cols[c].min_off = off;
+      off += n_cells;
+    }
+  sl.first_keys_off = off;
+  off += n_first;
+  sl.min_len = off - sl.min_off;
+  sl.max_off = off;
+  for (uint32_t c = 0; c < q->n_columns; c++)
+    if (q->columns[c].agg_mask & TSKV_AGG_MAX) {
+      cols[c].max_off = off;
+      off += n_cells;
+    }
+  sl.last_keys_off = off;
+  off += n_last;
+  sl.max_len = off - sl.max_off;
+  sl.selval_off = off;
+  off += n_first + n_last;
+  sl.selval_len = n_first + n_last;
+  off = (off + 1) & ~1ull;  // 16-byte alignment of the pair arrays
+  sl.first_pairs_off = off;
+  {
+    uint64_t o = off;
+    for (uint32_t c = 0; c < q->n_columns; c++)
+      if (q->columns[c].agg_mask & TSKV_AGG_FIRST) {
+        cols[c].first_off = o;
+        o += 2 * n_cells;
+      }
+    off = o;
+  }
+  sl.last_pairs_off = off;
+  {
+    uint64_t o = off;
+    for (uint32_t c = 0; c < q->n_columns; c++)
+      if (q->columns[c].agg_mask & TSKV_AGG_LAST) {
+        cols[c].last_off = o;
+        o += 2 * n_cells;
+      }
+    off = o;
+  }
+  sl.snap_off = off;
+  off += n_first + n_last;
+  for (uint32_t c = 0; c < q->n_columns; c++)
+    if (msum_off[c]) {
+      cols[c].sumhi_off = off;
+      means.push_back(MeanExport{cols[c].sum_off, off, msum_off[c], q->columns[c].phys_type == TSKV_PT_I64 ? 1u : 0u, 0});
+      off += n_cells;
+    }
+  sl.total = off;
+  return plan;
+}
+
 // Per-scan buffers are stream-ordered (cudaMallocAsync on the context stream): no device-wide
 // synchronisation on the query path, memory is recycled by the pool.
 void free_scan(tskv_scan *s) {
@@ -353,7 +465,7 @@ void free_scan(tskv_scan *s) {
   void *bufs[] = {s->d_series, s->d_rank_slot, s->d_bucket, s->d_cg_slot, s->d_item_flag, s->d_block_count, s->d_work_page, s->d_work_slot,
                   s->d_work_qcol, s->d_bin_cstart, s->d_cols, s->d_outs, s->d_means, s->d_state,
                   s->d_task_counter, s->d_values, s->d_validity, s->d_gor_scratch[0], s->d_gor_scratch[1], s->d_gathered, s->d_row_keep,
-                  s->d_mcg_active, s->d_mvals, s->d_mvalid, s->d_mpage, s->d_mrow_off, s->d_mbm_off};
+                  s->d_mcg_active, s->d_mvals, s->d_mvalid, s->d_mpage, s->d_mrow_off, s->d_mbm_off, s->d_pane_state, s->d_combine};
   for (void *b : bufs)
     if (b) cudaFreeAsync(b, st);
   if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
@@ -1150,8 +1262,65 @@ tskv_status tskvgpu_query_output_layout(const tskv_pages *pages, const tskv_quer
   return compute_layout(pages, q, out);
 }
 
-tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q,
-                                 tskv_scan **out_scan) {
+// Sliding windows of `q` (window q->width, slide < q->width) by panes: the refusals of tskvgpu_scan_prepare_sliding
+// (DESIGN.md section 7) and the pane grid. Called under ctx->mu.
+static tskv_status check_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide, uint32_t *out_k) {
+  for (uint32_t c = 0; c < q->n_columns; c++)
+    if (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) {
+      ctx->set_error("sliding windows: FIRST / LAST drop a (page, window) run on a NULL at its first / last row, which "
+                     "pane partials cannot rebuild");
+      return TSKV_ERR_UNSUPPORTED;
+    }
+  if (slide > q->width) {
+    ctx->set_error("sliding windows: a slide wider than the window (rows between windows) is not pushed down");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  if (q->width >= (int64_t)1 << 61) {
+    ctx->set_error("sliding windows: window of 2^61 or more");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  const uint64_t k = ((uint64_t)q->width - 1) / (uint64_t)slide + 1;  // windows per row, ceil(window / slide)
+  if (k > 100) {
+    ctx->set_error("sliding windows: more than 100 windows per row (Too many overlapping windows)");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  if (q->n_buckets < k) {
+    ctx->set_error("sliding windows: n_buckets must be at least ceil(window / slide)");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  if ((unsigned __int128)q->n_buckets * (uint64_t)slide > (unsigned __int128)1 << 63) {
+    ctx->set_error("sliding windows: the window grid spans more than 2^63");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  // With window % slide != 0 the reference keeps a row's copies by the test window-0 start <= t < end, which passes for
+  // every row whose dividend t - start_time % window + slide is >= 0 and whose window end does not wrap, and fails for
+  // other rows unless the remainder is 0: refuse unless every row the query can select is of the first kind.
+  if (q->width % slide != 0 && pages->n_cg) {
+    ensure_time_bounds(ctx, pages);
+    int64_t lo = pages->ts_min, hi = pages->ts_max;
+    if (q->n_time_ranges > 0) {
+      int64_t qlo = q->time_ranges[0].min_ts, qhi = q->time_ranges[0].max_ts;
+      for (uint32_t r = 1; r < q->n_time_ranges; r++) {
+        qlo = std::min(qlo, q->time_ranges[r].min_ts);
+        qhi = std::max(qhi, q->time_ranges[r].max_ts);
+      }
+      lo = std::max(lo, qlo);
+      hi = std::min(hi, qhi);
+    }
+    const __int128 om = q->origin % q->width;
+    if (lo <= hi && ((__int128)lo - om + slide < 0 || (__int128)hi - om + slide > (__int128)INT64_MAX ||
+                     (__int128)hi + q->width > (__int128)INT64_MAX)) {
+      ctx->set_error("sliding windows: window % slide != 0 and rows in the truncating-% or wrapping range of the window "
+                     "expression");
+      return TSKV_ERR_UNSUPPORTED;
+    }
+  }
+  *out_k = (uint32_t)k;
+  return TSKV_OK;
+}
+
+// tskvgpu_scan_prepare; slide > 0: tskvgpu_scan_prepare_sliding with slide < width.
+static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide, tskv_scan **out_scan) {
   if (!ctx || !pages || !q || !out_scan) return TSKV_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(ctx->mu);
   ctx->set_error("");
@@ -1206,6 +1375,11 @@ tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const t
       return TSKV_ERR_INVALID_ARG;
     }
   }
+  uint32_t win_k = 1;
+  if (slide) {
+    st = check_sliding(ctx, pages, q, slide, &win_k);
+    if (st != TSKV_OK) return st;
+  }
   cudaSetDevice(ctx->device);
   tskv_scan *s = new tskv_scan();
   s->pages = pages;
@@ -1213,6 +1387,12 @@ tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const t
   s->n_cols = q->n_columns;
   s->n_out = (uint32_t)L.n_out;
   const uint64_t n_cells = L.n_cells;
+  // the fused kernels' bucket grid: the query's, or for a sliding scan the panes of width `slide`, from the start of the
+  // last pane of window 0 to the start of the last window
+  s->win_k = win_k;
+  s->n_windows = q->n_buckets;
+  s->n_panes = q->n_buckets - win_k + 1;
+  const uint64_t kern_cells = L.n_groups * s->n_panes;
 
   // ---- first/last key budget ---------------------------------------------------------------------
   bool any_sel = false;
@@ -1261,115 +1441,48 @@ tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const t
   }
 
   // ---- state layout ------------------------------------------------------------------------------
-  std::vector<ColState> cols(q->n_columns);
-  StateLayout &sl = s->sl;
-  uint64_t off = 0;
-  sl.sum_i64_off = off;
-  for (uint32_t c = 0; c < q->n_columns; c++) {
-    const tskv_agg_column &qc = q->columns[c];
-    cols[c] = ColState{};
-    cols[c].column_id = qc.column_id;
-    cols[c].phys_type = qc.phys_type;
-    cols[c].agg_mask = qc.agg_mask;
-    cols[c].count_off = off;
-    off += n_cells;
-    if ((qc.agg_mask & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) && qc.phys_type != TSKV_PT_F64) {
-      cols[c].sum_off = off;
-      off += n_cells;
-    }
-  }
-  sl.sum_i64_len = off - sl.sum_i64_off;
-  sl.sum_f64_off = off;
-  for (uint32_t c = 0; c < q->n_columns; c++)
-    if ((q->columns[c].agg_mask & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) && q->columns[c].phys_type == TSKV_PT_F64) {
-      cols[c].sum_off = off;
-      off += n_cells;
-    }
-  std::vector<MeanExport> means;
-  std::vector<uint64_t> msum_off(q->n_columns, 0);
-  for (uint32_t c = 0; c < q->n_columns; c++)
-    if ((q->columns[c].agg_mask & TSKV_AGG_MEAN) && q->columns[c].phys_type != TSKV_PT_F64) {
-      msum_off[c] = off;  // exported exact integer sum as f64 (all-reducible)
-      off += n_cells;
-    }
-  sl.sum_f64_len = off - sl.sum_f64_off;
-  uint64_t n_first = 0, n_last = 0;
-  for (uint32_t c = 0; c < q->n_columns; c++) {
-    if (q->columns[c].agg_mask & TSKV_AGG_FIRST) n_first += n_cells;
-    if (q->columns[c].agg_mask & TSKV_AGG_LAST) n_last += n_cells;
-  }
-  sl.first_cells = n_first;
-  sl.last_cells = n_last;
-  sl.min_off = off;
-  for (uint32_t c = 0; c < q->n_columns; c++)
-    if (q->columns[c].agg_mask & TSKV_AGG_MIN) {
-      cols[c].min_off = off;
-      off += n_cells;
-    }
-  sl.first_keys_off = off;
-  off += n_first;
-  sl.min_len = off - sl.min_off;
-  sl.max_off = off;
-  for (uint32_t c = 0; c < q->n_columns; c++)
-    if (q->columns[c].agg_mask & TSKV_AGG_MAX) {
-      cols[c].max_off = off;
-      off += n_cells;
-    }
-  sl.last_keys_off = off;
-  off += n_last;
-  sl.max_len = off - sl.max_off;
-  sl.selval_off = off;
-  off += n_first + n_last;
-  sl.selval_len = n_first + n_last;
-  off = (off + 1) & ~1ull;  // 16-byte alignment of the pair arrays
-  sl.first_pairs_off = off;
-  {
-    uint64_t o = off;
-    for (uint32_t c = 0; c < q->n_columns; c++)
-      if (q->columns[c].agg_mask & TSKV_AGG_FIRST) {
-        cols[c].first_off = o;
-        o += 2 * n_cells;
+  // a sliding scan: what the fused kernels write (panes) and what the rest of the pass sees (windows)
+  const StatePlan win = plan_state(q, n_cells);
+  const StatePlan pane = slide ? plan_state(q, kern_cells) : StatePlan{};
+  s->sl = win.sl;
+  s->kern_sl = slide ? pane.sl : win.sl;
+  std::vector<ColState> cols = slide ? pane.cols : win.cols;
+  const std::vector<MeanExport> &means = win.means;
+  const std::vector<uint64_t> &msum_off = win.msum_off;
+  const StateLayout &sl = s->sl;
+  std::vector<CombineOp> combine;
+  if (slide) {
+    for (uint32_t c = 0; c < q->n_columns; c++) {
+      const ColState &p = pane.cols[c], &w = win.cols[c];
+      const uint8_t m = q->columns[c].agg_mask;
+      combine.push_back(CombineOp{p.count_off, w.count_off, 0, 0, COMBINE_ADD, 0});
+      if (m & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) {
+        if (q->columns[c].phys_type == TSKV_PT_F64) combine.push_back(CombineOp{p.sum_off, w.sum_off, 0, 0, COMBINE_F64_SUM, 0});
+        else combine.push_back(CombineOp{p.sum_off, w.sum_off, p.sumhi_off, w.sumhi_off, COMBINE_INT_SUM, (m & TSKV_AGG_MEAN) ? 1u : 0u});
       }
-    off = o;
-  }
-  sl.last_pairs_off = off;
-  {
-    uint64_t o = off;
-    for (uint32_t c = 0; c < q->n_columns; c++)
-      if (q->columns[c].agg_mask & TSKV_AGG_LAST) {
-        cols[c].last_off = o;
-        o += 2 * n_cells;
-      }
-    off = o;
-  }
-  sl.snap_off = off;
-  off += n_first + n_last;
-  for (uint32_t c = 0; c < q->n_columns; c++)
-    if (msum_off[c]) {
-      cols[c].sumhi_off = off;
-      means.push_back(MeanExport{cols[c].sum_off, off, msum_off[c], q->columns[c].phys_type == TSKV_PT_I64 ? 1u : 0u, 0});
-      off += n_cells;
+      if (m & TSKV_AGG_MIN) combine.push_back(CombineOp{p.min_off, w.min_off, 0, 0, COMBINE_MIN, 0});
+      if (m & TSKV_AGG_MAX) combine.push_back(CombineOp{p.max_off, w.max_off, 0, 0, COMBINE_MAX, 0});
     }
-  sl.total = off;
+  }
 
   // output column table
   std::vector<OutCol> outs;
   {
-    uint64_t fk = sl.first_keys_off, lk = sl.last_keys_off, fv = sl.selval_off, lv = sl.selval_off + n_first;
+    uint64_t fk = sl.first_keys_off, lk = sl.last_keys_off, fv = sl.selval_off, lv = sl.selval_off + sl.first_cells;
     for (uint32_t c = 0; c < q->n_columns; c++) {
       const tskv_agg_column &qc = q->columns[c];
       for (unsigned bit = 0; bit < 7; bit++) {
         unsigned agg = 1u << bit;
         if (!(qc.agg_mask & agg)) continue;
         OutCol oc{};
-        oc.count_off = cols[c].count_off;
+        oc.count_off = win.cols[c].count_off;
         oc.agg = (uint8_t)agg;
         oc.phys_type = qc.phys_type;
         switch (agg) {
-          case TSKV_AGG_SUM: oc.src_off = cols[c].sum_off; break;
-          case TSKV_AGG_MEAN: oc.src_off = msum_off[c] ? msum_off[c] : cols[c].sum_off; break;
-          case TSKV_AGG_MIN: oc.src_off = cols[c].min_off; break;
-          case TSKV_AGG_MAX: oc.src_off = cols[c].max_off; break;
+          case TSKV_AGG_SUM: oc.src_off = win.cols[c].sum_off; break;
+          case TSKV_AGG_MEAN: oc.src_off = msum_off[c] ? msum_off[c] : win.cols[c].sum_off; break;
+          case TSKV_AGG_MIN: oc.src_off = win.cols[c].min_off; break;
+          case TSKV_AGG_MAX: oc.src_off = win.cols[c].max_off; break;
           case TSKV_AGG_FIRST: oc.src_off = fk; oc.val_off = fv; break;
           case TSKV_AGG_LAST: oc.src_off = lk; oc.val_off = lv; break;
           default: break;
@@ -1425,6 +1538,11 @@ tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const t
   if (e == cudaSuccess && !means.empty())
     e = cudaMemcpyAsync(s->d_means, means.data(), means.size() * sizeof(MeanExport), cudaMemcpyHostToDevice, ctx->stream);
   if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_state, sl.total);
+  if (e == cudaSuccess && slide) e = stream_alloc(ctx, &s->d_pane_state, s->kern_sl.total);
+  s->n_combine = (uint32_t)combine.size();
+  if (e == cudaSuccess && slide) e = stream_alloc(ctx, &s->d_combine, combine.size());
+  if (e == cudaSuccess && slide)
+    e = cudaMemcpyAsync(s->d_combine, combine.data(), combine.size() * sizeof(CombineOp), cudaMemcpyHostToDevice, ctx->stream);
   s->preds.n = q->n_predicates;
   for (uint32_t k = 0; k < q->n_predicates; k++) s->preds.p[k] = q->predicates[k];
   if (q->n_predicates) ensure_page_stats(ctx, pages);  // value-statistics pruning (filter_column_groups, reader/chunk.rs:12-50)
@@ -1435,7 +1553,8 @@ tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const t
   if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_values, L.n_out * L.n_cells);
   if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_validity, L.validity_bytes + 8);
   if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_outs, outs.data(), outs.size() * sizeof(OutCol), cudaMemcpyHostToDevice, ctx->stream);
-  h2d += cols.size() * sizeof(ColState) + outs.size() * sizeof(OutCol) + means.size() * sizeof(MeanExport) + sizeof(ScanParams);
+  h2d += cols.size() * sizeof(ColState) + outs.size() * sizeof(OutCol) + means.size() * sizeof(MeanExport) + sizeof(ScanParams) +
+         combine.size() * sizeof(CombineOp);
   if (e != cudaSuccess) {
     ctx->set_error(std::string("scan_prepare: ") + cudaGetErrorString(e));
     free_scan(s);
@@ -1461,7 +1580,7 @@ tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const t
   P.work_qcol = s->d_work_qcol;
   P.bin_cstart = s->d_bin_cstart;
   P.cols = s->d_cols;
-  P.state = s->d_state;
+  P.state = slide ? s->d_pane_state : s->d_state;
   P.task_counter = s->d_task_counter;
   P.status = s->d_status;
   P.err_page = s->d_err_page;
@@ -1473,12 +1592,18 @@ tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const t
     s->prune.n = q->n_time_ranges;
     for (uint32_t k = 0; k < q->n_time_ranges; k++) s->prune.r[k] = q->time_ranges[k];
   }
-  P.width = q->width;
-  P.origin_mod = q->width > 0 ? q->origin % q->width : 0;
-  P.first_bucket_start = q->first_bucket_start;
-  P.n_buckets = q->n_buckets;
+  P.width = slide ? slide : q->width;
+  P.origin_mod = q->width > 0 ? q->origin % q->width : 0;  // (a sliding scan: start_time % window, as the reference)
+  if (P.width > 0) {
+    const __int128 cap = (__int128)INT64_MAX - ((__int128)P.width - P.origin_mod);
+    const __int128 wlo = (__int128)INT64_MIN + ((__int128)P.origin_mod - P.width);
+    P.floor_cap = cap > (__int128)INT64_MAX ? INT64_MAX : (int64_t)cap;
+    P.wrap_lo = wlo < (__int128)INT64_MIN ? INT64_MIN : (int64_t)wlo;
+  }
+  P.first_bucket_start = (int64_t)((uint64_t)q->first_bucket_start + (uint64_t)(win_k - 1) * (uint64_t)P.width);
+  P.n_buckets = s->n_panes;
   P.group_by_series = q->group_by_series;
-  P.n_cells = n_cells;
+  P.n_cells = kern_cells;
   P.slot_bits = slot_bits;
   P.slot_max = slot_bits ? (uint32_t)((1ull << slot_bits) - 1) : 0;
   P.rel_base = rel_base;
@@ -1488,12 +1613,12 @@ tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const t
     for (uint32_t c = 0; c < q->n_columns; c++) {
       const uint8_t m = q->columns[c].agg_mask;
       const bool is_int = q->columns[c].phys_type != TSKV_PT_F64;
-      cols[c].s_count = words; words += (uint32_t)n_cells;
-      if (m & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) { cols[c].s_sum = words; words += (uint32_t)n_cells; }
-      if ((m & TSKV_AGG_MEAN) && is_int) { cols[c].s_hi = words; words += (uint32_t)n_cells; }
-      if (m & TSKV_AGG_MIN) { cols[c].s_min = words; words += (uint32_t)n_cells; }
-      if (m & TSKV_AGG_MAX) { cols[c].s_max = words; words += (uint32_t)n_cells; }
-      if (n_cells > (1u << 20)) { words = UINT32_MAX / 2; break; }
+      cols[c].s_count = words; words += (uint32_t)kern_cells;
+      if (m & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) { cols[c].s_sum = words; words += (uint32_t)kern_cells; }
+      if ((m & TSKV_AGG_MEAN) && is_int) { cols[c].s_hi = words; words += (uint32_t)kern_cells; }
+      if (m & TSKV_AGG_MIN) { cols[c].s_min = words; words += (uint32_t)kern_cells; }
+      if (m & TSKV_AGG_MAX) { cols[c].s_max = words; words += (uint32_t)kern_cells; }
+      if (kern_cells > (1u << 20)) { words = UINT32_MAX / 2; break; }
     }
     // table limit 32 KB: larger tables cost more in occupancy than the contention they remove (H100, C3: 10 columns x
     // 168 buckets, 53 KB table: 7.8 ms vs 5.4 ms with global atomics); TSKV_SMEM_TABLE_KB overrides
@@ -1676,11 +1801,11 @@ tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const t
       s->coop.gor_scratch[k] = s->d_gor_scratch[k];
     }
     // bucket arithmetic of the cooperative kernels: multiply-high division by the invariant width
-    if (q->width > 0) {
-      s->coop.div = make_magic((uint64_t)q->width);
-      const int64_t d0 = (int64_t)((uint64_t)q->first_bucket_start - (uint64_t)P.origin_mod + (uint64_t)q->width);
-      s->coop.grid_ok = (d0 >= 0 && d0 % q->width == 0) ? 1u : 0u;
-      s->coop.q0 = s->coop.grid_ok ? d0 / q->width : 0;
+    if (P.width > 0) {
+      s->coop.div = make_magic((uint64_t)P.width);
+      const int64_t d0 = (int64_t)((uint64_t)P.first_bucket_start - (uint64_t)P.origin_mod + (uint64_t)P.width);
+      s->coop.grid_ok = (d0 >= 0 && d0 % P.width == 0) ? 1u : 0u;
+      s->coop.q0 = s->coop.grid_ok ? d0 / P.width : 0;
     }
   }
   // ---- merge pass over the overlapping chunks (merge_kernels.cuh): which merge column groups this scan reads
@@ -1767,6 +1892,22 @@ tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const t
   return TSKV_OK;
 }
 
+tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, tskv_scan **out_scan) {
+  return prepare_scan(ctx, pages, q, 0, out_scan);
+}
+
+tskv_status tskvgpu_scan_prepare_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
+                                         tskv_scan **out_scan) {
+  if (!ctx || !pages || !q || !out_scan) return TSKV_ERR_INVALID_ARG;
+  if (slide <= 0 || q->width <= 0) {
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    ctx->set_error("sliding windows: slide and window must be > 0");
+    *out_scan = nullptr;
+    return TSKV_ERR_INVALID_ARG;
+  }
+  return prepare_scan(ctx, pages, q, slide == q->width ? 0 : slide, out_scan);  // slide == window: a tumbling window
+}
+
 // Enqueues one full pass on the context stream, no host synchronisation:
 //   selection -> compacted work list -> (host-resident arenas: PCIe gather of the selected pages)
 //   -> state init -> one fused decode/filter/reduce kernel per decode-kind bin -> export.
@@ -1787,9 +1928,9 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
   unsigned long long *aux = reinterpret_cast<unsigned long long *>(s->d_task_counter);
   uint64_t launches = 0;
   {  // state identities + the pass's scratch (task counters / status / counters, bin starts, work-list buckets): one launch
-    const uint32_t init_blocks = (uint32_t)std::min<uint64_t>((s->sl.total + 255) / 256, 4096);
-    k_init_state<<<std::max(1u, init_blocks), 256, 0, ctx->stream>>>(s->d_state, s->sl, aux, 32, s->d_bin_cstart, N_BINS + 2, s->d_bucket,
-                                                                   N_BINS * s->n_cols);
+    const uint32_t init_blocks = (uint32_t)std::min<uint64_t>((s->kern_sl.total + 255) / 256, 4096);
+    k_init_state<<<std::max(1u, init_blocks), 256, 0, ctx->stream>>>(s->params.state, s->kern_sl, aux, 32, s->d_bin_cstart, N_BINS + 2,
+                                                                   s->d_bucket, N_BINS * s->n_cols);
     launches++;
   }
   // slot of every column group: the row filter, the merge pass and the item-driven work list need it per GROUP; the
@@ -1948,6 +2089,12 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     cudaStreamWaitEvent(ctx->stream, ev, 0);
   }
   if (!capturing) cudaEventRecord(s->ev_bin[N_BINS], ctx->stream);
+  if (s->n_combine) {  // sliding windows: every window folds its panes (it writes every array the kernels fill)
+    const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
+    k_window_combine<<<dim3(std::max(1u, bx), s->n_combine), 256, 0, ctx->stream>>>(
+        s->d_pane_state, s->d_state, s->d_combine, (uint32_t)s->layout.n_groups, s->n_windows, s->n_panes, s->win_k);
+    launches++;
+  }
   if (s->has_sel || s->n_means) {
     uint64_t work = std::max(std::max(s->sl.first_cells, s->sl.last_cells), s->n_means ? s->layout.n_cells : 0);
     uint32_t b = (uint32_t)std::min<uint64_t>((work + 255) / 256, 4096);
@@ -2180,17 +2327,33 @@ void tskvgpu_scan_destroy(tskv_ctx *ctx, tskv_scan *s) {
   free_scan(s);
 }
 
-tskv_status tskvgpu_scan_aggregate(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q,
-                                   uint64_t *out_values, uint8_t *out_validity) {
+static tskv_status scan_aggregate(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
+                                  uint64_t *out_values, uint8_t *out_validity) {
   if (!out_values || !out_validity) return TSKV_ERR_INVALID_ARG;
   tskv_scan *s = nullptr;
-  tskv_status st = tskvgpu_scan_prepare(ctx, pages, q, &s);
+  tskv_status st = slide ? tskvgpu_scan_prepare_sliding(ctx, pages, q, slide, &s) : tskvgpu_scan_prepare(ctx, pages, q, &s);
   if (st != TSKV_OK) return st;
   st = tskvgpu_scan_run(ctx, s);
   if (st == TSKV_OK) st = tskvgpu_scan_finalize(ctx, s, out_values, out_validity);
   ctx->counters.kernel_launches += 1;
   tskvgpu_scan_destroy(ctx, s);
   return st;
+}
+
+tskv_status tskvgpu_scan_aggregate(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q,
+                                   uint64_t *out_values, uint8_t *out_validity) {
+  return scan_aggregate(ctx, pages, q, 0, out_values, out_validity);
+}
+
+tskv_status tskvgpu_scan_aggregate_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
+                                           uint64_t *out_values, uint8_t *out_validity) {
+  if (slide <= 0) {  // (slide 0 would select the tumbling scan)
+    if (!ctx) return TSKV_ERR_INVALID_ARG;
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    ctx->set_error("sliding windows: slide and window must be > 0");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  return scan_aggregate(ctx, pages, q, slide, out_values, out_validity);
 }
 
 }  // extern "C"

@@ -19,6 +19,34 @@ AGG_BITS = {"count": TSKV_AGG_COUNT, "sum": TSKV_AGG_SUM, "min": TSKV_AGG_MIN, "
             "mean": TSKV_AGG_MEAN, "avg": TSKV_AGG_MEAN, "first": TSKV_AGG_FIRST, "last": TSKV_AGG_LAST}
 
 
+def _wrap64(x):
+    x &= (1 << 64) - 1
+    return x - (1 << 64) if x >> 63 else x
+
+
+def _cmod(a, b):
+    """a % b with the sign of a (C / Rust `%`)."""
+    r = abs(a) % abs(b)
+    return -r if a < 0 else r
+
+
+def window_last_start(t, window, slide, origin):
+    """Start of the last window holding t: t - ((t - origin % window) + slide) % slide, with truncating `%` and wrapping
+    i64 arithmetic like the reference's window expression (transform_time_window.rs:251-296)."""
+    return _wrap64(t - _cmod(_wrap64(_wrap64(t - _cmod(origin, window)) + slide), slide))
+
+
+def sliding_window_grid(lo, hi, window, slide, origin=0):
+    """(first_bucket_start, n_buckets) of the windows of time_window(time, window, slide, origin) that hold the rows of
+    the closed range [lo, hi]: from the first window of lo, last_start(lo) - (k - 1) * slide with k = ceil(window /
+    slide), to the last window of hi, last_start(hi). For rows whose dividend t - origin % window + slide is >= 0 and
+    does not wrap (the reference's floor regime)."""
+    k = -(-window // slide)
+    first = window_last_start(lo, window, slide, origin) - (k - 1) * slide
+    last = window_last_start(hi, window, slide, origin)
+    return first, (last - first) // slide + 1
+
+
 class TskvError(RuntimeError):
     """Mirrors TskvError::Decode / TsmPageFileHashCheckFailed: carries the status code."""
 
@@ -343,19 +371,30 @@ class Engine:
             raise TskvError(st, "invalid query")
         return L
 
-    def scan_aggregate(self, pages, query):
-        """End-to-end call: query args H2D, fused scan, result D2H (BatchReader::process analogue)."""
+    def scan_aggregate(self, pages, query, slide=None):
+        """End-to-end call: query args H2D, fused scan, result D2H (BatchReader::process analogue).
+        slide: sliding windows time_window(time, query.width, slide, query.origin); output bucket j is the window
+        starting at query.first_bucket_start + j * slide (sliding_window_grid sizes that grid)."""
         L = self.output_layout(pages, query)
         values = np.empty(int(L.n_out * L.n_cells), dtype=np.uint64)
         bitmaps = np.empty(int(L.validity_bytes), dtype=np.uint8)
         q = query.to_c()
-        self._check(self.lib.tskvgpu_scan_aggregate(self.ctx, pages.handle, C.byref(q),
-                                                    values.ctypes.data, bitmaps.ctypes.data))
+        if slide is None:
+            st = self.lib.tskvgpu_scan_aggregate(self.ctx, pages.handle, C.byref(q), values.ctypes.data, bitmaps.ctypes.data)
+        else:
+            st = self.lib.tskvgpu_scan_aggregate_sliding(self.ctx, pages.handle, C.byref(q), int(slide),
+                                                         values.ctypes.data, bitmaps.ctypes.data)
+        self._check(st)
         return ScanResult(query, L, values, bitmaps)
 
-    def prepare(self, pages, query):
+    def prepare(self, pages, query, slide=None):
+        """Device-resident scan (run / enqueue / partials / exchange / finalize); slide: as in scan_aggregate."""
         L = self.output_layout(pages, query)
         q = query.to_c()
         h = C.c_void_p()
-        self._check(self.lib.tskvgpu_scan_prepare(self.ctx, pages.handle, C.byref(q), C.byref(h)))
+        if slide is None:
+            st = self.lib.tskvgpu_scan_prepare(self.ctx, pages.handle, C.byref(q), C.byref(h))
+        else:
+            st = self.lib.tskvgpu_scan_prepare_sliding(self.ctx, pages.handle, C.byref(q), int(slide), C.byref(h))
+        self._check(st)
         return PreparedScan(self, pages, query, h, L)

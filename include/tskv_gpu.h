@@ -379,6 +379,27 @@ tskv_status tskvgpu_scan_finalize_device(tskv_ctx *ctx, tskv_scan *scan, uint64_
                                          uint64_t *out_validity_dptr);
 void tskvgpu_scan_destroy(tskv_ctx *ctx, tskv_scan *scan);
 
+/* ---- sliding windows: time_window(time, window, slide[, start_time]) --------------------------
+ * The reference expands every row into k = ceil(window / slide) copies, one per window starting at
+ * last_start(t) - i * slide (i < k), last_start(t) = t - ((t - start_time % window) + slide) % slide with truncating %
+ * and wrapping arithmetic (build_sliding_window_plan, query_server/query/src/extension/analyse/transform_time_window.rs:
+ * 251-393). These calls decode, filter and aggregate each row once, into panes one slide wide, and fold every run of k
+ * consecutive panes into a window. The query's fields keep their meaning: width = window, origin = start_time; output
+ * bucket j is the window starting at first_bucket_start + j * slide (n_buckets windows; tskvgpu_query_output_layout
+ * describes the result). Every window of every selected row must lie on that grid, else TSKV_ERR_BUCKET_RANGE. The scan
+ * returned works with every tskvgpu_scan_* call above. slide == width is the tumbling scan (tskvgpu_scan_prepare).
+ * Refused before any launch:
+ *   TSKV_ERR_INVALID_ARG   slide <= 0, width <= 0, k > 100 ("Too many overlapping windows"), n_buckets < k, or a grid
+ *                          n_buckets * slide wider than 2^63
+ *   TSKV_ERR_UNSUPPORTED   FIRST / LAST; slide > width; width >= 2^61; width % slide != 0 when a row the query can
+ *                          select (time ranges x the page set's time bounds) has t - start_time % window + slide < 0, or
+ *                          that dividend or t + window wraps (there the reference drops copies by the window-0 test:
+ *                          see DESIGN.md section 7) */
+tskv_status tskvgpu_scan_prepare_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q,
+                                         int64_t slide, tskv_scan **out_scan);
+tskv_status tskvgpu_scan_aggregate_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q,
+                                           int64_t slide, uint64_t *out_values, uint8_t *out_validity);
+
 /* Library version / build info ("tskv-b200 <semver> sm_90a"). */
 const char *tskvgpu_version(void);
 

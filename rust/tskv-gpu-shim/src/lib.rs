@@ -115,7 +115,14 @@ impl GpuEngine {
         self.check(unsafe { sys::tskvgpu_query_output_layout(pages.pages, &raw, &mut layout) })?;
         let mut values = vec![0u64; (layout.n_out * layout.n_cells) as usize];
         let mut validity = vec![0u8; layout.validity_bytes as usize];
-        self.check(unsafe { sys::tskvgpu_scan_aggregate(self.ctx, pages.pages, &raw, values.as_mut_ptr(), validity.as_mut_ptr()) })?;
+        self.check(unsafe {
+            match q.slide {
+                None => sys::tskvgpu_scan_aggregate(self.ctx, pages.pages, &raw, values.as_mut_ptr(), validity.as_mut_ptr()),
+                Some(slide) => {
+                    sys::tskvgpu_scan_aggregate_sliding(self.ctx, pages.pages, &raw, slide, values.as_mut_ptr(), validity.as_mut_ptr())
+                }
+            }
+        })?;
         Ok(AggregateResult { layout, values, validity })
     }
 
@@ -131,7 +138,12 @@ impl GpuEngine {
         let mut layout = sys::tskv_output_layout::default();
         self.check(unsafe { sys::tskvgpu_query_output_layout(pages.pages, &raw, &mut layout) })?;
         let mut scan = std::ptr::null_mut();
-        self.check(unsafe { sys::tskvgpu_scan_prepare(self.ctx, pages.pages, &raw, &mut scan) })?;
+        self.check(unsafe {
+            match q.slide {
+                None => sys::tskvgpu_scan_prepare(self.ctx, pages.pages, &raw, &mut scan),
+                Some(slide) => sys::tskvgpu_scan_prepare_sliding(self.ctx, pages.pages, &raw, slide, &mut scan),
+            }
+        })?;
         let mut values = vec![0u64; (layout.n_out * layout.n_cells) as usize];
         let mut validity = vec![0u8; layout.validity_bytes as usize];
         let run = || -> GpuResult<()> {
@@ -214,10 +226,13 @@ pub struct Query {
     pub series_ids: Option<Vec<u32>>,
     pub time_ranges: Vec<tskv_time_range>,
     pub origin: i64,
-    /// bucket width in the time column's unit; <= 0: no bucketing
+    /// bucket width in the time column's unit; <= 0: no bucketing. With `slide`: the window length
     pub width: i64,
     pub first_bucket_start: i64,
     pub n_buckets: u32,
+    /// `time_window(time, width, slide, origin)`: output bucket j is the window starting at
+    /// `first_bucket_start + j * slide`; `None` = tumbling buckets of `width`
+    pub slide: Option<i64>,
     pub group_by_series: bool,
     pub columns: Vec<tskv_agg_column>,
     pub predicates: Vec<tskv_field_predicate>,

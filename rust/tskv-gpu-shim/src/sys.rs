@@ -270,6 +270,21 @@ extern "C" {
         q: *const tskv_query,
         out_scan: *mut *mut tskv_scan,
     ) -> tskv_status;
+    pub fn tskvgpu_scan_prepare_sliding(
+        ctx: *mut tskv_ctx,
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        slide: i64,
+        out_scan: *mut *mut tskv_scan,
+    ) -> tskv_status;
+    pub fn tskvgpu_scan_aggregate_sliding(
+        ctx: *mut tskv_ctx,
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        slide: i64,
+        out_values: *mut u64,
+        out_validity: *mut u8,
+    ) -> tskv_status;
     pub fn tskvgpu_scan_run(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
     pub fn tskvgpu_scan_enqueue(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
     pub fn tskvgpu_scan_sync(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
