@@ -125,6 +125,7 @@ GPU_SYMBOLS = [
     "tskvgpu_scan_snapshot_keys", "tskvgpu_scan_mask_values", "tskvgpu_scan_finalize",
     "tskvgpu_scan_finalize_device", "tskvgpu_scan_destroy", "tskvgpu_version",
     "tskvgpu_scan_prepare_sliding", "tskvgpu_scan_aggregate_sliding",
+    "tskvgpu_query_output_layout_grouped", "tskvgpu_scan_prepare_grouped", "tskvgpu_scan_aggregate_grouped",
 ]
 
 
@@ -188,6 +189,9 @@ def load_gpu_library():
     lib.tskvgpu_scan_prepare.argtypes = [vp, vp, C.POINTER(Query), C.POINTER(vp)]
     lib.tskvgpu_scan_aggregate_sliding.argtypes = [vp, vp, C.POINTER(Query), C.c_int64, vp, vp]
     lib.tskvgpu_scan_prepare_sliding.argtypes = [vp, vp, C.POINTER(Query), C.c_int64, C.POINTER(vp)]
+    lib.tskvgpu_query_output_layout_grouped.argtypes = [vp, C.POINTER(Query), vp, C.c_uint32, C.POINTER(OutputLayout)]
+    lib.tskvgpu_scan_prepare_grouped.argtypes = [vp, vp, C.POINTER(Query), vp, C.c_uint32, C.c_int64, C.POINTER(vp)]
+    lib.tskvgpu_scan_aggregate_grouped.argtypes = [vp, vp, C.POINTER(Query), vp, C.c_uint32, C.c_int64, vp, vp]
     lib.tskvgpu_scan_run.argtypes = [vp, vp]
     lib.tskvgpu_scan_enqueue.argtypes = [vp, vp]
     lib.tskvgpu_scan_sync.argtypes = [vp, vp]

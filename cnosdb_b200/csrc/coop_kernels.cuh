@@ -463,7 +463,7 @@ __device__ __forceinline__ void scan_page_coop(const ScanParams &P, const CoopPa
   // ---- D. lane-per-segment reduce ---------------------------------------------------------------------
   const uint64_t flip = pt == TSKV_PT_U64 ? 0x8000000000000000ull : 0ull;
   const bool mean_hi = (mask & TSKV_AGG_MEAN) != 0;
-  const uint64_t group_base = P.group_by_series ? (uint64_t)slot * P.n_buckets : 0;
+  const uint64_t group_base = group_cell_base(P, slot);
   for (uint32_t s0 = 0; s0 < n_seg; s0 += 32) {
     const uint32_t s = s0 + lane;
     if (s < n_seg) {

@@ -80,6 +80,8 @@ struct ScanParams {
   uint32_t n_buckets;
   uint32_t group_by_series;
   uint64_t n_cells;
+  // GROUP BY tags: group of every slot, < n_groups with n_groups * n_buckets < 2^32 (host-checked); null otherwise
+  const uint32_t *slot_group;
   // first/last tie-break key. slot_bits == 0 (one slot per cell): key = timestamp itself.
   // Otherwise key = rel << slot_bits | slot with rel = t - (bucket_start - width) in (0, 2*width)
   // for bucketed scans and rel = t - rel_base for unbucketed ones; the host checked the bit budget.
@@ -114,6 +116,13 @@ struct ScanParams {
   uint32_t bin_parts[N_BINS];
   uint32_t bin_part_rows[N_BINS];
 };
+
+// First cell of the group a work item's series belongs to: GROUP BY tags slot_group[slot], GROUP BY series the slot
+// itself, GROUP BY bucket the one group. Read once per page.
+__device__ __forceinline__ uint64_t group_cell_base(const ScanParams &P, uint32_t slot) {
+  if (P.slot_group) return (uint64_t)__ldg(P.slot_group + slot) * P.n_buckets;
+  return P.group_by_series ? (uint64_t)slot * P.n_buckets : 0;
+}
 
 // ------------------------------------------------------------------------------------------------
 // selection / compaction
@@ -313,6 +322,9 @@ struct WorkListArgs {
   uint32_t n_set_series;
   const uint32_t *series_ids;    // the selection (null: every series, slot = rank)
   uint32_t n_sel;                // threads: selected ids, or n_set_series
+  // GROUP BY tags: thread i walks slot walk[i], the slots stably sorted by group, so that the items of a (bin, column)
+  // bucket come group by group and a warp's 32 pages mostly share a group (null: thread i walks slot i)
+  const uint32_t *walk;
   const ColState *cols;
   uint32_t n_cols;
   const tskv_time_range *cg_bounds;  // statistics pruning (null: none)
@@ -389,7 +401,7 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_count(const WorkListArg
   __syncthreads();
   const uint32_t i = blockIdx.x * WL_THREADS + threadIdx.x;
   if (i < A.n_sel)
-    worklist_walk(A, i, true, [&](uint32_t, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &d, bool first_in_group, uint32_t tp) {
+    worklist_walk(A, A.walk ? __ldg(A.walk + i) : i, true, [&](uint32_t, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &d, bool first_in_group, uint32_t tp) {
       atomicAdd(&s_hist[bin * A.n_cols + qc], 1u);
       // the reader metrics (page_read_count / page_read_bytes) count the time page once per column group
       unsigned long long bytes = d.size, pages = 1;
@@ -459,8 +471,9 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_emit(const WorkListArgs
   for (uint32_t k = threadIdx.x; k < 2 * n_buckets; k += WL_THREADS) s_hist[k] = 0;
   __syncthreads();
   const uint32_t i = blockIdx.x * WL_THREADS + threadIdx.x;
+  const uint32_t slot = (i < A.n_sel && A.walk) ? __ldg(A.walk + i) : i;
   if (i < A.n_sel)
-    worklist_walk(A, i, false, [&](uint32_t, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &, bool, uint32_t) {
+    worklist_walk(A, slot, false, [&](uint32_t, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &, bool, uint32_t) {
       atomicAdd(&s_base[bin * A.n_cols + qc], 1u);
     });
   __syncthreads();
@@ -468,11 +481,11 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_emit(const WorkListArgs
     if (s_base[k]) s_base[k] = A.bucket_off[k] + atomicAdd(&A.bucket_count[k], s_base[k]);
   __syncthreads();
   if (i < A.n_sel)
-    worklist_walk(A, i, false, [&](uint32_t page, uint32_t bin, uint32_t qc, bool with_time, const tskv_page_desc &, bool, uint32_t) {
+    worklist_walk(A, slot, false, [&](uint32_t page, uint32_t bin, uint32_t qc, bool with_time, const tskv_page_desc &, bool, uint32_t) {
       const uint32_t key = bin * A.n_cols + qc;
       const uint32_t pos = s_base[key] + atomicAdd(&s_cur[key], 1u);
       A.work_page[pos] = page;
-      A.work_slot[pos] = i;
+      A.work_slot[pos] = slot;
       A.work_qcol[pos] = (uint8_t)(qc | (with_time ? 0x80 : 0));
     });
 }
@@ -1098,7 +1111,6 @@ __device__ __forceinline__ void scan_chunk_rows(const ScanParams &P, uint32_t it
   uint32_t n_points = 0, n_inrange = 0;
   const bool is_f64 = pt == TSKV_PT_F64;
   const bool mean_hi = !is_f64 && (mask & TSKV_AGG_MEAN);
-  const uint64_t group_base = P.group_by_series ? (uint64_t)slot * P.n_buckets : 0;
 
   for (;;) {
     const bool has = row < n_rows;
@@ -1152,7 +1164,7 @@ __device__ __forceinline__ void scan_chunk_rows(const ScanParams &P, uint32_t it
     } else {
       flush = have_run;
     }
-    warp_flush<SEL>(P, stab, flush, qcol, group_base + run_idx, (int64_t)run_idx, pt, mask, acc, slot);
+    warp_flush<SEL>(P, stab, flush, qcol, group_cell_base(P, slot) + run_idx, (int64_t)run_idx, pt, mask, acc, slot);
     if (flush) have_run = false;
     if (has && inr) {
       if (newrun) {
@@ -1332,7 +1344,8 @@ __device__ __forceinline__ void flush_runs(const ScanParams &P, uint64_t *stab, 
   const uint64_t gcell = ((uint64_t)qcol << 32) | (uint32_t)cell;
   const int leader = __ffs(m) - 1;
   const uint64_t lcell = shfl_u64(gcell, leader);
-  // (GROUP BY bucket only: cells of a per-series grouping can exceed 32 bits, and its lanes never share one.) The staged
+  // (Not for GROUP BY series: its cells can exceed 32 bits, and its lanes never share one. GROUP BY tags keeps its cells
+  // below 2^32, and its lanes share a cell whenever their series share a group.) The staged
   // path also serves tables too large for shared memory - the reduced partial then goes to the global state with one
   // atomic per quantity instead of 32 contended ones.
   const bool same = !P.group_by_series && __all_sync(FULL, !active || gcell == lcell);
@@ -1474,7 +1487,9 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   uint32_t kword = 0xffffffffu;                        // row-filter bits of the same 32 rows (all ones without predicates)
   bool first_pending = false;                          // FIRST/LAST: the run has not seen a kept row yet
   const uint64_t flip = pt == TSKV_PT_U64 ? 0x8000000000000000ull : 0ull;
-  const uint64_t group_base = P.group_by_series ? (uint64_t)slot * P.n_buckets : 0;
+  // (the FIRST / LAST variants read the slot and its group again at each flush: holding them takes registers those
+  // kernels do not have, ptxas spills)
+  const uint64_t group_base = SEL ? 0 : group_cell_base(P, slot);
   uint32_t staged = 0;  // staged flush slots in use (warp-uniform)
 
   // Finished runs of the flushing lanes -> partial tables.
@@ -1483,7 +1498,8 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
     if (SEL) {
       if (__any_sync(FULL, flush)) {
         acc.count = va.count; acc.sum = va.sum; acc.sum_hi = va.sum_hi; acc.kmin = va.kmin; acc.kmax = va.kmax;
-        warp_flush<SEL>(P, stab, flush, qcol, group_base + run_idx, (int64_t)run_idx, pt, mask, acc, slot);
+        const uint32_t fslot = have_item ? __ldg(P.work_slot + item) : 0u;
+        warp_flush<SEL>(P, stab, flush, qcol, group_cell_base(P, fslot) + run_idx, (int64_t)run_idx, pt, mask, acc, fslot);
       }
     } else {
       flush_runs<VK>(P, stab, stage, staged, flush, qcol, group_base + run_idx, pt, mask, va);
@@ -1563,7 +1579,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
     fast = __all_sync(FULL, elig);
   }
 
-  // ---- Uniform schedule (RLE timestamps, GROUP BY bucket, no FIRST / LAST). When every lane that holds rows starts at
+  // ---- Uniform schedule (RLE timestamps, GROUP BY bucket or tags, no FIRST / LAST). When every lane that holds rows starts at
   // the same row and time, steps by the same delta, has the same range rows [ra, rb1), the same bucket state and the same
   // query column (TSBS-aligned pages: 80 % of C4's), the bucket edges fall on the same rows in every lane. The warp then
   // walks ONE schedule, the leader's: per bitmap word one dense / sparse vote, per bucket its rows and one staged store
@@ -1576,12 +1592,14 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
     const uint32_t with_rows = __ballot_sync(FULL, mine);
     const int src = with_rows ? __ffs(with_rows) - 1 : 0;
     const uint64_t t_first = rle_t0 + (uint64_t)row * rle_delta;
-    // (`&`, not `&&`: every lane must reach every shuffle)
+    // (`&`, not `&&`: every lane must reach every shuffle. GROUP BY tags: the lanes' groups agree too, and a group's
+    // cells stay below 2^32)
     const bool agree = (shfl_u64(rle_delta, src) == rle_delta) & (shfl_u64(t_first, src) == t_first) &
                        (shfl_u64(e_off, src) == e_off) & (__shfl_sync(FULL, row, src) == row) &
                        (__shfl_sync(FULL, n_rows, src) == n_rows) & (__shfl_sync(FULL, ra, src) == ra) &
                        (__shfl_sync(FULL, rb1, src) == rb1) & (__shfl_sync(FULL, bidx, src) == bidx) &
-                       (__shfl_sync(FULL, nb, src) == nb) & (__shfl_sync(FULL, qcol, src) == qcol);
+                       (__shfl_sync(FULL, nb, src) == nb) & (__shfl_sync(FULL, qcol, src) == qcol) &
+                       (__shfl_sync(FULL, (uint32_t)group_base, src) == (uint32_t)group_base);
     if (with_rows && __all_sync(FULL, !mine || agree)) {
       // the leader's schedule in every lane (lanes without rows may hold other values)
       rle_delta = shfl_u64(rle_delta, src);
@@ -1593,7 +1611,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
       rb1 = __shfl_sync(FULL, rb1, src);
       bidx = __shfl_sync(FULL, bidx, src);
       nb = __shfl_sync(FULL, nb, src);
-      const uint64_t col = (uint64_t)__shfl_sync(FULL, qcol, src) << 32;
+      const uint64_t col = ((uint64_t)__shfl_sync(FULL, qcol, src) << 32) | __shfl_sync(FULL, (uint32_t)group_base, src);
       uint32_t end = __shfl_sync(FULL, n_rows, src);
       while (row < end) {  // one bitmap word per pass (`row` is a multiple of 32 here)
         if (n_rows) {      // this lane still decodes: take the prefetched word, prefetch the next
@@ -1651,7 +1669,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           if (n_rows) check_values();
           if (in && (nb == 0 || r == rb1)) {  // the bucket's last row: its partial goes to the staging area
             va.fold(pt);
-            stage_partial<VK>(P, stab, stage, staged, n_rows && va.count, va, lane == 0, col | bidx);
+            stage_partial<VK>(P, stab, stage, staged, n_rows && va.count, va, lane == 0, col + bidx);
             va.reset();
           }
         }
@@ -1662,7 +1680,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   }
 
   // The warp walks its 32 pages SEGMENT by segment (a segment = rows of one page sharing (selected, bucket)), and for
-  // GROUP BY bucket it keeps the lanes aligned on the BUCKET: in every iteration only the lanes whose next selected
+  // GROUP BY bucket / tags it keeps the lanes aligned on the BUCKET: in every iteration only the lanes whose next selected
   // segment lies in the smallest pending bucket go ahead (the others keep their segment pending, at most an iteration
   // or two). Pages whose first row falls just before a bucket edge would otherwise run one segment ahead of their
   // neighbours for the whole page, no two lanes would ever finish a run for the same cell in the same iteration, and

@@ -7,6 +7,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <numeric>
 #include <string>
 #include <thread>
 #include <vector>
@@ -191,6 +192,9 @@ struct tskv_scan {
   uint64_t *d_pane_state = nullptr;
   CombineOp *d_combine = nullptr;
   uint32_t n_combine = 0, win_k = 1, n_panes = 0, n_windows = 0;
+  // GROUP BY tags: the group of every slot (params.slot_group) and the work-list walk order, slots sorted by group (null
+  // when that is the selection order)
+  uint32_t *d_slot_group = nullptr, *d_walk = nullptr;
 };
 
 namespace {
@@ -336,13 +340,36 @@ void ensure_page_stats(tskv_ctx *ctx, const tskv_pages *pg) {
   pg->d_page_stats = d;
 }
 
-tskv_status compute_layout(const tskv_pages *pages, const tskv_query *q, tskv_output_layout *out) {
+// GROUP BY tags (the *_grouped entry points): group of every selected series slot, and the number of groups.
+struct TagGroups {
+  bool on = false;
+  const uint32_t *ids = nullptr;
+  uint32_t n = 0;
+};
+
+uint64_t selected_slots(const tskv_pages *pages, const tskv_query *q) { return q->series_ids ? q->n_series : pages->series.size(); }
+
+// Why a group map is refused (TSKV_ERR_INVALID_ARG), or null.
+const char *tag_groups_refusal(const tskv_pages *pages, const tskv_query *q, const TagGroups &tg) {
+  if (!tg.on) return nullptr;
+  if (!tg.ids || tg.n == 0) return "GROUP BY tags: group_ids must be non-null and n_groups >= 1";
+  if (q->group_by_series) return "GROUP BY tags: group_by_series must be 0 (the group map replaces it)";
+  if ((uint64_t)tg.n * q->n_buckets > TSKV_MAX_GROUPED_CELLS) return "GROUP BY tags: n_groups x n_buckets exceeds TSKV_MAX_GROUPED_CELLS";
+  const uint64_t n_slots = selected_slots(pages, q);
+  for (uint64_t i = 0; i < n_slots; i++)
+    if (tg.ids[i] >= tg.n) return "GROUP BY tags: a group id is >= n_groups";
+  return nullptr;
+}
+
+tskv_status compute_layout(const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, tskv_output_layout *out) {
   if (!pages || !q || !out || q->n_buckets == 0 || q->n_columns == 0 || !q->columns) return TSKV_ERR_INVALID_ARG;
   if (q->width <= 0 && q->n_buckets != 1) return TSKV_ERR_INVALID_ARG;
+  if (tag_groups_refusal(pages, q, tg)) return TSKV_ERR_INVALID_ARG;
   uint64_t n_out = 0;
   for (uint32_t c = 0; c < q->n_columns; c++) n_out += popc8(q->columns[c].agg_mask);
   uint64_t n_groups = 1;
-  if (q->group_by_series) n_groups = q->series_ids ? q->n_series : pages->series.size();
+  if (q->group_by_series) n_groups = selected_slots(pages, q);
+  if (tg.on) n_groups = tg.n;
   out->n_out = n_out;
   out->n_groups = n_groups;
   out->n_cells = n_groups * q->n_buckets;
@@ -465,7 +492,8 @@ void free_scan(tskv_scan *s) {
   void *bufs[] = {s->d_series, s->d_rank_slot, s->d_bucket, s->d_cg_slot, s->d_item_flag, s->d_block_count, s->d_work_page, s->d_work_slot,
                   s->d_work_qcol, s->d_bin_cstart, s->d_cols, s->d_outs, s->d_means, s->d_state,
                   s->d_task_counter, s->d_values, s->d_validity, s->d_gor_scratch[0], s->d_gor_scratch[1], s->d_gathered, s->d_row_keep,
-                  s->d_mcg_active, s->d_mvals, s->d_mvalid, s->d_mpage, s->d_mrow_off, s->d_mbm_off, s->d_pane_state, s->d_combine};
+                  s->d_mcg_active, s->d_mvals, s->d_mvalid, s->d_mpage, s->d_mrow_off, s->d_mbm_off, s->d_pane_state, s->d_combine,
+                  s->d_slot_group, s->d_walk};
   for (void *b : bufs)
     if (b) cudaFreeAsync(b, st);
   if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
@@ -1259,7 +1287,12 @@ tskv_status tskvgpu_decode_pages(tskv_ctx *ctx, const tskv_pages *pages, uint64_
 // ------------------------------------------------------------------------------------------------
 tskv_status tskvgpu_query_output_layout(const tskv_pages *pages, const tskv_query *q,
                                         tskv_output_layout *out) {
-  return compute_layout(pages, q, out);
+  return compute_layout(pages, q, TagGroups{}, out);
+}
+
+tskv_status tskvgpu_query_output_layout_grouped(const tskv_pages *pages, const tskv_query *q, const uint32_t *group_ids,
+                                                uint32_t n_groups, tskv_output_layout *out) {
+  return compute_layout(pages, q, TagGroups{true, group_ids, n_groups}, out);
 }
 
 // Sliding windows of `q` (window q->width, slide < q->width) by panes: the refusals of tskvgpu_scan_prepare_sliding
@@ -1319,14 +1352,19 @@ static tskv_status check_sliding(tskv_ctx *ctx, const tskv_pages *pages, const t
   return TSKV_OK;
 }
 
-// tskvgpu_scan_prepare; slide > 0: tskvgpu_scan_prepare_sliding with slide < width.
-static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide, tskv_scan **out_scan) {
+// tskvgpu_scan_prepare; slide > 0: tskvgpu_scan_prepare_sliding with slide < width; tg.on: GROUP BY tags.
+static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
+                                const TagGroups &tg, tskv_scan **out_scan) {
   if (!ctx || !pages || !q || !out_scan) return TSKV_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(ctx->mu);
   ctx->set_error("");
   *out_scan = nullptr;
+  if (const char *why = tag_groups_refusal(pages, q, tg)) {
+    ctx->set_error(why);
+    return TSKV_ERR_INVALID_ARG;
+  }
   tskv_output_layout L;
-  tskv_status st = compute_layout(pages, q, &L);
+  tskv_status st = compute_layout(pages, q, tg, &L);
   if (st != TSKV_OK) {
     ctx->set_error("invalid query (buckets / columns)");
     return st;
@@ -1368,10 +1406,10 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
         return TSKV_ERR_INVALID_ARG;
       }
   if ((q->reserved & TSKV_QUERY_MULTI_RANK) && !q->series_ids) {
-    bool needs_slots = q->group_by_series != 0;
+    bool needs_slots = q->group_by_series != 0 || tg.on;
     for (uint32_t c = 0; c < q->n_columns; c++) needs_slots |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
     if (needs_slots) {
-      ctx->set_error("multi-rank scan: GROUP BY series and first/last need the global series_ids list (slots are positions in it)");
+      ctx->set_error("multi-rank scan: GROUP BY series / tags and first/last need the global series_ids list (slots are positions in it)");
       return TSKV_ERR_INVALID_ARG;
     }
   }
@@ -1515,6 +1553,29 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
       e = cudaMemcpyAsync(s->d_series, q->series_ids, (size_t)q->n_series * 4, cudaMemcpyHostToDevice, ctx->stream);
     h2d += (uint64_t)q->n_series * 4;
   }
+  if (tg.on) {  // GROUP BY tags: the group map, and the slots in group order for the work-list walk
+    const uint64_t n_slots = selected_slots(pages, q);
+    std::vector<uint32_t> walk;
+    if (!std::is_sorted(tg.ids, tg.ids + n_slots)) {  // (already in group order: the walk stays the selection order)
+      walk.resize(n_slots);
+      if (tg.n <= n_slots) {  // stable counting sort
+        std::vector<uint32_t> next(tg.n + 1, 0);
+        for (uint64_t i = 0; i < n_slots; i++) next[tg.ids[i] + 1]++;
+        for (uint32_t g = 0; g < tg.n; g++) next[g + 1] += next[g];
+        for (uint64_t i = 0; i < n_slots; i++) walk[next[tg.ids[i]]++] = (uint32_t)i;
+      } else {
+        std::iota(walk.begin(), walk.end(), 0u);
+        std::stable_sort(walk.begin(), walk.end(), [&](uint32_t a, uint32_t b) { return tg.ids[a] < tg.ids[b]; });
+      }
+    }
+    if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_slot_group, n_slots);
+    if (e == cudaSuccess && n_slots)
+      e = cudaMemcpyAsync(s->d_slot_group, tg.ids, (size_t)n_slots * 4, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess && !walk.empty()) e = stream_alloc(ctx, &s->d_walk, n_slots);
+    if (e == cudaSuccess && !walk.empty())
+      e = cudaMemcpyAsync(s->d_walk, walk.data(), (size_t)n_slots * 4, cudaMemcpyHostToDevice, ctx->stream);
+    h2d += (n_slots + walk.size()) * 4;
+  }
   if (e == cudaSuccess && q->series_ids) e = stream_alloc(ctx, &s->d_rank_slot, pages->series.size());
   if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_bucket, (size_t)2 * N_BINS * q->n_columns + 1);
   {
@@ -1604,10 +1665,11 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   P.n_buckets = s->n_panes;
   P.group_by_series = q->group_by_series;
   P.n_cells = kern_cells;
+  P.slot_group = s->d_slot_group;
   P.slot_bits = slot_bits;
   P.slot_max = slot_bits ? (uint32_t)((1ull << slot_bits) - 1) : 0;
   P.rel_base = rel_base;
-  // per-CTA shared-memory partial table (GROUP BY bucket): count | sum | hi | min | max per column
+  // per-CTA shared-memory partial table (GROUP BY bucket / tags): count | sum | hi | min | max per column
   {
     uint32_t words = 0;
     for (uint32_t c = 0; c < q->n_columns; c++) {
@@ -1893,11 +1955,11 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
 }
 
 tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, tskv_scan **out_scan) {
-  return prepare_scan(ctx, pages, q, 0, out_scan);
+  return prepare_scan(ctx, pages, q, 0, TagGroups{}, out_scan);
 }
 
-tskv_status tskvgpu_scan_prepare_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
-                                         tskv_scan **out_scan) {
+static tskv_status prepare_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
+                                   const TagGroups &tg, tskv_scan **out_scan) {
   if (!ctx || !pages || !q || !out_scan) return TSKV_ERR_INVALID_ARG;
   if (slide <= 0 || q->width <= 0) {
     std::lock_guard<std::mutex> lock(ctx->mu);
@@ -1905,7 +1967,18 @@ tskv_status tskvgpu_scan_prepare_sliding(tskv_ctx *ctx, const tskv_pages *pages,
     *out_scan = nullptr;
     return TSKV_ERR_INVALID_ARG;
   }
-  return prepare_scan(ctx, pages, q, slide == q->width ? 0 : slide, out_scan);  // slide == window: a tumbling window
+  return prepare_scan(ctx, pages, q, slide == q->width ? 0 : slide, tg, out_scan);  // slide == window: a tumbling window
+}
+
+tskv_status tskvgpu_scan_prepare_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
+                                         tskv_scan **out_scan) {
+  return prepare_sliding(ctx, pages, q, slide, TagGroups{}, out_scan);
+}
+
+tskv_status tskvgpu_scan_prepare_grouped(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const uint32_t *group_ids,
+                                         uint32_t n_groups, int64_t slide, tskv_scan **out_scan) {
+  const TagGroups tg{true, group_ids, n_groups};
+  return slide ? prepare_sliding(ctx, pages, q, slide, tg, out_scan) : prepare_scan(ctx, pages, q, 0, tg, out_scan);
 }
 
 // Enqueues one full pass on the context stream, no host synchronisation:
@@ -1980,6 +2053,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     A.n_set_series = (uint32_t)pages->series.size();
     A.series_ids = s->d_series;
     A.n_sel = s->d_series ? s->n_series_sel : (uint32_t)pages->series.size();
+    A.walk = s->d_walk;
     A.cols = s->d_cols;
     A.n_cols = s->n_cols;
     A.cg_bounds = s->prune.n ? pages->d_cg_bounds : nullptr;
@@ -2328,10 +2402,10 @@ void tskvgpu_scan_destroy(tskv_ctx *ctx, tskv_scan *s) {
 }
 
 static tskv_status scan_aggregate(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
-                                  uint64_t *out_values, uint8_t *out_validity) {
+                                  const TagGroups &tg, uint64_t *out_values, uint8_t *out_validity) {
   if (!out_values || !out_validity) return TSKV_ERR_INVALID_ARG;
   tskv_scan *s = nullptr;
-  tskv_status st = slide ? tskvgpu_scan_prepare_sliding(ctx, pages, q, slide, &s) : tskvgpu_scan_prepare(ctx, pages, q, &s);
+  tskv_status st = slide ? prepare_sliding(ctx, pages, q, slide, tg, &s) : prepare_scan(ctx, pages, q, 0, tg, &s);
   if (st != TSKV_OK) return st;
   st = tskvgpu_scan_run(ctx, s);
   if (st == TSKV_OK) st = tskvgpu_scan_finalize(ctx, s, out_values, out_validity);
@@ -2342,7 +2416,7 @@ static tskv_status scan_aggregate(tskv_ctx *ctx, const tskv_pages *pages, const 
 
 tskv_status tskvgpu_scan_aggregate(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q,
                                    uint64_t *out_values, uint8_t *out_validity) {
-  return scan_aggregate(ctx, pages, q, 0, out_values, out_validity);
+  return scan_aggregate(ctx, pages, q, 0, TagGroups{}, out_values, out_validity);
 }
 
 tskv_status tskvgpu_scan_aggregate_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
@@ -2353,7 +2427,12 @@ tskv_status tskvgpu_scan_aggregate_sliding(tskv_ctx *ctx, const tskv_pages *page
     ctx->set_error("sliding windows: slide and window must be > 0");
     return TSKV_ERR_INVALID_ARG;
   }
-  return scan_aggregate(ctx, pages, q, slide, out_values, out_validity);
+  return scan_aggregate(ctx, pages, q, slide, TagGroups{}, out_values, out_validity);
+}
+
+tskv_status tskvgpu_scan_aggregate_grouped(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const uint32_t *group_ids,
+                                           uint32_t n_groups, int64_t slide, uint64_t *out_values, uint8_t *out_validity) {
+  return scan_aggregate(ctx, pages, q, slide, TagGroups{true, group_ids, n_groups}, out_values, out_validity);
 }
 
 }  // extern "C"

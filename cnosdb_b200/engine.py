@@ -363,23 +363,44 @@ class Engine:
             bo += b
         return out
 
-    def output_layout(self, pages, query):
+    @staticmethod
+    def _group_map(group_ids, n_groups):
+        """GROUP BY tags arguments: (pointer or None, n_groups, array kept alive), or None for an ungrouped call.
+        n_groups defaults to max(group_ids) + 1."""
+        if group_ids is None and n_groups is None:
+            return None
+        ids = None if group_ids is None else np.ascontiguousarray(group_ids, dtype=np.uint32)
+        if n_groups is None:
+            n_groups = int(ids.max()) + 1 if ids is not None and ids.size else 1
+        return (None if ids is None else ids.ctypes.data), int(n_groups), ids
+
+    def output_layout(self, pages, query, group_ids=None, n_groups=None):
         L = cabi.OutputLayout()
         q = query.to_c()
-        st = self.lib.tskvgpu_query_output_layout(pages.handle, C.byref(q), C.byref(L))
+        g = self._group_map(group_ids, n_groups)
+        if g is None:
+            st = self.lib.tskvgpu_query_output_layout(pages.handle, C.byref(q), C.byref(L))
+        else:
+            st = self.lib.tskvgpu_query_output_layout_grouped(pages.handle, C.byref(q), g[0], g[1], C.byref(L))
         if st != cabi.TSKV_OK:
             raise TskvError(st, "invalid query")
         return L
 
-    def scan_aggregate(self, pages, query, slide=None):
+    def scan_aggregate(self, pages, query, slide=None, group_ids=None, n_groups=None):
         """End-to-end call: query args H2D, fused scan, result D2H (BatchReader::process analogue).
         slide: sliding windows time_window(time, query.width, slide, query.origin); output bucket j is the window
-        starting at query.first_bucket_start + j * slide (sliding_window_grid sizes that grid)."""
-        L = self.output_layout(pages, query)
+        starting at query.first_bucket_start + j * slide (sliding_window_grid sizes that grid).
+        group_ids: GROUP BY tags, group_ids[slot] = group of the slot-th selected series (n_groups groups, default
+        max + 1; the result has one row of buckets per group)."""
+        L = self.output_layout(pages, query, group_ids, n_groups)
         values = np.empty(int(L.n_out * L.n_cells), dtype=np.uint64)
         bitmaps = np.empty(int(L.validity_bytes), dtype=np.uint8)
+        g = self._group_map(group_ids, n_groups)
         q = query.to_c()
-        if slide is None:
+        if g is not None:
+            st = self.lib.tskvgpu_scan_aggregate_grouped(self.ctx, pages.handle, C.byref(q), g[0], g[1], int(slide or 0),
+                                                         values.ctypes.data, bitmaps.ctypes.data)
+        elif slide is None:
             st = self.lib.tskvgpu_scan_aggregate(self.ctx, pages.handle, C.byref(q), values.ctypes.data, bitmaps.ctypes.data)
         else:
             st = self.lib.tskvgpu_scan_aggregate_sliding(self.ctx, pages.handle, C.byref(q), int(slide),
@@ -387,12 +408,15 @@ class Engine:
         self._check(st)
         return ScanResult(query, L, values, bitmaps)
 
-    def prepare(self, pages, query, slide=None):
-        """Device-resident scan (run / enqueue / partials / exchange / finalize); slide: as in scan_aggregate."""
-        L = self.output_layout(pages, query)
+    def prepare(self, pages, query, slide=None, group_ids=None, n_groups=None):
+        """Device-resident scan (run / enqueue / partials / exchange / finalize); slide, group_ids: as in scan_aggregate."""
+        L = self.output_layout(pages, query, group_ids, n_groups)
+        g = self._group_map(group_ids, n_groups)
         q = query.to_c()
         h = C.c_void_p()
-        if slide is None:
+        if g is not None:
+            st = self.lib.tskvgpu_scan_prepare_grouped(self.ctx, pages.handle, C.byref(q), g[0], g[1], int(slide or 0), C.byref(h))
+        elif slide is None:
             st = self.lib.tskvgpu_scan_prepare(self.ctx, pages.handle, C.byref(q), C.byref(h))
         else:
             st = self.lib.tskvgpu_scan_prepare_sliding(self.ctx, pages.handle, C.byref(q), int(slide), C.byref(h))

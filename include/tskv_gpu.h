@@ -175,7 +175,7 @@ typedef struct tskv_query {
  * so a shim can wrap each output column zero-copy as an Arrow array. */
 typedef struct tskv_output_layout {
   uint64_t n_out;         /* number of output columns */
-  uint64_t n_groups;      /* 1, or number of series slots when group_by_series */
+  uint64_t n_groups;      /* 1, number of series slots when group_by_series, or n_groups of a *_grouped call */
   uint64_t n_cells;       /* n_groups * n_buckets */
   uint64_t bitmap_stride; /* bytes per validity bitmap, multiple of 8 */
   uint64_t values_bytes;  /* n_out * n_cells * 8 */
@@ -399,6 +399,28 @@ tskv_status tskvgpu_scan_prepare_sliding(tskv_ctx *ctx, const tskv_pages *pages,
                                          int64_t slide, tskv_scan **out_scan);
 tskv_status tskvgpu_scan_aggregate_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q,
                                            int64_t slide, uint64_t *out_values, uint8_t *out_validity);
+
+/* ---- GROUP BY <tags>[, bucket] ---------------------------------------------------------------
+ * Tags are not stored in pages: SeriesReader appends them per series from the SeriesKey (tskv/src/reader/series.rs:
+ * 55-90,146-154), so grouping by a set of tags is a grouping of series the host knows before the scan.
+ * group_ids[slot] in [0, n_groups) is the group of the slot-th selected series (q->series_ids order; every series of the
+ * page set in ascending id order when series_ids == NULL). Output cell c = group * n_buckets + bucket. A group's cell
+ * aggregates every selected row of every series in the group that falls in the bucket / window; FIRST / LAST pick the
+ * group's earliest / latest row, ties to the lower slot (the keys and budget of the ungrouped scan), so group g's result
+ * equals the ungrouped scan whose series_ids are g's members. A group without a selected row reads like an empty bucket.
+ * slide == 0 or slide == q->width: tumbling buckets; otherwise the sliding windows (and every refusal) of
+ * tskvgpu_scan_prepare_sliding. The scan returned works with every tskvgpu_scan_* call above; multi-rank scans
+ * (TSKV_QUERY_MULTI_RANK) pass the same global series_ids and the same group_ids on every rank.
+ * Refused before any launch with TSKV_ERR_INVALID_ARG: group_ids == NULL, n_groups == 0, a group id >= n_groups,
+ * q->group_by_series != 0, or n_groups * n_buckets > TSKV_MAX_GROUPED_CELLS. */
+#define TSKV_MAX_GROUPED_CELLS 0xffffffffu
+tskv_status tskvgpu_query_output_layout_grouped(const tskv_pages *pages, const tskv_query *q,
+                                                const uint32_t *group_ids, uint32_t n_groups, tskv_output_layout *out);
+tskv_status tskvgpu_scan_prepare_grouped(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q,
+                                         const uint32_t *group_ids, uint32_t n_groups, int64_t slide, tskv_scan **out);
+tskv_status tskvgpu_scan_aggregate_grouped(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q,
+                                           const uint32_t *group_ids, uint32_t n_groups, int64_t slide,
+                                           uint64_t *out_values, uint8_t *out_validity);
 
 /* Library version / build info ("tskv-b200 <semver> sm_90a"). */
 const char *tskvgpu_version(void);

@@ -111,19 +111,31 @@ impl GpuEngine {
     /// The end-to-end call a `BatchReader::process()` makes: query arguments H2D, fused scan, dense result D2H.
     pub fn scan_aggregate(&self, pages: &PageSet<'_>, q: &Query) -> GpuResult<AggregateResult> {
         let raw = q.as_raw();
-        let mut layout = sys::tskv_output_layout::default();
-        self.check(unsafe { sys::tskvgpu_query_output_layout(pages.pages, &raw, &mut layout) })?;
+        let layout = self.output_layout(pages, q, &raw)?;
         let mut values = vec![0u64; (layout.n_out * layout.n_cells) as usize];
         let mut validity = vec![0u8; layout.validity_bytes as usize];
         self.check(unsafe {
-            match q.slide {
-                None => sys::tskvgpu_scan_aggregate(self.ctx, pages.pages, &raw, values.as_mut_ptr(), validity.as_mut_ptr()),
-                Some(slide) => {
+            match (&q.groups, q.slide) {
+                (Some((ids, n)), slide) => sys::tskvgpu_scan_aggregate_grouped(
+                    self.ctx, pages.pages, &raw, ids.as_ptr(), *n, slide.unwrap_or(0), values.as_mut_ptr(), validity.as_mut_ptr()),
+                (None, None) => sys::tskvgpu_scan_aggregate(self.ctx, pages.pages, &raw, values.as_mut_ptr(), validity.as_mut_ptr()),
+                (None, Some(slide)) => {
                     sys::tskvgpu_scan_aggregate_sliding(self.ctx, pages.pages, &raw, slide, values.as_mut_ptr(), validity.as_mut_ptr())
                 }
             }
         })?;
         Ok(AggregateResult { layout, values, validity })
+    }
+
+    fn output_layout(&self, pages: &PageSet<'_>, q: &Query, raw: &sys::tskv_query) -> GpuResult<sys::tskv_output_layout> {
+        let mut layout = sys::tskv_output_layout::default();
+        self.check(unsafe {
+            match &q.groups {
+                Some((ids, n)) => sys::tskvgpu_query_output_layout_grouped(pages.pages, raw, ids.as_ptr(), *n, &mut layout),
+                None => sys::tskvgpu_query_output_layout(pages.pages, raw, &mut layout),
+            }
+        })?;
+        Ok(layout)
     }
 
     /// Multi-GPU: this engine's rank in an NCCL communicator (collective: every rank calls it with rank 0's id).
@@ -135,13 +147,15 @@ impl GpuEngine {
     /// partial state with one ncclAllGather inside the library and finalises the merged result.
     pub fn scan_aggregate_sharded(&self, pages: &PageSet<'_>, q: &Query) -> GpuResult<AggregateResult> {
         let raw = q.as_raw();
-        let mut layout = sys::tskv_output_layout::default();
-        self.check(unsafe { sys::tskvgpu_query_output_layout(pages.pages, &raw, &mut layout) })?;
+        let layout = self.output_layout(pages, q, &raw)?;
         let mut scan = std::ptr::null_mut();
         self.check(unsafe {
-            match q.slide {
-                None => sys::tskvgpu_scan_prepare(self.ctx, pages.pages, &raw, &mut scan),
-                Some(slide) => sys::tskvgpu_scan_prepare_sliding(self.ctx, pages.pages, &raw, slide, &mut scan),
+            match (&q.groups, q.slide) {
+                (Some((ids, n)), slide) => {
+                    sys::tskvgpu_scan_prepare_grouped(self.ctx, pages.pages, &raw, ids.as_ptr(), *n, slide.unwrap_or(0), &mut scan)
+                }
+                (None, None) => sys::tskvgpu_scan_prepare(self.ctx, pages.pages, &raw, &mut scan),
+                (None, Some(slide)) => sys::tskvgpu_scan_prepare_sliding(self.ctx, pages.pages, &raw, slide, &mut scan),
             }
         })?;
         let mut values = vec![0u64; (layout.n_out * layout.n_cells) as usize];
@@ -234,6 +248,9 @@ pub struct Query {
     /// `first_bucket_start + j * slide`; `None` = tumbling buckets of `width`
     pub slide: Option<i64>,
     pub group_by_series: bool,
+    /// GROUP BY tags: (group id of every selected series slot, number of groups); output cell = group * n_buckets +
+    /// bucket. The shim derives dense ids from the `SeriesKey` tag values (INTEGRATION.md section 6).
+    pub groups: Option<(Vec<u32>, u32)>,
     pub columns: Vec<tskv_agg_column>,
     pub predicates: Vec<tskv_field_predicate>,
     pub multi_rank: bool,

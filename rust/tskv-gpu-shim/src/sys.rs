@@ -36,6 +36,7 @@ pub const TSKV_UPLOAD_HOST_RESIDENT: u32 = 2;
 pub const TSKV_UPLOAD_VERIFY_ON_READ: u32 = 4;
 pub const TSKV_TOMB_ALL: u32 = 0xffff_ffff;
 pub const TSKV_QUERY_MULTI_RANK: u32 = 1;
+pub const TSKV_MAX_GROUPED_CELLS: u64 = 0xffff_ffff;
 pub const TSKV_MAX_PREDICATES: usize = 8;
 pub const TSKV_NCCL_UNIQUE_ID_BYTES: usize = 128;
 
@@ -281,6 +282,32 @@ extern "C" {
         ctx: *mut tskv_ctx,
         pages: *const tskv_pages,
         q: *const tskv_query,
+        slide: i64,
+        out_values: *mut u64,
+        out_validity: *mut u8,
+    ) -> tskv_status;
+    pub fn tskvgpu_query_output_layout_grouped(
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        group_ids: *const u32,
+        n_groups: u32,
+        out: *mut tskv_output_layout,
+    ) -> tskv_status;
+    pub fn tskvgpu_scan_prepare_grouped(
+        ctx: *mut tskv_ctx,
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        group_ids: *const u32,
+        n_groups: u32,
+        slide: i64,
+        out_scan: *mut *mut tskv_scan,
+    ) -> tskv_status;
+    pub fn tskvgpu_scan_aggregate_grouped(
+        ctx: *mut tskv_ctx,
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        group_ids: *const u32,
+        n_groups: u32,
         slide: i64,
         out_values: *mut u64,
         out_validity: *mut u8,
