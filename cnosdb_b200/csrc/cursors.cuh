@@ -548,7 +548,7 @@ struct S8bCursor {
     }
   }
 
-  __device__ __forceinline__ uint64_t next() {
+  __device__ __forceinline__ void refill() {
     if (in_word == 0) {
       w = bs.next();
       const uint32_t sel = (uint32_t)(w >> 60);
@@ -561,10 +561,26 @@ struct S8bCursor {
       }
     }
     in_word--;
+  }
+  __device__ __forceinline__ uint64_t next() {
+    refill();
     const uint64_t u = (w & mask) | ones;
     w >>= bits;  // bits <= 60
     v += ZZ ? (uint64_t)zigzag_dec(u) : u * scaler;
     return v;
+  }
+  // next() in 32-bit arithmetic (ZZ only), for pages whose values all sign-extend from their low 32 bits: returns the
+  // value's low word. The running value's low word is the sum of the deltas' low words mod 2^32, and the low word of
+  // zigzag_dec(u) depends only on bits 0..32 of u (a 60-bit code included). The high word of `v` goes stale.
+  __device__ __forceinline__ uint32_t next32() {
+    static_assert(ZZ, "next32: zig-zag deltas only");
+    refill();
+    const uint32_t lo = ((uint32_t)w & (uint32_t)mask) | ones;
+    const uint32_t b32 = (uint32_t)(w >> 32) & (uint32_t)(mask >> 32);  // bit 32 of the code
+    w >>= bits;
+    const uint32_t v32 = (uint32_t)v + (__funnelshift_r(lo, b32, 1) ^ (0u - (lo & 1u)));
+    v = (v & 0xffffffff00000000ull) | v32;
+    return v32;
   }
 };
 

@@ -115,6 +115,10 @@ struct ScanParams {
   const SkipEntry *skip;
   uint32_t bin_parts[N_BINS];
   uint32_t bin_part_rows[N_BINS];
+  // page_narrow[page] = 1: every value of the simple8b integer page lies in [-2^31, 2^31) (i64) or [0, 2^31) (u64)
+  // (k_build_skip, from the decoded values; null or 0: not known). Chunks whose pages are all narrow accumulate in 32-bit
+  // arithmetic.
+  const uint8_t *page_narrow;
 };
 
 // First cell of the group a work item's series belongs to: GROUP BY tags slot_group[slot], GROUP BY series the slot
@@ -304,12 +308,15 @@ __global__ void k_flag_items(const tskv_page_desc *descs, const uint4 *item_info
 // their field pages, so the cost follows the selection (C4: 10 % of the series) instead of the page set. Two passes
 // over the same walk - count per (decode-kind bin, query column) bucket, then place - with a block-local histogram in
 // shared memory so that the global atomics are one per (block, bucket). Inside a bucket the order is arbitrary (the
-// fused kernels only need warps that are homogeneous in codec and, for GROUP BY bucket, in column).
+// fused kernels only need warps that are homogeneous in codec and, for GROUP BY bucket, in column). A (bin, column)
+// bucket is split in two by the page's narrow flag (WL_SUB buckets, ScanParams.page_narrow): its wide pages come first,
+// then its narrow ones, so that all chunks of the bucket but the one across the boundary are uniformly narrow or wide.
 // Same outputs as k_flag_items / k_scan_blocks / k_scatter_items: work_page / work_slot / work_qcol (bit 7 = "brings
 // the column group's time page": the first selected field page of each value class of a group), bin_cstart, the
 // reader counters, statistics pruning.
 // ------------------------------------------------------------------------------------------------
 constexpr int WL_THREADS = 256;
+constexpr uint32_t WL_SUB = 2;  // work-list buckets per (bin, query column): wide pages, narrow pages
 struct WorkListArgs {
   const tskv_page_desc *descs;
   uint64_t n_descs;
@@ -318,6 +325,7 @@ struct WorkListArgs {
   const uint32_t *rank_cg_start; // [n_set_series + 1] CSR: column groups of the series with this rank
   const uint32_t *rank_cg;
   const uint8_t *page_bin;       // [n_descs] decode-kind bin of a field page
+  const uint8_t *page_narrow;    // [n_descs] narrow flags (null: every page is wide)
   const uint32_t *set_series;    // the page set's distinct series ids, ascending
   uint32_t n_set_series;
   const uint32_t *series_ids;    // the selection (null: every series, slot = rank)
@@ -332,13 +340,18 @@ struct WorkListArgs {
   const uint8_t *cg_merge;       // column groups of overlapping chunks go through the merge pass
   const int64_t *page_stats;     // value-statistics pruning against `preds` (null: none)
   PredicateSet preds;
-  uint32_t *bucket_count;        // [N_BINS * n_cols] totals (pass 1), then running cursors (pass 2)
-  uint32_t *bucket_off;          // [N_BINS * n_cols + 1] exclusive offsets (k_worklist_offsets)
+  uint32_t *bucket_count;        // [N_BINS * n_cols * WL_SUB] totals (pass 1), then running cursors (pass 2)
+  uint32_t *bucket_off;          // [N_BINS * n_cols * WL_SUB + 1] exclusive offsets (k_worklist_offsets)
   uint32_t *work_page, *work_slot;
   uint8_t *work_qcol;
   unsigned long long *counters;  // [0] pages [1] bytes [2 + bin] bytes per bin [2 + N_BINS] pruned pages
   int32_t *status;
 };
+
+// Work-list bucket of a page: (bin, query column, narrow flag).
+__device__ __forceinline__ uint32_t worklist_key(const WorkListArgs &A, uint32_t page, uint32_t bin, uint32_t qc) {
+  return (bin * A.n_cols + qc) * WL_SUB + ((A.page_narrow && A.page_narrow[page]) ? 1u : 0u);
+}
 
 // Walks the items of selected series i; F(page, bin, qcol, with_time, desc).
 template <typename F>
@@ -392,17 +405,17 @@ __device__ __forceinline__ void worklist_walk(const WorkListArgs &A, uint32_t i,
 
 // Pass 1: bucket totals + the reader counters.
 __global__ void __launch_bounds__(WL_THREADS) k_worklist_count(const WorkListArgs A) {
-  extern __shared__ uint32_t s_hist[];  // [N_BINS * n_cols]
+  extern __shared__ uint32_t s_hist[];  // [N_BINS * n_cols * WL_SUB]
   __shared__ unsigned long long s_pages, s_bytes[N_BINS];
-  const uint32_t n_buckets = N_BINS * A.n_cols;
+  const uint32_t n_buckets = N_BINS * A.n_cols * WL_SUB;
   for (uint32_t k = threadIdx.x; k < n_buckets; k += WL_THREADS) s_hist[k] = 0;
   if (threadIdx.x == 0) s_pages = 0;
   if (threadIdx.x < N_BINS) s_bytes[threadIdx.x] = 0;
   __syncthreads();
   const uint32_t i = blockIdx.x * WL_THREADS + threadIdx.x;
   if (i < A.n_sel)
-    worklist_walk(A, A.walk ? __ldg(A.walk + i) : i, true, [&](uint32_t, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &d, bool first_in_group, uint32_t tp) {
-      atomicAdd(&s_hist[bin * A.n_cols + qc], 1u);
+    worklist_walk(A, A.walk ? __ldg(A.walk + i) : i, true, [&](uint32_t page, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &d, bool first_in_group, uint32_t tp) {
+      atomicAdd(&s_hist[worklist_key(A, page, bin, qc)], 1u);
       // the reader metrics (page_read_count / page_read_bytes) count the time page once per column group
       unsigned long long bytes = d.size, pages = 1;
       if (first_in_group) { bytes += A.descs[tp].size; pages += 1; }
@@ -419,11 +432,12 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_count(const WorkListArg
   }
 }
 
-// Exclusive offsets of the buckets (bin-major), bin_cstart, and the cursors reset for pass 2. One block.
-__global__ void k_worklist_offsets(uint32_t *bucket_count, uint32_t *bucket_off, uint32_t n_cols, uint32_t *bin_cstart) {
+// Exclusive offsets of the buckets (bin-major, `per_bin` buckets per bin), bin_cstart, and the cursors reset for pass 2.
+// One block.
+__global__ void k_worklist_offsets(uint32_t *bucket_count, uint32_t *bucket_off, uint32_t per_bin, uint32_t *bin_cstart) {
   __shared__ uint32_t s_carry;
   __shared__ uint32_t s_warp[32];
-  const uint32_t n_buckets = N_BINS * n_cols;
+  const uint32_t n_buckets = N_BINS * per_bin;
   if (threadIdx.x == 0) s_carry = 0;
   __syncthreads();
   for (uint32_t base = 0; base < n_buckets; base += blockDim.x) {
@@ -450,7 +464,7 @@ __global__ void k_worklist_offsets(uint32_t *bucket_count, uint32_t *bucket_off,
     if (k < n_buckets) {
       bucket_off[k] = excl;
       bucket_count[k] = 0;  // pass 2's cursor
-      if (k % n_cols == 0) bin_cstart[k / n_cols] = excl;
+      if (k % per_bin == 0) bin_cstart[k / per_bin] = excl;
     }
     __syncthreads();
     if (threadIdx.x == blockDim.x - 1) s_carry = excl + v;
@@ -465,16 +479,16 @@ __global__ void k_worklist_offsets(uint32_t *bucket_count, uint32_t *bucket_off,
 
 // Pass 2: the same walk; a block reserves its share of every bucket with one atomic and places its items inside it.
 __global__ void __launch_bounds__(WL_THREADS) k_worklist_emit(const WorkListArgs A) {
-  extern __shared__ uint32_t s_hist[];  // [2][N_BINS * n_cols]: block counts -> block bases, and the running cursors
-  const uint32_t n_buckets = N_BINS * A.n_cols;
+  extern __shared__ uint32_t s_hist[];  // [2][N_BINS * n_cols * WL_SUB]: block counts -> block bases, and the running cursors
+  const uint32_t n_buckets = N_BINS * A.n_cols * WL_SUB;
   uint32_t *s_base = s_hist, *s_cur = s_hist + n_buckets;
   for (uint32_t k = threadIdx.x; k < 2 * n_buckets; k += WL_THREADS) s_hist[k] = 0;
   __syncthreads();
   const uint32_t i = blockIdx.x * WL_THREADS + threadIdx.x;
   const uint32_t slot = (i < A.n_sel && A.walk) ? __ldg(A.walk + i) : i;
   if (i < A.n_sel)
-    worklist_walk(A, slot, false, [&](uint32_t, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &, bool, uint32_t) {
-      atomicAdd(&s_base[bin * A.n_cols + qc], 1u);
+    worklist_walk(A, slot, false, [&](uint32_t page, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &, bool, uint32_t) {
+      atomicAdd(&s_base[worklist_key(A, page, bin, qc)], 1u);
     });
   __syncthreads();
   for (uint32_t k = threadIdx.x; k < n_buckets; k += WL_THREADS)
@@ -482,7 +496,7 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_emit(const WorkListArgs
   __syncthreads();
   if (i < A.n_sel)
     worklist_walk(A, slot, false, [&](uint32_t page, uint32_t bin, uint32_t qc, bool with_time, const tskv_page_desc &, bool, uint32_t) {
-      const uint32_t key = bin * A.n_cols + qc;
+      const uint32_t key = worklist_key(A, page, bin, qc);
       const uint32_t pos = s_base[key] + atomicAdd(&s_cur[key], 1u);
       A.work_page[pos] = page;
       A.work_slot[pos] = slot;
@@ -1221,7 +1235,22 @@ struct ValueAcc {  // count / sum / min / max of one run; VK fixes the arithmeti
   uint64_t sum;    // f64: the sum's bits. Integers, while accumulating: sum of the values' LOW 32-bit halves
   int64_t sum_hi;  // integers, while accumulating: sum of the HIGH halves (sign- / zero-extended); see fold()
   int64_t kmin, kmax;
-  __device__ __forceinline__ void reset() { count = 0; sum = 0; sum_hi = 0; kmin = INT64_MAX; kmax = INT64_MIN; }
+  // Narrow runs (add32: integer values that sign-extend from their low 32 bits) keep `sum` = the exact 64-bit sum of the
+  // values (|sum| < 2^63 for 2^32 rows) and the 32-bit min / max in the LOW words of kmin / kmax; fold(pt, true) turns
+  // them into the wide run's (sum, sum_hi, keys). A run is narrow or wide from reset to fold.
+  __device__ __forceinline__ void reset(bool narrow = false) {
+    count = 0; sum = 0; sum_hi = 0;
+    kmin = narrow ? INT32_MAX : INT64_MAX;
+    kmax = narrow ? INT32_MIN : INT64_MIN;
+  }
+  __device__ __forceinline__ static int64_t with_lo(int64_t x, int32_t lo) {
+    return (int64_t)(((uint64_t)x & 0xffffffff00000000ull) | (uint32_t)lo);
+  }
+  __device__ __forceinline__ void add32(uint32_t v) {
+    sum += (uint64_t)(int64_t)(int32_t)v;
+    kmin = with_lo(kmin, min((int32_t)kmin, (int32_t)v));
+    kmax = with_lo(kmax, max((int32_t)kmax, (int32_t)v));
+  }
   // pt / flip are per-lane constants (flip = okey's xor mask for integer columns).
   // Integer sums are kept as two 64-bit accumulators of 32-bit halves: exact for 2^32 rows without any carry
   // bookkeeping per value (the wrapping SUM and the exact 128-bit sum MEAN needs both fall out of fold()).
@@ -1240,8 +1269,15 @@ struct ValueAcc {  // count / sum / min / max of one run; VK fixes the arithmeti
   }
   // End of the run: integers -> (sum, sum_hi) = low / high word of the exact 128-bit sum (sum = the reference's wrapping
   // i64 / u64 SUM). Call once, right before the partial is handed to a flush.
-  __device__ __forceinline__ void fold(uint8_t pt) {
+  __device__ __forceinline__ void fold(uint8_t pt, bool narrow = false) {
     if (VK == VK_GOR || (VK == VK_GEN && pt == TSKV_PT_F64)) return;
+    if (narrow) {  // u64 values of a narrow run lie in [0, 2^31): their sum is >= 0 like the i64 sign extension says
+      const uint64_t flip = pt == TSKV_PT_U64 ? 0x8000000000000000ull : 0ull;
+      sum_hi = (int64_t)sum >> 63;
+      kmin = (int64_t)((uint64_t)(int64_t)(int32_t)kmin ^ flip);
+      kmax = (int64_t)((uint64_t)(int64_t)(int32_t)kmax ^ flip);
+      return;
+    }
     const uint64_t x = (uint64_t)sum_hi << 32;
     const uint64_t lo = x + sum;
     sum_hi = (pt == TSKV_PT_I64 ? (sum_hi >> 32) : (int64_t)((uint64_t)sum_hi >> 32)) + (lo < x ? 1 : 0);
@@ -1377,7 +1413,9 @@ __device__ __forceinline__ uint32_t rle_rows_within(uint64_t d, uint64_t delta, 
   return (uint32_t)min((uint64_t)left, q + 1);
 }
 
-template <int TK, int VK, bool SEL>
+// NARROW (simple8b integer values, no FIRST / LAST): every page of the chunk is narrow (ScanParams.page_narrow), so the
+// values are decoded and accumulated in 32-bit arithmetic (S8bCursor::next32, ValueAcc::add32).
+template <int TK, int VK, bool SEL, bool NARROW>
 __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t item_begin, uint32_t item_end,
                                                uint32_t ring_base, uint64_t *stab, uint64_t *stage,
                                                uint32_t part, uint32_t n_parts, uint32_t part_rows) {
@@ -1473,8 +1511,9 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   const bool to_page_end = n_rows == page_rows;  // this lane reaches the end of the page's streams
   ring_drain();  // the rings' initial fills have landed before the first step (once per page)
 
+  static_assert(!NARROW || (VK == VK_S8B && !SEL), "narrow chunks: simple8b integer values, no FIRST / LAST");
   ValueAcc<VK> va;
-  va.reset();
+  va.reset(NARROW);
   RunAcc acc;  // flush image (+ first/last state when SEL)
   acc.first_ts = acc.last_ts = 0; acc.first_val = acc.last_val = 0; acc.first_ok = acc.last_ok = false;
   BucketState bk; bk.valid = false; bk.floor_regime = false; bk.lo = 0; bk.hi = 0; bk.idx = 0;
@@ -1494,7 +1533,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
 
   // Finished runs of the flushing lanes -> partial tables.
   auto flush_now = [&](bool flush) {
-    if (flush) va.fold(pt);
+    if (flush) va.fold(pt, NARROW);
     if (SEL) {
       if (__any_sync(FULL, flush)) {
         acc.count = va.count; acc.sum = va.sum; acc.sum_hi = va.sum_hi; acc.kmin = va.kmin; acc.kmax = va.kmax;
@@ -1517,11 +1556,26 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
     kept = (kword >> (row & 31)) & 1;
     uint64_t v = 0;
     if (vv) {
-      v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
       n_points++;
-      if (accumulate && kept) { va.count++; va.add(v, pt, flip); }
+      if constexpr (NARROW) {
+        const uint32_t v32 = vcur_d.next32();
+        if (accumulate && kept) { va.count++; va.add32(v32); }
+      } else {
+        v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
+        if (accumulate && kept) { va.count++; va.add(v, pt, flip); }
+      }
     }
-    return v;
+    return v;  // (0 for narrow chunks: only FIRST / LAST use it)
+  };
+  // The next value, accumulated when `take` (every value is decoded: the streams are sequential).
+  auto next_add = [&](bool take) {
+    if constexpr (NARROW) {
+      const uint32_t v32 = vcur_d.next32();
+      if (take) va.add32(v32);
+    } else {
+      const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
+      if (take) va.add(v, pt, flip);
+    }
   };
   auto check_values = [&]() {
     const bool bad = VK == VK_GOR ? vcur_g.failed() : cursor_exhausted(vcur_d);
@@ -1654,23 +1708,17 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           va.count += __popc(tp);
           if (dense) {
 #pragma unroll 1
-            for (uint32_t n = __popc(mp); n; n--) {
-              const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
-              va.add(v, pt, flip);
-            }
+            for (uint32_t n = __popc(mp); n; n--) next_add(true);
           } else {  // only the rows holding a value
 #pragma unroll 1
-            for (uint32_t b = mp; b; b &= b - 1) {
-              const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
-              if (tp & b & (0u - b)) va.add(v, pt, flip);
-            }
+            for (uint32_t b = mp; b; b &= b - 1) next_add(tp & b & (0u - b));
           }
           r = pend;
           if (n_rows) check_values();
           if (in && (nb == 0 || r == rb1)) {  // the bucket's last row: its partial goes to the staging area
-            va.fold(pt);
+            va.fold(pt, NARROW);
             stage_partial<VK>(P, stab, stage, staged, n_rows && va.count, va, lane == 0, col + bidx);
-            va.reset();
+            va.reset(NARROW);
           }
         }
         row = r;
@@ -1769,7 +1817,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
     if (newrun) {
       have_run = true;
       run_idx = seg_b;
-      va.reset();
+      va.reset(NARROW);
       if (SEL) { acc.first_ok = acc.last_ok = false; first_pending = true; }
     }
     // ---- 3. the segment's rows --------------------------------------------------------------------------
@@ -1802,16 +1850,10 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
             // same result, so which lanes the vote sees only decides the speed.)
             if (__all_sync(__activemask(), take == m)) {
 #pragma unroll 1
-              for (uint32_t n = __popc(m); n; n--) {
-                const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
-                va.add(v, pt, flip);
-              }
+              for (uint32_t n = __popc(m); n; n--) next_add(true);
             } else {  // only the rows holding a value
 #pragma unroll 1
-              for (uint32_t b = m; b; b &= b - 1) {
-                const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
-                if (take & b & (0u - b)) va.add(v, pt, flip);
-              }
+              for (uint32_t b = m; b; b &= b - 1) next_add(take & b & (0u - b));
             }
           } else {  // FIRST / LAST wanted: the run's first and last KEPT rows keep (ts, value, valid)
             for (uint32_t j = 0; j < span; j++) {
@@ -1896,8 +1938,13 @@ __host__ __device__ constexpr uint32_t scan_ring_bytes_per_warp(int tk) {
 __host__ __device__ constexpr uint32_t scan_warp_bytes(int tk) {
   return tk == TK_GEN ? 0 : scan_ring_bytes_per_warp(tk) + FLUSH_STAGE_BYTES;
 }
-template <int TK, int VK, bool SEL>
+// Narrow pages of a simple8b-value bin (ScanParams.page_narrow), per page set: none, some or all of them. NARROW_SOME
+// kernels choose per chunk; NARROW_ALL kernels hold the narrow arithmetic only (a kernel that holds both row loops runs
+// its narrow chunks ~1.5 % slower on C4: H100, see DESIGN.md §5).
+enum { NARROW_NONE = 0, NARROW_SOME = 1, NARROW_ALL = 2 };
+template <int TK, int VK, bool SEL, int NARROW>
 __global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, SEL)) k_scan_aggregate(const __grid_constant__ ScanParams P, int bin) {
+  static_assert(NARROW == NARROW_NONE || (TK != TK_GEN && VK == VK_S8B && !SEL), "narrow kernels: simple8b values, no FIRST / LAST");
   // dynamic shared memory: [per-CTA partial table, P.smem_words 8-byte words (or empty)] [staging rings, per warp:
   // a value ring, preceded by a time ring when the timestamps are simple8b]
   extern __shared__ __align__(16) uint64_t s_tab[];
@@ -1931,8 +1978,17 @@ __global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, SEL)) k_scan
     const uint32_t part = c - group * n_parts;
     const uint32_t begin = begin0 + (group << 5);
     const uint32_t end = min(begin + 32, end0);
-    if constexpr (TK == TK_GEN) scan_chunk_rows<TK, VK, SEL>(P, begin, end, ring_base, s_tab);
-    else scan_chunk_seg<TK, VK, SEL>(P, begin, end, ring_base, s_tab, stage, part, n_parts, part_rows);
+    if constexpr (TK == TK_GEN) {
+      scan_chunk_rows<TK, VK, SEL>(P, begin, end, ring_base, s_tab);
+    } else if constexpr (NARROW == NARROW_SOME) {
+      // 32-bit arithmetic when all of the chunk's pages are narrow (the work list keeps a bin's narrow pages together)
+      const uint32_t item = begin + lane;
+      const bool narrow = __all_sync(FULL, item >= end || __ldg(P.page_narrow + __ldg(P.work_page + item)));
+      if (narrow) scan_chunk_seg<TK, VK, SEL, true>(P, begin, end, ring_base, s_tab, stage, part, n_parts, part_rows);
+      else scan_chunk_seg<TK, VK, SEL, false>(P, begin, end, ring_base, s_tab, stage, part, n_parts, part_rows);
+    } else {
+      scan_chunk_seg<TK, VK, SEL, NARROW == NARROW_ALL>(P, begin, end, ring_base, s_tab, stage, part, n_parts, part_rows);
+    }
   }
   if (P.use_smem) {  // merge this CTA's table into the global state, once
     __syncthreads();

@@ -100,6 +100,11 @@ struct tskv_pages {
   uint32_t *d_skip_off = nullptr;
   SkipEntry *d_skip = nullptr;
   uint64_t n_skip = 0;
+  // per page 1 = a simple8b integer page whose values all lie in [-2^31, 2^31) (i64) / [0, 2^31) (u64) (k_build_skip;
+  // null for host-resident page sets: every page is then wide), and per bin whether none, some or all of its pages are
+  // narrow (NARROW_*: which variant of the fused kernel runs the bin)
+  uint8_t *d_narrow = nullptr;
+  uint8_t h_bin_narrow[N_BINS]{};
   uint32_t h_bin_maxrows[N_BINS]{};  // longest field page of each bin (parts per page when a scan cuts the bin's pages)
   // overlapping chunks (tskvgpu_pages_set_chunk_files, merge_kernels.cuh): the plan, its device copies and the merge
   // rows' timestamps (decoded once); the epoch invalidates scans prepared before a change
@@ -128,7 +133,7 @@ struct tskv_scan {
   // device buffers
   uint32_t *d_series = nullptr;
   int32_t *d_rank_slot = nullptr;  // rank of a series in the page set -> position in the selection list (or -1)
-  uint32_t *d_bucket = nullptr;    // selection-driven work list: [N_BINS * n_cols] counts / cursors | [.. + 1] offsets
+  uint32_t *d_bucket = nullptr;    // selection-driven work list: [N_BINS * n_cols * WL_SUB] counts / cursors | [.. + 1] offsets
   bool worklist_by_items = false;  // TSKV_WORKLIST=items: the round-1 pass over every field page of the page set
   int32_t *d_cg_slot = nullptr;
   uint8_t *d_item_flag = nullptr;
@@ -234,18 +239,26 @@ unsigned bits_for(uint64_t max_value) {  // bits needed to represent values in [
 unsigned popc8(unsigned x) { return (unsigned)__builtin_popcount(x & TSKV_AGG_ALL); }
 
 typedef void (*scan_kernel_t)(const ScanParams, int);
+// `narrow`: NARROW_* of the bin's pages (tskv_pages::h_bin_narrow); only the simple8b-value kernels without FIRST / LAST
+// have narrow variants
 template <bool SEL>
-scan_kernel_t scan_kernel_for(int bin) {
+scan_kernel_t scan_kernel_for(int bin, int narrow = NARROW_NONE) {
+  if constexpr (!SEL) {
+    if (narrow == NARROW_SOME && bin == TK_RLE * N_VK + VK_S8B) return k_scan_aggregate<TK_RLE, VK_S8B, false, NARROW_SOME>;
+    if (narrow == NARROW_SOME && bin == TK_S8B * N_VK + VK_S8B) return k_scan_aggregate<TK_S8B, VK_S8B, false, NARROW_SOME>;
+    if (narrow == NARROW_ALL && bin == TK_RLE * N_VK + VK_S8B) return k_scan_aggregate<TK_RLE, VK_S8B, false, NARROW_ALL>;
+    if (narrow == NARROW_ALL && bin == TK_S8B * N_VK + VK_S8B) return k_scan_aggregate<TK_S8B, VK_S8B, false, NARROW_ALL>;
+  }
   switch (bin) {
-    case TK_RLE * N_VK + VK_S8B: return k_scan_aggregate<TK_RLE, VK_S8B, SEL>;
-    case TK_RLE * N_VK + VK_GOR: return k_scan_aggregate<TK_RLE, VK_GOR, SEL>;
-    case TK_RLE * N_VK + VK_GEN: return k_scan_aggregate<TK_RLE, VK_GEN, SEL>;
-    case TK_S8B * N_VK + VK_S8B: return k_scan_aggregate<TK_S8B, VK_S8B, SEL>;
-    case TK_S8B * N_VK + VK_GOR: return k_scan_aggregate<TK_S8B, VK_GOR, SEL>;
-    case TK_S8B * N_VK + VK_GEN: return k_scan_aggregate<TK_S8B, VK_GEN, SEL>;
-    case TK_GEN * N_VK + VK_S8B: return k_scan_aggregate<TK_GEN, VK_S8B, SEL>;
-    case TK_GEN * N_VK + VK_GOR: return k_scan_aggregate<TK_GEN, VK_GOR, SEL>;
-    default: return k_scan_aggregate<TK_GEN, VK_GEN, SEL>;
+    case TK_RLE * N_VK + VK_S8B: return k_scan_aggregate<TK_RLE, VK_S8B, SEL, NARROW_NONE>;
+    case TK_RLE * N_VK + VK_GOR: return k_scan_aggregate<TK_RLE, VK_GOR, SEL, NARROW_NONE>;
+    case TK_RLE * N_VK + VK_GEN: return k_scan_aggregate<TK_RLE, VK_GEN, SEL, NARROW_NONE>;
+    case TK_S8B * N_VK + VK_S8B: return k_scan_aggregate<TK_S8B, VK_S8B, SEL, NARROW_NONE>;
+    case TK_S8B * N_VK + VK_GOR: return k_scan_aggregate<TK_S8B, VK_GOR, SEL, NARROW_NONE>;
+    case TK_S8B * N_VK + VK_GEN: return k_scan_aggregate<TK_S8B, VK_GEN, SEL, NARROW_NONE>;
+    case TK_GEN * N_VK + VK_S8B: return k_scan_aggregate<TK_GEN, VK_S8B, SEL, NARROW_NONE>;
+    case TK_GEN * N_VK + VK_GOR: return k_scan_aggregate<TK_GEN, VK_GOR, SEL, NARROW_NONE>;
+    default: return k_scan_aggregate<TK_GEN, VK_GEN, SEL, NARROW_NONE>;
   }
 }
 // relative cost of one item of a bin (sizes the bins' shares of the SMs)
@@ -667,7 +680,7 @@ tskv_status tskvgpu_ctx_create(int32_t device_id, tskv_ctx **out_ctx) {
         cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes);
     };
     for (int b = 0; b < N_SERIAL_BINS; b++) {
-      raise((const void *)scan_kernel_for<false>(b));
+      for (int nm = NARROW_NONE; nm <= NARROW_ALL; nm++) raise((const void *)scan_kernel_for<false>(b, nm));
       raise((const void *)scan_kernel_for<true>(b));
     }
     for (int b = N_SERIAL_BINS; b < N_BINS; b++) {
@@ -926,9 +939,10 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
     pg->verify_on_read = true;  // like the reference: every read of a page re-checks its CRC (device side)
     e = up(&pg->d_crc_tables, crc32_tables(), 2048);
   }
-  // ---- restart points of the simple8b / gorilla pages (pages resident in HBM only) -----------------------
+  // ---- restart points of the simple8b / gorilla pages and narrow flags of the simple8b integer pages (pages resident in
+  // HBM only; the flags do not depend on TSKV_NO_SKIP) --------------------------------------------------------------
   const bool no_skip = getenv("TSKV_NO_SKIP") != nullptr;
-  if (e == cudaSuccess && !no_skip && !(flags & TSKV_UPLOAD_HOST_RESIDENT) && n_descs) {
+  if (e == cudaSuccess && !(flags & TSKV_UPLOAD_HOST_RESIDENT) && n_descs) {
     std::vector<uint32_t> skip_off(n_descs, SKIP_NONE), list[3];
     uint64_t n_skip = 0;
     for (uint64_t i = 0; i < n_descs; i++) {
@@ -937,17 +951,27 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
       if (d.phys_type == TSKV_PT_TIME) kind = (d.reserved == DK_S8B_SC && !time_has_nulls[i]) ? SKIP_KIND_TIME_S8B : -1;
       else if (d.reserved == DK_S8B_ZZ) kind = SKIP_KIND_VALUE_S8B;
       else if (d.reserved == DK_GORILLA) kind = SKIP_KIND_VALUE_GORILLA;
-      if (kind < 0 || d.num_values <= SKIP_ROWS || n_skip + d.num_values / SKIP_ROWS >= SKIP_NONE) continue;
-      skip_off[i] = (uint32_t)n_skip;
-      n_skip += (d.num_values - 1) / SKIP_ROWS;
+      if (kind < 0) continue;
+      if (!no_skip && d.num_values > SKIP_ROWS && n_skip + d.num_values / SKIP_ROWS < SKIP_NONE) {
+        skip_off[i] = (uint32_t)n_skip;
+        n_skip += (d.num_values - 1) / SKIP_ROWS;
+      } else if (kind != SKIP_KIND_VALUE_S8B) {
+        continue;
+      }
       list[kind].push_back((uint32_t)i);
+    }
+    if (!list[SKIP_KIND_VALUE_S8B].empty()) {
+      e = dev_alloc(&pg->d_narrow, n_descs);
+      if (e == cudaSuccess) e = cudaMemsetAsync(pg->d_narrow, 0, n_descs, ctx->stream);
     }
     if (n_skip) {
       pg->n_skip = n_skip;
-      e = up(&pg->d_skip_off, skip_off.data(), n_descs);
+      if (e == cudaSuccess) e = up(&pg->d_skip_off, skip_off.data(), n_descs);
       if (e == cudaSuccess) e = dev_alloc(&pg->d_skip, n_skip);
+    }
+    const size_t n_list = list[0].size() + list[1].size() + list[2].size();
+    if (n_list) {
       uint32_t *d_list = nullptr;
-      const size_t n_list = list[0].size() + list[1].size() + list[2].size();
       if (e == cudaSuccess) e = cudaMallocAsync(reinterpret_cast<void **>(&d_list), n_list * 4, ctx->stream);
       size_t lo = 0;
       for (int k = 0; k < 3 && e == cudaSuccess; k++) {
@@ -957,17 +981,29 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
         if (e != cudaSuccess) break;
         const uint32_t blocks = (n + SKIP_THREADS - 1) / SKIP_THREADS;
         if (k == SKIP_KIND_TIME_S8B)
-          k_build_skip<SKIP_KIND_TIME_S8B><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream>>>(pg->d_arena, pg->d_descs, d_list + lo, n, pg->d_skip_off, pg->d_skip);
+          k_build_skip<SKIP_KIND_TIME_S8B><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream>>>(pg->d_arena, pg->d_descs, d_list + lo, n, pg->d_skip_off, pg->d_skip, nullptr);
         else if (k == SKIP_KIND_VALUE_S8B)
-          k_build_skip<SKIP_KIND_VALUE_S8B><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream>>>(pg->d_arena, pg->d_descs, d_list + lo, n, pg->d_skip_off, pg->d_skip);
+          k_build_skip<SKIP_KIND_VALUE_S8B><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream>>>(pg->d_arena, pg->d_descs, d_list + lo, n, pg->d_skip_off, pg->d_skip, pg->d_narrow);
         else
-          k_build_skip<SKIP_KIND_VALUE_GORILLA><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream>>>(pg->d_arena, pg->d_descs, d_list + lo, n, pg->d_skip_off, pg->d_skip);
+          k_build_skip<SKIP_KIND_VALUE_GORILLA><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream>>>(pg->d_arena, pg->d_descs, d_list + lo, n, pg->d_skip_off, pg->d_skip, nullptr);
         lo += n;
       }
       if (e == cudaSuccess) e = cudaGetLastError();
       // the page lists are read by kernels still in flight: host vectors stay alive until the sync below
       if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
       if (d_list) cudaFreeAsync(d_list, ctx->stream);
+    }
+    if (e == cudaSuccess && pg->d_narrow) {
+      std::vector<uint8_t> narrow(n_descs);
+      e = cudaMemcpyAsync(narrow.data(), pg->d_narrow, n_descs, cudaMemcpyDeviceToHost, ctx->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+      uint64_t n_narrow[N_BINS] = {0}, n_pages[N_BINS] = {0};
+      for (uint32_t k = 0; k < pg->n_items; k++) {
+        n_narrow[page_bin[item_page[k]]] += narrow[item_page[k]];
+        n_pages[page_bin[item_page[k]]]++;
+      }
+      for (int b = 0; b < N_BINS; b++)
+        pg->h_bin_narrow[b] = n_narrow[b] == 0 ? NARROW_NONE : n_narrow[b] == n_pages[b] ? NARROW_ALL : NARROW_SOME;
     }
   }
   cudaEventRecord(ctx->ev1, ctx->stream);
@@ -993,6 +1029,7 @@ void tskvgpu_pages_destroy(tskv_ctx *ctx, tskv_pages *pg) {
   cudaFree(pg->d_arena);
   cudaFree(pg->d_skip_off);
   cudaFree(pg->d_skip);
+  cudaFree(pg->d_narrow);
   free_overlap(pg);
   cudaFree(pg->d_descs);
   cudaFree(pg->d_time_page_of);
@@ -1577,7 +1614,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
     h2d += (n_slots + walk.size()) * 4;
   }
   if (e == cudaSuccess && q->series_ids) e = stream_alloc(ctx, &s->d_rank_slot, pages->series.size());
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_bucket, (size_t)2 * N_BINS * q->n_columns + 1);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_bucket, (size_t)2 * N_BINS * q->n_columns * WL_SUB + 1);
   {
     // One thread walks ALL column groups of a selected series: right for many series with a few groups each (TSBS
     // shapes), serial for a handful of series with thousands of groups (one host over a year) - those take the pass
@@ -1692,6 +1729,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
     P.row_keep = s->d_row_keep;
     P.keep_off = pages->d_keep_off;
     P.skip_off = pages->d_skip_off;
+    P.page_narrow = pages->d_narrow;
     P.skip = pages->d_skip;
     for (int b = 0; b < N_BINS; b++) { P.bin_parts[b] = 1; P.bin_part_rows[b] = 0; }
     P.has_tomb = pages->n_tomb_ranges ? 1u : 0u;
@@ -1779,9 +1817,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
       int occ = 0;
       if (!s->use_coop[b]) {
         const int sb = serial_bin_of(b);
-        const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb));
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb),
-                                                      SCAN_THREADS, serial_smem_bytes(sb, P.smem_words));
+        const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, SCAN_THREADS, serial_smem_bytes(sb, P.smem_words));
       } else {
         const void *fn = coop_kernel_for(b, s->has_sel);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, SCAN_THREADS, coop_smem_bytes(b, P.smem_words));
@@ -2003,7 +2040,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
   {  // state identities + the pass's scratch (task counters / status / counters, bin starts, work-list buckets): one launch
     const uint32_t init_blocks = (uint32_t)std::min<uint64_t>((s->kern_sl.total + 255) / 256, 4096);
     k_init_state<<<std::max(1u, init_blocks), 256, 0, ctx->stream>>>(s->params.state, s->kern_sl, aux, 32, s->d_bin_cstart, N_BINS + 2,
-                                                                   s->d_bucket, N_BINS * s->n_cols);
+                                                                   s->d_bucket, N_BINS * s->n_cols * WL_SUB);
     launches++;
   }
   // slot of every column group: the row filter, the merge pass and the item-driven work list need it per GROUP; the
@@ -2049,6 +2086,9 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     A.rank_cg_start = pages->d_rank_cg_start;
     A.rank_cg = pages->d_rank_cg;
     A.page_bin = pages->d_page_bin;
+    // narrow pages apart only where a bin holds both kinds (NARROW_SOME kernels choose per chunk)
+    A.page_narrow = std::any_of(pages->h_bin_narrow, pages->h_bin_narrow + N_BINS, [](uint8_t m) { return m == NARROW_SOME; })
+                        ? pages->d_narrow : nullptr;
     A.set_series = pages->d_series_sorted;
     A.n_set_series = (uint32_t)pages->series.size();
     A.series_ids = s->d_series;
@@ -2061,7 +2101,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     A.cg_merge = pages->d_cg_merge;
     A.page_stats = s->preds.n ? pages->d_page_stats : nullptr;
     A.preds = s->preds;
-    const uint32_t n_buckets = N_BINS * s->n_cols;
+    const uint32_t n_buckets = N_BINS * s->n_cols * WL_SUB;
     A.bucket_count = s->d_bucket;
     A.bucket_off = s->d_bucket + n_buckets;
     A.work_page = s->d_work_page;
@@ -2071,7 +2111,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     A.status = s->d_status;
     const uint32_t wblocks = std::max(1u, (A.n_sel + WL_THREADS - 1) / WL_THREADS);
     if (A.n_sel) k_worklist_count<<<wblocks, WL_THREADS, n_buckets * 4, ctx->stream>>>(A);
-    k_worklist_offsets<<<1, 256, 0, ctx->stream>>>(s->d_bucket, s->d_bucket + n_buckets, s->n_cols, s->d_bin_cstart);
+    k_worklist_offsets<<<1, 256, 0, ctx->stream>>>(s->d_bucket, s->d_bucket + n_buckets, s->n_cols * WL_SUB, s->d_bin_cstart);
     if (A.n_sel) k_worklist_emit<<<wblocks, WL_THREADS, 2 * n_buckets * 4, ctx->stream>>>(A);
     launches += 3;
   }
@@ -2145,7 +2185,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     if (!s->use_coop[b]) {
       const int sb = serial_bin_of(b);
       void *args[] = {(void *)&s->params, (void *)&bin};
-      const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb));
+      const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
       CU_TRY(ctx, cudaLaunchKernel(fn, dim3(s->grid[b]), dim3(SCAN_THREADS), args, serial_smem_bytes(sb, s->params.smem_words), ctx->bin_stream[b]));
     } else {
       void *args[] = {(void *)&s->params, (void *)&s->coop, (void *)&bin};
