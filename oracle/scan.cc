@@ -31,7 +31,7 @@ inline void sliding_window(int64_t t, int64_t w, int64_t s, int64_t start_time, 
 }
 
 // Total order on f64 bit patterns (NaN handling of DataFusion min/max is unpinned in the
-// reference tree; generators never aggregate NaN).
+// reference tree; the f64 edge tests aggregate NaNs of both signs and check MIN / MAX under this order).
 inline int64_t f64_okey(uint64_t b) { return (int64_t)(b ^ (((int64_t)b >> 63) & 0x7fffffffffffffffll)); }
 
 inline bool less_typed(uint8_t pt, uint64_t a, uint64_t b) {

@@ -79,8 +79,9 @@ def make_query(fields, aggs=ALL_AGGS, **kw):
 
 # ---- exact reference ---------------------------------------------------------------------------------------------------
 # Aggregates computed from the generated arrays themselves (no page is decoded), so they share nothing with the oracle or
-# the kernels. Integer sums are exact Python ints; f64 sums come with an error bound that holds for any summation order.
-# FIRST / LAST are not restated here: compare those with the oracle.
+# the kernels. Integer sums are exact Python ints; f64 sums are a class that holds for any summation order starting from
+# +0.0 (NaN, an infinity, or finite with an error bound: f64_sum_class). FIRST / LAST are not restated here: compare those
+# with the oracle.
 
 I64_MIN, I64_MAX = -2**63, 2**63 - 1
 _U = 2.0 ** -53  # unit roundoff of f64
@@ -184,9 +185,49 @@ def gamma(k):
     return k * _U / (1 - k * _U)
 
 
+DBL_MAX = float(np.finfo(np.float64).max)
+_SCALE = 2.0 ** -64  # magnitudes are compared scaled, so that sums up to 2^1088 stay finite in the reference itself
+
+
+class OrderDependentSum(ValueError):
+    """An f64 cell whose class (finite, +-inf or NaN) depends on the summation order: arenas must not make one."""
+
+
+def f64_sum_class(x):
+    """-> (value, sum|x|) of the f64 SUM of the values x of one cell, the same in every summation order that starts
+    from +0.0:
+      NaN    if some value is NaN, or the cell holds both +inf and -inf;
+      +-inf  if it holds one sign of inf (and the finite values of the other sign cannot overflow), or when its finite
+             values all but have one sign and their exact sum is so large that no order stays finite;
+      finite otherwise, exactly rounded (math.fsum; +0.0 for a zero sum), when sum|x| (1 + gamma_{n-1}) <= DBL_MAX,
+             so that no partial sum of any order overflows (n: the nonzero values). Its error bound comes from sum|x|.
+    Raises OrderDependentSum for anything else."""
+    x = np.asarray(x, dtype=np.float64)
+    if np.isnan(x).any():
+        return math.nan, 0.0
+    pinf, ninf = bool((x == np.inf).any()), bool((x == -np.inf).any())
+    if pinf and ninf:
+        return math.nan, 0.0
+    f = x[np.isfinite(x)] * _SCALE  # (values below 2^-1010 lose bits here: far too little to move a threshold)
+    pos, neg = math.fsum(f[f > 0]), -math.fsum(f[f < 0])
+    g = 1 + gamma(max(np.count_nonzero(x) - 1, 0))  # (adding a zero is exact)
+    if pinf or ninf:
+        if (pos if ninf else neg) * g < DBL_MAX * _SCALE:
+            return (math.inf if pinf else -math.inf), 0.0
+        raise OrderDependentSum("one sign of inf, and finite values of the other sign that may overflow")
+    if (pos + neg) * g <= DBL_MAX * _SCALE:
+        s = math.fsum(x)
+        return (s if s != 0 else 0.0), math.fsum(np.abs(x))
+    s = pos - neg  # any finite result is within gamma_{n-1} (pos + neg) of s: when that is past DBL_MAX, none is finite
+    if abs(s) - (g - 1) * (pos + neg) > DBL_MAX * _SCALE and min(pos, neg) * g < DBL_MAX * _SCALE:
+        return math.copysign(math.inf, s), 0.0
+    raise OrderDependentSum("sum|x| = %g * 2^64 may overflow in some orders" % (pos + neg))
+
+
 class ExactResult:
     """Expected dense result: values[j, cell] (u64 bits) and validity[j, cell] like ScanResult. For f64 SUM / MEAN
-    `center[j]` holds the exactly rounded value (math.fsum) and `bound[j]` the largest error any summation order makes."""
+    `center[j]` holds the exactly rounded value (math.fsum) and `bound[j]` the largest error any summation order makes;
+    a NaN or infinite center (bound 0) is the class every order gives."""
 
     def __init__(self, query, n_groups):
         self.names = query.output_names()
@@ -261,15 +302,17 @@ def exact_aggregate(truth, query):
             parts = np.split(v[order], np.cumsum(count)[:-1].astype(np.int64))
             fs, ab = np.zeros(n_cells), np.zeros(n_cells)
             for k in live:
-                fs[k] = math.fsum(parts[k])
-                ab[k] = math.fsum(np.abs(parts[k]))
+                fs[k], ab[k] = f64_sum_class(parts[k])
             n = count.astype(np.float64)
-            # fsum is the exactly rounded sum: half an ulp more than gamma_{n-1} for the exact one
-            sb = gamma(np.maximum(n - 1, 0)) * ab * (1 + 2 * _U) + _U * np.abs(fs)
-            cen_mean = np.where(have, fs / np.maximum(n, 1), 0.0)
+            fin = np.isfinite(fs)
+            with np.errstate(invalid="ignore"):
+                # fsum is the exactly rounded sum: half an ulp more than gamma_{n-1} for the exact one
+                sb = np.where(fin, gamma(np.maximum(n - 1, 0)) * ab * (1 + 2 * _U) + _U * np.abs(fs), 0.0)
+                cen_mean = np.where(have, fs / np.maximum(n, 1), 0.0)
             sums = fs.view(np.uint64).copy()
             means = cen_mean.view(np.uint64).copy()
-            res_f64 = {"sum": (fs, sb), "mean": (cen_mean, sb / np.maximum(n, 1) + 2 * _U * np.abs(cen_mean))}
+            mb = np.where(fin, sb / np.maximum(n, 1) + 2 * _U * np.abs(np.where(fin, cen_mean, 0.0)), 0.0)
+            res_f64 = {"sum": (fs, sb), "mean": (cen_mean, mb)}
         else:
             # exact S from the 32-bit halves: |sum of halves| < 2^63 for < 2^31 rows per cell
             b = v.view(np.uint64)
@@ -300,7 +343,9 @@ def exact_aggregate(truth, query):
 
 def assert_matches_exact(got, exp, what="", int_mean=True):
     """got: ScanResult; exp: ExactResult. COUNT / integer SUM / MIN / MAX bit-exact, integer MEAN bit-exact
-    (= float(S) / float(n)) unless int_mean=False, f64 SUM / MEAN within the bound. FIRST / LAST are not checked."""
+    (= float(S) / float(n)) unless int_mean=False. f64 SUM / MEAN by class (f64_sum_class): a NaN cell must hold some
+    NaN (the payload depends on the order), an inf cell that inf, a finite cell a value within the bound, and a zero
+    +0.0. FIRST / LAST are not checked."""
     assert got.names == exp.names
     for j, (col, agg) in enumerate(got.names):
         if agg in ("first", "last") or (agg == "mean" and not int_mean and exp.phys[col] != cabi.TSKV_PT_F64):
@@ -309,11 +354,16 @@ def assert_matches_exact(got, exp, what="", int_mean=True):
         bad = np.nonzero(gv != ev)[0]
         assert bad.size == 0, "%s col %s %s: validity differs at cells %s" % (what, col, agg, bad[:5])
         if j in exp.center:
-            g = got.values[j].view(np.float64)[ev]
-            err = np.abs(g - exp.center[j][ev])
-            bad = np.nonzero(~(err <= exp.bound[j][ev]))[0]
-            assert bad.size == 0, "%s col %s %s: got %s, exact %s, bound %s" % (
-                what, col, agg, g[bad[:3]], exp.center[j][ev][bad[:3]], exp.bound[j][ev][bad[:3]])
+            cells = np.nonzero(ev)[0]
+            g, c, b = got.values[j].view(np.float64)[ev], exp.center[j][ev], exp.bound[j][ev]
+            nan, inf = np.isnan(c), np.isinf(c)
+            fin = ~(nan | inf)
+            with np.errstate(invalid="ignore"):
+                ok = np.where(nan, np.isnan(g), np.where(inf, g == c, np.abs(g - c) <= b))
+            ok &= ~(fin & (got.values[j][ev] == np.uint64(1 << 63)))  # a zero sum is +0.0
+            bad = np.nonzero(~ok)[0]
+            assert bad.size == 0, "%s col %s %s at cells %s: got %s, exact %s, bound %s" % (
+                what, col, agg, cells[bad[:3]], g[bad[:3]], c[bad[:3]], b[bad[:3]])
         else:
             g, e = got.values[j][ev], exp.values[j][ev]
             bad = np.nonzero(g != e)[0]
@@ -579,3 +629,174 @@ def geometry_queries(case, ranges, truth):
         ("unbucketed", make_query(GEOM_FIELDS, ALL_AGGS, time_ranges=ranges)),
         ("predicate", make_query(GEOM_FIELDS, GEOM_AGGS, time_ranges=ranges, predicates=pred, **grid)),
     ]
+
+
+# ---- f64 edge values ---------------------------------------------------------------------------------------------------
+# Arenas of f64 pages whose bit patterns reach the rare branches of the Gorilla decoders (meaningful = 64 written as 0,
+# leading zeros past the encoder's cap of 31, long runs of repeats, 77-bit elements) and whose values are IEEE special
+# values. Every column group holds column 1 (Gorilla) and column 2 (raw: the generic value kernels) with the same rows.
+# Four blocks of F64_BLOCK series, by their time pages:
+#   A  identical RLE timestamps (whole warps run the uniform bucket schedule);
+#   B  RLE timestamps starting sid % 7 rows later (the per-lane segment loop);
+#   C  jittered timestamps (simple8b time pages: the fused timestamp + value loop);
+#   D  block A's timestamps with the last row moved 2^61 ns later: a raw time page (the generic-time kernels, where the
+#      scan decodes Gorilla with GorillaCursor). Bucketed queries leave that row out with a time range.
+# The value kind of a series is sid % 10 (F64_KINDS). Rows 127-129 and 255-257 hold the hardest patterns, so that the
+# restart points (every 128 rows) and the cuts between page parts land on them.
+
+F64_FIELDS = ((1, cabi.TSKV_PT_F64), (2, cabi.TSKV_PT_F64))
+F64_BLOCK = 32
+F64_SERIES = 4 * F64_BLOCK
+F64_T0, F64_STEP = 10**12 + 17, 1000
+F64_LENGTHS = (1, 31, 32, 33, 127, 128, 129, 257, 4097)
+F64_KINDS = ("random", "signflip", "bit0_bit63", "runs", "small_xor", "specials", "okey_alone", "okey_mixed", "dbl_max",
+             "all_nan")
+GORILLA_EOS = 0x7FF80000000000FF  # the Gorilla end-of-stream marker: the encoder refuses it as a value
+OKEY_MAX, OKEY_MIN = 0x7FFFFFFFFFFFFFFF, 0xFFFFFFFFFFFFFFFF  # NaNs whose ordered keys are INT64_MAX / INT64_MIN
+F64_SPECIALS = np.array([
+    0x0000000000000000, 0x8000000000000000,  # +-0.0
+    0x7FF0000000000000, 0xFFF0000000000000,  # +-inf
+    0x0010000000000000, 0x8010000000000000,  # +-DBL_MIN
+    0x0000000000000001, 0x8000000000000001,  # +-2^-1074
+    0x000FFFFFFFFFFFFF,                      # the largest subnormal
+    0x7FF8000000000000, 0xFFF8000000000000,  # quiet NaNs
+    0x7FF0000000000001, 0xFFF4000000000000,  # signalling NaNs
+    0x7FF80000000000FE, 0x7FF8000000000100,  # the neighbours of GORILLA_EOS
+    OKEY_MAX, OKEY_MIN,
+], dtype=np.uint64)
+# Finite values are kept below 2^1000 so that no cell's sum|x| comes near DBL_MAX (f64_sum_class): only the dbl_max
+# series (+DBL_MAX or -DBL_MAX, one sign per series) overflow, in every order, wherever a cell holds two of their rows.
+
+
+def _clamp_exp(b):
+    """Random bit patterns -> finite values below 2^1000: an exponent field above 2022 loses its top bit."""
+    b = np.asarray(b, dtype=np.uint64)
+    big = ((b >> np.uint64(52)) & np.uint64(0x7FF)) > 2022
+    return np.where(big, b ^ np.uint64(1 << 62), b)
+
+
+def f64_kind(sid):
+    return F64_KINDS[sid % len(F64_KINDS)]
+
+
+def f64_edge_bits(rng, sid, n):
+    """The value bit patterns (uint64) of series `sid` with n rows."""
+    kind = f64_kind(sid)
+    r = rng.integers(0, 2**64, n, dtype=np.uint64, endpoint=False)
+    if kind == "random":
+        b = _clamp_exp(r)
+    elif kind == "signflip":  # consecutive values differ in bits 63 and 0: leading = 0, meaningful = 64
+        odd = (np.arange(n) & 1).astype(np.uint64)
+        b = (_clamp_exp(r) & ~np.uint64((1 << 63) | 1)) | (odd << np.uint64(63)) | odd
+    elif kind == "bit0_bit63":  # each row flips bit 0, bit 63 or nothing of the row before
+        flips = np.array([0, 1, 1 << 63], dtype=np.uint64)[rng.integers(0, 3, n)]
+        b = np.bitwise_xor.accumulate(np.concatenate([_clamp_exp(r[:1]), flips[1:]]))
+    elif kind == "runs":  # runs of 1 to 300 repeats, then a fresh value
+        starts = np.cumsum(rng.integers(1, 301, n))
+        b = _clamp_exp(r)[np.searchsorted(starts, np.arange(n), side="right")]
+    elif kind == "small_xor":  # XORs below 2^32: 32 to 63 leading zeros (past the cap of 31)
+        x = r >> np.uint64(32)
+        x >>= rng.integers(0, 32, n).astype(np.uint64)
+        b = np.bitwise_xor.accumulate(np.concatenate([_clamp_exp(r[:1]), x[1:]]))
+    elif kind == "specials":
+        norm = rng.normal(0, 1e3, n).view(np.uint64)
+        b = np.where(rng.random(n) < 0.6, F64_SPECIALS[rng.integers(0, F64_SPECIALS.size, n)], norm)
+        if sid % 20 == 5:
+            b[0] = 0xFFF8000000000000  # a NaN at the first row: FIRST must return it
+    elif kind == "okey_alone":
+        b = np.full(n, OKEY_MAX if sid % 20 == 6 else OKEY_MIN, dtype=np.uint64)
+    elif kind == "okey_mixed":
+        b = _clamp_exp(r)
+        b[rng.random(n) < 0.05] = OKEY_MAX if sid % 20 == 7 else OKEY_MIN
+        b[rng.random(n) < 0.02] = OKEY_MIN if sid % 20 == 7 else OKEY_MAX
+    elif kind == "dbl_max":
+        b = np.full(n, 0x7FEFFFFFFFFFFFFF | ((sid // 10 % 2) << 63), dtype=np.uint64)
+    else:  # all_nan
+        b = F64_SPECIALS[9:17][rng.integers(0, 8, n)]  # NaNs of both signs and several payloads
+    if kind in ("random", "signflip", "bit0_bit63", "runs", "small_xor", "okey_mixed", "specials"):
+        # the hardest transitions around rows 128 and 256: a 77-bit element (meaningful 64), an XOR of one bit
+        # (leading 63), a repeat, and for the specials a NaN, -inf and the INT64_MAX key
+        for r0 in (127, 255):
+            if n > r0 + 2:
+                if kind == "specials":
+                    b[r0:r0 + 3] = [OKEY_MIN, 0xFFF0000000000000, OKEY_MAX]
+                else:
+                    h = int(b[r0 - 1]) ^ 0x8000000000000001
+                    b[r0:r0 + 3] = [h, h ^ 1, h ^ 1]
+    assert not (b == GORILLA_EOS).any()
+    return b
+
+
+def f64_finite_series(ids):
+    """The series of `ids` whose values are all finite and below 2^1000 (their sums are finite in every cell)."""
+    return np.array([s for s in ids if f64_kind(s) in ("random", "signflip", "bit0_bit63", "runs", "small_xor")],
+                    dtype=np.uint32)
+
+
+def f64_edge_timestamps(rng, sid, n):
+    blk = sid // F64_BLOCK
+    k = np.arange(n, dtype=np.int64)
+    if blk == 1:
+        start = sid % 7 if n > 14 else 0
+        k = k[: n - start] + start
+    ts = F64_T0 + k * F64_STEP
+    if blk == 2 and n > 2:
+        jit = rng.integers(0, F64_STEP, n)
+        jit[0] = jit[-1] = 0
+        ts = ts + jit
+    if blk == 3 and n > 1:
+        ts[-1] = F64_T0 + 2**61  # a delta past 2^60: the writer falls back to a raw time page
+    return ts
+
+
+def f64_edge_arena(seed, n, ids=range(F64_SERIES)):
+    """-> (arena, descs, truth) of f64 edge pages of n rows (block B: fewer) for the series `ids`; series 3, 10, 17, ...
+    hold nulls."""
+    rng = np.random.default_rng(seed)
+    b = datagen.ArenaBuilder()
+    truth = {}
+    for sid in ids:
+        ts = f64_edge_timestamps(rng, sid, n)
+        m = ts.size
+        bits = f64_edge_bits(rng, sid, m)
+        valid = rng.random(m) >= 0.25 if sid % 7 == 3 else np.ones(m, dtype=bool)
+        vals = bits.view(np.float64)
+        vv = None if valid.all() else valid
+        b.add_column_group(sid, ts, [(1, cabi.TSKV_PT_F64, vals, vv), (2, cabi.TSKV_PT_F64, vals, vv, datagen.encode_raw)])
+        truth[sid] = [(ts, {1: (vals, valid), 2: (vals, valid)})]
+    arena, descs = b.finish()
+    return arena, descs, truth
+
+
+def f64_edge_queries(n, ids=range(F64_SERIES)):
+    """[(name, query, extra)]: extra = {} or {"group_ids": ..., "n_groups": ...} (GROUP BY tags) or {"slide": ...}."""
+    w = F64_STEP * max(1, n // 5)
+    fbs, nb = bucket_spec(F64_T0, F64_T0 + n * F64_STEP, w)
+    grid = dict(width=w, first_bucket_start=fbs, n_buckets=nb, time_ranges=[(F64_T0, F64_T0 + n * F64_STEP)])
+    aggs = ("count", "sum", "min", "max", "mean")
+    mixed = np.array([s for s in ids if f64_kind(s) != "dbl_max"], dtype=np.uint32)  # (two signs of DBL_MAX in a cell
+    finite = f64_finite_series(ids)                                                   # may or may not overflow)
+    k = 3
+    sgrid = dict(width=k * w, first_bucket_start=fbs - (k - 1) * w, n_buckets=nb + k - 1,
+                 time_ranges=grid["time_ranges"])
+    return [
+        ("bucket", make_query(F64_FIELDS, aggs, series_ids=mixed, **grid), {}),
+        ("bucket+sel", make_query(F64_FIELDS, ALL_AGGS, series_ids=mixed, **grid), {}),
+        ("bucket_finite", make_query(F64_FIELDS, aggs, series_ids=finite, **grid), {}),
+        ("by_series", make_query(F64_FIELDS, ALL_AGGS, group_by_series=True, **grid), {}),
+        ("unbucketed", make_query(F64_FIELDS, aggs, series_ids=mixed), {}),
+        ("tags", make_query(F64_FIELDS, aggs, series_ids=mixed, **grid),
+         {"group_ids": (mixed % 5).astype(np.uint32), "n_groups": 5}),
+        ("sliding", make_query(F64_FIELDS, aggs, series_ids=mixed, **sgrid), {"slide": w}),
+    ]
+
+
+def f64_edge_expected(truth, query, extra):
+    """The exact reference of one f64_edge_queries entry."""
+    from tests.group_reference import exact_aggregate_grouped
+    from tests.sliding_reference import expand_aggregate
+    if "group_ids" in extra:
+        return exact_aggregate_grouped(truth, query, extra["group_ids"], extra["n_groups"])
+    if "slide" in extra:
+        return expand_aggregate(truth, query, extra["slide"])
+    return exact_aggregate(truth, query)

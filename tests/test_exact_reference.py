@@ -2,13 +2,16 @@
 known-answer vectors and the oracle's restatement, and its aggregates against the oracle on every arena of the bucket
 geometry sweep. COUNT / SUM / MIN / MAX must agree bit for bit; f64 sums within the order-free bound; the integer MEAN is
 not compared (the oracle keeps an f64 running sum, the reference the exact one)."""
+import math
+
 import numpy as np
 import pytest
 
 from oracle import pyoracle as orc
-from tests.helpers import (GEOMETRY_CASES, I64_MAX, I64_MIN, ReferenceError, assert_matches_exact, ceil_sliding_window,
-                           exact_aggregate, floor_sliding_window, geometry_arena, geometry_queries, geometry_ranges,
-                           make_query, sliding_window, split_ranges)
+from tests.helpers import (DBL_MAX, F64_LENGTHS, GEOMETRY_CASES, I64_MAX, I64_MIN, OrderDependentSum, ReferenceError,
+                           assert_matches_exact, ceil_sliding_window, exact_aggregate, f64_edge_arena, f64_edge_expected,
+                           f64_edge_queries, f64_sum_class, floor_sliding_window, geometry_arena, geometry_queries,
+                           geometry_ranges, make_query, sliding_window, split_ranges)
 from cnosdb_b200 import cabi
 
 
@@ -90,3 +93,37 @@ def test_bucket_grid_one_short_is_an_error_for_both():
                 orc.scan_aggregate(arena, descs, q)
             assert oe.value.status == cabi.TSKV_ERR_BUCKET_RANGE
         break
+
+
+def test_f64_sum_classes():
+    """NaN and infinities decide an f64 sum in every order; a finite one is exactly rounded, +0.0 when zero; a sum that
+    overflows in some orders only is refused."""
+    inf, nan, big = math.inf, math.nan, DBL_MAX
+    assert math.isnan(f64_sum_class([1.0, nan])[0]) and math.isnan(f64_sum_class([inf, -inf, 2.0])[0])
+    assert f64_sum_class([-inf, 5.0, -big]) == (-inf, 0.0)
+    assert f64_sum_class([big, big, -1.0]) == (inf, 0.0)            # every order overflows: exact sum >= 2 DBL_MAX
+    assert f64_sum_class([-big] * 3) == (-inf, 0.0)
+    assert f64_sum_class([big]) == (big, big) and f64_sum_class([-big, -0.0]) == (-big, big)
+    s = f64_sum_class([-0.0, -0.0])[0]
+    assert s == 0 and math.copysign(1, s) == 1
+    assert f64_sum_class([1e300, -1e300, 5e-324]) == (5e-324, 2e300)
+    for x in ([big, -big, 1.0], [inf, -big, -big], [big, big, -big, -big]):
+        with pytest.raises(OrderDependentSum):
+            f64_sum_class(x)
+
+
+@pytest.mark.parametrize("n", F64_LENGTHS)
+def test_reference_matches_oracle_on_f64_edges(n):
+    """The extended reference against the oracle on the f64 edge arenas: COUNT / MIN / MAX bit for bit, SUM / MEAN by
+    class and within the bound (the oracle sums in row order, from +0.0)."""
+    arena, descs, truth = f64_edge_arena(n, n)
+    for name, q, extra in f64_edge_queries(n):
+        exp = f64_edge_expected(truth, q, extra)
+        if "group_ids" in extra or "slide" in extra:
+            continue  # (the oracle has no GROUP BY tags or sliding windows; their references build on this one)
+        got = orc.scan_aggregate(arena, descs, q)
+        assert_matches_exact(got, exp, what="n=%d %s" % (n, name))
+        # the arenas reach every class
+        if name == "by_series" and n >= 31:
+            c = exp.center[1]
+            assert np.isnan(c).any() and np.isposinf(c).any() and np.isneginf(c).any() and np.isfinite(c).any()
