@@ -60,9 +60,15 @@ struct BeStream {
 // Shared-memory staging of a lane's byte stream (round 2). One lane owns one page, so a warp reads 32 different
 // pages: each lane stages ITS stream through a private ring of RING_CHUNKS 16-byte chunks filled by 128-bit cp.async
 // (LDGSTS.128, L2 -> shared memory without a register round trip). A lane's ring is contiguous (RING_BYTES bytes) and
-// the lanes' rings are RING_LANE_STRIDE = RING_BYTES + 16 bytes apart: word k of the stream lives at
-//   ring + lane * RING_LANE_STRIDE + (k mod 2 * RING_CHUNKS) * 8
-// (one AND + one scaled add per word; the 16 bytes of skew spread lanes that sit at the same ring offset over the banks).
+// the lanes' rings are RING_BYTES apart. Each lane's chunk slots are rotated by its lane index: chunk c of the stream
+// lives at slot (c + rot) mod RING_CHUNKS, rot = lane mod RING_CHUNKS. Without the rotation every ring would start on
+// the same bank; with it, lanes that sit at the same stream offset spread over min(RING_CHUNKS, 8) 16-byte bank groups,
+// as a 16-byte skew between the rings would, without the skew's 16 bytes per lane. The rotation costs nothing per word:
+// the decoders keep their stream positions in RING COORDINATES, i.e. counted from chunk rot (word index k = the word's
+// index from the stream's aligned start + 2 rot, bit position + 128 rot), so word k lives at
+//   ring + lane * RING_BYTES + (k mod 2 * RING_CHUNKS) * 8
+// (one AND + one scaled add per word). Restart points (SkipEntry) hold positions relative to the stream's start, so an
+// entry saved by one lane restores on any other.
 // A decoder calls step(c) once per element / word BEFORE reading, c = the chunk its read window starts in; a window
 // never spans more than chunks c and c + 1, and c advances by at most one per step (an element is <= 77 bits, a word
 // 64). step() issues at most one new chunk - a predicated LDGSTS - commits exactly one group and waits until at most
@@ -78,9 +84,8 @@ struct BeStream {
 #define TSKV_RING_CHUNKS 8
 #endif
 constexpr int RING_CHUNKS = TSKV_RING_CHUNKS;
-constexpr uint32_t RING_BYTES = RING_CHUNKS * 16;            // one lane, one stream
-constexpr uint32_t RING_LANE_STRIDE = RING_BYTES + 16;
-constexpr uint32_t RING_BYTES_PER_WARP = 32 * RING_LANE_STRIDE;  // one stream of one warp
+constexpr uint32_t RING_BYTES = RING_CHUNKS * 16;       // one lane, one stream
+constexpr uint32_t RING_BYTES_PER_WARP = 32 * RING_BYTES;  // one stream of one warp
 static_assert((RING_CHUNKS & (RING_CHUNKS - 1)) == 0 && RING_CHUNKS >= 4, "ring size must be a power of two >= 4");
 static_assert(ARENA_SLACK >= RING_BYTES + 32, "the arena slack has to cover the rings' read-ahead");
 
@@ -90,6 +95,9 @@ struct ChunkRing {
   uint32_t snext;        // ring offset (bytes) the next chunk goes to
   uint32_t trig;         // the next chunk is issued once the read window reaches chunk `trig` (0xffffffff: none left)
   uint32_t trig_last;    // value of `trig` at which the page's last chunk goes out
+  // The calling lane's rotation in chunks (ring coordinates, above). The ring always belongs to the calling lane, so
+  // the rotation comes from the lane index rather than from per-ring state.
+  static __device__ __forceinline__ uint32_t rot() { return threadIdx.x & 31 & (RING_CHUNKS - 1); }
   __device__ __forceinline__ void issue_one() {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" :: "r"(sbase + snext), "l"(gnext) : "memory");
     gnext += 16;
@@ -97,28 +105,29 @@ struct ChunkRing {
   }
   __device__ __forceinline__ void init(const uint8_t *start, const uint8_t *end, uint32_t lane_ring) {
     const uintptr_t a = reinterpret_cast<uintptr_t>(start) & ~(uintptr_t)15, e = reinterpret_cast<uintptr_t>(end);
+    const uint32_t r = rot();
     gnext = reinterpret_cast<const uint8_t *>(a);
     const uint32_t n_chunks = e > a ? (uint32_t)((e - a + 15) >> 4) : 0u;  // chunks that intersect the stream
     sbase = lane_ring;
-    snext = 0;
+    snext = r * 16;  // the stream's first chunk
 #pragma unroll
     for (int i = 0; i < RING_CHUNKS; i++) issue_one();  // (a short stream's fill reads < RING_BYTES past its end)
-    trig = n_chunks > RING_CHUNKS ? 1u : 0xffffffffu;   // chunk RING_CHUNKS goes out when the window reaches chunk 1
-    trig_last = n_chunks - RING_CHUNKS;
+    trig = n_chunks > RING_CHUNKS ? r + 1 : 0xffffffffu;  // chunk RING_CHUNKS goes out when the window reaches chunk 1
+    trig_last = n_chunks - RING_CHUNKS + r;
   }
   // The same ring entered in the middle of the stream (restart points, SkipEntry below): the first chunk staged is
-  // chunk c0 (counted from the stream's aligned start, like every chunk / word index of the decoders) and it lands at
-  // ring offset (c0 mod RING_CHUNKS) * 16, so word k of the stream stays at (k mod 2 * RING_CHUNKS) * 8.
+  // chunk c0, in ring coordinates like every chunk / word index of the decoders.
   __device__ __forceinline__ void init_at(const uint8_t *start, const uint8_t *end, uint32_t lane_ring, uint32_t c0) {
     const uintptr_t a = reinterpret_cast<uintptr_t>(start) & ~(uintptr_t)15, e = reinterpret_cast<uintptr_t>(end);
+    const uint32_t r = rot();
     const uint32_t n_chunks = e > a ? (uint32_t)((e - a + 15) >> 4) : 0u;
-    gnext = reinterpret_cast<const uint8_t *>(a) + (size_t)c0 * 16;
+    gnext = reinterpret_cast<const uint8_t *>(a) + (size_t)(c0 - r) * 16;
     sbase = lane_ring;
     snext = (c0 & (RING_CHUNKS - 1)) * 16;
 #pragma unroll
     for (int i = 0; i < RING_CHUNKS; i++) issue_one();  // (near the end of the stream: < RING_BYTES past its end)
-    trig = n_chunks > c0 + RING_CHUNKS ? c0 + 1 : 0xffffffffu;
-    trig_last = n_chunks - RING_CHUNKS;
+    trig = n_chunks + r > c0 + RING_CHUNKS ? c0 + 1 : 0xffffffffu;
+    trig_last = n_chunks - RING_CHUNKS + r;
   }
   // One decoder step whose read window starts in chunk c (see above). Nothing is issued past the stream's last chunk,
   // however far a decoder that ran off a truncated block pushes its window.
@@ -136,7 +145,7 @@ struct ChunkRing {
     asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];\n" : "=r"(v.x), "=r"(v.y) : "r"(addr) : "memory");
     return v;
   }
-  // 64-bit word k of the stream (8-byte units from the aligned start), as stored (little-endian load of stream bytes)
+  // 64-bit word k of the stream (8-byte units, ring coordinates), as stored (little-endian load of stream bytes)
   __device__ __forceinline__ uint2 word(uint32_t k) const { return lds64(sbase + ((k & (2 * RING_CHUNKS - 1)) << 3)); }
   // words k, k + 1, k + 2
   __device__ __forceinline__ void words3(uint32_t k, uint2 &w0, uint2 &w1, uint2 &w2) const {
@@ -184,7 +193,7 @@ __device__ __forceinline__ SkipEntry load_skip(const SkipEntry *p) {
 // Same interface as BeStream.
 struct SeqStream {
   ChunkRing ring;
-  uint32_t k;     // index of the last aligned word loaded
+  uint32_t k;     // index of the last aligned word loaded (ring coordinates)
   uint32_t psel;  // byte-permute selector: the big-endian word at the stream's (constant) byte misalignment
   bool high;      // the misalignment is >= 4 bytes
   uint2 cur;      // last aligned word, as stored
@@ -194,7 +203,7 @@ struct SeqStream {
     const uint32_t o = (uint32_t)(a & 7), q = o & 3;
     high = o >= 4;
     psel = (q + 3) | ((q + 2) << 4) | ((q + 1) << 8) | (q << 12);  // result byte 3 (most significant) = stream byte q
-    k = (uint32_t)(a & 15) >> 3;
+    k = first_word_index(p);
     const uint64_t w = __ldg(reinterpret_cast<const uint64_t *>(a & ~(uintptr_t)7));  // the first word straight from global memory
     cur = make_uint2((uint32_t)w, (uint32_t)(w >> 32));
   }
@@ -205,12 +214,16 @@ struct SeqStream {
     const uint32_t o = (uint32_t)(a & 7), q = o & 3;
     high = o >= 4;
     psel = (q + 3) | ((q + 2) << 4) | ((q + 1) << 8) | (q << 12);
-    k = ((uint32_t)(a & 15) >> 3) + rel;
+    const uint32_t kk = ((uint32_t)(a & 15) >> 3) + rel;  // from the aligned start
+    k = kk + 2 * ChunkRing::rot();
     ring.init_at(p, end, lane_slot, k >> 1);
-    const uint64_t w = __ldg(reinterpret_cast<const uint64_t *>(a & ~(uintptr_t)15) + k);
+    const uint64_t w = __ldg(reinterpret_cast<const uint64_t *>(a & ~(uintptr_t)15) + kk);
     cur = make_uint2((uint32_t)w, (uint32_t)(w >> 32));
   }
-  __device__ __forceinline__ uint32_t first_word_index(const uint8_t *p) const { return (uint32_t)(reinterpret_cast<uintptr_t>(p) & 15) >> 3; }
+  // ring-coordinate index of the aligned word that holds the stream's first byte
+  static __device__ __forceinline__ uint32_t first_word_index(const uint8_t *p) {
+    return ((uint32_t)(reinterpret_cast<uintptr_t>(p) & 15) >> 3) + 2 * ChunkRing::rot();
+  }
   __device__ __forceinline__ uint64_t next() {
     k++;
     ring.step(k >> 1);
@@ -695,7 +708,7 @@ struct GorillaCursor {
 struct GorillaRing {
   ChunkRing ring;
   uint64_t val;         // value the next call returns
-  uint32_t pos;         // bit position of the next element, from the ring's aligned start
+  uint32_t pos;         // bit position of the next element (ring coordinates)
   uint32_t end_pos;     // bit position of the end of the block
   uint32_t meaningful, trailing;
   bool cur_ok;          // `val` is a real value (not the terminating sentinel)
@@ -706,7 +719,7 @@ struct GorillaRing {
     const uint8_t *d = pv.data;  // id | 0x10 | first(8) | bit stream
     val = load_be64(d + 2);
     ring.init(d + 10, d + pv.data_len, lane_slot);
-    pos = (uint32_t)(reinterpret_cast<uintptr_t>(d + 10) & 15) * 8;
+    pos = start_pos(d);
     end_pos = pos + (pv.data_len - 10) * 8;
     meaningful = 64;
     trailing = 0;
@@ -719,18 +732,22 @@ struct GorillaRing {
     cur_ok = false; done = any = false;
   }
   __device__ __forceinline__ bool consumed_any() const { return any; }
+  // ring-coordinate bit position of the stream's first bit (data = id | 0x10 | first(8) | bit stream)
+  static __device__ __forceinline__ uint32_t start_pos(const uint8_t *data) {
+    return (uint32_t)(reinterpret_cast<uintptr_t>(data + 10) & 15) * 8 + ChunkRing::rot() * 128;
+  }
   // Restart points (SkipEntry): the state before some next() call, and a cursor re-entered there.
   __device__ __forceinline__ SkipEntry save(const PageView &pv) const {
     SkipEntry e;
     e.v = val;
-    e.a = pos - (uint32_t)(reinterpret_cast<uintptr_t>(pv.data + 10) & 15) * 8;
+    e.a = pos - start_pos(pv.data);
     e.b = meaningful | (trailing << 8) | ((cur_ok ? 1u : 0u) << 16) | ((any ? 1u : 0u) << 17);
     return e;
   }
   __device__ __forceinline__ void restore(const PageView &pv, uint32_t lane_slot, const SkipEntry &e) {
     const uint8_t *d = pv.data;
     val = e.v;
-    const uint32_t pos0 = (uint32_t)(reinterpret_cast<uintptr_t>(d + 10) & 15) * 8;
+    const uint32_t pos0 = start_pos(d);
     pos = pos0 + e.a;
     end_pos = pos0 + (pv.data_len - 10) * 8;
     ring.init_at(d + 10, d + pv.data_len, lane_slot, pos >> 7);

@@ -1066,7 +1066,7 @@ __device__ __forceinline__ uint4 tomb_lookup(const ScanParams &P, uint32_t serie
 // SEL: the query wants FIRST/LAST somewhere (tracks the (ts, value) of each run's end rows).
 template <int TK, int VK, bool SEL>
 __device__ __forceinline__ void scan_chunk_rows(const ScanParams &P, uint32_t item_begin, uint32_t item_end,
-                                             uint32_t /*ring_base*/, uint64_t *stab) {
+                                             uint32_t /*ring_base*/, uint64_t *stab, uint4 *s_tomb) {
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t item = item_begin + lane;
   const bool have_item = item < item_end;
@@ -1076,7 +1076,6 @@ __device__ __forceinline__ void scan_chunk_rows(const ScanParams &P, uint32_t it
   uint8_t pt = TSKV_PT_I64, mask = 0;
   PageView tpv, vpv;
   BitCursor tbits, vbits;
-  __shared__ uint4 s_tomb[SCAN_THREADS];  // per lane tombstone lists (only touched when the page set has any)
   DeltaCursor<TK == TK_RLE ? DK_RLE_SC : TK == TK_S8B ? DK_S8B_SC : -1, BeStream> tcur;
   DeltaCursor<VK == VK_S8B ? DK_S8B_ZZ : -1, BeStream> vcur_d;
   GorillaCursor<BeStream> vcur_g;
@@ -1291,34 +1290,40 @@ struct ValueAcc {  // count / sum / min / max of one run; VK fixes the arithmeti
 // with warp reductions (REDUX / butterflies) and then updating the shared table with CAS-loop atomics costs ~230
 // instructions per 6-row segment. Instead every lane parks its partial in a per-warp staging area
 //   stage[slot][quantity][lane]          (one conflict-free STS.64 per quantity)
-// and every FLUSH_SLOTS flushes the warp reduces the parked partials TRANSPOSED: lane j owns slot j % FLUSH_SLOTS and
-// sums the partials of FLUSH_SLOTS source lanes serially (every lane does useful work on every instruction),
-// xor-shuffle steps combine the 32 / FLUSH_SLOTS lane groups, and FLUSH_SLOTS lanes update the CTA table.
+// and every NS flushes the warp reduces the parked partials TRANSPOSED: lane j owns slot j % NS and sums the partials
+// of NS source lanes serially (every lane does useful work on every instruction), xor-shuffle steps combine the 32 / NS
+// lane groups, and NS lanes update the CTA table.
+// NS = flush_slots(TK) slots per warp: 4 (5 152 bytes) for the RLE-timestamp kernels, 2 (2 576 bytes) for the
+// simple8b-timestamp kernels, whose two staging rings per warp would otherwise keep them at 3 CTAs per SM. A jittered
+// simple8b time page flushes about once per bucket after a few hundred instructions per row, so the extra reduce pass
+// per two flushes costs little there. Building with -DTSKV_FLUSH_SLOTS=n gives every kernel n slots.
 // ------------------------------------------------------------------------------------------------
-#ifndef TSKV_FLUSH_SLOTS
-#define TSKV_FLUSH_SLOTS 4
+#ifdef TSKV_FLUSH_SLOTS
+constexpr int FLUSH_SLOTS = TSKV_FLUSH_SLOTS;
+__host__ __device__ constexpr int flush_slots(int /*tk*/) { return FLUSH_SLOTS; }
+#else
+constexpr int FLUSH_SLOTS = 4;
+__host__ __device__ constexpr int flush_slots(int tk) { return tk == TK_S8B ? 2 : FLUSH_SLOTS; }
 #endif
-constexpr int FLUSH_SLOTS = TSKV_FLUSH_SLOTS;  // 2: 2.6 KB per warp (5 CTAs of 4 warps per SM), 4: fewer reduce passes
 constexpr int FLUSH_Q = 5;  // count | sum | sum_hi | min key | max key
-constexpr uint32_t FLUSH_STAGE_WORDS = FLUSH_SLOTS * FLUSH_Q * 32 + FLUSH_SLOTS;  // + one meta word per slot
-constexpr uint32_t FLUSH_STAGE_BYTES = FLUSH_STAGE_WORDS * 8;
+__host__ __device__ constexpr uint32_t flush_stage_bytes(int ns) { return (ns * FLUSH_Q * 32 + ns) * 8; }  // + one meta word per slot
 
-template <int VK>
+template <int VK, int NS>
 __device__ __forceinline__ void reduce_staged(const ScanParams &P, uint64_t *stab, uint64_t *stage, uint32_t n_slots) {
   __syncwarp();
   const uint32_t lane = threadIdx.x & 31;
-  const uint32_t s = lane & (FLUSH_SLOTS - 1), g = lane / FLUSH_SLOTS;
-  const uint64_t meta = stage[FLUSH_SLOTS * FLUSH_Q * 32 + s];  // (query column << 32) | cell
+  const uint32_t s = lane & (NS - 1), g = lane / NS;
+  const uint64_t meta = stage[NS * FLUSH_Q * 32 + s];  // (query column << 32) | cell
   const uint32_t qcol = (uint32_t)(meta >> 32);
   const ColState &cs = P.cols[s < n_slots ? qcol : 0];
   const bool is_f64 = VK == VK_GOR || (VK == VK_GEN && cs.phys_type == TSKV_PT_F64);
   uint64_t cnt = 0, sum = 0;
   int64_t hi = 0, kmin = INT64_MAX, kmax = INT64_MIN;
   const uint64_t *base = stage + (size_t)s * FLUSH_Q * 32;
-  static_assert(FLUSH_SLOTS == 2 || FLUSH_SLOTS == 4, "reduce_staged: lane j owns slot j % FLUSH_SLOTS");
+  static_assert(NS == 2 || NS == 4, "reduce_staged: lane j owns slot j % NS");
 #pragma unroll
-  for (int i = 0; i < FLUSH_SLOTS; i++) {  // FLUSH_SLOTS source lanes per lane group, rotated by the slot: conflict-free
-    const uint32_t src = g * FLUSH_SLOTS + ((i + s) & (FLUSH_SLOTS - 1));
+  for (int i = 0; i < NS; i++) {  // NS source lanes per lane group, rotated by the slot: conflict-free
+    const uint32_t src = g * NS + ((i + s) & (NS - 1));
     const uint64_t c = base[src], v = base[32 + src];
     cnt += c;
     if (is_f64) {
@@ -1332,7 +1337,7 @@ __device__ __forceinline__ void reduce_staged(const ScanParams &P, uint64_t *sta
     kmax = b > kmax ? b : kmax;
   }
 #pragma unroll
-  for (int o = FLUSH_SLOTS; o < 32; o <<= 1) {  // lanes j, j ^ o own the same slot
+  for (int o = NS; o < 32; o <<= 1) {  // lanes j, j ^ o own the same slot
     cnt += shfl_xor_u64(cnt, o);
     const uint64_t v = shfl_xor_u64(sum, o);
     // (every shuffle outside the is_f64 branch: slots of a generic-kind warp can hold columns of different types)
@@ -1353,8 +1358,8 @@ __device__ __forceinline__ void reduce_staged(const ScanParams &P, uint64_t *sta
 }
 
 // Every lane parks its partial (identities unless `live`) in staging slot `seq`, the lane `meta_lane` records the slot's
-// (query column << 32) | cell, and every FLUSH_SLOTS slots the warp reduces them. Called by all 32 lanes.
-template <int VK>
+// (query column << 32) | cell, and every NS slots the warp reduces them. Called by all 32 lanes.
+template <int VK, int NS>
 __device__ __forceinline__ void stage_partial(const ScanParams &P, uint64_t *stab, uint64_t *stage, uint32_t &seq, bool live,
                                               const ValueAcc<VK> &va, bool meta_lane, uint64_t gcell) {
   uint64_t *q = stage + (size_t)seq * FLUSH_Q * 32 + (threadIdx.x & 31);
@@ -1363,15 +1368,15 @@ __device__ __forceinline__ void stage_partial(const ScanParams &P, uint64_t *sta
   if (VK != VK_GOR) q[64] = live ? (uint64_t)va.sum_hi : 0;
   q[96] = live ? (uint64_t)va.kmin : (uint64_t)INT64_MAX;
   q[128] = live ? (uint64_t)va.kmax : (uint64_t)INT64_MIN;
-  if (meta_lane) stage[FLUSH_SLOTS * FLUSH_Q * 32 + seq] = gcell;
-  if (++seq == FLUSH_SLOTS) {
-    reduce_staged<VK>(P, stab, stage, seq);
+  if (meta_lane) stage[NS * FLUSH_Q * 32 + seq] = gcell;
+  if (++seq == NS) {
+    reduce_staged<VK, NS>(P, stab, stage, seq);
     seq = 0;
   }
 }
 
 // Flush of one finished run per flushing lane (no FIRST/LAST). `seq` = staged slots in use (warp-uniform).
-template <int VK>
+template <int VK, int NS>
 __device__ __forceinline__ void flush_runs(const ScanParams &P, uint64_t *stab, uint64_t *stage, uint32_t &seq, bool active,
                                            uint32_t qcol, uint64_t cell, uint8_t pt, uint8_t mask, const ValueAcc<VK> &va) {
   const uint32_t m = __ballot_sync(FULL, active);
@@ -1386,7 +1391,7 @@ __device__ __forceinline__ void flush_runs(const ScanParams &P, uint64_t *stab, 
   // atomic per quantity instead of 32 contended ones.
   const bool same = !P.group_by_series && __all_sync(FULL, !active || gcell == lcell);
   if (same) {
-    stage_partial<VK>(P, stab, stage, seq, active && va.count, va, (int)lane == leader, lcell);
+    stage_partial<VK, NS>(P, stab, stage, seq, active && va.count, va, (int)lane == leader, lcell);
   } else if (active && va.count) {  // lanes on different cells (GROUP BY series, unaligned pages): one update each
     table_update(P, stab, P.cols[qcol], cell, mask, VK == VK_GOR || (VK == VK_GEN && pt == TSKV_PT_F64), va.count, va.sum,
                  va.sum_hi, va.kmin, va.kmax);
@@ -1417,14 +1422,15 @@ __device__ __forceinline__ uint32_t rle_rows_within(uint64_t d, uint64_t delta, 
 // values are decoded and accumulated in 32-bit arithmetic (S8bCursor::next32, ValueAcc::add32).
 template <int TK, int VK, bool SEL, bool NARROW>
 __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t item_begin, uint32_t item_end,
-                                               uint32_t ring_base, uint64_t *stab, uint64_t *stage,
+                                               uint32_t ring_base, uint64_t *stab, uint64_t *stage, uint4 *s_tomb,
                                                uint32_t part, uint32_t n_parts, uint32_t part_rows) {
+  constexpr int NS = flush_slots(TK);  // staging slots of the staged flush
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t item = item_begin + lane;
   const bool have_item = item < item_end;
   // this lane's slots in the warp's staging rings: [time ring (simple8b timestamps only)] [value ring]
-  const uint32_t tslot = ring_base + lane * RING_LANE_STRIDE;
-  const uint32_t vslot = ring_base + (TK == TK_S8B ? RING_BYTES_PER_WARP : 0) + lane * RING_LANE_STRIDE;
+  const uint32_t tslot = ring_base + lane * RING_BYTES;
+  const uint32_t vslot = ring_base + (TK == TK_S8B ? RING_BYTES_PER_WARP : 0) + lane * RING_BYTES;
 
   uint32_t page = 0, slot = 0, qcol = 0, n_rows = 0;
   uint8_t pt = VK == VK_GOR ? TSKV_PT_F64 : TSKV_PT_I64, mask = 0;
@@ -1438,7 +1444,6 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   const uint32_t *keepw = nullptr;  // row-filter keep bits of the column group (k_row_filter), or null
   bool allnull = false;
   int64_t pend_t = 0;  // timestamp of row `row`
-  __shared__ uint4 s_tomb[SCAN_THREADS];  // per lane tombstone lists (only touched when the page set has any)
 
   if (TK == TK_S8B) tcur.reset(tslot);
   if (VK == VK_GOR) vcur_g.reset(vslot);
@@ -1541,7 +1546,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
         warp_flush<SEL>(P, stab, flush, qcol, group_cell_base(P, fslot) + run_idx, (int64_t)run_idx, pt, mask, acc, fslot);
       }
     } else {
-      flush_runs<VK>(P, stab, stage, staged, flush, qcol, group_base + run_idx, pt, mask, va);
+      flush_runs<VK, NS>(P, stab, stage, staged, flush, qcol, group_base + run_idx, pt, mask, va);
     }
   };
   // One row's value: validity bit, decode (every valid row is decoded - rows outside the time ranges too, the streams
@@ -1717,7 +1722,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           if (n_rows) check_values();
           if (in && (nb == 0 || r == rb1)) {  // the bucket's last row: its partial goes to the staging area
             va.fold(pt, NARROW);
-            stage_partial<VK>(P, stab, stage, staged, n_rows && va.count, va, lane == 0, col + bidx);
+            stage_partial<VK, NS>(P, stab, stage, staged, n_rows && va.count, va, lane == 0, col + bidx);
             va.reset(NARROW);
           }
         }
@@ -1904,7 +1909,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
     }
   }
   if (!SEL && staged) {  // partials still parked in the staging area
-    reduce_staged<VK>(P, stab, stage, staged);
+    reduce_staged<VK, NS>(P, stab, stage, staged);
     staged = 0;
   }
   // (only the lane that decodes the page's last rows walks on to the sentinel)
@@ -1936,8 +1941,10 @@ __host__ __device__ constexpr uint32_t scan_ring_bytes_per_warp(int tk) {
 }
 // per-warp shared memory of the fused kernel: staging rings + the staged-flush area
 __host__ __device__ constexpr uint32_t scan_warp_bytes(int tk) {
-  return tk == TK_GEN ? 0 : scan_ring_bytes_per_warp(tk) + FLUSH_STAGE_BYTES;
+  return tk == TK_GEN ? 0 : scan_ring_bytes_per_warp(tk) + flush_stage_bytes(flush_slots(tk));
 }
+// per-lane tombstone lists (tomb_lookup), after the warps' areas; allocated only when the page set has tombstones
+constexpr uint32_t SCAN_TOMB_BYTES = SCAN_THREADS * sizeof(uint4);
 // Narrow pages of a simple8b-value bin (ScanParams.page_narrow), per page set: none, some or all of them. NARROW_SOME
 // kernels choose per chunk; NARROW_ALL kernels hold the narrow arithmetic only (a kernel that holds both row loops runs
 // its narrow chunks ~1.5 % slower on C4: H100, see DESIGN.md §5).
@@ -1945,8 +1952,9 @@ enum { NARROW_NONE = 0, NARROW_SOME = 1, NARROW_ALL = 2 };
 template <int TK, int VK, bool SEL, int NARROW>
 __global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, SEL)) k_scan_aggregate(const __grid_constant__ ScanParams P, int bin) {
   static_assert(NARROW == NARROW_NONE || (TK != TK_GEN && VK == VK_S8B && !SEL), "narrow kernels: simple8b values, no FIRST / LAST");
-  // dynamic shared memory: [per-CTA partial table, P.smem_words 8-byte words (or empty)] [staging rings, per warp:
-  // a value ring, preceded by a time ring when the timestamps are simple8b]
+  // dynamic shared memory: [per-CTA partial table, P.smem_words 8-byte words (or empty)] [per warp: a value ring,
+  // preceded by a time ring when the timestamps are simple8b, then the staged-flush area] [tombstone lists, only when
+  // P.has_tomb]
   extern __shared__ __align__(16) uint64_t s_tab[];
   if (P.use_smem) {  // identities: 0 for counts / sums, +-inf keys for min / max
     for (uint32_t i = threadIdx.x; i < P.smem_words; i += SCAN_THREADS) s_tab[i] = 0;
@@ -1964,6 +1972,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, SEL)) k_scan
   uint64_t *warp_area = s_tab + ((P.smem_words + 1) & ~1u) + (size_t)(threadIdx.x >> 5) * (scan_warp_bytes(TK) / 8);
   const uint32_t ring_base = (uint32_t)__cvta_generic_to_shared(warp_area);
   uint64_t *stage = warp_area + scan_ring_bytes_per_warp(TK) / 8;
+  uint4 *s_tomb = reinterpret_cast<uint4 *>(s_tab + ((P.smem_words + 1) & ~1u) + (SCAN_THREADS / 32) * (scan_warp_bytes(TK) / 8));
   const uint32_t begin0 = __ldg(P.bin_cstart + bin), end0 = __ldg(P.bin_cstart + bin + 1);
   // pages cut at restart points: n_parts chunks per group of 32 pages (consecutive chunk numbers = the parts of one group)
   const uint32_t n_parts = (TK == TK_GEN || VK == VK_GEN || SEL) ? 1u : P.bin_parts[bin];
@@ -1979,15 +1988,15 @@ __global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, SEL)) k_scan
     const uint32_t begin = begin0 + (group << 5);
     const uint32_t end = min(begin + 32, end0);
     if constexpr (TK == TK_GEN) {
-      scan_chunk_rows<TK, VK, SEL>(P, begin, end, ring_base, s_tab);
+      scan_chunk_rows<TK, VK, SEL>(P, begin, end, ring_base, s_tab, s_tomb);
     } else if constexpr (NARROW == NARROW_SOME) {
       // 32-bit arithmetic when all of the chunk's pages are narrow (the work list keeps a bin's narrow pages together)
       const uint32_t item = begin + lane;
       const bool narrow = __all_sync(FULL, item >= end || __ldg(P.page_narrow + __ldg(P.work_page + item)));
-      if (narrow) scan_chunk_seg<TK, VK, SEL, true>(P, begin, end, ring_base, s_tab, stage, part, n_parts, part_rows);
-      else scan_chunk_seg<TK, VK, SEL, false>(P, begin, end, ring_base, s_tab, stage, part, n_parts, part_rows);
+      if (narrow) scan_chunk_seg<TK, VK, SEL, true>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
+      else scan_chunk_seg<TK, VK, SEL, false>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
     } else {
-      scan_chunk_seg<TK, VK, SEL, NARROW == NARROW_ALL>(P, begin, end, ring_base, s_tab, stage, part, n_parts, part_rows);
+      scan_chunk_seg<TK, VK, SEL, NARROW == NARROW_ALL>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
     }
   }
   if (P.use_smem) {  // merge this CTA's table into the global state, once

@@ -28,7 +28,7 @@ __global__ void __launch_bounds__(SKIP_THREADS) k_build_skip(const uint8_t *aren
                                                              uint32_t *skip_off, SkipEntry *skip, uint8_t *narrow) {
   extern __shared__ __align__(16) uint8_t s_rings[];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t slot = (uint32_t)__cvta_generic_to_shared(s_rings) + warp * RING_BYTES_PER_WARP + lane * RING_LANE_STRIDE;
+  const uint32_t slot = (uint32_t)__cvta_generic_to_shared(s_rings) + warp * RING_BYTES_PER_WARP + lane * RING_BYTES;
   const uint32_t i = blockIdx.x * SKIP_THREADS + threadIdx.x;
   const bool have = i < n_pages;
   uint32_t page = 0, n_rows = 0, page_rows = 0, off = SKIP_NONE;

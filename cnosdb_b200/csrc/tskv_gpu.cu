@@ -156,6 +156,7 @@ struct tskv_scan {
   uint64_t *d_values = nullptr;
   uint8_t *d_validity = nullptr;
   int grid[N_BINS] = {0};
+  int occ[N_BINS] = {0};  // resident CTAs per SM of each bin's kernel at this scan's shared memory size
   bool use_coop[N_BINS] = {false};  // cooperative-eligible bins: which kernel family runs them
   CoopParams coop{};
   tskv_ctx *ctx = nullptr;
@@ -277,9 +278,11 @@ double bin_cost(int bin, bool coop) {
   return tk[sb / N_VK] * vk[sb % N_VK] * (coop ? 1.8 : 1.0);
 }
 
-// dynamic shared memory of a lane-per-page kernel: the per-CTA table + the warps' staging rings
-size_t serial_smem_bytes(int serial_bin, uint32_t table_words) {
-  return (size_t)((table_words + 1) & ~1u) * 8 + (size_t)scan_warp_bytes(serial_bin / N_VK) * (SCAN_THREADS / 32);
+// dynamic shared memory of a lane-per-page kernel: the per-CTA table + the warps' staging rings and flush areas + the
+// lanes' tombstone lists when the page set has tombstones
+size_t serial_smem_bytes(int serial_bin, uint32_t table_words, bool has_tomb) {
+  return (size_t)((table_words + 1) & ~1u) * 8 + (size_t)scan_warp_bytes(serial_bin / N_VK) * (SCAN_THREADS / 32) +
+         (has_tomb ? SCAN_TOMB_BYTES : 0);
 }
 // Serial time of one row of one 32-page chunk, relative: simple8b timestamps cost more than RLE ones (closed form),
 // gorilla values more than simple8b ones, generic codecs most. Only the order and rough ratios matter: they rank the
@@ -1782,6 +1785,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
     // few selected pages that chain is the scan's makespan, and with many the makespan is still quantised in chunk
     // times. Cut the pages of the simple8b / gorilla bins into parts so that the scan has about PARTS_TARGET chunks
     // per resident warp (more parts = shorter chains, but one more page open + two more run flushes per part).
+    // With every bin at 4 CTAs per SM, 8 chunks per resident warp measured best on C4 (H100: 4 parts of 256 rows per
+    // 1000-row page instead of 3 uneven parts of 384 / 384 / 232 rows at a target of 4; DESIGN.md §5).
     uint32_t parts[N_BINS];
     for (int b = 0; b < N_BINS; b++) parts[b] = 1;
     if (pages->d_skip && !s->has_sel) {
@@ -1789,7 +1794,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
       for (int b = 0; b < N_BINS; b++) est_chunks += std::ceil((pages->h_bin_start[b + 1] - pages->h_bin_start[b]) * sel_frac / 32.0);
       const double resident_warps = (double)ctx->sm_count * SCAN_MIN_BLOCKS * (SCAN_THREADS / 32);
       const char *pt_env = getenv("TSKV_PARTS_TARGET");
-      uint32_t want = plan_parts_wanted(est_chunks, resident_warps, pt_env ? atof(pt_env) : 4.0);
+      uint32_t want = plan_parts_wanted(est_chunks, resident_warps, pt_env ? atof(pt_env) : 8.0);
       const char *parts_env = getenv("TSKV_PARTS");  // fixed number of parts (1 = never cut)
       if (parts_env) want = (uint32_t)std::max(1, atoi(parts_env));
       for (int b = 0; b < N_BINS; b++) {
@@ -1818,13 +1823,14 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
       if (!s->use_coop[b]) {
         const int sb = serial_bin_of(b);
         const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, SCAN_THREADS, serial_smem_bytes(sb, P.smem_words));
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, SCAN_THREADS, serial_smem_bytes(sb, P.smem_words, P.has_tomb));
       } else {
         const void *fn = coop_kernel_for(b, s->has_sel);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, SCAN_THREADS, coop_smem_bytes(b, P.smem_words));
       }
       occ = std::max(1, occ);
       occ_bin[b] = occ;
+      s->occ[b] = occ;
       const double est_items = n_bin * sel_frac * 1.02 + 32;
       const uint32_t per_task = !s->use_coop[b] ? 32u : is_gor_coop_bin(b) ? gor_group : 1u;  // pages per warp task
       const double tasks = est_items / per_task * parts[b];
@@ -2186,7 +2192,8 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       const int sb = serial_bin_of(b);
       void *args[] = {(void *)&s->params, (void *)&bin};
       const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
-      CU_TRY(ctx, cudaLaunchKernel(fn, dim3(s->grid[b]), dim3(SCAN_THREADS), args, serial_smem_bytes(sb, s->params.smem_words), ctx->bin_stream[b]));
+      CU_TRY(ctx, cudaLaunchKernel(fn, dim3(s->grid[b]), dim3(SCAN_THREADS), args, serial_smem_bytes(sb, s->params.smem_words, s->params.has_tomb),
+                                   ctx->bin_stream[b]));
     } else {
       void *args[] = {(void *)&s->params, (void *)&s->coop, (void *)&bin};
       CU_TRY(ctx, cudaLaunchKernel(coop_kernel_for(b, s->has_sel), dim3(s->grid[b]), dim3(SCAN_THREADS), args,
@@ -2260,8 +2267,8 @@ static tskv_status sync_scan(tskv_ctx *ctx, tskv_scan *s) {
     if (getenv("TSKV_DEBUG_BINS")) {
       float t0 = 0;
       cudaEventElapsedTime(&t0, s->ev_bin[0], s->ev_bin_start[b]);
-      fprintf(stderr, "[tskv] bin %d%s grid %d: start +%.3f ms, run %.3f ms, %llu bytes\n", b, s->use_coop[b] ? " (coop)" : "",
-              s->grid[b], t0, t, aux[4 + b]);
+      fprintf(stderr, "[tskv] bin %d%s grid %d, %d CTAs/SM: start +%.3f ms, run %.3f ms, %llu bytes\n", b,
+              s->use_coop[b] ? " (coop)" : "", s->grid[b], s->occ[b], t0, t, aux[4 + b]);
     }
     if (t > ctx->counters.dominant_kernel_ms) {
       ctx->counters.dominant_kernel_ms = t;
