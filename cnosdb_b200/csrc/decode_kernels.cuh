@@ -1,8 +1,8 @@
 // decode_kernels.cuh — decode-only path (Page::to_arrow_array / data_buf_to_arrow_array, tsm/reader.rs:658-731):
 // values + Arrow validity bitmap of whole pages to HBM (BASELINE config C1, and the debugging / export path).
 //
-//   k_decode_warp   one WARP per page. Codecs whose values are independent given a prefix sum are decoded
-//                   cooperatively - simple8b words lane-per-word (coalesced 8-byte loads, selector lookup, warp
+//   k_decode_warp   one WARP per page. Codecs whose values are independent given a prefix sum are decoded by
+//                   the whole warp - simple8b words lane-per-word (coalesced 8-byte loads, selector lookup, warp
 //                   exclusive scan of the counts for the output offsets, warp inclusive scan of the per-word delta
 //                   sums for the running value), raw pages lane-per-value, RLE pages in closed form from the validity
 //                   ranks - so a single long page (C1: one series x 10 000 points) uses 32 lanes and every store is to
@@ -11,7 +11,7 @@
 //                   are decoded by lane 0 with the streaming cursors of cursors.cuh.
 // Same formats and error classes as the fused scan (cursors.cuh cites the reference lines).
 #pragma once
-#include "coop_kernels.cuh"
+#include "scan_kernels.cuh"
 
 namespace tskv {
 
@@ -54,6 +54,35 @@ __device__ inline tskv_status decode_page_serial(const uint8_t *arena, const tsk
   }
   *points_out = points;
   return st;
+}
+
+__device__ __forceinline__ uint64_t load_be64_any(const uint8_t *p) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+  const uint64_t *ap = reinterpret_cast<const uint64_t *>(a & ~(uintptr_t)7);
+  const uint32_t sh = (uint32_t)(a & 7) * 8;
+  const uint64_t lo = __ldg(ap), hi = __ldg(ap + 1);
+  return bswap64((lo >> sh) | ((hi << 1) << (63 - sh)));
+}
+
+__device__ __forceinline__ uint32_t warp_excl_scan_u32(uint32_t v, uint32_t *total) {
+  const uint32_t lane = threadIdx.x & 31;
+  uint32_t x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t y = __shfl_up_sync(FULL, x, o);
+    if (lane >= (uint32_t)o) x += y;
+  }
+  *total = __shfl_sync(FULL, x, 31);
+  return x - v;
+}
+__device__ __forceinline__ uint64_t warp_incl_scan_u64(uint64_t v) {
+  const uint32_t lane = threadIdx.x & 31;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t lo = __shfl_up_sync(FULL, (uint32_t)v, o), hi = __shfl_up_sync(FULL, (uint32_t)(v >> 32), o);
+    if (lane >= (uint32_t)o) v += ((uint64_t)hi << 32) | lo;
+  }
+  return v;
 }
 
 // Cooperative simple8b delta decode straight to global memory: dst[i] = first + sum_{j<=i} d(u_j) for i < cap.

@@ -54,16 +54,6 @@ double plan_selected_fraction(const uint32_t *arena_series, uint64_t n_arena, co
   return std::min(1.0, (double)in_range / (double)n_arena);
 }
 
-bool plan_use_cooperative(double est_selected_pages, int sm_count, int min_blocks_per_sm, int threads_per_block) {
-  return est_selected_pages < 0.25 * (double)sm_count * min_blocks_per_sm * threads_per_block;
-}
-
-uint32_t plan_gorilla_group(double est_gorilla_pages, double resident_warps) {
-  uint32_t g = 1;
-  while (g < 32 && est_gorilla_pages / g > 0.75 * resident_warps) g *= 2;
-  return g;
-}
-
 void plan_serial_grids(int n_bins, const double *chunks, const double *t_chunk, const int *occ, int sm_count,
                        int warps_per_block, int *grid_out) {
   std::vector<double> cand;

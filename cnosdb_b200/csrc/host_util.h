@@ -36,12 +36,6 @@ bool parse_page(const uint8_t *page, uint64_t size, PageHeader *out);
 // caller hands the whole selection to every shard): only ids inside the arena's id range can match.
 // Both lists sorted ascending; n_sel == 0 with sel == nullptr means "all series".
 double plan_selected_fraction(const uint32_t *arena_series, uint64_t n_arena, const uint32_t *sel, uint64_t n_sel);
-// Cooperative (warp-per-page) kernels for the eligible bins when the selected pages cannot fill the machine with
-// lane-per-page work (>= ~1/4 of the resident lanes), where one page's serial decode would be the makespan.
-bool plan_use_cooperative(double est_selected_pages, int sm_count, int min_blocks_per_sm, int threads_per_block);
-// Pages per warp task of the cooperative gorilla bins: the smallest power of two that fits the tasks in 3/4 of the
-// resident warps (H100, 1/8 of C4: groups of 1-8 pages all take 0.8-1.2 ms, no size is consistently best).
-uint32_t plan_gorilla_group(double est_gorilla_pages, double resident_warps);
 // Grid sizes of the lane-per-page kernels of one scan (one persistent kernel per decode-kind bin, all launched
 // concurrently; a warp repeatedly takes a chunk of 32 pages of its bin). A chunk is ONE serial task of t_chunk[b]
 // (relative units: rows x cost of the bin's codec pair), so a bin finishes after ceil(chunks / warps) rounds of

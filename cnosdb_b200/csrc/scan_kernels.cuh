@@ -18,11 +18,15 @@ constexpr uint32_t FULL = 0xffffffffu;
 constexpr int MAX_RANGES = 8;
 constexpr int N_TK = 3;  // time-cursor specialisations: RLE, S8B scaled, generic
 constexpr int N_VK = 3;  // value-cursor specialisations: S8B zig-zag, gorilla, generic
-constexpr int N_SERIAL_BINS = N_TK * N_VK;  // lane-per-page kernels (scan_kernels.cuh)
-// + warp-cooperative kernels (coop_kernels.cuh): zig-zag simple8b or gorilla values (<= COOP_TILE rows) with
-// RLE / simple8b timestamps
-enum { BIN_COOP_RLE_S8B = N_SERIAL_BINS, BIN_COOP_S8B_S8B = N_SERIAL_BINS + 1, BIN_COOP_RLE_GOR = N_SERIAL_BINS + 2,
-       BIN_COOP_S8B_GOR = N_SERIAL_BINS + 3 };
+constexpr int N_SERIAL_BINS = N_TK * N_VK;  // bins 0-8: time class * N_VK + value class
+// + the short-page bins: zig-zag simple8b or gorilla values of at most SHORT_PAGE_ROWS rows with RLE / simple8b
+// timestamps. The kernel of the matching class (serial_bin_of) runs them; they stay apart because plan_bin_parts sizes
+// a bin's parts from its longest page (short pages in a bin with long ones would get coarser parts), because each
+// bin stream's priority is its chunk_cost rank among all the bins, and because the dominant_kernel_bin counter and
+// the benchmark report these bin numbers.
+constexpr uint32_t SHORT_PAGE_ROWS = 1024;
+enum { BIN_SHORT_RLE_S8B = N_SERIAL_BINS, BIN_SHORT_S8B_S8B = N_SERIAL_BINS + 1, BIN_SHORT_RLE_GOR = N_SERIAL_BINS + 2,
+       BIN_SHORT_S8B_GOR = N_SERIAL_BINS + 3 };
 constexpr int N_BINS = N_SERIAL_BINS + 4;
 
 enum { TK_RLE = 0, TK_S8B = 1, TK_GEN = 2 };

@@ -142,7 +142,6 @@ struct tskv_scan {
   uint32_t *d_work_page = nullptr, *d_work_slot = nullptr;
   uint8_t *d_work_qcol = nullptr;
   uint32_t *d_bin_cstart = nullptr;  // [N_BINS+1] then [1] total
-  uint32_t *d_gor_scratch[2] = {nullptr, nullptr};  // element records of the cooperative gorilla bins
   ColState *d_cols = nullptr;
   OutCol *d_outs = nullptr;
   MeanExport *d_means = nullptr;
@@ -157,8 +156,6 @@ struct tskv_scan {
   uint8_t *d_validity = nullptr;
   int grid[N_BINS] = {0};
   int occ[N_BINS] = {0};  // resident CTAs per SM of each bin's kernel at this scan's shared memory size
-  bool use_coop[N_BINS] = {false};  // cooperative-eligible bins: which kernel family runs them
-  CoopParams coop{};
   tskv_ctx *ctx = nullptr;
   uint32_t n_series_sel = 0;
   bool enqueued = false;
@@ -262,20 +259,13 @@ scan_kernel_t scan_kernel_for(int bin, int narrow = NARROW_NONE) {
     default: return k_scan_aggregate<TK_GEN, VK_GEN, SEL, NARROW_NONE>;
   }
 }
-// relative cost of one item of a bin (sizes the bins' shares of the SMs)
-// serial (lane-per-page) kernel bin whose code also handles a cooperative-eligible bin
+// the bin among 0-8 whose lane-per-page kernel also runs a short-page bin
 int serial_bin_of(int bin) {
-  if (bin == BIN_COOP_RLE_S8B) return TK_RLE * N_VK + VK_S8B;
-  if (bin == BIN_COOP_S8B_S8B) return TK_S8B * N_VK + VK_S8B;
-  if (bin == BIN_COOP_RLE_GOR) return TK_RLE * N_VK + VK_GOR;
-  if (bin == BIN_COOP_S8B_GOR) return TK_S8B * N_VK + VK_GOR;
+  if (bin == BIN_SHORT_RLE_S8B) return TK_RLE * N_VK + VK_S8B;
+  if (bin == BIN_SHORT_S8B_S8B) return TK_S8B * N_VK + VK_S8B;
+  if (bin == BIN_SHORT_RLE_GOR) return TK_RLE * N_VK + VK_GOR;
+  if (bin == BIN_SHORT_S8B_GOR) return TK_S8B * N_VK + VK_GOR;
   return bin;
-}
-bool is_gor_coop_bin(int bin) { return bin == BIN_COOP_RLE_GOR || bin == BIN_COOP_S8B_GOR; }
-double bin_cost(int bin, bool coop) {
-  static const double tk[N_TK] = {1.0, 1.5, 2.0}, vk[N_VK] = {1.0, 1.4, 1.6};
-  const int sb = serial_bin_of(bin);
-  return tk[sb / N_VK] * vk[sb % N_VK] * (coop ? 1.8 : 1.0);
 }
 
 // dynamic shared memory of a lane-per-page kernel: the per-CTA table + the warps' staging rings and flush areas + the
@@ -291,31 +281,6 @@ double chunk_cost(int bin) {
   static const double tk[N_TK] = {0.0, 0.16, 0.35}, vk[N_VK] = {0.28, 0.31, 0.45};
   const int sb = serial_bin_of(bin);
   return tk[sb / N_VK] + vk[sb % N_VK];
-}
-size_t coop_smem_bytes(int bin, uint32_t table_words) {
-  size_t per_warp = bin == BIN_COOP_S8B_S8B   ? sizeof(CoopSmem<true, false>)
-                    : bin == BIN_COOP_RLE_S8B ? sizeof(CoopSmem<false, false>)
-                    : bin == BIN_COOP_S8B_GOR ? sizeof(CoopSmem<true, true>)
-                                              : sizeof(CoopSmem<false, true>);
-  per_warp = (per_warp + 15) & ~(size_t)15;
-  return (size_t)((table_words + 1) & ~1u) * 8 + per_warp * (SCAN_THREADS / 32);
-}
-const void *coop_kernel_for(int bin, bool sel) {
-  switch (bin) {
-    case BIN_COOP_RLE_S8B: return sel ? (const void *)k_scan_coop<TK_RLE, VK_S8B, true> : (const void *)k_scan_coop<TK_RLE, VK_S8B, false>;
-    case BIN_COOP_S8B_S8B: return sel ? (const void *)k_scan_coop<TK_S8B, VK_S8B, true> : (const void *)k_scan_coop<TK_S8B, VK_S8B, false>;
-    case BIN_COOP_RLE_GOR: return sel ? (const void *)k_scan_coop<TK_RLE, VK_GOR, true> : (const void *)k_scan_coop<TK_RLE, VK_GOR, false>;
-    default: return sel ? (const void *)k_scan_coop<TK_S8B, VK_GOR, true> : (const void *)k_scan_coop<TK_S8B, VK_GOR, false>;
-  }
-}
-
-MagicDiv make_magic(uint64_t d) {  // d >= 1
-  MagicDiv md{0, 0};
-  uint32_t l = 0;
-  while (l < 64 && ((unsigned __int128)1 << l) < d) l++;
-  md.l = l;
-  if (l) md.m = (uint64_t)(((((unsigned __int128)1 << l) - d) << 64) / d) + 1;
-  return md;
 }
 
 // Lazily computes the arena's min / max timestamp on the device (one lane per time page).
@@ -507,7 +472,7 @@ void free_scan(tskv_scan *s) {
   cudaStream_t st = s->ctx ? s->ctx->stream : nullptr;
   void *bufs[] = {s->d_series, s->d_rank_slot, s->d_bucket, s->d_cg_slot, s->d_item_flag, s->d_block_count, s->d_work_page, s->d_work_slot,
                   s->d_work_qcol, s->d_bin_cstart, s->d_cols, s->d_outs, s->d_means, s->d_state,
-                  s->d_task_counter, s->d_values, s->d_validity, s->d_gor_scratch[0], s->d_gor_scratch[1], s->d_gathered, s->d_row_keep,
+                  s->d_task_counter, s->d_values, s->d_validity, s->d_gathered, s->d_row_keep,
                   s->d_mcg_active, s->d_mvals, s->d_mvalid, s->d_mpage, s->d_mrow_off, s->d_mbm_off, s->d_pane_state, s->d_combine,
                   s->d_slot_group, s->d_walk};
   for (void *b : bufs)
@@ -686,10 +651,6 @@ tskv_status tskvgpu_ctx_create(int32_t device_id, tskv_ctx **out_ctx) {
       for (int nm = NARROW_NONE; nm <= NARROW_ALL; nm++) raise((const void *)scan_kernel_for<false>(b, nm));
       raise((const void *)scan_kernel_for<true>(b));
     }
-    for (int b = N_SERIAL_BINS; b < N_BINS; b++) {
-      raise(coop_kernel_for(b, false));
-      raise(coop_kernel_for(b, true));
-    }
     cudaGetLastError();
   }
   // per-scan buffers come from the stream-ordered pool; keep freed memory cached in the pool
@@ -863,12 +824,10 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
       const tskv_page_desc &td = pg->h_descs[time_page_of[item_page[k]]];
       int tclass = time_has_nulls[time_page_of[item_page[k]]] ? TK_GEN : time_class(td.reserved);
       uint64_t bin = (uint64_t)tclass * N_VK + value_class(vd.reserved);
-      // pages that decode in parallel go to the warp-cooperative kernels
-      static const bool no_coop = getenv("TSKV_NO_COOP") != nullptr;
-      if (!no_coop && vd.num_values <= COOP_TILE && vd.reserved == DK_S8B_ZZ && tclass != TK_GEN)
-        bin = tclass == TK_RLE ? BIN_COOP_RLE_S8B : BIN_COOP_S8B_S8B;
-      if (!no_coop && vd.num_values <= COOP_TILE && vd.reserved == DK_GORILLA && tclass != TK_GEN)
-        bin = tclass == TK_RLE ? BIN_COOP_RLE_GOR : BIN_COOP_S8B_GOR;
+      if (vd.num_values <= SHORT_PAGE_ROWS && vd.reserved == DK_S8B_ZZ && tclass != TK_GEN)
+        bin = tclass == TK_RLE ? BIN_SHORT_RLE_S8B : BIN_SHORT_S8B_S8B;
+      if (vd.num_values <= SHORT_PAGE_ROWS && vd.reserved == DK_GORILLA && tclass != TK_GEN)
+        bin = tclass == TK_RLE ? BIN_SHORT_RLE_GOR : BIN_SHORT_S8B_GOR;
       key[k] = (bin << 48) | ((uint64_t)vd.column_id << 32) | k;
       order[k] = k;
       page_bin[item_page[k]] = (uint8_t)bin;
@@ -1750,37 +1709,10 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   }
 
   {
-    // Cooperative (one page per warp) vs lane-per-page for the eligible bins: lane-per-page needs fewer
-    // instructions per point but one page is a long serial chain, so it only pays when the selected
-    // pages can fill the machine (>= ~1/4 of the resident lanes); otherwise go cooperative.
-    const char *mode = getenv("TSKV_COOP");  // "0" never, "1" always, unset = auto
     const double sel_frac = plan_selected_fraction(pages->series.data(), pages->series.size(), q->series_ids, q->n_series);
-    const double est_total = (double)pages->n_items * sel_frac;  // selected field pages, all bins
-    for (int b = N_SERIAL_BINS; b < N_BINS; b++)
-      // The lane-per-page kernels (staged streams, fused row loops, cut pages) beat the cooperative kernels even on
-      // small shards (H100, 1/8 of C4: 0.23 ms vs 0.81-1.16 ms per scan), so those run only on request.
-      s->use_coop[b] = (pages->n_tomb_ranges || q->n_predicates) ? false  // tombstones / row filters: lane-per-page kernels only
-                       : mode             ? (mode[0] == '1')
-                                          : false;
-    (void)est_total;
     // Grid sizes. Every kernel is persistent (warps pull tasks from their bin's counter). If the resident
     // capacity allows, each bin gets one warp per estimated task (a single round: the makespan of a bin is
-    // quantised in units of one task = one page's serial decode); otherwise the blocks are split by cost.
-    // Gorilla coop bins: pages per warp task (phase 1 parses them lane-per-page) so that the selected pages make
-    // about one task per resident warp; TSKV_GOR_GROUP overrides.
-    uint32_t gor_group = 1;
-    {
-      double est_gor = 0;
-      for (int b = N_SERIAL_BINS; b < N_BINS; b++)
-        if (is_gor_coop_bin(b) && s->use_coop[b]) est_gor += (pages->h_bin_start[b + 1] - pages->h_bin_start[b]) * sel_frac;
-      int gocc = 0;  // resident CTAs per SM of the gorilla cooperative kernel (shared memory bound)
-      const void *gfn = coop_kernel_for(BIN_COOP_RLE_GOR, s->has_sel);
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&gocc, gfn, SCAN_THREADS, coop_smem_bytes(BIN_COOP_RLE_GOR, P.smem_words));
-      const double resident_warps = (double)ctx->sm_count * std::max(1, gocc) * (SCAN_THREADS / 32);
-      gor_group = plan_gorilla_group(est_gor, resident_warps);
-      if (const char *g = getenv("TSKV_GOR_GROUP")) gor_group = (uint32_t)std::min(32, std::max(1, atoi(g)));
-      s->coop.gor_group = gor_group;
-    }
+    // quantised in units of one task = one chunk's serial decode); otherwise plan_serial_grids splits the blocks.
     // Pages cut at restart points (skip_kernels.cuh): a chunk of 32 whole pages is one serial task of ~1000 rows; with
     // few selected pages that chain is the scan's makespan, and with many the makespan is still quantised in chunk
     // times. Cut the pages of the simple8b / gorilla bins into parts so that the scan has about PARTS_TARGET chunks
@@ -1799,7 +1731,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
       if (parts_env) want = (uint32_t)std::max(1, atoi(parts_env));
       for (int b = 0; b < N_BINS; b++) {
         const int sb = serial_bin_of(b);
-        if (s->use_coop[b] || sb / N_VK == TK_GEN || sb % N_VK == VK_GEN) continue;
+        if (sb / N_VK == TK_GEN || sb % N_VK == VK_GEN) continue;
         uint32_t want_b = want;
         if (sb / N_VK == TK_S8B) {  // TSKV_PARTS_TS: another number of parts for the simple8b-timestamp bins (their rows cost
           // ~1.6 x the rows of RLE-timestamp pages; H100, C4: twice the parts changes nothing, 1.03-1.05 vs 1.02 ms per scan)
@@ -1812,27 +1744,20 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
         P.bin_part_rows[b] = part_rows;
       }
     }
-    double w[N_BINS], wsum = 0, need_sum = 0, occ_weighted = 0;
+    double need_sum = 0, occ_weighted = 0;
     int need[N_BINS] = {0}, occ_bin[N_BINS] = {0};
     for (int b = 0; b < N_BINS; b++) {
       uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
-      w[b] = n_bin * bin_cost(b, s->use_coop[b]);
-      wsum += w[b];
       if (!n_bin) continue;
       int occ = 0;
-      if (!s->use_coop[b]) {
-        const int sb = serial_bin_of(b);
-        const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, SCAN_THREADS, serial_smem_bytes(sb, P.smem_words, P.has_tomb));
-      } else {
-        const void *fn = coop_kernel_for(b, s->has_sel);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, SCAN_THREADS, coop_smem_bytes(b, P.smem_words));
-      }
+      const int sb = serial_bin_of(b);
+      const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, SCAN_THREADS, serial_smem_bytes(sb, P.smem_words, P.has_tomb));
       occ = std::max(1, occ);
       occ_bin[b] = occ;
       s->occ[b] = occ;
       const double est_items = n_bin * sel_frac * 1.02 + 32;
-      const uint32_t per_task = !s->use_coop[b] ? 32u : is_gor_coop_bin(b) ? gor_group : 1u;  // pages per warp task
+      const uint32_t per_task = 32;  // pages per warp task: one chunk
       const double tasks = est_items / per_task * parts[b];
       need[b] = (int)(tasks / (SCAN_THREADS / 32)) + 1;
       need[b] = std::min(need[b], (int)(((uint64_t)(n_bin + per_task - 1) / per_task * parts[b] + SCAN_THREADS / 32 - 1) / (SCAN_THREADS / 32)));
@@ -1840,14 +1765,12 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
       occ_weighted += (double)need[b] * occ;
     }
     const double capacity = need_sum > 0 ? (occ_weighted / need_sum) * ctx->sm_count : 0;  // resident blocks, mixed kernels
-    bool any_coop = false;
-    for (int b = N_SERIAL_BINS; b < N_BINS; b++) any_coop |= s->use_coop[b] && need[b];
     if (need_sum <= capacity) {
       for (int b = 0; b < N_BINS; b++)
         if (need[b]) s->grid[b] = std::max(1, need[b]);
-    } else if (!any_coop) {
-      // lane-per-page kernels only: a chunk of 32 pages is one long serial task, so a bin's time is quantised in rounds
-      // of its chunk time - choose the grids that minimise the makespan (plan_serial_grids)
+    } else {
+      // a chunk of 32 pages is one long serial task, so a bin's time is quantised in rounds of its chunk time - choose
+      // the grids that minimise the makespan (plan_serial_grids)
       double chunks[N_BINS], t_chunk[N_BINS];
       for (int b = 0; b < N_BINS; b++) {
         const uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
@@ -1872,45 +1795,6 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
       const char *gm = getenv("TSKV_GRID_MODE");
       if (gm && gm[0] == '1')
         for (int b = 0; b < N_BINS; b++) s->grid[b] = need[b];
-    } else {
-      // water-filling: bins that need less than their cost share keep their need, the rest split what is left
-      bool fixed[N_BINS] = {false};
-      double cap_left = capacity, w_left = 0;
-      for (int b = 0; b < N_BINS; b++) w_left += need[b] ? w[b] : 0;
-      for (int round = 0; round < N_BINS; round++) {
-        bool changed = false;
-        for (int b = 0; b < N_BINS; b++) {
-          if (!need[b] || fixed[b]) continue;
-          if (need[b] <= cap_left * w[b] / w_left) {
-            s->grid[b] = std::max(1, need[b]);
-            fixed[b] = true;
-            cap_left -= s->grid[b];
-            w_left -= w[b];
-            changed = true;
-          }
-        }
-        if (!changed) break;
-      }
-      for (int b = 0; b < N_BINS; b++)
-        if (need[b] && !fixed[b]) s->grid[b] = std::max(1, std::min(need[b], (int)(cap_left * w[b] / w_left + 0.5)));
-    }
-    for (int b = N_SERIAL_BINS; b < N_BINS; b++) {
-      if (!is_gor_coop_bin(b) || !s->use_coop[b] || !s->grid[b]) continue;
-      const int k = b == BIN_COOP_RLE_GOR ? 0 : 1;
-      const size_t words = (size_t)s->grid[b] * (SCAN_THREADS / 32) * gor_group * GOR_REC_STRIDE;
-      if (stream_alloc(ctx, &s->d_gor_scratch[k], words) != cudaSuccess) {
-        ctx->set_error("scan_prepare: out of memory for the gorilla record scratch");
-        free_scan(s);
-        return TSKV_ERR_OOM;
-      }
-      s->coop.gor_scratch[k] = s->d_gor_scratch[k];
-    }
-    // bucket arithmetic of the cooperative kernels: multiply-high division by the invariant width
-    if (P.width > 0) {
-      s->coop.div = make_magic((uint64_t)P.width);
-      const int64_t d0 = (int64_t)((uint64_t)P.first_bucket_start - (uint64_t)P.origin_mod + (uint64_t)P.width);
-      s->coop.grid_ok = (d0 >= 0 && d0 % P.width == 0) ? 1u : 0u;
-      s->coop.q0 = s->coop.grid_ok ? d0 / P.width : 0;
     }
   }
   // ---- merge pass over the overlapping chunks (merge_kernels.cuh): which merge column groups this scan reads
@@ -2188,17 +2072,11 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       launches++;
     }
     if (!capturing) cudaEventRecord(s->ev_bin_start[b], ctx->bin_stream[b]);
-    if (!s->use_coop[b]) {
-      const int sb = serial_bin_of(b);
-      void *args[] = {(void *)&s->params, (void *)&bin};
-      const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
-      CU_TRY(ctx, cudaLaunchKernel(fn, dim3(s->grid[b]), dim3(SCAN_THREADS), args, serial_smem_bytes(sb, s->params.smem_words, s->params.has_tomb),
-                                   ctx->bin_stream[b]));
-    } else {
-      void *args[] = {(void *)&s->params, (void *)&s->coop, (void *)&bin};
-      CU_TRY(ctx, cudaLaunchKernel(coop_kernel_for(b, s->has_sel), dim3(s->grid[b]), dim3(SCAN_THREADS), args,
-                                   coop_smem_bytes(b, s->params.smem_words), ctx->bin_stream[b]));
-    }
+    const int sb = serial_bin_of(b);
+    void *args[] = {(void *)&s->params, (void *)&bin};
+    const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
+    CU_TRY(ctx, cudaLaunchKernel(fn, dim3(s->grid[b]), dim3(SCAN_THREADS), args, serial_smem_bytes(sb, s->params.smem_words, s->params.has_tomb),
+                                 ctx->bin_stream[b]));
     cudaEvent_t ev_done = capturing ? s->ev_cjoin[b] : s->ev_bin_done[b];
     cudaEventRecord(ev_done, ctx->bin_stream[b]);
     cudaStreamWaitEvent(ctx->stream, ev_done, 0);  // join
@@ -2267,8 +2145,8 @@ static tskv_status sync_scan(tskv_ctx *ctx, tskv_scan *s) {
     if (getenv("TSKV_DEBUG_BINS")) {
       float t0 = 0;
       cudaEventElapsedTime(&t0, s->ev_bin[0], s->ev_bin_start[b]);
-      fprintf(stderr, "[tskv] bin %d%s grid %d, %d CTAs/SM: start +%.3f ms, run %.3f ms, %llu bytes\n", b,
-              s->use_coop[b] ? " (coop)" : "", s->grid[b], s->occ[b], t0, t, aux[4 + b]);
+      fprintf(stderr, "[tskv] bin %d grid %d, %d CTAs/SM: start +%.3f ms, run %.3f ms, %llu bytes\n", b,
+              s->grid[b], s->occ[b], t0, t, aux[4 + b]);
     }
     if (t > ctx->counters.dominant_kernel_ms) {
       ctx->counters.dominant_kernel_ms = t;

@@ -195,7 +195,8 @@ typedef struct tskv_counters {
   double elapsed_fused_ms;      /* device time of the fused decode/filter/reduce kernels alone */
   double dominant_kernel_ms;    /* slowest fused kernel (one per decode-kind bin) of the last scan */
   uint64_t dominant_kernel_bytes; /* encoded page bytes that kernel read (its algorithmic bytes) */
-  uint64_t dominant_kernel_bin; /* time-codec class * 3 + value-codec class (see DESIGN.md) */
+  uint64_t dominant_kernel_bin; /* 0-8: time-codec class * 3 + value-codec class; 9-12: the short-page bins
+                                   (pages of <= 1024 rows, see DESIGN.md) */
   uint64_t h2d_bytes;           /* query arguments copied host->device by the last prepare */
   uint64_t pruned_page_count;   /* selected field pages the last scan skipped because their column group's time bounds
                                    miss every query range (filter_column_groups, reader/chunk.rs:12-50) */

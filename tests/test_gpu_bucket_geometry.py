@@ -1,9 +1,8 @@
 """The fused scan's bucket arithmetic at the edges of its time geometry (see GEOMETRY_CASES in tests/helpers.py): steps
 from 0 to 2^40 + 3, widths that are and are not multiples of the step, narrower than it, up to 2^63 - 1, origins that are
 negative or >= the width, rows on both sides of the truncating-% regime and at the i64 limits, and time ranges on, beside
-and between rows and bucket edges. Every query runs with the cooperative kernels off and on and with pages whole or cut
-into 3 parts, and every single-range query runs again with its range split in two (two ranges turn the row-space fast
-path off): COUNT / SUM / MIN / MAX must be bit-identical across the two and equal the exact reference; FIRST / LAST are
+and between rows and bucket edges. Every query runs with pages whole and cut into 3 parts, and every single-range query
+runs again with its range split in two (two ranges turn the row-space fast path off): COUNT / SUM / MIN / MAX must be bit-identical across the two and equal the exact reference; FIRST / LAST are
 compared with the oracle."""
 import numpy as np
 import pytest
@@ -17,7 +16,7 @@ from tests.helpers import (GEOM_BLOCK, GEOMETRY_CASES, I64_MIN, ReferenceError, 
 
 pytestmark = pytest.mark.gpu
 
-ENVS = [("0", "1"), ("0", "3"), ("1", "1"), ("1", "3")]  # (TSKV_COOP, TSKV_PARTS)
+ENVS = ("1", "3")  # TSKV_PARTS
 
 
 def _scan(engine, pages, q):
@@ -79,10 +78,9 @@ def test_bucket_geometry(engine, case, monkeypatch):
                 # deviation, DESIGN section 7)
                 ora = orc.scan_aggregate(arena, descs, q) if (sel and step and err is None and not unsupported and
                                                                not (qname == "by_series" and t0 == I64_MIN)) else None
-                for coop, parts in ENVS:
-                    monkeypatch.setenv("TSKV_COOP", coop)
+                for parts in ENVS:
                     monkeypatch.setenv("TSKV_PARTS", parts)
-                    wh = "%s coop=%s parts=%s" % (what, coop, parts)
+                    wh = "%s parts=%s" % (what, parts)
                     got, st = _scan(engine, pages, q)
                     if unsupported:
                         assert st == cabi.TSKV_ERR_UNSUPPORTED, wh
@@ -107,8 +105,7 @@ def test_bucket_geometry(engine, case, monkeypatch):
                     with pytest.raises(orc.OracleError) as oe:
                         orc.scan_aggregate(arena, descs, q)
                     assert oe.value.status == cabi.TSKV_ERR_BUCKET_RANGE
-                    for coop, parts in ENVS:
-                        monkeypatch.setenv("TSKV_COOP", coop)
+                    for parts in ENVS:
                         monkeypatch.setenv("TSKV_PARTS", parts)
                         assert _scan(engine, pages, q)[1] == cabi.TSKV_ERR_BUCKET_RANGE, "%s short grid %d" % (name, fbs)
     pages.close()

@@ -1,7 +1,6 @@
 """f64 pages of IEEE special values and adversarial bit patterns through every Gorilla decoder of the scan (see
 f64_edge_arena in tests/helpers.py): GorillaCursor (k_decode_warp, the generic-time rows loop), GorillaRing (the fused
-bins, k_build_skip's restart points, pages cut into parts) and the cooperative two-phase parse, next to the raw twin of
-every page. COUNT / MIN / MAX (IEEE totalOrder, so the NaN keys 0x7FFF...FFFF and 0xFFFF...FFFF are the MIN and MAX
+bins, k_build_skip's restart points, pages cut into parts), next to the raw twin of every page. COUNT / MIN / MAX (IEEE totalOrder, so the NaN keys 0x7FFF...FFFF and 0xFFFF...FFFF are the MIN and MAX
 identities) must equal the exact reference bit for bit, SUM / MEAN its class (NaN, the exact inf, or finite within the
 order-free bound, +0.0 when zero), and FIRST / LAST the oracle bit for bit, NaN payloads included."""
 import numpy as np
@@ -15,8 +14,7 @@ from tests.helpers import (ALL_AGGS, F64_FIELDS, F64_LENGTHS, F64_SERIES, F64_ST
 
 pytestmark = pytest.mark.gpu
 
-# (TSKV_COOP, TSKV_PARTS, TSKV_GOR_GROUP)
-ENVS = [("0", "1", None), ("0", "3", None), ("1", "1", "1"), ("1", "3", "32"), ("1", "1", "32"), ("1", "3", "1")]
+ENVS = ("1", "3")  # TSKV_PARTS
 
 
 def _first_last_equal(got, exp, what):
@@ -44,16 +42,6 @@ def _check(got, exp, ora, what):
         _first_last_equal(got, ora, what)
 
 
-def _set_env(monkeypatch, env):
-    coop, parts, group = env
-    monkeypatch.setenv("TSKV_COOP", coop)
-    monkeypatch.setenv("TSKV_PARTS", parts)
-    if group is None:
-        monkeypatch.delenv("TSKV_GOR_GROUP", raising=False)
-    else:
-        monkeypatch.setenv("TSKV_GOR_GROUP", group)
-
-
 @pytest.mark.parametrize("n", F64_LENGTHS)
 def test_f64_edges(engine, n, monkeypatch):
     arena, descs, truth = f64_edge_arena(n, n)
@@ -73,11 +61,11 @@ def test_f64_edges(engine, n, monkeypatch):
         sel = any(c.agg_mask & (cabi.TSKV_AGG_FIRST | cabi.TSKV_AGG_LAST) for c in q.columns)
         ora = orc.scan_aggregate(arena, descs, q) if sel else None
         kw = dict(slide=extra.get("slide"), group_ids=extra.get("group_ids"), n_groups=extra.get("n_groups"))
-        for env in ENVS:
-            _set_env(monkeypatch, env)
-            what = "n=%d %s env=%s" % (n, name, env)
+        for parts in ENVS:
+            monkeypatch.setenv("TSKV_PARTS", parts)
+            what = "n=%d %s parts=%s" % (n, name, parts)
             _check(engine.scan_aggregate(pages, q, **kw), exp, ora, what)
-        _set_env(monkeypatch, ENVS[0])
+        monkeypatch.setenv("TSKV_PARTS", ENVS[0])
         _check(engine.scan_aggregate(hp, q, **kw), exp, ora, "n=%d %s host-resident" % (n, name))
         if name == "bucket+sel":  # a second pass of a prepared scan replays its graph
             s = engine.prepare(pages, q)

@@ -20,7 +20,7 @@ from tests.test_gpu_parity import random_tombstones
 
 pytestmark = pytest.mark.gpu
 
-ENVS = [("0", "1"), ("0", "3"), ("1", "1"), ("1", "3")]  # (TSKV_COOP, TSKV_PARTS)
+ENVS = ("1", "3")  # TSKV_PARTS
 FIELDS = ((1, cabi.TSKV_PT_I64), (2, cabi.TSKV_PT_F64), (3, cabi.TSKV_PT_U64))
 AGGS = ("count", "sum", "min", "max", "mean")
 
@@ -81,8 +81,7 @@ def make_map(rng, n_slots, n_groups):
     return ids
 
 
-def _set_env(monkeypatch, coop, parts):
-    monkeypatch.setenv("TSKV_COOP", coop)
+def _set_env(monkeypatch, parts):
     monkeypatch.setenv("TSKV_PARTS", parts)
 
 
@@ -99,9 +98,9 @@ def test_identities(engine, monkeypatch):
         q = make_query(FIELDS, ALL_AGGS, width=30_000, origin=11, first_bucket_start=fbs, n_buckets=nb, series_ids=ids)
         gbs = make_query(FIELDS, ALL_AGGS, width=30_000, origin=11, first_bucket_start=fbs, n_buckets=nb, series_ids=ids,
                          group_by_series=True)
-        for coop, parts in ENVS:
-            _set_env(monkeypatch, coop, parts)
-            what = "sel=%s coop=%s parts=%s" % (ids is not None, coop, parts)
+        for parts in ENVS:
+            _set_env(monkeypatch, parts)
+            what = "sel=%s parts=%s" % (ids is not None, parts)
             assert_same(engine.scan_aggregate(pages, q, group_ids=np.zeros(n, dtype=np.uint32), n_groups=1),
                         engine.scan_aggregate(pages, q), "one group " + what)
             assert_same(engine.scan_aggregate(pages, q, group_ids=np.arange(n, dtype=np.uint32), n_groups=n),
@@ -137,10 +136,10 @@ def test_subset_equivalence(engine, monkeypatch):
                            predicates=pr, time_ranges=[(1_020_000, 1_500_000)])
             for n_groups in (2, 7, 64, len(slot_ids) // 3):
                 gmap = make_map(rng, len(slot_ids), n_groups)
-                for coop, parts in ENVS:
-                    _set_env(monkeypatch, coop, parts)
-                    assert_groups_match_subsets(engine, pages, q, gmap, n_groups, slot_ids, "%s sel=%s G=%d coop=%s parts=%s" % (
-                        name, ids is not None, n_groups, coop, parts))
+                for parts in ENVS:
+                    _set_env(monkeypatch, parts)
+                    assert_groups_match_subsets(engine, pages, q, gmap, n_groups, slot_ids, "%s sel=%s G=%d parts=%s" % (
+                        name, ids is not None, n_groups, parts))
         pages.close()
 
 
@@ -165,9 +164,9 @@ def test_exact_reference_geometry(engine, case, monkeypatch):
                 exp, err = exact_aggregate_grouped(truth, q, gmap, n_groups), None
             except ReferenceError as e:
                 exp, err = None, e.status
-            for coop, parts in ENVS:
-                _set_env(monkeypatch, coop, parts)
-                what = "%s %s %s coop=%s parts=%s" % (name, kind, lname, coop, parts)
+            for parts in ENVS:
+                _set_env(monkeypatch, parts)
+                what = "%s %s %s parts=%s" % (name, kind, lname, parts)
                 try:
                     got, st = engine.scan_aggregate(pages, q, group_ids=gmap, n_groups=n_groups), None
                 except TskvError as e:
@@ -205,9 +204,9 @@ def test_other_paths(engine, monkeypatch):
         for env, val in (("TSKV_WORKLIST", "items"), ("TSKV_SMEM_TABLE_KB", "0")):
             with monkeypatch.context() as m:
                 m.setenv(env, val)
-                for coop, parts in ENVS[::3]:
-                    _set_env(m, coop, parts)
-                    assert_groups_match_subsets(engine, dp, q, gmap, 7, all_ids, "%s=%s %s coop=%s" % (env, val, aggs, coop))
+                for parts in ENVS:
+                    _set_env(m, parts)
+                    assert_groups_match_subsets(engine, dp, q, gmap, 7, all_ids, "%s=%s %s parts=%s" % (env, val, aggs, parts))
     hp.close()
     dp.close()
 
@@ -222,9 +221,9 @@ def test_sliding_windows(engine, monkeypatch):
     ids = np.arange(60, dtype=np.uint32)
     for n_groups in (2, 7, 20):
         gmap = make_map(rng, 60, n_groups)
-        for coop, parts in ENVS:
-            _set_env(monkeypatch, coop, parts)
-            assert_groups_match_subsets(engine, pages, q, gmap, n_groups, ids, "sliding G=%d coop=%s parts=%s" % (n_groups, coop, parts),
+        for parts in ENVS:
+            _set_env(monkeypatch, parts)
+            assert_groups_match_subsets(engine, pages, q, gmap, n_groups, ids, "sliding G=%d parts=%s" % (n_groups, parts),
                                         slide=slide)
     # slide == window: the tumbling grouped scan
     fbs, nb = bucket_spec(1_000_000 - 2_000, 1_000_000 + 1_200_000, window)

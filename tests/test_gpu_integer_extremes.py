@@ -3,7 +3,7 @@ values near the i64 / u64 limits (simple8b walks, cancelling blocks of +-2^62..2
 pages), 2 000 series into a few cells (the table atomics carry into the high word), and 102 400-row pages of INT64_MAX.
 SUM must equal S mod 2^64 and MEAN float(S) / float(n), bit for bit; COUNT / MIN / MAX exactly. f64 columns (magnitudes
 up to 1e290, cancelling +-1e16 blocks, +-0.0) stay within the order-free bound of their exact sum. The data runs through
-the uniform bucket schedule, the segment loop, the FIRST / LAST kernels, the cooperative kernels, group_by_series, the
+the uniform bucket schedule, the segment loop, the FIRST / LAST kernels, group_by_series, the
 global-atomics table, the overlap merge and a two-shard exchange."""
 from fractions import Fraction
 
@@ -102,10 +102,9 @@ def queries(nb_rows):
     ]
 
 
-@pytest.mark.parametrize("env", ["default", "coop", "global_atomics", "parts3"])
+@pytest.mark.parametrize("env", ["default", "global_atomics", "parts3"])
 def test_integer_extremes_are_exact(engine, extremes, env, monkeypatch):
     arena, descs, truth = extremes
-    monkeypatch.setenv("TSKV_COOP", "1" if env == "coop" else "0")
     monkeypatch.setenv("TSKV_PARTS", "3" if env == "parts3" else "1")
     if env == "global_atomics":
         monkeypatch.setenv("TSKV_SMEM_TABLE_KB", "0")

@@ -6,7 +6,7 @@ import pytest
 from cnosdb_b200 import cabi, datagen
 from cnosdb_b200.engine import PushedAggregate, QueryOption, TskvError
 from oracle import pyoracle as orc
-from tests.helpers import ALL_AGGS, assert_results_equal, bucket_spec, make_query, random_arena
+from tests.helpers import ALL_AGGS, assert_results_equal, bucket_spec, make_query, random_arena, time_page_is_rle
 
 pytestmark = pytest.mark.gpu
 
@@ -409,23 +409,21 @@ def test_two_shard_exchange_matches_whole_scan(engine):
         pages.close()
 
 
-@pytest.mark.parametrize("mode", ["0", "1"])
-def test_both_kernel_families_agree_with_oracle(engine, mode, monkeypatch):
-    """TSKV_COOP=0 forces the lane-per-page kernels, =1 the warp-cooperative ones, for the eligible pages
-    (zig-zag simple8b values, RLE / simple8b timestamps, <= 1024 rows). Default is chosen per scan."""
-    monkeypatch.setenv("TSKV_COOP", mode)
+@pytest.mark.parametrize("gbs", [False, True])
+def test_short_jittered_pages_with_nulls_agree_with_oracle(engine, gbs):
+    """Jittered, null-bearing pages of the short-page bins (zig-zag simple8b values, RLE / simple8b timestamps,
+    <= 1024 rows), with and without GROUP BY series."""
     g = datagen.generate(3000, n_fields=2, n_points=777, value_kind=datagen.I64_WALK, seed=77, jitter_permille=400,
                          jitter_max=999_999, null_page_permille=300, null_row_permille=150)
     pages = engine.upload_pages(g.arena, g.descs)
     w = 60_000_000_000
     fbs, nb = bucket_spec(datagen.TSBS_T0 - 1_000_000, datagen.TSBS_T0 + 776 * datagen.TSBS_STEP + 1_000_000, w)
     sel = np.arange(0, 3000, 3, dtype=np.uint32)
-    for gbs in (False, True):
-        q = QueryOption([PushedAggregate(c, cabi.TSKV_PT_I64, ALL_AGGS) for c in (1, 2)], series_ids=sel,
-                        time_ranges=[(datagen.TSBS_T0 + 7 * datagen.TSBS_STEP, datagen.TSBS_T0 + 700 * datagen.TSBS_STEP)],
-                        width=w, first_bucket_start=fbs, n_buckets=nb, group_by_series=gbs)
-        assert_results_equal(engine.scan_aggregate(pages, q), orc.scan_aggregate(g.arena, g.descs, q, n_threads=4),
-                             what="coop=%s gbs=%s" % (mode, gbs))
+    q = QueryOption([PushedAggregate(c, cabi.TSKV_PT_I64, ALL_AGGS) for c in (1, 2)], series_ids=sel,
+                    time_ranges=[(datagen.TSBS_T0 + 7 * datagen.TSBS_STEP, datagen.TSBS_T0 + 700 * datagen.TSBS_STEP)],
+                    width=w, first_bucket_start=fbs, n_buckets=nb, group_by_series=gbs)
+    assert_results_equal(engine.scan_aggregate(pages, q), orc.scan_aggregate(g.arena, g.descs, q, n_threads=4),
+                         what="gbs=%s" % gbs)
     pages.close()
 
 
@@ -747,13 +745,10 @@ def test_tombstones_golden_generic_time_pages_and_api_rules(engine):
     pages.close()
 
 
-@pytest.mark.parametrize("group", ["1", "4", "32"])
-def test_gorilla_two_phase_cooperative_scan(engine, group, monkeypatch):
-    """Gorilla pages through the warp-cooperative kernels (phase 1: lane-per-page control-bit parse of a group of
-    pages, phase 2: warp-per-page extraction + XOR scan), for several group sizes, against the oracle and against the
-    lane-per-page kernels."""
-    monkeypatch.setenv("TSKV_GOR_GROUP", group)
-    g = datagen.generate(1500, n_fields=2, n_points=1000, value_kind=datagen.MIXED, seed=int(group) + 5, jitter_permille=300,
+@pytest.mark.parametrize("seed", [6, 9, 37])
+def test_gorilla_mixed_pages_agree_with_oracle(engine, seed):
+    """Gorilla pages of mixed values (jittered, with nulls, <= 1024 rows: the short-page bins) against the oracle."""
+    g = datagen.generate(1500, n_fields=2, n_points=1000, value_kind=datagen.MIXED, seed=seed, jitter_permille=300,
                          jitter_max=999_999, null_page_permille=300, null_row_permille=120)
     pages = engine.upload_pages(g.arena, g.descs)
     w = 60_000_000_000
@@ -764,24 +759,25 @@ def test_gorilla_two_phase_cooperative_scan(engine, group, monkeypatch):
     for gbs in (False, True):
         q = QueryOption(cols, series_ids=sel, time_ranges=[(datagen.TSBS_T0 + 7 * datagen.TSBS_STEP, datagen.TSBS_T0 + 900 * datagen.TSBS_STEP)],
                         width=w, first_bucket_start=fbs, n_buckets=nb, group_by_series=gbs)
-        exp = orc.scan_aggregate(g.arena, g.descs, q, n_threads=4)
-        for mode in ("1", "0"):
-            monkeypatch.setenv("TSKV_COOP", mode)
-            assert_results_equal(engine.scan_aggregate(pages, q), exp, what="gorilla coop=%s group=%s gbs=%s" % (mode, group, gbs))
+        assert_results_equal(engine.scan_aggregate(pages, q), orc.scan_aggregate(g.arena, g.descs, q, n_threads=4),
+                             what="gorilla seed=%d gbs=%s" % (seed, gbs))
     pages.close()
 
 
 @pytest.mark.parametrize("case,status", [("extra_values", 0), ("early_sentinel", cabi.TSKV_ERR_BITSET_MISMATCH),
                                          ("truncated", cabi.TSKV_ERR_SHORT_BLOCK), ("sentinel_valued_data", 0),
                                          ("first_value_only", cabi.TSKV_ERR_SHORT_BLOCK)])
-@pytest.mark.parametrize("mode", ["0", "1"])
-def test_gorilla_stream_end_cases_in_both_kernel_families(engine, case, status, mode, monkeypatch):
+@pytest.mark.parametrize("jitter", [False, True])
+def test_gorilla_stream_end_cases(engine, case, status, jitter):
     """The end of a gorilla stream (float.rs:480-591): more values than valid rows are decoded and ignored, a
-    sentinel before the bitset is served is a mismatch, a stream without sentinel is an unexpected end of block."""
-    monkeypatch.setenv("TSKV_COOP", mode)
+    sentinel before the bitset is served is a mismatch, a stream without sentinel is an unexpected end of block.
+    Regular timestamps make a run-length time page, jittered ones a simple8b time page: the two time classes of the
+    short Gorilla bins."""
     n = 200
     vals = np.cumsum(np.arange(n) % 5).astype(np.float64) * 0.37 + 1.5
     ts = datagen.TSBS_T0 + np.arange(n, dtype=np.int64) * datagen.TSBS_STEP
+    if jitter:
+        ts += np.random.default_rng(11).integers(0, datagen.TSBS_STEP // 2, n)
     b = datagen.ArenaBuilder()
     b.add_page(datagen.build_page(datagen.encode_timestamps(ts), n), 5, 0, cabi.TSKV_PT_TIME, n)
     if case == "extra_values":    # 230 encoded values for 200 rows
@@ -805,6 +801,7 @@ def test_gorilla_stream_end_cases_in_both_kernel_families(engine, case, status, 
     b.add_page(datagen.build_page(data, n), 5, 1, cabi.TSKV_PT_F64, n)
     b.add_column_group(6, ts, [(1, cabi.TSKV_PT_F64, np.arange(n) * 0.5, None)])
     arena, descs = b.finish()
+    assert time_page_is_rle(arena, descs[0]) != jitter
     aggs = ("count", "first", "last") if case == "sentinel_valued_data" else ALL_AGGS  # (no NaN into sum/min/max)
     q = QueryOption([PushedAggregate(1, cabi.TSKV_PT_F64, aggs)], group_by_series=True,
                     time_ranges=[(int(ts[0]), int(ts[6]))] if case == "sentinel_valued_data" else [])

@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 
 REGISTER_LIMITED_CTAS = 4  # SCAN_MIN_BLOCKS in scan_kernels.cuh
 C4_BINS = {9, 10, 11, 12}  # RLE ts + simple8b, simple8b ts + simple8b, RLE ts + Gorilla, simple8b ts + Gorilla values
-LINE = re.compile(r"\[tskv\] bin (\d+)( \(coop\))? grid (\d+), (\d+) CTAs/SM")
+LINE = re.compile(r"\[tskv\] bin (\d+) grid (\d+), (\d+) CTAs/SM")
 
 
 @pytest.mark.parametrize("tombstones", [False, True])
@@ -29,7 +29,7 @@ def test_c4_bins_reach_register_limited_occupancy(engine, tombstones, capfd, mon
     capfd.readouterr()
     res = engine.scan_aggregate(pages, bench.make_query(select_tag_subset(n_series, 10)))
     err = capfd.readouterr().err
-    occ = {int(m.group(1)): int(m.group(4)) for m in LINE.finditer(err) if not m.group(2)}
+    occ = {int(m.group(1)): int(m.group(3)) for m in LINE.finditer(err)}
     assert set(occ) == C4_BINS, err
     for b, ctas in sorted(occ.items()):
         assert ctas >= REGISTER_LIMITED_CTAS, "bin %d: %d CTAs per SM\n%s" % (b, ctas, err)

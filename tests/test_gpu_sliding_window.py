@@ -18,7 +18,7 @@ from tests.test_sliding_reference import slt_cases, slt_queries
 
 pytestmark = pytest.mark.gpu
 
-ENVS = [("0", "1"), ("0", "3"), ("1", "1"), ("1", "3")]  # (TSKV_COOP, TSKV_PARTS)
+ENVS = ("1", "3")  # TSKV_PARTS
 FIELDS = ((1, cabi.TSKV_PT_I64), (2, cabi.TSKV_PT_F64), (3, cabi.TSKV_PT_U64))
 AGGS = ("count", "sum", "min", "max", "mean")
 
@@ -122,10 +122,9 @@ def test_sliding_geometry(engine, case, monkeypatch):
                     exp, err = None, e.status
                 if qname.startswith("short"):
                     assert err == cabi.TSKV_ERR_BUCKET_RANGE, what
-                for coop, parts in ENVS:
-                    monkeypatch.setenv("TSKV_COOP", coop)
+                for parts in ENVS:
                     monkeypatch.setenv("TSKV_PARTS", parts)
-                    wh = "%s coop=%s parts=%s" % (what, coop, parts)
+                    wh = "%s parts=%s" % (what, parts)
                     got, st = _scan(engine, pages, q, slide)
                     assert st == err, "%s: status %s, expected %s" % (wh, st, err)
                     if err is None:

@@ -1,5 +1,6 @@
-"""Host-side scan planning heuristics (cnosdb_b200/csrc/host_util.cc), exercised through the host library: which kernel
-family a scan gets and how gorilla pages are grouped, for the shard sizes of the C4 strong-scaling run. No GPU needed."""
+"""Host-side scan planning heuristics (cnosdb_b200/csrc/host_util.cc), exercised through the host library: the selected
+fraction of a shard, the grids of the lane-per-page kernels, the overlap groups of the merge pass and the page parts.
+No GPU needed."""
 import ctypes as C
 
 import numpy as np
@@ -12,10 +13,6 @@ def lib():
     L = cabi.load_hostgen_library()
     L.tskvplan_selected_fraction.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
     L.tskvplan_selected_fraction.restype = C.c_double
-    L.tskvplan_use_cooperative.argtypes = [C.c_double, C.c_int, C.c_int, C.c_int]
-    L.tskvplan_use_cooperative.restype = C.c_int
-    L.tskvplan_gorilla_group.argtypes = [C.c_double, C.c_double]
-    L.tskvplan_gorilla_group.restype = C.c_uint32
     return L
 
 
@@ -66,19 +63,6 @@ def test_serial_grid_planner_minimises_the_quantised_makespan():
     # a machine too small even for the largest round count considered still gets a valid (over-subscribed) plan
     g1 = plan([1000], [1.0], [1], sm=2, wpb=4)
     assert g1[0] >= 1
-
-
-def test_kernel_family_and_group_size_for_the_c4_shards():
-    """The round-1 crossover between the kernel families (the cooperative kernels are opt-in since round 2, TSKV_COOP=1;
-    the rule still sizes their gorilla page groups)."""
-    L = lib()
-    selected_pages = {1: 100_000, 2: 50_000, 4: 25_000, 8: 12_500}  # 10 % of 1 M series, one field page each
-    family = {w: bool(L.tskvplan_use_cooperative(float(p), 132, 4, 128)) for w, p in selected_pages.items()}
-    assert family == {1: False, 2: False, 4: False, 8: True}
-    resident_warps = 132 * 4 * 4
-    assert L.tskvplan_gorilla_group(6250.0, float(resident_warps)) == 4
-    assert L.tskvplan_gorilla_group(100.0, float(resident_warps)) == 1
-    assert L.tskvplan_gorilla_group(1e9, float(resident_warps)) == 32
 
 
 def test_overlap_groups_follow_the_reference_grouping():

@@ -5,9 +5,9 @@ TAG=${1:-q}
 mkdir -p profile_out
 python -m pytest tests -m gpu -x -q 2>&1 | tail -3
 TSKV_DEBUG_BINS=1 python tools/profile_scan.py --series 1000000 --steps 4 2>&1 | tail -5
-TSKV_DEBUG_BINS=1 TSKV_COOP=0 python tools/profile_scan.py --series 125000 --steps 4 2>&1 | tail -5
+TSKV_DEBUG_BINS=1 python tools/profile_scan.py --series 125000 --steps 4 2>&1 | tail -5
 M="smsp__inst_executed.sum,gpu__time_duration.sum,smsp__issue_active.avg.pct_of_peak_sustained_active,launch__registers_per_thread,launch__grid_size,sm__warps_active.avg.pct_of_peak_sustained_active,dram__bytes_read.sum"
-ncu --metrics $M --clock-control none -k "regex:k_scan_(aggregate|coop)" -s 8 -c 4 --csv --log-file profile_out/${TAG}_inst.csv \
+ncu --metrics $M --clock-control none -k "regex:k_scan_aggregate" -s 8 -c 4 --csv --log-file profile_out/${TAG}_inst.csv \
   python tools/profile_scan.py --series 1000000 --steps 3 > /dev/null 2>&1
 python - <<PY
 import csv

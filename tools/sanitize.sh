@@ -1,7 +1,7 @@
 #!/bin/bash
 # Run on a GPU machine: compute-sanitizer over the parity tests that exercise the newest device code
-# (round 2: pages cut at restart points, the overlap-merge pass, boolean pages; round 1: cooperative gorilla decode,
-# tombstones, device CRC, error paths). memcheck slows kernels 10-50x, the selected tests use small arenas.
+# (pages cut at restart points, the overlap-merge pass, boolean pages, gorilla decode, tombstones, device CRC, error
+# paths). memcheck slows kernels 10-50x, the selected tests use small arenas.
 # Usage: bash tools/sanitize.sh [memcheck|racecheck|initcheck] [-k expression]
 TOOL=${1:-memcheck}
 SEL=${2:-"gorilla or tombstone or small or errors or crc or empty or maximum or predicates or pruning or concurrent or host_resident or decode or parts or malformed or merge or overlapping or bool"}
