@@ -8,10 +8,12 @@ import numpy as np
 from tests.helpers import ExactResult, exact_aggregate
 
 
-def exact_aggregate_grouped(truth, query, group_ids, n_groups):
+def exact_aggregate_grouped(truth, query, group_ids, n_groups, tombstones=None, files=None):
     """ExactResult of `query` (GROUP BY bucket, not by series) with group_ids[slot] in [0, n_groups) the group of the
     slot-th selected series (series_ids order, or every series of `truth` in ascending id order). Cell c = group *
-    n_buckets + bucket; a group without members reads like an empty bucket."""
+    n_buckets + bucket; a group without members reads like an empty bucket. FIRST / LAST keep the keys of the whole
+    selection (ties to the lower slot, which the members keep in their order); tombstones / files: as in
+    exact_aggregate."""
     assert not query.group_by_series
     slots = np.asarray(query.series_ids if query.series_ids is not None else sorted(truth), dtype=np.uint32)
     gid = np.asarray(group_ids)
@@ -22,7 +24,7 @@ def exact_aggregate_grouped(truth, query, group_ids, n_groups):
         sub = copy.copy(query)
         sub.series_ids = slots[gid == g]
         sub._keep = None
-        e = exact_aggregate(truth, sub)
+        e = exact_aggregate(truth, sub, tombstones=tombstones, files=files, key_slots=slots.size)
         cells = slice(g * nb, (g + 1) * nb)
         res.values[:, cells] = e.values
         res.validity[:, cells] = e.validity

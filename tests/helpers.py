@@ -80,8 +80,11 @@ def make_query(fields, aggs=ALL_AGGS, **kw):
 # ---- exact reference ---------------------------------------------------------------------------------------------------
 # Aggregates computed from the generated arrays themselves (no page is decoded), so they share nothing with the oracle or
 # the kernels. Integer sums are exact Python ints; f64 sums are a class that holds for any summation order starting from
-# +0.0 (NaN, an infinity, or finite with an error bound: f64_sum_class). FIRST / LAST are not restated here: compare those
-# with the oracle.
+# +0.0 (NaN, an infinity, or finite with an error bound: f64_sum_class). FIRST / LAST follow DESIGN section 7: a run is
+# the selected rows of one (slot, column group, bucket) - of one (slot, overlap group, bucket) for merged chunks - and
+# only its min-time (max-time) row may contribute, and only with a value; the cell takes the smallest (t, slot) for
+# FIRST, the largest t and on a tie the smallest slot for LAST. Tombstones and the overlap merge of chunk files are
+# restated here as well (exact_aggregate's `tombstones=` / `files=`).
 
 I64_MIN, I64_MAX = -2**63, 2**63 - 1
 _U = 2.0 ** -53  # unit roundoff of f64
@@ -240,50 +243,211 @@ class ExactResult:
         self.exact_sums = {}  # column id -> {cell: (S, n)} of integer columns
 
 
-def exact_aggregate(truth, query):
-    """COUNT / SUM / MIN / MAX / MEAN of `query` over `truth` ({series id: [(timestamps, {column id: (values,
-    validity)}), ...]}, one entry per column group). Raises ReferenceError(TSKV_ERR_BUCKET_RANGE) when a selected row
-    (time ranges, AND-ed predicates) has no bucket. A column group that holds none of the query columns is never read."""
+def _in_ranges(ts, ranges):
+    """Rows of `ts` inside one of the closed ranges (an empty range, a > b, holds none)."""
+    m = np.zeros(ts.size, dtype=bool)
+    for a, b in ranges:
+        m |= (ts >= a) & (ts <= b)
+    return m
+
+
+def tombstone_lists(tombstones):
+    """TOMBSTONE_DTYPE array -> (ranges that drop rows of every series, {series: ranges that drop its rows},
+    {(series, column): ranges in which the column reads as NULL}). Empty ranges (min > max) are left out."""
+    glob, rows, cols = [], {}, {}
+    for tb in (tombstones if tombstones is not None else []):
+        s, c, a, b = int(tb["series_id"]), int(tb["column_id"]), int(tb["min_ts"]), int(tb["max_ts"])
+        if a > b:
+            continue
+        if s == cabi.TSKV_TOMB_ALL:
+            glob.append((a, b))
+        elif c == cabi.TSKV_TOMB_ALL:
+            rows.setdefault(s, []).append((a, b))
+        else:
+            cols.setdefault((s, c), []).append((a, b))
+    return glob, rows, cols
+
+
+def _predicates_hold(query, ts, cols):
+    """The AND-ed predicates of every row (NULL or an absent column: the comparison is not TRUE)."""
+    sel = np.ones(ts.size, dtype=bool)
+    for pc, ppt, op, c in query.predicates:
+        if pc not in cols:
+            sel[:] = False
+        else:
+            pv, pvalid = cols[pc]
+            sel &= np.asarray(pvalid, dtype=bool) & _cmp(ppt, op, pv, c)
+    return sel
+
+
+def overlap_groups(cgs, files):
+    """The overlap groups of one series' column groups `cgs` ([(ts, cols)]) with file ids `files` (None: one group per
+    column group). A chunk is the column groups of one file, bounded by their min / max time; chunks sorted by (lo, hi,
+    file) chain while lo <= the running max hi. -> [[stream, ...]]: a stream per chunk, ordered by file id, each the
+    chunk's column group indices by min time."""
+    if files is None:
+        return [[[k]] for k in range(len(cgs))]
+    chunks = {}
+    for k, (ts, _) in enumerate(cgs):
+        chunks.setdefault(int(files[k]), []).append(k)
+    bounds = []
+    for f, ks in chunks.items():
+        lo = min(int(np.min(cgs[k][0])) for k in ks)
+        hi = max(int(np.max(cgs[k][0])) for k in ks)
+        bounds.append((lo, hi, f))
+    bounds.sort()
+    groups, cur, run_max = [], [], None
+    for lo, hi, f in bounds:
+        if cur and not lo <= run_max:
+            groups.append(cur)
+            cur = []
+        cur.append(f)
+        run_max = hi if run_max is None else max(run_max, hi)
+    groups.append(cur)
+    return [[sorted(chunks[f], key=lambda k: int(np.min(cgs[k][0]))) for f in sorted(g)] for g in groups]
+
+
+def _merged_rows(cgs, streams, query, qcols, row_drop):
+    """The merged rows of one overlap group of two or more chunks: rows of the column groups this scan reads that pass
+    the predicates (on their own column group) and no row tombstone; equal times collapse, every query column takes the
+    last non-null value in (stream, row) order. -> (times, {column: (values, validity)})."""
+    t_all, order_vals = [], {c: ([], []) for c in qcols}
+    for stream in streams:
+        for k in stream:
+            ts, cols = cgs[k]
+            if not any(c in cols for c in qcols):
+                continue  # a column group without a query column is not read
+            ts = np.asarray(ts, dtype=np.int64)
+            keep = _predicates_hold(query, ts, cols) & ~_in_ranges(ts, row_drop)
+            t_all.append(ts[keep])
+            for c in qcols:
+                v, valid = cols[c] if c in cols else (np.zeros(ts.size, dtype=np.uint64), np.zeros(ts.size, dtype=bool))
+                order_vals[c][0].append(_typed(query_phys(query, c), v)[keep].view(np.uint64))
+                order_vals[c][1].append(np.asarray(valid, dtype=bool)[keep])
+    t = np.concatenate(t_all) if t_all else np.zeros(0, dtype=np.int64)
+    order = np.argsort(t, kind="stable")  # equal times keep their (stream, row) order
+    t = t[order]
+    starts = np.flatnonzero(np.concatenate([[True], t[1:] != t[:-1]])) if t.size else np.zeros(0, dtype=np.int64)
+    out = {}
+    for c in qcols:
+        v = np.concatenate(order_vals[c][0])[order] if t.size else np.zeros(0, dtype=np.uint64)
+        valid = np.concatenate(order_vals[c][1])[order] if t.size else np.zeros(0, dtype=bool)
+        if not t.size:
+            out[c] = (v, valid)
+            continue
+        last = np.maximum.reduceat(np.where(valid, np.arange(t.size), -1), starts)
+        out[c] = (np.where(last >= 0, v[np.maximum(last, 0)], 0).astype(np.uint64), last >= 0)
+    return t[starts] if t.size else t, out
+
+
+def query_phys(query, column_id):
+    return next(c.phys_type for c in query.columns if c.column_id == column_id)
+
+
+def first_last_rel_bits(truth, query):
+    """bits of the time part of the FIRST / LAST tie-break keys: 2 * width when bucketed, else the span of the selected
+    times - the query's ranges, tightened on a single-rank scan by the page set's own min / max time."""
+    if query.width > 0:
+        return bits_for(2 * query.width) if query.width < 2**61 else 64
+    lo, hi = I64_MIN, I64_MAX
+    if not query.multi_rank:
+        lo = min(int(np.min(ts)) for cgs in truth.values() for ts, _ in cgs if len(ts))
+        hi = max(int(np.max(ts)) for cgs in truth.values() for ts, _ in cgs if len(ts))
+    if query.time_ranges:
+        lo = max(lo, min(a for a, _ in query.time_ranges))
+        hi = min(hi, max(b for _, b in query.time_ranges))
+    return 0 if hi < lo else bits_for(hi - lo)
+
+
+def exact_aggregate(truth, query, tombstones=None, files=None, key_slots=None):
+    """COUNT / SUM / MIN / MAX / MEAN / FIRST / LAST of `query` over `truth` ({series id: [(timestamps, {column id:
+    (values, validity)}), ...]}, one entry per column group). A column group that holds none of the query columns is
+    never read.
+      tombstones  TOMBSTONE_DTYPE array: a row whose time lies in a global or a (series, ALL) range is dropped; a value
+                  whose time lies in a (series, column) range reads as NULL.
+      files       the file id of every column group, in truth's order (series by series): the chunks of a series that
+                  overlap are merged (overlap_groups, _merged_rows), and their merged rows of a bucket form one FIRST /
+                  LAST run.
+      key_slots   the slot count the tie-break keys are built for (default: the selection's; GROUP BY tags: the whole
+                  selection's).
+    Raises ReferenceError(TSKV_ERR_UNSUPPORTED) when FIRST / LAST across slots do not fit the 62-bit key, and
+    ReferenceError(TSKV_ERR_BUCKET_RANGE) when a selected row (time ranges, predicates, tombstones) has no bucket."""
     slots = [int(s) for s in query.series_ids] if query.series_ids is not None else sorted(truth)
     n_groups = len(slots) if query.group_by_series else 1
     nb = query.n_buckets
     n_cells = n_groups * nb
     qcols = [c.column_id for c in query.columns]
+    want_sel = any(c.agg_mask & (cabi.TSKV_AGG_FIRST | cabi.TSKV_AGG_LAST) for c in query.columns)
+    n_key = key_slots if key_slots is not None else (len(query.series_ids) if query.series_ids is not None else len(truth))
+    slot_bits = 0 if (query.group_by_series or n_key <= 1) else bits_for(n_key - 1)
+    if want_sel and slot_bits and first_last_rel_bits(truth, query) + slot_bits > 62:
+        raise ReferenceError(cabi.TSKV_ERR_UNSUPPORTED)
+    glob, row_tomb, col_tomb = tombstone_lists(tombstones)
+    file_of, k = {}, 0
+    if files is not None:
+        for sid, cgs in truth.items():
+            file_of[sid] = list(files[k:k + len(cgs)])
+            k += len(cgs)
+        assert k == len(files)
+    units = []  # (slot, times, selected rows, {column: (u64 values, validity)}): one FIRST / LAST run per bucket
+    for slot, sid in enumerate(slots):
+        cgs = truth.get(sid, [])
+        row_drop = glob + row_tomb.get(sid, [])
+        for streams in overlap_groups(cgs, file_of.get(sid) if files is not None else None):
+            if len(streams) >= 2:
+                ts, cols = _merged_rows(cgs, streams, query, qcols, row_drop)
+                units.append((slot, ts, np.ones(ts.size, dtype=bool), cols))
+                continue
+            for k in streams[0]:
+                ts, cols = cgs[k]
+                if not any(c in cols for c in qcols):
+                    continue
+                ts = np.asarray(ts, dtype=np.int64)
+                sel = _predicates_hold(query, ts, cols) & ~_in_ranges(ts, row_drop)
+                units.append((slot, ts, sel, {c: (_typed(query_phys(query, c), cols[c][0]).view(np.uint64),
+                                                  np.asarray(cols[c][1], dtype=bool)) for c in qcols if c in cols}))
     cells = {c: [] for c in qcols}
     vals = {c: [] for c in qcols}
-    for slot, sid in enumerate(slots):
-        for ts, cols in truth.get(sid, []):
-            if not any(c in cols for c in qcols):
-                continue
-            ts = np.asarray(ts, dtype=np.int64)
-            sel = np.ones(ts.size, dtype=bool)
-            for pc, ppt, op, c in query.predicates:  # NULL or an absent column: the comparison is not TRUE
-                if pc not in cols:
-                    sel[:] = False
-                else:
-                    pv, pvalid = cols[pc]
-                    sel &= np.asarray(pvalid, dtype=bool) & _cmp(ppt, op, pv, c)
-            if query.time_ranges:
-                inr = np.zeros(ts.size, dtype=bool)
-                for a, b in query.time_ranges:
-                    inr |= (ts >= a) & (ts <= b)
-                sel &= inr
-            idx, ok = bucket_index(ts, query)
-            if (sel & ~ok).any():
-                raise ReferenceError(cabi.TSKV_ERR_BUCKET_RANGE)
-            cell = (slot if query.group_by_series else 0) * nb + idx
-            for c in qcols:
-                if c in cols:
-                    v, valid = cols[c]
-                    m = sel & np.asarray(valid, dtype=bool)
-                    cells[c].append(cell[m])
-                    vals[c].append(np.asarray(v)[m])
+    firsts = {c: [] for c in qcols}  # (cell, t, slot, value) of every run whose min-time row holds a value
+    lasts = {c: [] for c in qcols}
+    for slot, ts, sel, cols in units:
+        if query.time_ranges:
+            sel = sel & _in_ranges(ts, query.time_ranges)
+        idx, ok = bucket_index(ts, query)
+        if (sel & ~ok).any():
+            raise ReferenceError(cabi.TSKV_ERR_BUCKET_RANGE)
+        cell = (slot if query.group_by_series else 0) * nb + idx
+        rows = np.flatnonzero(sel)
+        _, fi = np.unique(idx[rows], return_index=True)  # times ascend: a bucket's first / last selected row
+        _, li = np.unique(idx[rows][::-1], return_index=True)
+        fr, lr = rows[fi], rows[rows.size - 1 - li]
+        for c, (v, valid) in cols.items():
+            valid = valid & ~_in_ranges(ts, col_tomb.get((slots[slot], c), []))
+            m = sel & valid
+            cells[c].append(cell[m])
+            vals[c].append(v[m])
+            for r, out in ((fr, firsts[c]), (lr, lasts[c])):
+                r = r[valid[r]]
+                out.append((cell[r], ts[r], np.full(r.size, slot, dtype=np.int64), v[r]))
+    sel_out = {}
+    for c in qcols:
+        for name, cands in (("first", firsts[c]), ("last", lasts[c])):
+            cl, t, s, v = (np.concatenate(x) for x in zip(*cands)) if cands else (np.zeros(0, dtype=np.int64),) * 4
+            order = np.lexsort((s, t if name == "first" else ~t, cl))
+            cl, t, v = cl[order], t[order], np.asarray(v, dtype=np.uint64)[order] if v.size else v.astype(np.uint64)
+            head = np.flatnonzero(np.concatenate([[True], cl[1:] != cl[:-1]])) if cl.size else cl
+            value, have = np.zeros(n_cells, dtype=np.uint64), np.zeros(n_cells, dtype=bool)
+            value[cl[head]], have[cl[head]] = v[head], True
+            if not slot_bits:  # keys are the raw times: a FIRST at INT64_MAX / LAST at INT64_MIN is the empty key
+                edge = cl[head][t[head] == (I64_MAX if name == "first" else I64_MIN)]
+                value[edge], have[edge] = 0, False
+            sel_out[(c, name)] = (value, have)
     res = ExactResult(query, n_groups)
     j = 0
     for qc in query.columns:
         c, pt = qc.column_id, qc.phys_type
         cl = np.concatenate(cells[c]) if cells[c] else np.zeros(0, dtype=np.int64)
-        v = _typed(pt, np.concatenate(vals[c]) if vals[c] else [])
+        v = (np.concatenate(vals[c]) if vals[c] else np.zeros(0, dtype=np.uint64)).view(_typed(pt, []).dtype)
         count = np.bincount(cl, minlength=n_cells).astype(np.uint64)
         have = count > 0
         out = {"count": (count, np.ones(n_cells, dtype=bool))}
@@ -331,6 +495,7 @@ def exact_aggregate(truth, query):
             res_f64 = {}
         out["sum"] = (sums, have)
         out["mean"] = (means, have)
+        out["first"], out["last"] = sel_out[(c, "first")], sel_out[(c, "last")]
         for a in qc.agg_list():
             name = cabi.AGG_NAMES[a]
             if name in out:
@@ -341,14 +506,15 @@ def exact_aggregate(truth, query):
     return res
 
 
-def assert_matches_exact(got, exp, what="", int_mean=True):
-    """got: ScanResult; exp: ExactResult. COUNT / integer SUM / MIN / MAX bit-exact, integer MEAN bit-exact
-    (= float(S) / float(n)) unless int_mean=False. f64 SUM / MEAN by class (f64_sum_class): a NaN cell must hold some
-    NaN (the payload depends on the order), an inf cell that inf, a finite cell a value within the bound, and a zero
-    +0.0. FIRST / LAST are not checked."""
+def assert_matches_exact(got, exp, what="", int_mean=True, first_last=True):
+    """got: ScanResult; exp: ExactResult. COUNT / integer SUM / MIN / MAX / FIRST / LAST bit-exact (FIRST / LAST
+    unless first_last=False), integer MEAN bit-exact (= float(S) / float(n)) unless int_mean=False. f64 SUM / MEAN by
+    class (f64_sum_class): a NaN cell must hold some NaN (the payload depends on the order), an inf cell that inf, a
+    finite cell a value within the bound, and a zero +0.0."""
     assert got.names == exp.names
     for j, (col, agg) in enumerate(got.names):
-        if agg in ("first", "last") or (agg == "mean" and not int_mean and exp.phys[col] != cabi.TSKV_PT_F64):
+        if (agg in ("first", "last") and not first_last) or \
+                (agg == "mean" and not int_mean and exp.phys[col] != cabi.TSKV_PT_F64):
             continue
         gv, ev = got.validity[j], exp.validity[j]
         bad = np.nonzero(gv != ev)[0]
@@ -601,16 +767,17 @@ def sel_unsupported(query, truth):
     slot_bits = 0 if (query.group_by_series or n_slots <= 1) else bits_for(n_slots - 1)
     if slot_bits == 0:
         return False
-    if query.width > 0:
-        rel = bits_for(2 * query.width) if query.width < 2**61 else 64
-    else:
-        lo = min(int(ts.min()) for cgs in truth.values() for ts, _ in cgs)
-        hi = max(int(ts.max()) for cgs in truth.values() for ts, _ in cgs)
-        if query.time_ranges:
-            lo = max(lo, min(a for a, _ in query.time_ranges))
-            hi = min(hi, max(b for _, b in query.time_ranges))
-        rel = 0 if hi < lo else bits_for(hi - lo)
-    return rel + slot_bits > 62
+    return first_last_rel_bits(truth, query) + slot_bits > 62
+
+
+def raw_key_edge(query, truth):
+    """The scan's FIRST / LAST keys are raw row times (group_by_series, or one selected series) and a row lies at
+    INT64_MIN or INT64_MAX: there the exact reference keeps the engine's known deviation (DESIGN section 7), which the
+    oracle does not have."""
+    n_slots = len(query.series_ids) if query.series_ids is not None else len(truth)
+    if not (query.group_by_series or n_slots <= 1):
+        return False
+    return any(((np.asarray(ts) == I64_MIN) | (np.asarray(ts) == I64_MAX)).any() for cgs in truth.values() for ts, _ in cgs)
 
 
 def geometry_queries(case, ranges, truth):

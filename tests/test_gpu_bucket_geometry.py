@@ -2,8 +2,9 @@
 from 0 to 2^40 + 3, widths that are and are not multiples of the step, narrower than it, up to 2^63 - 1, origins that are
 negative or >= the width, rows on both sides of the truncating-% regime and at the i64 limits, and time ranges on, beside
 and between rows and bucket edges. Every query runs with pages whole and cut into 3 parts, and every single-range query
-runs again with its range split in two (two ranges turn the row-space fast path off): COUNT / SUM / MIN / MAX must be bit-identical across the two and equal the exact reference; FIRST / LAST are
-compared with the oracle."""
+runs again with its range split in two (two ranges turn the row-space fast path off): COUNT / SUM / MIN / MAX must be
+bit-identical across the two and equal the exact reference. FIRST / LAST must equal the exact reference (which keeps the
+known deviation at the i64 limits) and the oracle wherever a page's timestamps are distinct."""
 import numpy as np
 import pytest
 
@@ -89,7 +90,7 @@ def test_bucket_geometry(engine, case, monkeypatch):
                         assert st == err, "%s: status %s, expected %s" % (wh, st, err)
                         continue
                     assert st is None, "%s: status %s" % (wh, st)
-                    assert_matches_exact(got, exp, what=wh)
+                    assert_matches_exact(got, exp, what=wh, first_last=bool(step))
                     if ora is not None:
                         _first_last_equal(got, ora, wh)
                     if first is None:

@@ -104,7 +104,7 @@ def test_f64_edges_through_the_overlap_merge(engine):
         sids = None if gbs else np.array([s for s in ids if s % 10 not in (8,)], dtype=np.uint32)
         q = make_query(F64_FIELDS, ALL_AGGS, width=w, first_bucket_start=fbs, n_buckets=nb, group_by_series=gbs,
                        series_ids=sids)
-        exp = exact_aggregate(truth, q)
+        exp = exact_aggregate(truth, q, files=files)
         ora = orc.scan_aggregate(arena, descs, q, chunk_files=files)
         _check(engine.scan_aggregate(pages, q), exp, ora, "overlap merge gbs=%s" % gbs)
     pages.close()

@@ -143,7 +143,7 @@ def test_overlap_merge_keeps_exact_sums(engine):
     pages = engine.upload_pages(arena, descs)
     pages.set_chunk_files(files)
     for name, q in queries(4 * 300):
-        exp = exact_aggregate(truth, q)
+        exp = exact_aggregate(truth, q, files=files)
         assert_matches_exact(engine.scan_aggregate(pages, q), exp, what="overlap merge " + name)
         if name == "bucket+sel":
             ora = orc.scan_aggregate(arena, descs, q, chunk_files=files)
