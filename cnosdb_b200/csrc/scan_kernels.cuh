@@ -217,13 +217,17 @@ __device__ __forceinline__ int find_qcol(const ColState *cols, uint32_t n_cols, 
   return -1;
 }
 
+// The reader counters of a scan pass, in unsigned long long words: pages read, their bytes, the bytes each bin's fused
+// kernel reads, and the field pages that statistics pruning dropped.
+constexpr uint32_t CTR_PAGES = 0, CTR_BYTES = 1, CTR_BIN_BYTES = 2, CTR_PRUNED = CTR_BIN_BYTES + N_BINS,
+                   N_COUNTERS = CTR_PRUNED + 1;
+
 // One thread per item (field page, in kind-sorted order): selected? -> flag (query column + 1, bit 7 =
 // "this item also brings its column group's time page"), per-block counts and the byte/page counters
 // of the reference's reader metrics (column_group/mod.rs:141-193), split per decode-kind bin.
-// counters: [0] pages, [1] bytes, [2 + bin] bytes read by bin's fused kernel.
 // Statistics pruning (filter_column_groups, tskv/src/reader/chunk.rs:12-50 with the column group's time_range(),
 // tsm/column_group.rs:9-17): a group whose [min_ts, max_ts] overlaps none of the query's time ranges is dropped here,
-// so its pages are neither gathered nor decoded. counters[2 + N_BINS] counts the pruned groups' field pages.
+// so its pages are neither gathered nor decoded.
 struct PruneRanges {
   tskv_time_range r[MAX_RANGES];
   uint32_t n;
@@ -262,7 +266,7 @@ __global__ void k_flag_items(const tskv_page_desc *descs, const uint4 *item_info
       const uint64_t end = cg + 1 < n_cg ? (uint64_t)cg_time_page[cg + 1] : n_descs;
       if (cg_ruled_out_by_stats(descs, tp0, end, preds, page_stats)) in_time = false;
     }
-    if (!in_time && qc >= 0 && cg_slot[cg] >= 0 && !(cg_merge && cg_merge[cg])) atomicAdd(&counters[2 + N_BINS], 1ull);
+    if (!in_time && qc >= 0 && cg_slot[cg] >= 0 && !(cg_merge && cg_merge[cg])) atomicAdd(&counters[CTR_PRUNED], 1ull);
     // (column groups of overlapping chunks go through the merge pass instead, merge_kernels.cuh)
     if (qc >= 0 && cg_slot[cg] >= 0 && in_time && !(cg_merge && cg_merge[cg])) {
       if (cols[qc].phys_type != d.phys_type) {
@@ -299,11 +303,11 @@ __global__ void k_flag_items(const tskv_page_desc *descs, const uint4 *item_info
   __syncthreads();
   if (threadIdx.x == 0) {
     block_count[blockIdx.x] = s_cnt;
-    if (s_pages) atomicAdd(&counters[0], s_pages);
+    if (s_pages) atomicAdd(&counters[CTR_PAGES], s_pages);
   }
   if (threadIdx.x < N_BINS && s_bytes[threadIdx.x]) {
-    atomicAdd(&counters[1], s_bytes[threadIdx.x]);
-    atomicAdd(&counters[2 + threadIdx.x], s_bytes[threadIdx.x]);
+    atomicAdd(&counters[CTR_BYTES], s_bytes[threadIdx.x]);
+    atomicAdd(&counters[CTR_BIN_BYTES + threadIdx.x], s_bytes[threadIdx.x]);
   }
 }
 
@@ -348,7 +352,7 @@ struct WorkListArgs {
   uint32_t *bucket_off;          // [N_BINS * n_cols * WL_SUB + 1] exclusive offsets (k_worklist_offsets)
   uint32_t *work_page, *work_slot;
   uint8_t *work_qcol;
-  unsigned long long *counters;  // [0] pages [1] bytes [2 + bin] bytes per bin [2 + N_BINS] pruned pages
+  unsigned long long *counters;  // [N_COUNTERS] CTR_*
   int32_t *status;
 };
 
@@ -391,7 +395,7 @@ __device__ __forceinline__ void worklist_walk(const WorkListArgs &A, uint32_t i,
       const int qc = find_qcol(A.cols, A.n_cols, d.column_id);
       if (qc < 0) continue;
       if (!in_time) {
-        if (count_stats) atomicAdd(&A.counters[2 + N_BINS], 1ull);
+        if (count_stats) atomicAdd(&A.counters[CTR_PRUNED], 1ull);
         continue;
       }
       if (A.cols[qc].phys_type != d.phys_type) {
@@ -429,10 +433,10 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_count(const WorkListArg
   __syncthreads();
   for (uint32_t k = threadIdx.x; k < n_buckets; k += WL_THREADS)
     if (s_hist[k]) atomicAdd(&A.bucket_count[k], s_hist[k]);
-  if (threadIdx.x == 0 && s_pages) atomicAdd(&A.counters[0], s_pages);
+  if (threadIdx.x == 0 && s_pages) atomicAdd(&A.counters[CTR_PAGES], s_pages);
   if (threadIdx.x < N_BINS && s_bytes[threadIdx.x]) {
-    atomicAdd(&A.counters[1], s_bytes[threadIdx.x]);
-    atomicAdd(&A.counters[2 + threadIdx.x], s_bytes[threadIdx.x]);
+    atomicAdd(&A.counters[CTR_BYTES], s_bytes[threadIdx.x]);
+    atomicAdd(&A.counters[CTR_BIN_BYTES + threadIdx.x], s_bytes[threadIdx.x]);
   }
 }
 
@@ -2041,8 +2045,19 @@ struct StateLayout {
   uint64_t total;
 };
 
-// Identities of the partial state; the same launch zeroes the scan's small per-pass scratch (task counters / status /
-// counters, bin starts, work-list buckets) so that a pass starts with ONE node instead of three memsets + a kernel.
+// The scan's per-pass scratch ("aux" block): word offsets (8-byte words) of its parts.
+constexpr uint32_t AUX_TASK_COUNTERS = 0;  // u32 ScanParams::task_counter[N_BINS]
+constexpr uint32_t AUX_STATUS = 8;         // i32 ScanParams::status
+constexpr uint32_t AUX_ERR_PAGE = 9;
+constexpr uint32_t AUX_STATS = 10;         // ScanParams::stats[2]
+constexpr uint32_t AUX_COUNTERS = 12;      // the reader counters (CTR_*)
+constexpr uint32_t AUX_CRC_STATUS = AUX_COUNTERS + N_COUNTERS;  // i32: a page of k_verify_crc failed
+constexpr uint32_t AUX_CRC_ERR_PAGE = AUX_CRC_STATUS + 1;
+constexpr uint32_t AUX_WORDS = 32;
+static_assert(N_BINS * 4 <= (AUX_STATUS - AUX_TASK_COUNTERS) * 8 && AUX_CRC_ERR_PAGE < AUX_WORDS, "scan aux block layout");
+
+// Identities of the partial state; the same launch zeroes the scan's small per-pass scratch (the aux block, bin starts,
+// work-list buckets) so that a pass starts with ONE node instead of three memsets + a kernel.
 __global__ void k_init_state(uint64_t *state, StateLayout L, unsigned long long *aux, uint32_t aux_words, uint32_t *zero32,
                              uint32_t n_zero32, uint32_t *zero32b, uint32_t n_zero32b) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -37,7 +37,6 @@ struct tskv_ctx {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   cudaStream_t bin_stream[N_BINS] = {nullptr};  // the per-bin fused kernels run concurrently
-  cudaStream_t crc_stream = nullptr;            // per-read CRC checks of HBM-resident pages, next to the fused kernels
   int sm_count = 132;
   int max_dyn_smem = 48 * 1024;
   ncclComm_t comm = nullptr;  // tskvgpu_comm_init
@@ -147,11 +146,11 @@ struct tskv_scan {
   MeanExport *d_means = nullptr;
   uint32_t n_means = 0;
   uint64_t *d_state = nullptr;
-  uint32_t *d_task_counter = nullptr;
+  uint32_t *d_task_counter = nullptr;  // the aux block (AUX_*); the pointers below point into it
   int32_t *d_status = nullptr;
   unsigned long long *d_err_page = nullptr;
   unsigned long long *d_stats = nullptr;     // [0] points [1] rows in range
-  unsigned long long *d_counters = nullptr;  // [0] pages [1] bytes
+  unsigned long long *d_counters = nullptr;  // CTR_*
   uint64_t *d_values = nullptr;
   uint8_t *d_validity = nullptr;
   int grid[N_BINS] = {0};
@@ -169,8 +168,7 @@ struct tskv_scan {
   // for a capture.
   cudaGraphExec_t graph_exec = nullptr;
   cudaEvent_t ev_cfork = nullptr, ev_cjoin[N_BINS] = {nullptr};  // dependency-only events of the captured pass
-  cudaEvent_t ev_crc = nullptr, ev_ccrc = nullptr;  // join of the concurrent CRC checks (plain / captured pass)
-  int32_t *d_crc_status = nullptr;                  // a CRC mismatch outranks whatever the decoders made of the bad page
+  int32_t *d_crc_status = nullptr;  // a CRC mismatch outranks whatever the decoders made of the bad page
   unsigned long long *d_crc_err_page = nullptr;
   uint32_t n_enqueued = 0;
   bool graph_failed = false;
@@ -342,21 +340,30 @@ const char *tag_groups_refusal(const tskv_pages *pages, const tskv_query *q, con
   return nullptr;
 }
 
-tskv_status compute_layout(const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, tskv_output_layout *out) {
-  if (!pages || !q || !out || q->n_buckets == 0 || q->n_columns == 0 || !q->columns) return TSKV_ERR_INVALID_ARG;
-  if (q->width <= 0 && q->n_buckets != 1) return TSKV_ERR_INVALID_ARG;
-  if (tag_groups_refusal(pages, q, tg)) return TSKV_ERR_INVALID_ARG;
+bool query_shape_ok(const tskv_query *q) {
+  return q->n_buckets != 0 && q->n_columns != 0 && q->columns && (q->width > 0 || q->n_buckets == 1);
+}
+
+// Output layout of a query that passed query_shape_ok and tag_groups_refusal.
+tskv_output_layout output_layout(const tskv_pages *pages, const tskv_query *q, const TagGroups &tg) {
+  tskv_output_layout out;
   uint64_t n_out = 0;
   for (uint32_t c = 0; c < q->n_columns; c++) n_out += popc8(q->columns[c].agg_mask);
   uint64_t n_groups = 1;
   if (q->group_by_series) n_groups = selected_slots(pages, q);
   if (tg.on) n_groups = tg.n;
-  out->n_out = n_out;
-  out->n_groups = n_groups;
-  out->n_cells = n_groups * q->n_buckets;
-  out->bitmap_stride = (out->n_cells + 63) / 64 * 8;
-  out->values_bytes = n_out * out->n_cells * 8;
-  out->validity_bytes = n_out * out->bitmap_stride;
+  out.n_out = n_out;
+  out.n_groups = n_groups;
+  out.n_cells = n_groups * q->n_buckets;
+  out.bitmap_stride = (out.n_cells + 63) / 64 * 8;
+  out.values_bytes = n_out * out.n_cells * 8;
+  out.validity_bytes = n_out * out.bitmap_stride;
+  return out;
+}
+
+tskv_status compute_layout(const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, tskv_output_layout *out) {
+  if (!pages || !q || !out || !query_shape_ok(q) || tag_groups_refusal(pages, q, tg)) return TSKV_ERR_INVALID_ARG;
+  *out = output_layout(pages, q, tg);
   return TSKV_OK;
 }
 
@@ -479,8 +486,6 @@ void free_scan(tskv_scan *s) {
     if (b) cudaFreeAsync(b, st);
   if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
   if (s->ev_cfork) cudaEventDestroy(s->ev_cfork);
-  if (s->ev_crc) cudaEventDestroy(s->ev_crc);
-  if (s->ev_ccrc) cudaEventDestroy(s->ev_ccrc);
   for (int b = 0; b < N_BINS; b++)
     if (s->ev_cjoin[b]) cudaEventDestroy(s->ev_cjoin[b]);
   if (s->ev0) cudaEventDestroy(s->ev0);
@@ -549,6 +554,510 @@ const NcclApi &nccl_api() {
     api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllGather && api.GetErrorString;
   });
   return api;
+}
+
+// Narrows [lo, hi] to the span of the query's time ranges (no ranges: every timestamp); lo > hi: nothing in range.
+void clip_to_query_ranges(const tskv_query *q, int64_t &lo, int64_t &hi) {
+  if (q->n_time_ranges == 0) return;
+  int64_t qlo = q->time_ranges[0].min_ts, qhi = q->time_ranges[0].max_ts;
+  for (uint32_t r = 1; r < q->n_time_ranges; r++) {
+    qlo = std::min(qlo, q->time_ranges[r].min_ts);
+    qhi = std::max(qhi, q->time_ranges[r].max_ts);
+  }
+  lo = std::max(lo, qlo);
+  hi = std::min(hi, qhi);
+}
+
+// Sliding windows of `q` (window q->width, slide < q->width) by panes: the refusals of tskvgpu_scan_prepare_sliding
+// (DESIGN.md section 7) and the pane grid. Called under ctx->mu.
+tskv_status check_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide, uint32_t *out_k) {
+  for (uint32_t c = 0; c < q->n_columns; c++)
+    if (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) {
+      ctx->set_error("sliding windows: FIRST / LAST drop a (page, window) run on a NULL at its first / last row, which "
+                     "pane partials cannot rebuild");
+      return TSKV_ERR_UNSUPPORTED;
+    }
+  if (slide > q->width) {
+    ctx->set_error("sliding windows: a slide wider than the window (rows between windows) is not pushed down");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  if (q->width >= (int64_t)1 << 61) {
+    ctx->set_error("sliding windows: window of 2^61 or more");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  const uint64_t k = ((uint64_t)q->width - 1) / (uint64_t)slide + 1;  // windows per row, ceil(window / slide)
+  if (k > 100) {
+    ctx->set_error("sliding windows: more than 100 windows per row (Too many overlapping windows)");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  if (q->n_buckets < k) {
+    ctx->set_error("sliding windows: n_buckets must be at least ceil(window / slide)");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  if ((unsigned __int128)q->n_buckets * (uint64_t)slide > (unsigned __int128)1 << 63) {
+    ctx->set_error("sliding windows: the window grid spans more than 2^63");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  // With window % slide != 0 the reference keeps a row's copies by the test window-0 start <= t < end, which passes for
+  // every row whose dividend t - start_time % window + slide is >= 0 and whose window end does not wrap, and fails for
+  // other rows unless the remainder is 0: refuse unless every row the query can select is of the first kind.
+  if (q->width % slide != 0 && pages->n_cg) {
+    ensure_time_bounds(ctx, pages);
+    int64_t lo = pages->ts_min, hi = pages->ts_max;
+    clip_to_query_ranges(q, lo, hi);
+    const __int128 om = q->origin % q->width;
+    if (lo <= hi && ((__int128)lo - om + slide < 0 || (__int128)hi - om + slide > (__int128)INT64_MAX ||
+                     (__int128)hi + q->width > (__int128)INT64_MAX)) {
+      ctx->set_error("sliding windows: window % slide != 0 and rows in the truncating-% or wrapping range of the window "
+                     "expression");
+      return TSKV_ERR_UNSUPPORTED;
+    }
+  }
+  *out_k = (uint32_t)k;
+  return TSKV_OK;
+}
+
+// The refusals of the tskvgpu_scan_prepare* calls: sets the error and returns its status, or returns TSKV_OK with the
+// windows per row (1 unless slide > 0). Called under ctx->mu.
+tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide, const TagGroups &tg,
+                           uint32_t *win_k) {
+  if (const char *why = tag_groups_refusal(pages, q, tg)) {
+    ctx->set_error(why);
+    return TSKV_ERR_INVALID_ARG;
+  }
+  if (!query_shape_ok(q)) {
+    ctx->set_error("invalid query (buckets / columns)");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  if (q->n_columns > 126 || q->n_time_ranges > MAX_RANGES || (q->n_time_ranges && !q->time_ranges)) {
+    ctx->set_error("invalid query: at most 126 columns and 8 time ranges");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  if (q->n_predicates > TSKV_MAX_PREDICATES || (q->n_predicates && !q->predicates)) {
+    ctx->set_error("invalid query: at most 8 field predicates");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  for (uint32_t k = 0; k < q->n_predicates; k++)
+    if (q->predicates[k].phys_type < TSKV_PT_I64 || q->predicates[k].phys_type > TSKV_PT_F64 || q->predicates[k].op > TSKV_CMP_GE) {
+      ctx->set_error("invalid field predicate (type or operator)");
+      return TSKV_ERR_INVALID_ARG;
+    }
+  for (uint32_t c = 0; c < q->n_columns; c++) {
+    const tskv_agg_column &qc = q->columns[c];
+    if (qc.phys_type < TSKV_PT_I64 || qc.phys_type > TSKV_PT_BOOL || (qc.agg_mask & ~TSKV_AGG_ALL) || qc.agg_mask == 0) {
+      ctx->set_error("invalid query column (type or aggregate mask)");
+      return TSKV_ERR_INVALID_ARG;
+    }
+    if (qc.phys_type == TSKV_PT_BOOL && (qc.agg_mask & (TSKV_AGG_SUM | TSKV_AGG_MEAN))) {
+      ctx->set_error("sum / mean of a boolean column");
+      return TSKV_ERR_INVALID_ARG;
+    }
+    for (uint32_t c2 = 0; c2 < c; c2++)
+      if (q->columns[c2].column_id == qc.column_id) {
+        ctx->set_error("duplicate query column id");
+        return TSKV_ERR_INVALID_ARG;
+      }
+  }
+  if (q->series_ids)
+    for (uint32_t i = 1; i < q->n_series; i++)
+      if (q->series_ids[i] <= q->series_ids[i - 1]) {
+        ctx->set_error("series_ids must be sorted ascending and unique");
+        return TSKV_ERR_INVALID_ARG;
+      }
+  if ((q->reserved & TSKV_QUERY_MULTI_RANK) && !q->series_ids) {
+    bool needs_slots = q->group_by_series != 0 || tg.on;
+    for (uint32_t c = 0; c < q->n_columns; c++) needs_slots |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
+    if (needs_slots) {
+      ctx->set_error("multi-rank scan: GROUP BY series / tags and first/last need the global series_ids list (slots are positions in it)");
+      return TSKV_ERR_INVALID_ARG;
+    }
+  }
+  *win_k = 1;
+  return slide ? check_sliding(ctx, pages, q, slide, win_k) : TSKV_OK;
+}
+
+// FIRST / LAST tie-break key (ScanParams::slot_bits / rel_base) of a scan with FIRST / LAST (has_sel). Refuses
+// (TSKV_ERR_UNSUPPORTED) a scan whose keys do not fit 62 bits.
+tskv_status plan_keys(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, bool has_sel, uint32_t *slot_bits,
+                      int64_t *rel_base) {
+  const uint64_t n_slots = selected_slots(pages, q);
+  *slot_bits = (q->group_by_series || n_slots <= 1) ? 0 : bits_for(n_slots - 1);
+  *rel_base = 0;
+  if (!has_sel || *slot_bits == 0) return TSKV_OK;
+  unsigned rel_bits = 64;
+  if (q->width > 0) {
+    if (q->width < (int64_t)1 << 61) rel_bits = bits_for(2 * (uint64_t)q->width);
+  } else {
+    // unbucketed: rel = t - (lower bound of every in-range timestamp). A single-rank scan tightens unbounded / loose
+    // query ranges with the arena's own time bounds; a scan whose partials are merged with other ranks'
+    // (TSKV_QUERY_MULTI_RANK) must build keys every rank agrees on, i.e. from the query alone.
+    int64_t lo = INT64_MIN, hi = INT64_MAX;
+    if (!(q->reserved & TSKV_QUERY_MULTI_RANK)) {
+      ensure_time_bounds(ctx, pages);
+      lo = pages->ts_min;
+      hi = pages->ts_max;
+    }
+    clip_to_query_ranges(q, lo, hi);
+    if (hi < lo) {
+      rel_bits = 0;  // nothing can be in range
+    } else {
+      rel_bits = bits_for((uint64_t)hi - (uint64_t)lo);
+      *rel_base = lo;
+    }
+  }
+  if (rel_bits + *slot_bits > 62) {
+    ctx->set_error("first/last across series: (bucket width or time span) x series count does not fit the 62-bit tie-break key");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  return TSKV_OK;
+}
+
+// The state of a scan and the tables the host builds from its layout.
+struct ScanLayout {
+  StateLayout sl{};       // the state export, exchange, partials and finalize see
+  StateLayout kern_sl{};  // the state the fused kernels write: sl, or for a sliding scan the panes' state
+  std::vector<ColState> cols;      // the fused kernels' column table (offsets into kern_sl's state)
+  std::vector<CombineOp> combine;  // a sliding scan: pane state -> window state
+  std::vector<MeanExport> means;
+  std::vector<OutCol> outs;
+  uint32_t use_smem = 0, smem_words = 0;  // the per-CTA shared-memory partial table (ScanParams)
+};
+
+// n_cells: cells of the query's grid (a sliding scan: windows); kern_cells: cells of the fused kernels' grid (panes).
+ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint64_t kern_cells) {
+  ScanLayout out;
+  const StatePlan win = plan_state(q, n_cells);
+  const StatePlan pane = sliding ? plan_state(q, kern_cells) : StatePlan{};
+  out.sl = win.sl;
+  out.kern_sl = sliding ? pane.sl : win.sl;
+  out.cols = sliding ? pane.cols : win.cols;
+  out.means = win.means;
+  if (sliding) {
+    for (uint32_t c = 0; c < q->n_columns; c++) {
+      const ColState &p = pane.cols[c], &w = win.cols[c];
+      const uint8_t m = q->columns[c].agg_mask;
+      out.combine.push_back(CombineOp{p.count_off, w.count_off, 0, 0, COMBINE_ADD, 0});
+      if (m & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) {
+        if (q->columns[c].phys_type == TSKV_PT_F64) out.combine.push_back(CombineOp{p.sum_off, w.sum_off, 0, 0, COMBINE_F64_SUM, 0});
+        else out.combine.push_back(CombineOp{p.sum_off, w.sum_off, p.sumhi_off, w.sumhi_off, COMBINE_INT_SUM, (m & TSKV_AGG_MEAN) ? 1u : 0u});
+      }
+      if (m & TSKV_AGG_MIN) out.combine.push_back(CombineOp{p.min_off, w.min_off, 0, 0, COMBINE_MIN, 0});
+      if (m & TSKV_AGG_MAX) out.combine.push_back(CombineOp{p.max_off, w.max_off, 0, 0, COMBINE_MAX, 0});
+    }
+  }
+
+  // output column table
+  uint64_t fk = out.sl.first_keys_off, lk = out.sl.last_keys_off, fv = out.sl.selval_off, lv = out.sl.selval_off + out.sl.first_cells;
+  for (uint32_t c = 0; c < q->n_columns; c++) {
+    const tskv_agg_column &qc = q->columns[c];
+    for (unsigned bit = 0; bit < 7; bit++) {
+      unsigned agg = 1u << bit;
+      if (!(qc.agg_mask & agg)) continue;
+      OutCol oc{};
+      oc.count_off = win.cols[c].count_off;
+      oc.agg = (uint8_t)agg;
+      oc.phys_type = qc.phys_type;
+      switch (agg) {
+        case TSKV_AGG_SUM: oc.src_off = win.cols[c].sum_off; break;
+        case TSKV_AGG_MEAN: oc.src_off = win.msum_off[c] ? win.msum_off[c] : win.cols[c].sum_off; break;
+        case TSKV_AGG_MIN: oc.src_off = win.cols[c].min_off; break;
+        case TSKV_AGG_MAX: oc.src_off = win.cols[c].max_off; break;
+        case TSKV_AGG_FIRST: oc.src_off = fk; oc.val_off = fv; break;
+        case TSKV_AGG_LAST: oc.src_off = lk; oc.val_off = lv; break;
+        default: break;
+      }
+      out.outs.push_back(oc);
+    }
+    if (qc.agg_mask & TSKV_AGG_FIRST) { fk += n_cells; fv += n_cells; }
+    if (qc.agg_mask & TSKV_AGG_LAST) { lk += n_cells; lv += n_cells; }
+  }
+
+  // per-CTA shared-memory partial table (GROUP BY bucket / tags): count | sum | hi | min | max per column
+  std::vector<ColState> &cols = out.cols;
+  uint32_t words = 0;
+  for (uint32_t c = 0; c < q->n_columns; c++) {
+    const uint8_t m = q->columns[c].agg_mask;
+    const bool is_int = q->columns[c].phys_type != TSKV_PT_F64;
+    cols[c].s_count = words; words += (uint32_t)kern_cells;
+    if (m & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) { cols[c].s_sum = words; words += (uint32_t)kern_cells; }
+    if ((m & TSKV_AGG_MEAN) && is_int) { cols[c].s_hi = words; words += (uint32_t)kern_cells; }
+    if (m & TSKV_AGG_MIN) { cols[c].s_min = words; words += (uint32_t)kern_cells; }
+    if (m & TSKV_AGG_MAX) { cols[c].s_max = words; words += (uint32_t)kern_cells; }
+    if (kern_cells > (1u << 20)) { words = UINT32_MAX / 2; break; }
+  }
+  // table limit 32 KB: larger tables cost more in occupancy than the contention they remove (H100, C3: 10 columns x
+  // 168 buckets, 53 KB table: 7.8 ms vs 5.4 ms with global atomics); TSKV_SMEM_TABLE_KB overrides
+  const char *lim_env = getenv("TSKV_SMEM_TABLE_KB");
+  const uint64_t limit = (lim_env ? (uint64_t)atoi(lim_env) : 32) * 1024;
+  out.use_smem = (!q->group_by_series && (uint64_t)words * 8 <= limit) ? 1u : 0u;
+  out.smem_words = out.use_smem ? words : 0;
+  return out;
+}
+
+// Parts per page, resident CTAs per SM and grid of every bin's fused kernel (grid 0: the bin is not launched).
+void plan_grids(const tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, bool has_sel, uint32_t smem_words,
+                uint32_t has_tomb, int grid[N_BINS], int occ[N_BINS], uint32_t parts[N_BINS], uint32_t part_rows[N_BINS]) {
+  for (int b = 0; b < N_BINS; b++) { grid[b] = occ[b] = 0; parts[b] = 1; part_rows[b] = 0; }
+  const double sel_frac = plan_selected_fraction(pages->series.data(), pages->series.size(), q->series_ids, q->n_series);
+  // Grid sizes. Every kernel is persistent (warps pull tasks from their bin's counter). If the resident
+  // capacity allows, each bin gets one warp per estimated task (a single round: the makespan of a bin is
+  // quantised in units of one task = one chunk's serial decode); otherwise plan_serial_grids splits the blocks.
+  // Pages cut at restart points (skip_kernels.cuh): a chunk of 32 whole pages is one serial task of ~1000 rows; with
+  // few selected pages that chain is the scan's makespan, and with many the makespan is still quantised in chunk
+  // times. Cut the pages of the simple8b / gorilla bins into parts so that the scan has about 8 chunks per resident
+  // warp (more parts = shorter chains, but one more page open + two more run flushes per part).
+  // With every bin at 4 CTAs per SM, 8 chunks per resident warp measured best on C4 (H100: 4 parts of 256 rows per
+  // 1000-row page instead of 3 uneven parts of 384 / 384 / 232 rows at a target of 4; DESIGN.md §5). The
+  // simple8b-timestamp bins take the same parts although their rows cost ~1.6 x the rows of RLE-timestamp pages: twice
+  // the parts changed nothing (H100, C4: 1.03-1.05 vs 1.02 ms per scan).
+  if (pages->d_skip && !has_sel) {
+    double est_chunks = 0;
+    for (int b = 0; b < N_BINS; b++) est_chunks += std::ceil((pages->h_bin_start[b + 1] - pages->h_bin_start[b]) * sel_frac / 32.0);
+    const double resident_warps = (double)ctx->sm_count * SCAN_MIN_BLOCKS * (SCAN_THREADS / 32);
+    uint32_t want = plan_parts_wanted(est_chunks, resident_warps, 8.0);
+    const char *parts_env = getenv("TSKV_PARTS");  // fixed number of parts (1 = never cut)
+    if (parts_env) want = (uint32_t)std::max(1, atoi(parts_env));
+    for (int b = 0; b < N_BINS; b++) {
+      const int sb = serial_bin_of(b);
+      if (sb / N_VK == TK_GEN || sb % N_VK == VK_GEN) continue;
+      parts[b] = plan_bin_parts(pages->h_bin_maxrows[b], SKIP_ROWS, want, &part_rows[b]);
+    }
+  }
+  double need_sum = 0, occ_weighted = 0;
+  int need[N_BINS] = {0};
+  for (int b = 0; b < N_BINS; b++) {
+    uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
+    if (!n_bin) continue;
+    const int sb = serial_bin_of(b);
+    const void *fn = (const void *)(!has_sel ? scan_kernel_for<false>(sb, pages->h_bin_narrow[b]) : scan_kernel_for<true>(sb));
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[b], fn, SCAN_THREADS, serial_smem_bytes(sb, smem_words, has_tomb));
+    occ[b] = std::max(1, occ[b]);
+    const double est_items = n_bin * sel_frac * 1.02 + 32;
+    const uint32_t per_task = 32;  // pages per warp task: one chunk
+    const double tasks = est_items / per_task * parts[b];
+    need[b] = (int)(tasks / (SCAN_THREADS / 32)) + 1;
+    need[b] = std::min(need[b], (int)(((uint64_t)(n_bin + per_task - 1) / per_task * parts[b] + SCAN_THREADS / 32 - 1) / (SCAN_THREADS / 32)));
+    need_sum += need[b];
+    occ_weighted += (double)need[b] * occ[b];
+  }
+  const double capacity = need_sum > 0 ? (occ_weighted / need_sum) * ctx->sm_count : 0;  // resident blocks, mixed kernels
+  if (need_sum <= capacity) {
+    for (int b = 0; b < N_BINS; b++)
+      if (need[b]) grid[b] = std::max(1, need[b]);
+    return;
+  }
+  // a chunk of 32 pages is one long serial task, so a bin's time is quantised in rounds of its chunk time - choose
+  // the grids that minimise the makespan (plan_serial_grids)
+  double chunks[N_BINS], t_chunk[N_BINS];
+  for (int b = 0; b < N_BINS; b++) {
+    const uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
+    chunks[b] = need[b] ? std::ceil((n_bin * sel_frac * 1.02 + 16) / 32.0) * parts[b] : 0;
+    // (+ 12 rows' worth per chunk for opening its pages)
+    t_chunk[b] = n_bin ? chunk_cost(b) * ((double)pages->h_bin_rows[b] / n_bin / parts[b] + 12.0) : 1.0;
+  }
+  plan_serial_grids(N_BINS, chunks, t_chunk, occ, ctx->sm_count, SCAN_THREADS / 32, grid);
+  for (int b = 0; b < N_BINS; b++) grid[b] = std::min(grid[b], std::max(need[b], 0));
+  // The planned blocks per bin x 4, at most one warp per chunk: the blocks that are not resident at first start as the
+  // bins that finish early retire theirs and pick up what is left of the slower bins' chunks.
+  // H100, C4 at N = 1 (pages cut in 3 parts), ms per scan: planned grids 1.43-1.50, 2 x 1.10, 4 x 1.02 = one warp per
+  // chunk 1.02-1.03. Uncut pages too: planned grids 1.26-1.34, 4 x 1.12; FIRST / LAST scans (C5 shape) and
+  // host-resident page sets are the same with either (31.0-31.7 ms).
+  for (int b = 0; b < N_BINS; b++) grid[b] = std::min(std::max(need[b], 0), 4 * grid[b]);
+}
+
+// The merge pass over the overlapping chunks (merge_kernels.cuh) of one scan: which merge column groups it reads
+// (series selected, not pruned by its time bounds), the field pages of the query's columns to decode for them and where
+// their values / validity bits go, and the pass's share of the reader counters.
+struct MergePages {
+  std::vector<uint8_t> active;
+  std::vector<uint32_t> page;
+  std::vector<uint64_t> row_off, bm_off;
+  uint64_t bytes = 0, read_pages = 0;
+};
+// Refuses (TSKV_ERR_INVALID_ARG, with the page) a page whose type does not match its query column.
+tskv_status plan_merge_pages(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, MergePages *m) {
+  const OverlapPlan &op = pages->overlap;
+  m->active.assign(op.mcg_cg.size(), 0);
+  for (size_t k = 0; k < op.mcg_cg.size(); k++) {
+    const uint32_t cg = op.mcg_cg[k], tp = pages->h_cg_time_page[cg];
+    const tskv_page_desc &td = pages->h_descs[tp];
+    if (q->series_ids && !std::binary_search(q->series_ids, q->series_ids + q->n_series, td.series_id)) continue;
+    if (q->n_time_ranges) {  // filter_column_groups (reader/chunk.rs:12-50)
+      bool overlaps = false;
+      for (uint32_t r = 0; r < q->n_time_ranges; r++)
+        overlaps = overlaps || (pages->h_cg_bounds[cg].min_ts <= q->time_ranges[r].max_ts && pages->h_cg_bounds[cg].max_ts >= q->time_ranges[r].min_ts);
+      if (!overlaps) continue;
+    }
+    bool any = false;
+    for (uint64_t p = (uint64_t)tp + 1; p < pages->n_descs && pages->h_descs[p].phys_type != TSKV_PT_TIME; p++)
+      for (uint32_t c = 0; c < q->n_columns; c++)
+        if (pages->h_descs[p].column_id == q->columns[c].column_id) {
+          if (pages->h_descs[p].phys_type != q->columns[c].phys_type) {
+            ctx->set_error("page type does not match the query column type", (int64_t)p);
+            return TSKV_ERR_INVALID_ARG;
+          }
+          any = true;
+          m->page.push_back((uint32_t)p);
+          m->row_off.push_back((uint64_t)c * pages->merge_rows + op.mcg_row0[k]);
+          m->bm_off.push_back(((uint64_t)c * pages->merge_bm_words + pages->h_mcg_bm0[k]) * 4);
+          m->bytes += pages->h_descs[p].size;
+        }
+    if (!any) continue;  // a column group without any projected column yields no batch (column_group/mod.rs:43-52)
+    m->active[k] = 1;
+    m->bytes += td.size;
+    m->read_pages++;
+  }
+  m->read_pages += m->page.size();
+  return TSKV_OK;
+}
+
+// Creates the scan's events, allocates its device buffers (stream-ordered) and uploads the query's tables; sets the
+// error. *h2d: the bytes uploaded.
+tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, bool sliding,
+                       const ScanLayout &lay, tskv_scan *s, uint64_t *h2d) {
+  const uint32_t n_items = pages->n_items;
+  cudaEventCreate(&s->ev0);
+  cudaEventCreate(&s->ev1);
+  for (int b = 0; b <= N_BINS; b++) cudaEventCreate(&s->ev_bin[b]);
+  for (int b = 0; b < N_BINS; b++) {
+    cudaEventCreate(&s->ev_bin_start[b]);
+    cudaEventCreate(&s->ev_bin_done[b]);
+    cudaEventCreateWithFlags(&s->ev_gather[b], cudaEventDisableTiming);
+  }
+  s->n_series_sel = q->series_ids ? q->n_series : 0;
+  s->n_blocks = (n_items + 1023) / 1024;
+  cudaError_t e = cudaSuccess;
+  if (q->series_ids) {
+    e = stream_alloc(ctx, &s->d_series, q->n_series);
+    if (e == cudaSuccess && q->n_series)
+      e = cudaMemcpyAsync(s->d_series, q->series_ids, (size_t)q->n_series * 4, cudaMemcpyHostToDevice, ctx->stream);
+    *h2d += (uint64_t)q->n_series * 4;
+  }
+  if (tg.on) {  // GROUP BY tags: the group map, and the slots in group order for the work-list walk
+    const uint64_t n_slots = selected_slots(pages, q);
+    std::vector<uint32_t> walk;
+    if (!std::is_sorted(tg.ids, tg.ids + n_slots)) {  // (already in group order: the walk stays the selection order)
+      walk.resize(n_slots);
+      if (tg.n <= n_slots) {  // stable counting sort
+        std::vector<uint32_t> next(tg.n + 1, 0);
+        for (uint64_t i = 0; i < n_slots; i++) next[tg.ids[i] + 1]++;
+        for (uint32_t g = 0; g < tg.n; g++) next[g + 1] += next[g];
+        for (uint64_t i = 0; i < n_slots; i++) walk[next[tg.ids[i]]++] = (uint32_t)i;
+      } else {
+        std::iota(walk.begin(), walk.end(), 0u);
+        std::stable_sort(walk.begin(), walk.end(), [&](uint32_t a, uint32_t b) { return tg.ids[a] < tg.ids[b]; });
+      }
+    }
+    if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_slot_group, n_slots);
+    if (e == cudaSuccess && n_slots)
+      e = cudaMemcpyAsync(s->d_slot_group, tg.ids, (size_t)n_slots * 4, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess && !walk.empty()) e = stream_alloc(ctx, &s->d_walk, n_slots);
+    if (e == cudaSuccess && !walk.empty())
+      e = cudaMemcpyAsync(s->d_walk, walk.data(), (size_t)n_slots * 4, cudaMemcpyHostToDevice, ctx->stream);
+    *h2d += (n_slots + walk.size()) * 4;
+  }
+  if (e == cudaSuccess && q->series_ids) e = stream_alloc(ctx, &s->d_rank_slot, pages->series.size());
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_bucket, (size_t)2 * N_BINS * q->n_columns * WL_SUB + 1);
+  {
+    // One thread walks ALL column groups of a selected series: right for many series with a few groups each (TSBS
+    // shapes), serial for a handful of series with thousands of groups (one host over a year) - those take the pass
+    // over every field page instead, which is parallel in the pages. TSKV_WORKLIST=items / series forces one.
+    const char *wl = getenv("TSKV_WORKLIST");
+    s->worklist_by_items = wl ? wl[0] == 'i' : (uint64_t)pages->n_cg > 32ull * std::max<uint64_t>(1, pages->series.size());
+  }
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_cg_slot, pages->n_cg);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_item_flag, n_items);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_block_count, s->n_blocks);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_page, n_items);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_slot, n_items);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_qcol, n_items);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_bin_cstart, N_BINS + 2);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_cols, lay.cols.size());
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_outs, lay.outs.size());
+  s->n_means = (uint32_t)lay.means.size();
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_means, lay.means.size());
+  if (e == cudaSuccess && !lay.means.empty())
+    e = cudaMemcpyAsync(s->d_means, lay.means.data(), lay.means.size() * sizeof(MeanExport), cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_state, s->sl.total);
+  if (e == cudaSuccess && sliding) e = stream_alloc(ctx, &s->d_pane_state, s->kern_sl.total);
+  s->n_combine = (uint32_t)lay.combine.size();
+  if (e == cudaSuccess && sliding) e = stream_alloc(ctx, &s->d_combine, lay.combine.size());
+  if (e == cudaSuccess && sliding)
+    e = cudaMemcpyAsync(s->d_combine, lay.combine.data(), lay.combine.size() * sizeof(CombineOp), cudaMemcpyHostToDevice, ctx->stream);
+  s->preds.n = q->n_predicates;
+  for (uint32_t k = 0; k < q->n_predicates; k++) s->preds.p[k] = q->predicates[k];
+  if (q->n_predicates) ensure_page_stats(ctx, pages);  // value-statistics pruning (filter_column_groups, reader/chunk.rs:12-50)
+  if (e == cudaSuccess && q->n_predicates) e = stream_alloc(ctx, &s->d_row_keep, (size_t)pages->keep_words);
+  if (e == cudaSuccess) e = stream_alloc(ctx, reinterpret_cast<unsigned long long **>(&s->d_task_counter), AUX_WORDS);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_values, s->layout.n_out * s->layout.n_cells);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_validity, s->layout.validity_bytes + 8);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(s->d_outs, lay.outs.data(), lay.outs.size() * sizeof(OutCol), cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(s->d_cols, lay.cols.data(), lay.cols.size() * sizeof(ColState), cudaMemcpyHostToDevice, ctx->stream);
+  *h2d += lay.cols.size() * sizeof(ColState) + lay.outs.size() * sizeof(OutCol) + lay.means.size() * sizeof(MeanExport) +
+          sizeof(ScanParams) + lay.combine.size() * sizeof(CombineOp);
+  if (e != cudaSuccess) {
+    ctx->set_error(std::string("scan_prepare: ") + cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? TSKV_ERR_OOM : TSKV_ERR_CUDA;
+  }
+  unsigned long long *aux = reinterpret_cast<unsigned long long *>(s->d_task_counter);
+  s->d_status = reinterpret_cast<int32_t *>(aux + AUX_STATUS);
+  s->d_err_page = aux + AUX_ERR_PAGE;
+  s->d_stats = aux + AUX_STATS;
+  s->d_counters = aux + AUX_COUNTERS;
+  s->d_crc_status = reinterpret_cast<int32_t *>(aux + AUX_CRC_STATUS);
+  s->d_crc_err_page = aux + AUX_CRC_ERR_PAGE;
+  return TSKV_OK;
+}
+
+// The merge pass of a scan over a page set with overlapping chunks: its page list on the device and s->merge; sets the
+// error. *h2d: the bytes uploaded.
+tskv_status prepare_merge(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, tskv_scan *s, uint64_t *h2d) {
+  MergePages mp;
+  const tskv_status st = plan_merge_pages(ctx, pages, q, &mp);
+  if (st != TSKV_OK) return st;
+  const size_t n_mcg = mp.active.size(), n_mpages = mp.page.size();
+  s->n_merge_pages = (uint32_t)n_mpages;
+  s->merge_page_bytes = mp.bytes;
+  s->merge_read_pages = mp.read_pages;
+  cudaError_t e = stream_alloc(ctx, &s->d_mcg_active, n_mcg);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_mcg_active, mp.active.data(), n_mcg, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_mvals, (size_t)q->n_columns * pages->merge_rows);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_mvalid, (size_t)q->n_columns * pages->merge_bm_words);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_mpage, n_mpages);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_mrow_off, n_mpages);
+  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_mbm_off, n_mpages);
+  if (e == cudaSuccess && n_mpages) {
+    e = cudaMemcpyAsync(s->d_mpage, mp.page.data(), n_mpages * 4, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_mrow_off, mp.row_off.data(), n_mpages * 8, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_mbm_off, mp.bm_off.data(), n_mpages * 8, cudaMemcpyHostToDevice, ctx->stream);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);  // the host vectors go out of scope
+  if (e != cudaSuccess) {
+    ctx->set_error(std::string("scan_prepare (merge pass): ") + cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? TSKV_ERR_OOM : TSKV_ERR_CUDA;
+  }
+  *h2d += n_mcg + n_mpages * 20;
+  MergeParams &M = s->merge;
+  M.ts = pages->d_merge_ts;
+  M.mcg_row0 = pages->d_mcg_row0;
+  M.mcg_cg = pages->d_mcg_cg;
+  M.mcg_stream = pages->d_mcg_stream;
+  M.stream_group = pages->d_stream_group;
+  M.stream_first_mcg = pages->d_stream_first_mcg;
+  M.group_first_stream = pages->d_group_first_stream;
+  M.mcg_active = s->d_mcg_active;
+  M.vals = s->d_mvals;
+  M.valid = s->d_mvalid;
+  M.mcg_bm0 = pages->d_mcg_bm0;
+  M.cg_time_page = pages->d_cg_time_page;
+  M.cg_slot = s->d_cg_slot;
+  M.n_rows = pages->merge_rows;
+  M.bm_words = pages->merge_bm_words;
+  M.n_mcg = (uint32_t)n_mcg;
+  M.sel = s->has_sel ? 1u : 0u;
+  return TSKV_OK;
 }
 
 }  // namespace
@@ -632,9 +1141,6 @@ tskv_status tskvgpu_ctx_create(int32_t device_id, tskv_ctx **out_ctx) {
       if (cudaStreamCreateWithPriority(&ctx->bin_stream[b], cudaStreamNonBlocking, prio) != cudaSuccess)
         cudaStreamCreateWithFlags(&ctx->bin_stream[b], cudaStreamNonBlocking);
     }
-    // (TSKV_CRC_CONCURRENT: the per-read CRC checks on a stream of their own)
-    if (cudaStreamCreateWithPriority(&ctx->crc_stream, cudaStreamNonBlocking, greatest) != cudaSuccess)
-      cudaStreamCreateWithFlags(&ctx->crc_stream, cudaStreamNonBlocking);
   }
   // Dynamic shared memory ceiling of every scan kernel, set ONCE: the attribute belongs to the kernel, not to a launch,
   // so per-scan values would race between host threads that prepare scans with different table sizes.
@@ -675,7 +1181,6 @@ void tskvgpu_ctx_destroy(tskv_ctx *ctx) {
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
   for (int b = 0; b < N_BINS; b++)
     if (ctx->bin_stream[b]) cudaStreamDestroy(ctx->bin_stream[b]);
-  if (ctx->crc_stream) cudaStreamDestroy(ctx->crc_stream);
   delete ctx;
 }
 
@@ -1294,63 +1799,6 @@ tskv_status tskvgpu_query_output_layout_grouped(const tskv_pages *pages, const t
   return compute_layout(pages, q, TagGroups{true, group_ids, n_groups}, out);
 }
 
-// Sliding windows of `q` (window q->width, slide < q->width) by panes: the refusals of tskvgpu_scan_prepare_sliding
-// (DESIGN.md section 7) and the pane grid. Called under ctx->mu.
-static tskv_status check_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide, uint32_t *out_k) {
-  for (uint32_t c = 0; c < q->n_columns; c++)
-    if (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) {
-      ctx->set_error("sliding windows: FIRST / LAST drop a (page, window) run on a NULL at its first / last row, which "
-                     "pane partials cannot rebuild");
-      return TSKV_ERR_UNSUPPORTED;
-    }
-  if (slide > q->width) {
-    ctx->set_error("sliding windows: a slide wider than the window (rows between windows) is not pushed down");
-    return TSKV_ERR_UNSUPPORTED;
-  }
-  if (q->width >= (int64_t)1 << 61) {
-    ctx->set_error("sliding windows: window of 2^61 or more");
-    return TSKV_ERR_UNSUPPORTED;
-  }
-  const uint64_t k = ((uint64_t)q->width - 1) / (uint64_t)slide + 1;  // windows per row, ceil(window / slide)
-  if (k > 100) {
-    ctx->set_error("sliding windows: more than 100 windows per row (Too many overlapping windows)");
-    return TSKV_ERR_INVALID_ARG;
-  }
-  if (q->n_buckets < k) {
-    ctx->set_error("sliding windows: n_buckets must be at least ceil(window / slide)");
-    return TSKV_ERR_INVALID_ARG;
-  }
-  if ((unsigned __int128)q->n_buckets * (uint64_t)slide > (unsigned __int128)1 << 63) {
-    ctx->set_error("sliding windows: the window grid spans more than 2^63");
-    return TSKV_ERR_INVALID_ARG;
-  }
-  // With window % slide != 0 the reference keeps a row's copies by the test window-0 start <= t < end, which passes for
-  // every row whose dividend t - start_time % window + slide is >= 0 and whose window end does not wrap, and fails for
-  // other rows unless the remainder is 0: refuse unless every row the query can select is of the first kind.
-  if (q->width % slide != 0 && pages->n_cg) {
-    ensure_time_bounds(ctx, pages);
-    int64_t lo = pages->ts_min, hi = pages->ts_max;
-    if (q->n_time_ranges > 0) {
-      int64_t qlo = q->time_ranges[0].min_ts, qhi = q->time_ranges[0].max_ts;
-      for (uint32_t r = 1; r < q->n_time_ranges; r++) {
-        qlo = std::min(qlo, q->time_ranges[r].min_ts);
-        qhi = std::max(qhi, q->time_ranges[r].max_ts);
-      }
-      lo = std::max(lo, qlo);
-      hi = std::min(hi, qhi);
-    }
-    const __int128 om = q->origin % q->width;
-    if (lo <= hi && ((__int128)lo - om + slide < 0 || (__int128)hi - om + slide > (__int128)INT64_MAX ||
-                     (__int128)hi + q->width > (__int128)INT64_MAX)) {
-      ctx->set_error("sliding windows: window % slide != 0 and rows in the truncating-% or wrapping range of the window "
-                     "expression");
-      return TSKV_ERR_UNSUPPORTED;
-    }
-  }
-  *out_k = (uint32_t)k;
-  return TSKV_OK;
-}
-
 // tskvgpu_scan_prepare; slide > 0: tskvgpu_scan_prepare_sliding with slide < width; tg.on: GROUP BY tags.
 static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
                                 const TagGroups &tg, tskv_scan **out_scan) {
@@ -1358,279 +1806,37 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   std::lock_guard<std::mutex> lock(ctx->mu);
   ctx->set_error("");
   *out_scan = nullptr;
-  if (const char *why = tag_groups_refusal(pages, q, tg)) {
-    ctx->set_error(why);
-    return TSKV_ERR_INVALID_ARG;
-  }
-  tskv_output_layout L;
-  tskv_status st = compute_layout(pages, q, tg, &L);
-  if (st != TSKV_OK) {
-    ctx->set_error("invalid query (buckets / columns)");
-    return st;
-  }
-  if (q->n_columns > 126 || q->n_time_ranges > MAX_RANGES || (q->n_time_ranges && !q->time_ranges) ||
-      (q->series_ids == nullptr && q->n_series != 0 && false)) {
-    ctx->set_error("invalid query: at most 126 columns and 8 time ranges");
-    return TSKV_ERR_INVALID_ARG;
-  }
-  if (q->n_predicates > TSKV_MAX_PREDICATES || (q->n_predicates && !q->predicates)) {
-    ctx->set_error("invalid query: at most 8 field predicates");
-    return TSKV_ERR_INVALID_ARG;
-  }
-  for (uint32_t k = 0; k < q->n_predicates; k++)
-    if (q->predicates[k].phys_type < TSKV_PT_I64 || q->predicates[k].phys_type > TSKV_PT_F64 || q->predicates[k].op > TSKV_CMP_GE) {
-      ctx->set_error("invalid field predicate (type or operator)");
-      return TSKV_ERR_INVALID_ARG;
-    }
-  for (uint32_t c = 0; c < q->n_columns; c++) {
-    const tskv_agg_column &qc = q->columns[c];
-    if (qc.phys_type < TSKV_PT_I64 || qc.phys_type > TSKV_PT_BOOL || (qc.agg_mask & ~TSKV_AGG_ALL) || qc.agg_mask == 0) {
-      ctx->set_error("invalid query column (type or aggregate mask)");
-      return TSKV_ERR_INVALID_ARG;
-    }
-    if (qc.phys_type == TSKV_PT_BOOL && (qc.agg_mask & (TSKV_AGG_SUM | TSKV_AGG_MEAN))) {
-      ctx->set_error("sum / mean of a boolean column");
-      return TSKV_ERR_INVALID_ARG;
-    }
-    for (uint32_t c2 = 0; c2 < c; c2++)
-      if (q->columns[c2].column_id == qc.column_id) {
-        ctx->set_error("duplicate query column id");
-        return TSKV_ERR_INVALID_ARG;
-      }
-  }
-  if (q->series_ids)
-    for (uint32_t i = 1; i < q->n_series; i++)
-      if (q->series_ids[i] <= q->series_ids[i - 1]) {
-        ctx->set_error("series_ids must be sorted ascending and unique");
-        return TSKV_ERR_INVALID_ARG;
-      }
-  if ((q->reserved & TSKV_QUERY_MULTI_RANK) && !q->series_ids) {
-    bool needs_slots = q->group_by_series != 0 || tg.on;
-    for (uint32_t c = 0; c < q->n_columns; c++) needs_slots |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
-    if (needs_slots) {
-      ctx->set_error("multi-rank scan: GROUP BY series / tags and first/last need the global series_ids list (slots are positions in it)");
-      return TSKV_ERR_INVALID_ARG;
-    }
-  }
   uint32_t win_k = 1;
-  if (slide) {
-    st = check_sliding(ctx, pages, q, slide, &win_k);
-    if (st != TSKV_OK) return st;
-  }
+  tskv_status st = validate_query(ctx, pages, q, slide, tg, &win_k);
+  if (st != TSKV_OK) return st;
+  const tskv_output_layout L = output_layout(pages, q, tg);
   cudaSetDevice(ctx->device);
+  bool has_sel = false;  // any FIRST / LAST
+  for (uint32_t c = 0; c < q->n_columns; c++) has_sel |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
+  uint32_t slot_bits = 0;
+  int64_t rel_base = 0;
+  st = plan_keys(ctx, pages, q, has_sel, &slot_bits, &rel_base);
+  if (st != TSKV_OK) return st;
   tskv_scan *s = new tskv_scan();
+  s->ctx = ctx;
   s->pages = pages;
   s->layout = L;
   s->n_cols = q->n_columns;
   s->n_out = (uint32_t)L.n_out;
-  const uint64_t n_cells = L.n_cells;
+  s->has_sel = has_sel;
   // the fused kernels' bucket grid: the query's, or for a sliding scan the panes of width `slide`, from the start of the
   // last pane of window 0 to the start of the last window
   s->win_k = win_k;
   s->n_windows = q->n_buckets;
   s->n_panes = q->n_buckets - win_k + 1;
-  const uint64_t kern_cells = L.n_groups * s->n_panes;
-
-  // ---- first/last key budget ---------------------------------------------------------------------
-  bool any_sel = false;
-  for (uint32_t c = 0; c < q->n_columns; c++) any_sel |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
-  s->has_sel = any_sel;
-  uint64_t n_slots = q->series_ids ? q->n_series : pages->series.size();
-  uint32_t slot_bits = (q->group_by_series || n_slots <= 1) ? 0 : bits_for(n_slots - 1);
-  int64_t rel_base = 0;
-  if (any_sel && slot_bits > 0) {
-    unsigned rel_bits = 64;
-    if (q->width > 0) {
-      if (q->width < (int64_t)1 << 61) rel_bits = bits_for(2 * (uint64_t)q->width);
-    } else {
-      // unbucketed: rel = t - (lower bound of every in-range timestamp). A single-rank scan tightens unbounded / loose
-      // query ranges with the arena's own time bounds; a scan whose partials are merged with other ranks'
-      // (TSKV_QUERY_MULTI_RANK) must build keys every rank agrees on, i.e. from the query alone.
-      const bool multi_rank = (q->reserved & TSKV_QUERY_MULTI_RANK) != 0;
-      int64_t lo = INT64_MIN, hi = INT64_MAX;
-      if (!multi_rank) {
-        ensure_time_bounds(ctx, pages);
-        lo = pages->ts_min;
-        hi = pages->ts_max;
-      }
-      if (q->n_time_ranges > 0) {
-        int64_t qlo = q->time_ranges[0].min_ts, qhi = q->time_ranges[0].max_ts;
-        for (uint32_t k = 1; k < q->n_time_ranges; k++) {
-          qlo = std::min(qlo, q->time_ranges[k].min_ts);
-          qhi = std::max(qhi, q->time_ranges[k].max_ts);
-        }
-        lo = std::max(lo, qlo);
-        hi = std::min(hi, qhi);
-      }
-      if (hi < lo) {
-        rel_bits = 0;  // nothing can be in range
-      } else {
-        uint64_t span = (uint64_t)hi - (uint64_t)lo;
-        rel_bits = bits_for(span);
-        rel_base = lo;
-      }
-    }
-    if (rel_bits + slot_bits > 62) {
-      ctx->set_error("first/last across series: (bucket width or time span) x series count does not fit the 62-bit tie-break key");
-      delete s;
-      return TSKV_ERR_UNSUPPORTED;
-    }
-  }
-
-  // ---- state layout ------------------------------------------------------------------------------
-  // a sliding scan: what the fused kernels write (panes) and what the rest of the pass sees (windows)
-  const StatePlan win = plan_state(q, n_cells);
-  const StatePlan pane = slide ? plan_state(q, kern_cells) : StatePlan{};
-  s->sl = win.sl;
-  s->kern_sl = slide ? pane.sl : win.sl;
-  std::vector<ColState> cols = slide ? pane.cols : win.cols;
-  const std::vector<MeanExport> &means = win.means;
-  const std::vector<uint64_t> &msum_off = win.msum_off;
-  const StateLayout &sl = s->sl;
-  std::vector<CombineOp> combine;
-  if (slide) {
-    for (uint32_t c = 0; c < q->n_columns; c++) {
-      const ColState &p = pane.cols[c], &w = win.cols[c];
-      const uint8_t m = q->columns[c].agg_mask;
-      combine.push_back(CombineOp{p.count_off, w.count_off, 0, 0, COMBINE_ADD, 0});
-      if (m & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) {
-        if (q->columns[c].phys_type == TSKV_PT_F64) combine.push_back(CombineOp{p.sum_off, w.sum_off, 0, 0, COMBINE_F64_SUM, 0});
-        else combine.push_back(CombineOp{p.sum_off, w.sum_off, p.sumhi_off, w.sumhi_off, COMBINE_INT_SUM, (m & TSKV_AGG_MEAN) ? 1u : 0u});
-      }
-      if (m & TSKV_AGG_MIN) combine.push_back(CombineOp{p.min_off, w.min_off, 0, 0, COMBINE_MIN, 0});
-      if (m & TSKV_AGG_MAX) combine.push_back(CombineOp{p.max_off, w.max_off, 0, 0, COMBINE_MAX, 0});
-    }
-  }
-
-  // output column table
-  std::vector<OutCol> outs;
-  {
-    uint64_t fk = sl.first_keys_off, lk = sl.last_keys_off, fv = sl.selval_off, lv = sl.selval_off + sl.first_cells;
-    for (uint32_t c = 0; c < q->n_columns; c++) {
-      const tskv_agg_column &qc = q->columns[c];
-      for (unsigned bit = 0; bit < 7; bit++) {
-        unsigned agg = 1u << bit;
-        if (!(qc.agg_mask & agg)) continue;
-        OutCol oc{};
-        oc.count_off = win.cols[c].count_off;
-        oc.agg = (uint8_t)agg;
-        oc.phys_type = qc.phys_type;
-        switch (agg) {
-          case TSKV_AGG_SUM: oc.src_off = win.cols[c].sum_off; break;
-          case TSKV_AGG_MEAN: oc.src_off = msum_off[c] ? msum_off[c] : win.cols[c].sum_off; break;
-          case TSKV_AGG_MIN: oc.src_off = win.cols[c].min_off; break;
-          case TSKV_AGG_MAX: oc.src_off = win.cols[c].max_off; break;
-          case TSKV_AGG_FIRST: oc.src_off = fk; oc.val_off = fv; break;
-          case TSKV_AGG_LAST: oc.src_off = lk; oc.val_off = lv; break;
-          default: break;
-        }
-        outs.push_back(oc);
-      }
-      if (qc.agg_mask & TSKV_AGG_FIRST) { fk += n_cells; fv += n_cells; }
-      if (qc.agg_mask & TSKV_AGG_LAST) { lk += n_cells; lv += n_cells; }
-    }
-  }
-
-  // ---- device allocations (stream-ordered) + query arguments H2D --------------------------------------
-  const uint32_t n_items = pages->n_items;
-  s->ctx = ctx;
-  cudaEventCreate(&s->ev0);
-  cudaEventCreate(&s->ev1);
-  for (int b = 0; b <= N_BINS; b++) cudaEventCreate(&s->ev_bin[b]);
-  for (int b = 0; b < N_BINS; b++) {
-    cudaEventCreate(&s->ev_bin_start[b]);
-    cudaEventCreate(&s->ev_bin_done[b]);
-    cudaEventCreateWithFlags(&s->ev_gather[b], cudaEventDisableTiming);
-  }
-  s->n_series_sel = q->series_ids ? q->n_series : 0;
-  s->n_blocks = (n_items + 1023) / 1024;
-  cudaError_t e = cudaSuccess;
+  const ScanLayout lay = plan_layout(q, slide != 0, L.n_cells, L.n_groups * s->n_panes);
+  s->sl = lay.sl;
+  s->kern_sl = lay.kern_sl;
   uint64_t h2d = 0;
-  if (q->series_ids) {
-    e = stream_alloc(ctx, &s->d_series, q->n_series);
-    if (e == cudaSuccess && q->n_series)
-      e = cudaMemcpyAsync(s->d_series, q->series_ids, (size_t)q->n_series * 4, cudaMemcpyHostToDevice, ctx->stream);
-    h2d += (uint64_t)q->n_series * 4;
-  }
-  if (tg.on) {  // GROUP BY tags: the group map, and the slots in group order for the work-list walk
-    const uint64_t n_slots = selected_slots(pages, q);
-    std::vector<uint32_t> walk;
-    if (!std::is_sorted(tg.ids, tg.ids + n_slots)) {  // (already in group order: the walk stays the selection order)
-      walk.resize(n_slots);
-      if (tg.n <= n_slots) {  // stable counting sort
-        std::vector<uint32_t> next(tg.n + 1, 0);
-        for (uint64_t i = 0; i < n_slots; i++) next[tg.ids[i] + 1]++;
-        for (uint32_t g = 0; g < tg.n; g++) next[g + 1] += next[g];
-        for (uint64_t i = 0; i < n_slots; i++) walk[next[tg.ids[i]]++] = (uint32_t)i;
-      } else {
-        std::iota(walk.begin(), walk.end(), 0u);
-        std::stable_sort(walk.begin(), walk.end(), [&](uint32_t a, uint32_t b) { return tg.ids[a] < tg.ids[b]; });
-      }
-    }
-    if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_slot_group, n_slots);
-    if (e == cudaSuccess && n_slots)
-      e = cudaMemcpyAsync(s->d_slot_group, tg.ids, (size_t)n_slots * 4, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess && !walk.empty()) e = stream_alloc(ctx, &s->d_walk, n_slots);
-    if (e == cudaSuccess && !walk.empty())
-      e = cudaMemcpyAsync(s->d_walk, walk.data(), (size_t)n_slots * 4, cudaMemcpyHostToDevice, ctx->stream);
-    h2d += (n_slots + walk.size()) * 4;
-  }
-  if (e == cudaSuccess && q->series_ids) e = stream_alloc(ctx, &s->d_rank_slot, pages->series.size());
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_bucket, (size_t)2 * N_BINS * q->n_columns * WL_SUB + 1);
-  {
-    // One thread walks ALL column groups of a selected series: right for many series with a few groups each (TSBS
-    // shapes), serial for a handful of series with thousands of groups (one host over a year) - those take the pass
-    // over every field page instead, which is parallel in the pages. TSKV_WORKLIST=items / series forces one.
-    const char *wl = getenv("TSKV_WORKLIST");
-    s->worklist_by_items = wl ? wl[0] == 'i' : (uint64_t)pages->n_cg > 32ull * std::max<uint64_t>(1, pages->series.size());
-  }
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_cg_slot, pages->n_cg);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_item_flag, n_items);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_block_count, s->n_blocks);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_page, n_items);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_slot, n_items);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_qcol, n_items);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_bin_cstart, N_BINS + 2);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_cols, cols.size());
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_outs, outs.size());
-  s->n_means = (uint32_t)means.size();
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_means, means.size());
-  if (e == cudaSuccess && !means.empty())
-    e = cudaMemcpyAsync(s->d_means, means.data(), means.size() * sizeof(MeanExport), cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_state, sl.total);
-  if (e == cudaSuccess && slide) e = stream_alloc(ctx, &s->d_pane_state, s->kern_sl.total);
-  s->n_combine = (uint32_t)combine.size();
-  if (e == cudaSuccess && slide) e = stream_alloc(ctx, &s->d_combine, combine.size());
-  if (e == cudaSuccess && slide)
-    e = cudaMemcpyAsync(s->d_combine, combine.data(), combine.size() * sizeof(CombineOp), cudaMemcpyHostToDevice, ctx->stream);
-  s->preds.n = q->n_predicates;
-  for (uint32_t k = 0; k < q->n_predicates; k++) s->preds.p[k] = q->predicates[k];
-  if (q->n_predicates) ensure_page_stats(ctx, pages);  // value-statistics pruning (filter_column_groups, reader/chunk.rs:12-50)
-  if (e == cudaSuccess && q->n_predicates) e = stream_alloc(ctx, &s->d_row_keep, (size_t)pages->keep_words);
-  // aux block (8-byte units): [0..7] task counters (N_BINS x u32) | 8 status | 9 err_page | 10,11 stats
-  //                           | 12 pages 13 bytes 14..22 per-bin bytes
-  if (e == cudaSuccess) e = stream_alloc(ctx, reinterpret_cast<unsigned long long **>(&s->d_task_counter), 32);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_values, L.n_out * L.n_cells);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_validity, L.validity_bytes + 8);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_outs, outs.data(), outs.size() * sizeof(OutCol), cudaMemcpyHostToDevice, ctx->stream);
-  h2d += cols.size() * sizeof(ColState) + outs.size() * sizeof(OutCol) + means.size() * sizeof(MeanExport) + sizeof(ScanParams) +
-         combine.size() * sizeof(CombineOp);
-  if (e != cudaSuccess) {
-    ctx->set_error(std::string("scan_prepare: ") + cudaGetErrorString(e));
+  if ((st = alloc_scan(ctx, pages, q, tg, slide != 0, lay, s, &h2d)) != TSKV_OK) {
     free_scan(s);
-    return e == cudaErrorMemoryAllocation ? TSKV_ERR_OOM : TSKV_ERR_CUDA;
+    return st;
   }
-  unsigned long long *aux = reinterpret_cast<unsigned long long *>(s->d_task_counter);
-  s->d_status = reinterpret_cast<int32_t *>(aux + 8);
-  s->d_err_page = aux + 9;
-  s->d_stats = aux + 10;
-  s->d_counters = aux + 12;
-  s->d_crc_status = reinterpret_cast<int32_t *>(aux + 28);
-  s->d_crc_err_page = aux + 29;
-  cudaEventCreateWithFlags(&s->ev_crc, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&s->ev_ccrc, cudaEventDisableTiming);
-
-  // ---- kernel parameters ------------------------------------------------------------------------------
   ScanParams &P = s->params;
   P.arena = pages->d_arena;
   P.descs = pages->d_descs;
@@ -1663,218 +1869,31 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   P.first_bucket_start = (int64_t)((uint64_t)q->first_bucket_start + (uint64_t)(win_k - 1) * (uint64_t)P.width);
   P.n_buckets = s->n_panes;
   P.group_by_series = q->group_by_series;
-  P.n_cells = kern_cells;
+  P.n_cells = L.n_groups * s->n_panes;
   P.slot_group = s->d_slot_group;
   P.slot_bits = slot_bits;
   P.slot_max = slot_bits ? (uint32_t)((1ull << slot_bits) - 1) : 0;
   P.rel_base = rel_base;
-  // per-CTA shared-memory partial table (GROUP BY bucket / tags): count | sum | hi | min | max per column
-  {
-    uint32_t words = 0;
-    for (uint32_t c = 0; c < q->n_columns; c++) {
-      const uint8_t m = q->columns[c].agg_mask;
-      const bool is_int = q->columns[c].phys_type != TSKV_PT_F64;
-      cols[c].s_count = words; words += (uint32_t)kern_cells;
-      if (m & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) { cols[c].s_sum = words; words += (uint32_t)kern_cells; }
-      if ((m & TSKV_AGG_MEAN) && is_int) { cols[c].s_hi = words; words += (uint32_t)kern_cells; }
-      if (m & TSKV_AGG_MIN) { cols[c].s_min = words; words += (uint32_t)kern_cells; }
-      if (m & TSKV_AGG_MAX) { cols[c].s_max = words; words += (uint32_t)kern_cells; }
-      if (kern_cells > (1u << 20)) { words = UINT32_MAX / 2; break; }
-    }
-    // table limit 32 KB: larger tables cost more in occupancy than the contention they remove (H100, C3: 10 columns x
-    // 168 buckets, 53 KB table: 7.8 ms vs 5.4 ms with global atomics); TSKV_SMEM_TABLE_KB overrides
-    const char *lim_env = getenv("TSKV_SMEM_TABLE_KB");
-    const uint64_t limit = (lim_env ? (uint64_t)atoi(lim_env) : 32) * 1024;
-    P.use_smem = (!q->group_by_series && (uint64_t)words * 8 <= limit) ? 1u : 0u;
-    P.smem_words = P.use_smem ? words : 0;
-    P.n_cols = q->n_columns;
-    P.row_keep = s->d_row_keep;
-    P.keep_off = pages->d_keep_off;
-    P.skip_off = pages->d_skip_off;
-    P.page_narrow = pages->d_narrow;
-    P.skip = pages->d_skip;
-    for (int b = 0; b < N_BINS; b++) { P.bin_parts[b] = 1; P.bin_part_rows[b] = 0; }
-    P.has_tomb = pages->n_tomb_ranges ? 1u : 0u;
-    P.tomb_keys = pages->d_tomb_keys;
-    P.tomb_off = pages->d_tomb_off;
-    P.tomb_ranges = pages->d_tomb_ranges;
-    P.n_tomb_keys = pages->n_tomb_keys;
-    P.n_tomb_global = pages->n_tomb_global;
-    s->tomb_epoch = pages->tomb_epoch;
-  }
-  if (cudaMemcpyAsync(s->d_cols, cols.data(), cols.size() * sizeof(ColState), cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) {
-    ctx->set_error("scan_prepare: column table upload failed");
-    free_scan(s);
-    return TSKV_ERR_CUDA;
-  }
-
-  {
-    const double sel_frac = plan_selected_fraction(pages->series.data(), pages->series.size(), q->series_ids, q->n_series);
-    // Grid sizes. Every kernel is persistent (warps pull tasks from their bin's counter). If the resident
-    // capacity allows, each bin gets one warp per estimated task (a single round: the makespan of a bin is
-    // quantised in units of one task = one chunk's serial decode); otherwise plan_serial_grids splits the blocks.
-    // Pages cut at restart points (skip_kernels.cuh): a chunk of 32 whole pages is one serial task of ~1000 rows; with
-    // few selected pages that chain is the scan's makespan, and with many the makespan is still quantised in chunk
-    // times. Cut the pages of the simple8b / gorilla bins into parts so that the scan has about PARTS_TARGET chunks
-    // per resident warp (more parts = shorter chains, but one more page open + two more run flushes per part).
-    // With every bin at 4 CTAs per SM, 8 chunks per resident warp measured best on C4 (H100: 4 parts of 256 rows per
-    // 1000-row page instead of 3 uneven parts of 384 / 384 / 232 rows at a target of 4; DESIGN.md §5).
-    uint32_t parts[N_BINS];
-    for (int b = 0; b < N_BINS; b++) parts[b] = 1;
-    if (pages->d_skip && !s->has_sel) {
-      double est_chunks = 0;
-      for (int b = 0; b < N_BINS; b++) est_chunks += std::ceil((pages->h_bin_start[b + 1] - pages->h_bin_start[b]) * sel_frac / 32.0);
-      const double resident_warps = (double)ctx->sm_count * SCAN_MIN_BLOCKS * (SCAN_THREADS / 32);
-      const char *pt_env = getenv("TSKV_PARTS_TARGET");
-      uint32_t want = plan_parts_wanted(est_chunks, resident_warps, pt_env ? atof(pt_env) : 8.0);
-      const char *parts_env = getenv("TSKV_PARTS");  // fixed number of parts (1 = never cut)
-      if (parts_env) want = (uint32_t)std::max(1, atoi(parts_env));
-      for (int b = 0; b < N_BINS; b++) {
-        const int sb = serial_bin_of(b);
-        if (sb / N_VK == TK_GEN || sb % N_VK == VK_GEN) continue;
-        uint32_t want_b = want;
-        if (sb / N_VK == TK_S8B) {  // TSKV_PARTS_TS: another number of parts for the simple8b-timestamp bins (their rows cost
-          // ~1.6 x the rows of RLE-timestamp pages; H100, C4: twice the parts changes nothing, 1.03-1.05 vs 1.02 ms per scan)
-          const char *ts_env = getenv("TSKV_PARTS_TS");
-          if (ts_env) want_b = (uint32_t)std::max(1, atoi(ts_env));
-        }
-        uint32_t part_rows = 0;
-        parts[b] = plan_bin_parts(pages->h_bin_maxrows[b], SKIP_ROWS, want_b, &part_rows);
-        P.bin_parts[b] = parts[b];
-        P.bin_part_rows[b] = part_rows;
-      }
-    }
-    double need_sum = 0, occ_weighted = 0;
-    int need[N_BINS] = {0}, occ_bin[N_BINS] = {0};
-    for (int b = 0; b < N_BINS; b++) {
-      uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
-      if (!n_bin) continue;
-      int occ = 0;
-      const int sb = serial_bin_of(b);
-      const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, SCAN_THREADS, serial_smem_bytes(sb, P.smem_words, P.has_tomb));
-      occ = std::max(1, occ);
-      occ_bin[b] = occ;
-      s->occ[b] = occ;
-      const double est_items = n_bin * sel_frac * 1.02 + 32;
-      const uint32_t per_task = 32;  // pages per warp task: one chunk
-      const double tasks = est_items / per_task * parts[b];
-      need[b] = (int)(tasks / (SCAN_THREADS / 32)) + 1;
-      need[b] = std::min(need[b], (int)(((uint64_t)(n_bin + per_task - 1) / per_task * parts[b] + SCAN_THREADS / 32 - 1) / (SCAN_THREADS / 32)));
-      need_sum += need[b];
-      occ_weighted += (double)need[b] * occ;
-    }
-    const double capacity = need_sum > 0 ? (occ_weighted / need_sum) * ctx->sm_count : 0;  // resident blocks, mixed kernels
-    if (need_sum <= capacity) {
-      for (int b = 0; b < N_BINS; b++)
-        if (need[b]) s->grid[b] = std::max(1, need[b]);
-    } else {
-      // a chunk of 32 pages is one long serial task, so a bin's time is quantised in rounds of its chunk time - choose
-      // the grids that minimise the makespan (plan_serial_grids)
-      double chunks[N_BINS], t_chunk[N_BINS];
-      for (int b = 0; b < N_BINS; b++) {
-        const uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
-        chunks[b] = need[b] ? std::ceil((n_bin * sel_frac * 1.02 + 16) / 32.0) * parts[b] : 0;
-        // (+ 12 rows' worth per chunk for opening its pages)
-        t_chunk[b] = n_bin ? chunk_cost(b) * ((double)pages->h_bin_rows[b] / n_bin / parts[b] + 12.0) : 1.0;
-      }
-      plan_serial_grids(N_BINS, chunks, t_chunk, occ_bin, ctx->sm_count, SCAN_THREADS / 32, s->grid);
-      for (int b = 0; b < N_BINS; b++) s->grid[b] = std::min(s->grid[b], std::max(need[b], 0));
-      // TSKV_GRID_OVERSUB=f: f x the planned blocks per bin; the blocks that are not resident at first start as the
-      // bins that finish early retire theirs and pick up what is left of the slower bins' chunks
-      // H100, C4 at N = 1 (pages cut in 3 parts), ms per scan: planned grids 1.43-1.50, 2 x 1.10, 4 x 1.02 = one warp per
-      // chunk 1.02-1.03. Uncut pages too: planned grids 1.26-1.34, 4 x 1.12; FIRST / LAST scans (C5 shape) and
-      // host-resident page sets are the same with either (31.0-31.7 ms).
-      {
-        const char *ov = getenv("TSKV_GRID_OVERSUB");
-        const double f = ov ? atof(ov) : 4.0;
-        if (f > 1.0)
-          for (int b = 0; b < N_BINS; b++) s->grid[b] = std::min(std::max(need[b], 0), (int)std::ceil(s->grid[b] * f));
-      }
-      // TSKV_GRID_MODE=1: one warp per chunk for every bin; the block scheduler queues what does not fit
-      const char *gm = getenv("TSKV_GRID_MODE");
-      if (gm && gm[0] == '1')
-        for (int b = 0; b < N_BINS; b++) s->grid[b] = need[b];
-    }
-  }
-  // ---- merge pass over the overlapping chunks (merge_kernels.cuh): which merge column groups this scan reads
-  // (series selected, not pruned by its time bounds), and the field pages of the query's columns to decode for them
+  P.use_smem = lay.use_smem;
+  P.smem_words = lay.smem_words;
+  P.n_cols = q->n_columns;
+  P.row_keep = s->d_row_keep;
+  P.keep_off = pages->d_keep_off;
+  P.skip_off = pages->d_skip_off;
+  P.page_narrow = pages->d_narrow;
+  P.skip = pages->d_skip;
+  P.has_tomb = pages->n_tomb_ranges ? 1u : 0u;
+  P.tomb_keys = pages->d_tomb_keys;
+  P.tomb_off = pages->d_tomb_off;
+  P.tomb_ranges = pages->d_tomb_ranges;
+  P.n_tomb_keys = pages->n_tomb_keys;
+  P.n_tomb_global = pages->n_tomb_global;
+  s->tomb_epoch = pages->tomb_epoch;
+  plan_grids(ctx, pages, q, has_sel, P.smem_words, P.has_tomb, s->grid, s->occ, P.bin_parts, P.bin_part_rows);
   s->chunk_epoch = pages->chunk_epoch;
-  if (pages->merge_rows) {
-    const OverlapPlan &op = pages->overlap;
-    const size_t n_mcg = op.mcg_cg.size();
-    std::vector<uint8_t> active(n_mcg, 0);
-    std::vector<uint32_t> mpage;
-    std::vector<uint64_t> mrow_off, mbm_off;
-    for (size_t k = 0; k < n_mcg; k++) {
-      const uint32_t cg = op.mcg_cg[k], tp = pages->h_cg_time_page[cg];
-      const tskv_page_desc &td = pages->h_descs[tp];
-      if (q->series_ids && !std::binary_search(q->series_ids, q->series_ids + q->n_series, td.series_id)) continue;
-      if (q->n_time_ranges) {  // filter_column_groups (reader/chunk.rs:12-50)
-        bool overlaps = false;
-        for (uint32_t r = 0; r < q->n_time_ranges; r++)
-          overlaps = overlaps || (pages->h_cg_bounds[cg].min_ts <= q->time_ranges[r].max_ts && pages->h_cg_bounds[cg].max_ts >= q->time_ranges[r].min_ts);
-        if (!overlaps) continue;
-      }
-      bool any = false;
-      for (uint64_t p = (uint64_t)tp + 1; p < pages->n_descs && pages->h_descs[p].phys_type != TSKV_PT_TIME; p++)
-        for (uint32_t c = 0; c < q->n_columns; c++)
-          if (pages->h_descs[p].column_id == q->columns[c].column_id) {
-            if (pages->h_descs[p].phys_type != q->columns[c].phys_type) {
-              ctx->set_error("page type does not match the query column type", (int64_t)p);
-              free_scan(s);
-              return TSKV_ERR_INVALID_ARG;
-            }
-            any = true;
-            mpage.push_back((uint32_t)p);
-            mrow_off.push_back((uint64_t)c * pages->merge_rows + op.mcg_row0[k]);
-            mbm_off.push_back(((uint64_t)c * pages->merge_bm_words + pages->h_mcg_bm0[k]) * 4);
-            s->merge_page_bytes += pages->h_descs[p].size;
-          }
-      if (!any) continue;  // a column group without any projected column yields no batch (column_group/mod.rs:43-52)
-      active[k] = 1;
-      s->merge_page_bytes += td.size;
-      s->merge_read_pages++;
-    }
-    s->n_merge_pages = (uint32_t)mpage.size();
-    s->merge_read_pages += mpage.size();
-    cudaError_t me = stream_alloc(ctx, &s->d_mcg_active, n_mcg);
-    if (me == cudaSuccess) me = cudaMemcpyAsync(s->d_mcg_active, active.data(), n_mcg, cudaMemcpyHostToDevice, ctx->stream);
-    if (me == cudaSuccess) me = stream_alloc(ctx, &s->d_mvals, (size_t)q->n_columns * pages->merge_rows);
-    if (me == cudaSuccess) me = stream_alloc(ctx, &s->d_mvalid, (size_t)q->n_columns * pages->merge_bm_words);
-    if (me == cudaSuccess) me = stream_alloc(ctx, &s->d_mpage, mpage.size());
-    if (me == cudaSuccess) me = stream_alloc(ctx, &s->d_mrow_off, mpage.size());
-    if (me == cudaSuccess) me = stream_alloc(ctx, &s->d_mbm_off, mpage.size());
-    if (me == cudaSuccess && !mpage.empty()) {
-      me = cudaMemcpyAsync(s->d_mpage, mpage.data(), mpage.size() * 4, cudaMemcpyHostToDevice, ctx->stream);
-      if (me == cudaSuccess) me = cudaMemcpyAsync(s->d_mrow_off, mrow_off.data(), mpage.size() * 8, cudaMemcpyHostToDevice, ctx->stream);
-      if (me == cudaSuccess) me = cudaMemcpyAsync(s->d_mbm_off, mbm_off.data(), mpage.size() * 8, cudaMemcpyHostToDevice, ctx->stream);
-    }
-    if (me == cudaSuccess) me = cudaStreamSynchronize(ctx->stream);  // the host vectors go out of scope
-    if (me != cudaSuccess) {
-      ctx->set_error(std::string("scan_prepare (merge pass): ") + cudaGetErrorString(me));
-      free_scan(s);
-      return me == cudaErrorMemoryAllocation ? TSKV_ERR_OOM : TSKV_ERR_CUDA;
-    }
-    h2d += n_mcg + mpage.size() * 20;
-    MergeParams &M = s->merge;
-    M.ts = pages->d_merge_ts;
-    M.mcg_row0 = pages->d_mcg_row0;
-    M.mcg_cg = pages->d_mcg_cg;
-    M.mcg_stream = pages->d_mcg_stream;
-    M.stream_group = pages->d_stream_group;
-    M.stream_first_mcg = pages->d_stream_first_mcg;
-    M.group_first_stream = pages->d_group_first_stream;
-    M.mcg_active = s->d_mcg_active;
-    M.vals = s->d_mvals;
-    M.valid = s->d_mvalid;
-    M.mcg_bm0 = pages->d_mcg_bm0;
-    M.cg_time_page = pages->d_cg_time_page;
-    M.cg_slot = s->d_cg_slot;
-    M.n_rows = pages->merge_rows;
-    M.bm_words = pages->merge_bm_words;
-    M.n_mcg = (uint32_t)n_mcg;
-    M.sel = s->has_sel ? 1u : 0u;
+  if (pages->merge_rows && (st = prepare_merge(ctx, pages, q, s, &h2d)) != TSKV_OK) {
+    free_scan(s);
+    return st;
   }
   ctx->counters.h2d_bytes = h2d;
   *out_scan = s;
@@ -1929,7 +1948,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
   uint64_t launches = 0;
   {  // state identities + the pass's scratch (task counters / status / counters, bin starts, work-list buckets): one launch
     const uint32_t init_blocks = (uint32_t)std::min<uint64_t>((s->kern_sl.total + 255) / 256, 4096);
-    k_init_state<<<std::max(1u, init_blocks), 256, 0, ctx->stream>>>(s->params.state, s->kern_sl, aux, 32, s->d_bin_cstart, N_BINS + 2,
+    k_init_state<<<std::max(1u, init_blocks), 256, 0, ctx->stream>>>(s->params.state, s->kern_sl, aux, AUX_WORDS, s->d_bin_cstart, N_BINS + 2,
                                                                    s->d_bucket, N_BINS * s->n_cols * WL_SUB);
     launches++;
   }
@@ -2022,21 +2041,19 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
   // bin's tail is exposed after the last byte has arrived.
   int order[N_BINS];
   for (int b = 0; b < N_BINS; b++) order[b] = b;
-  static const bool gather_concurrent = getenv("TSKV_GATHER_CONCURRENT") != nullptr;
-  if (pages->h_mapped && !gather_concurrent)
+  if (pages->h_mapped)
     std::stable_sort(order, order + N_BINS, [&](int a, int b) { return pages->h_bin_bytes[a] > pages->h_bin_bytes[b]; });
-  else if (!pages->h_mapped)
+  else
     std::stable_sort(order, order + N_BINS, [&](int a, int b) { return chunk_cost(a) > chunk_cost(b); });
   int prev_gather = -1;
-  bool crc_forked = false;
   for (int oi = 0; oi < N_BINS; oi++) {
     const int b = order[oi];
     if (!s->grid[b]) continue;
     cudaStreamWaitEvent(ctx->bin_stream[b], ev_fork, 0);
     int bin = b;
+    const uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
     if (pages->h_mapped) {
-      if (prev_gather >= 0 && !gather_concurrent) cudaStreamWaitEvent(ctx->bin_stream[b], s->ev_gather[prev_gather], 0);
-      uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
+      if (prev_gather >= 0) cudaStreamWaitEvent(ctx->bin_stream[b], s->ev_gather[prev_gather], 0);
       uint32_t gblocks = std::max(1u, std::min<uint32_t>((uint32_t)ctx->sm_count * 4, (n_bin + 7) / 8));
       k_gather_pages<<<gblocks, 256, 0, ctx->bin_stream[b]>>>(pages->h_mapped, pages->d_arena, pages->d_descs,
                                                               pages->d_time_page_of, s->d_work_page, s->d_work_qcol,
@@ -2046,29 +2063,15 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       prev_gather = b;
     }
     if (pages->verify_on_read) {  // Page::crc_validation on every read (tsm/reader.rs:259), also for pages resident in HBM
-      uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
       // In front of the bin's fused kernel (HBM-resident pages) / after the bin's transfer, under the next bin's
-      // (host-resident pages). TSKV_CRC_CONCURRENT=1 runs the checks of HBM-resident pages BESIDE the fused kernels on a
-      // stream of their own instead - H100, C4: 1.84-2.03 ms per scan with 1-8 CRC blocks per SM against
-      // 1.39 ms in line (the check needs the whole machine's lanes to hide its dependent table lookups; a slice of the
-      // machine makes it the step's critical path). A mismatch is reported in its own status slot either way and outranks
-      // whatever the decoders made of the corrupt page.
-      const bool crc_concurrent = !pages->h_mapped && getenv("TSKV_CRC_CONCURRENT") != nullptr;
-      if (!crc_concurrent) {
-        uint32_t gblocks = std::max(1u, std::min<uint32_t>((uint32_t)ctx->sm_count * 4, (n_bin + 7) / 8));
-        k_verify_crc<<<gblocks, 256, 0, ctx->bin_stream[b]>>>(pages->d_arena, pages->d_descs, pages->d_time_page_of,
-                                                              s->d_work_page, s->d_work_qcol, s->d_bin_cstart, bin,
-                                                              pages->d_crc_tables, s->d_crc_status, s->d_crc_err_page);
-      } else {
-        if (!crc_forked) cudaStreamWaitEvent(ctx->crc_stream, ev_fork, 0);
-        crc_forked = true;
-        const char *bps_env = getenv("TSKV_CRC_BLOCKS_PER_SM");
-        const uint32_t bps = bps_env ? (uint32_t)std::max(1, atoi(bps_env)) : 1u;
-        uint32_t gblocks = std::max(1u, std::min<uint32_t>((uint32_t)ctx->sm_count * bps, (n_bin + 255) / 256));
-        k_verify_crc<<<gblocks, 256, 0, ctx->crc_stream>>>(pages->d_arena, pages->d_descs, pages->d_time_page_of,
-                                                           s->d_work_page, s->d_work_qcol, s->d_bin_cstart, bin,
-                                                           pages->d_crc_tables, s->d_crc_status, s->d_crc_err_page);
-      }
+      // (host-resident pages). Beside the fused kernels on a stream of its own the check was slower (H100, C4: 1.84-2.03
+      // ms per scan with 1-8 CRC blocks per SM against 1.39 ms in line): it needs the whole machine's lanes to hide its
+      // dependent table lookups. A mismatch is reported in its own status slot and outranks whatever the decoders made of
+      // the corrupt page.
+      uint32_t gblocks = std::max(1u, std::min<uint32_t>((uint32_t)ctx->sm_count * 4, (n_bin + 7) / 8));
+      k_verify_crc<<<gblocks, 256, 0, ctx->bin_stream[b]>>>(pages->d_arena, pages->d_descs, pages->d_time_page_of,
+                                                            s->d_work_page, s->d_work_qcol, s->d_bin_cstart, bin,
+                                                            pages->d_crc_tables, s->d_crc_status, s->d_crc_err_page);
       launches++;
     }
     if (!capturing) cudaEventRecord(s->ev_bin_start[b], ctx->bin_stream[b]);
@@ -2081,11 +2084,6 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     cudaEventRecord(ev_done, ctx->bin_stream[b]);
     cudaStreamWaitEvent(ctx->stream, ev_done, 0);  // join
     launches++;
-  }
-  if (crc_forked) {  // join the concurrent CRC checks
-    cudaEvent_t ev = capturing ? s->ev_ccrc : s->ev_crc;
-    cudaEventRecord(ev, ctx->crc_stream);
-    cudaStreamWaitEvent(ctx->stream, ev, 0);
   }
   if (!capturing) cudaEventRecord(s->ev_bin[N_BINS], ctx->stream);
   if (s->n_combine) {  // sliding windows: every window folds its panes (it writes every array the kernels fill)
@@ -2115,16 +2113,17 @@ static tskv_status sync_scan(tskv_ctx *ctx, tskv_scan *s) {
     if (st == TSKV_ERR_INVALID_ARG) ctx->set_error("page type does not match the query column type", ctx->err_page);
     return st;
   }
-  unsigned long long aux[5 + N_BINS] = {0};  // stats[2], pages, bytes, per-bin bytes[N_BINS], pruned pages
-  CU_TRY(ctx, cudaMemcpy(aux, s->d_stats, (5 + N_BINS) * 8, cudaMemcpyDeviceToHost));
-  ctx->counters.pruned_page_count = aux[4 + N_BINS];
+  unsigned long long aux[AUX_COUNTERS + N_COUNTERS - AUX_STATS] = {0};  // the stats, then the reader counters
+  CU_TRY(ctx, cudaMemcpy(aux, s->d_stats, sizeof(aux), cudaMemcpyDeviceToHost));
+  const unsigned long long *ctr = aux + (AUX_COUNTERS - AUX_STATS);
+  ctx->counters.pruned_page_count = ctr[CTR_PRUNED];
   float ms = 0;
   cudaEventElapsedTime(&ms, s->ev0, s->ev1);
   ctx->counters.elapsed_scan_ms = ms;
   ctx->counters.points_decoded = aux[0];
   ctx->counters.rows_in_range = aux[1];
-  ctx->counters.page_read_count = aux[2] + s->merge_read_pages;
-  ctx->counters.page_read_bytes = aux[3] + s->merge_page_bytes;
+  ctx->counters.page_read_count = ctr[CTR_PAGES] + s->merge_read_pages;
+  ctx->counters.page_read_bytes = ctr[CTR_BYTES] + s->merge_page_bytes;
   float fused = 0;
   cudaEventElapsedTime(&fused, s->ev_bin[0], s->ev_bin[N_BINS]);
   ctx->counters.elapsed_fused_ms = fused;
@@ -2146,11 +2145,11 @@ static tskv_status sync_scan(tskv_ctx *ctx, tskv_scan *s) {
       float t0 = 0;
       cudaEventElapsedTime(&t0, s->ev_bin[0], s->ev_bin_start[b]);
       fprintf(stderr, "[tskv] bin %d grid %d, %d CTAs/SM: start +%.3f ms, run %.3f ms, %llu bytes\n", b,
-              s->grid[b], s->occ[b], t0, t, aux[4 + b]);
+              s->grid[b], s->occ[b], t0, t, ctr[CTR_BIN_BYTES + b]);
     }
     if (t > ctx->counters.dominant_kernel_ms) {
       ctx->counters.dominant_kernel_ms = t;
-      ctx->counters.dominant_kernel_bytes = aux[4 + b];
+      ctx->counters.dominant_kernel_bytes = ctr[CTR_BIN_BYTES + b];
       ctx->counters.dominant_kernel_bin = (uint64_t)b;
     }
   }

@@ -1,6 +1,6 @@
 """TSKV_UPLOAD_VERIFY_ON_READ for pages resident in HBM: every scan re-checks the CRC32 of the pages it reads (the
-reference's Page::crc_validation on every read, tsm/reader.rs:259), in front of each bin's fused kernel or (opt-in)
-beside them on a stream of its own; a mismatch outranks whatever the decoders made of the corrupt page."""
+reference's Page::crc_validation on every read, tsm/reader.rs:259), in front of each bin's fused kernel; a mismatch
+outranks whatever the decoders made of the corrupt page."""
 import numpy as np
 import pytest
 
@@ -12,10 +12,7 @@ from tests.helpers import assert_results_equal, bucket_spec
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("concurrent", [False, True])
-def test_verify_on_read_in_hbm(engine, concurrent, monkeypatch):
-    if concurrent:
-        monkeypatch.setenv("TSKV_CRC_CONCURRENT", "1")  # the checks beside the fused kernels instead of in front of them
+def test_verify_on_read_in_hbm(engine):
     g = datagen.generate(3000, n_fields=2, n_points=600, value_kind=datagen.MIXED, seed=21, jitter_permille=300, jitter_max=999_999,
                          null_page_permille=100, null_row_permille=50)
     w = 60_000_000_000
@@ -27,7 +24,7 @@ def test_verify_on_read_in_hbm(engine, concurrent, monkeypatch):
     exp = orc.scan_aggregate(g.arena, g.descs, q, n_threads=8)
     pages = engine.upload_pages(g.arena, g.descs, verify_crc=True, verify_on_read=True)
     scan = engine.prepare(pages, q)
-    for _ in range(4):  # the second enqueue onwards replays the captured graph (CRC stream forked and joined inside it)
+    for _ in range(4):  # the second enqueue onwards replays the captured graph (CRC checks on the bin streams inside it)
         scan.enqueue()
         assert_results_equal(scan.finalize(), exp, what="verify on read, clean pages")
     scan.close()
