@@ -100,6 +100,13 @@ uint32_t plan_bin_parts(uint32_t maxrows, uint32_t skip_rows, uint32_t want, uin
   return (units + m - 1) / m;
 }
 
+uint32_t plan_walk_split(uint32_t max_groups, uint64_t n_walk, uint64_t n_items, uint32_t min_threads) {
+  uint32_t s = 1;
+  while (s < 1024 && ((uint64_t)max_groups + s - 1) / s > 32) s <<= 1;
+  while (s > 1 && n_walk * s > std::max<uint64_t>(n_items, min_threads)) s >>= 1;
+  return s;
+}
+
 void plan_overlap_groups(uint64_t n_cg, const uint32_t *cg_series, const uint32_t *cg_rows, const tskv_time_range *cg_bounds,
                          const uint64_t *cg_file, OverlapPlan *out) {
   *out = OverlapPlan{};

@@ -51,6 +51,10 @@ uint32_t plan_parts_wanted(double est_chunks, double resident_warps, double targ
 // Parts of a bin whose longest page has `maxrows` rows when `want` parts are wanted: parts are whole multiples of the
 // restart interval (`skip_rows` rows), at most one part per interval. Returns the parts; *part_rows = rows per part.
 uint32_t plan_bin_parts(uint32_t maxrows, uint32_t skip_rows, uint32_t want, uint32_t *part_rows);
+// Threads S per walked series of the work-list walk (a power of two): the smallest S that leaves each thread at most 32
+// of the `max_groups` column groups of the page set's largest series, at most 1024, then halved while the walk would
+// launch more threads than max(n_items, min_threads) (n_walk = the series walked: selected ids or every series).
+uint32_t plan_walk_split(uint32_t max_groups, uint64_t n_walk, uint64_t n_items, uint32_t min_threads);
 
 uint8_t classify_page(const PageHeader &h, uint8_t phys_type);
 

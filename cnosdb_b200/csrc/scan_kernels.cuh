@@ -1,7 +1,7 @@
 // scan_kernels.cuh — sm_90a kernels of the tskv scan path:
-//   k_select_cg / k_flag_items / k_scan_blocks / k_scatter_items : series selection -> compacted,
-//       kind-sorted work list (replaces get_series_id_by_filter's consumer side,
-//       tskv/src/reader/iterator.rs:915-929 + SeriesGroupBatchReaderFactory::create :123-264)
+//   k_worklist_count / k_worklist_offsets / k_worklist_emit : series selection -> compacted, kind-binned work list
+//       (replaces get_series_id_by_filter's consumer side, tskv/src/reader/iterator.rs:915-929 +
+//       SeriesGroupBatchReaderFactory::create :123-264); k_select_ids / k_select_cg: slot of every column group
 //   k_scan_aggregate<TK,VK> : fused decode -> closed time-range filter -> bucket id -> reduce
 //       (replaces ColumnGroupReader::read + decode_pages + DataFilter + the DataFusion
 //        projection/AggregateExec above the scan; SURVEY.md §3.1 hot loops A, B and C)
@@ -222,106 +222,27 @@ __device__ __forceinline__ int find_qcol(const ColState *cols, uint32_t n_cols, 
 constexpr uint32_t CTR_PAGES = 0, CTR_BYTES = 1, CTR_BIN_BYTES = 2, CTR_PRUNED = CTR_BIN_BYTES + N_BINS,
                    N_COUNTERS = CTR_PRUNED + 1;
 
-// One thread per item (field page, in kind-sorted order): selected? -> flag (query column + 1, bit 7 =
-// "this item also brings its column group's time page"), per-block counts and the byte/page counters
-// of the reference's reader metrics (column_group/mod.rs:141-193), split per decode-kind bin.
 // Statistics pruning (filter_column_groups, tskv/src/reader/chunk.rs:12-50 with the column group's time_range(),
-// tsm/column_group.rs:9-17): a group whose [min_ts, max_ts] overlaps none of the query's time ranges is dropped here,
-// so its pages are neither gathered nor decoded.
+// tsm/column_group.rs:9-17): a group whose [min_ts, max_ts] overlaps none of the query's time ranges is dropped by the
+// work-list walk, so its pages are neither gathered nor decoded.
 struct PruneRanges {
   tskv_time_range r[MAX_RANGES];
   uint32_t n;
   uint32_t pad;
 };
-// item_info[i] = {page, column group, page size, column id | phys type << 16 | decode kind << 24} (built at upload: one
-// coalesced 16-byte load per item instead of the item -> page -> descriptor chain).
-__global__ void k_flag_items(const tskv_page_desc *descs, const uint4 *item_info,
-                             const uint32_t *cg_time_page, uint32_t n_items,
-                             const int32_t *cg_slot, const ColState *cols, uint32_t n_cols,
-                             const uint32_t *bin_start, uint8_t *item_flag, uint32_t *block_count,
-                             unsigned long long *counters, int32_t *status, const tskv_time_range *cg_bounds,
-                             const PruneRanges prune, const uint8_t *cg_merge, const int64_t *page_stats,
-                             const PredicateSet preds, uint64_t n_descs, uint32_t n_cg) {
-  __shared__ uint32_t s_cnt;
-  __shared__ unsigned long long s_pages, s_bytes[N_BINS];
-  if (threadIdx.x == 0) { s_cnt = 0; s_pages = 0; }
-  if (threadIdx.x < N_BINS) s_bytes[threadIdx.x] = 0;
-  __syncthreads();
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  bool sel = false;
-  if (i < n_items) {
-    const uint4 info = __ldg(item_info + i);
-    const uint32_t p = info.x, cg = info.y;
-    struct { uint32_t size; uint16_t column_id; uint8_t phys_type, reserved; } d = {info.z, (uint16_t)(info.w & 0xffff), (uint8_t)((info.w >> 16) & 0xff), (uint8_t)(info.w >> 24)};
-    int qc = find_qcol(cols, n_cols, d.column_id);
-    bool first_sel = false;
-    bool in_time = true;
-    if (cg_bounds && prune.n) {  // TimeRange::overlaps against the group's statistics
-      const tskv_time_range b = cg_bounds[cg];
-      in_time = false;
-      for (uint32_t k = 0; k < prune.n; k++) in_time = in_time || (b.min_ts <= prune.r[k].max_ts && b.max_ts >= prune.r[k].min_ts);
-    }
-    if (in_time && page_stats && qc >= 0 && cg_slot[cg] >= 0) {  // value statistics against the pushed predicates
-      const uint32_t tp0 = cg_time_page[cg];
-      const uint64_t end = cg + 1 < n_cg ? (uint64_t)cg_time_page[cg + 1] : n_descs;
-      if (cg_ruled_out_by_stats(descs, tp0, end, preds, page_stats)) in_time = false;
-    }
-    if (!in_time && qc >= 0 && cg_slot[cg] >= 0 && !(cg_merge && cg_merge[cg])) atomicAdd(&counters[CTR_PRUNED], 1ull);
-    // (column groups of overlapping chunks go through the merge pass instead, merge_kernels.cuh)
-    if (qc >= 0 && cg_slot[cg] >= 0 && in_time && !(cg_merge && cg_merge[cg])) {
-      if (cols[qc].phys_type != d.phys_type) {
-        atomicCAS(status, 0, TSKV_ERR_INVALID_ARG);
-      } else {
-        sel = true;
-        unsigned long long bytes = d.size, pages = 1;
-        // The time page of a column group is brought along (PCIe gather, CRC check, byte counters) by the first selected
-        // field page of the group IN EACH DECODE-KIND BIN: the bins' gathers and fused kernels run on different streams,
-        // so a bin must not rely on another bin having copied the time page (a series with an i64 and an f64 field
-        // selected together lands in two bins). Field pages of a group are contiguous after the time page and share its
-        // time class, so "same bin" is "same value class".
-        // The reader metrics (page_read_count / page_read_bytes) count the time page once per column group.
-        uint32_t tp = cg_time_page[cg];
-        first_sel = true;
-        bool first_in_group = true;
-        const int vclass = value_class(d.reserved);
-        for (uint32_t q = tp + 1; q < p; q++)
-          if (find_qcol(cols, n_cols, descs[q].column_id) >= 0) {
-            first_in_group = false;
-            if (value_class(descs[q].reserved) == vclass) { first_sel = false; break; }
-          }
-        if (first_in_group) { bytes += descs[tp].size; pages += 1; }
-        int bin = 0;
-        for (int k = 1; k < N_BINS; k++) bin += (i >= bin_start[k]) ? 1 : 0;
-        atomicAdd(&s_bytes[bin], bytes);
-        atomicAdd(&s_pages, pages);
-      }
-    }
-    item_flag[i] = sel ? (uint8_t)((qc + 1) | (first_sel ? 0x80 : 0)) : 0;
-  }
-  uint32_t m = __ballot_sync(FULL, sel);
-  if ((threadIdx.x & 31) == 0 && m) atomicAdd(&s_cnt, __popc(m));
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    block_count[blockIdx.x] = s_cnt;
-    if (s_pages) atomicAdd(&counters[CTR_PAGES], s_pages);
-  }
-  if (threadIdx.x < N_BINS && s_bytes[threadIdx.x]) {
-    atomicAdd(&counters[CTR_BYTES], s_bytes[threadIdx.x]);
-    atomicAdd(&counters[CTR_BIN_BYTES + threadIdx.x], s_bytes[threadIdx.x]);
-  }
-}
 
 // ------------------------------------------------------------------------------------------------
-// Work list driven by the SELECTION (round 2): one thread per selected series walks that series' column groups and
-// their field pages, so the cost follows the selection (C4: 10 % of the series) instead of the page set. Two passes
-// over the same walk - count per (decode-kind bin, query column) bucket, then place - with a block-local histogram in
-// shared memory so that the global atomics are one per (block, bucket). Inside a bucket the order is arbitrary (the
-// fused kernels only need warps that are homogeneous in codec and, for GROUP BY bucket, in column). A (bin, column)
-// bucket is split in two by the page's narrow flag (WL_SUB buckets, ScanParams.page_narrow): its wide pages come first,
-// then its narrow ones, so that all chunks of the bucket but the one across the boundary are uniformly narrow or wide.
-// Same outputs as k_flag_items / k_scan_blocks / k_scatter_items: work_page / work_slot / work_qcol (bit 7 = "brings
-// the column group's time page": the first selected field page of each value class of a group), bin_cstart, the
-// reader counters, statistics pruning.
+// Work list driven by the SELECTION: 2^split_log2 threads per selected series walk that series' column groups (thread j
+// of a series takes groups j, j + S, j + 2S, ... of it) and their field pages, so the cost follows the selection (C4:
+// 10 % of the series) instead of the page set, and a series with thousands of groups is not walked by one thread.
+// Two passes over the same walk - count per (decode-kind bin, query column) bucket, then place - with a block-local
+// histogram in shared memory so that the global atomics are one per (block, bucket). Inside a bucket the order is
+// arbitrary (the fused kernels only need warps that are homogeneous in codec and, for GROUP BY bucket, in column). A
+// (bin, column) bucket is split in two by the page's narrow flag (WL_SUB buckets, ScanParams.page_narrow): its wide
+// pages come first, then its narrow ones, so that all chunks of the bucket but the one across the boundary are
+// uniformly narrow or wide. Outputs: work_page / work_slot / work_qcol (bit 7 = "brings the column group's time page":
+// the first selected field page of each value class of a group), bin_cstart, the reader counters (the reference's
+// reader metrics, column_group/mod.rs:141-193, split per decode-kind bin), statistics pruning.
 // ------------------------------------------------------------------------------------------------
 constexpr int WL_THREADS = 256;
 constexpr uint32_t WL_SUB = 2;  // work-list buckets per (bin, query column): wide pages, narrow pages
@@ -337,9 +258,10 @@ struct WorkListArgs {
   const uint32_t *set_series;    // the page set's distinct series ids, ascending
   uint32_t n_set_series;
   const uint32_t *series_ids;    // the selection (null: every series, slot = rank)
-  uint32_t n_sel;                // threads: selected ids, or n_set_series
-  // GROUP BY tags: thread i walks slot walk[i], the slots stably sorted by group, so that the items of a (bin, column)
-  // bucket come group by group and a warp's 32 pages mostly share a group (null: thread i walks slot i)
+  uint32_t n_sel;                // walk indices: selected ids, or n_set_series
+  uint32_t split_log2;           // log2 of the threads per walk index (plan_walk_split)
+  // GROUP BY tags: walk index i walks slot walk[i], the slots stably sorted by group, so that the items of a (bin,
+  // column) bucket come group by group and a warp's 32 pages mostly share a group (null: walk index i walks slot i)
   const uint32_t *walk;
   const ColState *cols;
   uint32_t n_cols;
@@ -361,9 +283,10 @@ __device__ __forceinline__ uint32_t worklist_key(const WorkListArgs &A, uint32_t
   return (bin * A.n_cols + qc) * WL_SUB + ((A.page_narrow && A.page_narrow[page]) ? 1u : 0u);
 }
 
-// Walks the items of selected series i; F(page, bin, qcol, with_time, desc).
+// Walks the items of column groups j, j + S, ... of selected series i (S = 2^split_log2); everything per column group
+// stays inside one thread. F(page, bin, qcol, with_time, desc, first_in_group, time page).
 template <typename F>
-__device__ __forceinline__ void worklist_walk(const WorkListArgs &A, uint32_t i, bool count_stats, F &&emit) {
+__device__ __forceinline__ void worklist_walk(const WorkListArgs &A, uint32_t i, uint32_t j, bool count_stats, F &&emit) {
   uint32_t rank = i;
   if (A.series_ids) {
     const uint32_t id = __ldg(A.series_ids + i);
@@ -376,7 +299,7 @@ __device__ __forceinline__ void worklist_walk(const WorkListArgs &A, uint32_t i,
     rank = lo;
   }
   const uint32_t c0 = __ldg(A.rank_cg_start + rank), c1 = __ldg(A.rank_cg_start + rank + 1);
-  for (uint32_t k = c0; k < c1; k++) {
+  for (uint32_t k = c0 + j; k < c1; k += 1u << A.split_log2) {
     const uint32_t cg = __ldg(A.rank_cg + k);
     if (A.cg_merge && A.cg_merge[cg]) continue;
     bool in_time = true;
@@ -388,6 +311,10 @@ __device__ __forceinline__ void worklist_walk(const WorkListArgs &A, uint32_t i,
     const uint32_t tp = __ldg(A.cg_time_page + cg);
     const uint64_t end = cg + 1 < A.n_cg ? (uint64_t)__ldg(A.cg_time_page + cg + 1) : A.n_descs;
     if (in_time && A.page_stats && cg_ruled_out_by_stats(A.descs, tp, end, A.preds, A.page_stats)) in_time = false;
+    // The time page of a column group is brought along (PCIe gather, CRC check) by the first selected field page of the
+    // group IN EACH DECODE-KIND BIN: the bins' gathers and fused kernels run on different streams, so a bin must not rely
+    // on another bin having copied it (an i64 and an f64 field of one series land in two bins). Field pages of a group
+    // share its time class, so "same bin" is "same value class".
     uint32_t seen_classes = 0;  // value classes that already brought the time page
     bool any = false;
     for (uint64_t p = (uint64_t)tp + 1; p < end; p++) {
@@ -420,9 +347,9 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_count(const WorkListArg
   if (threadIdx.x == 0) s_pages = 0;
   if (threadIdx.x < N_BINS) s_bytes[threadIdx.x] = 0;
   __syncthreads();
-  const uint32_t i = blockIdx.x * WL_THREADS + threadIdx.x;
+  const uint32_t t = blockIdx.x * WL_THREADS + threadIdx.x, i = t >> A.split_log2, j = t & ((1u << A.split_log2) - 1);
   if (i < A.n_sel)
-    worklist_walk(A, A.walk ? __ldg(A.walk + i) : i, true, [&](uint32_t page, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &d, bool first_in_group, uint32_t tp) {
+    worklist_walk(A, A.walk ? __ldg(A.walk + i) : i, j, true, [&](uint32_t page, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &d, bool first_in_group, uint32_t tp) {
       atomicAdd(&s_hist[worklist_key(A, page, bin, qc)], 1u);
       // the reader metrics (page_read_count / page_read_bytes) count the time page once per column group
       unsigned long long bytes = d.size, pages = 1;
@@ -492,10 +419,10 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_emit(const WorkListArgs
   uint32_t *s_base = s_hist, *s_cur = s_hist + n_buckets;
   for (uint32_t k = threadIdx.x; k < 2 * n_buckets; k += WL_THREADS) s_hist[k] = 0;
   __syncthreads();
-  const uint32_t i = blockIdx.x * WL_THREADS + threadIdx.x;
+  const uint32_t t = blockIdx.x * WL_THREADS + threadIdx.x, i = t >> A.split_log2, j = t & ((1u << A.split_log2) - 1);
   const uint32_t slot = (i < A.n_sel && A.walk) ? __ldg(A.walk + i) : i;
   if (i < A.n_sel)
-    worklist_walk(A, slot, false, [&](uint32_t page, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &, bool, uint32_t) {
+    worklist_walk(A, slot, j, false, [&](uint32_t page, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &, bool, uint32_t) {
       atomicAdd(&s_base[worklist_key(A, page, bin, qc)], 1u);
     });
   __syncthreads();
@@ -503,7 +430,7 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_emit(const WorkListArgs
     if (s_base[k]) s_base[k] = A.bucket_off[k] + atomicAdd(&A.bucket_count[k], s_base[k]);
   __syncthreads();
   if (i < A.n_sel)
-    worklist_walk(A, slot, false, [&](uint32_t page, uint32_t bin, uint32_t qc, bool with_time, const tskv_page_desc &, bool, uint32_t) {
+    worklist_walk(A, slot, j, false, [&](uint32_t page, uint32_t bin, uint32_t qc, bool with_time, const tskv_page_desc &, bool, uint32_t) {
       const uint32_t key = worklist_key(A, page, bin, qc);
       const uint32_t pos = s_base[key] + atomicAdd(&s_cur[key], 1u);
       A.work_page[pos] = page;
@@ -533,81 +460,6 @@ __global__ void k_gather_pages(const uint8_t *host_arena, uint8_t *dev_arena, co
       const uint32_t tail = d.size & 15;
       if (lane < tail) dev_arena[d.offset + (n16 << 4) + lane] = host_arena[d.offset + (n16 << 4) + lane];
     }
-  }
-}
-
-// Single-block exclusive scan of the per-block counts (n_blocks is small: n_items / 1024).
-__global__ void k_scan_blocks(uint32_t *block_count, uint32_t n_blocks, uint32_t *total) {
-  __shared__ uint32_t s_warp[32];
-  __shared__ uint32_t s_carry;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
-  for (uint32_t base = 0; base < n_blocks; base += blockDim.x) {
-    uint32_t i = base + threadIdx.x;
-    uint32_t v = i < n_blocks ? block_count[i] : 0;
-    uint32_t x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-      uint32_t y = __shfl_up_sync(FULL, x, o);
-      if ((threadIdx.x & 31) >= o) x += y;
-    }
-    if ((threadIdx.x & 31) == 31) s_warp[threadIdx.x >> 5] = x;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      uint32_t w = threadIdx.x < (blockDim.x >> 5) ? s_warp[threadIdx.x] : 0;
-      uint32_t xs = w;
-      for (int o = 1; o < 32; o <<= 1) {
-        uint32_t y = __shfl_up_sync(FULL, xs, o);
-        if (threadIdx.x >= o) xs += y;
-      }
-      s_warp[threadIdx.x] = xs - w;  // exclusive warp offsets
-    }
-    __syncthreads();
-    uint32_t excl = s_carry + s_warp[threadIdx.x >> 5] + x - v;
-    if (i < n_blocks) block_count[i] = excl;
-    __syncthreads();
-    if (threadIdx.x == blockDim.x - 1) s_carry = excl + v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total = s_carry;
-}
-
-// Ordered scatter: keeps the kind-sorted order, so the compacted list is still binned by kind;
-// bin_cstart[k] = compacted position of the first item of bin k.
-__global__ void k_scatter_items(const uint32_t *item_page, const uint32_t *item_cg, uint32_t n_items,
-                                const uint8_t *item_flag, const uint32_t *block_offset,
-                                const int32_t *cg_slot, const uint32_t *bin_start, uint32_t *work_page,
-                                uint32_t *work_slot, uint8_t *work_qcol, uint32_t *bin_cstart,
-                                const uint32_t *total) {
-  __shared__ uint32_t s_warp[32];
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  uint8_t f = i < n_items ? item_flag[i] : 0;
-  uint32_t m = __ballot_sync(FULL, f != 0);
-  uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) s_warp[wid] = __popc(m);
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    uint32_t w = threadIdx.x < (blockDim.x >> 5) ? s_warp[threadIdx.x] : 0;
-    uint32_t xs = w;
-    for (int o = 1; o < 32; o <<= 1) {
-      uint32_t y = __shfl_up_sync(FULL, xs, o);
-      if (threadIdx.x >= o) xs += y;
-    }
-    s_warp[threadIdx.x] = xs - w;
-  }
-  __syncthreads();
-  uint32_t pos = block_offset[blockIdx.x] + s_warp[wid] + __popc(m & ((1u << lane) - 1));
-  if (i < n_items) {
-    if (f) {
-      work_page[pos] = item_page[i];
-      work_slot[pos] = (uint32_t)cg_slot[item_cg[i]];
-      work_qcol[pos] = (uint8_t)(((f & 0x7f) - 1) | (f & 0x80));
-    }
-    for (int k = 0; k < N_BINS; k++)
-      if (bin_start[k] == i) bin_cstart[k] = pos;
-  }
-  if (i == 0) {
-    for (int k = 0; k <= N_BINS; k++)
-      if (bin_start[k] >= n_items) bin_cstart[k] = *total;
   }
 }
 

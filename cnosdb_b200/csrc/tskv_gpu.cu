@@ -67,17 +67,14 @@ struct tskv_pages {
   uint32_t *d_cg_time_page = nullptr;
   uint32_t *d_cg_series_rank = nullptr;
   uint32_t *d_series_sorted = nullptr;  // the page set's distinct series ids, ascending (rank -> id)
-  uint4 *d_item_info = nullptr;         // per item: page, column group, size, column id | type | kind
   uint32_t *d_rank_cg_start = nullptr, *d_rank_cg = nullptr;  // CSR: series rank -> its column groups (arena order)
+  uint32_t max_series_cg = 0;           // most column groups of one series (plan_walk_split)
   uint8_t *d_page_bin = nullptr;        // decode-kind bin of every field page
   mutable int64_t *d_page_stats = nullptr;  // {min key, max key} of every field page (k_page_stats), built on first use
-  uint32_t n_items = 0;
-  uint32_t *d_item_page = nullptr;
-  uint32_t *d_item_cg = nullptr;
-  uint32_t h_bin_start[N_BINS + 1]{};
+  uint32_t n_items = 0;              // field pages
+  uint32_t h_bin_pages[N_BINS]{};    // field pages per bin
   uint64_t h_bin_bytes[N_BINS]{};    // field-page bytes per bin (orders the PCIe gathers of host-resident scans)
   uint64_t h_bin_rows[N_BINS]{};     // rows of the bin's field pages (serial cost of its chunks)
-  uint32_t *d_bin_start = nullptr;
   // tombstones (tskvgpu_pages_set_tombstones); the epoch invalidates scans prepared before a change
   uint64_t *d_tomb_keys = nullptr;
   uint32_t *d_tomb_off = nullptr;
@@ -133,11 +130,8 @@ struct tskv_scan {
   uint32_t *d_series = nullptr;
   int32_t *d_rank_slot = nullptr;  // rank of a series in the page set -> position in the selection list (or -1)
   uint32_t *d_bucket = nullptr;    // selection-driven work list: [N_BINS * n_cols * WL_SUB] counts / cursors | [.. + 1] offsets
-  bool worklist_by_items = false;  // TSKV_WORKLIST=items: the round-1 pass over every field page of the page set
+  uint32_t walk_split_log2 = 0;    // log2 of the work-list walk's threads per series (plan_walk_split)
   int32_t *d_cg_slot = nullptr;
-  uint8_t *d_item_flag = nullptr;
-  uint32_t *d_block_count = nullptr;
-  uint32_t n_blocks = 0;
   uint32_t *d_work_page = nullptr, *d_work_slot = nullptr;
   uint8_t *d_work_qcol = nullptr;
   uint32_t *d_bin_cstart = nullptr;  // [N_BINS+1] then [1] total
@@ -477,7 +471,7 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
 void free_scan(tskv_scan *s) {
   if (!s) return;
   cudaStream_t st = s->ctx ? s->ctx->stream : nullptr;
-  void *bufs[] = {s->d_series, s->d_rank_slot, s->d_bucket, s->d_cg_slot, s->d_item_flag, s->d_block_count, s->d_work_page, s->d_work_slot,
+  void *bufs[] = {s->d_series, s->d_rank_slot, s->d_bucket, s->d_cg_slot, s->d_work_page, s->d_work_slot,
                   s->d_work_qcol, s->d_bin_cstart, s->d_cols, s->d_outs, s->d_means, s->d_state,
                   s->d_task_counter, s->d_values, s->d_validity, s->d_gathered, s->d_row_keep,
                   s->d_mcg_active, s->d_mvals, s->d_mvalid, s->d_mpage, s->d_mrow_off, s->d_mbm_off, s->d_pane_state, s->d_combine,
@@ -812,7 +806,7 @@ void plan_grids(const tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *
   // the parts changed nothing (H100, C4: 1.03-1.05 vs 1.02 ms per scan).
   if (pages->d_skip && !has_sel) {
     double est_chunks = 0;
-    for (int b = 0; b < N_BINS; b++) est_chunks += std::ceil((pages->h_bin_start[b + 1] - pages->h_bin_start[b]) * sel_frac / 32.0);
+    for (int b = 0; b < N_BINS; b++) est_chunks += std::ceil(pages->h_bin_pages[b] * sel_frac / 32.0);
     const double resident_warps = (double)ctx->sm_count * SCAN_MIN_BLOCKS * (SCAN_THREADS / 32);
     uint32_t want = plan_parts_wanted(est_chunks, resident_warps, 8.0);
     const char *parts_env = getenv("TSKV_PARTS");  // fixed number of parts (1 = never cut)
@@ -826,7 +820,7 @@ void plan_grids(const tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *
   double need_sum = 0, occ_weighted = 0;
   int need[N_BINS] = {0};
   for (int b = 0; b < N_BINS; b++) {
-    uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
+    uint32_t n_bin = pages->h_bin_pages[b];
     if (!n_bin) continue;
     const int sb = serial_bin_of(b);
     const void *fn = (const void *)(!has_sel ? scan_kernel_for<false>(sb, pages->h_bin_narrow[b]) : scan_kernel_for<true>(sb));
@@ -850,7 +844,7 @@ void plan_grids(const tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *
   // the grids that minimise the makespan (plan_serial_grids)
   double chunks[N_BINS], t_chunk[N_BINS];
   for (int b = 0; b < N_BINS; b++) {
-    const uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
+    const uint32_t n_bin = pages->h_bin_pages[b];
     chunks[b] = need[b] ? std::ceil((n_bin * sel_frac * 1.02 + 16) / 32.0) * parts[b] : 0;
     // (+ 12 rows' worth per chunk for opening its pages)
     t_chunk[b] = n_bin ? chunk_cost(b) * ((double)pages->h_bin_rows[b] / n_bin / parts[b] + 12.0) : 1.0;
@@ -925,7 +919,6 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
     cudaEventCreateWithFlags(&s->ev_gather[b], cudaEventDisableTiming);
   }
   s->n_series_sel = q->series_ids ? q->n_series : 0;
-  s->n_blocks = (n_items + 1023) / 1024;
   cudaError_t e = cudaSuccess;
   if (q->series_ids) {
     e = stream_alloc(ctx, &s->d_series, q->n_series);
@@ -959,15 +952,12 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
   if (e == cudaSuccess && q->series_ids) e = stream_alloc(ctx, &s->d_rank_slot, pages->series.size());
   if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_bucket, (size_t)2 * N_BINS * q->n_columns * WL_SUB + 1);
   {
-    // One thread walks ALL column groups of a selected series: right for many series with a few groups each (TSBS
-    // shapes), serial for a handful of series with thousands of groups (one host over a year) - those take the pass
-    // over every field page instead, which is parallel in the pages. TSKV_WORKLIST=items / series forces one.
-    const char *wl = getenv("TSKV_WORKLIST");
-    s->worklist_by_items = wl ? wl[0] == 'i' : (uint64_t)pages->n_cg > 32ull * std::max<uint64_t>(1, pages->series.size());
+    // A series with thousands of column groups (one host over a year) is walked by several threads
+    const uint64_t n_walk = q->series_ids ? q->n_series : pages->series.size();
+    const uint32_t split = plan_walk_split(pages->max_series_cg, n_walk, n_items, WL_THREADS);
+    while ((1u << s->walk_split_log2) < split) s->walk_split_log2++;
   }
   if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_cg_slot, pages->n_cg);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_item_flag, n_items);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_block_count, s->n_blocks);
   if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_page, n_items);
   if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_slot, n_items);
   if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_qcol, n_items);
@@ -1268,8 +1258,8 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
     return st;
   }
 
-  // ---- column groups, items (field pages) sorted by decode-kind bin ---------------------------
-  std::vector<uint32_t> time_page_of(n_descs, 0), cg_time_page, item_page, item_cg;
+  // ---- column groups ----------------------------------------------------------------------------
+  std::vector<uint32_t> time_page_of(n_descs, 0), cg_time_page;
   {
     uint64_t i = 0;
     while (i < n_descs) {
@@ -1278,7 +1268,6 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
         delete pg;
         return TSKV_ERR_INVALID_ARG;
       }
-      uint32_t cg = (uint32_t)cg_time_page.size();
       cg_time_page.push_back((uint32_t)i);
       time_page_of[i] = (uint32_t)i;
       uint64_t j = i + 1;
@@ -1289,15 +1278,13 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
           return TSKV_ERR_INVALID_ARG;
         }
         time_page_of[j] = (uint32_t)i;
-        item_page.push_back((uint32_t)j);
-        item_cg.push_back(cg);
         j++;
       }
       i = j;
     }
   }
   pg->n_cg = (uint32_t)cg_time_page.size();
-  pg->n_items = (uint32_t)item_page.size();
+  pg->n_items = (uint32_t)(n_descs - cg_time_page.size());
   pg->h_cg_time_page = cg_time_page;
   pg->h_time_has_nulls = time_has_nulls;
   std::vector<uint32_t> keep_off(n_descs, 0);
@@ -1318,41 +1305,22 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
   std::vector<uint32_t> cg_rank(pg->n_cg);
   for (uint32_t cg = 0; cg < pg->n_cg; cg++)
     cg_rank[cg] = (uint32_t)(std::lower_bound(pg->series.begin(), pg->series.end(), pg->h_descs[cg_time_page[cg]].series_id) - pg->series.begin());
+  // decode-kind bin of every field page, and the bins' page counts, bytes, rows and longest pages
   std::vector<uint8_t> page_bin(n_descs, 0);
-  // sort items by (bin, column id, arena order): warps are homogeneous in codec and, for GROUP BY
-  // bucket, lanes of a warp flush the same (column, bucket) cell in lock step.
-  {
-    std::vector<uint32_t> order(pg->n_items);
-    std::vector<uint64_t> key(pg->n_items);
-    for (uint32_t k = 0; k < pg->n_items; k++) {
-      const tskv_page_desc &vd = pg->h_descs[item_page[k]];
-      const tskv_page_desc &td = pg->h_descs[time_page_of[item_page[k]]];
-      int tclass = time_has_nulls[time_page_of[item_page[k]]] ? TK_GEN : time_class(td.reserved);
-      uint64_t bin = (uint64_t)tclass * N_VK + value_class(vd.reserved);
-      if (vd.num_values <= SHORT_PAGE_ROWS && vd.reserved == DK_S8B_ZZ && tclass != TK_GEN)
-        bin = tclass == TK_RLE ? BIN_SHORT_RLE_S8B : BIN_SHORT_S8B_S8B;
-      if (vd.num_values <= SHORT_PAGE_ROWS && vd.reserved == DK_GORILLA && tclass != TK_GEN)
-        bin = tclass == TK_RLE ? BIN_SHORT_RLE_GOR : BIN_SHORT_S8B_GOR;
-      key[k] = (bin << 48) | ((uint64_t)vd.column_id << 32) | k;
-      order[k] = k;
-      page_bin[item_page[k]] = (uint8_t)bin;
-    }
-    std::sort(key.begin(), key.end());
-    std::vector<uint32_t> ip(pg->n_items), ic(pg->n_items);
-    uint32_t counts[N_BINS] = {0};
-    for (uint32_t k = 0; k < pg->n_items; k++) {
-      uint32_t src = (uint32_t)(key[k] & 0xffffffffu);
-      ip[k] = item_page[src];
-      ic[k] = item_cg[src];
-      counts[key[k] >> 48]++;
-      pg->h_bin_bytes[key[k] >> 48] += pg->h_descs[item_page[src]].size;
-      pg->h_bin_rows[key[k] >> 48] += pg->h_descs[item_page[src]].num_values;
-      pg->h_bin_maxrows[key[k] >> 48] = std::max(pg->h_bin_maxrows[key[k] >> 48], pg->h_descs[item_page[src]].num_values);
-    }
-    item_page.swap(ip);
-    item_cg.swap(ic);
-    pg->h_bin_start[0] = 0;
-    for (int b = 0; b < N_BINS; b++) pg->h_bin_start[b + 1] = pg->h_bin_start[b] + counts[b];
+  for (uint64_t p = 0; p < n_descs; p++) {
+    const tskv_page_desc &vd = pg->h_descs[p];
+    if (vd.phys_type == TSKV_PT_TIME) continue;
+    const int tclass = time_has_nulls[time_page_of[p]] ? TK_GEN : time_class(pg->h_descs[time_page_of[p]].reserved);
+    int bin = tclass * N_VK + value_class(vd.reserved);
+    if (vd.num_values <= SHORT_PAGE_ROWS && vd.reserved == DK_S8B_ZZ && tclass != TK_GEN)
+      bin = tclass == TK_RLE ? BIN_SHORT_RLE_S8B : BIN_SHORT_S8B_S8B;
+    if (vd.num_values <= SHORT_PAGE_ROWS && vd.reserved == DK_GORILLA && tclass != TK_GEN)
+      bin = tclass == TK_RLE ? BIN_SHORT_RLE_GOR : BIN_SHORT_S8B_GOR;
+    page_bin[p] = (uint8_t)bin;
+    pg->h_bin_pages[bin]++;
+    pg->h_bin_bytes[bin] += vd.size;
+    pg->h_bin_rows[bin] += vd.num_values;
+    pg->h_bin_maxrows[bin] = std::max(pg->h_bin_maxrows[bin], vd.num_values);
   }
 
   // ---- device copies ----------------------------------------------------------------------------
@@ -1382,25 +1350,19 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
   if (e == cudaSuccess) e = up(&pg->d_cg_time_page, cg_time_page.data(), pg->n_cg);
   if (e == cudaSuccess) e = up(&pg->d_cg_series_rank, cg_rank.data(), pg->n_cg);
   if (e == cudaSuccess) e = up(&pg->d_series_sorted, pg->series.data(), pg->series.size());
-  std::vector<uint4> item_info(pg->n_items);
-  for (uint32_t k = 0; k < pg->n_items; k++) {
-    const tskv_page_desc &d = pg->h_descs[item_page[k]];
-    item_info[k] = make_uint4(item_page[k], item_cg[k], d.size, (uint32_t)d.column_id | ((uint32_t)d.phys_type << 16) | ((uint32_t)d.reserved << 24));
-  }
-  if (e == cudaSuccess) e = up(&pg->d_item_info, item_info.data(), pg->n_items);
   {  // series rank -> its column groups (the selection-driven work list walks a selected series' groups)
     std::vector<uint32_t> start(pg->series.size() + 1, 0), list(pg->n_cg);
     for (uint32_t cg = 0; cg < pg->n_cg; cg++) start[cg_rank[cg] + 1]++;
-    for (size_t r = 0; r < pg->series.size(); r++) start[r + 1] += start[r];
+    for (size_t r = 0; r < pg->series.size(); r++) {
+      pg->max_series_cg = std::max(pg->max_series_cg, start[r + 1]);
+      start[r + 1] += start[r];
+    }
     std::vector<uint32_t> cur(start.begin(), start.end() - 1);
     for (uint32_t cg = 0; cg < pg->n_cg; cg++) list[cur[cg_rank[cg]]++] = cg;
     if (e == cudaSuccess) e = up(&pg->d_rank_cg_start, start.data(), start.size());
     if (e == cudaSuccess) e = up(&pg->d_rank_cg, list.data(), list.size());
     if (e == cudaSuccess) e = up(&pg->d_page_bin, page_bin.data(), n_descs);
   }
-  if (e == cudaSuccess) e = up(&pg->d_item_page, item_page.data(), pg->n_items);
-  if (e == cudaSuccess) e = up(&pg->d_item_cg, item_cg.data(), pg->n_items);
-  if (e == cudaSuccess) e = up(&pg->d_bin_start, pg->h_bin_start, N_BINS + 1);
   if (e == cudaSuccess) e = up(&pg->d_keep_off, keep_off.data(), n_descs);
   if (e == cudaSuccess && (((flags & TSKV_UPLOAD_VERIFY_CRC) && (flags & TSKV_UPLOAD_HOST_RESIDENT)) || (flags & TSKV_UPLOAD_VERIFY_ON_READ))) {
     pg->verify_on_read = true;  // like the reference: every read of a page re-checks its CRC (device side)
@@ -1464,13 +1426,11 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
       std::vector<uint8_t> narrow(n_descs);
       e = cudaMemcpyAsync(narrow.data(), pg->d_narrow, n_descs, cudaMemcpyDeviceToHost, ctx->stream);
       if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-      uint64_t n_narrow[N_BINS] = {0}, n_pages[N_BINS] = {0};
-      for (uint32_t k = 0; k < pg->n_items; k++) {
-        n_narrow[page_bin[item_page[k]]] += narrow[item_page[k]];
-        n_pages[page_bin[item_page[k]]]++;
-      }
+      uint64_t n_narrow[N_BINS] = {0};
+      for (uint64_t p = 0; p < n_descs; p++)
+        if (pg->h_descs[p].phys_type != TSKV_PT_TIME) n_narrow[page_bin[p]] += narrow[p];
       for (int b = 0; b < N_BINS; b++)
-        pg->h_bin_narrow[b] = n_narrow[b] == 0 ? NARROW_NONE : n_narrow[b] == n_pages[b] ? NARROW_ALL : NARROW_SOME;
+        pg->h_bin_narrow[b] = n_narrow[b] == 0 ? NARROW_NONE : n_narrow[b] == pg->h_bin_pages[b] ? NARROW_ALL : NARROW_SOME;
     }
   }
   cudaEventRecord(ctx->ev1, ctx->stream);
@@ -1503,14 +1463,10 @@ void tskvgpu_pages_destroy(tskv_ctx *ctx, tskv_pages *pg) {
   cudaFree(pg->d_cg_time_page);
   cudaFree(pg->d_cg_series_rank);
   cudaFree(pg->d_series_sorted);
-  cudaFree(pg->d_item_info);
   cudaFree(pg->d_rank_cg_start);
   cudaFree(pg->d_rank_cg);
   cudaFree(pg->d_page_bin);
   cudaFree(pg->d_page_stats);
-  cudaFree(pg->d_item_page);
-  cudaFree(pg->d_item_cg);
-  cudaFree(pg->d_bin_start);
   cudaFree(pg->d_crc_tables);
   cudaFree(pg->d_tomb_keys);
   cudaFree(pg->d_tomb_off);
@@ -1952,9 +1908,9 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
                                                                    s->d_bucket, N_BINS * s->n_cols * WL_SUB);
     launches++;
   }
-  // slot of every column group: the row filter, the merge pass and the item-driven work list need it per GROUP; the
-  // selection-driven work list finds a selected series' groups itself
-  const bool need_cg_slot = s->worklist_by_items || s->preds.n || (s->merge.n_rows && s->n_merge_pages);
+  // slot of every column group: the row filter and the merge pass need it per GROUP; the work list finds a selected
+  // series' groups itself
+  const bool need_cg_slot = s->preds.n || (s->merge.n_rows && s->n_merge_pages);
   if (pages->n_cg && need_cg_slot) {
     if (s->d_rank_slot) {
       CU_TRY(ctx, cudaMemsetAsync(s->d_rank_slot, 0xff, pages->series.size() * 4, ctx->stream));
@@ -1973,20 +1929,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
                                                                      s->preds, pages->d_keep_off, s->d_row_keep, s->d_status, s->d_err_page);
     launches++;
   }
-  if (n_items && s->worklist_by_items) {
-    k_flag_items<<<s->n_blocks, 1024, 0, ctx->stream>>>(pages->d_descs, pages->d_item_info,
-                                                        pages->d_cg_time_page, n_items, s->d_cg_slot, s->d_cols,
-                                                        s->n_cols, pages->d_bin_start, s->d_item_flag,
-                                                        s->d_block_count, s->d_counters, s->d_status,
-                                                        s->prune.n ? pages->d_cg_bounds : nullptr, s->prune, pages->d_cg_merge,
-                                                        s->preds.n ? pages->d_page_stats : nullptr, s->preds, pages->n_descs, pages->n_cg);
-    k_scan_blocks<<<1, 1024, 0, ctx->stream>>>(s->d_block_count, s->n_blocks, s->d_bin_cstart + N_BINS + 1);
-    k_scatter_items<<<s->n_blocks, 1024, 0, ctx->stream>>>(pages->d_item_page, pages->d_item_cg, n_items, s->d_item_flag,
-                                                           s->d_block_count, s->d_cg_slot, pages->d_bin_start,
-                                                           s->d_work_page, s->d_work_slot, s->d_work_qcol,
-                                                           s->d_bin_cstart, s->d_bin_cstart + N_BINS + 1);
-    launches += 3;
-  } else if (n_items) {
+  if (n_items) {
     WorkListArgs A{};
     A.descs = pages->d_descs;
     A.n_descs = pages->n_descs;
@@ -2002,6 +1945,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     A.n_set_series = (uint32_t)pages->series.size();
     A.series_ids = s->d_series;
     A.n_sel = s->d_series ? s->n_series_sel : (uint32_t)pages->series.size();
+    A.split_log2 = s->walk_split_log2;
     A.walk = s->d_walk;
     A.cols = s->d_cols;
     A.n_cols = s->n_cols;
@@ -2018,7 +1962,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     A.work_qcol = s->d_work_qcol;
     A.counters = s->d_counters;
     A.status = s->d_status;
-    const uint32_t wblocks = std::max(1u, (A.n_sel + WL_THREADS - 1) / WL_THREADS);
+    const uint32_t wblocks = std::max(1u, (uint32_t)((((uint64_t)A.n_sel << A.split_log2) + WL_THREADS - 1) / WL_THREADS));
     if (A.n_sel) k_worklist_count<<<wblocks, WL_THREADS, n_buckets * 4, ctx->stream>>>(A);
     k_worklist_offsets<<<1, 256, 0, ctx->stream>>>(s->d_bucket, s->d_bucket + n_buckets, s->n_cols * WL_SUB, s->d_bin_cstart);
     if (A.n_sel) k_worklist_emit<<<wblocks, WL_THREADS, 2 * n_buckets * 4, ctx->stream>>>(A);
@@ -2051,7 +1995,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     if (!s->grid[b]) continue;
     cudaStreamWaitEvent(ctx->bin_stream[b], ev_fork, 0);
     int bin = b;
-    const uint32_t n_bin = pages->h_bin_start[b + 1] - pages->h_bin_start[b];
+    const uint32_t n_bin = pages->h_bin_pages[b];
     if (pages->h_mapped) {
       if (prev_gather >= 0) cudaStreamWaitEvent(ctx->bin_stream[b], s->ev_gather[prev_gather], 0);
       uint32_t gblocks = std::max(1u, std::min<uint32_t>((uint32_t)ctx->sm_count * 4, (n_bin + 7) / 8));

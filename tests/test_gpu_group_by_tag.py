@@ -16,6 +16,7 @@ from tests.helpers import (ALL_AGGS, GEOM_AGGS, GEOM_FIELDS, GEOMETRY_CASES, Ref
 from tests.group_reference import exact_aggregate_grouped
 from tests.test_gpu_bool import bool_arena
 from tests.test_gpu_overlap_merge import overlapping_arena
+from tests.test_gpu_page_parts import many_groups_arena
 from tests.test_gpu_parity import random_tombstones
 
 pytestmark = pytest.mark.gpu
@@ -178,8 +179,9 @@ def test_exact_reference_geometry(engine, case, monkeypatch):
 
 
 def test_other_paths(engine, monkeypatch):
-    """Overlapping chunks (the merge pass), a host-resident page set, the item-driven work list and a table too large for
-    shared memory: each grouped scan against the subset scans of the same configuration."""
+    """Overlapping chunks (the merge pass), a host-resident page set, a table too large for shared memory and series of
+    100 column groups each (the work-list walk splits a series over 4 threads and walks the slots in group order): each
+    grouped scan against the subset scans of the same configuration."""
     rng = np.random.default_rng(23)
     fbs, nb = bucket_spec(1_000_000, 1_000_000 + 3_000_000, 60_000)
     arena, descs, files = overlapping_arena(rng, n_series=50)
@@ -201,14 +203,27 @@ def test_other_paths(engine, monkeypatch):
         q = make_query(FIELDS, aggs, width=20_000, first_bucket_start=fbs, n_buckets=nb)
         gmap = make_map(rng, 80, 7)
         assert_groups_match_subsets(engine, hp, q, gmap, 7, all_ids, "host-resident %s" % (aggs,))
-        for env, val in (("TSKV_WORKLIST", "items"), ("TSKV_SMEM_TABLE_KB", "0")):
-            with monkeypatch.context() as m:
-                m.setenv(env, val)
-                for parts in ENVS:
-                    _set_env(m, parts)
-                    assert_groups_match_subsets(engine, dp, q, gmap, 7, all_ids, "%s=%s %s parts=%s" % (env, val, aggs, parts))
+        with monkeypatch.context() as m:
+            m.setenv("TSKV_SMEM_TABLE_KB", "0")
+            for parts in ENVS:
+                _set_env(m, parts)
+                assert_groups_match_subsets(engine, dp, q, gmap, 7, all_ids, "TSKV_SMEM_TABLE_KB=0 %s parts=%s" % (aggs, parts))
     hp.close()
     dp.close()
+
+    arena, descs, _, _ = many_groups_arena(rng, {sid: 100 for sid in range(12)}, 60, fields=FIELDS)
+    pages = engine.upload_pages(arena, descs)
+    all_ids = np.arange(12, dtype=np.uint32)
+    fbs, nb = bucket_spec(1_000_000, 1_000_000 + 100 * 60 * 1000, 200_000)
+    for aggs in (AGGS, ALL_AGGS):
+        q = make_query(FIELDS, aggs, width=200_000, first_bucket_start=fbs, n_buckets=nb, predicates=[(1, cabi.TSKV_PT_I64, ">", -30)])
+        for n_groups in (2, 5):
+            gmap = make_map(rng, 12, n_groups)
+            for parts in ENVS:
+                _set_env(monkeypatch, parts)
+                assert_groups_match_subsets(engine, pages, q, gmap, n_groups, all_ids,
+                                            "many groups G=%d %s parts=%s" % (n_groups, aggs, parts))
+    pages.close()
 
 
 def test_sliding_windows(engine, monkeypatch):

@@ -85,9 +85,10 @@ def timestamps(rng, sid, m):
 NARROW_I64, NARROW_U64 = (0, 1, 2, 5, 6), (0, 1)
 
 
-def build(seed, narrow_only=False):
+def build(seed, narrow_only=False, cuts=1):
     """narrow_only: every page narrow (the bins run the kernels that hold the 32-bit arithmetic only); otherwise narrow
-    and wide pages share the bins (kernels that choose per chunk)."""
+    and wide pages share the bins (kernels that choose per chunk). cuts: column groups per series (its rows cut into
+    consecutive runs)."""
     rng = np.random.default_rng(seed)
     b = datagen.ArenaBuilder()
     truth = {}
@@ -97,9 +98,11 @@ def build(seed, narrow_only=False):
         ik, uk = (NARROW_I64[sid % 5], NARROW_U64[sid % 2]) if narrow_only else (sid, sid)
         iv, uv = i64_values(rng, ik, m), u64_values(rng, uk, m)
         valid = rng.random(m) >= 0.3 if sid % 13 == 6 else np.ones(m, dtype=bool)
-        vv = None if valid.all() else valid
-        b.add_column_group(sid, ts, [(1, cabi.TSKV_PT_I64, iv, vv), (3, cabi.TSKV_PT_U64, uv, vv)])
-        truth[sid] = [(ts, {1: (iv, valid), 3: (uv, valid)})]
+        truth[sid] = []
+        for r in np.array_split(np.arange(m), cuts):
+            vv = None if valid[r].all() else valid[r]
+            b.add_column_group(sid, ts[r], [(1, cabi.TSKV_PT_I64, iv[r], vv), (3, cabi.TSKV_PT_U64, uv[r], vv)])
+            truth[sid].append((ts[r], {1: (iv[r], valid[r]), 3: (uv[r], valid[r])}))
     arena, descs = b.finish()
     return arena, descs, truth
 
@@ -107,6 +110,11 @@ def build(seed, narrow_only=False):
 @pytest.fixture(scope="module")
 def narrow_set():
     return build(11)
+
+
+@pytest.fixture(scope="module")
+def narrow_cut_set():
+    return build(11, cuts=3)
 
 
 @pytest.fixture(scope="module")
@@ -148,14 +156,53 @@ def assert_oracle_equal(got, ora, what):
         assert bad.size == 0, "%s col %s %s differs from the oracle at %s" % (what, col, agg, bad[:5])
 
 
-@pytest.mark.parametrize("env", ["parts1", "parts3", "items"])
-def test_narrow_pages_are_exact(engine, narrow_set, env, monkeypatch):
-    """parts1 / parts3: pages whole or cut in three at restart points; items: the item-driven work list, which does not
-    sort narrow pages apart, so most chunks mix narrow and wide pages."""
-    arena, descs, truth = narrow_set
+def mixed_chunks(arena, descs, truth):
+    """Where a scan of every page puts narrow and wide pages into one 32-page chunk, restated from the arrays. Every
+    simple8b value page here has at most 1024 rows, so its bin is the short-page bin of its time page's codec (run-length
+    or simple8b). The work list holds a bin's pages column by column (the query's column order), each column's wide
+    pages before its narrow ones, and cuts the bin into chunks of 32 from its start: a chunk mixes the two kinds where
+    a wide / narrow boundary falls off a multiple of 32. Returns [(time codec, boundary)]."""
+    def int_kind(d):  # integer encoding of the page's data (page.rs framing): 1 = simple8b, 2 = run-length
+        off = int(d["offset"])
+        return int(arena[off + 16 + int.from_bytes(arena[off:off + 4].tobytes(), "big") + 1]) >> 4
+
+    groups = [(ts, cols) for cgs in truth.values() for ts, cols in cgs]
+    tps = np.nonzero(descs["phys_type"] == cabi.TSKV_PT_TIME)[0]
+    assert len(tps) == len(groups)
+    count = {}  # (time codec, column, narrow) -> pages
+    for k, (ts, cols) in enumerate(groups):
+        tk = int_kind(descs[tps[k]])
+        for p in range(tps[k] + 1, tps[k + 1] if k + 1 < len(tps) else len(descs)):
+            d = descs[p]
+            if int_kind(d) != 1:
+                continue  # a run-length value page: a bin of its own, never narrow
+            assert int(d["num_values"]) <= 1024
+            v, valid = cols[int(d["column_id"])]
+            v = v[valid]
+            narrow = bool((v <= I32_MAX).all() and (v >= (I32_MIN if v.dtype == np.int64 else 0)).all())
+            key = (tk, int(d["column_id"]), narrow)
+            count[key] = count.get(key, 0) + 1
+    out = []
+    for tk in (1, 2):
+        pos, last = 0, None
+        for col, _ in FIELDS:
+            for narrow in (False, True):
+                n = count.get((tk, col, narrow), 0)
+                if n and last is not None and last != narrow and pos % 32:
+                    out.append((tk, pos))
+                if n:
+                    pos, last = pos + n, narrow
+    return out
+
+
+@pytest.mark.parametrize("env", ["parts1", "parts3", "cut"])
+def test_narrow_pages_are_exact(engine, narrow_set, narrow_cut_set, env, monkeypatch):
+    """parts1 / parts3: pages whole or cut in three at restart points; cut: every series cut into three column groups,
+    which puts wide / narrow boundaries inside 32-page chunks (mixed_chunks), so those chunks take the per-chunk choice."""
+    arena, descs, truth = narrow_cut_set if env == "cut" else narrow_set
     monkeypatch.setenv("TSKV_PARTS", "3" if env == "parts3" else "1")
-    if env == "items":
-        monkeypatch.setenv("TSKV_WORKLIST", "items")
+    if env == "cut":
+        assert mixed_chunks(arena, descs, truth)
     pages = engine.upload_pages(arena, descs)
     for name, q in queries():
         got = engine.scan_aggregate(pages, q)

@@ -178,54 +178,165 @@ def test_cut_and_whole_scans_agree_bit_for_bit_on_integers(engine, monkeypatch):
     pages.close()
 
 
-def test_item_driven_work_list_still_agrees(engine, monkeypatch):
-    """TSKV_WORKLIST=items: the round-1 work list (every field page of the page set flagged, ordered compaction) must
-    give what the selection-driven one gives - with a selection list, without one, with pruning and a row filter."""
-    g = datagen.generate(4000, n_fields=2, n_points=700, value_kind=datagen.MIXED, seed=77, jitter_permille=300, jitter_max=999_999,
-                         null_page_permille=100, null_row_permille=80)
-    pages = engine.upload_pages(g.arena, g.descs)
-    w = 60_000_000_000
-    fbs, nb = bucket_spec(datagen.TSBS_T0 - 1_000_000, datagen.TSBS_T0 + 999 * datagen.TSBS_STEP + 1_000_000, w)
-    cols = [PushedAggregate(1, cabi.TSKV_PT_I64, AGGS + ("first", "last")), PushedAggregate(3, cabi.TSKV_PT_F64, AGGS)]
-    t0, st = datagen.TSBS_T0, datagen.TSBS_STEP
-    for sel in (np.arange(0, 4000, 7, dtype=np.uint32), None):
-        for kw in (dict(), dict(time_ranges=[(t0 + 100 * st, t0 + 300 * st)]), dict(predicates=[(1, cabi.TSKV_PT_I64, ">", 10)])):
-            q = QueryOption(cols, series_ids=sel, width=w, first_bucket_start=fbs, n_buckets=nb, **kw)
-            exp = orc.scan_aggregate(g.arena, g.descs, q, n_threads=8)
-            for mode in ("items", "series"):
-                monkeypatch.setenv("TSKV_WORKLIST", mode)
-                got = engine.scan_aggregate(pages, q)
-                assert_results_equal(got, exp, what="work list %s sel=%s %s" % (mode, sel is not None, kw))
-                c = engine.counters()
-                if mode == "items":
-                    ref_counts = (c["page_read_count"], c["page_read_bytes"], c["pruned_page_count"])
+def expected_reads(descs, truth, qcols, sel=None, ranges=(), preds=()):
+    """(page_read_count, page_read_bytes, pruned_page_count) restated from the generated arrays. Per column group of a
+    selected series: its pages of the query columns `qcols` are pruned when its [min_ts, max_ts] meets none of the time
+    ranges, or when one predicate's page in the group has no non-null value that satisfies the comparison (predicates
+    with <, <=, > or >=, whose truth on [min, max] is decided at an end); otherwise they are read, with the group's time
+    page once. truth lists the column groups in descriptor order (ArenaBuilder order)."""
+    ops = {"<": np.less, "<=": np.less_equal, ">": np.greater, ">=": np.greater_equal}
+    groups = [(sid, ts, cols) for sid, cgs in truth.items() for ts, cols in cgs]
+    tps = np.nonzero(descs["phys_type"] == cabi.TSKV_PT_TIME)[0]
+    assert len(tps) == len(groups)
+    sel = None if sel is None else set(int(x) for x in sel)
+    pages = nbytes = pruned = 0
+    for k, (sid, ts, cols) in enumerate(groups):
+        tp = int(tps[k])
+        end = int(tps[k + 1]) if k + 1 < len(tps) else len(descs)
+        assert int(descs[tp]["series_id"]) == sid and int(descs[tp]["num_values"]) == len(ts)
+        if sel is not None and sid not in sel:
+            continue
+        q = [p for p in range(tp + 1, end) if int(descs[p]["column_id"]) in qcols]
+        if not q:
+            continue
+        keep = not ranges or any(ts.min() <= hi and ts.max() >= lo for lo, hi in ranges)
+        for col, pt, op, c in preds:
+            if keep and col in cols:
+                v, valid = cols[col]
+                v = v[valid]
+                keep = v.size > 0 and bool(ops[op](v.min(), c) or ops[op](v.max(), c))
+        if keep:
+            pages += len(q) + 1
+            nbytes += sum(int(descs[p]["size"]) for p in q) + int(descs[tp]["size"])
+        else:
+            pruned += len(q)
+    return pages, nbytes, pruned
+
+
+def many_groups_arena(rng, groups, max_rows, fields=FIELDS, overlap_every=0, t0=1_000_000):
+    """groups: {series id: column groups}. A series' groups follow each other in time, 1..max_rows rows each; with
+    overlap_every = k, every k-th group starts inside the one before it. Returns (arena, descs, truth, file id of every
+    column group: one chunk per group)."""
+    b = datagen.ArenaBuilder()
+    truth, files = {}, []
+    for sid, n_cg in groups.items():
+        t = t0
+        for g in range(n_cg):
+            n = int(rng.integers(1, max_rows + 1))
+            if overlap_every and g % overlap_every == overlap_every - 1:
+                t -= 500 * int(rng.integers(1, 40))
+            ts = t + np.arange(n, dtype=np.int64) * 1000
+            t = int(ts[-1]) + 1000
+            fl, cols = [], {}
+            for col, pt in fields:
+                valid = rng.random(n) > 0.1
+                if pt == cabi.TSKV_PT_F64:
+                    v = np.cumsum(rng.integers(-3, 4, n)) + rng.random(n)
+                elif pt == cabi.TSKV_PT_U64:
+                    v = np.cumsum(rng.integers(0, 5, n)).astype(np.uint64)
                 else:
-                    assert (c["page_read_count"], c["page_read_bytes"], c["pruned_page_count"]) == ref_counts
-    pages.close()
+                    v = np.cumsum(rng.integers(-9, 10, n)).astype(np.int64)
+                fl.append((col, pt, v, valid))
+                cols[col] = (v, valid)
+            b.add_column_group(sid, ts, fl)
+            truth.setdefault(sid, []).append((ts, cols))
+            files.append(len(files) + 1)
+    arena, descs = b.finish()
+    return arena, descs, truth, files
+
+
+def check_reads(engine, pages, arena, descs, truth, sel, kw, what, value_stats=True):
+    """value_stats=False: a host-resident page set without caller-supplied statistics (no value-statistics pruning)."""
+    q = make_query(FIELDS[:2], aggs=AGGS + ("first", "last"), series_ids=sel, **kw)
+    assert_results_equal(engine.scan_aggregate(pages, q), orc.scan_aggregate(arena, descs, q, n_threads=8), what=what)
+    c = engine.counters()
+    got = (c["page_read_count"], c["page_read_bytes"], c["pruned_page_count"])
+    exp = expected_reads(descs, truth, (1, 2), sel, kw.get("time_ranges", ()), kw.get("predicates", ()) if value_stats else ())
+    assert got == exp, "%s: read / bytes / pruned %s, expected %s" % (what, got, exp)
+
+
+def test_work_list_reads_exactly_the_selected_pages(engine):
+    """The work list against the oracle and against reader counters restated from the arrays, with a selection list,
+    without one, with time pruning and with value-statistics pruning plus the row filter, on two shapes: 2000 series of
+    one column group each (one walk thread per series) and 6 series x 150 groups (8 walk threads per series). Column 3
+    is never queried, so the counters must leave its pages out."""
+    rng = np.random.default_rng(77)
+    t0 = 1_000_000
+    shapes = (("one group per series", {sid: 1 for sid in range(2000)}, 300, np.arange(0, 2000, 7, dtype=np.uint32)),
+              ("many groups", {sid: 150 for sid in (2, 3, 5, 8, 13, 21)}, 80, np.array([3, 8, 21], dtype=np.uint32)))
+    for shape, groups, max_rows, sel in shapes:
+        arena, descs, truth, _ = many_groups_arena(rng, groups, max_rows)
+        t_end = max(int(ts.max()) for cgs in truth.values() for ts, _ in cgs)
+        w = (t_end - t0) // 40 + 1
+        fbs, nb = bucket_spec(t0, t_end, w)
+        pages = engine.upload_pages(arena, descs)
+        for s in (sel, None):
+            for kw in (dict(), dict(time_ranges=[(t0 + 40_000, t0 + 250_000), (t0 + 2_000_000, t0 + 3_000_000)]),
+                       dict(predicates=[(1, cabi.TSKV_PT_I64, ">", 10)])):
+                check_reads(engine, pages, arena, descs, truth, s, dict(width=w, first_bucket_start=fbs, n_buckets=nb,
+                                                                       group_by_series=True, **kw),
+                            "%s sel=%s %s" % (shape, s is not None, kw))
+        pages.close()
 
 
 def test_few_series_with_many_column_groups(engine):
-    """3 series x 90 column groups: the work list is built by the pass over the field pages (a thread per selected series
-    would walk 90 groups serially); same results as the oracle either way."""
+    """3 series x 90 column groups: the work-list walk splits each series over 4 threads (at most 32 groups per
+    thread). Results as the oracle's and reader counters as restated from the arrays, with time ranges, predicates
+    (value-statistics pruning and the row filter), tombstones, FIRST / LAST, a host-resident page set and overlapping
+    chunk files (every 7th group overlaps the one before it: merge groups between groups the walk reads)."""
     rng = np.random.default_rng(8)
-    b = datagen.ArenaBuilder()
-    for sid in (4, 9, 11):
-        t = 1_000_000
-        for _ in range(90):
-            n = int(rng.integers(1, 400))
-            ts = t + np.arange(n, dtype=np.int64) * 1000
-            t = int(ts[-1]) + 1000
-            b.add_column_group(sid, ts, [(1, cabi.TSKV_PT_I64, np.cumsum(rng.integers(-9, 10, n)), rng.random(n) > 0.1),
-                                         (2, cabi.TSKV_PT_F64, np.cumsum(rng.integers(-3, 4, n)) + rng.random(n), None)])
-    arena, descs = b.finish()
+    arena, descs, truth, files = many_groups_arena(rng, {4: 90, 9: 90, 11: 90}, 400)
     pages = engine.upload_pages(arena, descs)
-    fbs, nb = bucket_spec(1_000_000, 1_000_000 + 90 * 400 * 1000, 500_000)
+    host = engine.upload_pages(arena, descs, host_resident=True)
+    t0 = 1_000_000
+    fbs, nb = bucket_spec(t0, t0 + 90 * 400 * 1000, 500_000)
+    grid = dict(width=500_000, first_bucket_start=fbs, n_buckets=nb, group_by_series=True)
+    preds = [(1, cabi.TSKV_PT_I64, ">", -20), (2, cabi.TSKV_PT_F64, "<=", 9.5)]
     for sel in (None, np.array([4, 11], dtype=np.uint32)):
-        for ranges in ([], [(1_000_000 + 3_000_000, 1_000_000 + 9_000_000)]):
-            q = make_query(FIELDS[:2], aggs=AGGS + ("first", "last"), series_ids=sel, time_ranges=ranges, width=500_000, first_bucket_start=fbs,
-                           n_buckets=nb, group_by_series=True)
-            got = engine.scan_aggregate(pages, q)
-            exp, pts = orc.scan_aggregate(arena, descs, q, return_points=True)
-            assert_results_equal(got, exp, what="many groups sel=%s %s" % (sel is not None, ranges))
+        for kw in (dict(), dict(time_ranges=[(t0 + 3_000_000, t0 + 9_000_000)]), dict(predicates=preds),
+                   dict(time_ranges=[(t0 + 1_000_000, t0 + 20_000_000)], predicates=preds[:1])):
+            what = "many groups sel=%s %s" % (sel is not None, kw)
+            check_reads(engine, pages, arena, descs, truth, sel, dict(grid, **kw), what)
+            check_reads(engine, host, arena, descs, truth, sel, dict(grid, **kw), "host-resident " + what, value_stats=False)
+            q = make_query(FIELDS[:2], aggs=AGGS + ("first", "last"), series_ids=sel, **grid, **kw)
+            _, pts = orc.scan_aggregate(arena, descs, q, return_points=True)
+            engine.scan_aggregate(pages, q)
             assert engine.counters()["points_decoded"] == pts
+    host.close()
+    tombs = random_tombstones(rng, descs, t0, t0 + 90 * 200 * 1000)
+    pages.set_tombstones(tombs)
+    for sel in (None, np.array([9], dtype=np.uint32)):
+        q = make_query(FIELDS[:2], aggs=AGGS + ("first", "last"), series_ids=sel, time_ranges=[(t0 + 500_000, t0 + 30_000_000)], **grid)
+        assert_results_equal(engine.scan_aggregate(pages, q), orc.scan_aggregate(arena, descs, q, tombstones=tombs),
+                             what="tombstones sel=%s" % (sel is not None))
+    pages.close()
+
+    arena, descs, truth, files = many_groups_arena(rng, {4: 90, 9: 90, 11: 90}, 300, overlap_every=7)
+    pages = engine.upload_pages(arena, descs)
+    pages.set_chunk_files(files)
+    for sel in (None, np.array([4, 11], dtype=np.uint32)):
+        for kw in (dict(), dict(predicates=preds)):
+            q = make_query(FIELDS[:2], aggs=AGGS + ("first", "last"), series_ids=sel, **grid, **kw)
+            assert_results_equal(engine.scan_aggregate(pages, q), orc.scan_aggregate(arena, descs, q, chunk_files=files),
+                                 what="overlapping chunks sel=%s %s" % (sel is not None, kw))
+    pages.close()
+
+
+def test_skewed_page_set_caps_the_walk_threads(engine):
+    """One series of 1000 column groups among 3000 single-group series (12 000 field pages). The large series wants 32
+    walk threads, but the walk may not launch more threads than there are field pages: 2000 selected series get 4
+    threads each, all 3001 series 2 each. Results and reader counters as without the split."""
+    rng = np.random.default_rng(31)
+    groups = {0: 1000}
+    groups.update({sid: 1 for sid in range(1, 3001)})
+    arena, descs, truth, _ = many_groups_arena(rng, groups, 30)
+    pages = engine.upload_pages(arena, descs)
+    t0 = 1_000_000
+    fbs, nb = bucket_spec(t0, t0 + 1000 * 30 * 1000, 2_000_000)
+    sel = np.concatenate([[0], rng.choice(np.arange(1, 3001), 1999, replace=False)]).astype(np.uint32)
+    sel.sort()
+    for s in (sel, None):
+        for kw in (dict(), dict(time_ranges=[(t0 + 15_000, t0 + 9_000_000)]), dict(predicates=[(1, cabi.TSKV_PT_I64, ">", 3)])):
+            check_reads(engine, pages, arena, descs, truth, s, dict(width=2_000_000, first_bucket_start=fbs, n_buckets=nb, **kw),
+                        "skewed sel=%s %s" % (s is not None, kw))
     pages.close()

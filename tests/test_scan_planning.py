@@ -128,3 +128,32 @@ def test_page_parts_follow_the_selection_size():
         for want in (2, 3, 5, 8, 64, 4096):
             parts, rows = bin_parts(maxrows, want)
             assert rows % 128 == 0 and parts * rows >= maxrows and (parts - 1) * rows < maxrows and parts <= max(want, 1)
+
+
+def test_walk_split_follows_the_largest_series():
+    """plan_walk_split: threads per walked series of the work-list walk. The smallest power of two that leaves a thread at
+    most 32 column groups of the largest series, at most 1024, halved while the walk would launch more threads than
+    max(field pages, 256)."""
+    L = lib()
+    L.tskvplan_walk_split.argtypes = [C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32]
+    L.tskvplan_walk_split.restype = C.c_uint32
+
+    def split(max_groups, n_walk, n_items, min_threads=256):
+        return L.tskvplan_walk_split(max_groups, n_walk, n_items, min_threads)
+
+    # up to 32 groups per series (TSBS shapes: one): one thread per series
+    for g in (0, 1, 2, 31, 32):
+        assert split(g, 100_000, 400_000) == 1, g
+    # above that, powers of two with at most 32 groups per thread
+    assert [split(g, 3, 10**6) for g in (33, 64, 65, 90, 128, 129, 2000, 32 * 1024)] == [2, 2, 4, 4, 4, 8, 64, 1024]
+    # capped at 1024 threads per series, however many groups
+    assert split(32 * 1024 + 1, 1, 10**6) == 1024 and split(2**32 - 1, 1, 2**33) == 1024
+    # no selection: every series of the page set is walked (3 series x 90 groups x 2 fields)
+    assert split(90, 3, 540) == 4
+    # the thread cap: a series of 1000 groups among 5000 selected single-group series (2 fields: 12 000 field pages)
+    # wants 32 threads per series, but 5000 x S may not exceed 12 000 -> S = 2
+    assert split(1000, 5000, 12_000) == 2
+    assert split(1000, 6001, 12_000) == 1 and split(1000, 6000, 12_000) == 2
+    # a small page set may still launch one block's worth of threads
+    assert split(40, 128, 100) == 2 and split(40, 129, 100) == 1
+    assert split(40, 129, 100, min_threads=512) == 2
