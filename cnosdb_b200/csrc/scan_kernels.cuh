@@ -720,10 +720,6 @@ struct RunAcc {
   bool first_ok, last_ok;  // the run's min/max-time row had a non-null value (first.rs:91-94)
 };
 
-struct ScanCtx {
-  const ScanParams *P;
-};
-
 // Warp-converged flush of run partials into the global state. `active` lanes carry a finished
 // run for cell `gcell` (= qcol * n_cells + cell). When every flushing lane targets the same cell
 // (the common lock-step case of GROUP BY bucket) the partials are combined with a butterfly first
@@ -920,167 +916,8 @@ __device__ __forceinline__ uint4 tomb_lookup(const ScanParams &P, uint32_t serie
   return out;
 }
 
-// One chunk of <= 32 work items, one lane per field page. The whole warp stays converged; lanes
-// without a page (or past their last row) idle through the loop. Generic path (time pages with NULLs or raw / unusual
-// time encodings - nothing the reference's writer produces): row by row, streams read straight from global memory.
-// SEL: the query wants FIRST/LAST somewhere (tracks the (ts, value) of each run's end rows).
-template <int TK, int VK, bool SEL>
-__device__ __forceinline__ void scan_chunk_rows(const ScanParams &P, uint32_t item_begin, uint32_t item_end,
-                                             uint32_t /*ring_base*/, uint64_t *stab, uint4 *s_tomb) {
-  const uint32_t lane = threadIdx.x & 31;
-  const uint32_t item = item_begin + lane;
-  const bool have_item = item < item_end;
-  const uint32_t tslot = 0, vslot = 0;
-
-  uint32_t page = 0, slot = 0, qcol = 0, n_rows = 0;
-  uint8_t pt = TSKV_PT_I64, mask = 0;
-  PageView tpv, vpv;
-  BitCursor tbits, vbits;
-  DeltaCursor<TK == TK_RLE ? DK_RLE_SC : TK == TK_S8B ? DK_S8B_SC : -1, BeStream> tcur;
-  DeltaCursor<VK == VK_S8B ? DK_S8B_ZZ : -1, BeStream> vcur_d;
-  GorillaCursor<BeStream> vcur_g;
-  bool allnull = false;
-  const uint32_t *keepw = nullptr;  // row-filter keep bits of the column group (k_row_filter), or null
-  uint32_t kword = 0xffffffffu;
-
-  if (have_item) {
-    page = P.work_page[item];
-    slot = P.work_slot[item];
-    qcol = P.work_qcol[item] & 0x7f;
-    const tskv_page_desc vd = P.descs[page];
-    const uint32_t tpage = P.time_page_of[page];
-    const tskv_page_desc td = P.descs[tpage];
-    if (P.row_keep) keepw = P.row_keep + P.keep_off[tpage];
-    pt = P.cols[qcol].phys_type;
-    mask = P.cols[qcol].agg_mask;
-    if (P.has_tomb) s_tomb[threadIdx.x] = tomb_lookup(P, vd.series_id, vd.column_id);
-    tskv_status st = kind_status(td.reserved);
-    if (st == TSKV_OK) st = kind_status(vd.reserved);
-    if (st != TSKV_OK) {
-      report_error(P, st, st == kind_status(td.reserved) ? tpage : page);
-    } else {
-      tpv.open(P.arena, td);
-      vpv.open(P.arena, vd);
-      n_rows = vd.num_values;
-      tbits.init(tpv.bitset);
-      vbits.init(vpv.bitset);
-      st = tcur.open(tpv, td.reserved, tslot);
-      if (st == TSKV_OK) {
-        if (VK == VK_GOR) st = vcur_g.open(vpv, vslot);
-        else { st = vcur_d.open(vpv, vd.reserved, vslot); allnull = vd.reserved == DK_ALLNULL; }
-      }
-      if (st != TSKV_OK) { report_error(P, st, page); n_rows = 0; }
-      if (td.reserved == DK_ALLNULL) n_rows = 0;  // no time values: every row fails is_not_null(time)
-    }
-  }
-
-  RunAcc acc;
-  acc.count = 0; acc.sum = 0; acc.sum_hi = 0; acc.kmin = INT64_MAX; acc.kmax = INT64_MIN;
-  acc.first_ts = acc.last_ts = 0; acc.first_val = acc.last_val = 0; acc.first_ok = acc.last_ok = false;
-  BucketState bk; bk.valid = false; bk.floor_regime = false; bk.lo = 0; bk.hi = 0; bk.idx = 0;
-  bool have_run = false;
-  uint32_t run_idx = 0;
-  uint32_t row = 0;
-  uint32_t n_points = 0, n_inrange = 0;
-  const bool is_f64 = pt == TSKV_PT_F64;
-  const bool mean_hi = !is_f64 && (mask & TSKV_AGG_MEAN);
-
-  for (;;) {
-    const bool has = row < n_rows;
-    if (!__any_sync(FULL, has || have_run)) break;
-    bool flush = false, inr = false, vv = false, newrun = false;
-    int64_t t = 0;
-    uint64_t v = 0;
-    if (has) {
-      const bool tv = tbits.next(row);
-      vv = vbits.next(row) && !allnull;
-      bool ok = true;
-      if (tv) { t = (int64_t)tcur.next(); ok = !tcur.exhausted; }
-      else if (row == 0) tcur.skip_first_if_s8b_sc();
-      if (!ok) { report_error(P, TSKV_ERR_BITSET_MISMATCH, P.time_page_of[page]); n_rows = 0; }
-      if (vv && ok) {
-        v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
-        ok = VK == VK_GOR ? !vcur_g.done : !vcur_d.exhausted;
-        if (!ok) {
-          report_error(P, (VK == VK_GOR && vcur_g.err) ? TSKV_ERR_SHORT_BLOCK : TSKV_ERR_BITSET_MISMATCH, page);
-          n_rows = 0;
-        } else {
-          n_points++;
-        }
-      }
-      if (keepw && (row & 31) == 0) kword = __ldg(keepw + (row >> 5));
-      const bool kept = (kword >> (row & 31)) & 1;  // the row filter (DataFilter) drops the row like the time ranges do
-      row++;
-      if (ok && tv && kept) {
-        inr = P.n_ranges == 0;
-#pragma unroll 1
-        for (uint32_t k = 0; k < P.n_ranges && !inr; k++) inr = t >= P.ranges[k].min_ts && t <= P.ranges[k].max_ts;
-        if (P.has_tomb && inr) {  // decode_pages' tombstone handling, row by row (reader.rs:507-551)
-          const uint4 tl = s_tomb[threadIdx.x];
-          int64_t lo = INT64_MIN, hi = INT64_MAX;
-          if (tomb_span(P.tomb_ranges, P.n_tomb_global, t, lo, hi) || tomb_span(P.tomb_ranges + tl.x, tl.y, t, lo, hi)) inr = false;
-          else if (tomb_span(P.tomb_ranges + tl.z, tl.w, t, lo, hi)) vv = false;
-        }
-      }
-      if (inr) {
-        n_inrange++;
-        bool same_bucket = bk.valid && t >= bk.lo && t <= bk.hi;
-        if (!same_bucket) {
-          if (!locate_bucket(P, t, bk)) {
-            report_error(P, TSKV_ERR_BUCKET_RANGE, page);
-            inr = false;
-            bk.valid = false;
-          }
-        }
-        if (inr && (!have_run || bk.idx != run_idx)) { newrun = true; flush = have_run; }
-      }
-    } else {
-      flush = have_run;
-    }
-    warp_flush<SEL>(P, stab, flush, qcol, group_cell_base(P, slot) + run_idx, (int64_t)run_idx, pt, mask, acc, slot);
-    if (flush) have_run = false;
-    if (has && inr) {
-      if (newrun) {
-        have_run = true;
-        run_idx = bk.idx;
-        acc.count = 0; acc.sum = 0; acc.sum_hi = 0; acc.kmin = INT64_MAX; acc.kmax = INT64_MIN;
-        if (SEL) {
-          acc.first_ts = acc.last_ts = t;
-          acc.first_val = acc.last_val = v;
-          acc.first_ok = acc.last_ok = vv;
-        }
-      } else if (SEL) {
-        if (t < acc.first_ts) { acc.first_ts = t; acc.first_val = v; acc.first_ok = vv; }
-        if (t > acc.last_ts) { acc.last_ts = t; acc.last_val = v; acc.last_ok = vv; }
-      }
-      if (vv) {
-        acc.count++;
-        if (is_f64) acc.sum = (uint64_t)__double_as_longlong(__longlong_as_double((long long)acc.sum) + __longlong_as_double((long long)v));
-        else {
-          acc.sum += v;
-          if (mean_hi) acc.sum_hi += (acc.sum < v ? 1 : 0) + (pt == TSKV_PT_I64 ? ((int64_t)v >> 63) : 0);
-        }
-        int64_t k = okey(v, pt);
-        acc.kmin = k < acc.kmin ? k : acc.kmin;
-        acc.kmax = k > acc.kmax ? k : acc.kmax;
-      }
-    }
-  }
-  // The reference decodes a gorilla page to its sentinel (float.rs:480-591): a stream that ends
-  // without one is an error even when enough values were produced.
-  if (VK == VK_GOR && have_item && n_rows != 0 && vcur_g.consumed_any() && !vcur_g.drain())
-    report_error(P, TSKV_ERR_SHORT_BLOCK, page);
-  // statistics
-  n_points = __reduce_add_sync(FULL, n_points);
-  n_inrange = __reduce_add_sync(FULL, n_inrange);
-  if (lane == 0) {
-    if (n_points) atomicAdd(&P.stats[0], (unsigned long long)n_points);
-    if (n_inrange) atomicAdd(&P.stats[1], (unsigned long long)n_inrange);
-  }
-}
-
-// Segment-wise variant for time pages without nulls (every reference-written page: flush rejects a
-// time column with nulls, mem_cache/series_data.rs:303-340) - the fast path. Per lane:
+// The row engine of the fused scan: one chunk of <= 32 work items, one lane per field page, the whole warp converged.
+// Per lane:
 //   1. a lean look-ahead loop over the TIMESTAMPS finds the next segment = maximal run of rows whose
 //      (selected by the time ranges, bucket) is the same;
 //   2. the warp flushes finished runs (converged, once per segment instead of once per row);
@@ -1278,6 +1115,19 @@ __device__ __forceinline__ uint32_t rle_rows_within(uint64_t d, uint64_t delta, 
   return (uint32_t)min((uint64_t)left, q + 1);
 }
 
+// Time cursor of TK_GEN: any time codec straight from global memory, with the time validity bitmap. (The bitmap state
+// lives in the cursor so that the other time classes declare nothing they do not use.)
+struct GenTimeCursor : DeltaCursor<-1, BeStream> {
+  const uint32_t *bm = nullptr;  // time validity bitmap
+  uint32_t word = 0;             // its word of row `row`
+  bool none = false;             // the page has no valid time row
+};
+
+// TK = the time class: RLE timestamps in closed form, simple8b ones staged through a time ring, or generic (TK_GEN: time
+// pages that are raw-encoded, hold NULLs or fail to decode - nothing the reference's writer produces, flush rejects a
+// time column with nulls, mem_cache/series_data.rs:303-340) read from global memory. A NULL-time row fails
+// is_not_null(time) like a row the row filter drops: its keep bit is cleared, its value is still decoded. It keeps the
+// timestamp of the row before it (leading NULLs: of the first valid row), so it never cuts a segment of its own.
 // NARROW (simple8b integer values, no FIRST / LAST): every page of the chunk is narrow (ScanParams.page_narrow), so the
 // values are decoded and accumulated in 32-bit arithmetic (S8bCursor::next32, ValueAcc::add32).
 template <int TK, int VK, bool SEL, bool NARROW>
@@ -1295,7 +1145,8 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   uint32_t page = 0, slot = 0, qcol = 0, n_rows = 0;
   uint8_t pt = VK == VK_GOR ? TSKV_PT_F64 : TSKV_PT_I64, mask = 0;
   PageView tpv, vpv;
-  S8bCursor<false> tcur;                       // TK_S8B: timestamps staged through the time ring
+  // TK_S8B: timestamps staged through the time ring; TK_GEN: GenTimeCursor
+  typename std::conditional<TK == TK_GEN, GenTimeCursor, S8bCursor<false>>::type tcur;
   uint64_t rle_t0 = 0, rle_delta = 0;          // TK_RLE: t(row) = rle_t0 + row * rle_delta (wrapping), closed form
   double rle_inv = 0.0;
   typename std::conditional<VK == VK_S8B, S8bCursor<true>, DeltaCursor<-1, SeqStream>>::type vcur_d;
@@ -1305,7 +1156,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   bool allnull = false;
   int64_t pend_t = 0;  // timestamp of row `row`
 
-  if (TK == TK_S8B) tcur.reset(tslot);
+  if constexpr (TK == TK_S8B) tcur.reset(tslot);
   if (VK == VK_GOR) vcur_g.reset(vslot);
   else cursor_reset(vcur_d, vslot);
   // This lane decodes rows [r0, n_rows) of its page: the whole page, or - the bin's pages are cut at restart points
@@ -1331,11 +1182,15 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
       split = sk_v != SKIP_NONE && sk_t != SKIP_NONE;
     }
     r0 = part * part_rows;
-    tskv_status st = kind_status(vd.reserved);  // the time page is RLE / simple8b here: always decodable
+    tskv_status st = kind_status(vd.reserved);  // (RLE / simple8b time pages always decode)
+    uint32_t st_page = page;
+    if constexpr (TK == TK_GEN) {  // the time page's error comes first
+      if (kind_status(td.reserved) != TSKV_OK) { st = kind_status(td.reserved); st_page = tpage; }
+    }
     if (part != 0 && (!split || r0 >= page_rows)) {
       // nothing for this lane: the page ends before this part, or part 0's lane decodes all of it
     } else if (st != TSKV_OK) {
-      report_error(P, st, page);
+      report_error(P, st, st_page);
     } else {
       tpv.open(P.arena, td);
       vpv.open(P.arena, vd);
@@ -1351,7 +1206,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
         if ((int64_t)rle_delta > 0) rle_inv = 1.0 / (double)rle_delta;
       } else if (part == 0) {
         st = tcur.open(tpv, td.reserved, tslot);
-      } else {
+      } else if constexpr (TK == TK_S8B) {
         tcur.restore(tpv, tslot, load_skip(P.skip + sk_t + ent));  // the state after row r0's timestamp
       }
       if (st == TSKV_OK) {
@@ -1365,10 +1220,31 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           // (generic value codecs are never cut: n_parts == 1)
         }
       }
+      if constexpr (TK == TK_GEN) {
+        if (td.reserved == DK_ALLNULL) n_rows = 0;  // no time values: every row fails is_not_null(time)
+        tcur.bm = reinterpret_cast<const uint32_t *>(tpv.bitset);
+      }
       if (st == TSKV_OK && n_rows) {
-        if (TK == TK_RLE) pend_t = (int64_t)(rle_t0 + (uint64_t)r0 * rle_delta);
-        else if (part == 0) pend_t = (int64_t)tcur.next();  // the first value: no ring access (cursors.cuh)
-        else pend_t = (int64_t)tcur.v;
+        if (TK == TK_RLE) {
+          pend_t = (int64_t)(rle_t0 + (uint64_t)r0 * rle_delta);
+        } else if constexpr (TK == TK_GEN) {
+          uint32_t f = 0, w = 0;  // the first valid time row: its timestamp is row 0's (rows before it are NULL)
+          while (f < n_rows && (w = __ldg(tcur.bm + (f >> 5))) == 0) f += 32;
+          if (f < n_rows) f += __ffs(w) - 1;
+          tcur.none = f >= n_rows;
+          if (f == 0) {
+            pend_t = (int64_t)tcur.next();
+          } else if (!tcur.none) {  // peek: row f takes the value when the row loop reaches it
+            tcur.skip_first_if_s8b_sc();
+            DeltaCursor<-1, BeStream> peek = tcur;
+            pend_t = (int64_t)peek.next();
+          }
+          tcur.word = __ldg(tcur.bm);
+        } else if (part == 0) {
+          pend_t = (int64_t)tcur.next();  // the first value: no ring access (cursors.cuh)
+        } else {
+          pend_t = (int64_t)tcur.v;
+        }
       }
       if (st != TSKV_OK) { report_error(P, st, st == TSKV_ERR_BITSET_MISMATCH ? tpage : page); n_rows = 0; }
     }
@@ -1415,7 +1291,8 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
     if ((row & 31) == 0) {  // entering a new bitmap word: take the prefetched one, prefetch the next
       vword = vahead;
       vahead = __ldg(vbm + (row >> 5) + 1);  // reads at most 8 bytes past the bitmap (inside the page)
-      if (keepw) kword = __ldg(keepw + (row >> 5));
+      if constexpr (TK == TK_GEN) kword = (keepw ? __ldg(keepw + (row >> 5)) : 0xffffffffu) & tcur.word;
+      else if (keepw) kword = __ldg(keepw + (row >> 5));
     }
     vv = ((vword >> (row & 31)) & 1) && !allnull;
     kept = (kword >> (row & 31)) & 1;
@@ -1636,6 +1513,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
       } else {
         lim_lo = lim_hi = pend_t;
         seg_in = range_span(P, pend_t, lim_lo, lim_hi);
+        if constexpr (TK == TK_GEN) seg_in = seg_in && !tcur.none;
         if (P.has_tomb) {  // decode_pages' tombstone handling (reader.rs:507-551) as two more segment attributes
           const uint4 tl = s_tomb[threadIdx.x];
           const bool dropped = tomb_span(P.tomb_ranges, P.n_tomb_global, pend_t, lim_lo, lim_hi) |
@@ -1759,11 +1637,21 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           }
           if (seg_in && kept) n_inrange++;
           row++;
-          t = (int64_t)tcur.next();  // (past the last row this runs one value too far - harmless)
+          if constexpr (TK == TK_GEN) {  // only rows with a timestamp advance the cursor, never past the last row
+            if (row < n_rows) {
+              if ((row & 31) == 0) tcur.word = __ldg(tcur.bm + (row >> 5));
+              if ((tcur.word >> (row & 31)) & 1) t = (int64_t)tcur.next();
+            }
+          } else {
+            t = (int64_t)tcur.next();  // (past the last row this runs one value too far - harmless)
+          }
           more = row < n_rows && (uint64_t)t - (uint64_t)lim_lo <= span;
         } while (more);
         pend_t = t;
-        if (tcur.exhausted() && row < n_rows) { report_error(P, TSKV_ERR_BITSET_MISMATCH, P.time_page_of[page]); n_rows = row; }
+        if (cursor_exhausted(tcur) && (TK == TK_GEN || row < n_rows)) {
+          report_error(P, TSKV_ERR_BITSET_MISMATCH, P.time_page_of[page]);
+          n_rows = row;
+        }
       }
       check_values();
     }
@@ -1787,7 +1675,8 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
 // The fused decode -> filter -> bucket-reduce kernel, one instantiation per decode-kind bin (time codec x
 // value codec) and SEL (= the query asks for FIRST/LAST) so that each keeps its state in registers.
 // The bins' kernels run concurrently on separate streams, each with a persistent grid sized to its share
-// of the work; a warp repeatedly grabs one 32-item chunk of its bin from the bin's global counter.
+// of the work; a warp repeatedly grabs one 32-item chunk of its bin from the bin's global counter and runs it through
+// scan_chunk_seg, whatever the bin's time class.
 #ifndef SCAN_MIN_BLOCKS
 #define SCAN_MIN_BLOCKS 4
 #endif
@@ -1795,13 +1684,14 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
 // LAST free of spills; the FIRST / LAST variants spill 4-146 bytes. A fifth block per SM would cap them at 96 registers
 // and move the row loop's state into local memory.
 __host__ __device__ constexpr int scan_min_blocks(int /*tk*/, bool /*sel*/) { return SCAN_MIN_BLOCKS; }
-// staging-ring bytes one warp of the fused kernel needs (generic time pages read from global memory)
+// staging-ring bytes one warp of the fused kernel needs: a value ring, and a time ring for simple8b timestamps (generic
+// time pages are read from global memory)
 __host__ __device__ constexpr uint32_t scan_ring_bytes_per_warp(int tk) {
-  return tk == TK_RLE ? RING_BYTES_PER_WARP : tk == TK_S8B ? 2 * RING_BYTES_PER_WARP : 0;
+  return tk == TK_S8B ? 2 * RING_BYTES_PER_WARP : RING_BYTES_PER_WARP;
 }
 // per-warp shared memory of the fused kernel: staging rings + the staged-flush area
 __host__ __device__ constexpr uint32_t scan_warp_bytes(int tk) {
-  return tk == TK_GEN ? 0 : scan_ring_bytes_per_warp(tk) + flush_stage_bytes(flush_slots(tk));
+  return scan_ring_bytes_per_warp(tk) + flush_stage_bytes(flush_slots(tk));
 }
 // per-lane tombstone lists (tomb_lookup), after the warps' areas; allocated only when the page set has tombstones
 constexpr uint32_t SCAN_TOMB_BYTES = SCAN_THREADS * sizeof(uint4);
@@ -1847,9 +1737,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, SEL)) k_scan
     const uint32_t part = c - group * n_parts;
     const uint32_t begin = begin0 + (group << 5);
     const uint32_t end = min(begin + 32, end0);
-    if constexpr (TK == TK_GEN) {
-      scan_chunk_rows<TK, VK, SEL>(P, begin, end, ring_base, s_tab, s_tomb);
-    } else if constexpr (NARROW == NARROW_SOME) {
+    if constexpr (NARROW == NARROW_SOME) {
       // 32-bit arithmetic when all of the chunk's pages are narrow (the work list keeps a bin's narrow pages together)
       const uint32_t item = begin + lane;
       const bool narrow = __all_sync(FULL, item >= end || __ldg(P.page_narrow + __ldg(P.work_page + item)));

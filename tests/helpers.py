@@ -806,8 +806,8 @@ def geometry_queries(case, ranges, truth):
 #   A  identical RLE timestamps (whole warps run the uniform bucket schedule);
 #   B  RLE timestamps starting sid % 7 rows later (the per-lane segment loop);
 #   C  jittered timestamps (simple8b time pages: the fused timestamp + value loop);
-#   D  block A's timestamps with the last row moved 2^61 ns later: a raw time page (the generic-time kernels, where the
-#      scan decodes Gorilla with GorillaCursor). Bucketed queries leave that row out with a time range.
+#   D  block A's timestamps with the last row moved 2^61 ns later: a raw time page (the generic-time kernels, which read
+#      the timestamps from global memory). Bucketed queries leave that row out with a time range.
 # The value kind of a series is sid % 10 (F64_KINDS). Rows 127-129 and 255-257 hold the hardest patterns, so that the
 # restart points (every 128 rows) and the cuts between page parts land on them.
 

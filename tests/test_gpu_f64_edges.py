@@ -1,6 +1,6 @@
 """f64 pages of IEEE special values and adversarial bit patterns through every Gorilla decoder of the scan (see
-f64_edge_arena in tests/helpers.py): GorillaCursor (k_decode_warp, the generic-time rows loop), GorillaRing (the fused
-bins, k_build_skip's restart points, pages cut into parts), next to the raw twin of every page. COUNT / MIN / MAX (IEEE totalOrder, so the NaN keys 0x7FFF...FFFF and 0xFFFF...FFFF are the MIN and MAX
+f64_edge_arena in tests/helpers.py): GorillaCursor (k_decode_warp), GorillaRing (every fused
+bin, k_build_skip's restart points, pages cut into parts), next to the raw twin of every page. COUNT / MIN / MAX (IEEE totalOrder, so the NaN keys 0x7FFF...FFFF and 0xFFFF...FFFF are the MIN and MAX
 identities) must equal the exact reference bit for bit, SUM / MEAN its class (NaN, the exact inf, or finite within the
 order-free bound, +0.0 when zero), and FIRST / LAST the oracle bit for bit, NaN payloads included."""
 import numpy as np
