@@ -6,10 +6,12 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <numeric>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include <cuda_runtime.h>
@@ -32,11 +34,41 @@ using namespace tskv;
     }                                                                                  \
   } while (0)
 
+// Owners of the library's CUDA resources: each handle is released by its deleter when its owner goes away or is
+// replaced.
+struct DevFree {
+  void operator()(void *p) const { cudaFree(p); }
+};
+struct AsyncFree {  // stream-ordered: the buffer returns to the pool after the work enqueued before the free
+  cudaStream_t stream = nullptr;
+  void operator()(void *p) const { cudaFreeAsync(p, stream); }
+};
+struct EventDestroy {
+  void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
+};
+struct StreamDestroy {
+  void operator()(cudaStream_t st) const { cudaStreamDestroy(st); }
+};
+struct GraphExecDestroy {
+  void operator()(cudaGraphExec_t g) const { cudaGraphExecDestroy(g); }
+};
+struct HostUnregister {
+  void operator()(void *p) const { cudaHostUnregister(p); }
+};
+template <typename T>
+using dev_ptr = std::unique_ptr<T[], DevFree>;
+template <typename T>
+using async_ptr = std::unique_ptr<T[], AsyncFree>;
+using event_ptr = std::unique_ptr<CUevent_st, EventDestroy>;
+using stream_ptr = std::unique_ptr<CUstream_st, StreamDestroy>;
+using graph_exec_ptr = std::unique_ptr<CUgraphExec_st, GraphExecDestroy>;
+using host_reg_ptr = std::unique_ptr<void, HostUnregister>;
+
 struct tskv_ctx {
   int device = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  cudaStream_t bin_stream[N_BINS] = {nullptr};  // the per-bin fused kernels run concurrently
+  stream_ptr stream;
+  event_ptr ev0, ev1;
+  stream_ptr bin_stream[N_BINS];  // the per-bin fused kernels run concurrently
   int sm_count = 132;
   int max_dyn_smem = 48 * 1024;
   ncclComm_t comm = nullptr;  // tskvgpu_comm_init
@@ -51,35 +83,52 @@ struct tskv_ctx {
   }
 };
 
+// Tombstone tables (tskvgpu_pages_set_tombstones): the all-series ranges first, then one CSR row per (series, column) key
+struct TombTables {
+  dev_ptr<uint64_t> keys;
+  dev_ptr<uint32_t> off;
+  dev_ptr<tskv_time_range> ranges;
+  uint32_t n_keys = 0, n_global = 0, n_ranges = 0;
+};
+
+// Overlapping chunks (tskvgpu_pages_set_chunk_files, merge_kernels.cuh): the plan, its device copies and the merge rows'
+// timestamps (decoded once)
+struct OverlapTables {
+  OverlapPlan plan;
+  dev_ptr<uint8_t> d_cg_merge;
+  dev_ptr<int64_t> d_merge_ts;
+  dev_ptr<uint64_t> d_mcg_row0, d_mcg_bm0;
+  dev_ptr<uint32_t> d_mcg_cg, d_mcg_stream, d_stream_group, d_stream_first_mcg, d_group_first_stream;
+  std::vector<uint64_t> h_mcg_bm0;
+  uint64_t merge_rows = 0, merge_bm_words = 0;
+};
+
 struct tskv_pages {
   tskv_ctx *ctx = nullptr;
-  uint8_t *d_arena = nullptr;       // device copy (or, host-resident mode: gather target)
+  dev_ptr<uint8_t> d_arena;          // device copy (or, host-resident mode: gather target)
   const uint8_t *h_mapped = nullptr; // host-resident mode: device-visible alias of the caller's arena
   bool verify_on_read = false;       // host-resident + VERIFY_CRC: CRC32 checked on the device on every scan
-  uint32_t *d_crc_tables = nullptr;
-  void *h_registered = nullptr;      // range this library page-locked (unregistered on destroy)
+  dev_ptr<uint32_t> d_crc_tables;
+  host_reg_ptr h_registered;         // range this library page-locked
   uint64_t arena_len = 0;
-  tskv_page_desc *d_descs = nullptr;
+  dev_ptr<tskv_page_desc> d_descs;
   std::vector<tskv_page_desc> h_descs;  // with .reserved = DK kind
   uint64_t n_descs = 0;
-  uint32_t *d_time_page_of = nullptr;
+  dev_ptr<uint32_t> d_time_page_of;
   uint32_t n_cg = 0;
-  uint32_t *d_cg_time_page = nullptr;
-  uint32_t *d_cg_series_rank = nullptr;
-  uint32_t *d_series_sorted = nullptr;  // the page set's distinct series ids, ascending (rank -> id)
-  uint32_t *d_rank_cg_start = nullptr, *d_rank_cg = nullptr;  // CSR: series rank -> its column groups (arena order)
+  dev_ptr<uint32_t> d_cg_time_page;
+  dev_ptr<uint32_t> d_cg_series_rank;
+  dev_ptr<uint32_t> d_series_sorted;  // the page set's distinct series ids, ascending (rank -> id)
+  dev_ptr<uint32_t> d_rank_cg_start, d_rank_cg;  // CSR: series rank -> its column groups (arena order)
   uint32_t max_series_cg = 0;           // most column groups of one series (plan_walk_split)
-  uint8_t *d_page_bin = nullptr;        // decode-kind bin of every field page
-  mutable int64_t *d_page_stats = nullptr;  // {min key, max key} of every field page (k_page_stats), built on first use
+  dev_ptr<uint8_t> d_page_bin;          // decode-kind bin of every field page
+  mutable dev_ptr<int64_t> d_page_stats;  // {min key, max key} of every field page (k_page_stats), built on first use
   uint32_t n_items = 0;              // field pages
   uint32_t h_bin_pages[N_BINS]{};    // field pages per bin
   uint64_t h_bin_bytes[N_BINS]{};    // field-page bytes per bin (orders the PCIe gathers of host-resident scans)
   uint64_t h_bin_rows[N_BINS]{};     // rows of the bin's field pages (serial cost of its chunks)
-  // tombstones (tskvgpu_pages_set_tombstones); the epoch invalidates scans prepared before a change
-  uint64_t *d_tomb_keys = nullptr;
-  uint32_t *d_tomb_off = nullptr;
-  tskv_time_range *d_tomb_ranges = nullptr;
-  uint32_t n_tomb_keys = 0, n_tomb_global = 0, n_tomb_ranges = 0;
+  // the epoch invalidates scans prepared before a change of the tombstones
+  TombTables tomb;
   uint64_t tomb_epoch = 0;
   std::vector<uint32_t> series;  // sorted distinct ids
   // arena-wide time bounds, computed on first use by k_time_bounds (the reference keeps them in
@@ -88,33 +137,25 @@ struct tskv_pages {
   mutable int64_t ts_min = INT64_MIN, ts_max = INT64_MAX;
   // per-column-group [min_ts, max_ts] (ColumnGroup::time_range()): handed in by the caller
   // (tskvgpu_pages_set_time_bounds) or computed together with the arena-wide bounds; drives statistics pruning
-  mutable tskv_time_range *d_cg_bounds = nullptr;
+  mutable dev_ptr<tskv_time_range> d_cg_bounds;
   // row-filter masks: 32-bit words per column group, offset stored at the index of the group's time page
-  uint32_t *d_keep_off = nullptr;
+  dev_ptr<uint32_t> d_keep_off;
   uint64_t keep_words = 0;
   // restart points (skip_kernels.cuh): per page the index of its first entry (or SKIP_NONE), built once at upload
-  uint32_t *d_skip_off = nullptr;
-  SkipEntry *d_skip = nullptr;
+  dev_ptr<uint32_t> d_skip_off;
+  dev_ptr<SkipEntry> d_skip;
   uint64_t n_skip = 0;
   // per page 1 = a simple8b integer page whose values all lie in [-2^31, 2^31) (i64) / [0, 2^31) (u64) (k_build_skip;
   // null for host-resident page sets: every page is then wide), and per bin whether none, some or all of its pages are
   // narrow (NARROW_*: which variant of the fused kernel runs the bin)
-  uint8_t *d_narrow = nullptr;
+  dev_ptr<uint8_t> d_narrow;
   uint8_t h_bin_narrow[N_BINS]{};
   uint32_t h_bin_maxrows[N_BINS]{};  // longest field page of each bin (parts per page when a scan cuts the bin's pages)
-  // overlapping chunks (tskvgpu_pages_set_chunk_files, merge_kernels.cuh): the plan, its device copies and the merge
-  // rows' timestamps (decoded once); the epoch invalidates scans prepared before a change
   std::vector<uint32_t> h_cg_time_page, h_cg_series;
   std::vector<uint8_t> h_time_has_nulls;
-  OverlapPlan overlap;
   std::vector<tskv_time_range> h_cg_bounds;
-  uint8_t *d_cg_merge = nullptr;
-  int64_t *d_merge_ts = nullptr;
-  uint64_t *d_mcg_row0 = nullptr, *d_mcg_bm0 = nullptr;
-  uint32_t *d_mcg_cg = nullptr, *d_mcg_stream = nullptr, *d_stream_group = nullptr, *d_stream_first_mcg = nullptr,
-           *d_group_first_stream = nullptr;
-  std::vector<uint64_t> h_mcg_bm0;
-  uint64_t merge_rows = 0, merge_bm_words = 0;
+  // the epoch invalidates scans prepared before a change of the chunk files
+  OverlapTables overlap;
   uint64_t chunk_epoch = 0;
 };
 
@@ -126,70 +167,71 @@ struct tskv_scan {
   ScanParams params{};
   uint32_t n_cols = 0, n_out = 0;
   bool has_sel = false;  // any FIRST/LAST
-  // device buffers
-  uint32_t *d_series = nullptr;
-  int32_t *d_rank_slot = nullptr;  // rank of a series in the page set -> position in the selection list (or -1)
-  uint32_t *d_bucket = nullptr;    // selection-driven work list: [N_BINS * n_cols * WL_SUB] counts / cursors | [.. + 1] offsets
+  // device buffers, stream-ordered on the context stream (cudaMallocAsync): no device-wide synchronisation on the query
+  // path, memory is recycled by the pool
+  async_ptr<uint32_t> d_series;
+  async_ptr<int32_t> d_rank_slot;  // rank of a series in the page set -> position in the selection list (or -1)
+  async_ptr<uint32_t> d_bucket;    // selection-driven work list: [N_BINS * n_cols * WL_SUB] counts / cursors | [.. + 1] offsets
   uint32_t walk_split_log2 = 0;    // log2 of the work-list walk's threads per series (plan_walk_split)
-  int32_t *d_cg_slot = nullptr;
-  uint32_t *d_work_page = nullptr, *d_work_slot = nullptr;
-  uint8_t *d_work_qcol = nullptr;
-  uint32_t *d_bin_cstart = nullptr;  // [N_BINS+1] then [1] total
-  ColState *d_cols = nullptr;
-  OutCol *d_outs = nullptr;
-  MeanExport *d_means = nullptr;
+  async_ptr<int32_t> d_cg_slot;
+  async_ptr<uint32_t> d_work_page, d_work_slot;
+  async_ptr<uint8_t> d_work_qcol;
+  async_ptr<uint32_t> d_bin_cstart;  // [N_BINS+1] then [1] total
+  async_ptr<ColState> d_cols;
+  async_ptr<OutCol> d_outs;
+  async_ptr<MeanExport> d_means;
   uint32_t n_means = 0;
-  uint64_t *d_state = nullptr;
-  uint32_t *d_task_counter = nullptr;  // the aux block (AUX_*); the pointers below point into it
+  async_ptr<uint64_t> d_state;
+  async_ptr<unsigned long long> d_aux;  // the aux block (AUX_*); the pointers below point into it
   int32_t *d_status = nullptr;
   unsigned long long *d_err_page = nullptr;
   unsigned long long *d_stats = nullptr;     // [0] points [1] rows in range
   unsigned long long *d_counters = nullptr;  // CTR_*
-  uint64_t *d_values = nullptr;
-  uint8_t *d_validity = nullptr;
+  async_ptr<uint64_t> d_values;
+  async_ptr<uint8_t> d_validity;
   int grid[N_BINS] = {0};
   int occ[N_BINS] = {0};  // resident CTAs per SM of each bin's kernel at this scan's shared memory size
   tskv_ctx *ctx = nullptr;
   uint32_t n_series_sel = 0;
   bool enqueued = false;
   // timing / ordering events of THIS scan (several scans of one context may be in flight from different host threads)
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  cudaEvent_t ev_bin[N_BINS + 1] = {nullptr};  // [0] fork, [N_BINS] join of the fused phase
-  cudaEvent_t ev_bin_start[N_BINS] = {nullptr}, ev_bin_done[N_BINS] = {nullptr}, ev_gather[N_BINS] = {nullptr};
+  event_ptr ev0, ev1;
+  event_ptr ev_bin[N_BINS + 1];  // [0] fork, [N_BINS] join of the fused phase
+  event_ptr ev_bin_start[N_BINS], ev_bin_done[N_BINS], ev_gather[N_BINS];
   tskv_counters counters{};  // of the last completed pass of this scan
   // A scan that is enqueued repeatedly replays its whole pass (2 memsets, ~7 small kernels, the fused kernels forked
   // over the bin streams, export) as ONE CUDA graph launch: captured on the second enqueue, so one-shot scans never pay
   // for a capture.
-  cudaGraphExec_t graph_exec = nullptr;
-  cudaEvent_t ev_cfork = nullptr, ev_cjoin[N_BINS] = {nullptr};  // dependency-only events of the captured pass
+  graph_exec_ptr graph_exec;
+  event_ptr ev_cfork, ev_cjoin[N_BINS];  // dependency-only events of the captured pass
   int32_t *d_crc_status = nullptr;  // a CRC mismatch outranks whatever the decoders made of the bad page
   unsigned long long *d_crc_err_page = nullptr;
   uint32_t n_enqueued = 0;
   bool graph_failed = false;
   PruneRanges prune{};
-  uint64_t *d_gathered = nullptr;  // all ranks' exchange regions (tskvgpu_scan_exchange)
+  async_ptr<uint64_t> d_gathered;  // all ranks' exchange regions (tskvgpu_scan_exchange)
   PredicateSet preds{};            // pushed field predicates (row filter)
-  uint32_t *d_row_keep = nullptr;  // one keep bit per row of every column group (k_row_filter)
+  async_ptr<uint32_t> d_row_keep;  // one keep bit per row of every column group (k_row_filter)
   // merge pass over the overlapping chunks this scan reads (merge_kernels.cuh)
   uint64_t chunk_epoch = 0;
   MergeParams merge{};
   uint32_t n_merge_pages = 0;      // field pages decoded per pass
   uint64_t merge_page_bytes = 0, merge_read_pages = 0;
-  uint8_t *d_mcg_active = nullptr;
-  uint64_t *d_mvals = nullptr;
-  uint32_t *d_mvalid = nullptr;
-  uint32_t *d_mpage = nullptr;
-  uint64_t *d_mrow_off = nullptr, *d_mbm_off = nullptr;
+  async_ptr<uint8_t> d_mcg_active;
+  async_ptr<uint64_t> d_mvals;
+  async_ptr<uint32_t> d_mvalid;
+  async_ptr<uint32_t> d_mpage;
+  async_ptr<uint64_t> d_mrow_off, d_mbm_off;
   // Layout of the state the fused kernels write at params.state: d_state / sl for a tumbling scan. A sliding scan's
   // kernels fill d_pane_state (panes one slide wide) and k_window_combine folds every run of win_k panes into the
   // windows of d_state / sl, which export, exchange, partials and finalize see.
   StateLayout kern_sl{};
-  uint64_t *d_pane_state = nullptr;
-  CombineOp *d_combine = nullptr;
+  async_ptr<uint64_t> d_pane_state;
+  async_ptr<CombineOp> d_combine;
   uint32_t n_combine = 0, win_k = 1, n_panes = 0, n_windows = 0;
   // GROUP BY tags: the group of every slot (params.slot_group) and the work-list walk order, slots sorted by group (null
   // when that is the selection order)
-  uint32_t *d_slot_group = nullptr, *d_walk = nullptr;
+  async_ptr<uint32_t> d_slot_group, d_walk;
 };
 
 namespace {
@@ -212,9 +254,47 @@ const char *status_text(tskv_status st) {
   }
 }
 
+// Fill `p` with n elements; a zero-length array still gets one element (a valid, distinct address).
 template <typename T>
-cudaError_t dev_alloc(T **p, size_t n) {
-  return cudaMalloc(reinterpret_cast<void **>(p), std::max<size_t>(n, 1) * sizeof(T));
+cudaError_t dev_alloc(dev_ptr<T> &p, size_t n) {
+  T *raw = nullptr;
+  const cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&raw), std::max<size_t>(n, 1) * sizeof(T));
+  p.reset(e == cudaSuccess ? raw : nullptr);
+  return e;
+}
+// Stream-ordered on `stream`, and freed on it.
+template <typename T>
+cudaError_t stream_alloc(async_ptr<T> &p, size_t n, cudaStream_t stream) {
+  T *raw = nullptr;
+  const cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&raw), std::max<size_t>(n, 1) * sizeof(T), stream);
+  p = async_ptr<T>(e == cudaSuccess ? raw : nullptr, AsyncFree{stream});
+  return e;
+}
+// Allocates n elements as dev_alloc / stream_alloc do and copies src[0, n) into them on `stream`. The copy is ordered
+// before any later work on `stream`; src must stay alive until then or until the stream is synchronised.
+template <typename T, typename Free>
+cudaError_t upload(std::unique_ptr<T[], Free> &p, const T *src, size_t n, cudaStream_t stream) {
+  cudaError_t e;
+  if constexpr (std::is_same_v<Free, AsyncFree>) e = stream_alloc(p, n, stream);
+  else e = dev_alloc(p, n);
+  if (e == cudaSuccess && n) e = cudaMemcpyAsync(p.get(), src, n * sizeof(T), cudaMemcpyHostToDevice, stream);
+  return e;
+}
+// Copies src[0, n) into a page set's table on `stream` and waits for the copy. A table already in place is overwritten
+// where it lies: a scan captured into a CUDA graph holds its address. A new table is published only once it is filled.
+template <typename T>
+cudaError_t fill_table(dev_ptr<T> &table, const T *src, size_t n, cudaStream_t stream) {
+  dev_ptr<T> fresh;
+  cudaError_t e = table ? cudaSuccess : dev_alloc(fresh, n);
+  if (e == cudaSuccess && n) e = cudaMemcpyAsync(table ? table.get() : fresh.get(), src, n * sizeof(T), cudaMemcpyHostToDevice, stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+  if (e == cudaSuccess && fresh) table = std::move(fresh);
+  return e;
+}
+
+event_ptr new_event(unsigned flags = cudaEventDefault) {
+  cudaEvent_t ev = nullptr;
+  return event_ptr(cudaEventCreateWithFlags(&ev, flags) == cudaSuccess ? ev : nullptr);
 }
 
 unsigned bits_for(uint64_t max_value) {  // bits needed to represent values in [0, max_value]
@@ -278,21 +358,19 @@ double chunk_cost(int bin) {
 // Lazily computes the arena's min / max timestamp on the device (one lane per time page).
 void ensure_time_bounds(tskv_ctx *ctx, const tskv_pages *pg) {
   if (pg->bounds_known || pg->n_cg == 0) return;
-  long long *d_bounds = nullptr;
-  if (cudaMalloc(reinterpret_cast<void **>(&d_bounds), 16) != cudaSuccess) return;
+  dev_ptr<long long> d_bounds;
+  if (dev_alloc(d_bounds, 2) != cudaSuccess) return;
   long long b[2] = {INT64_MAX, INT64_MIN};
-  cudaMemcpyAsync(d_bounds, b, sizeof(b), cudaMemcpyHostToDevice, ctx->stream);
-  if (!pg->d_cg_bounds && cudaMalloc(reinterpret_cast<void **>(&pg->d_cg_bounds), (size_t)pg->n_cg * sizeof(tskv_time_range)) != cudaSuccess)
-    pg->d_cg_bounds = nullptr;
-  k_time_bounds<<<(pg->n_cg + 127) / 128, 128, 0, ctx->stream>>>(pg->h_mapped ? pg->h_mapped : pg->d_arena, pg->d_descs,
-                                                                pg->d_cg_time_page, pg->n_cg, d_bounds, pg->d_cg_bounds);
-  if (cudaMemcpyAsync(b, d_bounds, sizeof(b), cudaMemcpyDeviceToHost, ctx->stream) == cudaSuccess &&
-      cudaStreamSynchronize(ctx->stream) == cudaSuccess && b[0] <= b[1]) {
+  cudaMemcpyAsync(d_bounds.get(), b, sizeof(b), cudaMemcpyHostToDevice, ctx->stream.get());
+  if (!pg->d_cg_bounds) dev_alloc(pg->d_cg_bounds, pg->n_cg);
+  k_time_bounds<<<(pg->n_cg + 127) / 128, 128, 0, ctx->stream.get()>>>(pg->h_mapped ? pg->h_mapped : pg->d_arena.get(), pg->d_descs.get(),
+                                                                pg->d_cg_time_page.get(), pg->n_cg, d_bounds.get(), pg->d_cg_bounds.get());
+  if (cudaMemcpyAsync(b, d_bounds.get(), sizeof(b), cudaMemcpyDeviceToHost, ctx->stream.get()) == cudaSuccess &&
+      cudaStreamSynchronize(ctx->stream.get()) == cudaSuccess && b[0] <= b[1]) {
     pg->ts_min = b[0];
     pg->ts_max = b[1];
   }
   pg->bounds_known = true;
-  cudaFree(d_bounds);
 }
 
 // Value statistics of the field pages, computed on the device the first time a scan with field predicates is prepared
@@ -300,17 +378,14 @@ void ensure_time_bounds(tskv_ctx *ctx, const tskv_pages *pg) {
 void ensure_page_stats(tskv_ctx *ctx, const tskv_pages *pg) {
   static const bool off = getenv("TSKV_NO_VALUE_STATS") != nullptr;
   if (off || pg->d_page_stats || pg->h_mapped || pg->n_descs == 0) return;
-  int64_t *d = nullptr;
-  if (cudaMalloc(reinterpret_cast<void **>(&d), (size_t)pg->n_descs * 16) != cudaSuccess) {
+  dev_ptr<int64_t> d;
+  if (dev_alloc(d, 2 * (size_t)pg->n_descs) != cudaSuccess) {
     cudaGetLastError();
     return;
   }
-  k_page_stats<<<(unsigned)((pg->n_descs + 127) / 128), 128, 0, ctx->stream>>>(pg->d_arena, pg->d_descs, pg->n_descs, d);
-  if (cudaGetLastError() != cudaSuccess || cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-    cudaFree(d);
-    return;
-  }
-  pg->d_page_stats = d;
+  k_page_stats<<<(unsigned)((pg->n_descs + 127) / 128), 128, 0, ctx->stream.get()>>>(pg->d_arena.get(), pg->d_descs.get(), pg->n_descs, d.get());
+  if (cudaGetLastError() != cudaSuccess || cudaStreamSynchronize(ctx->stream.get()) != cudaSuccess) return;
+  pg->d_page_stats = std::move(d);
 }
 
 // GROUP BY tags (the *_grouped entry points): group of every selected series slot, and the number of groups.
@@ -466,57 +541,13 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
   return plan;
 }
 
-// Per-scan buffers are stream-ordered (cudaMallocAsync on the context stream): no device-wide
-// synchronisation on the query path, memory is recycled by the pool.
-void free_scan(tskv_scan *s) {
-  if (!s) return;
-  cudaStream_t st = s->ctx ? s->ctx->stream : nullptr;
-  void *bufs[] = {s->d_series, s->d_rank_slot, s->d_bucket, s->d_cg_slot, s->d_work_page, s->d_work_slot,
-                  s->d_work_qcol, s->d_bin_cstart, s->d_cols, s->d_outs, s->d_means, s->d_state,
-                  s->d_task_counter, s->d_values, s->d_validity, s->d_gathered, s->d_row_keep,
-                  s->d_mcg_active, s->d_mvals, s->d_mvalid, s->d_mpage, s->d_mrow_off, s->d_mbm_off, s->d_pane_state, s->d_combine,
-                  s->d_slot_group, s->d_walk};
-  for (void *b : bufs)
-    if (b) cudaFreeAsync(b, st);
-  if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
-  if (s->ev_cfork) cudaEventDestroy(s->ev_cfork);
-  for (int b = 0; b < N_BINS; b++)
-    if (s->ev_cjoin[b]) cudaEventDestroy(s->ev_cjoin[b]);
-  if (s->ev0) cudaEventDestroy(s->ev0);
-  if (s->ev1) cudaEventDestroy(s->ev1);
-  for (int b = 0; b <= N_BINS; b++)
-    if (s->ev_bin[b]) cudaEventDestroy(s->ev_bin[b]);
-  for (int b = 0; b < N_BINS; b++) {
-    if (s->ev_bin_start[b]) cudaEventDestroy(s->ev_bin_start[b]);
-    if (s->ev_bin_done[b]) cudaEventDestroy(s->ev_bin_done[b]);
-    if (s->ev_gather[b]) cudaEventDestroy(s->ev_gather[b]);
-  }
-  delete s;
-}
-
-void free_overlap(tskv_pages *pg) {
-  void *bufs[] = {pg->d_cg_merge, pg->d_merge_ts, pg->d_mcg_row0, pg->d_mcg_bm0, pg->d_mcg_cg, pg->d_mcg_stream,
-                  pg->d_stream_group, pg->d_stream_first_mcg, pg->d_group_first_stream};
-  for (void *b : bufs) cudaFree(b);
-  pg->d_cg_merge = nullptr; pg->d_merge_ts = nullptr; pg->d_mcg_row0 = nullptr; pg->d_mcg_bm0 = nullptr; pg->d_mcg_cg = nullptr;
-  pg->d_mcg_stream = nullptr; pg->d_stream_group = nullptr; pg->d_stream_first_mcg = nullptr; pg->d_group_first_stream = nullptr;
-  pg->overlap = OverlapPlan{};
-  pg->merge_rows = pg->merge_bm_words = 0;
-  pg->h_mcg_bm0.clear();
-}
-
-template <typename T>
-cudaError_t stream_alloc(tskv_ctx *ctx, T **p, size_t n) {
-  return cudaMallocAsync(reinterpret_cast<void **>(p), std::max<size_t>(n, 1) * sizeof(T), ctx->stream);
-}
-
 // Reads back the device status word; maps it to a message.
 tskv_status fetch_status(tskv_ctx *ctx, int32_t *d_status, unsigned long long *d_err_page) {
   int32_t st = 0;
   unsigned long long pg = 0;
-  if (cudaMemcpyAsync(&st, d_status, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-      cudaMemcpyAsync(&pg, d_err_page, sizeof(pg), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-      cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
+  if (cudaMemcpyAsync(&st, d_status, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream.get()) != cudaSuccess ||
+      cudaMemcpyAsync(&pg, d_err_page, sizeof(pg), cudaMemcpyDeviceToHost, ctx->stream.get()) != cudaSuccess ||
+      cudaStreamSynchronize(ctx->stream.get()) != cudaSuccess) {
     ctx->set_error(std::string("status readback: ") + cudaGetErrorString(cudaGetLastError()));
     return TSKV_ERR_CUDA;
   }
@@ -870,7 +901,8 @@ struct MergePages {
 };
 // Refuses (TSKV_ERR_INVALID_ARG, with the page) a page whose type does not match its query column.
 tskv_status plan_merge_pages(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, MergePages *m) {
-  const OverlapPlan &op = pages->overlap;
+  const OverlapTables &ov = pages->overlap;
+  const OverlapPlan &op = ov.plan;
   m->active.assign(op.mcg_cg.size(), 0);
   for (size_t k = 0; k < op.mcg_cg.size(); k++) {
     const uint32_t cg = op.mcg_cg[k], tp = pages->h_cg_time_page[cg];
@@ -892,8 +924,8 @@ tskv_status plan_merge_pages(tskv_ctx *ctx, const tskv_pages *pages, const tskv_
           }
           any = true;
           m->page.push_back((uint32_t)p);
-          m->row_off.push_back((uint64_t)c * pages->merge_rows + op.mcg_row0[k]);
-          m->bm_off.push_back(((uint64_t)c * pages->merge_bm_words + pages->h_mcg_bm0[k]) * 4);
+          m->row_off.push_back((uint64_t)c * ov.merge_rows + op.mcg_row0[k]);
+          m->bm_off.push_back(((uint64_t)c * ov.merge_bm_words + ov.h_mcg_bm0[k]) * 4);
           m->bytes += pages->h_descs[p].size;
         }
     if (!any) continue;  // a column group without any projected column yields no batch (column_group/mod.rs:43-52)
@@ -910,20 +942,19 @@ tskv_status plan_merge_pages(tskv_ctx *ctx, const tskv_pages *pages, const tskv_
 tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, bool sliding,
                        const ScanLayout &lay, tskv_scan *s, uint64_t *h2d) {
   const uint32_t n_items = pages->n_items;
-  cudaEventCreate(&s->ev0);
-  cudaEventCreate(&s->ev1);
-  for (int b = 0; b <= N_BINS; b++) cudaEventCreate(&s->ev_bin[b]);
+  cudaStream_t st = ctx->stream.get();
+  s->ev0 = new_event();
+  s->ev1 = new_event();
+  for (int b = 0; b <= N_BINS; b++) s->ev_bin[b] = new_event();
   for (int b = 0; b < N_BINS; b++) {
-    cudaEventCreate(&s->ev_bin_start[b]);
-    cudaEventCreate(&s->ev_bin_done[b]);
-    cudaEventCreateWithFlags(&s->ev_gather[b], cudaEventDisableTiming);
+    s->ev_bin_start[b] = new_event();
+    s->ev_bin_done[b] = new_event();
+    s->ev_gather[b] = new_event(cudaEventDisableTiming);
   }
   s->n_series_sel = q->series_ids ? q->n_series : 0;
   cudaError_t e = cudaSuccess;
   if (q->series_ids) {
-    e = stream_alloc(ctx, &s->d_series, q->n_series);
-    if (e == cudaSuccess && q->n_series)
-      e = cudaMemcpyAsync(s->d_series, q->series_ids, (size_t)q->n_series * 4, cudaMemcpyHostToDevice, ctx->stream);
+    e = upload(s->d_series, q->series_ids, q->n_series, st);
     *h2d += (uint64_t)q->n_series * 4;
   }
   if (tg.on) {  // GROUP BY tags: the group map, and the slots in group order for the work-list walk
@@ -941,57 +972,45 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
         std::stable_sort(walk.begin(), walk.end(), [&](uint32_t a, uint32_t b) { return tg.ids[a] < tg.ids[b]; });
       }
     }
-    if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_slot_group, n_slots);
-    if (e == cudaSuccess && n_slots)
-      e = cudaMemcpyAsync(s->d_slot_group, tg.ids, (size_t)n_slots * 4, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess && !walk.empty()) e = stream_alloc(ctx, &s->d_walk, n_slots);
-    if (e == cudaSuccess && !walk.empty())
-      e = cudaMemcpyAsync(s->d_walk, walk.data(), (size_t)n_slots * 4, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = upload(s->d_slot_group, tg.ids, n_slots, st);
+    if (e == cudaSuccess && !walk.empty()) e = upload(s->d_walk, walk.data(), n_slots, st);
     *h2d += (n_slots + walk.size()) * 4;
   }
-  if (e == cudaSuccess && q->series_ids) e = stream_alloc(ctx, &s->d_rank_slot, pages->series.size());
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_bucket, (size_t)2 * N_BINS * q->n_columns * WL_SUB + 1);
+  if (e == cudaSuccess && q->series_ids) e = stream_alloc(s->d_rank_slot, pages->series.size(), st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_bucket, (size_t)2 * N_BINS * q->n_columns * WL_SUB + 1, st);
   {
     // A series with thousands of column groups (one host over a year) is walked by several threads
     const uint64_t n_walk = q->series_ids ? q->n_series : pages->series.size();
     const uint32_t split = plan_walk_split(pages->max_series_cg, n_walk, n_items, WL_THREADS);
     while ((1u << s->walk_split_log2) < split) s->walk_split_log2++;
   }
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_cg_slot, pages->n_cg);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_page, n_items);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_slot, n_items);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_work_qcol, n_items);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_bin_cstart, N_BINS + 2);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_cols, lay.cols.size());
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_outs, lay.outs.size());
+  if (e == cudaSuccess) e = stream_alloc(s->d_cg_slot, pages->n_cg, st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_work_page, n_items, st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_work_slot, n_items, st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_work_qcol, n_items, st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_bin_cstart, N_BINS + 2, st);
+  if (e == cudaSuccess) e = upload(s->d_cols, lay.cols.data(), lay.cols.size(), st);
+  if (e == cudaSuccess) e = upload(s->d_outs, lay.outs.data(), lay.outs.size(), st);
   s->n_means = (uint32_t)lay.means.size();
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_means, lay.means.size());
-  if (e == cudaSuccess && !lay.means.empty())
-    e = cudaMemcpyAsync(s->d_means, lay.means.data(), lay.means.size() * sizeof(MeanExport), cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_state, s->sl.total);
-  if (e == cudaSuccess && sliding) e = stream_alloc(ctx, &s->d_pane_state, s->kern_sl.total);
+  if (e == cudaSuccess) e = upload(s->d_means, lay.means.data(), lay.means.size(), st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_state, s->sl.total, st);
+  if (e == cudaSuccess && sliding) e = stream_alloc(s->d_pane_state, s->kern_sl.total, st);
   s->n_combine = (uint32_t)lay.combine.size();
-  if (e == cudaSuccess && sliding) e = stream_alloc(ctx, &s->d_combine, lay.combine.size());
-  if (e == cudaSuccess && sliding)
-    e = cudaMemcpyAsync(s->d_combine, lay.combine.data(), lay.combine.size() * sizeof(CombineOp), cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess && sliding) e = upload(s->d_combine, lay.combine.data(), lay.combine.size(), st);
   s->preds.n = q->n_predicates;
   for (uint32_t k = 0; k < q->n_predicates; k++) s->preds.p[k] = q->predicates[k];
   if (q->n_predicates) ensure_page_stats(ctx, pages);  // value-statistics pruning (filter_column_groups, reader/chunk.rs:12-50)
-  if (e == cudaSuccess && q->n_predicates) e = stream_alloc(ctx, &s->d_row_keep, (size_t)pages->keep_words);
-  if (e == cudaSuccess) e = stream_alloc(ctx, reinterpret_cast<unsigned long long **>(&s->d_task_counter), AUX_WORDS);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_values, s->layout.n_out * s->layout.n_cells);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_validity, s->layout.validity_bytes + 8);
-  if (e == cudaSuccess)
-    e = cudaMemcpyAsync(s->d_outs, lay.outs.data(), lay.outs.size() * sizeof(OutCol), cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess)
-    e = cudaMemcpyAsync(s->d_cols, lay.cols.data(), lay.cols.size() * sizeof(ColState), cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess && q->n_predicates) e = stream_alloc(s->d_row_keep, (size_t)pages->keep_words, st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_aux, AUX_WORDS, st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_values, s->layout.n_out * s->layout.n_cells, st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_validity, s->layout.validity_bytes + 8, st);
   *h2d += lay.cols.size() * sizeof(ColState) + lay.outs.size() * sizeof(OutCol) + lay.means.size() * sizeof(MeanExport) +
           sizeof(ScanParams) + lay.combine.size() * sizeof(CombineOp);
   if (e != cudaSuccess) {
     ctx->set_error(std::string("scan_prepare: ") + cudaGetErrorString(e));
     return e == cudaErrorMemoryAllocation ? TSKV_ERR_OOM : TSKV_ERR_CUDA;
   }
-  unsigned long long *aux = reinterpret_cast<unsigned long long *>(s->d_task_counter);
+  unsigned long long *aux = s->d_aux.get();
   s->d_status = reinterpret_cast<int32_t *>(aux + AUX_STATUS);
   s->d_err_page = aux + AUX_ERR_PAGE;
   s->d_stats = aux + AUX_STATS;
@@ -1011,40 +1030,36 @@ tskv_status prepare_merge(tskv_ctx *ctx, const tskv_pages *pages, const tskv_que
   s->n_merge_pages = (uint32_t)n_mpages;
   s->merge_page_bytes = mp.bytes;
   s->merge_read_pages = mp.read_pages;
-  cudaError_t e = stream_alloc(ctx, &s->d_mcg_active, n_mcg);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_mcg_active, mp.active.data(), n_mcg, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_mvals, (size_t)q->n_columns * pages->merge_rows);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_mvalid, (size_t)q->n_columns * pages->merge_bm_words);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_mpage, n_mpages);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_mrow_off, n_mpages);
-  if (e == cudaSuccess) e = stream_alloc(ctx, &s->d_mbm_off, n_mpages);
-  if (e == cudaSuccess && n_mpages) {
-    e = cudaMemcpyAsync(s->d_mpage, mp.page.data(), n_mpages * 4, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_mrow_off, mp.row_off.data(), n_mpages * 8, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(s->d_mbm_off, mp.bm_off.data(), n_mpages * 8, cudaMemcpyHostToDevice, ctx->stream);
-  }
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);  // the host vectors go out of scope
+  const OverlapTables &ov = pages->overlap;
+  cudaStream_t stream = ctx->stream.get();
+  cudaError_t e = upload(s->d_mcg_active, mp.active.data(), n_mcg, stream);
+  if (e == cudaSuccess) e = stream_alloc(s->d_mvals, (size_t)q->n_columns * ov.merge_rows, stream);
+  if (e == cudaSuccess) e = stream_alloc(s->d_mvalid, (size_t)q->n_columns * ov.merge_bm_words, stream);
+  if (e == cudaSuccess) e = upload(s->d_mpage, mp.page.data(), n_mpages, stream);
+  if (e == cudaSuccess) e = upload(s->d_mrow_off, mp.row_off.data(), n_mpages, stream);
+  if (e == cudaSuccess) e = upload(s->d_mbm_off, mp.bm_off.data(), n_mpages, stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);  // the host vectors go out of scope
   if (e != cudaSuccess) {
     ctx->set_error(std::string("scan_prepare (merge pass): ") + cudaGetErrorString(e));
     return e == cudaErrorMemoryAllocation ? TSKV_ERR_OOM : TSKV_ERR_CUDA;
   }
   *h2d += n_mcg + n_mpages * 20;
   MergeParams &M = s->merge;
-  M.ts = pages->d_merge_ts;
-  M.mcg_row0 = pages->d_mcg_row0;
-  M.mcg_cg = pages->d_mcg_cg;
-  M.mcg_stream = pages->d_mcg_stream;
-  M.stream_group = pages->d_stream_group;
-  M.stream_first_mcg = pages->d_stream_first_mcg;
-  M.group_first_stream = pages->d_group_first_stream;
-  M.mcg_active = s->d_mcg_active;
-  M.vals = s->d_mvals;
-  M.valid = s->d_mvalid;
-  M.mcg_bm0 = pages->d_mcg_bm0;
-  M.cg_time_page = pages->d_cg_time_page;
-  M.cg_slot = s->d_cg_slot;
-  M.n_rows = pages->merge_rows;
-  M.bm_words = pages->merge_bm_words;
+  M.ts = ov.d_merge_ts.get();
+  M.mcg_row0 = ov.d_mcg_row0.get();
+  M.mcg_cg = ov.d_mcg_cg.get();
+  M.mcg_stream = ov.d_mcg_stream.get();
+  M.stream_group = ov.d_stream_group.get();
+  M.stream_first_mcg = ov.d_stream_first_mcg.get();
+  M.group_first_stream = ov.d_group_first_stream.get();
+  M.mcg_active = s->d_mcg_active.get();
+  M.vals = s->d_mvals.get();
+  M.valid = s->d_mvalid.get();
+  M.mcg_bm0 = ov.d_mcg_bm0.get();
+  M.cg_time_page = pages->d_cg_time_page.get();
+  M.cg_slot = s->d_cg_slot.get();
+  M.n_rows = ov.merge_rows;
+  M.bm_words = ov.merge_bm_words;
   M.n_mcg = (uint32_t)n_mcg;
   M.sel = s->has_sel ? 1u : 0u;
   return TSKV_OK;
@@ -1097,7 +1112,7 @@ void tskvgpu_comm_destroy(tskv_ctx *ctx) {
   if (!ctx || !ctx->comm) return;
   std::lock_guard<std::mutex> lock(ctx->mu);
   cudaSetDevice(ctx->device);
-  cudaStreamSynchronize(ctx->stream);
+  cudaStreamSynchronize(ctx->stream.get());
   nccl_api().CommDestroy(ctx->comm);
   ctx->comm = nullptr;
   ctx->n_ranks = 1;
@@ -1112,9 +1127,10 @@ tskv_status tskvgpu_ctx_create(int32_t device_id, tskv_ctx **out_ctx) {
   if (cudaGetDeviceCount(&n) != cudaSuccess || device_id < 0 || device_id >= n) return TSKV_ERR_CUDA;
   tskv_ctx *ctx = new tskv_ctx();
   ctx->device = device_id;
-  if (cudaSetDevice(device_id) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreate(&ctx->ev0) != cudaSuccess || cudaEventCreate(&ctx->ev1) != cudaSuccess) {
+  cudaStream_t st = nullptr;
+  const bool ok = cudaSetDevice(device_id) == cudaSuccess && cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) == cudaSuccess;
+  ctx->stream.reset(ok ? st : nullptr);
+  if (!ok || !(ctx->ev0 = new_event()) || !(ctx->ev1 = new_event())) {
     delete ctx;
     return TSKV_ERR_CUDA;
   }
@@ -1128,8 +1144,10 @@ tskv_status tskvgpu_ctx_create(int32_t device_id, tskv_ctx **out_ctx) {
       int rank = 0;
       for (int o = 0; o < N_BINS; o++) rank += chunk_cost(o) > chunk_cost(b) ? 1 : 0;
       const int prio = std::min(least, greatest + rank / 2);
-      if (cudaStreamCreateWithPriority(&ctx->bin_stream[b], cudaStreamNonBlocking, prio) != cudaSuccess)
-        cudaStreamCreateWithFlags(&ctx->bin_stream[b], cudaStreamNonBlocking);
+      cudaStream_t bs = nullptr;
+      if (cudaStreamCreateWithPriority(&bs, cudaStreamNonBlocking, prio) != cudaSuccess)
+        cudaStreamCreateWithFlags(&bs, cudaStreamNonBlocking);
+      ctx->bin_stream[b].reset(bs);
     }
   }
   // Dynamic shared memory ceiling of every scan kernel, set ONCE: the attribute belongs to the kernel, not to a launch,
@@ -1163,14 +1181,7 @@ void tskvgpu_ctx_destroy(tskv_ctx *ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   if (ctx->comm) tskvgpu_comm_destroy(ctx);
-  if (ctx->stream) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaStreamDestroy(ctx->stream);
-  }
-  if (ctx->ev0) cudaEventDestroy(ctx->ev0);
-  if (ctx->ev1) cudaEventDestroy(ctx->ev1);
-  for (int b = 0; b < N_BINS; b++)
-    if (ctx->bin_stream[b]) cudaStreamDestroy(ctx->bin_stream[b]);
+  if (ctx->stream) cudaStreamSynchronize(ctx->stream.get());
   delete ctx;
 }
 
@@ -1181,7 +1192,7 @@ tskv_status tskvgpu_get_counters(const tskv_ctx *ctx, tskv_counters *out) {
   *out = ctx->counters;
   return TSKV_OK;
 }
-uint64_t tskvgpu_ctx_stream(const tskv_ctx *ctx) { return ctx ? (uint64_t)(uintptr_t)ctx->stream : 0; }
+uint64_t tskvgpu_ctx_stream(const tskv_ctx *ctx) { return ctx ? (uint64_t)(uintptr_t)ctx->stream.get() : 0; }
 
 // ------------------------------------------------------------------------------------------------
 tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t arena_len,
@@ -1196,7 +1207,7 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
     return TSKV_ERR_INVALID_ARG;
   }
   cudaSetDevice(ctx->device);
-  tskv_pages *pg = new tskv_pages();
+  std::unique_ptr<tskv_pages> pg(new tskv_pages());
   pg->ctx = ctx;
   pg->arena_len = arena_len;
   pg->n_descs = n_descs;
@@ -1254,7 +1265,6 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
     ctx->set_error(st == TSKV_ERR_CRC_MISMATCH ? "TsmPageFileHashCheckFailed: page crc32 mismatch"
                                                : "malformed page descriptor (alignment, bounds, type or reserved != 0)",
                    bad_page.load());
-    delete pg;
     return st;
   }
 
@@ -1265,7 +1275,6 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
     while (i < n_descs) {
       if (pg->h_descs[i].phys_type != TSKV_PT_TIME) {
         ctx->set_error("descriptor table: column group does not start with a time page", (int64_t)i);
-        delete pg;
         return TSKV_ERR_INVALID_ARG;
       }
       cg_time_page.push_back((uint32_t)i);
@@ -1274,7 +1283,6 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
       while (j < n_descs && pg->h_descs[j].phys_type != TSKV_PT_TIME) {
         if (pg->h_descs[j].series_id != pg->h_descs[i].series_id || pg->h_descs[j].num_values != pg->h_descs[i].num_values) {
           ctx->set_error("descriptor table: field page disagrees with its time page", (int64_t)j);
-          delete pg;
           return TSKV_ERR_INVALID_ARG;
         }
         time_page_of[j] = (uint32_t)i;
@@ -1294,7 +1302,6 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
   }
   if (pg->keep_words >= (1ull << 32)) {
     ctx->set_error("too many rows for one arena (2^37)");
-    delete pg;
     return TSKV_ERR_INVALID_ARG;
   }
   // series ranks
@@ -1324,32 +1331,27 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
   }
 
   // ---- device copies ----------------------------------------------------------------------------
-  cudaEventRecord(ctx->ev0, ctx->stream);
-  auto up = [&](auto **dptr, const auto *src, size_t n) -> cudaError_t {
-    cudaError_t e = dev_alloc(dptr, n);
-    if (e != cudaSuccess) return e;
-    if (n) e = cudaMemcpyAsync(*dptr, src, n * sizeof(**dptr), cudaMemcpyHostToDevice, ctx->stream);
-    return e;
-  };
-  cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&pg->d_arena), arena_len + ARENA_SLACK);
-  if (e == cudaSuccess) e = cudaMemsetAsync(pg->d_arena + arena_len, 0, ARENA_SLACK, ctx->stream);
+  cudaStream_t st = ctx->stream.get();
+  cudaEventRecord(ctx->ev0.get(), st);
+  cudaError_t e = dev_alloc(pg->d_arena, arena_len + ARENA_SLACK);
+  if (e == cudaSuccess) e = cudaMemsetAsync(pg->d_arena.get() + arena_len, 0, ARENA_SLACK, ctx->stream.get());
   if (e == cudaSuccess && arena_len && (flags & TSKV_UPLOAD_HOST_RESIDENT)) {
     // pages stay in (page-locked) host memory like the reference's page cache; each scan pulls the
     // selected pages over PCIe itself (k_gather_pages)
     e = cudaHostRegister(const_cast<uint8_t *>(arena), arena_len, cudaHostRegisterMapped | cudaHostRegisterPortable);
-    if (e == cudaSuccess) pg->h_registered = const_cast<uint8_t *>(arena);
+    if (e == cudaSuccess) pg->h_registered.reset(const_cast<uint8_t *>(arena));
     else if (e == cudaErrorHostMemoryAlreadyRegistered) { cudaGetLastError(); e = cudaSuccess; }
     void *dp = nullptr;
     if (e == cudaSuccess) e = cudaHostGetDevicePointer(&dp, const_cast<uint8_t *>(arena), 0);
     pg->h_mapped = static_cast<const uint8_t *>(dp);
   } else if (e == cudaSuccess && arena_len) {
-    e = cudaMemcpyAsync(pg->d_arena, arena, arena_len, cudaMemcpyHostToDevice, ctx->stream);
+    e = cudaMemcpyAsync(pg->d_arena.get(), arena, arena_len, cudaMemcpyHostToDevice, ctx->stream.get());
   }
-  if (e == cudaSuccess) e = up(&pg->d_descs, pg->h_descs.data(), n_descs);
-  if (e == cudaSuccess) e = up(&pg->d_time_page_of, time_page_of.data(), n_descs);
-  if (e == cudaSuccess) e = up(&pg->d_cg_time_page, cg_time_page.data(), pg->n_cg);
-  if (e == cudaSuccess) e = up(&pg->d_cg_series_rank, cg_rank.data(), pg->n_cg);
-  if (e == cudaSuccess) e = up(&pg->d_series_sorted, pg->series.data(), pg->series.size());
+  if (e == cudaSuccess) e = upload(pg->d_descs, pg->h_descs.data(), n_descs, st);
+  if (e == cudaSuccess) e = upload(pg->d_time_page_of, time_page_of.data(), n_descs, st);
+  if (e == cudaSuccess) e = upload(pg->d_cg_time_page, cg_time_page.data(), pg->n_cg, st);
+  if (e == cudaSuccess) e = upload(pg->d_cg_series_rank, cg_rank.data(), pg->n_cg, st);
+  if (e == cudaSuccess) e = upload(pg->d_series_sorted, pg->series.data(), pg->series.size(), st);
   {  // series rank -> its column groups (the selection-driven work list walks a selected series' groups)
     std::vector<uint32_t> start(pg->series.size() + 1, 0), list(pg->n_cg);
     for (uint32_t cg = 0; cg < pg->n_cg; cg++) start[cg_rank[cg] + 1]++;
@@ -1359,14 +1361,14 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
     }
     std::vector<uint32_t> cur(start.begin(), start.end() - 1);
     for (uint32_t cg = 0; cg < pg->n_cg; cg++) list[cur[cg_rank[cg]]++] = cg;
-    if (e == cudaSuccess) e = up(&pg->d_rank_cg_start, start.data(), start.size());
-    if (e == cudaSuccess) e = up(&pg->d_rank_cg, list.data(), list.size());
-    if (e == cudaSuccess) e = up(&pg->d_page_bin, page_bin.data(), n_descs);
+    if (e == cudaSuccess) e = upload(pg->d_rank_cg_start, start.data(), start.size(), st);
+    if (e == cudaSuccess) e = upload(pg->d_rank_cg, list.data(), list.size(), st);
+    if (e == cudaSuccess) e = upload(pg->d_page_bin, page_bin.data(), n_descs, st);
   }
-  if (e == cudaSuccess) e = up(&pg->d_keep_off, keep_off.data(), n_descs);
+  if (e == cudaSuccess) e = upload(pg->d_keep_off, keep_off.data(), n_descs, st);
   if (e == cudaSuccess && (((flags & TSKV_UPLOAD_VERIFY_CRC) && (flags & TSKV_UPLOAD_HOST_RESIDENT)) || (flags & TSKV_UPLOAD_VERIFY_ON_READ))) {
     pg->verify_on_read = true;  // like the reference: every read of a page re-checks its CRC (device side)
-    e = up(&pg->d_crc_tables, crc32_tables(), 2048);
+    e = upload(pg->d_crc_tables, crc32_tables(), 2048, st);
   }
   // ---- restart points of the simple8b / gorilla pages and narrow flags of the simple8b integer pages (pages resident in
   // HBM only; the flags do not depend on TSKV_NO_SKIP) --------------------------------------------------------------
@@ -1390,42 +1392,41 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
       list[kind].push_back((uint32_t)i);
     }
     if (!list[SKIP_KIND_VALUE_S8B].empty()) {
-      e = dev_alloc(&pg->d_narrow, n_descs);
-      if (e == cudaSuccess) e = cudaMemsetAsync(pg->d_narrow, 0, n_descs, ctx->stream);
+      e = dev_alloc(pg->d_narrow, n_descs);
+      if (e == cudaSuccess) e = cudaMemsetAsync(pg->d_narrow.get(), 0, n_descs, st);
     }
     if (n_skip) {
       pg->n_skip = n_skip;
-      if (e == cudaSuccess) e = up(&pg->d_skip_off, skip_off.data(), n_descs);
-      if (e == cudaSuccess) e = dev_alloc(&pg->d_skip, n_skip);
+      if (e == cudaSuccess) e = upload(pg->d_skip_off, skip_off.data(), n_descs, st);
+      if (e == cudaSuccess) e = dev_alloc(pg->d_skip, n_skip);
     }
     const size_t n_list = list[0].size() + list[1].size() + list[2].size();
     if (n_list) {
-      uint32_t *d_list = nullptr;
-      if (e == cudaSuccess) e = cudaMallocAsync(reinterpret_cast<void **>(&d_list), n_list * 4, ctx->stream);
+      async_ptr<uint32_t> d_list;  // freed on the stream after the kernels that read it
+      if (e == cudaSuccess) e = stream_alloc(d_list, n_list, st);
       size_t lo = 0;
       for (int k = 0; k < 3 && e == cudaSuccess; k++) {
         const uint32_t n = (uint32_t)list[k].size();
         if (!n) continue;
-        e = cudaMemcpyAsync(d_list + lo, list[k].data(), (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream);
+        e = cudaMemcpyAsync(d_list.get() + lo, list[k].data(), (size_t)n * 4, cudaMemcpyHostToDevice, st);
         if (e != cudaSuccess) break;
         const uint32_t blocks = (n + SKIP_THREADS - 1) / SKIP_THREADS;
         if (k == SKIP_KIND_TIME_S8B)
-          k_build_skip<SKIP_KIND_TIME_S8B><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream>>>(pg->d_arena, pg->d_descs, d_list + lo, n, pg->d_skip_off, pg->d_skip, nullptr);
+          k_build_skip<SKIP_KIND_TIME_S8B><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream.get()>>>(pg->d_arena.get(), pg->d_descs.get(), d_list.get() + lo, n, pg->d_skip_off.get(), pg->d_skip.get(), nullptr);
         else if (k == SKIP_KIND_VALUE_S8B)
-          k_build_skip<SKIP_KIND_VALUE_S8B><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream>>>(pg->d_arena, pg->d_descs, d_list + lo, n, pg->d_skip_off, pg->d_skip, pg->d_narrow);
+          k_build_skip<SKIP_KIND_VALUE_S8B><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream.get()>>>(pg->d_arena.get(), pg->d_descs.get(), d_list.get() + lo, n, pg->d_skip_off.get(), pg->d_skip.get(), pg->d_narrow.get());
         else
-          k_build_skip<SKIP_KIND_VALUE_GORILLA><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream>>>(pg->d_arena, pg->d_descs, d_list + lo, n, pg->d_skip_off, pg->d_skip, nullptr);
+          k_build_skip<SKIP_KIND_VALUE_GORILLA><<<blocks, SKIP_THREADS, SKIP_SMEM_BYTES, ctx->stream.get()>>>(pg->d_arena.get(), pg->d_descs.get(), d_list.get() + lo, n, pg->d_skip_off.get(), pg->d_skip.get(), nullptr);
         lo += n;
       }
       if (e == cudaSuccess) e = cudaGetLastError();
       // the page lists are read by kernels still in flight: host vectors stay alive until the sync below
-      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-      if (d_list) cudaFreeAsync(d_list, ctx->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     }
     if (e == cudaSuccess && pg->d_narrow) {
       std::vector<uint8_t> narrow(n_descs);
-      e = cudaMemcpyAsync(narrow.data(), pg->d_narrow, n_descs, cudaMemcpyDeviceToHost, ctx->stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+      e = cudaMemcpyAsync(narrow.data(), pg->d_narrow.get(), n_descs, cudaMemcpyDeviceToHost, ctx->stream.get());
+      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream.get());
       uint64_t n_narrow[N_BINS] = {0};
       for (uint64_t p = 0; p < n_descs; p++)
         if (pg->h_descs[p].phys_type != TSKV_PT_TIME) n_narrow[page_bin[p]] += narrow[p];
@@ -1433,17 +1434,17 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
         pg->h_bin_narrow[b] = n_narrow[b] == 0 ? NARROW_NONE : n_narrow[b] == pg->h_bin_pages[b] ? NARROW_ALL : NARROW_SOME;
     }
   }
-  cudaEventRecord(ctx->ev1, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  cudaEventRecord(ctx->ev1.get(), ctx->stream.get());
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream.get());
   if (e != cudaSuccess) {
     ctx->set_error(std::string("upload: ") + cudaGetErrorString(e));
-    tskvgpu_pages_destroy(nullptr, pg);
+    tskvgpu_pages_destroy(nullptr, pg.release());
     return e == cudaErrorMemoryAllocation ? TSKV_ERR_OOM : TSKV_ERR_CUDA;
   }
   float ms = 0;
-  cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
+  cudaEventElapsedTime(&ms, ctx->ev0.get(), ctx->ev1.get());
   ctx->counters.elapsed_h2d_ms = ms;
-  *out_pages = pg;
+  *out_pages = pg.release();
   return TSKV_OK;
 }
 
@@ -1451,28 +1452,7 @@ void tskvgpu_pages_destroy(tskv_ctx *ctx, tskv_pages *pg) {
   (void)ctx;
   if (!pg) return;
   if (pg->ctx) cudaSetDevice(pg->ctx->device);
-  if (pg->ctx && pg->ctx->stream) cudaStreamSynchronize(pg->ctx->stream);
-  if (pg->h_registered) cudaHostUnregister(pg->h_registered);
-  cudaFree(pg->d_arena);
-  cudaFree(pg->d_skip_off);
-  cudaFree(pg->d_skip);
-  cudaFree(pg->d_narrow);
-  free_overlap(pg);
-  cudaFree(pg->d_descs);
-  cudaFree(pg->d_time_page_of);
-  cudaFree(pg->d_cg_time_page);
-  cudaFree(pg->d_cg_series_rank);
-  cudaFree(pg->d_series_sorted);
-  cudaFree(pg->d_rank_cg_start);
-  cudaFree(pg->d_rank_cg);
-  cudaFree(pg->d_page_bin);
-  cudaFree(pg->d_page_stats);
-  cudaFree(pg->d_crc_tables);
-  cudaFree(pg->d_tomb_keys);
-  cudaFree(pg->d_tomb_off);
-  cudaFree(pg->d_tomb_ranges);
-  cudaFree(pg->d_cg_bounds);
-  cudaFree(pg->d_keep_off);
+  if (pg->ctx && pg->ctx->stream) cudaStreamSynchronize(pg->ctx->stream.get());
   delete pg;
 }
 
@@ -1483,8 +1463,7 @@ tskv_status tskvgpu_pages_set_time_bounds(tskv_ctx *ctx, tskv_pages *pg, const t
   std::lock_guard<std::mutex> lock(ctx->mu);
   ctx->set_error("");
   CU_TRY(ctx, cudaSetDevice(ctx->device));
-  if (!pg->d_cg_bounds) CU_TRY(ctx, cudaMalloc(reinterpret_cast<void **>(&pg->d_cg_bounds), std::max<size_t>(n, 1) * sizeof(tskv_time_range)));
-  CU_TRY(ctx, cudaMemcpy(pg->d_cg_bounds, bounds, n * sizeof(tskv_time_range), cudaMemcpyHostToDevice));
+  CU_TRY(ctx, fill_table(pg->d_cg_bounds, bounds, n, ctx->stream.get()));
   int64_t lo = INT64_MAX, hi = INT64_MIN;
   for (uint64_t i = 0; i < n; i++)
     if (bounds[i].min_ts <= bounds[i].max_ts) {
@@ -1521,9 +1500,7 @@ tskv_status tskvgpu_pages_set_value_stats(tskv_ctx *ctx, tskv_pages *pg, const t
     keys[2 * i] = kmin;
     keys[2 * i + 1] = kmax;
   }
-  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  if (!pg->d_page_stats) CU_TRY(ctx, cudaMalloc(reinterpret_cast<void **>(&pg->d_page_stats), std::max<size_t>(keys.size(), 1) * 8));
-  CU_TRY(ctx, cudaMemcpy(pg->d_page_stats, keys.data(), keys.size() * 8, cudaMemcpyHostToDevice));
+  CU_TRY(ctx, fill_table(pg->d_page_stats, keys.data(), keys.size(), ctx->stream.get()));
   return TSKV_OK;
 }
 
@@ -1535,8 +1512,8 @@ tskv_status tskvgpu_pages_set_chunk_files(tskv_ctx *ctx, tskv_pages *pg, const u
     std::lock_guard<std::mutex> lock(ctx->mu);
     ctx->set_error("");
     CU_TRY(ctx, cudaSetDevice(ctx->device));
-    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    free_overlap(pg);
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream.get()));
+    pg->overlap = OverlapTables{};
     pg->chunk_epoch++;
     if (n_cg == 0) return TSKV_OK;
     ensure_time_bounds(ctx, pg);  // ColumnGroup::time_range() of every group (the caller's, or one pass over the time pages)
@@ -1545,77 +1522,77 @@ tskv_status tskvgpu_pages_set_chunk_files(tskv_ctx *ctx, tskv_pages *pg, const u
       return TSKV_ERR_CUDA;
     }
     pg->h_cg_bounds.resize(pg->n_cg);
-    CU_TRY(ctx, cudaMemcpy(pg->h_cg_bounds.data(), pg->d_cg_bounds, (size_t)pg->n_cg * sizeof(tskv_time_range), cudaMemcpyDeviceToHost));
+    CU_TRY(ctx, cudaMemcpy(pg->h_cg_bounds.data(), pg->d_cg_bounds.get(), (size_t)pg->n_cg * sizeof(tskv_time_range), cudaMemcpyDeviceToHost));
     std::vector<uint32_t> cg_series(pg->n_cg), cg_rows(pg->n_cg);
     for (uint32_t cg = 0; cg < pg->n_cg; cg++) {
       cg_series[cg] = pg->h_descs[pg->h_cg_time_page[cg]].series_id;
       cg_rows[cg] = pg->h_descs[pg->h_cg_time_page[cg]].num_values;
     }
-    plan_overlap_groups(pg->n_cg, cg_series.data(), cg_rows.data(), pg->h_cg_bounds.data(), cg_file_id, &pg->overlap);
-    const OverlapPlan &op = pg->overlap;
+    // built here and published only when complete: a failed call leaves the page set without an overlap plan
+    OverlapTables t;
+    plan_overlap_groups(pg->n_cg, cg_series.data(), cg_rows.data(), pg->h_cg_bounds.data(), cg_file_id, &t.plan);
+    const OverlapPlan &op = t.plan;
     const size_t n_mcg = op.mcg_cg.size();
-    if (n_mcg == 0) return TSKV_OK;  // no two chunks of a series overlap: nothing to merge
+    if (n_mcg == 0) {  // no two chunks of a series overlap: nothing to merge
+      pg->overlap = std::move(t);
+      return TSKV_OK;
+    }
     for (uint32_t cg : op.mcg_cg)
       if (pg->h_time_has_nulls[pg->h_cg_time_page[cg]] || dk_is_error(pg->h_descs[pg->h_cg_time_page[cg]].reserved)) {
         ctx->set_error("set_chunk_files: a time page of an overlapping chunk holds NULLs or does not decode", pg->h_cg_time_page[cg]);
-        free_overlap(pg);
         return TSKV_ERR_UNSUPPORTED;
       }
-    pg->merge_rows = op.mcg_row0.back();
-    pg->h_mcg_bm0.assign(n_mcg, 0);
+    t.merge_rows = op.mcg_row0.back();
+    t.h_mcg_bm0.assign(n_mcg, 0);
     uint64_t w = 0;
     for (size_t k = 0; k < n_mcg; k++) {
-      pg->h_mcg_bm0[k] = w;
+      t.h_mcg_bm0[k] = w;
       w += ((op.mcg_row0[k + 1] - op.mcg_row0[k] + 63) / 64) * 2;  // 8-byte padded bitmaps, in 32-bit words
     }
-    pg->merge_bm_words = w;
-    auto up = [&](auto **dptr, const auto &vec) -> cudaError_t {
-      cudaError_t e = dev_alloc(dptr, vec.size());
-      if (e == cudaSuccess && !vec.empty()) e = cudaMemcpy(*dptr, vec.data(), vec.size() * sizeof(vec[0]), cudaMemcpyHostToDevice);
-      return e;
-    };
-    cudaError_t e = up(&pg->d_cg_merge, op.cg_merge);
-    if (e == cudaSuccess) e = up(&pg->d_mcg_row0, op.mcg_row0);
-    if (e == cudaSuccess) e = up(&pg->d_mcg_bm0, pg->h_mcg_bm0);
-    if (e == cudaSuccess) e = up(&pg->d_mcg_cg, op.mcg_cg);
-    if (e == cudaSuccess) e = up(&pg->d_mcg_stream, op.mcg_stream);
-    if (e == cudaSuccess) e = up(&pg->d_stream_group, op.stream_group);
-    if (e == cudaSuccess) e = up(&pg->d_stream_first_mcg, op.stream_first_mcg);
-    if (e == cudaSuccess) e = up(&pg->d_group_first_stream, op.group_first_stream);
-    if (e == cudaSuccess) e = dev_alloc(&pg->d_merge_ts, (size_t)pg->merge_rows);
+    t.merge_bm_words = w;
+    cudaStream_t st = ctx->stream.get();
+    cudaError_t e = upload(t.d_cg_merge, op.cg_merge.data(), op.cg_merge.size(), st);
+    if (e == cudaSuccess) e = upload(t.d_mcg_row0, op.mcg_row0.data(), op.mcg_row0.size(), st);
+    if (e == cudaSuccess) e = upload(t.d_mcg_bm0, t.h_mcg_bm0.data(), t.h_mcg_bm0.size(), st);
+    if (e == cudaSuccess) e = upload(t.d_mcg_cg, op.mcg_cg.data(), op.mcg_cg.size(), st);
+    if (e == cudaSuccess) e = upload(t.d_mcg_stream, op.mcg_stream.data(), op.mcg_stream.size(), st);
+    if (e == cudaSuccess) e = upload(t.d_stream_group, op.stream_group.data(), op.stream_group.size(), st);
+    if (e == cudaSuccess) e = upload(t.d_stream_first_mcg, op.stream_first_mcg.data(), op.stream_first_mcg.size(), st);
+    if (e == cudaSuccess) e = upload(t.d_group_first_stream, op.group_first_stream.data(), op.group_first_stream.size(), st);
+    if (e == cudaSuccess) e = dev_alloc(t.d_merge_ts, (size_t)t.merge_rows);
     // the merge rows' timestamps: the time pages of the merge column groups, decoded in merge-row order
     std::vector<uint32_t> tpages(n_mcg);
     std::vector<uint64_t> row_off(n_mcg), bm_off(n_mcg);
     for (size_t k = 0; k < n_mcg; k++) {
       tpages[k] = pg->h_cg_time_page[op.mcg_cg[k]];
       row_off[k] = op.mcg_row0[k];
-      bm_off[k] = pg->h_mcg_bm0[k] * 4;
+      bm_off[k] = t.h_mcg_bm0[k] * 4;
     }
-    uint32_t *d_list = nullptr;
-    uint64_t *d_ro = nullptr, *d_bo = nullptr;
-    uint8_t *d_bm = nullptr;
-    int32_t *d_st = nullptr;
-    if (e == cudaSuccess) e = up(&d_list, tpages);
-    if (e == cudaSuccess) e = up(&d_ro, row_off);
-    if (e == cudaSuccess) e = up(&d_bo, bm_off);
-    if (e == cudaSuccess) e = dev_alloc(&d_bm, (size_t)pg->merge_bm_words * 4);
-    if (e == cudaSuccess) e = dev_alloc(&d_st, 8);  // status | err page (2 x 8 bytes) | points
+    dev_ptr<uint32_t> d_list;
+    dev_ptr<uint64_t> d_ro, d_bo;
+    dev_ptr<uint8_t> d_bm;
+    dev_ptr<int32_t> d_st;
+    if (e == cudaSuccess) e = upload(d_list, tpages.data(), n_mcg, st);
+    if (e == cudaSuccess) e = upload(d_ro, row_off.data(), n_mcg, st);
+    if (e == cudaSuccess) e = upload(d_bo, bm_off.data(), n_mcg, st);
+    if (e == cudaSuccess) e = dev_alloc(d_bm, (size_t)t.merge_bm_words * 4);
+    if (e == cudaSuccess) e = dev_alloc(d_st, 8);  // status | err page (2 x 8 bytes) | points
     tskv_status ret = TSKV_OK;
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_st, 0, 32, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_st.get(), 0, 32, st);
     if (e == cudaSuccess) {
-      unsigned long long *aux = reinterpret_cast<unsigned long long *>(d_st);
+      unsigned long long *aux = reinterpret_cast<unsigned long long *>(d_st.get());
       const uint32_t blocks = (uint32_t)((n_mcg * 32 + DECODE_THREADS - 1) / DECODE_THREADS);
-      k_decode_warp<<<blocks, DECODE_THREADS, 0, ctx->stream>>>(pg->h_mapped ? pg->h_mapped : pg->d_arena, pg->d_descs, 0, d_list, (uint32_t)n_mcg,
-                                                               d_ro, d_bo, reinterpret_cast<uint64_t *>(pg->d_merge_ts), d_bm, d_st, aux + 1, aux + 2);
+      k_decode_warp<<<blocks, DECODE_THREADS, 0, st>>>(pg->h_mapped ? pg->h_mapped : pg->d_arena.get(), pg->d_descs.get(), 0, d_list.get(),
+                                                       (uint32_t)n_mcg, d_ro.get(), d_bo.get(), reinterpret_cast<uint64_t *>(t.d_merge_ts.get()),
+                                                       d_bm.get(), d_st.get(), aux + 1, aux + 2);
       e = cudaGetLastError();
-      if (e == cudaSuccess) ret = fetch_status(ctx, d_st, aux + 1);
+      if (e == cudaSuccess) ret = fetch_status(ctx, d_st.get(), aux + 1);
     }
-    cudaFree(d_list); cudaFree(d_ro); cudaFree(d_bo); cudaFree(d_bm); cudaFree(d_st);
     if (e != cudaSuccess || ret != TSKV_OK) {
       if (e != cudaSuccess) ctx->set_error(std::string("set_chunk_files: ") + cudaGetErrorString(e));
-      free_overlap(pg);
       return e == cudaErrorMemoryAllocation ? TSKV_ERR_OOM : (e != cudaSuccess ? TSKV_ERR_CUDA : ret);
     }
+    pg->overlap = std::move(t);
   }
   return TSKV_OK;
 }
@@ -1650,25 +1627,19 @@ tskv_status tskvgpu_pages_set_tombstones(tskv_ctx *ctx, tskv_pages *pg, const ts
     ranges.push_back(kr.second);
   }
   off.push_back((uint32_t)ranges.size());
-  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // no scan of this page set may be in flight
-  cudaFree(pg->d_tomb_keys);
-  cudaFree(pg->d_tomb_off);
-  cudaFree(pg->d_tomb_ranges);
-  pg->d_tomb_keys = nullptr;
-  pg->d_tomb_off = nullptr;
-  pg->d_tomb_ranges = nullptr;
-  pg->n_tomb_keys = (uint32_t)keys.size();
-  pg->n_tomb_global = n_global;
-  pg->n_tomb_ranges = (uint32_t)ranges.size();
-  pg->tomb_epoch++;
+  TombTables t;
+  t.n_keys = (uint32_t)keys.size();
+  t.n_global = n_global;
+  t.n_ranges = (uint32_t)ranges.size();
+  cudaStream_t st = ctx->stream.get();
   if (!ranges.empty()) {
-    CU_TRY(ctx, cudaMalloc(&pg->d_tomb_ranges, ranges.size() * sizeof(tskv_time_range)));
-    CU_TRY(ctx, cudaMemcpy(pg->d_tomb_ranges, ranges.data(), ranges.size() * sizeof(tskv_time_range), cudaMemcpyHostToDevice));
-    CU_TRY(ctx, cudaMalloc(&pg->d_tomb_keys, std::max<size_t>(keys.size(), 1) * 8));
-    if (!keys.empty()) CU_TRY(ctx, cudaMemcpy(pg->d_tomb_keys, keys.data(), keys.size() * 8, cudaMemcpyHostToDevice));
-    CU_TRY(ctx, cudaMalloc(&pg->d_tomb_off, off.size() * 4));
-    CU_TRY(ctx, cudaMemcpy(pg->d_tomb_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    CU_TRY(ctx, upload(t.ranges, ranges.data(), ranges.size(), st));
+    CU_TRY(ctx, upload(t.keys, keys.data(), keys.size(), st));
+    CU_TRY(ctx, upload(t.off, off.data(), off.size(), st));
   }
+  CU_TRY(ctx, cudaStreamSynchronize(st));  // the tables are filled and no scan of this page set is in flight
+  pg->tomb = std::move(t);
+  pg->tomb_epoch++;
   return TSKV_OK;
 }
 
@@ -1689,58 +1660,48 @@ tskv_status tskvgpu_decode_pages(tskv_ctx *ctx, const tskv_pages *pages, uint64_
     rows += pages->h_descs[first_page + i].num_values;
     bm += ((uint64_t)pages->h_descs[first_page + i].num_values + 63) / 64 * 8;
   }
-  uint64_t *d_row_off = nullptr, *d_bm_off = nullptr, *d_vals = nullptr;
-  uint8_t *d_valid = nullptr;
-  int32_t *d_status = nullptr;
-  unsigned long long *d_aux = nullptr;  // [0] err_page, [1] points
+  cudaStream_t st = ctx->stream.get();
+  dev_ptr<uint64_t> d_row_off, d_bm_off, d_vals;
+  dev_ptr<uint8_t> d_valid;
+  dev_ptr<int32_t> d_status;
+  dev_ptr<unsigned long long> d_aux;  // [0] err_page, [1] points
   tskv_status ret = TSKV_OK;
-  auto cleanup = [&]() {
-    cudaFree(d_row_off);
-    cudaFree(d_bm_off);
-    cudaFree(d_vals);
-    cudaFree(d_valid);
-    cudaFree(d_status);
-    cudaFree(d_aux);
-  };
-  cudaError_t e = dev_alloc(&d_row_off, n_pages);
-  if (e == cudaSuccess) e = dev_alloc(&d_bm_off, n_pages);
-  if (e == cudaSuccess) e = dev_alloc(&d_vals, rows);
-  if (e == cudaSuccess) e = dev_alloc(&d_valid, bm);
-  if (e == cudaSuccess) e = dev_alloc(&d_status, 1);
-  if (e == cudaSuccess) e = dev_alloc(&d_aux, 2);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_row_off, row_off.data(), n_pages * 8, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_bm_off, bm_off.data(), n_pages * 8, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_status, 0, 4, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_aux, 0, 16, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_vals, 0, std::max<uint64_t>(rows, 1) * 8, ctx->stream);
+  cudaError_t e = upload(d_row_off, row_off.data(), n_pages, st);
+  if (e == cudaSuccess) e = upload(d_bm_off, bm_off.data(), n_pages, st);
+  if (e == cudaSuccess) e = dev_alloc(d_vals, rows);
+  if (e == cudaSuccess) e = dev_alloc(d_valid, bm);
+  if (e == cudaSuccess) e = dev_alloc(d_status, 1);
+  if (e == cudaSuccess) e = dev_alloc(d_aux, 2);
+  if (e == cudaSuccess) e = cudaMemsetAsync(d_status.get(), 0, 4, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(d_aux.get(), 0, 16, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(d_vals.get(), 0, std::max<uint64_t>(rows, 1) * 8, st);
   if (e == cudaSuccess) {
-    cudaEventRecord(ctx->ev0, ctx->stream);
+    cudaEventRecord(ctx->ev0.get(), ctx->stream.get());
     uint32_t blocks = (uint32_t)((n_pages * 32 + DECODE_THREADS - 1) / DECODE_THREADS);  // one warp per page
     // host-resident page sets: d_arena is only the scans' gather target, the pages are read through the mapped host range
-    k_decode_warp<<<blocks, DECODE_THREADS, 0, ctx->stream>>>(pages->h_mapped ? pages->h_mapped : pages->d_arena, pages->d_descs, first_page, nullptr, (uint32_t)n_pages,
-                                                        d_row_off, d_bm_off, d_vals, d_valid, d_status, d_aux, d_aux + 1);
-    cudaEventRecord(ctx->ev1, ctx->stream);
+    k_decode_warp<<<blocks, DECODE_THREADS, 0, ctx->stream.get()>>>(pages->h_mapped ? pages->h_mapped : pages->d_arena.get(), pages->d_descs.get(), first_page, nullptr, (uint32_t)n_pages,
+                                                        d_row_off.get(), d_bm_off.get(), d_vals.get(), d_valid.get(), d_status.get(), d_aux.get(), d_aux.get() + 1);
+    cudaEventRecord(ctx->ev1.get(), ctx->stream.get());
     e = cudaGetLastError();
   }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out_values, d_vals, rows * 8, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out_validity, d_valid, bm, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out_values, d_vals.get(), rows * 8, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out_validity, d_valid.get(), bm, cudaMemcpyDeviceToHost, st);
   unsigned long long points = 0;
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&points, d_aux + 1, 8, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&points, d_aux.get() + 1, 8, cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) {
-    ret = fetch_status(ctx, d_status, d_aux);
+    ret = fetch_status(ctx, d_status.get(), d_aux.get());
   } else {
     ctx->set_error(std::string("decode: ") + cudaGetErrorString(e));
     ret = e == cudaErrorMemoryAllocation ? TSKV_ERR_OOM : TSKV_ERR_CUDA;
   }
   if (ret == TSKV_OK) {
     float ms = 0;
-    cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
+    cudaEventElapsedTime(&ms, ctx->ev0.get(), ctx->ev1.get());
     ctx->counters.elapsed_scan_ms = ms;
     ctx->counters.points_decoded = points;
     ctx->counters.kernel_launches = 1;
     ctx->counters.page_read_count = n_pages;
   }
-  cleanup();
   return ret;
 }
 
@@ -1790,20 +1751,20 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   s->kern_sl = lay.kern_sl;
   uint64_t h2d = 0;
   if ((st = alloc_scan(ctx, pages, q, tg, slide != 0, lay, s, &h2d)) != TSKV_OK) {
-    free_scan(s);
+    delete s;
     return st;
   }
   ScanParams &P = s->params;
-  P.arena = pages->d_arena;
-  P.descs = pages->d_descs;
-  P.time_page_of = pages->d_time_page_of;
-  P.work_page = s->d_work_page;
-  P.work_slot = s->d_work_slot;
-  P.work_qcol = s->d_work_qcol;
-  P.bin_cstart = s->d_bin_cstart;
-  P.cols = s->d_cols;
-  P.state = slide ? s->d_pane_state : s->d_state;
-  P.task_counter = s->d_task_counter;
+  P.arena = pages->d_arena.get();
+  P.descs = pages->d_descs.get();
+  P.time_page_of = pages->d_time_page_of.get();
+  P.work_page = s->d_work_page.get();
+  P.work_slot = s->d_work_slot.get();
+  P.work_qcol = s->d_work_qcol.get();
+  P.bin_cstart = s->d_bin_cstart.get();
+  P.cols = s->d_cols.get();
+  P.state = slide ? s->d_pane_state.get() : s->d_state.get();
+  P.task_counter = reinterpret_cast<uint32_t *>(s->d_aux.get());
   P.status = s->d_status;
   P.err_page = s->d_err_page;
   P.stats = s->d_stats;
@@ -1826,29 +1787,29 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   P.n_buckets = s->n_panes;
   P.group_by_series = q->group_by_series;
   P.n_cells = L.n_groups * s->n_panes;
-  P.slot_group = s->d_slot_group;
+  P.slot_group = s->d_slot_group.get();
   P.slot_bits = slot_bits;
   P.slot_max = slot_bits ? (uint32_t)((1ull << slot_bits) - 1) : 0;
   P.rel_base = rel_base;
   P.use_smem = lay.use_smem;
   P.smem_words = lay.smem_words;
   P.n_cols = q->n_columns;
-  P.row_keep = s->d_row_keep;
-  P.keep_off = pages->d_keep_off;
-  P.skip_off = pages->d_skip_off;
-  P.page_narrow = pages->d_narrow;
-  P.skip = pages->d_skip;
-  P.has_tomb = pages->n_tomb_ranges ? 1u : 0u;
-  P.tomb_keys = pages->d_tomb_keys;
-  P.tomb_off = pages->d_tomb_off;
-  P.tomb_ranges = pages->d_tomb_ranges;
-  P.n_tomb_keys = pages->n_tomb_keys;
-  P.n_tomb_global = pages->n_tomb_global;
+  P.row_keep = s->d_row_keep.get();
+  P.keep_off = pages->d_keep_off.get();
+  P.skip_off = pages->d_skip_off.get();
+  P.page_narrow = pages->d_narrow.get();
+  P.skip = pages->d_skip.get();
+  P.has_tomb = pages->tomb.n_ranges ? 1u : 0u;
+  P.tomb_keys = pages->tomb.keys.get();
+  P.tomb_off = pages->tomb.off.get();
+  P.tomb_ranges = pages->tomb.ranges.get();
+  P.n_tomb_keys = pages->tomb.n_keys;
+  P.n_tomb_global = pages->tomb.n_global;
   s->tomb_epoch = pages->tomb_epoch;
   plan_grids(ctx, pages, q, has_sel, P.smem_words, P.has_tomb, s->grid, s->occ, P.bin_parts, P.bin_part_rows);
   s->chunk_epoch = pages->chunk_epoch;
-  if (pages->merge_rows && (st = prepare_merge(ctx, pages, q, s, &h2d)) != TSKV_OK) {
-    free_scan(s);
+  if (pages->overlap.merge_rows && (st = prepare_merge(ctx, pages, q, s, &h2d)) != TSKV_OK) {
+    delete s;
     return st;
   }
   ctx->counters.h2d_bytes = h2d;
@@ -1899,13 +1860,13 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     ctx->set_error("the page set's chunk files changed after this scan was prepared", -1);
     return TSKV_ERR_INVALID_ARG;
   }
-  if (!capturing) cudaEventRecord(s->ev0, ctx->stream);
-  unsigned long long *aux = reinterpret_cast<unsigned long long *>(s->d_task_counter);
+  if (!capturing) cudaEventRecord(s->ev0.get(), ctx->stream.get());
+  unsigned long long *aux = s->d_aux.get();
   uint64_t launches = 0;
   {  // state identities + the pass's scratch (task counters / status / counters, bin starts, work-list buckets): one launch
     const uint32_t init_blocks = (uint32_t)std::min<uint64_t>((s->kern_sl.total + 255) / 256, 4096);
-    k_init_state<<<std::max(1u, init_blocks), 256, 0, ctx->stream>>>(s->params.state, s->kern_sl, aux, AUX_WORDS, s->d_bin_cstart, N_BINS + 2,
-                                                                   s->d_bucket, N_BINS * s->n_cols * WL_SUB);
+    k_init_state<<<std::max(1u, init_blocks), 256, 0, ctx->stream.get()>>>(s->params.state, s->kern_sl, aux, AUX_WORDS, s->d_bin_cstart.get(), N_BINS + 2,
+                                                                   s->d_bucket.get(), N_BINS * s->n_cols * WL_SUB);
     launches++;
   }
   // slot of every column group: the row filter and the merge pass need it per GROUP; the work list finds a selected
@@ -1913,73 +1874,73 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
   const bool need_cg_slot = s->preds.n || (s->merge.n_rows && s->n_merge_pages);
   if (pages->n_cg && need_cg_slot) {
     if (s->d_rank_slot) {
-      CU_TRY(ctx, cudaMemsetAsync(s->d_rank_slot, 0xff, pages->series.size() * 4, ctx->stream));
+      CU_TRY(ctx, cudaMemsetAsync(s->d_rank_slot.get(), 0xff, pages->series.size() * 4, ctx->stream.get()));
       if (s->n_series_sel) {
-        k_select_ids<<<(s->n_series_sel + 255) / 256, 256, 0, ctx->stream>>>(pages->d_series_sorted, (uint32_t)pages->series.size(), s->d_series,
-                                                                         s->n_series_sel, s->d_rank_slot);
+        k_select_ids<<<(s->n_series_sel + 255) / 256, 256, 0, ctx->stream.get()>>>(pages->d_series_sorted.get(), (uint32_t)pages->series.size(), s->d_series.get(),
+                                                                         s->n_series_sel, s->d_rank_slot.get());
         launches++;
       }
     }
-    k_select_cg<<<(pages->n_cg + 255) / 256, 256, 0, ctx->stream>>>(pages->n_cg, s->d_rank_slot, pages->d_cg_series_rank, s->d_cg_slot);
+    k_select_cg<<<(pages->n_cg + 255) / 256, 256, 0, ctx->stream.get()>>>(pages->n_cg, s->d_rank_slot.get(), pages->d_cg_series_rank.get(), s->d_cg_slot.get());
     launches++;
   }
   if (s->preds.n && pages->n_cg) {  // row filter: keep bits of every selected column group (host-resident pages: read in place)
-    k_row_filter<<<(pages->n_cg + 127) / 128, 128, 0, ctx->stream>>>(pages->h_mapped ? pages->h_mapped : pages->d_arena, pages->d_descs,
-                                                                     pages->n_descs, pages->d_cg_time_page, pages->n_cg, s->d_cg_slot,
-                                                                     s->preds, pages->d_keep_off, s->d_row_keep, s->d_status, s->d_err_page);
+    k_row_filter<<<(pages->n_cg + 127) / 128, 128, 0, ctx->stream.get()>>>(pages->h_mapped ? pages->h_mapped : pages->d_arena.get(), pages->d_descs.get(),
+                                                                     pages->n_descs, pages->d_cg_time_page.get(), pages->n_cg, s->d_cg_slot.get(),
+                                                                     s->preds, pages->d_keep_off.get(), s->d_row_keep.get(), s->d_status, s->d_err_page);
     launches++;
   }
   if (n_items) {
     WorkListArgs A{};
-    A.descs = pages->d_descs;
+    A.descs = pages->d_descs.get();
     A.n_descs = pages->n_descs;
-    A.cg_time_page = pages->d_cg_time_page;
+    A.cg_time_page = pages->d_cg_time_page.get();
     A.n_cg = pages->n_cg;
-    A.rank_cg_start = pages->d_rank_cg_start;
-    A.rank_cg = pages->d_rank_cg;
-    A.page_bin = pages->d_page_bin;
+    A.rank_cg_start = pages->d_rank_cg_start.get();
+    A.rank_cg = pages->d_rank_cg.get();
+    A.page_bin = pages->d_page_bin.get();
     // narrow pages apart only where a bin holds both kinds (NARROW_SOME kernels choose per chunk)
     A.page_narrow = std::any_of(pages->h_bin_narrow, pages->h_bin_narrow + N_BINS, [](uint8_t m) { return m == NARROW_SOME; })
-                        ? pages->d_narrow : nullptr;
-    A.set_series = pages->d_series_sorted;
+                        ? pages->d_narrow.get() : nullptr;
+    A.set_series = pages->d_series_sorted.get();
     A.n_set_series = (uint32_t)pages->series.size();
-    A.series_ids = s->d_series;
+    A.series_ids = s->d_series.get();
     A.n_sel = s->d_series ? s->n_series_sel : (uint32_t)pages->series.size();
     A.split_log2 = s->walk_split_log2;
-    A.walk = s->d_walk;
-    A.cols = s->d_cols;
+    A.walk = s->d_walk.get();
+    A.cols = s->d_cols.get();
     A.n_cols = s->n_cols;
-    A.cg_bounds = s->prune.n ? pages->d_cg_bounds : nullptr;
+    A.cg_bounds = s->prune.n ? pages->d_cg_bounds.get() : nullptr;
     A.prune = s->prune;
-    A.cg_merge = pages->d_cg_merge;
-    A.page_stats = s->preds.n ? pages->d_page_stats : nullptr;
+    A.cg_merge = pages->overlap.d_cg_merge.get();
+    A.page_stats = s->preds.n ? pages->d_page_stats.get() : nullptr;
     A.preds = s->preds;
     const uint32_t n_buckets = N_BINS * s->n_cols * WL_SUB;
-    A.bucket_count = s->d_bucket;
-    A.bucket_off = s->d_bucket + n_buckets;
-    A.work_page = s->d_work_page;
-    A.work_slot = s->d_work_slot;
-    A.work_qcol = s->d_work_qcol;
+    A.bucket_count = s->d_bucket.get();
+    A.bucket_off = s->d_bucket.get() + n_buckets;
+    A.work_page = s->d_work_page.get();
+    A.work_slot = s->d_work_slot.get();
+    A.work_qcol = s->d_work_qcol.get();
     A.counters = s->d_counters;
     A.status = s->d_status;
     const uint32_t wblocks = std::max(1u, (uint32_t)((((uint64_t)A.n_sel << A.split_log2) + WL_THREADS - 1) / WL_THREADS));
-    if (A.n_sel) k_worklist_count<<<wblocks, WL_THREADS, n_buckets * 4, ctx->stream>>>(A);
-    k_worklist_offsets<<<1, 256, 0, ctx->stream>>>(s->d_bucket, s->d_bucket + n_buckets, s->n_cols * WL_SUB, s->d_bin_cstart);
-    if (A.n_sel) k_worklist_emit<<<wblocks, WL_THREADS, 2 * n_buckets * 4, ctx->stream>>>(A);
+    if (A.n_sel) k_worklist_count<<<wblocks, WL_THREADS, n_buckets * 4, ctx->stream.get()>>>(A);
+    k_worklist_offsets<<<1, 256, 0, ctx->stream.get()>>>(s->d_bucket.get(), s->d_bucket.get() + n_buckets, s->n_cols * WL_SUB, s->d_bin_cstart.get());
+    if (A.n_sel) k_worklist_emit<<<wblocks, WL_THREADS, 2 * n_buckets * 4, ctx->stream.get()>>>(A);
     launches += 3;
   }
   if (s->merge.n_rows && s->n_merge_pages) {  // overlapping chunks: decode the query's columns, merge + aggregate per row
-    CU_TRY(ctx, cudaMemsetAsync(s->d_mvalid, 0, (size_t)s->n_cols * s->merge.bm_words * 4, ctx->stream));
+    CU_TRY(ctx, cudaMemsetAsync(s->d_mvalid.get(), 0, (size_t)s->n_cols * s->merge.bm_words * 4, ctx->stream.get()));
     const uint32_t dblocks = (uint32_t)(((uint64_t)s->n_merge_pages * 32 + DECODE_THREADS - 1) / DECODE_THREADS);
-    k_decode_warp<<<dblocks, DECODE_THREADS, 0, ctx->stream>>>(pages->h_mapped ? pages->h_mapped : pages->d_arena, pages->d_descs, 0, s->d_mpage,
-                                                              s->n_merge_pages, s->d_mrow_off, s->d_mbm_off, s->d_mvals,
-                                                              reinterpret_cast<uint8_t *>(s->d_mvalid), s->d_status, s->d_err_page, s->d_stats);
+    k_decode_warp<<<dblocks, DECODE_THREADS, 0, ctx->stream.get()>>>(pages->h_mapped ? pages->h_mapped : pages->d_arena.get(), pages->d_descs.get(), 0, s->d_mpage.get(),
+                                                              s->n_merge_pages, s->d_mrow_off.get(), s->d_mbm_off.get(), s->d_mvals.get(),
+                                                              reinterpret_cast<uint8_t *>(s->d_mvalid.get()), s->d_status, s->d_err_page, s->d_stats);
     const uint32_t mblocks = (uint32_t)((s->merge.n_rows + 127) / 128);
-    k_merge_chunks<<<mblocks, 128, 0, ctx->stream>>>(s->params, s->merge);
+    k_merge_chunks<<<mblocks, 128, 0, ctx->stream.get()>>>(s->params, s->merge);
     launches += 2;
   }
-  cudaEvent_t ev_fork = capturing ? s->ev_cfork : s->ev_bin[0];
-  cudaEventRecord(ev_fork, ctx->stream);  // fork
+  cudaEvent_t ev_fork = capturing ? s->ev_cfork.get() : s->ev_bin[0].get();
+  cudaEventRecord(ev_fork, ctx->stream.get());  // fork
   // Host-resident pages: one bin's gather already saturates PCIe, so the gathers are chained largest bin first
   // (an event per bin); each bin's CRC check and scan then overlap the next bins' transfers and only the smallest
   // bin's tail is exposed after the last byte has arrived.
@@ -1993,17 +1954,17 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
   for (int oi = 0; oi < N_BINS; oi++) {
     const int b = order[oi];
     if (!s->grid[b]) continue;
-    cudaStreamWaitEvent(ctx->bin_stream[b], ev_fork, 0);
+    cudaStreamWaitEvent(ctx->bin_stream[b].get(), ev_fork, 0);
     int bin = b;
     const uint32_t n_bin = pages->h_bin_pages[b];
     if (pages->h_mapped) {
-      if (prev_gather >= 0) cudaStreamWaitEvent(ctx->bin_stream[b], s->ev_gather[prev_gather], 0);
+      if (prev_gather >= 0) cudaStreamWaitEvent(ctx->bin_stream[b].get(), s->ev_gather[prev_gather].get(), 0);
       uint32_t gblocks = std::max(1u, std::min<uint32_t>((uint32_t)ctx->sm_count * 4, (n_bin + 7) / 8));
-      k_gather_pages<<<gblocks, 256, 0, ctx->bin_stream[b]>>>(pages->h_mapped, pages->d_arena, pages->d_descs,
-                                                              pages->d_time_page_of, s->d_work_page, s->d_work_qcol,
-                                                              s->d_bin_cstart, bin);
+      k_gather_pages<<<gblocks, 256, 0, ctx->bin_stream[b].get()>>>(pages->h_mapped, pages->d_arena.get(), pages->d_descs.get(),
+                                                              pages->d_time_page_of.get(), s->d_work_page.get(), s->d_work_qcol.get(),
+                                                              s->d_bin_cstart.get(), bin);
       launches++;
-      cudaEventRecord(s->ev_gather[b], ctx->bin_stream[b]);
+      cudaEventRecord(s->ev_gather[b].get(), ctx->bin_stream[b].get());
       prev_gather = b;
     }
     if (pages->verify_on_read) {  // Page::crc_validation on every read (tsm/reader.rs:259), also for pages resident in HBM
@@ -2013,36 +1974,36 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       // dependent table lookups. A mismatch is reported in its own status slot and outranks whatever the decoders made of
       // the corrupt page.
       uint32_t gblocks = std::max(1u, std::min<uint32_t>((uint32_t)ctx->sm_count * 4, (n_bin + 7) / 8));
-      k_verify_crc<<<gblocks, 256, 0, ctx->bin_stream[b]>>>(pages->d_arena, pages->d_descs, pages->d_time_page_of,
-                                                            s->d_work_page, s->d_work_qcol, s->d_bin_cstart, bin,
-                                                            pages->d_crc_tables, s->d_crc_status, s->d_crc_err_page);
+      k_verify_crc<<<gblocks, 256, 0, ctx->bin_stream[b].get()>>>(pages->d_arena.get(), pages->d_descs.get(), pages->d_time_page_of.get(),
+                                                            s->d_work_page.get(), s->d_work_qcol.get(), s->d_bin_cstart.get(), bin,
+                                                            pages->d_crc_tables.get(), s->d_crc_status, s->d_crc_err_page);
       launches++;
     }
-    if (!capturing) cudaEventRecord(s->ev_bin_start[b], ctx->bin_stream[b]);
+    if (!capturing) cudaEventRecord(s->ev_bin_start[b].get(), ctx->bin_stream[b].get());
     const int sb = serial_bin_of(b);
     void *args[] = {(void *)&s->params, (void *)&bin};
     const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
     CU_TRY(ctx, cudaLaunchKernel(fn, dim3(s->grid[b]), dim3(SCAN_THREADS), args, serial_smem_bytes(sb, s->params.smem_words, s->params.has_tomb),
-                                 ctx->bin_stream[b]));
-    cudaEvent_t ev_done = capturing ? s->ev_cjoin[b] : s->ev_bin_done[b];
-    cudaEventRecord(ev_done, ctx->bin_stream[b]);
-    cudaStreamWaitEvent(ctx->stream, ev_done, 0);  // join
+                                 ctx->bin_stream[b].get()));
+    cudaEvent_t ev_done = capturing ? s->ev_cjoin[b].get() : s->ev_bin_done[b].get();
+    cudaEventRecord(ev_done, ctx->bin_stream[b].get());
+    cudaStreamWaitEvent(ctx->stream.get(), ev_done, 0);  // join
     launches++;
   }
-  if (!capturing) cudaEventRecord(s->ev_bin[N_BINS], ctx->stream);
+  if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
   if (s->n_combine) {  // sliding windows: every window folds its panes (it writes every array the kernels fill)
     const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
-    k_window_combine<<<dim3(std::max(1u, bx), s->n_combine), 256, 0, ctx->stream>>>(
-        s->d_pane_state, s->d_state, s->d_combine, (uint32_t)s->layout.n_groups, s->n_windows, s->n_panes, s->win_k);
+    k_window_combine<<<dim3(std::max(1u, bx), s->n_combine), 256, 0, ctx->stream.get()>>>(
+        s->d_pane_state.get(), s->d_state.get(), s->d_combine.get(), (uint32_t)s->layout.n_groups, s->n_windows, s->n_panes, s->win_k);
     launches++;
   }
   if (s->has_sel || s->n_means) {
     uint64_t work = std::max(std::max(s->sl.first_cells, s->sl.last_cells), s->n_means ? s->layout.n_cells : 0);
     uint32_t b = (uint32_t)std::min<uint64_t>((work + 255) / 256, 4096);
-    k_export_pairs<<<std::max(1u, b), 256, 0, ctx->stream>>>(s->d_state, s->sl, s->d_means, s->n_means, s->layout.n_cells);
+    k_export_pairs<<<std::max(1u, b), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->sl, s->d_means.get(), s->n_means, s->layout.n_cells);
     launches++;
   }
-  if (!capturing) cudaEventRecord(s->ev1, ctx->stream);
+  if (!capturing) cudaEventRecord(s->ev1.get(), ctx->stream.get());
   CU_TRY(ctx, cudaGetLastError());
   ctx->counters.kernel_launches = launches;
   s->enqueued = true;
@@ -2062,32 +2023,32 @@ static tskv_status sync_scan(tskv_ctx *ctx, tskv_scan *s) {
   const unsigned long long *ctr = aux + (AUX_COUNTERS - AUX_STATS);
   ctx->counters.pruned_page_count = ctr[CTR_PRUNED];
   float ms = 0;
-  cudaEventElapsedTime(&ms, s->ev0, s->ev1);
+  cudaEventElapsedTime(&ms, s->ev0.get(), s->ev1.get());
   ctx->counters.elapsed_scan_ms = ms;
   ctx->counters.points_decoded = aux[0];
   ctx->counters.rows_in_range = aux[1];
   ctx->counters.page_read_count = ctr[CTR_PAGES] + s->merge_read_pages;
   ctx->counters.page_read_bytes = ctr[CTR_BYTES] + s->merge_page_bytes;
   float fused = 0;
-  cudaEventElapsedTime(&fused, s->ev_bin[0], s->ev_bin[N_BINS]);
+  cudaEventElapsedTime(&fused, s->ev_bin[0].get(), s->ev_bin[N_BINS].get());
   ctx->counters.elapsed_fused_ms = fused;
   ctx->counters.dominant_kernel_ms = 0;
   ctx->counters.dominant_kernel_bytes = 0;
   ctx->counters.dominant_kernel_bin = 0;
   if (getenv("TSKV_DEBUG_BINS")) {  // (events of the un-captured pass: meaningful with TSKV_NO_GRAPH=1)
     float pro = 0, epi = 0;
-    cudaEventElapsedTime(&pro, s->ev0, s->ev_bin[0]);
-    cudaEventElapsedTime(&epi, s->ev_bin[N_BINS], s->ev1);
+    cudaEventElapsedTime(&pro, s->ev0.get(), s->ev_bin[0].get());
+    cudaEventElapsedTime(&epi, s->ev_bin[N_BINS].get(), s->ev1.get());
     fprintf(stderr, "[tskv] prologue (select, work list, init%s) %.3f ms, fused %.3f ms, epilogue %.3f ms\n",
             s->merge.n_rows ? ", merge pass" : "", pro, fused, epi);
   }
   for (int b = 0; b < N_BINS; b++) {
     if (!s->grid[b]) continue;
     float t = 0;
-    cudaEventElapsedTime(&t, s->ev_bin_start[b], s->ev_bin_done[b]);
+    cudaEventElapsedTime(&t, s->ev_bin_start[b].get(), s->ev_bin_done[b].get());
     if (getenv("TSKV_DEBUG_BINS")) {
       float t0 = 0;
-      cudaEventElapsedTime(&t0, s->ev_bin[0], s->ev_bin_start[b]);
+      cudaEventElapsedTime(&t0, s->ev_bin[0].get(), s->ev_bin_start[b].get());
       fprintf(stderr, "[tskv] bin %d grid %d, %d CTAs/SM: start +%.3f ms, run %.3f ms, %llu bytes\n", b,
               s->grid[b], s->occ[b], t0, t, ctr[CTR_BIN_BYTES + b]);
     }
@@ -2110,25 +2071,26 @@ tskv_status tskvgpu_scan_enqueue(tskv_ctx *ctx, tskv_scan *s) {
   if (!s->graph_exec) {
     cudaGraph_t graph = nullptr;
     if (!s->ev_cfork) {
-      cudaEventCreateWithFlags(&s->ev_cfork, cudaEventDisableTiming);
-      for (int b = 0; b < N_BINS; b++) cudaEventCreateWithFlags(&s->ev_cjoin[b], cudaEventDisableTiming);
+      s->ev_cfork = new_event(cudaEventDisableTiming);
+      for (int b = 0; b < N_BINS; b++) s->ev_cjoin[b] = new_event(cudaEventDisableTiming);
     }
-    bool ok = cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
+    bool ok = cudaStreamBeginCapture(ctx->stream.get(), cudaStreamCaptureModeThreadLocal) == cudaSuccess;
     if (ok) {
       const tskv_status st = enqueue_scan(ctx, s, true);  // the bin streams join the capture through the fork event
-      const cudaError_t e = cudaStreamEndCapture(ctx->stream, &graph);
-      ok = st == TSKV_OK && e == cudaSuccess && graph && cudaGraphInstantiate(&s->graph_exec, graph, 0) == cudaSuccess;
+      const cudaError_t e = cudaStreamEndCapture(ctx->stream.get(), &graph);
+      cudaGraphExec_t exec = nullptr;
+      ok = st == TSKV_OK && e == cudaSuccess && graph && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess;
+      s->graph_exec.reset(ok ? exec : nullptr);
       if (graph) cudaGraphDestroy(graph);
     }
     if (!ok) {  // anything the capture did not like: replay the pass call by call, as before
       if (getenv("TSKV_DEBUG_BINS")) fprintf(stderr, "[tskv] graph capture failed (%s): direct launches\n", cudaGetErrorString(cudaGetLastError()));
       cudaGetLastError();
-      s->graph_exec = nullptr;
       s->graph_failed = true;
       return enqueue_scan(ctx, s);
     }
   }
-  CU_TRY(ctx, cudaGraphLaunch(s->graph_exec, ctx->stream));
+  CU_TRY(ctx, cudaGraphLaunch(s->graph_exec.get(), ctx->stream.get()));
   s->enqueued = true;
   return TSKV_OK;
 }
@@ -2152,7 +2114,7 @@ tskv_status tskvgpu_scan_run(tskv_ctx *ctx, tskv_scan *s) {
 tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_view *out) {
   if (!ctx || !s || !out) return TSKV_ERR_INVALID_ARG;
   const StateLayout &L = s->sl;
-  uint64_t base = (uint64_t)(uintptr_t)s->d_state;
+  uint64_t base = (uint64_t)(uintptr_t)s->d_state.get();
   out->sum_i64_ptr = base + L.sum_i64_off * 8;
   out->sum_i64_len = L.sum_i64_len;
   out->sum_f64_ptr = base + L.sum_f64_off * 8;
@@ -2170,7 +2132,7 @@ tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_vie
 
 tskv_status tskvgpu_scan_exchange_view(tskv_ctx *ctx, tskv_scan *s, uint64_t *out_dptr, uint64_t *out_words) {
   if (!ctx || !s || !out_dptr || !out_words) return TSKV_ERR_INVALID_ARG;
-  *out_dptr = (uint64_t)(uintptr_t)s->d_state;
+  *out_dptr = (uint64_t)(uintptr_t)s->d_state.get();
   *out_words = s->sl.selval_off + s->sl.selval_len;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values
   return TSKV_OK;
 }
@@ -2181,7 +2143,7 @@ tskv_status tskvgpu_scan_merge_gathered(tskv_ctx *ctx, tskv_scan *s, uint64_t ga
   cudaSetDevice(ctx->device);
   const uint64_t words = s->sl.selval_off + s->sl.selval_len;
   uint32_t blocks = (uint32_t)std::min<uint64_t>((words + 255) / 256, 2048);
-  k_merge_gathered<<<std::max(1u, blocks), 256, 0, ctx->stream>>>(s->d_state, s->sl, reinterpret_cast<const uint64_t *>((uintptr_t)gathered_dptr),
+  k_merge_gathered<<<std::max(1u, blocks), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->sl, reinterpret_cast<const uint64_t *>((uintptr_t)gathered_dptr),
                                                                    n_ranks, words);
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;
@@ -2197,14 +2159,14 @@ tskv_status tskvgpu_scan_exchange(tskv_ctx *ctx, tskv_scan *s) {
   }
   const NcclApi &N = nccl_api();
   const uint64_t words = s->sl.selval_off + s->sl.selval_len;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values
-  if (!s->d_gathered) CU_TRY(ctx, stream_alloc(ctx, &s->d_gathered, (size_t)ctx->n_ranks * words));
-  const ncclResult_t r = N.AllGather(s->d_state, s->d_gathered, words, ncclUint64, ctx->comm, ctx->stream);
+  if (!s->d_gathered) CU_TRY(ctx, stream_alloc(s->d_gathered, (size_t)ctx->n_ranks * words, ctx->stream.get()));
+  const ncclResult_t r = N.AllGather(s->d_state.get(), s->d_gathered.get(), words, ncclUint64, ctx->comm, ctx->stream.get());
   if (r != ncclSuccess) {
     ctx->set_error(std::string("ncclAllGather: ") + N.GetErrorString(r));
     return TSKV_ERR_NCCL;
   }
   uint32_t blocks = (uint32_t)std::min<uint64_t>((words + 255) / 256, 2048);
-  k_merge_gathered<<<std::max(1u, blocks), 256, 0, ctx->stream>>>(s->d_state, s->sl, s->d_gathered, (uint32_t)ctx->n_ranks, words);
+  k_merge_gathered<<<std::max(1u, blocks), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->sl, s->d_gathered.get(), (uint32_t)ctx->n_ranks, words);
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;
 }
@@ -2214,7 +2176,7 @@ tskv_status tskvgpu_scan_snapshot_keys(tskv_ctx *ctx, tskv_scan *s) {
   std::lock_guard<std::mutex> lock(ctx->mu);
   cudaSetDevice(ctx->device);
   if (s->has_sel) {
-    k_snapshot_keys<<<256, 256, 0, ctx->stream>>>(s->d_state, s->sl);
+    k_snapshot_keys<<<256, 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->sl);
     CU_TRY(ctx, cudaGetLastError());
   }
   return TSKV_OK;
@@ -2225,7 +2187,7 @@ tskv_status tskvgpu_scan_mask_values(tskv_ctx *ctx, tskv_scan *s) {
   std::lock_guard<std::mutex> lock(ctx->mu);
   cudaSetDevice(ctx->device);
   if (s->has_sel) {
-    k_mask_values<<<256, 256, 0, ctx->stream>>>(s->d_state, s->sl);
+    k_mask_values<<<256, 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->sl);
     CU_TRY(ctx, cudaGetLastError());
   }
   return TSKV_OK;
@@ -2234,8 +2196,8 @@ tskv_status tskvgpu_scan_mask_values(tskv_ctx *ctx, tskv_scan *s) {
 static tskv_status finalize_device(tskv_ctx *ctx, tskv_scan *s) {
   const tskv_output_layout &L = s->layout;
   dim3 grid((uint32_t)((L.n_cells + 255) / 256), s->n_out);
-  k_finalize<<<grid, 256, 0, ctx->stream>>>(s->d_state, s->d_outs, s->n_out, L.n_cells, L.bitmap_stride, s->d_values,
-                                            s->d_validity);
+  k_finalize<<<grid, 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_outs.get(), s->n_out, L.n_cells, L.bitmap_stride, s->d_values.get(),
+                                            s->d_validity.get());
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;
 }
@@ -2246,9 +2208,9 @@ tskv_status tskvgpu_scan_finalize(tskv_ctx *ctx, tskv_scan *s, uint64_t *out_val
   cudaSetDevice(ctx->device);
   tskv_status st = finalize_device(ctx, s);
   if (st != TSKV_OK) return st;
-  CU_TRY(ctx, cudaMemcpyAsync(out_values, s->d_values, s->layout.values_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-  CU_TRY(ctx, cudaMemcpyAsync(out_validity, s->d_validity, s->layout.validity_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  CU_TRY(ctx, cudaMemcpyAsync(out_values, s->d_values.get(), s->layout.values_bytes, cudaMemcpyDeviceToHost, ctx->stream.get()));
+  CU_TRY(ctx, cudaMemcpyAsync(out_validity, s->d_validity.get(), s->layout.validity_bytes, cudaMemcpyDeviceToHost, ctx->stream.get()));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream.get()));
   return TSKV_OK;
 }
 
@@ -2259,14 +2221,14 @@ tskv_status tskvgpu_scan_finalize_device(tskv_ctx *ctx, tskv_scan *s, uint64_t *
   cudaSetDevice(ctx->device);
   tskv_status st = finalize_device(ctx, s);
   if (st != TSKV_OK) return st;
-  if (out_values_dptr) *out_values_dptr = (uint64_t)(uintptr_t)s->d_values;
-  if (out_validity_dptr) *out_validity_dptr = (uint64_t)(uintptr_t)s->d_validity;
+  if (out_values_dptr) *out_values_dptr = (uint64_t)(uintptr_t)s->d_values.get();
+  if (out_validity_dptr) *out_validity_dptr = (uint64_t)(uintptr_t)s->d_validity.get();
   return TSKV_OK;
 }
 
 void tskvgpu_scan_destroy(tskv_ctx *ctx, tskv_scan *s) {
   if (ctx) cudaSetDevice(ctx->device);
-  free_scan(s);
+  delete s;
 }
 
 static tskv_status scan_aggregate(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,

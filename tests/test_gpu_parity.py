@@ -602,6 +602,12 @@ def test_statistics_pruning_skips_column_groups_outside_the_time_ranges(engine):
         engine.scan_aggregate(pages, all_time)
         c = engine.counters()
         assert c["page_read_count"] == 3 * len(groups) and c["pruned_page_count"] == 0
+        # bounds replaced by wider ones that overlap every query range: the scan follows the new bounds
+        q_lo, q_hi = min(a for a, _ in ranges), max(b for _, b in ranges)
+        pages.set_time_bounds([(min(int(ts.min()), q_lo), max(int(ts.max()), q_hi)) for _, ts in groups])
+        assert_results_equal(engine.scan_aggregate(pages, q), exp, what="scan after the bounds were replaced (given: %s)" % given)
+        c = engine.counters()
+        assert c["page_read_count"] == 3 * len(groups) and c["pruned_page_count"] == 0
         pages.close()
     with pytest.raises(TskvError):
         p2 = engine.upload_pages(arena, descs)
@@ -707,6 +713,13 @@ def test_scan_with_tombstones_matches_decode_pages_semantics(engine, variant):
         assert_results_equal(engine.scan_aggregate(pages, q), orc.scan_aggregate(arena, descs, q, tombstones=tombs), what="tomb unbucketed")
     q_plain = make_query(SCAN_FIELDS, aggs=("count", "sum"), series_ids=sel)
     with_t = engine.scan_aggregate(pages, q_plain)
+    tombs2 = random_tombstones(rng, descs, t_lo, 1_000_000 + 340_000)
+    pages.set_tombstones(tombs2)  # replaced by another set
+    for group_by_series in (False, True):
+        q = make_query(SCAN_FIELDS, series_ids=sel, origin=3, width=17_000, first_bucket_start=fbs, n_buckets=nb,
+                       group_by_series=group_by_series)
+        assert_results_equal(engine.scan_aggregate(pages, q), orc.scan_aggregate(arena, descs, q, tombstones=tombs2),
+                             what="tombstones replaced gbs=%s" % group_by_series)
     pages.set_tombstones([])  # cleared: back to the plain result
     without = engine.scan_aggregate(pages, q_plain)
     assert_results_equal(without, orc.scan_aggregate(arena, descs, q_plain), what="tombstones cleared")
