@@ -121,7 +121,7 @@ GPU_SYMBOLS = [
     "tskvgpu_pages_series_count", "tskvgpu_pages_set_time_bounds", "tskvgpu_pages_set_tombstones", "tskvgpu_pages_set_chunk_files", "tskvgpu_pages_set_value_stats", "tskvgpu_decode_pages",
     "tskvgpu_query_output_layout", "tskvgpu_comm_unique_id", "tskvgpu_comm_init", "tskvgpu_comm_destroy", "tskvgpu_scan_exchange",
     "tskvgpu_scan_aggregate", "tskvgpu_scan_prepare", "tskvgpu_scan_run", "tskvgpu_scan_enqueue",
-    "tskvgpu_scan_sync", "tskvgpu_scan_partials", "tskvgpu_scan_exchange_view", "tskvgpu_scan_merge_gathered",
+    "tskvgpu_scan_sync", "tskvgpu_scan_partials", "tskvgpu_scan_work_list", "tskvgpu_scan_exchange_view", "tskvgpu_scan_merge_gathered",
     "tskvgpu_scan_snapshot_keys", "tskvgpu_scan_mask_values", "tskvgpu_scan_finalize",
     "tskvgpu_scan_finalize_device", "tskvgpu_scan_destroy", "tskvgpu_version",
     "tskvgpu_scan_prepare_sliding", "tskvgpu_scan_aggregate_sliding",
@@ -196,6 +196,7 @@ def load_gpu_library():
     lib.tskvgpu_scan_enqueue.argtypes = [vp, vp]
     lib.tskvgpu_scan_sync.argtypes = [vp, vp]
     lib.tskvgpu_scan_partials.argtypes = [vp, vp, C.POINTER(PartialsView)]
+    lib.tskvgpu_scan_work_list.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.tskvgpu_scan_exchange_view.argtypes = [vp, vp, u64p, u64p]
     lib.tskvgpu_scan_merge_gathered.argtypes = [vp, vp, C.c_uint64, C.c_uint32]
     lib.tskvgpu_scan_snapshot_keys.argtypes = [vp, vp]

@@ -107,6 +107,21 @@ uint32_t plan_walk_split(uint32_t max_groups, uint64_t n_walk, uint64_t n_items,
   return s;
 }
 
+bool plan_series_map(uint32_t min_id, uint32_t max_id, uint64_t n_series) {
+  return n_series && (uint64_t)max_id - min_id + 1 <= 2 * n_series + SERIES_MAP_SLACK;
+}
+
+bool plan_worklist_regions(uint32_t n_buckets, const uint32_t *capacity, uint32_t *start) {
+  uint64_t at = 0;
+  for (uint32_t k = 0; k < n_buckets; k++) {
+    start[k] = (uint32_t)at;
+    at = (at + capacity[k] + 31) & ~31ull;
+    if (at > UINT32_MAX) return false;
+  }
+  start[n_buckets] = (uint32_t)at;
+  return true;
+}
+
 void plan_overlap_groups(uint64_t n_cg, const uint32_t *cg_series, const uint32_t *cg_rows, const tskv_time_range *cg_bounds,
                          const uint64_t *cg_file, OverlapPlan *out) {
   *out = OverlapPlan{};

@@ -55,6 +55,15 @@ uint32_t plan_bin_parts(uint32_t maxrows, uint32_t skip_rows, uint32_t want, uin
 // of the `max_groups` column groups of the page set's largest series, at most 1024, then halved while the walk would
 // launch more threads than max(n_items, min_threads) (n_walk = the series walked: selected ids or every series).
 uint32_t plan_walk_split(uint32_t max_groups, uint64_t n_walk, uint64_t n_items, uint32_t min_threads);
+// Does a page set whose n_series distinct ids span [min_id, max_id] get a direct id -> rank table (4 bytes per id of
+// the span) instead of a binary search? Yes when the span is at most 2 x n_series + SERIES_MAP_SLACK ids: the table then
+// costs at most twice the sorted id list plus 64 KB.
+constexpr uint64_t SERIES_MAP_SLACK = 16384;
+bool plan_series_map(uint32_t min_id, uint32_t max_id, uint64_t n_series);
+// Work-list regions: bucket k gets [start[k], start[k] + capacity[k]), every start a multiple of 32 (one chunk of the
+// fused kernels never holds items of two buckets). start has n_buckets + 1 entries; start[n_buckets] = the list's size.
+// Returns false when the list would not fit 32-bit item indices.
+bool plan_worklist_regions(uint32_t n_buckets, const uint32_t *capacity, uint32_t *start);
 
 uint8_t classify_page(const PageHeader &h, uint8_t phys_type);
 

@@ -1,5 +1,5 @@
 // scan_kernels.cuh — sm_90a kernels of the tskv scan path:
-//   k_worklist_count / k_worklist_offsets / k_worklist_emit : series selection -> compacted, kind-binned work list
+//   k_worklist : series selection -> work list in fixed (kind bin, column, narrow flag) bucket regions
 //       (replaces get_series_id_by_filter's consumer side, tskv/src/reader/iterator.rs:915-929 +
 //       SeriesGroupBatchReaderFactory::create :123-264); k_select_ids / k_select_cg: slot of every column group
 //   k_scan_aggregate<TK,VK> : fused decode -> closed time-range filter -> bucket id -> reduce
@@ -66,7 +66,10 @@ struct ScanParams {
   const uint32_t *work_page;
   const uint32_t *work_slot;
   const uint8_t *work_qcol;
-  const uint32_t *bin_cstart;  // [N_BINS + 1] starts of the kind bins in the work list
+  // bucket regions of the work list (k_worklist): bucket (bin, column, narrow flag) holds region_fill[k] items from
+  // region_start[k] on, k = (bin * n_cols + column) * WL_SUB + narrow flag
+  const uint32_t *region_start;
+  const uint32_t *region_fill;
   const ColState *cols;
   uint64_t *state;
   uint32_t *task_counter;       // [N_BINS] dynamic chunk schedulers
@@ -135,21 +138,36 @@ __device__ __forceinline__ uint64_t group_cell_base(const ScanParams &P, uint32_
 // ------------------------------------------------------------------------------------------------
 // selection / compaction
 // ------------------------------------------------------------------------------------------------
-// Series selection -> slot of every column group, in two steps: one thread per SELECTED id finds the id's rank among
-// the page set's series (binary search in the sorted distinct ids) and writes its position in the selection list to
-// rank_slot[rank] (memset to -1 before); then one thread per column group gathers rank_slot[rank of its series].
-// (Round 1 searched the selection list once per column group: 10 x the dependent loads for a 10 % selection.)
-__global__ void k_select_ids(const uint32_t *set_series, uint32_t n_set_series, const uint32_t *series_ids, uint32_t n_series,
-                             int32_t *rank_slot) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_series) return;
-  const uint32_t id = __ldg(series_ids + i);
-  uint32_t lo = 0, hi = n_set_series;
+// Series id -> rank among the page set's distinct ids (FULL: the page set does not hold the id). A page set whose ids
+// are dense (plan_series_map) has a direct table rank_of[id - min_id]: one load instead of a binary search of ~20
+// dependent steps over the sorted ids.
+struct SeriesIndex {
+  const uint32_t *sorted;   // the page set's distinct series ids, ascending
+  const uint32_t *rank_of;  // [span] rank of id min_id + k, FULL for an id without series (null: binary search)
+  uint32_t n, min_id, span;
+};
+__device__ __forceinline__ uint32_t series_rank(const SeriesIndex &S, uint32_t id) {
+  if (S.rank_of) {
+    const uint32_t k = id - S.min_id;  // ids below min_id wrap past the span
+    return k < S.span ? __ldg(S.rank_of + k) : FULL;
+  }
+  uint32_t lo = 0, hi = S.n;
   while (lo < hi) {
     const uint32_t mid = (lo + hi) >> 1;
-    if (__ldg(set_series + mid) < id) lo = mid + 1; else hi = mid;
+    if (__ldg(S.sorted + mid) < id) lo = mid + 1; else hi = mid;
   }
-  if (lo < n_set_series && __ldg(set_series + lo) == id) rank_slot[lo] = (int32_t)i;
+  return lo < S.n && __ldg(S.sorted + lo) == id ? lo : FULL;
+}
+
+// Series selection -> slot of every column group, in two steps: one thread per SELECTED id finds the id's rank among
+// the page set's series and writes its position in the selection list to rank_slot[rank] (memset to -1 before); then
+// one thread per column group gathers rank_slot[rank of its series].
+// (Round 1 searched the selection list once per column group: 10 x the dependent loads for a 10 % selection.)
+__global__ void k_select_ids(const SeriesIndex S, const uint32_t *series_ids, uint32_t n_series, int32_t *rank_slot) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_series) return;
+  const uint32_t rank = series_rank(S, __ldg(series_ids + i));
+  if (rank != FULL) rank_slot[rank] = (int32_t)i;
 }
 __global__ void k_select_cg(uint32_t n_cg, const int32_t *rank_slot, const uint32_t *cg_series_rank, int32_t *cg_slot) {
   const uint32_t cg = blockIdx.x * blockDim.x + threadIdx.x;
@@ -235,14 +253,16 @@ struct PruneRanges {
 // Work list driven by the SELECTION: 2^split_log2 threads per selected series walk that series' column groups (thread j
 // of a series takes groups j, j + S, j + 2S, ... of it) and their field pages, so the cost follows the selection (C4:
 // 10 % of the series) instead of the page set, and a series with thousands of groups is not walked by one thread.
-// Two passes over the same walk - count per (decode-kind bin, query column) bucket, then place - with a block-local
-// histogram in shared memory so that the global atomics are one per (block, bucket). Inside a bucket the order is
-// arbitrary (the fused kernels only need warps that are homogeneous in codec and, for GROUP BY bucket, in column). A
-// (bin, column) bucket is split in two by the page's narrow flag (WL_SUB buckets, ScanParams.page_narrow): its wide
-// pages come first, then its narrow ones, so that all chunks of the bucket but the one across the boundary are
-// uniformly narrow or wide. Outputs: work_page / work_slot / work_qcol (bit 7 = "brings the column group's time page":
-// the first selected field page of each value class of a group), bin_cstart, the reader counters (the reference's
-// reader metrics, column_group/mod.rs:141-193, split per decode-kind bin), statistics pruning.
+// Items go to buckets (decode-kind bin, query column, narrow flag): the fused kernels need warps that are homogeneous in
+// codec and, for GROUP BY bucket, in column, and a (bin, column) bucket is split in two by the page's narrow flag
+// (WL_SUB buckets, ScanParams.page_narrow) so that a chunk is uniformly narrow or wide. Every bucket owns a fixed region
+// of the work list, laid out by the host at prepare (plan_worklist_regions): it starts on a multiple of 32 and holds the
+// page set's field pages of the bucket's bin, column id and narrow flag, an upper bound for any selection. So one
+// kernel places every item without a pass over all blocks' counts in between, and no chunk of 32 items straddles two
+// buckets. Inside a bucket the order is arbitrary. Outputs:
+// work_page / work_slot / work_qcol (bit 7 = "brings the column group's time page": the first selected field page of
+// each value class of a group), the buckets' fill counts, the reader counters (the reference's reader metrics,
+// column_group/mod.rs:141-193, split per decode-kind bin), statistics pruning.
 // ------------------------------------------------------------------------------------------------
 constexpr int WL_THREADS = 256;
 constexpr uint32_t WL_SUB = 2;  // work-list buckets per (bin, query column): wide pages, narrow pages
@@ -255,8 +275,7 @@ struct WorkListArgs {
   const uint32_t *rank_cg;
   const uint8_t *page_bin;       // [n_descs] decode-kind bin of a field page
   const uint8_t *page_narrow;    // [n_descs] narrow flags (null: every page is wide)
-  const uint32_t *set_series;    // the page set's distinct series ids, ascending
-  uint32_t n_set_series;
+  SeriesIndex series;            // the page set's series ids -> ranks
   const uint32_t *series_ids;    // the selection (null: every series, slot = rank)
   uint32_t n_sel;                // walk indices: selected ids, or n_set_series
   uint32_t split_log2;           // log2 of the threads per walk index (plan_walk_split)
@@ -270,8 +289,8 @@ struct WorkListArgs {
   const uint8_t *cg_merge;       // column groups of overlapping chunks go through the merge pass
   const int64_t *page_stats;     // value-statistics pruning against `preds` (null: none)
   PredicateSet preds;
-  uint32_t *bucket_count;        // [N_BINS * n_cols * WL_SUB] totals (pass 1), then running cursors (pass 2)
-  uint32_t *bucket_off;          // [N_BINS * n_cols * WL_SUB + 1] exclusive offsets (k_worklist_offsets)
+  const uint32_t *region_start;  // [N_BINS * n_cols * WL_SUB + 1] first work-list index of every bucket's region
+  uint32_t *bucket_fill;         // [N_BINS * n_cols * WL_SUB] items placed in each bucket (zeroed by k_init_state)
   uint32_t *work_page, *work_slot;
   uint8_t *work_qcol;
   unsigned long long *counters;  // [N_COUNTERS] CTR_*
@@ -289,14 +308,8 @@ template <typename F>
 __device__ __forceinline__ void worklist_walk(const WorkListArgs &A, uint32_t i, uint32_t j, bool count_stats, F &&emit) {
   uint32_t rank = i;
   if (A.series_ids) {
-    const uint32_t id = __ldg(A.series_ids + i);
-    uint32_t lo = 0, hi = A.n_set_series;
-    while (lo < hi) {
-      const uint32_t mid = (lo + hi) >> 1;
-      if (__ldg(A.set_series + mid) < id) lo = mid + 1; else hi = mid;
-    }
-    if (lo >= A.n_set_series || __ldg(A.set_series + lo) != id) return;  // a selected id this page set does not hold
-    rank = lo;
+    rank = series_rank(A.series, __ldg(A.series_ids + i));
+    if (rank == FULL) return;  // a selected id this page set does not hold
   }
   const uint32_t c0 = __ldg(A.rank_cg_start + rank), c1 = __ldg(A.rank_cg_start + rank + 1);
   for (uint32_t k = c0 + j; k < c1; k += 1u << A.split_log2) {
@@ -338,19 +351,25 @@ __device__ __forceinline__ void worklist_walk(const WorkListArgs &A, uint32_t i,
   }
 }
 
-// Pass 1: bucket totals + the reader counters.
-__global__ void __launch_bounds__(WL_THREADS) k_worklist_count(const WorkListArgs A) {
-  extern __shared__ uint32_t s_hist[];  // [N_BINS * n_cols * WL_SUB]
+// The walk, twice over the block's series: first the block's items per bucket and the reader counters (per block in
+// shared memory), then - after one atomic per (block, bucket) on the bucket's fill count has reserved the block's share
+// of the region - the items' places. Inside a block the items keep the order of the shared-memory cursors, so scans of a
+// few blocks place their items in a stable order (float sums of two runs of one scan agree bit for bit); a warp-wide
+// reservation per item instead would interleave the warps of a block.
+__global__ void __launch_bounds__(WL_THREADS) k_worklist(const WorkListArgs A) {
+  extern __shared__ uint32_t s_hist[];  // [2][N_BINS * n_cols * WL_SUB]: block counts -> block bases, and the running cursors
   __shared__ unsigned long long s_pages, s_bytes[N_BINS];
   const uint32_t n_buckets = N_BINS * A.n_cols * WL_SUB;
-  for (uint32_t k = threadIdx.x; k < n_buckets; k += WL_THREADS) s_hist[k] = 0;
+  uint32_t *s_base = s_hist, *s_cur = s_hist + n_buckets;
+  for (uint32_t k = threadIdx.x; k < 2 * n_buckets; k += WL_THREADS) s_hist[k] = 0;
   if (threadIdx.x == 0) s_pages = 0;
   if (threadIdx.x < N_BINS) s_bytes[threadIdx.x] = 0;
   __syncthreads();
   const uint32_t t = blockIdx.x * WL_THREADS + threadIdx.x, i = t >> A.split_log2, j = t & ((1u << A.split_log2) - 1);
+  const uint32_t slot = (i < A.n_sel && A.walk) ? __ldg(A.walk + i) : i;
   if (i < A.n_sel)
-    worklist_walk(A, A.walk ? __ldg(A.walk + i) : i, j, true, [&](uint32_t page, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &d, bool first_in_group, uint32_t tp) {
-      atomicAdd(&s_hist[worklist_key(A, page, bin, qc)], 1u);
+    worklist_walk(A, slot, j, true, [&](uint32_t page, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &d, bool first_in_group, uint32_t tp) {
+      atomicAdd(&s_base[worklist_key(A, page, bin, qc)], 1u);
       // the reader metrics (page_read_count / page_read_bytes) count the time page once per column group
       unsigned long long bytes = d.size, pages = 1;
       if (first_in_group) { bytes += A.descs[tp].size; pages += 1; }
@@ -359,75 +378,12 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_count(const WorkListArg
     });
   __syncthreads();
   for (uint32_t k = threadIdx.x; k < n_buckets; k += WL_THREADS)
-    if (s_hist[k]) atomicAdd(&A.bucket_count[k], s_hist[k]);
+    if (s_base[k]) s_base[k] = A.region_start[k] + atomicAdd(&A.bucket_fill[k], s_base[k]);
   if (threadIdx.x == 0 && s_pages) atomicAdd(&A.counters[CTR_PAGES], s_pages);
   if (threadIdx.x < N_BINS && s_bytes[threadIdx.x]) {
     atomicAdd(&A.counters[CTR_BYTES], s_bytes[threadIdx.x]);
     atomicAdd(&A.counters[CTR_BIN_BYTES + threadIdx.x], s_bytes[threadIdx.x]);
   }
-}
-
-// Exclusive offsets of the buckets (bin-major, `per_bin` buckets per bin), bin_cstart, and the cursors reset for pass 2.
-// One block.
-__global__ void k_worklist_offsets(uint32_t *bucket_count, uint32_t *bucket_off, uint32_t per_bin, uint32_t *bin_cstart) {
-  __shared__ uint32_t s_carry;
-  __shared__ uint32_t s_warp[32];
-  const uint32_t n_buckets = N_BINS * per_bin;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
-  for (uint32_t base = 0; base < n_buckets; base += blockDim.x) {
-    const uint32_t k = base + threadIdx.x;
-    const uint32_t v = k < n_buckets ? bucket_count[k] : 0;
-    uint32_t x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t y = __shfl_up_sync(FULL, x, o);
-      if ((threadIdx.x & 31) >= (uint32_t)o) x += y;
-    }
-    if ((threadIdx.x & 31) == 31) s_warp[threadIdx.x >> 5] = x;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      const uint32_t w = threadIdx.x < (blockDim.x >> 5) ? s_warp[threadIdx.x] : 0;
-      uint32_t xs = w;
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(FULL, xs, o);
-        if (threadIdx.x >= (uint32_t)o) xs += y;
-      }
-      s_warp[threadIdx.x] = xs - w;
-    }
-    __syncthreads();
-    const uint32_t excl = s_carry + s_warp[threadIdx.x >> 5] + x - v;
-    if (k < n_buckets) {
-      bucket_off[k] = excl;
-      bucket_count[k] = 0;  // pass 2's cursor
-      if (k % per_bin == 0) bin_cstart[k / per_bin] = excl;
-    }
-    __syncthreads();
-    if (threadIdx.x == blockDim.x - 1) s_carry = excl + v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    bucket_off[n_buckets] = s_carry;
-    bin_cstart[N_BINS] = s_carry;
-    bin_cstart[N_BINS + 1] = s_carry;  // total
-  }
-}
-
-// Pass 2: the same walk; a block reserves its share of every bucket with one atomic and places its items inside it.
-__global__ void __launch_bounds__(WL_THREADS) k_worklist_emit(const WorkListArgs A) {
-  extern __shared__ uint32_t s_hist[];  // [2][N_BINS * n_cols * WL_SUB]: block counts -> block bases, and the running cursors
-  const uint32_t n_buckets = N_BINS * A.n_cols * WL_SUB;
-  uint32_t *s_base = s_hist, *s_cur = s_hist + n_buckets;
-  for (uint32_t k = threadIdx.x; k < 2 * n_buckets; k += WL_THREADS) s_hist[k] = 0;
-  __syncthreads();
-  const uint32_t t = blockIdx.x * WL_THREADS + threadIdx.x, i = t >> A.split_log2, j = t & ((1u << A.split_log2) - 1);
-  const uint32_t slot = (i < A.n_sel && A.walk) ? __ldg(A.walk + i) : i;
-  if (i < A.n_sel)
-    worklist_walk(A, slot, j, false, [&](uint32_t page, uint32_t bin, uint32_t qc, bool, const tskv_page_desc &, bool, uint32_t) {
-      atomicAdd(&s_base[worklist_key(A, page, bin, qc)], 1u);
-    });
-  __syncthreads();
-  for (uint32_t k = threadIdx.x; k < n_buckets; k += WL_THREADS)
-    if (s_base[k]) s_base[k] = A.bucket_off[k] + atomicAdd(&A.bucket_count[k], s_base[k]);
   __syncthreads();
   if (i < A.n_sel)
     worklist_walk(A, slot, j, false, [&](uint32_t page, uint32_t bin, uint32_t qc, bool with_time, const tskv_page_desc &, bool, uint32_t) {
@@ -444,11 +400,12 @@ __global__ void __launch_bounds__(WL_THREADS) k_worklist_emit(const WorkListArgs
 // file reads of TsmReader::read_adjacent_pages (tsm/reader.rs:236-264).
 __global__ void k_gather_pages(const uint8_t *host_arena, uint8_t *dev_arena, const tskv_page_desc *descs,
                                const uint32_t *time_page_of, const uint32_t *work_page,
-                               const uint8_t *work_qcol, const uint32_t *bin_cstart, int bin) {
-  const uint32_t w0 = bin_cstart[bin], n = bin_cstart[bin + 1];  // the bin's range of the work list
+                               const uint8_t *work_qcol, const uint32_t *region_start, const uint32_t *bucket_fill,
+                               uint32_t per_bin, int bin) {
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
-  for (uint32_t w = w0 + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5); w < n; w += warps) {
+  for (uint32_t k = bin * per_bin; k < (bin + 1) * per_bin; k++)  // the bin's bucket regions
+  for (uint32_t w = region_start[k] + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5), n = region_start[k] + bucket_fill[k]; w < n; w += warps) {
     const uint32_t page = work_page[w];
     const bool with_time = work_qcol[w] & 0x80;
     for (int pass = 0; pass < (with_time ? 2 : 1); pass++) {
@@ -475,14 +432,15 @@ __device__ __forceinline__ uint32_t crc_step8(const uint32_t (*t)[256], uint32_t
 
 __global__ void __launch_bounds__(256)
 k_verify_crc(const uint8_t *arena, const tskv_page_desc *descs, const uint32_t *time_page_of,
-             const uint32_t *work_page, const uint8_t *work_qcol, const uint32_t *bin_cstart, int bin,
+             const uint32_t *work_page, const uint8_t *work_qcol, const uint32_t *region_start, const uint32_t *bucket_fill,
+             uint32_t per_bin, int bin,
              const uint32_t *crc_tables /* [8][256] */, int32_t *status, unsigned long long *err_page) {
   __shared__ uint32_t s_t[8][256];
   for (uint32_t i = threadIdx.x; i < 2048; i += blockDim.x) s_t[i >> 8][i & 255] = crc_tables[i];
   __syncthreads();
-  const uint32_t w0 = bin_cstart[bin], n = bin_cstart[bin + 1];
   const uint32_t stride = gridDim.x * blockDim.x;
-  for (uint32_t w = w0 + blockIdx.x * blockDim.x + threadIdx.x; w < n; w += stride) {
+  for (uint32_t k = bin * per_bin; k < (bin + 1) * per_bin; k++)  // the bin's bucket regions
+  for (uint32_t w = region_start[k] + blockIdx.x * blockDim.x + threadIdx.x, n = region_start[k] + bucket_fill[k]; w < n; w += stride) {
     const uint32_t page = work_page[w];
     const bool with_time = work_qcol[w] & 0x80;
     for (int pass = 0; pass < (with_time ? 2 : 1); pass++) {
@@ -1723,22 +1681,33 @@ __global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, SEL)) k_scan
   const uint32_t ring_base = (uint32_t)__cvta_generic_to_shared(warp_area);
   uint64_t *stage = warp_area + scan_ring_bytes_per_warp(TK) / 8;
   uint4 *s_tomb = reinterpret_cast<uint4 *>(s_tab + ((P.smem_words + 1) & ~1u) + (SCAN_THREADS / 32) * (scan_warp_bytes(TK) / 8));
-  const uint32_t begin0 = __ldg(P.bin_cstart + bin), end0 = __ldg(P.bin_cstart + bin + 1);
+  // the bin's buckets (one per query column and narrow flag): groups of 32 items that never straddle two buckets
+  uint32_t n_groups = 0;
+  for (uint32_t k = bin * P.n_cols * WL_SUB; k < (bin + 1) * P.n_cols * WL_SUB; k++) n_groups += (__ldg(P.region_fill + k) + 31) >> 5;
   // pages cut at restart points: n_parts chunks per group of 32 pages (consecutive chunk numbers = the parts of one group)
   const uint32_t n_parts = (TK == TK_GEN || VK == VK_GEN || SEL) ? 1u : P.bin_parts[bin];
   const uint32_t part_rows = P.bin_part_rows[bin];
-  const uint32_t n_chunks = ((end0 - begin0 + 31) >> 5) * n_parts;
+  const uint32_t n_chunks = n_groups * n_parts;
   for (;;) {
     uint32_t c = 0;
     if (lane == 0) c = atomicAdd(P.task_counter + bin, 1u);
     c = __shfl_sync(FULL, c, 0);
     if (c >= n_chunks) break;
-    const uint32_t group = n_parts > 1 ? c / n_parts : c;
+    uint32_t group = n_parts > 1 ? c / n_parts : c;
     const uint32_t part = c - group * n_parts;
-    const uint32_t begin = begin0 + (group << 5);
-    const uint32_t end = min(begin + 32, end0);
+    uint32_t k = bin * P.n_cols * WL_SUB;
+    asm("" : "+r"(k));  // computed here, per chunk: addresses hoisted out of the loop would hold registers of the row loops
+    uint32_t fill = __ldg(P.region_fill + k);
+    while (group >= (fill + 31) >> 5) {  // the bucket of the group, and the group's number inside it
+      group -= (fill + 31) >> 5;
+      fill = __ldg(P.region_fill + ++k);
+    }
+    const uint32_t region = __ldg(P.region_start + k);
+    const uint32_t begin = region + (group << 5);
+    const uint32_t end = min(begin + 32, region + fill);
     if constexpr (NARROW == NARROW_SOME) {
-      // 32-bit arithmetic when all of the chunk's pages are narrow (the work list keeps a bin's narrow pages together)
+      // 32-bit arithmetic when all of the chunk's pages are narrow (a chunk holds one bucket: narrow or wide pages; the
+      // vote also covers page sets without narrow flags in the work list)
       const uint32_t item = begin + lane;
       const bool narrow = __all_sync(FULL, item >= end || __ldg(P.page_narrow + __ldg(P.work_page + item)));
       if (narrow) scan_chunk_seg<TK, VK, SEL, true>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
@@ -1796,15 +1765,14 @@ constexpr uint32_t AUX_CRC_ERR_PAGE = AUX_CRC_STATUS + 1;
 constexpr uint32_t AUX_WORDS = 32;
 static_assert(N_BINS * 4 <= (AUX_STATUS - AUX_TASK_COUNTERS) * 8 && AUX_CRC_ERR_PAGE < AUX_WORDS, "scan aux block layout");
 
-// Identities of the partial state; the same launch zeroes the scan's small per-pass scratch (the aux block, bin starts,
-// work-list buckets) so that a pass starts with ONE node instead of three memsets + a kernel.
+// Identities of the partial state; the same launch zeroes the scan's small per-pass scratch (the aux block, the
+// work-list buckets' fill counts) so that a pass starts with ONE node instead of three memsets + a kernel.
 __global__ void k_init_state(uint64_t *state, StateLayout L, unsigned long long *aux, uint32_t aux_words, uint32_t *zero32,
-                             uint32_t n_zero32, uint32_t *zero32b, uint32_t n_zero32b) {
+                             uint32_t n_zero32) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t k = i; k < aux_words; k += stride) aux[k] = 0;
   for (uint64_t k = i; k < n_zero32; k += stride) zero32[k] = 0;
-  for (uint64_t k = i; k < n_zero32b; k += stride) zero32b[k] = 0;
   for (uint64_t k = i; k < L.total; k += stride) {
     uint64_t v = 0;
     if (k >= L.min_off && k < L.min_off + L.min_len) v = 0x7fffffffffffffffull;

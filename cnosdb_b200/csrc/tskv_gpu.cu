@@ -12,6 +12,7 @@
 #include <string>
 #include <thread>
 #include <type_traits>
+#include <unordered_map>
 #include <vector>
 
 #include <cuda_runtime.h>
@@ -119,12 +120,18 @@ struct tskv_pages {
   dev_ptr<uint32_t> d_cg_time_page;
   dev_ptr<uint32_t> d_cg_series_rank;
   dev_ptr<uint32_t> d_series_sorted;  // the page set's distinct series ids, ascending (rank -> id)
+  // dense ids (plan_series_map): rank of id series_min + k at d_rank_of[k], k < series_span (null: binary search)
+  dev_ptr<uint32_t> d_rank_of;
+  uint32_t series_min = 0, series_span = 0;
   dev_ptr<uint32_t> d_rank_cg_start, d_rank_cg;  // CSR: series rank -> its column groups (arena order)
   uint32_t max_series_cg = 0;           // most column groups of one series (plan_walk_split)
   dev_ptr<uint8_t> d_page_bin;          // decode-kind bin of every field page
   mutable dev_ptr<int64_t> d_page_stats;  // {min key, max key} of every field page (k_page_stats), built on first use
   uint32_t n_items = 0;              // field pages
   uint32_t h_bin_pages[N_BINS]{};    // field pages per bin
+  // field pages per column id, then per (bin, narrow flag) at bin * WL_SUB + flag: the capacity of a scan's work-list
+  // bucket of that column
+  std::unordered_map<uint16_t, std::vector<uint32_t>> col_bucket_pages;
   uint64_t h_bin_bytes[N_BINS]{};    // field-page bytes per bin (orders the PCIe gathers of host-resident scans)
   uint64_t h_bin_rows[N_BINS]{};     // rows of the bin's field pages (serial cost of its chunks)
   // the epoch invalidates scans prepared before a change of the tombstones
@@ -171,12 +178,13 @@ struct tskv_scan {
   // path, memory is recycled by the pool
   async_ptr<uint32_t> d_series;
   async_ptr<int32_t> d_rank_slot;  // rank of a series in the page set -> position in the selection list (or -1)
-  async_ptr<uint32_t> d_bucket;    // selection-driven work list: [N_BINS * n_cols * WL_SUB] counts / cursors | [.. + 1] offsets
+  // selection-driven work list: [N_BINS * n_cols * WL_SUB] fill counts of the buckets, and their regions (+ 1: the end)
+  async_ptr<uint32_t> d_bucket, d_region;
+  bool split_narrow = false;       // the work list keeps narrow pages in buckets of their own (some bin has both kinds)
   uint32_t walk_split_log2 = 0;    // log2 of the work-list walk's threads per series (plan_walk_split)
   async_ptr<int32_t> d_cg_slot;
   async_ptr<uint32_t> d_work_page, d_work_slot;
   async_ptr<uint8_t> d_work_qcol;
-  async_ptr<uint32_t> d_bin_cstart;  // [N_BINS+1] then [1] total
   async_ptr<ColState> d_cols;
   async_ptr<OutCol> d_outs;
   async_ptr<MeanExport> d_means;
@@ -857,6 +865,8 @@ void plan_grids(const tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *
     const void *fn = (const void *)(!has_sel ? scan_kernel_for<false>(sb, pages->h_bin_narrow[b]) : scan_kernel_for<true>(sb));
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[b], fn, SCAN_THREADS, serial_smem_bytes(sb, smem_words, has_tomb));
     occ[b] = std::max(1, occ[b]);
+    // (an estimate: the work list rounds each (column, narrow flag) bucket of the bin up to 32 items on its own, so the bin
+    // may run up to n_cols * WL_SUB - 1 chunks more than items / 32; the kernels are persistent and take them all)
     const double est_items = n_bin * sel_frac * 1.02 + 32;
     const uint32_t per_task = 32;  // pages per warp task: one chunk
     const double tasks = est_items / per_task * parts[b];
@@ -977,7 +987,29 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
     *h2d += (n_slots + walk.size()) * 4;
   }
   if (e == cudaSuccess && q->series_ids) e = stream_alloc(s->d_rank_slot, pages->series.size(), st);
-  if (e == cudaSuccess) e = stream_alloc(s->d_bucket, (size_t)2 * N_BINS * q->n_columns * WL_SUB + 1, st);
+  // work-list regions: each (bin, query column, narrow flag) bucket holds as many items as the page set has field pages
+  // of the column's id in that bin with that flag (a later query column with the same id gets no items: find_qcol)
+  const uint32_t n_buckets = N_BINS * q->n_columns * WL_SUB;
+  s->split_narrow = std::any_of(pages->h_bin_narrow, pages->h_bin_narrow + N_BINS, [](uint8_t m) { return m == NARROW_SOME; });
+  std::vector<uint32_t> capacity(n_buckets, 0), region(n_buckets + 1);
+  for (uint32_t c = 0; c < q->n_columns; c++) {
+    const uint16_t id = q->columns[c].column_id;
+    const auto it = pages->col_bucket_pages.find(id);
+    if (it == pages->col_bucket_pages.end() ||
+        std::any_of(q->columns, q->columns + c, [&](const tskv_agg_column &o) { return o.column_id == id; }))
+      continue;
+    for (int b = 0; b < N_BINS; b++) {
+      const uint32_t k = (b * q->n_columns + c) * WL_SUB, wide = it->second[b * WL_SUB], narrow = it->second[b * WL_SUB + 1];
+      capacity[k] = s->split_narrow ? wide : wide + narrow;  // (without the split every item takes the wide bucket)
+      capacity[k + 1] = s->split_narrow ? narrow : 0;
+    }
+  }
+  if (!plan_worklist_regions(n_buckets, capacity.data(), region.data())) {
+    ctx->set_error("work list too large for 32-bit item indices");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  if (e == cudaSuccess) e = stream_alloc(s->d_bucket, n_buckets, st);
+  if (e == cudaSuccess) e = upload(s->d_region, region.data(), region.size(), st);
   {
     // A series with thousands of column groups (one host over a year) is walked by several threads
     const uint64_t n_walk = q->series_ids ? q->n_series : pages->series.size();
@@ -985,10 +1017,9 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
     while ((1u << s->walk_split_log2) < split) s->walk_split_log2++;
   }
   if (e == cudaSuccess) e = stream_alloc(s->d_cg_slot, pages->n_cg, st);
-  if (e == cudaSuccess) e = stream_alloc(s->d_work_page, n_items, st);
-  if (e == cudaSuccess) e = stream_alloc(s->d_work_slot, n_items, st);
-  if (e == cudaSuccess) e = stream_alloc(s->d_work_qcol, n_items, st);
-  if (e == cudaSuccess) e = stream_alloc(s->d_bin_cstart, N_BINS + 2, st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_work_page, region[n_buckets], st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_work_slot, region[n_buckets], st);
+  if (e == cudaSuccess) e = stream_alloc(s->d_work_qcol, region[n_buckets], st);
   if (e == cudaSuccess) e = upload(s->d_cols, lay.cols.data(), lay.cols.size(), st);
   if (e == cudaSuccess) e = upload(s->d_outs, lay.outs.data(), lay.outs.size(), st);
   s->n_means = (uint32_t)lay.means.size();
@@ -1325,6 +1356,9 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
       bin = tclass == TK_RLE ? BIN_SHORT_RLE_GOR : BIN_SHORT_S8B_GOR;
     page_bin[p] = (uint8_t)bin;
     pg->h_bin_pages[bin]++;
+    std::vector<uint32_t> &cb = pg->col_bucket_pages[vd.column_id];
+    if (cb.empty()) cb.assign(N_BINS * WL_SUB, 0);
+    cb[bin * WL_SUB]++;
     pg->h_bin_bytes[bin] += vd.size;
     pg->h_bin_rows[bin] += vd.num_values;
     pg->h_bin_maxrows[bin] = std::max(pg->h_bin_maxrows[bin], vd.num_values);
@@ -1352,6 +1386,14 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
   if (e == cudaSuccess) e = upload(pg->d_cg_time_page, cg_time_page.data(), pg->n_cg, st);
   if (e == cudaSuccess) e = upload(pg->d_cg_series_rank, cg_rank.data(), pg->n_cg, st);
   if (e == cudaSuccess) e = upload(pg->d_series_sorted, pg->series.data(), pg->series.size(), st);
+  if (e == cudaSuccess && plan_series_map(pg->series.empty() ? 0 : pg->series.front(), pg->series.empty() ? 0 : pg->series.back(),
+                                          pg->series.size())) {
+    pg->series_min = pg->series.front();
+    pg->series_span = pg->series.back() - pg->series.front() + 1;
+    std::vector<uint32_t> rank_of(pg->series_span, 0xffffffffu);
+    for (size_t r = 0; r < pg->series.size(); r++) rank_of[pg->series[r] - pg->series_min] = (uint32_t)r;
+    e = upload(pg->d_rank_of, rank_of.data(), rank_of.size(), st);
+  }
   {  // series rank -> its column groups (the selection-driven work list walks a selected series' groups)
     std::vector<uint32_t> start(pg->series.size() + 1, 0), list(pg->n_cg);
     for (uint32_t cg = 0; cg < pg->n_cg; cg++) start[cg_rank[cg] + 1]++;
@@ -1429,7 +1471,12 @@ tskv_status tskvgpu_upload_pages(tskv_ctx *ctx, const uint8_t *arena, uint64_t a
       if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream.get());
       uint64_t n_narrow[N_BINS] = {0};
       for (uint64_t p = 0; p < n_descs; p++)
-        if (pg->h_descs[p].phys_type != TSKV_PT_TIME) n_narrow[page_bin[p]] += narrow[p];
+        if (pg->h_descs[p].phys_type != TSKV_PT_TIME && narrow[p]) {
+          n_narrow[page_bin[p]]++;
+          std::vector<uint32_t> &cb = pg->col_bucket_pages[pg->h_descs[p].column_id];
+          cb[page_bin[p] * WL_SUB]--;
+          cb[page_bin[p] * WL_SUB + 1]++;
+        }
       for (int b = 0; b < N_BINS; b++)
         pg->h_bin_narrow[b] = n_narrow[b] == 0 ? NARROW_NONE : n_narrow[b] == pg->h_bin_pages[b] ? NARROW_ALL : NARROW_SOME;
     }
@@ -1761,7 +1808,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   P.work_page = s->d_work_page.get();
   P.work_slot = s->d_work_slot.get();
   P.work_qcol = s->d_work_qcol.get();
-  P.bin_cstart = s->d_bin_cstart.get();
+  P.region_start = s->d_region.get();
+  P.region_fill = s->d_bucket.get();
   P.cols = s->d_cols.get();
   P.state = slide ? s->d_pane_state.get() : s->d_state.get();
   P.task_counter = reinterpret_cast<uint32_t *>(s->d_aux.get());
@@ -1863,10 +1911,12 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
   if (!capturing) cudaEventRecord(s->ev0.get(), ctx->stream.get());
   unsigned long long *aux = s->d_aux.get();
   uint64_t launches = 0;
-  {  // state identities + the pass's scratch (task counters / status / counters, bin starts, work-list buckets): one launch
+  const SeriesIndex series{pages->d_series_sorted.get(), pages->d_rank_of.get(), (uint32_t)pages->series.size(), pages->series_min,
+                           pages->series_span};
+  {  // state identities + the pass's scratch (task counters / status / counters, work-list bucket fills): one launch
     const uint32_t init_blocks = (uint32_t)std::min<uint64_t>((s->kern_sl.total + 255) / 256, 4096);
-    k_init_state<<<std::max(1u, init_blocks), 256, 0, ctx->stream.get()>>>(s->params.state, s->kern_sl, aux, AUX_WORDS, s->d_bin_cstart.get(), N_BINS + 2,
-                                                                   s->d_bucket.get(), N_BINS * s->n_cols * WL_SUB);
+    k_init_state<<<std::max(1u, init_blocks), 256, 0, ctx->stream.get()>>>(s->params.state, s->kern_sl, aux, AUX_WORDS, s->d_bucket.get(),
+                                                                   N_BINS * s->n_cols * WL_SUB);
     launches++;
   }
   // slot of every column group: the row filter and the merge pass need it per GROUP; the work list finds a selected
@@ -1876,8 +1926,8 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     if (s->d_rank_slot) {
       CU_TRY(ctx, cudaMemsetAsync(s->d_rank_slot.get(), 0xff, pages->series.size() * 4, ctx->stream.get()));
       if (s->n_series_sel) {
-        k_select_ids<<<(s->n_series_sel + 255) / 256, 256, 0, ctx->stream.get()>>>(pages->d_series_sorted.get(), (uint32_t)pages->series.size(), s->d_series.get(),
-                                                                         s->n_series_sel, s->d_rank_slot.get());
+        k_select_ids<<<(s->n_series_sel + 255) / 256, 256, 0, ctx->stream.get()>>>(series, s->d_series.get(), s->n_series_sel,
+                                                                         s->d_rank_slot.get());
         launches++;
       }
     }
@@ -1900,10 +1950,8 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     A.rank_cg = pages->d_rank_cg.get();
     A.page_bin = pages->d_page_bin.get();
     // narrow pages apart only where a bin holds both kinds (NARROW_SOME kernels choose per chunk)
-    A.page_narrow = std::any_of(pages->h_bin_narrow, pages->h_bin_narrow + N_BINS, [](uint8_t m) { return m == NARROW_SOME; })
-                        ? pages->d_narrow.get() : nullptr;
-    A.set_series = pages->d_series_sorted.get();
-    A.n_set_series = (uint32_t)pages->series.size();
+    A.page_narrow = s->split_narrow ? pages->d_narrow.get() : nullptr;
+    A.series = series;
     A.series_ids = s->d_series.get();
     A.n_sel = s->d_series ? s->n_series_sel : (uint32_t)pages->series.size();
     A.split_log2 = s->walk_split_log2;
@@ -1915,19 +1963,18 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     A.cg_merge = pages->overlap.d_cg_merge.get();
     A.page_stats = s->preds.n ? pages->d_page_stats.get() : nullptr;
     A.preds = s->preds;
-    const uint32_t n_buckets = N_BINS * s->n_cols * WL_SUB;
-    A.bucket_count = s->d_bucket.get();
-    A.bucket_off = s->d_bucket.get() + n_buckets;
+    A.region_start = s->d_region.get();
+    A.bucket_fill = s->d_bucket.get();
     A.work_page = s->d_work_page.get();
     A.work_slot = s->d_work_slot.get();
     A.work_qcol = s->d_work_qcol.get();
     A.counters = s->d_counters;
     A.status = s->d_status;
     const uint32_t wblocks = std::max(1u, (uint32_t)((((uint64_t)A.n_sel << A.split_log2) + WL_THREADS - 1) / WL_THREADS));
-    if (A.n_sel) k_worklist_count<<<wblocks, WL_THREADS, n_buckets * 4, ctx->stream.get()>>>(A);
-    k_worklist_offsets<<<1, 256, 0, ctx->stream.get()>>>(s->d_bucket.get(), s->d_bucket.get() + n_buckets, s->n_cols * WL_SUB, s->d_bin_cstart.get());
-    if (A.n_sel) k_worklist_emit<<<wblocks, WL_THREADS, 2 * n_buckets * 4, ctx->stream.get()>>>(A);
-    launches += 3;
+    if (A.n_sel) {
+      k_worklist<<<wblocks, WL_THREADS, 2 * N_BINS * s->n_cols * WL_SUB * 4, ctx->stream.get()>>>(A);
+      launches++;
+    }
   }
   if (s->merge.n_rows && s->n_merge_pages) {  // overlapping chunks: decode the query's columns, merge + aggregate per row
     CU_TRY(ctx, cudaMemsetAsync(s->d_mvalid.get(), 0, (size_t)s->n_cols * s->merge.bm_words * 4, ctx->stream.get()));
@@ -1962,7 +2009,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       uint32_t gblocks = std::max(1u, std::min<uint32_t>((uint32_t)ctx->sm_count * 4, (n_bin + 7) / 8));
       k_gather_pages<<<gblocks, 256, 0, ctx->bin_stream[b].get()>>>(pages->h_mapped, pages->d_arena.get(), pages->d_descs.get(),
                                                               pages->d_time_page_of.get(), s->d_work_page.get(), s->d_work_qcol.get(),
-                                                              s->d_bin_cstart.get(), bin);
+                                                              s->d_region.get(), s->d_bucket.get(), s->n_cols * WL_SUB, bin);
       launches++;
       cudaEventRecord(s->ev_gather[b].get(), ctx->bin_stream[b].get());
       prev_gather = b;
@@ -1975,7 +2022,8 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       // the corrupt page.
       uint32_t gblocks = std::max(1u, std::min<uint32_t>((uint32_t)ctx->sm_count * 4, (n_bin + 7) / 8));
       k_verify_crc<<<gblocks, 256, 0, ctx->bin_stream[b].get()>>>(pages->d_arena.get(), pages->d_descs.get(), pages->d_time_page_of.get(),
-                                                            s->d_work_page.get(), s->d_work_qcol.get(), s->d_bin_cstart.get(), bin,
+                                                            s->d_work_page.get(), s->d_work_qcol.get(), s->d_region.get(), s->d_bucket.get(),
+                                                            s->n_cols * WL_SUB, bin,
                                                             pages->d_crc_tables.get(), s->d_crc_status, s->d_crc_err_page);
       launches++;
     }
@@ -2109,6 +2157,33 @@ tskv_status tskvgpu_scan_run(tskv_ctx *ctx, tskv_scan *s) {
   tskv_status st = enqueue_scan(ctx, s);
   if (st != TSKV_OK) return st;
   return sync_scan(ctx, s);
+}
+
+tskv_status tskvgpu_scan_work_list(tskv_ctx *ctx, tskv_scan *s, uint32_t *n_buckets, uint32_t *n_items, uint32_t *region_start,
+                                   uint32_t *fill, uint32_t *work_page, uint32_t *work_slot, uint8_t *work_qcol, uint8_t *page_bin,
+                                   uint8_t *page_narrow) {
+  if (!ctx || !s || !n_buckets || !n_items) return TSKV_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  ctx->set_error("");
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  const tskv_pages *pages = s->pages;
+  const uint32_t nb = N_BINS * s->n_cols * WL_SUB;
+  std::vector<uint32_t> start(nb + 1);
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream.get()));
+  CU_TRY(ctx, cudaMemcpy(start.data(), s->d_region.get(), start.size() * 4, cudaMemcpyDeviceToHost));
+  *n_buckets = nb;
+  *n_items = start[nb];
+  if (region_start) std::copy(start.begin(), start.end(), region_start);
+  if (fill) CU_TRY(ctx, cudaMemcpy(fill, s->d_bucket.get(), (size_t)nb * 4, cudaMemcpyDeviceToHost));
+  if (work_page && start[nb]) CU_TRY(ctx, cudaMemcpy(work_page, s->d_work_page.get(), (size_t)start[nb] * 4, cudaMemcpyDeviceToHost));
+  if (work_slot && start[nb]) CU_TRY(ctx, cudaMemcpy(work_slot, s->d_work_slot.get(), (size_t)start[nb] * 4, cudaMemcpyDeviceToHost));
+  if (work_qcol && start[nb]) CU_TRY(ctx, cudaMemcpy(work_qcol, s->d_work_qcol.get(), start[nb], cudaMemcpyDeviceToHost));
+  if (page_bin && pages->n_descs) CU_TRY(ctx, cudaMemcpy(page_bin, pages->d_page_bin.get(), pages->n_descs, cudaMemcpyDeviceToHost));
+  if (page_narrow && pages->n_descs) {
+    if (s->split_narrow) CU_TRY(ctx, cudaMemcpy(page_narrow, pages->d_narrow.get(), pages->n_descs, cudaMemcpyDeviceToHost));
+    else std::memset(page_narrow, 0, pages->n_descs);
+  }
+  return TSKV_OK;
 }
 
 tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_view *out) {

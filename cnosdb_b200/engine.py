@@ -226,6 +226,21 @@ class PreparedScan:
         self.engine._check(self.engine.lib.tskvgpu_scan_partials(self.engine.ctx, self.handle, C.byref(v)))
         return v
 
+    def work_list(self):
+        """The work list of the last pass (tskvgpu_scan_work_list): dict of region_start, fill, work_page, work_slot,
+        work_qcol and the page set's per-descriptor page_bin / page_narrow."""
+        lib, ctx = self.engine.lib, self.engine.ctx
+        nb, ni = C.c_uint32(0), C.c_uint32(0)
+        self.engine._check(lib.tskvgpu_scan_work_list(ctx, self.handle, C.byref(nb), C.byref(ni), *([None] * 7)))
+        n_descs = self.pages.n_pages
+        out = {"region_start": np.zeros(nb.value + 1, np.uint32), "fill": np.zeros(nb.value, np.uint32),
+               "work_page": np.zeros(ni.value, np.uint32), "work_slot": np.zeros(ni.value, np.uint32),
+               "work_qcol": np.zeros(ni.value, np.uint8), "page_bin": np.zeros(n_descs, np.uint8),
+               "page_narrow": np.zeros(n_descs, np.uint8)}
+        self.engine._check(lib.tskvgpu_scan_work_list(ctx, self.handle, C.byref(nb), C.byref(ni),
+                                                      *[a.ctypes.data for a in out.values()]))
+        return out
+
     def exchange_view(self):
         """(device pointer, length in 8-byte words) of the region a multi-GPU run all-gathers."""
         a, b = C.c_uint64(0), C.c_uint64(0)

@@ -350,6 +350,16 @@ tskv_status tskvgpu_scan_run(tskv_ctx *ctx, tskv_scan *scan);
 tskv_status tskvgpu_scan_enqueue(tskv_ctx *ctx, tskv_scan *scan);
 tskv_status tskvgpu_scan_sync(tskv_ctx *ctx, tskv_scan *scan);
 tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *scan, tskv_partials_view *out);
+/* The work list of the scan's last pass (after scan_run / scan_sync), for tests and diagnostics. Bucket
+ * k = (bin * n_columns + column) * 2 + narrow flag owns the items [region_start[k], region_start[k] + fill[k]).
+ * Outputs (each may be null): region_start [n_buckets + 1], fill [n_buckets], work_page / work_slot [n_items],
+ * work_qcol [n_items] (query column | 0x80 when the item brings its column group's time page), and per descriptor of
+ * the page set page_bin / page_narrow [n_descs] (decode-kind bin and narrow flag of a field page, what the walk keys
+ * its buckets on; page_narrow is all 0 when the scan does not keep narrow pages apart). *n_buckets and *n_items
+ * (= region_start[n_buckets]) are always written: call with null arrays first to size them. */
+tskv_status tskvgpu_scan_work_list(tskv_ctx *ctx, tskv_scan *scan, uint32_t *n_buckets, uint32_t *n_items,
+                                   uint32_t *region_start, uint32_t *fill, uint32_t *work_page, uint32_t *work_slot,
+                                   uint8_t *work_qcol, uint8_t *page_bin, uint8_t *page_narrow);
 /* Alternative with a single collective: all-gather the exchange region (device pointer + length in
  * 8-byte words) of every rank into `gathered` (rank-major, n_ranks * words) and merge locally. */
 tskv_status tskvgpu_scan_exchange_view(tskv_ctx *ctx, tskv_scan *scan, uint64_t *out_dptr, uint64_t *out_words);

@@ -316,6 +316,19 @@ extern "C" {
     pub fn tskvgpu_scan_enqueue(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
     pub fn tskvgpu_scan_sync(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
     pub fn tskvgpu_scan_partials(ctx: *mut tskv_ctx, scan: *mut tskv_scan, out: *mut tskv_partials_view) -> tskv_status;
+    pub fn tskvgpu_scan_work_list(
+        ctx: *mut tskv_ctx,
+        scan: *mut tskv_scan,
+        n_buckets: *mut u32,
+        n_items: *mut u32,
+        region_start: *mut u32,
+        fill: *mut u32,
+        work_page: *mut u32,
+        work_slot: *mut u32,
+        work_qcol: *mut u8,
+        page_bin: *mut u8,
+        page_narrow: *mut u8,
+    ) -> tskv_status;
     pub fn tskvgpu_scan_exchange_view(
         ctx: *mut tskv_ctx,
         scan: *mut tskv_scan,
