@@ -126,6 +126,7 @@ GPU_SYMBOLS = [
     "tskvgpu_scan_finalize_device", "tskvgpu_scan_destroy", "tskvgpu_version",
     "tskvgpu_scan_prepare_sliding", "tskvgpu_scan_aggregate_sliding",
     "tskvgpu_query_output_layout_grouped", "tskvgpu_scan_prepare_grouped", "tskvgpu_scan_aggregate_grouped",
+    "tskvgpu_query_output_layout_edges", "tskvgpu_scan_prepare_edges", "tskvgpu_scan_aggregate_edges",
 ]
 
 
@@ -192,6 +193,9 @@ def load_gpu_library():
     lib.tskvgpu_query_output_layout_grouped.argtypes = [vp, C.POINTER(Query), vp, C.c_uint32, C.POINTER(OutputLayout)]
     lib.tskvgpu_scan_prepare_grouped.argtypes = [vp, vp, C.POINTER(Query), vp, C.c_uint32, C.c_int64, C.POINTER(vp)]
     lib.tskvgpu_scan_aggregate_grouped.argtypes = [vp, vp, C.POINTER(Query), vp, C.c_uint32, C.c_int64, vp, vp]
+    lib.tskvgpu_query_output_layout_edges.argtypes = [vp, C.POINTER(Query), vp, vp, C.c_uint32, C.POINTER(OutputLayout)]
+    lib.tskvgpu_scan_prepare_edges.argtypes = [vp, vp, C.POINTER(Query), vp, vp, C.c_uint32, C.POINTER(vp)]
+    lib.tskvgpu_scan_aggregate_edges.argtypes = [vp, vp, C.POINTER(Query), vp, vp, C.c_uint32, vp, vp]
     lib.tskvgpu_scan_run.argtypes = [vp, vp]
     lib.tskvgpu_scan_enqueue.argtypes = [vp, vp]
     lib.tskvgpu_scan_sync.argtypes = [vp, vp]

@@ -122,7 +122,7 @@ __global__ void __launch_bounds__(128) k_merge_chunks(const ScanParams P, const 
   }
   BucketState bk;
   bk.valid = false; bk.floor_regime = false; bk.lo = 0; bk.hi = 0; bk.idx = 0;
-  if (!locate_bucket(P, t, bk)) {
+  if (!(P.edges ? locate_bucket<true>(P, t, bk) : locate_bucket<false>(P, t, bk))) {
     report_error(P, TSKV_ERR_BUCKET_RANGE, M.cg_time_page[cg]);
     return;
   }
@@ -192,8 +192,7 @@ __global__ void __launch_bounds__(128) k_merge_chunks(const ScanParams P, const 
       if (M.sel && (mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST))) {
         int64_t kf = t, kl = t;
         if (P.slot_bits) {
-          const uint64_t base = P.width > 0 ? (uint64_t)P.first_bucket_start + (uint64_t)((int64_t)bk.idx - 1) * (uint64_t)P.width
-                                            : (uint64_t)P.rel_base;
+          const uint64_t base = P.edges ? key_base<true>(P, (int64_t)bk.idx) : key_base<false>(P, (int64_t)bk.idx);
           kf = (int64_t)((((uint64_t)t - base) << P.slot_bits) | slot);
           kl = (int64_t)((((uint64_t)t - base) << P.slot_bits) | (P.slot_max - slot));
         }

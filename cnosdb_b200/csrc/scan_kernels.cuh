@@ -84,14 +84,18 @@ struct ScanParams {
   // wrap_lo = INT64_MIN). Floor-regime buckets end at floor_cap; rows below wrap_lo are located one by one.
   int64_t floor_cap, wrap_lo;
   int64_t first_bucket_start;
+  // Explicit time-bucket edges (tskvgpu_scan_prepare_edges; null for every other scan): bucket b is [edges[b], edges[b + 1]),
+  // n_buckets + 1 strictly increasing timestamps. width, origin_mod, floor_cap and wrap_lo are then unused (width = 0).
+  const int64_t *edges;
   uint32_t n_buckets;
   uint32_t group_by_series;
   uint64_t n_cells;
   // GROUP BY tags: group of every slot, < n_groups with n_groups * n_buckets < 2^32 (host-checked); null otherwise
   const uint32_t *slot_group;
   // first/last tie-break key. slot_bits == 0 (one slot per cell): key = timestamp itself.
-  // Otherwise key = rel << slot_bits | slot with rel = t - (bucket_start - width) in (0, 2*width)
-  // for bucketed scans and rel = t - rel_base for unbucketed ones; the host checked the bit budget.
+  // Otherwise key = rel << slot_bits | slot with rel = t - key_base(bucket): t - (bucket_start - width) in (0, 2*width)
+  // for tumbling scans, t - edges[b] + 1 in [1, edges[b + 1] - edges[b]] for edge scans and t - rel_base for unbucketed
+  // ones; the host checked the bit budget.
   uint32_t slot_bits;
   uint32_t slot_max;     // (1 << slot_bits) - 1
   int64_t rel_base;
@@ -667,6 +671,14 @@ __device__ __forceinline__ uint64_t warp_sum_u64(uint64_t v, uint32_t *carry) {
   return (low & 0xfffffffffffull) | (top << 44);
 }
 
+// Base of the FIRST / LAST tie-break key of bucket `bucket` (ScanParams::slot_bits): rel = t - base > 0. EDGES: an edge
+// scan (P.edges != null; a template argument so that the tumbling kernels hold none of its code).
+template <bool EDGES>
+__device__ __forceinline__ uint64_t key_base(const ScanParams &P, int64_t bucket) {
+  if constexpr (EDGES) return (uint64_t)__ldg(P.edges + bucket) - 1;
+  return P.width > 0 ? (uint64_t)P.first_bucket_start + (uint64_t)(bucket - 1) * (uint64_t)P.width : (uint64_t)P.rel_base;
+}
+
 // Partial aggregate of one (page, bucket) run, held in registers by one lane.
 struct RunAcc {
   uint32_t count;
@@ -682,7 +694,7 @@ struct RunAcc {
 // run for cell `gcell` (= qcol * n_cells + cell). When every flushing lane targets the same cell
 // (the common lock-step case of GROUP BY bucket) the partials are combined with a butterfly first
 // and one lane issues the atomics.
-template <bool SEL>
+template <bool SEL, bool EDGES>
 __device__ __forceinline__ void warp_flush(const ScanParams &P, uint64_t *stab, bool active, uint32_t qcol,
                                            uint64_t cell, int64_t bucket, uint8_t pt, uint8_t mask,
                                            RunAcc &a, uint32_t slot) {
@@ -696,8 +708,7 @@ __device__ __forceinline__ void warp_flush(const ScanParams &P, uint64_t *stab, 
   int64_t kf = a.first_ts, kl = a.last_ts;
   if (SEL && P.slot_bits) {
     // rel > 0 by construction (see ScanParams); the host checked rel_bits + slot_bits <= 62
-    uint64_t base = P.width > 0 ? (uint64_t)P.first_bucket_start + (uint64_t)(bucket - 1) * (uint64_t)P.width
-                                : (uint64_t)P.rel_base;
+    const uint64_t base = key_base<EDGES>(P, bucket);
     kf = (int64_t)((((uint64_t)a.first_ts - base) << P.slot_bits) | slot);
     kl = (int64_t)((((uint64_t)a.last_ts - base) << P.slot_bits) | (P.slot_max - slot));
   }
@@ -766,7 +777,33 @@ struct BucketState {
 
 // `sliding_window(t, w, w, origin, 0)` (time_window.rs:184-198): start = t - ((t - o + w) % w) with
 // truncating %, so for a negative dividend the window is (start - w, start] (kept as-is).
+// EDGES (an edge scan, P.edges): bucket b is [edges[b], edges[b + 1]) - floor semantics at every time, no wrapped regime.
+template <bool EDGES>
 __device__ __forceinline__ bool locate_bucket(const ScanParams &P, int64_t t, BucketState &b) {
+  if constexpr (EDGES) {
+    const int64_t *E = P.edges;
+    if (b.valid && t > b.hi && b.idx + 1 < P.n_buckets) {  // the next bucket: [b.hi + 1, edges[b.idx + 2])
+      const int64_t e2 = __ldg(E + b.idx + 2);
+      if (t < e2) {
+        b.lo = b.hi + 1;
+        b.hi = e2 - 1;
+        b.idx += 1;
+        return true;
+      }
+    }
+    if (t < __ldg(E) || t >= __ldg(E + P.n_buckets)) return false;
+    uint32_t lo = 0, hi = P.n_buckets - 1;  // the last bucket whose start is <= t
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi + 1) >> 1;
+      if (__ldg(E + mid) <= t) lo = mid; else hi = mid - 1;
+    }
+    b.lo = __ldg(E + lo);
+    b.hi = __ldg(E + lo + 1) - 1;
+    b.idx = lo;
+    b.valid = true;
+    b.floor_regime = true;
+    return true;
+  }
   if (P.width <= 0) {
     b.lo = INT64_MIN; b.hi = INT64_MAX; b.idx = 0; b.valid = true; b.floor_regime = false;
     return true;
@@ -1073,6 +1110,15 @@ __device__ __forceinline__ uint32_t rle_rows_within(uint64_t d, uint64_t delta, 
   return (uint32_t)min((uint64_t)left, q + 1);
 }
 
+// Edge scans, RLE row space: rows of the page from the row at time t (>= edges[b]) on that lie in bucket b, i.e. before
+// edges[b + 1] (0: the bucket ends before t). A bucket past the last one returns 1, so that the caller's step stops there
+// and reports TSKV_ERR_BUCKET_RANGE.
+__device__ __forceinline__ uint32_t edge_rows(const ScanParams &P, uint32_t b, uint64_t t, uint64_t delta, double inv) {
+  if (b >= P.n_buckets) return 1u;
+  const int64_t end = __ldg(P.edges + b + 1);
+  return (int64_t)t < end ? rle_rows_within((uint64_t)end - 1 - t, delta, inv, 0xffffffffu) : 0u;
+}
+
 // Time cursor of TK_GEN: any time codec straight from global memory, with the time validity bitmap. (The bitmap state
 // lives in the cursor so that the other time classes declare nothing they do not use.)
 struct GenTimeCursor : DeltaCursor<-1, BeStream> {
@@ -1088,7 +1134,7 @@ struct GenTimeCursor : DeltaCursor<-1, BeStream> {
 // timestamp of the row before it (leading NULLs: of the first valid row), so it never cuts a segment of its own.
 // NARROW (simple8b integer values, no FIRST / LAST): every page of the chunk is narrow (ScanParams.page_narrow), so the
 // values are decoded and accumulated in 32-bit arithmetic (S8bCursor::next32, ValueAcc::add32).
-template <int TK, int VK, bool SEL, bool NARROW>
+template <int TK, int VK, bool SEL, bool NARROW, bool EDGES>
 __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t item_begin, uint32_t item_end,
                                                uint32_t ring_base, uint64_t *stab, uint64_t *stage, uint4 *s_tomb,
                                                uint32_t part, uint32_t n_parts, uint32_t part_rows) {
@@ -1237,7 +1283,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
       if (__any_sync(FULL, flush)) {
         acc.count = va.count; acc.sum = va.sum; acc.sum_hi = va.sum_hi; acc.kmin = va.kmin; acc.kmax = va.kmax;
         const uint32_t fslot = have_item ? __ldg(P.work_slot + item) : 0u;
-        warp_flush<SEL>(P, stab, flush, qcol, group_cell_base(P, fslot) + run_idx, (int64_t)run_idx, pt, mask, acc, fslot);
+        warp_flush<SEL, EDGES>(P, stab, flush, qcol, group_cell_base(P, fslot) + run_idx, (int64_t)run_idx, pt, mask, acc, fslot);
       }
     } else {
       flush_runs<VK, NS>(P, stab, stage, staged, flush, qcol, group_base + run_idx, pt, mask, va);
@@ -1313,19 +1359,21 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
         }
         ra = min(max(ra, row), n_rows);  // this lane's rows: [row, n_rows)
         rb1 = min(max(rb1, row), n_rows);
-        if (P.width > 0 && ra < rb1) {
+        if ((P.width > 0 || EDGES) && ra < rb1) {
           const int64_t tr = (int64_t)(rle_t0 + (uint64_t)ra * rle_delta);
-          if ((int64_t)((uint64_t)tr - (uint64_t)P.origin_mod + (uint64_t)P.width) < 0) {
+          if (P.width > 0 && (int64_t)((uint64_t)tr - (uint64_t)P.origin_mod + (uint64_t)P.width) < 0) {
             elig = false;  // truncating-% regime (time_window.rs:184-198): general logic
-          } else if (!locate_bucket(P, tr, bk)) {
+          } else if (!locate_bucket<EDGES>(P, tr, bk)) {
             report_error(P, TSKV_ERR_BUCKET_RANGE, page);
             n_rows = 0;
           } else {
             bidx = bk.idx;
             nb = rle_rows_within((uint64_t)bk.hi - (uint64_t)tr, rle_delta, rle_inv, 0xffffffffu);
-            e_off = (uint64_t)tr + (uint64_t)nb * rle_delta - ((uint64_t)bk.hi + 1);
-            q32 = rle_rows_within((uint64_t)P.width, rle_delta, rle_inv, 0xffffffffu) - 1;
-            w_rem = (uint64_t)P.width - (uint64_t)q32 * rle_delta;
+            if (P.width > 0) {  // (edge scans step with edge_rows)
+              e_off = (uint64_t)tr + (uint64_t)nb * rle_delta - ((uint64_t)bk.hi + 1);
+              q32 = rle_rows_within((uint64_t)P.width, rle_delta, rle_inv, 0xffffffffu) - 1;
+              w_rem = (uint64_t)P.width - (uint64_t)q32 * rle_delta;
+            }
           }
         }
       }
@@ -1341,7 +1389,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   // same cell. The staged partials and their order are the ones the segment loop below makes for such a warp. Lanes
   // without rows walk along idle; a lane whose values run out stops decoding as there. (Not for the generic value
   // codecs: their larger cursor leaves no registers for a second loop.)
-  if (TK == TK_RLE && VK != VK_GEN && !SEL && fast && P.width > 0 && !P.group_by_series) {
+  if (TK == TK_RLE && VK != VK_GEN && !SEL && fast && (P.width > 0 || EDGES) && !P.group_by_series) {
     const bool mine = row < n_rows;
     const uint32_t with_rows = __ballot_sync(FULL, mine);
     const int src = with_rows ? __ffs(with_rows) - 1 : 0;
@@ -1365,6 +1413,10 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
       rb1 = __shfl_sync(FULL, rb1, src);
       bidx = __shfl_sync(FULL, bidx, src);
       nb = __shfl_sync(FULL, nb, src);
+      if (EDGES) {  // edge_rows steps from the row's time
+        rle_t0 = shfl_u64(rle_t0, src);
+        rle_inv = __longlong_as_double((long long)shfl_u64((uint64_t)__double_as_longlong(rle_inv), src));
+      }
       const uint64_t col = ((uint64_t)__shfl_sync(FULL, qcol, src) << 32) | __shfl_sync(FULL, (uint32_t)group_base, src);
       uint32_t end = __shfl_sync(FULL, n_rows, src);
       while (row < end) {  // one bitmap word per pass (`row` is a multiple of 32 here)
@@ -1386,11 +1438,18 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           uint32_t pend = r < ra ? min(ra, wend) : wend;
           if (in) {
             if (nb == 0) {  // next bucket (one narrower than the step may hold no row at all)
-              do {
-                bidx++;
-                nb = q32 + (e_off < w_rem ? 1u : 0u);
-                e_off = e_off + (uint64_t)nb * rle_delta - (uint64_t)P.width;
-              } while (nb == 0);
+              if (EDGES) {
+                do {
+                  bidx++;
+                  nb = edge_rows(P, bidx, rle_t0 + (uint64_t)r * rle_delta, rle_delta, rle_inv);
+                } while (nb == 0);
+              } else {
+                do {
+                  bidx++;
+                  nb = q32 + (e_off < w_rem ? 1u : 0u);
+                  e_off = e_off + (uint64_t)nb * rle_delta - (uint64_t)P.width;
+                } while (nb == 0);
+              }
               if (bidx >= P.n_buckets) {
                 if (n_rows) { report_error(P, TSKV_ERR_BUCKET_RANGE, page); n_rows = r; }
                 end = r;
@@ -1433,7 +1492,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   // or two). Pages whose first row falls just before a bucket edge would otherwise run one segment ahead of their
   // neighbours for the whole page, no two lanes would ever finish a run for the same cell in the same iteration, and
   // every flush would degenerate into 32 contended atomics instead of one staged store per lane.
-  const bool align = P.width > 0 && !P.group_by_series;
+  const bool align = (P.width > 0 || EDGES) && !P.group_by_series;
   bool pending = false;
   uint32_t seg_n = 0, seg_b = 0;  // pending segment: rows (RLE pages), bucket
   bool seg_in = false, seg_masked = false;
@@ -1454,8 +1513,12 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           seg_in = true;
           while (nb == 0) {  // next bucket (one narrower than the step may hold no row at all)
             bidx++;
-            nb = q32 + (e_off < w_rem ? 1u : 0u);
-            e_off = e_off + (uint64_t)nb * rle_delta - (uint64_t)P.width;
+            if (EDGES) {
+              nb = edge_rows(P, bidx, rle_t0 + (uint64_t)row * rle_delta, rle_delta, rle_inv);
+            } else {
+              nb = q32 + (e_off < w_rem ? 1u : 0u);
+              e_off = e_off + (uint64_t)nb * rle_delta - (uint64_t)P.width;
+            }
           }
           if (bidx >= P.n_buckets) {
             report_error(P, TSKV_ERR_BUCKET_RANGE, page);
@@ -1465,7 +1528,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           } else {
             seg_n = min(nb, rb1 - row);
             seg_b = bidx;
-            if (P.width > 0) nb -= seg_n;
+            if (P.width > 0 || EDGES) nb -= seg_n;
           }
         }
       } else {
@@ -1480,7 +1543,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           if (dropped) seg_in = false;
         }
         if (seg_in) {
-          if (!(bk.valid && pend_t >= bk.lo && pend_t <= bk.hi) && !locate_bucket(P, pend_t, bk)) {
+          if (!(bk.valid && pend_t >= bk.lo && pend_t <= bk.hi) && !locate_bucket<EDGES>(P, pend_t, bk)) {
             report_error(P, TSKV_ERR_BUCKET_RANGE, page);
             seg_in = false;
             bk.valid = false;
@@ -1657,7 +1720,7 @@ constexpr uint32_t SCAN_TOMB_BYTES = SCAN_THREADS * sizeof(uint4);
 // kernels choose per chunk; NARROW_ALL kernels hold the narrow arithmetic only (a kernel that holds both row loops runs
 // its narrow chunks ~1.5 % slower on C4: H100, see DESIGN.md §5).
 enum { NARROW_NONE = 0, NARROW_SOME = 1, NARROW_ALL = 2 };
-template <int TK, int VK, bool SEL, int NARROW>
+template <int TK, int VK, bool SEL, int NARROW, bool EDGES>
 __global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, SEL)) k_scan_aggregate(const __grid_constant__ ScanParams P, int bin) {
   static_assert(NARROW == NARROW_NONE || (TK != TK_GEN && VK == VK_S8B && !SEL), "narrow kernels: simple8b values, no FIRST / LAST");
   // dynamic shared memory: [per-CTA partial table, P.smem_words 8-byte words (or empty)] [per warp: a value ring,
@@ -1710,10 +1773,10 @@ __global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, SEL)) k_scan
       // vote also covers page sets without narrow flags in the work list)
       const uint32_t item = begin + lane;
       const bool narrow = __all_sync(FULL, item >= end || __ldg(P.page_narrow + __ldg(P.work_page + item)));
-      if (narrow) scan_chunk_seg<TK, VK, SEL, true>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
-      else scan_chunk_seg<TK, VK, SEL, false>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
+      if (narrow) scan_chunk_seg<TK, VK, SEL, true, EDGES>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
+      else scan_chunk_seg<TK, VK, SEL, false, EDGES>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
     } else {
-      scan_chunk_seg<TK, VK, SEL, NARROW == NARROW_ALL>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
+      scan_chunk_seg<TK, VK, SEL, NARROW == NARROW_ALL, EDGES>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
     }
   }
   if (P.use_smem) {  // merge this CTA's table into the global state, once

@@ -240,6 +240,8 @@ struct tskv_scan {
   // GROUP BY tags: the group of every slot (params.slot_group) and the work-list walk order, slots sorted by group (null
   // when that is the selection order)
   async_ptr<uint32_t> d_slot_group, d_walk;
+  // explicit time-bucket edges (params.edges; tskvgpu_scan_prepare_edges), null otherwise
+  async_ptr<int64_t> d_edges;
 };
 
 namespace {
@@ -318,26 +320,30 @@ unsigned popc8(unsigned x) { return (unsigned)__builtin_popcount(x & TSKV_AGG_AL
 
 typedef void (*scan_kernel_t)(const ScanParams, int);
 // `narrow`: NARROW_* of the bin's pages (tskv_pages::h_bin_narrow); only the simple8b-value kernels without FIRST / LAST
-// have narrow variants
-template <bool SEL>
+// have narrow variants; EDGES: the kernels of an edge scan (ScanParams.edges)
+template <bool SEL, bool EDGES>
 scan_kernel_t scan_kernel_for(int bin, int narrow = NARROW_NONE) {
   if constexpr (!SEL) {
-    if (narrow == NARROW_SOME && bin == TK_RLE * N_VK + VK_S8B) return k_scan_aggregate<TK_RLE, VK_S8B, false, NARROW_SOME>;
-    if (narrow == NARROW_SOME && bin == TK_S8B * N_VK + VK_S8B) return k_scan_aggregate<TK_S8B, VK_S8B, false, NARROW_SOME>;
-    if (narrow == NARROW_ALL && bin == TK_RLE * N_VK + VK_S8B) return k_scan_aggregate<TK_RLE, VK_S8B, false, NARROW_ALL>;
-    if (narrow == NARROW_ALL && bin == TK_S8B * N_VK + VK_S8B) return k_scan_aggregate<TK_S8B, VK_S8B, false, NARROW_ALL>;
+    if (narrow == NARROW_SOME && bin == TK_RLE * N_VK + VK_S8B) return k_scan_aggregate<TK_RLE, VK_S8B, false, NARROW_SOME, EDGES>;
+    if (narrow == NARROW_SOME && bin == TK_S8B * N_VK + VK_S8B) return k_scan_aggregate<TK_S8B, VK_S8B, false, NARROW_SOME, EDGES>;
+    if (narrow == NARROW_ALL && bin == TK_RLE * N_VK + VK_S8B) return k_scan_aggregate<TK_RLE, VK_S8B, false, NARROW_ALL, EDGES>;
+    if (narrow == NARROW_ALL && bin == TK_S8B * N_VK + VK_S8B) return k_scan_aggregate<TK_S8B, VK_S8B, false, NARROW_ALL, EDGES>;
   }
   switch (bin) {
-    case TK_RLE * N_VK + VK_S8B: return k_scan_aggregate<TK_RLE, VK_S8B, SEL, NARROW_NONE>;
-    case TK_RLE * N_VK + VK_GOR: return k_scan_aggregate<TK_RLE, VK_GOR, SEL, NARROW_NONE>;
-    case TK_RLE * N_VK + VK_GEN: return k_scan_aggregate<TK_RLE, VK_GEN, SEL, NARROW_NONE>;
-    case TK_S8B * N_VK + VK_S8B: return k_scan_aggregate<TK_S8B, VK_S8B, SEL, NARROW_NONE>;
-    case TK_S8B * N_VK + VK_GOR: return k_scan_aggregate<TK_S8B, VK_GOR, SEL, NARROW_NONE>;
-    case TK_S8B * N_VK + VK_GEN: return k_scan_aggregate<TK_S8B, VK_GEN, SEL, NARROW_NONE>;
-    case TK_GEN * N_VK + VK_S8B: return k_scan_aggregate<TK_GEN, VK_S8B, SEL, NARROW_NONE>;
-    case TK_GEN * N_VK + VK_GOR: return k_scan_aggregate<TK_GEN, VK_GOR, SEL, NARROW_NONE>;
-    default: return k_scan_aggregate<TK_GEN, VK_GEN, SEL, NARROW_NONE>;
+    case TK_RLE * N_VK + VK_S8B: return k_scan_aggregate<TK_RLE, VK_S8B, SEL, NARROW_NONE, EDGES>;
+    case TK_RLE * N_VK + VK_GOR: return k_scan_aggregate<TK_RLE, VK_GOR, SEL, NARROW_NONE, EDGES>;
+    case TK_RLE * N_VK + VK_GEN: return k_scan_aggregate<TK_RLE, VK_GEN, SEL, NARROW_NONE, EDGES>;
+    case TK_S8B * N_VK + VK_S8B: return k_scan_aggregate<TK_S8B, VK_S8B, SEL, NARROW_NONE, EDGES>;
+    case TK_S8B * N_VK + VK_GOR: return k_scan_aggregate<TK_S8B, VK_GOR, SEL, NARROW_NONE, EDGES>;
+    case TK_S8B * N_VK + VK_GEN: return k_scan_aggregate<TK_S8B, VK_GEN, SEL, NARROW_NONE, EDGES>;
+    case TK_GEN * N_VK + VK_S8B: return k_scan_aggregate<TK_GEN, VK_S8B, SEL, NARROW_NONE, EDGES>;
+    case TK_GEN * N_VK + VK_GOR: return k_scan_aggregate<TK_GEN, VK_GOR, SEL, NARROW_NONE, EDGES>;
+    default: return k_scan_aggregate<TK_GEN, VK_GEN, SEL, NARROW_NONE, EDGES>;
   }
+}
+template <bool SEL>
+scan_kernel_t scan_kernel_for(int bin, bool edges, int narrow = NARROW_NONE) {
+  return edges ? scan_kernel_for<SEL, true>(bin, narrow) : scan_kernel_for<SEL, false>(bin, narrow);
 }
 // the bin among 0-8 whose lane-per-page kernel also runs a short-page bin
 int serial_bin_of(int bin) {
@@ -417,8 +423,22 @@ const char *tag_groups_refusal(const tskv_pages *pages, const tskv_query *q, con
   return nullptr;
 }
 
-bool query_shape_ok(const tskv_query *q) {
-  return q->n_buckets != 0 && q->n_columns != 0 && q->columns && (q->width > 0 || q->n_buckets == 1);
+// Why an explicit time-bucket edge table (the *_edges entry points; `on`) is refused (TSKV_ERR_INVALID_ARG), or null.
+const char *edges_refusal(const tskv_query *q, bool on, const int64_t *edges) {
+  if (!on) return nullptr;
+  if (!edges || q->n_buckets == 0) return "time-bucket edges: edges must be non-null and n_buckets >= 1";
+  if (q->width != 0 || q->origin != 0 || q->first_bucket_start != 0)
+    return "time-bucket edges: width, origin and first_bucket_start must be 0 (the edges replace them)";
+  for (uint32_t b = 0; b < q->n_buckets; b++)
+    if (edges[b + 1] <= edges[b]) return "time-bucket edges: the edges must be strictly increasing";
+  if ((uint64_t)edges[q->n_buckets] - (uint64_t)edges[0] >= 1ull << 63)
+    return "time-bucket edges: edges[n_buckets] - edges[0] must be below 2^63";
+  return nullptr;
+}
+
+// (an edge scan's buckets come from its edge table, width = 0)
+bool query_shape_ok(const tskv_query *q, bool edges = false) {
+  return q->n_buckets != 0 && q->n_columns != 0 && q->columns && (q->width > 0 || q->n_buckets == 1 || edges);
 }
 
 // Output layout of a query that passed query_shape_ok and tag_groups_refusal.
@@ -438,8 +458,12 @@ tskv_output_layout output_layout(const tskv_pages *pages, const tskv_query *q, c
   return out;
 }
 
-tskv_status compute_layout(const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, tskv_output_layout *out) {
-  if (!pages || !q || !out || !query_shape_ok(q) || tag_groups_refusal(pages, q, tg)) return TSKV_ERR_INVALID_ARG;
+// edges_on: an edge scan's layout (tskvgpu_query_output_layout_edges), with its refusals.
+tskv_status compute_layout(const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, bool edges_on,
+                           const int64_t *edges, tskv_output_layout *out) {
+  if (!pages || !q || !out || edges_refusal(q, edges_on, edges) || !query_shape_ok(q, edges_on) ||
+      tag_groups_refusal(pages, q, tg))
+    return TSKV_ERR_INVALID_ARG;
   *out = output_layout(pages, q, tg);
   return TSKV_OK;
 }
@@ -653,12 +677,16 @@ tskv_status check_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_que
 // The refusals of the tskvgpu_scan_prepare* calls: sets the error and returns its status, or returns TSKV_OK with the
 // windows per row (1 unless slide > 0). Called under ctx->mu.
 tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide, const TagGroups &tg,
-                           uint32_t *win_k) {
+                           bool edges_on, const int64_t *edges, uint32_t *win_k) {
+  if (const char *why = edges_refusal(q, edges_on, edges)) {  // check_edges: the *_edges calls
+    ctx->set_error(why);
+    return TSKV_ERR_INVALID_ARG;
+  }
   if (const char *why = tag_groups_refusal(pages, q, tg)) {
     ctx->set_error(why);
     return TSKV_ERR_INVALID_ARG;
   }
-  if (!query_shape_ok(q)) {
+  if (!query_shape_ok(q, edges_on)) {
     ctx->set_error("invalid query (buckets / columns)");
     return TSKV_ERR_INVALID_ARG;
   }
@@ -711,14 +739,18 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
 
 // FIRST / LAST tie-break key (ScanParams::slot_bits / rel_base) of a scan with FIRST / LAST (has_sel). Refuses
 // (TSKV_ERR_UNSUPPORTED) a scan whose keys do not fit 62 bits.
-tskv_status plan_keys(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, bool has_sel, uint32_t *slot_bits,
-                      int64_t *rel_base) {
+tskv_status plan_keys(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges, bool has_sel,
+                      uint32_t *slot_bits, int64_t *rel_base) {
   const uint64_t n_slots = selected_slots(pages, q);
   *slot_bits = (q->group_by_series || n_slots <= 1) ? 0 : bits_for(n_slots - 1);
   *rel_base = 0;
   if (!has_sel || *slot_bits == 0) return TSKV_OK;
   unsigned rel_bits = 64;
-  if (q->width > 0) {
+  if (edges) {  // rel = t - edges[b] + 1 in [1, longest bucket]
+    uint64_t longest = 0;
+    for (uint32_t b = 0; b < q->n_buckets; b++) longest = std::max(longest, (uint64_t)edges[b + 1] - (uint64_t)edges[b]);
+    rel_bits = bits_for(longest);
+  } else if (q->width > 0) {
     if (q->width < (int64_t)1 << 61) rel_bits = bits_for(2 * (uint64_t)q->width);
   } else {
     // unbucketed: rel = t - (lower bound of every in-range timestamp). A single-rank scan tightens unbounded / loose
@@ -739,7 +771,8 @@ tskv_status plan_keys(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *
     }
   }
   if (rel_bits + *slot_bits > 62) {
-    ctx->set_error("first/last across series: (bucket width or time span) x series count does not fit the 62-bit tie-break key");
+    ctx->set_error("first/last across series: (bucket width, longest bucket or time span) x series count does not fit the 62-bit "
+                   "tie-break key");
     return TSKV_ERR_UNSUPPORTED;
   }
   return TSKV_OK;
@@ -828,7 +861,7 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
 }
 
 // Parts per page, resident CTAs per SM and grid of every bin's fused kernel (grid 0: the bin is not launched).
-void plan_grids(const tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, bool has_sel, uint32_t smem_words,
+void plan_grids(const tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, bool has_sel, bool edges, uint32_t smem_words,
                 uint32_t has_tomb, int grid[N_BINS], int occ[N_BINS], uint32_t parts[N_BINS], uint32_t part_rows[N_BINS]) {
   for (int b = 0; b < N_BINS; b++) { grid[b] = occ[b] = 0; parts[b] = 1; part_rows[b] = 0; }
   const double sel_frac = plan_selected_fraction(pages->series.data(), pages->series.size(), q->series_ids, q->n_series);
@@ -862,7 +895,7 @@ void plan_grids(const tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *
     uint32_t n_bin = pages->h_bin_pages[b];
     if (!n_bin) continue;
     const int sb = serial_bin_of(b);
-    const void *fn = (const void *)(!has_sel ? scan_kernel_for<false>(sb, pages->h_bin_narrow[b]) : scan_kernel_for<true>(sb));
+    const void *fn = (const void *)(!has_sel ? scan_kernel_for<false>(sb, edges, pages->h_bin_narrow[b]) : scan_kernel_for<true>(sb, edges));
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[b], fn, SCAN_THREADS, serial_smem_bytes(sb, smem_words, has_tomb));
     occ[b] = std::max(1, occ[b]);
     // (an estimate: the work list rounds each (column, narrow flag) bucket of the bin up to 32 items on its own, so the bin
@@ -950,7 +983,7 @@ tskv_status plan_merge_pages(tskv_ctx *ctx, const tskv_pages *pages, const tskv_
 // Creates the scan's events, allocates its device buffers (stream-ordered) and uploads the query's tables; sets the
 // error. *h2d: the bytes uploaded.
 tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, bool sliding,
-                       const ScanLayout &lay, tskv_scan *s, uint64_t *h2d) {
+                       const int64_t *edges, const ScanLayout &lay, tskv_scan *s, uint64_t *h2d) {
   const uint32_t n_items = pages->n_items;
   cudaStream_t st = ctx->stream.get();
   s->ev0 = new_event();
@@ -985,6 +1018,10 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
     if (e == cudaSuccess) e = upload(s->d_slot_group, tg.ids, n_slots, st);
     if (e == cudaSuccess && !walk.empty()) e = upload(s->d_walk, walk.data(), n_slots, st);
     *h2d += (n_slots + walk.size()) * 4;
+  }
+  if (edges) {  // explicit time-bucket edges (params.edges)
+    if (e == cudaSuccess) e = upload(s->d_edges, edges, (size_t)q->n_buckets + 1, st);
+    *h2d += ((uint64_t)q->n_buckets + 1) * 8;
   }
   if (e == cudaSuccess && q->series_ids) e = stream_alloc(s->d_rank_slot, pages->series.size(), st);
   // work-list regions: each (bin, query column, narrow flag) bucket holds as many items as the page set has field pages
@@ -1193,8 +1230,10 @@ tskv_status tskvgpu_ctx_create(int32_t device_id, tskv_ctx **out_ctx) {
         cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes);
     };
     for (int b = 0; b < N_SERIAL_BINS; b++) {
-      for (int nm = NARROW_NONE; nm <= NARROW_ALL; nm++) raise((const void *)scan_kernel_for<false>(b, nm));
-      raise((const void *)scan_kernel_for<true>(b));
+      for (const bool edges : {false, true}) {
+        for (int nm = NARROW_NONE; nm <= NARROW_ALL; nm++) raise((const void *)scan_kernel_for<false>(b, edges, nm));
+        raise((const void *)scan_kernel_for<true>(b, edges));
+      }
     }
     cudaGetLastError();
   }
@@ -1755,23 +1794,30 @@ tskv_status tskvgpu_decode_pages(tskv_ctx *ctx, const tskv_pages *pages, uint64_
 // ------------------------------------------------------------------------------------------------
 tskv_status tskvgpu_query_output_layout(const tskv_pages *pages, const tskv_query *q,
                                         tskv_output_layout *out) {
-  return compute_layout(pages, q, TagGroups{}, out);
+  return compute_layout(pages, q, TagGroups{}, false, nullptr, out);
 }
 
 tskv_status tskvgpu_query_output_layout_grouped(const tskv_pages *pages, const tskv_query *q, const uint32_t *group_ids,
                                                 uint32_t n_groups, tskv_output_layout *out) {
-  return compute_layout(pages, q, TagGroups{true, group_ids, n_groups}, out);
+  return compute_layout(pages, q, TagGroups{true, group_ids, n_groups}, false, nullptr, out);
 }
 
-// tskvgpu_scan_prepare; slide > 0: tskvgpu_scan_prepare_sliding with slide < width; tg.on: GROUP BY tags.
+tskv_status tskvgpu_query_output_layout_edges(const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                              const uint32_t *group_ids, uint32_t n_groups, tskv_output_layout *out) {
+  return compute_layout(pages, q, TagGroups{group_ids != nullptr, group_ids, n_groups}, true, edges, out);
+}
+
+// tskvgpu_scan_prepare; slide > 0: tskvgpu_scan_prepare_sliding with slide < width; tg.on: GROUP BY tags; edges_on:
+// tskvgpu_scan_prepare_edges (slide 0).
 static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
-                                const TagGroups &tg, tskv_scan **out_scan) {
+                                const TagGroups &tg, tskv_scan **out_scan, bool edges_on = false,
+                                const int64_t *edges = nullptr) {
   if (!ctx || !pages || !q || !out_scan) return TSKV_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(ctx->mu);
   ctx->set_error("");
   *out_scan = nullptr;
   uint32_t win_k = 1;
-  tskv_status st = validate_query(ctx, pages, q, slide, tg, &win_k);
+  tskv_status st = validate_query(ctx, pages, q, slide, tg, edges_on, edges, &win_k);
   if (st != TSKV_OK) return st;
   const tskv_output_layout L = output_layout(pages, q, tg);
   cudaSetDevice(ctx->device);
@@ -1779,7 +1825,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   for (uint32_t c = 0; c < q->n_columns; c++) has_sel |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
   uint32_t slot_bits = 0;
   int64_t rel_base = 0;
-  st = plan_keys(ctx, pages, q, has_sel, &slot_bits, &rel_base);
+  if (!edges_on) edges = nullptr;
+  st = plan_keys(ctx, pages, q, edges, has_sel, &slot_bits, &rel_base);
   if (st != TSKV_OK) return st;
   tskv_scan *s = new tskv_scan();
   s->ctx = ctx;
@@ -1797,7 +1844,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   s->sl = lay.sl;
   s->kern_sl = lay.kern_sl;
   uint64_t h2d = 0;
-  if ((st = alloc_scan(ctx, pages, q, tg, slide != 0, lay, s, &h2d)) != TSKV_OK) {
+  if ((st = alloc_scan(ctx, pages, q, tg, slide != 0, edges, lay, s, &h2d)) != TSKV_OK) {
     delete s;
     return st;
   }
@@ -1832,6 +1879,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
     P.wrap_lo = wlo < (__int128)INT64_MIN ? INT64_MIN : (int64_t)wlo;
   }
   P.first_bucket_start = (int64_t)((uint64_t)q->first_bucket_start + (uint64_t)(win_k - 1) * (uint64_t)P.width);
+  P.edges = s->d_edges.get();
   P.n_buckets = s->n_panes;
   P.group_by_series = q->group_by_series;
   P.n_cells = L.n_groups * s->n_panes;
@@ -1854,7 +1902,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   P.n_tomb_keys = pages->tomb.n_keys;
   P.n_tomb_global = pages->tomb.n_global;
   s->tomb_epoch = pages->tomb_epoch;
-  plan_grids(ctx, pages, q, has_sel, P.smem_words, P.has_tomb, s->grid, s->occ, P.bin_parts, P.bin_part_rows);
+  plan_grids(ctx, pages, q, has_sel, P.edges != nullptr, P.smem_words, P.has_tomb, s->grid, s->occ, P.bin_parts, P.bin_part_rows);
   s->chunk_epoch = pages->chunk_epoch;
   if (pages->overlap.merge_rows && (st = prepare_merge(ctx, pages, q, s, &h2d)) != TSKV_OK) {
     delete s;
@@ -1890,6 +1938,11 @@ tskv_status tskvgpu_scan_prepare_grouped(tskv_ctx *ctx, const tskv_pages *pages,
                                          uint32_t n_groups, int64_t slide, tskv_scan **out_scan) {
   const TagGroups tg{true, group_ids, n_groups};
   return slide ? prepare_sliding(ctx, pages, q, slide, tg, out_scan) : prepare_scan(ctx, pages, q, 0, tg, out_scan);
+}
+
+tskv_status tskvgpu_scan_prepare_edges(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                       const uint32_t *group_ids, uint32_t n_groups, tskv_scan **out_scan) {
+  return prepare_scan(ctx, pages, q, 0, TagGroups{group_ids != nullptr, group_ids, n_groups}, out_scan, true, edges);
 }
 
 // Enqueues one full pass on the context stream, no host synchronisation:
@@ -2030,7 +2083,8 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     if (!capturing) cudaEventRecord(s->ev_bin_start[b].get(), ctx->bin_stream[b].get());
     const int sb = serial_bin_of(b);
     void *args[] = {(void *)&s->params, (void *)&bin};
-    const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb) : scan_kernel_for<false>(sb, pages->h_bin_narrow[b]));
+    const bool edges = s->params.edges != nullptr;
+    const void *fn = (const void *)(s->has_sel ? scan_kernel_for<true>(sb, edges) : scan_kernel_for<false>(sb, edges, pages->h_bin_narrow[b]));
     CU_TRY(ctx, cudaLaunchKernel(fn, dim3(s->grid[b]), dim3(SCAN_THREADS), args, serial_smem_bytes(sb, s->params.smem_words, s->params.has_tomb),
                                  ctx->bin_stream[b].get()));
     cudaEvent_t ev_done = capturing ? s->ev_cjoin[b].get() : s->ev_bin_done[b].get();
@@ -2307,10 +2361,11 @@ void tskvgpu_scan_destroy(tskv_ctx *ctx, tskv_scan *s) {
 }
 
 static tskv_status scan_aggregate(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
-                                  const TagGroups &tg, uint64_t *out_values, uint8_t *out_validity) {
+                                  const TagGroups &tg, uint64_t *out_values, uint8_t *out_validity, bool edges_on = false,
+                                  const int64_t *edges = nullptr) {
   if (!out_values || !out_validity) return TSKV_ERR_INVALID_ARG;
   tskv_scan *s = nullptr;
-  tskv_status st = slide ? prepare_sliding(ctx, pages, q, slide, tg, &s) : prepare_scan(ctx, pages, q, 0, tg, &s);
+  tskv_status st = slide ? prepare_sliding(ctx, pages, q, slide, tg, &s) : prepare_scan(ctx, pages, q, 0, tg, &s, edges_on, edges);
   if (st != TSKV_OK) return st;
   st = tskvgpu_scan_run(ctx, s);
   if (st == TSKV_OK) st = tskvgpu_scan_finalize(ctx, s, out_values, out_validity);
@@ -2338,6 +2393,12 @@ tskv_status tskvgpu_scan_aggregate_sliding(tskv_ctx *ctx, const tskv_pages *page
 tskv_status tskvgpu_scan_aggregate_grouped(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const uint32_t *group_ids,
                                            uint32_t n_groups, int64_t slide, uint64_t *out_values, uint8_t *out_validity) {
   return scan_aggregate(ctx, pages, q, slide, TagGroups{true, group_ids, n_groups}, out_values, out_validity);
+}
+
+tskv_status tskvgpu_scan_aggregate_edges(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                         const uint32_t *group_ids, uint32_t n_groups, uint64_t *out_values, uint8_t *out_validity) {
+  return scan_aggregate(ctx, pages, q, 0, TagGroups{group_ids != nullptr, group_ids, n_groups}, out_values, out_validity, true,
+                        edges);
 }
 
 }  // extern "C"

@@ -47,6 +47,72 @@ def sliding_window_grid(lo, hi, window, slide, origin=0):
     return first, (last - first) // slide + 1
 
 
+_PER_SECOND = {"s": 1, "ms": 1_000, "us": 1_000_000, "ns": 1_000_000_000}
+_FIXED_DAYS = {"week": 7, "day": 1}
+_FIXED_SECONDS = {"hour": 3600, "minute": 60, "second": 1}
+CALENDAR_UNITS = ("year", "quarter", "month", "week", "day", "hour", "minute", "second")
+
+
+def _days_from_civil(y, m, d):
+    """Days since 1970-01-01 of the proleptic Gregorian date y-m-d (any year)."""
+    y -= m <= 2
+    era = y // 400
+    yoe = y - era * 400
+    doy = (153 * (m + (-3 if m > 2 else 9)) + 2) // 5 + d - 1
+    doe = yoe * 365 + yoe // 4 - yoe // 100 + doy
+    return era * 146097 + doe - 719468
+
+
+def _civil_from_days(z):
+    """(year, month, day) of the proleptic Gregorian date `z` days after 1970-01-01 (z may be negative)."""
+    z += 719468
+    era = z // 146097
+    doe = z - era * 146097
+    yoe = (doe - doe // 1460 + doe // 36524 - doe // 146096) // 365
+    doy = doe - (365 * yoe + yoe // 4 - yoe // 100)
+    mp = (5 * doy + 2) // 153
+    d = doy - (153 * mp + 2) // 5 + 1
+    m = mp + (3 if mp < 10 else -9)
+    return yoe + era * 400 + (m <= 2), m, d
+
+
+def calendar_edges(unit, t_lo, t_hi, precision="ns"):
+    """Time-bucket edges of GROUP BY date_trunc(unit, time) over the rows of [t_lo, t_hi] (int64 timestamps in
+    `precision`: "s", "ms", "us" or "ns"): an int64 array from date_trunc(unit, t_lo) to the first unit start after
+    t_hi, for Engine.scan_aggregate(..., edges=...). Proleptic Gregorian calendar in UTC (the time column carries no
+    zone), times before 1970 floor to the unit start at or before them, weeks start on Monday."""
+    if unit not in CALENDAR_UNITS:
+        raise ValueError("calendar_edges: unit must be one of %s" % (CALENDAR_UNITS,))
+    if precision not in _PER_SECOND:
+        raise ValueError("calendar_edges: precision must be one of %s" % (tuple(_PER_SECOND),))
+    t_lo, t_hi = int(t_lo), int(t_hi)
+    if t_lo > t_hi:
+        raise ValueError("calendar_edges: t_lo > t_hi")
+    per_day = 86400 * _PER_SECOND[precision]
+    if unit in _FIXED_SECONDS or unit in _FIXED_DAYS:
+        if unit in _FIXED_SECONDS:
+            w, start = _FIXED_SECONDS[unit] * _PER_SECOND[precision], 0
+        else:  # weeks from Monday 1969-12-29 (1970-01-01 is a Thursday)
+            w, start = _FIXED_DAYS[unit] * per_day, -3 * per_day if unit == "week" else 0
+        first = start + (t_lo - start) // w * w
+        n = (t_hi - first) // w + 1
+        edges = [first + k * w for k in range(n + 1)]
+    else:
+        months = {"year": 12, "quarter": 3, "month": 1}[unit]
+        y, m, _ = _civil_from_days(t_lo // per_day)
+        k = (y * 12 + m - 1) // months * months  # months since year 0 of the unit's start
+        edges = []
+        while True:
+            e = _days_from_civil(k // 12, k % 12 + 1, 1) * per_day
+            edges.append(e)
+            if e > t_hi:
+                break
+            k += months
+    if edges[0] < -2**63 or edges[-1] >= 2**63:
+        raise ValueError("calendar_edges: the edges leave the int64 range")
+    return np.array(edges, dtype=np.int64)
+
+
 class TskvError(RuntimeError):
     """Mirrors TskvError::Decode / TsmPageFileHashCheckFailed: carries the status code."""
 
@@ -389,11 +455,24 @@ class Engine:
             n_groups = int(ids.max()) + 1 if ids is not None and ids.size else 1
         return (None if ids is None else ids.ctypes.data), int(n_groups), ids
 
-    def output_layout(self, pages, query, group_ids=None, n_groups=None):
+    @staticmethod
+    def _edges(edges, slide):
+        """Explicit time-bucket edges as a contiguous int64 array (kept alive by the caller), or None."""
+        if edges is None:
+            return None
+        if slide is not None:
+            raise ValueError("edges and slide: sliding windows over explicit time-bucket edges are not supported")
+        return np.ascontiguousarray(edges, dtype=np.int64)
+
+    def output_layout(self, pages, query, group_ids=None, n_groups=None, edges=None):
         L = cabi.OutputLayout()
         q = query.to_c()
         g = self._group_map(group_ids, n_groups)
-        if g is None:
+        e = self._edges(edges, None)
+        if e is not None:
+            st = self.lib.tskvgpu_query_output_layout_edges(pages.handle, C.byref(q), e.ctypes.data,
+                                                            g[0] if g else None, g[1] if g else 0, C.byref(L))
+        elif g is None:
             st = self.lib.tskvgpu_query_output_layout(pages.handle, C.byref(q), C.byref(L))
         else:
             st = self.lib.tskvgpu_query_output_layout_grouped(pages.handle, C.byref(q), g[0], g[1], C.byref(L))
@@ -401,18 +480,25 @@ class Engine:
             raise TskvError(st, "invalid query")
         return L
 
-    def scan_aggregate(self, pages, query, slide=None, group_ids=None, n_groups=None):
+    def scan_aggregate(self, pages, query, slide=None, group_ids=None, n_groups=None, edges=None):
         """End-to-end call: query args H2D, fused scan, result D2H (BatchReader::process analogue).
         slide: sliding windows time_window(time, query.width, slide, query.origin); output bucket j is the window
         starting at query.first_bucket_start + j * slide (sliding_window_grid sizes that grid).
         group_ids: GROUP BY tags, group_ids[slot] = group of the slot-th selected series (n_groups groups, default
-        max + 1; the result has one row of buckets per group)."""
-        L = self.output_layout(pages, query, group_ids, n_groups)
+        max + 1; the result has one row of buckets per group).
+        edges: explicit time buckets [edges[b], edges[b + 1]) (query.n_buckets + 1 increasing timestamps, query.width,
+        origin and first_bucket_start 0; calendar_edges makes them for date_trunc). Not with slide."""
+        e = self._edges(edges, slide)
+        L = self.output_layout(pages, query, group_ids, n_groups, e)
         values = np.empty(int(L.n_out * L.n_cells), dtype=np.uint64)
         bitmaps = np.empty(int(L.validity_bytes), dtype=np.uint8)
         g = self._group_map(group_ids, n_groups)
         q = query.to_c()
-        if g is not None:
+        if e is not None:
+            st = self.lib.tskvgpu_scan_aggregate_edges(self.ctx, pages.handle, C.byref(q), e.ctypes.data,
+                                                       g[0] if g else None, g[1] if g else 0,
+                                                       values.ctypes.data, bitmaps.ctypes.data)
+        elif g is not None:
             st = self.lib.tskvgpu_scan_aggregate_grouped(self.ctx, pages.handle, C.byref(q), g[0], g[1], int(slide or 0),
                                                          values.ctypes.data, bitmaps.ctypes.data)
         elif slide is None:
@@ -423,13 +509,18 @@ class Engine:
         self._check(st)
         return ScanResult(query, L, values, bitmaps)
 
-    def prepare(self, pages, query, slide=None, group_ids=None, n_groups=None):
-        """Device-resident scan (run / enqueue / partials / exchange / finalize); slide, group_ids: as in scan_aggregate."""
-        L = self.output_layout(pages, query, group_ids, n_groups)
+    def prepare(self, pages, query, slide=None, group_ids=None, n_groups=None, edges=None):
+        """Device-resident scan (run / enqueue / partials / exchange / finalize); slide, group_ids, edges: as in
+        scan_aggregate."""
+        e = self._edges(edges, slide)
+        L = self.output_layout(pages, query, group_ids, n_groups, e)
         g = self._group_map(group_ids, n_groups)
         q = query.to_c()
         h = C.c_void_p()
-        if g is not None:
+        if e is not None:
+            st = self.lib.tskvgpu_scan_prepare_edges(self.ctx, pages.handle, C.byref(q), e.ctypes.data,
+                                                     g[0] if g else None, g[1] if g else 0, C.byref(h))
+        elif g is not None:
             st = self.lib.tskvgpu_scan_prepare_grouped(self.ctx, pages.handle, C.byref(q), g[0], g[1], int(slide or 0), C.byref(h))
         elif slide is None:
             st = self.lib.tskvgpu_scan_prepare(self.ctx, pages.handle, C.byref(q), C.byref(h))

@@ -433,6 +433,25 @@ tskv_status tskvgpu_scan_aggregate_grouped(tskv_ctx *ctx, const tskv_pages *page
                                            const uint32_t *group_ids, uint32_t n_groups, int64_t slide,
                                            uint64_t *out_values, uint8_t *out_validity);
 
+/* ---- explicit time-bucket edges: GROUP BY date_trunc(unit, time) and other irregular grids ----------------
+ * Time bucket b (0 <= b < q->n_buckets) is the half-open interval [edges[b], edges[b + 1]). edges holds q->n_buckets + 1
+ * strictly increasing timestamps (the time column's unit). q->width, q->origin and q->first_bucket_start must be 0: the
+ * edges replace them. A selected row outside [edges[0], edges[n_buckets]) is TSKV_ERR_BUCKET_RANGE, as a row off the
+ * tumbling grid is. group_ids == NULL: no tag groups (group_by_series may be set). Otherwise group_ids / n_groups work as in
+ * tskvgpu_scan_prepare_grouped. FIRST / LAST: (page, time bucket) runs and tie-break keys as in the tumbling scan, with
+ * rel = t - edges[b] + 1 and the 62-bit budget taken from the longest bucket. The scan returned works with every tskvgpu_scan_*
+ * call, including TSKV_QUERY_MULTI_RANK exchange (every rank passes the same edges).
+ * Refused before any launch:
+ *   TSKV_ERR_INVALID_ARG   edges == NULL, n_buckets == 0, edges not strictly increasing, edges[n] - edges[0] >= 2^63,
+ *                          width / origin / first_bucket_start != 0, a bad group map, or n_groups * n_buckets > TSKV_MAX_GROUPED_CELLS
+ *   TSKV_ERR_UNSUPPORTED   FIRST / LAST across series whose keys do not fit (bits(longest bucket) + slot bits > 62) */
+tskv_status tskvgpu_query_output_layout_edges(const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                              const uint32_t *group_ids, uint32_t n_groups, tskv_output_layout *out);
+tskv_status tskvgpu_scan_prepare_edges(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                       const uint32_t *group_ids, uint32_t n_groups, tskv_scan **out_scan);
+tskv_status tskvgpu_scan_aggregate_edges(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                         const uint32_t *group_ids, uint32_t n_groups, uint64_t *out_values, uint8_t *out_validity);
+
 /* Library version / build info ("tskv-b200 <semver> sm_90a"). */
 const char *tskvgpu_version(void);
 

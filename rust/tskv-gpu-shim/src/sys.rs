@@ -312,6 +312,33 @@ extern "C" {
         out_values: *mut u64,
         out_validity: *mut u8,
     ) -> tskv_status;
+    pub fn tskvgpu_query_output_layout_edges(
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        edges: *const i64,
+        group_ids: *const u32,
+        n_groups: u32,
+        out: *mut tskv_output_layout,
+    ) -> tskv_status;
+    pub fn tskvgpu_scan_prepare_edges(
+        ctx: *mut tskv_ctx,
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        edges: *const i64,
+        group_ids: *const u32,
+        n_groups: u32,
+        out_scan: *mut *mut tskv_scan,
+    ) -> tskv_status;
+    pub fn tskvgpu_scan_aggregate_edges(
+        ctx: *mut tskv_ctx,
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        edges: *const i64,
+        group_ids: *const u32,
+        n_groups: u32,
+        out_values: *mut u64,
+        out_validity: *mut u8,
+    ) -> tskv_status;
     pub fn tskvgpu_scan_run(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
     pub fn tskvgpu_scan_enqueue(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
     pub fn tskvgpu_scan_sync(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
