@@ -127,6 +127,7 @@ GPU_SYMBOLS = [
     "tskvgpu_scan_prepare_sliding", "tskvgpu_scan_aggregate_sliding",
     "tskvgpu_query_output_layout_grouped", "tskvgpu_scan_prepare_grouped", "tskvgpu_scan_aggregate_grouped",
     "tskvgpu_query_output_layout_edges", "tskvgpu_scan_prepare_edges", "tskvgpu_scan_aggregate_edges",
+    "tskvgpu_query_output_layout_labels", "tskvgpu_scan_prepare_labels", "tskvgpu_scan_aggregate_labels",
 ]
 
 
@@ -196,6 +197,10 @@ def load_gpu_library():
     lib.tskvgpu_query_output_layout_edges.argtypes = [vp, C.POINTER(Query), vp, vp, C.c_uint32, C.POINTER(OutputLayout)]
     lib.tskvgpu_scan_prepare_edges.argtypes = [vp, vp, C.POINTER(Query), vp, vp, C.c_uint32, C.POINTER(vp)]
     lib.tskvgpu_scan_aggregate_edges.argtypes = [vp, vp, C.POINTER(Query), vp, vp, C.c_uint32, vp, vp]
+    lib.tskvgpu_query_output_layout_labels.argtypes = [vp, C.POINTER(Query), vp, C.c_uint32, vp, vp, C.c_uint32,
+                                                       C.POINTER(OutputLayout)]
+    lib.tskvgpu_scan_prepare_labels.argtypes = [vp, vp, C.POINTER(Query), vp, C.c_uint32, vp, vp, C.c_uint32, C.POINTER(vp)]
+    lib.tskvgpu_scan_aggregate_labels.argtypes = [vp, vp, C.POINTER(Query), vp, C.c_uint32, vp, vp, C.c_uint32, vp, vp]
     lib.tskvgpu_scan_run.argtypes = [vp, vp]
     lib.tskvgpu_scan_enqueue.argtypes = [vp, vp]
     lib.tskvgpu_scan_sync.argtypes = [vp, vp]

@@ -126,7 +126,8 @@ __global__ void __launch_bounds__(128) k_merge_chunks(const ScanParams P, const 
     report_error(P, TSKV_ERR_BUCKET_RANGE, M.cg_time_page[cg]);
     return;
   }
-  const uint64_t cell = group_cell_base(P, slot) + bk.idx;
+  // (the edge scans' cell rule: every other scan has cell_buckets = 0, which gives the tumbling one)
+  const uint64_t cell = group_cell_base<true>(P, slot) + bucket_cell<true>(P, bk.idx);
 
   // ---- FIRST / LAST: is this the earliest / latest merged row of the group that lands in this bucket? (the merged rows of
   // a group are one record batch, so its rows of one bucket are one run: a surviving, in-range row of any stream with an

@@ -78,6 +78,11 @@ struct ScanParams {
   unsigned long long *stats;    // [0] points decoded, [1] rows in range
   tskv_time_range ranges[MAX_RANGES];
   uint32_t n_ranges;
+  // Labelled edge scans (tskvgpu_scan_prepare_labels; 0 for every other scan): the output buckets per group. Edge bucket
+  // b then aggregates into output bucket labels[b] < cell_buckets of its group (bucket_cell); the labels follow the
+  // n_buckets + 1 edges in the edge table's buffer. (A field in the padding after n_ranges, read only by the EDGES kernels
+  // and the merge pass: the tumbling kernels' parameters keep their offsets and their code stays as it was.)
+  uint32_t cell_buckets;
   int64_t width;         // <= 0: single bucket
   int64_t origin_mod;    // origin % width; a sliding scan's panes: origin % window, which may lie outside (-width, width)
   // Rows whose dividend t - origin_mod + width does not wrap: [wrap_lo, floor_cap] (set by the host; a tumbling scan has
@@ -87,10 +92,10 @@ struct ScanParams {
   // Explicit time-bucket edges (tskvgpu_scan_prepare_edges; null for every other scan): bucket b is [edges[b], edges[b + 1]),
   // n_buckets + 1 strictly increasing timestamps. width, origin_mod, floor_cap and wrap_lo are then unused (width = 0).
   const int64_t *edges;
-  uint32_t n_buckets;
+  uint32_t n_buckets;  // time buckets of the grid (edge scans: edge buckets; cell_buckets: a labelled scan's output buckets)
   uint32_t group_by_series;
   uint64_t n_cells;
-  // GROUP BY tags: group of every slot, < n_groups with n_groups * n_buckets < 2^32 (host-checked); null otherwise
+  // GROUP BY tags: group of every slot, < n_groups with n_groups * cell_buckets < 2^32 (host-checked); null otherwise
   const uint32_t *slot_group;
   // first/last tie-break key. slot_bits == 0 (one slot per cell): key = timestamp itself.
   // Otherwise key = rel << slot_bits | slot with rel = t - key_base(bucket): t - (bucket_start - width) in (0, 2*width)
@@ -133,10 +138,28 @@ struct ScanParams {
 };
 
 // First cell of the group a work item's series belongs to: GROUP BY tags slot_group[slot], GROUP BY series the slot
-// itself, GROUP BY bucket the one group. Read once per page.
+// itself, GROUP BY bucket the one group. Read once per page. A group holds n_buckets cells, or cell_buckets in a labelled
+// edge scan (EDGES: the kernels of an edge scan, the only ones that read cell_buckets).
+template <bool EDGES>
 __device__ __forceinline__ uint64_t group_cell_base(const ScanParams &P, uint32_t slot) {
+  if constexpr (EDGES) {
+    const uint64_t per = P.cell_buckets ? P.cell_buckets : P.n_buckets;
+    if (P.slot_group) return __ldg(P.slot_group + slot) * per;
+    return P.group_by_series ? slot * per : 0;
+  }
   if (P.slot_group) return (uint64_t)__ldg(P.slot_group + slot) * P.n_buckets;
   return P.group_by_series ? (uint64_t)slot * P.n_buckets : 0;
+}
+
+// Output bucket of bucket b within its group: labels[b] for a labelled edge scan, b for every other scan. Every bucket ->
+// cell step goes through here. `need`: the lane uses the result (a lane that does not skips the load).
+template <bool EDGES>
+__device__ __forceinline__ uint32_t bucket_cell(const ScanParams &P, uint32_t b, bool need = true) {
+  if constexpr (EDGES) {
+    const uint32_t *labels = reinterpret_cast<const uint32_t *>(P.edges + P.n_buckets + 1);
+    return (P.cell_buckets && need) ? __ldg(labels + b) : b;
+  }
+  return b;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1273,7 +1296,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   const uint64_t flip = pt == TSKV_PT_U64 ? 0x8000000000000000ull : 0ull;
   // (the FIRST / LAST variants read the slot and its group again at each flush: holding them takes registers those
   // kernels do not have, ptxas spills)
-  const uint64_t group_base = SEL ? 0 : group_cell_base(P, slot);
+  const uint64_t group_base = SEL ? 0 : group_cell_base<EDGES>(P, slot);
   uint32_t staged = 0;  // staged flush slots in use (warp-uniform)
 
   // Finished runs of the flushing lanes -> partial tables.
@@ -1283,10 +1306,11 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
       if (__any_sync(FULL, flush)) {
         acc.count = va.count; acc.sum = va.sum; acc.sum_hi = va.sum_hi; acc.kmin = va.kmin; acc.kmax = va.kmax;
         const uint32_t fslot = have_item ? __ldg(P.work_slot + item) : 0u;
-        warp_flush<SEL, EDGES>(P, stab, flush, qcol, group_cell_base(P, fslot) + run_idx, (int64_t)run_idx, pt, mask, acc, fslot);
+        warp_flush<SEL, EDGES>(P, stab, flush, qcol, group_cell_base<EDGES>(P, fslot) + bucket_cell<EDGES>(P, run_idx, flush),
+                               (int64_t)run_idx, pt, mask, acc, fslot);
       }
     } else {
-      flush_runs<VK, NS>(P, stab, stage, staged, flush, qcol, group_base + run_idx, pt, mask, va);
+      flush_runs<VK, NS>(P, stab, stage, staged, flush, qcol, group_base + bucket_cell<EDGES>(P, run_idx, flush), pt, mask, va);
     }
   };
   // One row's value: validity bit, decode (every valid row is decoded - rows outside the time ranges too, the streams
@@ -1476,7 +1500,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
           if (n_rows) check_values();
           if (in && (nb == 0 || r == rb1)) {  // the bucket's last row: its partial goes to the staging area
             va.fold(pt, NARROW);
-            stage_partial<VK, NS>(P, stab, stage, staged, n_rows && va.count, va, lane == 0, col + bidx);
+            stage_partial<VK, NS>(P, stab, stage, staged, n_rows && va.count, va, lane == 0, col + bucket_cell<EDGES>(P, bidx));
             va.reset(NARROW);
           }
         }

@@ -240,7 +240,8 @@ struct tskv_scan {
   // GROUP BY tags: the group of every slot (params.slot_group) and the work-list walk order, slots sorted by group (null
   // when that is the selection order)
   async_ptr<uint32_t> d_slot_group, d_walk;
-  // explicit time-bucket edges (params.edges; tskvgpu_scan_prepare_edges), null otherwise
+  // explicit time-bucket edges (params.edges; tskvgpu_scan_prepare_edges / _labels), null otherwise; a labelled scan's
+  // labels (uint32) follow its n + 1 edges
   async_ptr<int64_t> d_edges;
 };
 
@@ -423,17 +424,43 @@ const char *tag_groups_refusal(const tskv_pages *pages, const tskv_query *q, con
   return nullptr;
 }
 
-// Why an explicit time-bucket edge table (the *_edges entry points; `on`) is refused (TSKV_ERR_INVALID_ARG), or null.
-const char *edges_refusal(const tskv_query *q, bool on, const int64_t *edges) {
-  if (!on) return nullptr;
-  if (!edges || q->n_buckets == 0) return "time-bucket edges: edges must be non-null and n_buckets >= 1";
+// Explicit time-bucket edges (the *_edges and *_labels entry points; `on`): n edge buckets [edges[b], edges[b + 1]).
+// labelled (the *_labels calls): edge bucket b aggregates into output bucket labels[b] < q->n_buckets. Otherwise the edge
+// buckets are the output buckets, n = q->n_buckets.
+struct BucketEdges {
+  bool on = false;
+  const int64_t *edges = nullptr;
+  uint32_t n = 0;
+  bool labelled = false;
+  const uint32_t *labels = nullptr;
+};
+
+// Why an explicit time-bucket edge table or its labels are refused (TSKV_ERR_INVALID_ARG), or null.
+const char *edges_refusal(const tskv_query *q, const BucketEdges &E) {
+  if (!E.on) return nullptr;
+  if (E.labelled) {
+    if (!E.labels || E.n == 0 || q->n_buckets == 0)
+      return "bucket labels: labels must be non-null, n_edge >= 1 and n_buckets >= 1";
+    for (uint32_t b = 0; b < E.n; b++)
+      if (E.labels[b] >= q->n_buckets) return "bucket labels: a label is >= n_buckets";
+  }
+  if (!E.edges || E.n == 0) return "time-bucket edges: edges must be non-null and n_buckets >= 1";
   if (q->width != 0 || q->origin != 0 || q->first_bucket_start != 0)
     return "time-bucket edges: width, origin and first_bucket_start must be 0 (the edges replace them)";
-  for (uint32_t b = 0; b < q->n_buckets; b++)
-    if (edges[b + 1] <= edges[b]) return "time-bucket edges: the edges must be strictly increasing";
-  if ((uint64_t)edges[q->n_buckets] - (uint64_t)edges[0] >= 1ull << 63)
+  for (uint32_t b = 0; b < E.n; b++)
+    if (E.edges[b + 1] <= E.edges[b]) return "time-bucket edges: the edges must be strictly increasing";
+  if ((uint64_t)E.edges[E.n] - (uint64_t)E.edges[0] >= 1ull << 63)
     return "time-bucket edges: edges[n_buckets] - edges[0] must be below 2^63";
   return nullptr;
+}
+
+// Labelled edge scans refuse FIRST / LAST (TSKV_ERR_UNSUPPORTED): the reference takes a record batch's earliest row per
+// label, and the NULL rule at that row then acts across the page's edge buckets of one label (DESIGN.md section 7).
+bool labels_first_last(const tskv_query *q, const BucketEdges &E) {
+  if (!E.labelled) return false;
+  for (uint32_t c = 0; c < q->n_columns; c++)
+    if (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) return true;
+  return false;
 }
 
 // (an edge scan's buckets come from its edge table, width = 0)
@@ -458,12 +485,12 @@ tskv_output_layout output_layout(const tskv_pages *pages, const tskv_query *q, c
   return out;
 }
 
-// edges_on: an edge scan's layout (tskvgpu_query_output_layout_edges), with its refusals.
-tskv_status compute_layout(const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, bool edges_on,
-                           const int64_t *edges, tskv_output_layout *out) {
-  if (!pages || !q || !out || edges_refusal(q, edges_on, edges) || !query_shape_ok(q, edges_on) ||
-      tag_groups_refusal(pages, q, tg))
+// E.on: an edge scan's layout (tskvgpu_query_output_layout_edges / _labels), with its refusals.
+tskv_status compute_layout(const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, const BucketEdges &E,
+                           tskv_output_layout *out) {
+  if (!pages || !q || !out || edges_refusal(q, E) || !query_shape_ok(q, E.on) || tag_groups_refusal(pages, q, tg))
     return TSKV_ERR_INVALID_ARG;
+  if (labels_first_last(q, E)) return TSKV_ERR_UNSUPPORTED;
   *out = output_layout(pages, q, tg);
   return TSKV_OK;
 }
@@ -677,8 +704,8 @@ tskv_status check_sliding(tskv_ctx *ctx, const tskv_pages *pages, const tskv_que
 // The refusals of the tskvgpu_scan_prepare* calls: sets the error and returns its status, or returns TSKV_OK with the
 // windows per row (1 unless slide > 0). Called under ctx->mu.
 tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide, const TagGroups &tg,
-                           bool edges_on, const int64_t *edges, uint32_t *win_k) {
-  if (const char *why = edges_refusal(q, edges_on, edges)) {  // check_edges: the *_edges calls
+                           const BucketEdges &E, uint32_t *win_k) {
+  if (const char *why = edges_refusal(q, E)) {  // the *_edges and *_labels calls
     ctx->set_error(why);
     return TSKV_ERR_INVALID_ARG;
   }
@@ -686,7 +713,7 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
     ctx->set_error(why);
     return TSKV_ERR_INVALID_ARG;
   }
-  if (!query_shape_ok(q, edges_on)) {
+  if (!query_shape_ok(q, E.on)) {
     ctx->set_error("invalid query (buckets / columns)");
     return TSKV_ERR_INVALID_ARG;
   }
@@ -733,22 +760,26 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
       return TSKV_ERR_INVALID_ARG;
     }
   }
+  if (labels_first_last(q, E)) {
+    ctx->set_error("bucket labels: first / last are not supported (the reference takes each batch's earliest row per label)");
+    return TSKV_ERR_UNSUPPORTED;
+  }
   *win_k = 1;
   return slide ? check_sliding(ctx, pages, q, slide, win_k) : TSKV_OK;
 }
 
 // FIRST / LAST tie-break key (ScanParams::slot_bits / rel_base) of a scan with FIRST / LAST (has_sel). Refuses
 // (TSKV_ERR_UNSUPPORTED) a scan whose keys do not fit 62 bits.
-tskv_status plan_keys(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges, bool has_sel,
+tskv_status plan_keys(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const BucketEdges &E, bool has_sel,
                       uint32_t *slot_bits, int64_t *rel_base) {
   const uint64_t n_slots = selected_slots(pages, q);
   *slot_bits = (q->group_by_series || n_slots <= 1) ? 0 : bits_for(n_slots - 1);
   *rel_base = 0;
   if (!has_sel || *slot_bits == 0) return TSKV_OK;
   unsigned rel_bits = 64;
-  if (edges) {  // rel = t - edges[b] + 1 in [1, longest bucket]
+  if (E.on) {  // rel = t - edges[b] + 1 in [1, longest bucket]
     uint64_t longest = 0;
-    for (uint32_t b = 0; b < q->n_buckets; b++) longest = std::max(longest, (uint64_t)edges[b + 1] - (uint64_t)edges[b]);
+    for (uint32_t b = 0; b < E.n; b++) longest = std::max(longest, (uint64_t)E.edges[b + 1] - (uint64_t)E.edges[b]);
     rel_bits = bits_for(longest);
   } else if (q->width > 0) {
     if (q->width < (int64_t)1 << 61) rel_bits = bits_for(2 * (uint64_t)q->width);
@@ -983,7 +1014,7 @@ tskv_status plan_merge_pages(tskv_ctx *ctx, const tskv_pages *pages, const tskv_
 // Creates the scan's events, allocates its device buffers (stream-ordered) and uploads the query's tables; sets the
 // error. *h2d: the bytes uploaded.
 tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const TagGroups &tg, bool sliding,
-                       const int64_t *edges, const ScanLayout &lay, tskv_scan *s, uint64_t *h2d) {
+                       const BucketEdges &E, const ScanLayout &lay, tskv_scan *s, uint64_t *h2d) {
   const uint32_t n_items = pages->n_items;
   cudaStream_t st = ctx->stream.get();
   s->ev0 = new_event();
@@ -1019,9 +1050,14 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
     if (e == cudaSuccess && !walk.empty()) e = upload(s->d_walk, walk.data(), n_slots, st);
     *h2d += (n_slots + walk.size()) * 4;
   }
-  if (edges) {  // explicit time-bucket edges (params.edges)
-    if (e == cudaSuccess) e = upload(s->d_edges, edges, (size_t)q->n_buckets + 1, st);
-    *h2d += ((uint64_t)q->n_buckets + 1) * 8;
+  if (E.on) {  // explicit time-bucket edges (params.edges), then the labels of a labelled scan (bucket_cell)
+    std::vector<int64_t> table(E.edges, E.edges + (size_t)E.n + 1);
+    if (E.labelled) {
+      table.resize(table.size() + ((size_t)E.n + 1) / 2);
+      std::memcpy(table.data() + E.n + 1, E.labels, (size_t)E.n * 4);
+    }
+    if (e == cudaSuccess) e = upload(s->d_edges, table.data(), table.size(), st);
+    *h2d += ((uint64_t)E.n + 1) * 8 + (E.labelled ? (uint64_t)E.n * 4 : 0);
   }
   if (e == cudaSuccess && q->series_ids) e = stream_alloc(s->d_rank_slot, pages->series.size(), st);
   // work-list regions: each (bin, query column, narrow flag) bucket holds as many items as the page set has field pages
@@ -1794,30 +1830,41 @@ tskv_status tskvgpu_decode_pages(tskv_ctx *ctx, const tskv_pages *pages, uint64_
 // ------------------------------------------------------------------------------------------------
 tskv_status tskvgpu_query_output_layout(const tskv_pages *pages, const tskv_query *q,
                                         tskv_output_layout *out) {
-  return compute_layout(pages, q, TagGroups{}, false, nullptr, out);
+  return compute_layout(pages, q, TagGroups{}, BucketEdges{}, out);
 }
 
 tskv_status tskvgpu_query_output_layout_grouped(const tskv_pages *pages, const tskv_query *q, const uint32_t *group_ids,
                                                 uint32_t n_groups, tskv_output_layout *out) {
-  return compute_layout(pages, q, TagGroups{true, group_ids, n_groups}, false, nullptr, out);
+  return compute_layout(pages, q, TagGroups{true, group_ids, n_groups}, BucketEdges{}, out);
+}
+
+// The edges of the *_edges calls: q->n_buckets edge buckets, which are the output buckets.
+static BucketEdges plain_edges(const tskv_query *q, const int64_t *edges) {
+  return BucketEdges{true, edges, q ? q->n_buckets : 0u, false, nullptr};
 }
 
 tskv_status tskvgpu_query_output_layout_edges(const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
                                               const uint32_t *group_ids, uint32_t n_groups, tskv_output_layout *out) {
-  return compute_layout(pages, q, TagGroups{group_ids != nullptr, group_ids, n_groups}, true, edges, out);
+  return compute_layout(pages, q, TagGroups{group_ids != nullptr, group_ids, n_groups}, plain_edges(q, edges), out);
 }
 
-// tskvgpu_scan_prepare; slide > 0: tskvgpu_scan_prepare_sliding with slide < width; tg.on: GROUP BY tags; edges_on:
-// tskvgpu_scan_prepare_edges (slide 0).
+tskv_status tskvgpu_query_output_layout_labels(const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                               uint32_t n_edge, const uint32_t *labels, const uint32_t *group_ids,
+                                               uint32_t n_groups, tskv_output_layout *out) {
+  return compute_layout(pages, q, TagGroups{group_ids != nullptr, group_ids, n_groups},
+                        BucketEdges{true, edges, n_edge, true, labels}, out);
+}
+
+// tskvgpu_scan_prepare; slide > 0: tskvgpu_scan_prepare_sliding with slide < width; tg.on: GROUP BY tags; E.on:
+// tskvgpu_scan_prepare_edges / _labels (slide 0).
 static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
-                                const TagGroups &tg, tskv_scan **out_scan, bool edges_on = false,
-                                const int64_t *edges = nullptr) {
+                                const TagGroups &tg, tskv_scan **out_scan, const BucketEdges &E = BucketEdges{}) {
   if (!ctx || !pages || !q || !out_scan) return TSKV_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(ctx->mu);
   ctx->set_error("");
   *out_scan = nullptr;
   uint32_t win_k = 1;
-  tskv_status st = validate_query(ctx, pages, q, slide, tg, edges_on, edges, &win_k);
+  tskv_status st = validate_query(ctx, pages, q, slide, tg, E, &win_k);
   if (st != TSKV_OK) return st;
   const tskv_output_layout L = output_layout(pages, q, tg);
   cudaSetDevice(ctx->device);
@@ -1825,8 +1872,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   for (uint32_t c = 0; c < q->n_columns; c++) has_sel |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
   uint32_t slot_bits = 0;
   int64_t rel_base = 0;
-  if (!edges_on) edges = nullptr;
-  st = plan_keys(ctx, pages, q, edges, has_sel, &slot_bits, &rel_base);
+  st = plan_keys(ctx, pages, q, E, has_sel, &slot_bits, &rel_base);
   if (st != TSKV_OK) return st;
   tskv_scan *s = new tskv_scan();
   s->ctx = ctx;
@@ -1844,7 +1890,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   s->sl = lay.sl;
   s->kern_sl = lay.kern_sl;
   uint64_t h2d = 0;
-  if ((st = alloc_scan(ctx, pages, q, tg, slide != 0, edges, lay, s, &h2d)) != TSKV_OK) {
+  if ((st = alloc_scan(ctx, pages, q, tg, slide != 0, E, lay, s, &h2d)) != TSKV_OK) {
     delete s;
     return st;
   }
@@ -1880,7 +1926,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   }
   P.first_bucket_start = (int64_t)((uint64_t)q->first_bucket_start + (uint64_t)(win_k - 1) * (uint64_t)P.width);
   P.edges = s->d_edges.get();
-  P.n_buckets = s->n_panes;
+  P.n_buckets = E.on ? E.n : s->n_panes;  // (a labelled scan: its edge buckets; n_panes = its output buckets)
+  P.cell_buckets = E.labelled ? q->n_buckets : 0;
   P.group_by_series = q->group_by_series;
   P.n_cells = L.n_groups * s->n_panes;
   P.slot_group = s->d_slot_group.get();
@@ -1942,7 +1989,14 @@ tskv_status tskvgpu_scan_prepare_grouped(tskv_ctx *ctx, const tskv_pages *pages,
 
 tskv_status tskvgpu_scan_prepare_edges(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
                                        const uint32_t *group_ids, uint32_t n_groups, tskv_scan **out_scan) {
-  return prepare_scan(ctx, pages, q, 0, TagGroups{group_ids != nullptr, group_ids, n_groups}, out_scan, true, edges);
+  return prepare_scan(ctx, pages, q, 0, TagGroups{group_ids != nullptr, group_ids, n_groups}, out_scan, plain_edges(q, edges));
+}
+
+tskv_status tskvgpu_scan_prepare_labels(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                        uint32_t n_edge, const uint32_t *labels, const uint32_t *group_ids, uint32_t n_groups,
+                                        tskv_scan **out_scan) {
+  return prepare_scan(ctx, pages, q, 0, TagGroups{group_ids != nullptr, group_ids, n_groups}, out_scan,
+                      BucketEdges{true, edges, n_edge, true, labels});
 }
 
 // Enqueues one full pass on the context stream, no host synchronisation:
@@ -2361,11 +2415,11 @@ void tskvgpu_scan_destroy(tskv_ctx *ctx, tskv_scan *s) {
 }
 
 static tskv_status scan_aggregate(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, int64_t slide,
-                                  const TagGroups &tg, uint64_t *out_values, uint8_t *out_validity, bool edges_on = false,
-                                  const int64_t *edges = nullptr) {
+                                  const TagGroups &tg, uint64_t *out_values, uint8_t *out_validity,
+                                  const BucketEdges &E = BucketEdges{}) {
   if (!out_values || !out_validity) return TSKV_ERR_INVALID_ARG;
   tskv_scan *s = nullptr;
-  tskv_status st = slide ? prepare_sliding(ctx, pages, q, slide, tg, &s) : prepare_scan(ctx, pages, q, 0, tg, &s, edges_on, edges);
+  tskv_status st = slide ? prepare_sliding(ctx, pages, q, slide, tg, &s) : prepare_scan(ctx, pages, q, 0, tg, &s, E);
   if (st != TSKV_OK) return st;
   st = tskvgpu_scan_run(ctx, s);
   if (st == TSKV_OK) st = tskvgpu_scan_finalize(ctx, s, out_values, out_validity);
@@ -2397,8 +2451,15 @@ tskv_status tskvgpu_scan_aggregate_grouped(tskv_ctx *ctx, const tskv_pages *page
 
 tskv_status tskvgpu_scan_aggregate_edges(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
                                          const uint32_t *group_ids, uint32_t n_groups, uint64_t *out_values, uint8_t *out_validity) {
-  return scan_aggregate(ctx, pages, q, 0, TagGroups{group_ids != nullptr, group_ids, n_groups}, out_values, out_validity, true,
-                        edges);
+  return scan_aggregate(ctx, pages, q, 0, TagGroups{group_ids != nullptr, group_ids, n_groups}, out_values, out_validity,
+                        plain_edges(q, edges));
+}
+
+tskv_status tskvgpu_scan_aggregate_labels(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                          uint32_t n_edge, const uint32_t *labels, const uint32_t *group_ids, uint32_t n_groups,
+                                          uint64_t *out_values, uint8_t *out_validity) {
+  return scan_aggregate(ctx, pages, q, 0, TagGroups{group_ids != nullptr, group_ids, n_groups}, out_values, out_validity,
+                        BucketEdges{true, edges, n_edge, true, labels});
 }
 
 }  // extern "C"

@@ -113,6 +113,57 @@ def calendar_edges(unit, t_lo, t_hi, precision="ns"):
     return np.array(edges, dtype=np.int64)
 
 
+# date_part units calendar_parts supports: the date_trunc unit whose periods its edges follow, and the values of the
+# cyclic units (output bucket j holds the rows whose part is values[j]; year: the years present)
+PART_UNITS = {"year": ("year", None), "quarter": ("quarter", range(1, 5)), "month": ("month", range(1, 13)),
+              "week": ("week", range(1, 54)), "day": ("day", range(1, 32)), "doy": ("day", range(1, 367)),
+              "dow": ("day", range(0, 7)), "hour": ("hour", range(0, 24)), "minute": ("minute", range(0, 60))}
+
+
+def _iso_week(days):
+    """ISO 8601 week number of the Monday `days` days after 1970-01-01: the week of its Thursday, counted in the
+    Thursday's year (week 1 holds the year's first Thursday)."""
+    thu = days + 3
+    y, _, _ = _civil_from_days(thu)
+    return (thu - _days_from_civil(y, 1, 1)) // 7 + 1
+
+
+def calendar_parts(unit, t_lo, t_hi, precision="ns"):
+    """Labelled time buckets of GROUP BY date_part(unit, time) / EXTRACT(unit FROM time) over the rows of [t_lo, t_hi]:
+    (edges, labels, part_values) for Engine.scan_aggregate(..., edges=edges, labels=labels) with query.n_buckets =
+    len(part_values). edges are calendar_edges of the unit's periods (date_trunc('day') edges for day, doy and dow),
+    labels[b] is the output bucket of period b, and output bucket j holds the rows whose date_part(unit, time) equals
+    part_values[j] (float64, as date_part returns). Units: year (the years present), quarter 1-4, month 1-12, week (ISO
+    8601 week number 1-53: weeks start on Monday and belong to the year of their Thursday), day (of the month, 1-31), doy
+    (1-366), dow (0 = Sunday .. 6), hour 0-23 and minute 0-59. Proleptic Gregorian calendar in UTC, floor semantics
+    before 1970. second and finer units and epoch are refused: their parts are fractional, not a small set of groups."""
+    if unit not in PART_UNITS:
+        raise ValueError("calendar_parts: unit must be one of %s" % (tuple(PART_UNITS),))
+    period, values = PART_UNITS[unit]
+    edges = calendar_edges(period, t_lo, t_hi, precision)
+    starts = [int(e) for e in edges[:-1]]
+    per_day = 86400 * _PER_SECOND[precision]
+    if unit == "year":
+        values = [_civil_from_days(s // per_day)[0] for s in starts]
+        part = values
+    elif unit in ("hour", "minute"):
+        w = _FIXED_SECONDS[unit] * _PER_SECOND[precision]
+        part = [s // w % len(values) for s in starts]
+    elif unit == "week":
+        part = [_iso_week(s // per_day) for s in starts]
+    else:
+        part = []
+        for s in starts:
+            days = s // per_day
+            y, m, d = _civil_from_days(days)
+            part.append({"quarter": (m - 1) // 3 + 1, "month": m, "day": d, "doy": days - _days_from_civil(y, 1, 1) + 1,
+                         "dow": (days + 4) % 7}[unit])  # (1970-01-01 was a Thursday)
+    values = list(values)
+    index = {v: j for j, v in enumerate(values)}
+    labels = np.array([index[p] for p in part], dtype=np.uint32)
+    return edges, labels, np.array(values, dtype=np.float64)
+
+
 class TskvError(RuntimeError):
     """Mirrors TskvError::Decode / TsmPageFileHashCheckFailed: carries the status code."""
 
@@ -464,12 +515,29 @@ class Engine:
             raise ValueError("edges and slide: sliding windows over explicit time-bucket edges are not supported")
         return np.ascontiguousarray(edges, dtype=np.int64)
 
-    def output_layout(self, pages, query, group_ids=None, n_groups=None, edges=None):
+    @staticmethod
+    def _labels(labels, edges):
+        """Output bucket of every edge bucket as a contiguous uint32 array (kept alive by the caller), or None."""
+        if labels is None:
+            return None
+        if edges is None:
+            raise ValueError("labels need edges: label b names the output bucket of edge bucket b")
+        lab = np.ascontiguousarray(labels, dtype=np.uint32)
+        if lab.size != len(edges) - 1:
+            raise ValueError("labels: one label per edge bucket (len(edges) - 1 = %d), got %d" % (len(edges) - 1, lab.size))
+        return lab
+
+    def output_layout(self, pages, query, group_ids=None, n_groups=None, edges=None, labels=None):
         L = cabi.OutputLayout()
         q = query.to_c()
         g = self._group_map(group_ids, n_groups)
         e = self._edges(edges, None)
-        if e is not None:
+        lab = self._labels(labels, e)
+        if lab is not None:
+            st = self.lib.tskvgpu_query_output_layout_labels(pages.handle, C.byref(q), e.ctypes.data, lab.size,
+                                                             lab.ctypes.data, g[0] if g else None, g[1] if g else 0,
+                                                             C.byref(L))
+        elif e is not None:
             st = self.lib.tskvgpu_query_output_layout_edges(pages.handle, C.byref(q), e.ctypes.data,
                                                             g[0] if g else None, g[1] if g else 0, C.byref(L))
         elif g is None:
@@ -480,21 +548,28 @@ class Engine:
             raise TskvError(st, "invalid query")
         return L
 
-    def scan_aggregate(self, pages, query, slide=None, group_ids=None, n_groups=None, edges=None):
+    def scan_aggregate(self, pages, query, slide=None, group_ids=None, n_groups=None, edges=None, labels=None):
         """End-to-end call: query args H2D, fused scan, result D2H (BatchReader::process analogue).
         slide: sliding windows time_window(time, query.width, slide, query.origin); output bucket j is the window
         starting at query.first_bucket_start + j * slide (sliding_window_grid sizes that grid).
         group_ids: GROUP BY tags, group_ids[slot] = group of the slot-th selected series (n_groups groups, default
         max + 1; the result has one row of buckets per group).
         edges: explicit time buckets [edges[b], edges[b + 1]) (query.n_buckets + 1 increasing timestamps, query.width,
-        origin and first_bucket_start 0; calendar_edges makes them for date_trunc). Not with slide."""
+        origin and first_bucket_start 0; calendar_edges makes them for date_trunc). Not with slide.
+        labels: with edges, labels[b] < query.n_buckets is the output bucket of edge bucket b (one per edge bucket;
+        calendar_parts makes them for date_part). query.n_buckets is then the number of output buckets."""
         e = self._edges(edges, slide)
-        L = self.output_layout(pages, query, group_ids, n_groups, e)
+        lab = self._labels(labels, e)
+        L = self.output_layout(pages, query, group_ids, n_groups, e, lab)
         values = np.empty(int(L.n_out * L.n_cells), dtype=np.uint64)
         bitmaps = np.empty(int(L.validity_bytes), dtype=np.uint8)
         g = self._group_map(group_ids, n_groups)
         q = query.to_c()
-        if e is not None:
+        if lab is not None:
+            st = self.lib.tskvgpu_scan_aggregate_labels(self.ctx, pages.handle, C.byref(q), e.ctypes.data, lab.size,
+                                                        lab.ctypes.data, g[0] if g else None, g[1] if g else 0,
+                                                        values.ctypes.data, bitmaps.ctypes.data)
+        elif e is not None:
             st = self.lib.tskvgpu_scan_aggregate_edges(self.ctx, pages.handle, C.byref(q), e.ctypes.data,
                                                        g[0] if g else None, g[1] if g else 0,
                                                        values.ctypes.data, bitmaps.ctypes.data)
@@ -509,15 +584,19 @@ class Engine:
         self._check(st)
         return ScanResult(query, L, values, bitmaps)
 
-    def prepare(self, pages, query, slide=None, group_ids=None, n_groups=None, edges=None):
-        """Device-resident scan (run / enqueue / partials / exchange / finalize); slide, group_ids, edges: as in
+    def prepare(self, pages, query, slide=None, group_ids=None, n_groups=None, edges=None, labels=None):
+        """Device-resident scan (run / enqueue / partials / exchange / finalize); slide, group_ids, edges, labels: as in
         scan_aggregate."""
         e = self._edges(edges, slide)
-        L = self.output_layout(pages, query, group_ids, n_groups, e)
+        lab = self._labels(labels, e)
+        L = self.output_layout(pages, query, group_ids, n_groups, e, lab)
         g = self._group_map(group_ids, n_groups)
         q = query.to_c()
         h = C.c_void_p()
-        if e is not None:
+        if lab is not None:
+            st = self.lib.tskvgpu_scan_prepare_labels(self.ctx, pages.handle, C.byref(q), e.ctypes.data, lab.size,
+                                                      lab.ctypes.data, g[0] if g else None, g[1] if g else 0, C.byref(h))
+        elif e is not None:
             st = self.lib.tskvgpu_scan_prepare_edges(self.ctx, pages.handle, C.byref(q), e.ctypes.data,
                                                      g[0] if g else None, g[1] if g else 0, C.byref(h))
         elif g is not None:

@@ -452,6 +452,30 @@ tskv_status tskvgpu_scan_prepare_edges(tskv_ctx *ctx, const tskv_pages *pages, c
 tskv_status tskvgpu_scan_aggregate_edges(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
                                          const uint32_t *group_ids, uint32_t n_groups, uint64_t *out_values, uint8_t *out_validity);
 
+/* ---- labelled time buckets: GROUP BY date_part(unit, time) / EXTRACT(unit FROM time) ---------------------------------
+ * n_edge + 1 strictly increasing edges cut time into edge buckets [edges[b], edges[b + 1]), exactly as in
+ * tskvgpu_scan_prepare_edges, and labels[b] < q->n_buckets names the output bucket of edge bucket b: q->n_buckets is the
+ * number of output buckets per group. A selected row in edge bucket b aggregates into cell group * q->n_buckets + labels[b].
+ * Several edge buckets may share a label (the hour of the day over many days); an output bucket that no edge bucket maps
+ * to reads like an empty bucket. A selected row outside [edges[0], edges[n_edge]) is TSKV_ERR_BUCKET_RANGE. COUNT, SUM,
+ * MIN, MAX and MEAN are those of every other scan; labels[b] = b with q->n_buckets = n_edge gives the edge scan's result.
+ * group_ids / n_groups and group_by_series as in tskvgpu_scan_prepare_edges. The scan returned works with every
+ * tskvgpu_scan_* call, including TSKV_QUERY_MULTI_RANK exchange (every rank passes the same edges and labels).
+ * Refused before any launch:
+ *   TSKV_ERR_INVALID_ARG   labels == NULL, a label >= q->n_buckets, q->n_buckets == 0, and every refusal of the edges
+ *                          calls (with n_edge for their n_buckets; n_groups * q->n_buckets > TSKV_MAX_GROUPED_CELLS)
+ *   TSKV_ERR_UNSUPPORTED   FIRST / LAST (the reference takes each record batch's earliest row per label, so the NULL rule at
+ *                          that row acts across the page's edge buckets of one label: DESIGN.md section 7) */
+tskv_status tskvgpu_query_output_layout_labels(const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                               uint32_t n_edge, const uint32_t *labels, const uint32_t *group_ids,
+                                               uint32_t n_groups, tskv_output_layout *out);
+tskv_status tskvgpu_scan_prepare_labels(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                        uint32_t n_edge, const uint32_t *labels, const uint32_t *group_ids, uint32_t n_groups,
+                                        tskv_scan **out_scan);
+tskv_status tskvgpu_scan_aggregate_labels(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, const int64_t *edges,
+                                          uint32_t n_edge, const uint32_t *labels, const uint32_t *group_ids, uint32_t n_groups,
+                                          uint64_t *out_values, uint8_t *out_validity);
+
 /* Library version / build info ("tskv-b200 <semver> sm_90a"). */
 const char *tskvgpu_version(void);
 

@@ -339,6 +339,39 @@ extern "C" {
         out_values: *mut u64,
         out_validity: *mut u8,
     ) -> tskv_status;
+    pub fn tskvgpu_query_output_layout_labels(
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        edges: *const i64,
+        n_edge: u32,
+        labels: *const u32,
+        group_ids: *const u32,
+        n_groups: u32,
+        out: *mut tskv_output_layout,
+    ) -> tskv_status;
+    pub fn tskvgpu_scan_prepare_labels(
+        ctx: *mut tskv_ctx,
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        edges: *const i64,
+        n_edge: u32,
+        labels: *const u32,
+        group_ids: *const u32,
+        n_groups: u32,
+        out_scan: *mut *mut tskv_scan,
+    ) -> tskv_status;
+    pub fn tskvgpu_scan_aggregate_labels(
+        ctx: *mut tskv_ctx,
+        pages: *const tskv_pages,
+        q: *const tskv_query,
+        edges: *const i64,
+        n_edge: u32,
+        labels: *const u32,
+        group_ids: *const u32,
+        n_groups: u32,
+        out_values: *mut u64,
+        out_validity: *mut u8,
+    ) -> tskv_status;
     pub fn tskvgpu_scan_run(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
     pub fn tskvgpu_scan_enqueue(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
     pub fn tskvgpu_scan_sync(ctx: *mut tskv_ctx, scan: *mut tskv_scan) -> tskv_status;
