@@ -32,7 +32,9 @@ TSKV_ENC_GORILLA, TSKV_ENC_BITPACK, TSKV_ENC_DELTA_TS = 6, 10, 11
 
 TSKV_AGG_COUNT, TSKV_AGG_SUM, TSKV_AGG_MIN, TSKV_AGG_MAX = 1, 2, 4, 8
 TSKV_AGG_MEAN, TSKV_AGG_FIRST, TSKV_AGG_LAST, TSKV_AGG_ALL = 16, 32, 64, 0x7F
-AGG_NAMES = {1: "count", 2: "sum", 4: "min", 8: "max", 16: "mean", 32: "first", 64: "last"}
+# f64 sum of squared deviations from the cell mean (the variance state; engine.py derives var* / stddev* from it)
+TSKV_AGG_M2 = 0x80
+AGG_NAMES = {1: "count", 2: "sum", 4: "min", 8: "max", 16: "mean", 32: "first", 64: "last", 128: "m2"}
 TSKV_UPLOAD_VERIFY_CRC = 1
 TSKV_UPLOAD_HOST_RESIDENT = 2
 TSKV_UPLOAD_VERIFY_ON_READ = 4

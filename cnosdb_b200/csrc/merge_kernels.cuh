@@ -86,6 +86,9 @@ __device__ __forceinline__ bool merge_row_kept_in_stream(const ScanParams &P, co
   return merge_row_kept(P, M, i, k);
 }
 
+// M2: pass 2 of TSKV_AGG_M2 over the merged rows, with the pass-2 column table (k_scan_m2): the same merged rows and cells,
+// each M2 column's value adds d = (double)x - (its cell's shift) and d^2 to sum(d) / sum(d^2); other columns are skipped.
+template <bool M2>
 __global__ void __launch_bounds__(128) k_merge_chunks(const ScanParams P, const MergeParams M) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= M.n_rows) return;
@@ -133,7 +136,7 @@ __global__ void __launch_bounds__(128) k_merge_chunks(const ScanParams P, const 
   // a group are one record batch, so its rows of one bucket are one run: a surviving, in-range row of any stream with an
   // earlier / later timestamp inside the bucket takes that place)
   bool is_first = false, is_last = false;
-  if (M.sel) {
+  if (!M2 && M.sel) {
     is_first = is_last = true;
     auto counts = [&](uint64_t j, uint32_t s2) {  // does merge row j reach the aggregate?
       if (!merge_row_kept_in_stream(P, M, j, s2)) return false;
@@ -155,6 +158,7 @@ __global__ void __launch_bounds__(128) k_merge_chunks(const ScanParams P, const 
   // ---- per query column: the last surviving non-null value with this timestamp (take_last_and_merge)
   for (uint32_t c = 0; c < P.n_cols; c++) {
     const ColState cs = P.cols[c];
+    if (M2 && !(cs.agg_mask & TSKV_AGG_M2)) continue;
     bool have = false;
     uint64_t v = 0;
     bool masked = false;  // (series, column) tombstone: the column reads as NULL at this timestamp in every chunk
@@ -180,7 +184,13 @@ __global__ void __launch_bounds__(128) k_merge_chunks(const ScanParams P, const 
         }
       }
     }
-    if (have) {
+    if (M2 && have) {
+      const uint8_t pt = cs.phys_type;
+      const double x = pt == TSKV_PT_F64 ? __longlong_as_double((long long)v) : pt == TSKV_PT_I64 ? (double)(int64_t)v : (double)v;
+      const double d = x - __longlong_as_double((long long)P.state[cs.count_off + cell]);
+      atomicAdd(reinterpret_cast<double *>(P.state + cs.sum_off + cell), d);
+      atomicAdd(reinterpret_cast<double *>(P.state + cs.sumhi_off + cell), d * d);
+    } else if (have) {
       const uint8_t pt = cs.phys_type, mask = cs.agg_mask;
       const int64_t key = okey(v, pt);
       atomicAdd(reinterpret_cast<unsigned long long *>(P.state + cs.count_off + cell), 1ull);

@@ -999,6 +999,31 @@ struct ValueAcc {  // count / sum / min / max of one run; VK fixes the arithmeti
   }
 };
 
+// Pass 2 of TSKV_AGG_M2 (k_scan_m2): a run's ValueAcc holds sum(d) in `sum` and sum(d^2) in `sum_hi` (f64 bits) with
+// d = (double)x - shift, shift = the run's cell mean from pass 1 (k_m2_prep), held as f64 bits in `kmin` (unused by the
+// pass). Integers convert to f64 as DataFusion's variance does.
+template <int VK>
+__device__ __forceinline__ void m2_add(ValueAcc<VK> &va, uint64_t v, uint8_t pt) {
+  const double shift = __longlong_as_double((long long)va.kmin);
+  double x;
+  if (VK == VK_GOR || pt == TSKV_PT_F64) x = __longlong_as_double((long long)v);
+  else if (pt == TSKV_PT_I64) x = (double)(int64_t)v;
+  else x = (double)v;
+  const double d = x - shift;
+  va.sum = (uint64_t)__double_as_longlong(__longlong_as_double((long long)va.sum) + d);
+  va.sum_hi = __double_as_longlong(__longlong_as_double((long long)va.sum_hi) + d * d);
+}
+
+// sum(d) / sum(d^2) of one run (pass 2) into the partial table: the CTA's shared-memory table (s_sum / s_hi) or the
+// global state (sum_off / sumhi_off of the pass-2 column table, see M2Col).
+__device__ __forceinline__ void table_update_m2(const ScanParams &P, uint64_t *stab, const ColState &cs, uint64_t cell,
+                                                uint64_t sd, uint64_t sd2) {
+  const bool sm = P.use_smem != 0;
+  uint64_t *tab = sm ? stab : P.state;
+  atomicAdd(reinterpret_cast<double *>(tab + (sm ? cs.s_sum : cs.sum_off) + cell), __longlong_as_double((long long)sd));
+  atomicAdd(reinterpret_cast<double *>(tab + (sm ? cs.s_hi : cs.sumhi_off) + cell), __longlong_as_double((long long)sd2));
+}
+
 // ------------------------------------------------------------------------------------------------
 // Staged flush (GROUP BY bucket, no FIRST/LAST). The 32 pages of a warp usually cross a bucket boundary at the same
 // row (TSBS-aligned timestamps), so all lanes finish a run for the SAME cell at the same time. Combining 32 partials
@@ -1023,7 +1048,8 @@ __host__ __device__ constexpr int flush_slots(int tk) { return tk == TK_S8B ? 2 
 constexpr int FLUSH_Q = 5;  // count | sum | sum_hi | min key | max key
 __host__ __device__ constexpr uint32_t flush_stage_bytes(int ns) { return (ns * FLUSH_Q * 32 + ns) * 8; }  // + one meta word per slot
 
-template <int VK, int NS>
+// M2 (pass 2 of TSKV_AGG_M2): the staged quantities are count | sum(d) | sum(d^2), both sums f64.
+template <int VK, int NS, bool M2 = false>
 __device__ __forceinline__ void reduce_staged(const ScanParams &P, uint64_t *stab, uint64_t *stage, uint32_t n_slots) {
   __syncwarp();
   const uint32_t lane = threadIdx.x & 31;
@@ -1031,6 +1057,28 @@ __device__ __forceinline__ void reduce_staged(const ScanParams &P, uint64_t *sta
   const uint64_t meta = stage[NS * FLUSH_Q * 32 + s];  // (query column << 32) | cell
   const uint32_t qcol = (uint32_t)(meta >> 32);
   const ColState &cs = P.cols[s < n_slots ? qcol : 0];
+  if constexpr (M2) {
+    uint64_t cnt = 0;
+    double sd = 0.0, sd2 = 0.0;
+    const uint64_t *base = stage + (size_t)s * FLUSH_Q * 32;
+#pragma unroll
+    for (int i = 0; i < NS; i++) {
+      const uint32_t src = g * NS + ((i + s) & (NS - 1));
+      cnt += base[src];
+      sd += __longlong_as_double((long long)base[32 + src]);
+      sd2 += __longlong_as_double((long long)base[64 + src]);
+    }
+#pragma unroll
+    for (int o = NS; o < 32; o <<= 1) {
+      cnt += shfl_xor_u64(cnt, o);
+      sd += __longlong_as_double((long long)shfl_xor_u64((uint64_t)__double_as_longlong(sd), o));
+      sd2 += __longlong_as_double((long long)shfl_xor_u64((uint64_t)__double_as_longlong(sd2), o));
+    }
+    if (lane < n_slots && cnt)
+      table_update_m2(P, stab, cs, (uint64_t)(uint32_t)meta, (uint64_t)__double_as_longlong(sd), (uint64_t)__double_as_longlong(sd2));
+    __syncwarp();
+    return;
+  }
   const bool is_f64 = VK == VK_GOR || (VK == VK_GEN && cs.phys_type == TSKV_PT_F64);
   uint64_t cnt = 0, sum = 0;
   int64_t hi = 0, kmin = INT64_MAX, kmax = INT64_MIN;
@@ -1074,24 +1122,27 @@ __device__ __forceinline__ void reduce_staged(const ScanParams &P, uint64_t *sta
 
 // Every lane parks its partial (identities unless `live`) in staging slot `seq`, the lane `meta_lane` records the slot's
 // (query column << 32) | cell, and every NS slots the warp reduces them. Called by all 32 lanes.
-template <int VK, int NS>
+template <int VK, int NS, bool M2 = false>
 __device__ __forceinline__ void stage_partial(const ScanParams &P, uint64_t *stab, uint64_t *stage, uint32_t &seq, bool live,
                                               const ValueAcc<VK> &va, bool meta_lane, uint64_t gcell) {
   uint64_t *q = stage + (size_t)seq * FLUSH_Q * 32 + (threadIdx.x & 31);
   q[0] = live ? va.count : 0;
   q[32] = live ? va.sum : 0;  // 0 bits == +0.0
-  if (VK != VK_GOR) q[64] = live ? (uint64_t)va.sum_hi : 0;
-  q[96] = live ? (uint64_t)va.kmin : (uint64_t)INT64_MAX;
-  q[128] = live ? (uint64_t)va.kmax : (uint64_t)INT64_MIN;
+  if (VK != VK_GOR || M2) q[64] = live ? (uint64_t)va.sum_hi : 0;
+  if constexpr (!M2) {
+    q[96] = live ? (uint64_t)va.kmin : (uint64_t)INT64_MAX;
+    q[128] = live ? (uint64_t)va.kmax : (uint64_t)INT64_MIN;
+  }
   if (meta_lane) stage[NS * FLUSH_Q * 32 + seq] = gcell;
   if (++seq == NS) {
-    reduce_staged<VK, NS>(P, stab, stage, seq);
+    reduce_staged<VK, NS, M2>(P, stab, stage, seq);
     seq = 0;
   }
 }
 
-// Flush of one finished run per flushing lane (no FIRST/LAST). `seq` = staged slots in use (warp-uniform).
-template <int VK, int NS>
+// Flush of one finished run per flushing lane (no FIRST/LAST). `seq` = staged slots in use (warp-uniform). M2: pass 2 of
+// TSKV_AGG_M2 (sum(d) / sum(d^2) partials, m2_add).
+template <int VK, int NS, bool M2 = false>
 __device__ __forceinline__ void flush_runs(const ScanParams &P, uint64_t *stab, uint64_t *stage, uint32_t &seq, bool active,
                                            uint32_t qcol, uint64_t cell, uint8_t pt, uint8_t mask, const ValueAcc<VK> &va) {
   const uint32_t m = __ballot_sync(FULL, active);
@@ -1106,10 +1157,11 @@ __device__ __forceinline__ void flush_runs(const ScanParams &P, uint64_t *stab, 
   // atomic per quantity instead of 32 contended ones.
   const bool same = !P.group_by_series && __all_sync(FULL, !active || gcell == lcell);
   if (same) {
-    stage_partial<VK, NS>(P, stab, stage, seq, active && va.count, va, (int)lane == leader, lcell);
+    stage_partial<VK, NS, M2>(P, stab, stage, seq, active && va.count, va, (int)lane == leader, lcell);
   } else if (active && va.count) {  // lanes on different cells (GROUP BY series, unaligned pages): one update each
-    table_update(P, stab, P.cols[qcol], cell, mask, VK == VK_GOR || (VK == VK_GEN && pt == TSKV_PT_F64), va.count, va.sum,
-                 va.sum_hi, va.kmin, va.kmax);
+    if constexpr (M2) table_update_m2(P, stab, P.cols[qcol], cell, va.sum, (uint64_t)va.sum_hi);
+    else table_update(P, stab, P.cols[qcol], cell, mask, VK == VK_GOR || (VK == VK_GEN && pt == TSKV_PT_F64), va.count, va.sum,
+                      va.sum_hi, va.kmin, va.kmax);
   }
 }
 
@@ -1157,7 +1209,10 @@ struct GenTimeCursor : DeltaCursor<-1, BeStream> {
 // timestamp of the row before it (leading NULLs: of the first valid row), so it never cuts a segment of its own.
 // NARROW (simple8b integer values, no FIRST / LAST): every page of the chunk is narrow (ScanParams.page_narrow), so the
 // values are decoded and accumulated in 32-bit arithmetic (S8bCursor::next32, ValueAcc::add32).
-template <int TK, int VK, bool SEL, bool NARROW, bool EDGES>
+// M2 (k_scan_m2, pass 2 of TSKV_AGG_M2; never with SEL or NARROW): the same rows, segments and runs, but a run sums
+// d = x - (its cell's pass-1 mean) and d^2 (m2_add) instead of count / sum / min / max, and counts no points or rows.
+// The uniform schedule is left to the segment loop, which gives the same rows.
+template <int TK, int VK, bool SEL, bool NARROW, bool EDGES, bool M2 = false>
 __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t item_begin, uint32_t item_end,
                                                uint32_t ring_base, uint64_t *stab, uint64_t *stage, uint4 *s_tomb,
                                                uint32_t part, uint32_t n_parts, uint32_t part_rows) {
@@ -1280,6 +1335,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   ring_drain();  // the rings' initial fills have landed before the first step (once per page)
 
   static_assert(!NARROW || (VK == VK_S8B && !SEL), "narrow chunks: simple8b integer values, no FIRST / LAST");
+  static_assert(!M2 || (!SEL && !NARROW), "M2 pass: no FIRST / LAST, wide arithmetic");
   ValueAcc<VK> va;
   va.reset(NARROW);
   RunAcc acc;  // flush image (+ first/last state when SEL)
@@ -1301,6 +1357,10 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
 
   // Finished runs of the flushing lanes -> partial tables.
   auto flush_now = [&](bool flush) {
+    if constexpr (M2) {
+      flush_runs<VK, NS, true>(P, stab, stage, staged, flush, qcol, group_base + bucket_cell<EDGES>(P, run_idx, flush), pt, mask, va);
+      return;
+    }
     if (flush) va.fold(pt, NARROW);
     if (SEL) {
       if (__any_sync(FULL, flush)) {
@@ -1332,7 +1392,11 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
         if (accumulate && kept) { va.count++; va.add32(v32); }
       } else {
         v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
-        if (accumulate && kept) { va.count++; va.add(v, pt, flip); }
+        if constexpr (M2) {
+          if (accumulate && kept) { va.count++; m2_add(va, v, pt); }
+        } else {
+          if (accumulate && kept) { va.count++; va.add(v, pt, flip); }
+        }
       }
     }
     return v;  // (0 for narrow chunks: only FIRST / LAST use it)
@@ -1342,6 +1406,9 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
     if constexpr (NARROW) {
       const uint32_t v32 = vcur_d.next32();
       if (take) va.add32(v32);
+    } else if constexpr (M2) {
+      const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
+      if (take) m2_add(va, v, pt);
     } else {
       const uint64_t v = VK == VK_GOR ? vcur_g.next() : vcur_d.next();
       if (take) va.add(v, pt, flip);
@@ -1413,7 +1480,7 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
   // same cell. The staged partials and their order are the ones the segment loop below makes for such a warp. Lanes
   // without rows walk along idle; a lane whose values run out stops decoding as there. (Not for the generic value
   // codecs: their larger cursor leaves no registers for a second loop.)
-  if (TK == TK_RLE && VK != VK_GEN && !SEL && fast && (P.width > 0 || EDGES) && !P.group_by_series) {
+  if (TK == TK_RLE && VK != VK_GEN && !SEL && fast && (P.width > 0 || EDGES) && !P.group_by_series && !M2) {
     const bool mine = row < n_rows;
     const uint32_t with_rows = __ballot_sync(FULL, mine);
     const int src = with_rows ? __ffs(with_rows) - 1 : 0;
@@ -1607,6 +1674,8 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
       run_idx = seg_b;
       va.reset(NARROW);
       if (SEL) { acc.first_ok = acc.last_ok = false; first_pending = true; }
+      if constexpr (M2)  // a run never changes cell: its shift is loaded once (pass-2 columns keep it at count_off)
+        va.kmin = (int64_t)P.state[P.cols[qcol].count_off + group_base + bucket_cell<EDGES>(P, run_idx)];
     }
     // ---- 3. the segment's rows --------------------------------------------------------------------------
     if (go) {
@@ -1702,13 +1771,14 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
     }
   }
   if (!SEL && staged) {  // partials still parked in the staging area
-    reduce_staged<VK, NS>(P, stab, stage, staged);
+    reduce_staged<VK, NS, M2>(P, stab, stage, staged);
     staged = 0;
   }
   // (only the lane that decodes the page's last rows walks on to the sentinel)
   if (VK == VK_GOR && have_item && n_rows != 0 && to_page_end && vcur_g.consumed_any() && !vcur_g.drain())  // float.rs:480-591
     report_error(P, TSKV_ERR_SHORT_BLOCK, page);
   ring_drain();  // nothing in flight when the next chunk reuses the rings
+  if constexpr (M2) return;  // (pass 1 counted these rows)
   n_points = __reduce_add_sync(FULL, n_points);
   n_inrange = __reduce_add_sync(FULL, n_inrange);
   if (lane == 0) {
@@ -1820,6 +1890,59 @@ __global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, SEL)) k_scan
         }
         if (cs.agg_mask & TSKV_AGG_MIN) atomicMin(reinterpret_cast<long long *>(P.state + cs.min_off + i), (long long)s_tab[cs.s_min + i]);
         if (cs.agg_mask & TSKV_AGG_MAX) atomicMax(reinterpret_cast<long long *>(P.state + cs.max_off + i), (long long)s_tab[cs.s_max + i]);
+      }
+    }
+  }
+}
+
+// Pass 2 of TSKV_AGG_M2: the fused kernel of bin `bin` once more, over the work-list regions of the M2 columns only
+// (P.region_fill: pass 1's fills with every other column's set to 0, k_m2_prep), with the pass-2 column table (M2Col):
+// count_off = the cells' shifts, sum_off / sumhi_off = sum(d) / sum(d^2), s_sum / s_hi in the shared-memory table. Narrow
+// pages take the wide arithmetic. Own instantiations, so that the pass-1 kernels hold none of this code.
+template <int TK, int VK, bool EDGES>
+__global__ void __launch_bounds__(SCAN_THREADS, scan_min_blocks(TK, false)) k_scan_m2(const __grid_constant__ ScanParams P, int bin) {
+  extern __shared__ __align__(16) uint64_t s_tab[];
+  if (P.use_smem) {  // identities: +0.0
+    for (uint32_t i = threadIdx.x; i < P.smem_words; i += SCAN_THREADS) s_tab[i] = 0;
+    __syncthreads();
+  }
+  const uint32_t lane = threadIdx.x & 31;
+  uint64_t *warp_area = s_tab + ((P.smem_words + 1) & ~1u) + (size_t)(threadIdx.x >> 5) * (scan_warp_bytes(TK) / 8);
+  const uint32_t ring_base = (uint32_t)__cvta_generic_to_shared(warp_area);
+  uint64_t *stage = warp_area + scan_ring_bytes_per_warp(TK) / 8;
+  uint4 *s_tomb = reinterpret_cast<uint4 *>(s_tab + ((P.smem_words + 1) & ~1u) + (SCAN_THREADS / 32) * (scan_warp_bytes(TK) / 8));
+  uint32_t n_groups = 0;
+  for (uint32_t k = bin * P.n_cols * WL_SUB; k < (bin + 1) * P.n_cols * WL_SUB; k++) n_groups += (__ldg(P.region_fill + k) + 31) >> 5;
+  const uint32_t n_parts = (TK == TK_GEN || VK == VK_GEN) ? 1u : P.bin_parts[bin];
+  const uint32_t part_rows = P.bin_part_rows[bin];
+  const uint32_t n_chunks = n_groups * n_parts;
+  for (;;) {
+    uint32_t c = 0;
+    if (lane == 0) c = atomicAdd(P.task_counter + bin, 1u);
+    c = __shfl_sync(FULL, c, 0);
+    if (c >= n_chunks) break;
+    uint32_t group = n_parts > 1 ? c / n_parts : c;
+    const uint32_t part = c - group * n_parts;
+    uint32_t k = bin * P.n_cols * WL_SUB;
+    uint32_t fill = __ldg(P.region_fill + k);
+    while (group >= (fill + 31) >> 5) {
+      group -= (fill + 31) >> 5;
+      fill = __ldg(P.region_fill + ++k);
+    }
+    const uint32_t region = __ldg(P.region_start + k);
+    const uint32_t begin = region + (group << 5);
+    const uint32_t end = min(begin + 32, region + fill);
+    scan_chunk_seg<TK, VK, false, false, EDGES, true>(P, begin, end, ring_base, s_tab, stage, s_tomb, part, n_parts, part_rows);
+  }
+  if (P.use_smem) {  // merge this CTA's table into the global state, once
+    __syncthreads();
+    for (uint32_t c = 0; c < P.n_cols; c++) {
+      const ColState cs = P.cols[c];
+      if (!(cs.agg_mask & TSKV_AGG_M2)) continue;
+      for (uint32_t i = threadIdx.x; i < (uint32_t)P.n_cells; i += SCAN_THREADS) {
+        const uint64_t sd = s_tab[cs.s_sum + i], sd2 = s_tab[cs.s_hi + i];
+        if (sd) atomicAdd(reinterpret_cast<double *>(P.state + cs.sum_off + i), __longlong_as_double((long long)sd));
+        if (sd2) atomicAdd(reinterpret_cast<double *>(P.state + cs.sumhi_off + i), __longlong_as_double((long long)sd2));
       }
     }
   }
@@ -2033,6 +2156,68 @@ __global__ void k_merge_gathered(uint64_t *state, StateLayout L, const uint64_t 
   }
 }
 
+// TSKV_AGG_M2 of one query column: state offsets (8-byte words) of its pass-1 count and f64 sum (the f64 sum of an F64
+// column, the exported exact integer sum otherwise), and of its pass-2 arrays: the cells' shifts, sum(d) and sum(d^2).
+struct M2Col {
+  uint64_t count_off, sum_off, shift_off, sd_off, sd2_off;
+};
+
+// Between the passes: shift[cell] = pass-1 sum / count (0 for an empty cell) of every M2 column (blockIdx.y); block
+// (0, 0) also writes pass 2's bucket fills (pass 1's, with the buckets of columns without M2 set to 0: pass 2 launches
+// over the M2 columns' regions only) and zeroes pass 2's task counters.
+__global__ void k_m2_prep(uint64_t *state, const M2Col *m2, uint64_t n_cells, const uint32_t *fill, uint32_t *fill2,
+                          uint32_t n_buckets, const ColState *cols2, uint32_t n_cols, uint32_t *task_counter) {
+  const M2Col mc = m2[blockIdx.y];
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_cells; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t n = state[mc.count_off + i];
+    const double s = __longlong_as_double((long long)state[mc.sum_off + i]);
+    state[mc.shift_off + i] = (uint64_t)__double_as_longlong(n ? s / (double)n : 0.0);
+  }
+  if (blockIdx.x == 0 && blockIdx.y == 0) {
+    for (uint32_t k = threadIdx.x; k < n_buckets; k += blockDim.x)
+      fill2[k] = (cols2[(k / WL_SUB) % n_cols].agg_mask & TSKV_AGG_M2) ? fill[k] : 0u;
+    for (uint32_t b = threadIdx.x; b < N_BINS; b += blockDim.x) task_counter[b] = 0;
+  }
+}
+
+// Multi-GPU, after k_merge_gathered: M2 of every M2 column (blockIdx.y) and cell from the gathered ranks' (count n_r,
+// shift c_r, sum(d), sum(d^2)), each rank's d taken around its own shift: M2_r = sum(d^2) - sum(d)^2 / n_r, and the
+// rank's mean relative to the shift c of the first rank holding the cell, mu_r = (c_r - c) + sum(d) / n_r (close means:
+// the difference of the shifts is exact). Chan's merge M2 = sum M2_r + sum n_r (mu_r - mu)^2, mu = sum n_r mu_r / n.
+// (Relative means keep the digits that means near 2^63 as f64 would lose.) Writes sum(d) = 0 and sum(d^2) = M2, which
+// k_finalize turns into M2 again.
+__global__ void k_merge_m2(uint64_t *state, const M2Col *m2, uint64_t n_cells, const uint64_t *gathered, uint32_t n_ranks,
+                           uint64_t exch_words) {
+  const M2Col mc = m2[blockIdx.y];
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_cells; i += (uint64_t)gridDim.x * blockDim.x) {
+    auto at = [&](uint32_t r, uint64_t off) { return gathered[r * exch_words + off + i]; };
+    auto f64 = [&](uint32_t r, uint64_t off) { return __longlong_as_double((long long)at(r, off)); };
+    uint64_t n = 0;
+    double c = 0.0, mu_sum = 0.0;
+    bool have_c = false;
+    for (uint32_t r = 0; r < n_ranks; r++) {
+      const uint64_t nr = at(r, mc.count_off);
+      if (!nr) continue;
+      if (!have_c) { c = f64(r, mc.shift_off); have_c = true; }
+      n += nr;
+      mu_sum += (f64(r, mc.shift_off) - c) * (double)nr + f64(r, mc.sd_off);
+    }
+    double acc = 0.0;
+    if (n) {
+      const double mu = mu_sum / (double)n;
+      for (uint32_t r = 0; r < n_ranks; r++) {
+        const uint64_t nr = at(r, mc.count_off);
+        if (!nr) continue;
+        const double sd = f64(r, mc.sd_off), sd2 = f64(r, mc.sd2_off);
+        const double dm = (f64(r, mc.shift_off) - c) + sd / (double)nr - mu;
+        acc += (sd2 - sd * sd / (double)nr) + (double)nr * dm * dm;
+      }
+    }
+    state[mc.sd_off + i] = 0;
+    state[mc.sd2_off + i] = (uint64_t)__double_as_longlong(acc);
+  }
+}
+
 // Per output column: which state arrays feed it.
 struct OutCol {
   uint64_t count_off;  // counts of the source column
@@ -2066,6 +2251,14 @@ __global__ void k_finalize(const uint64_t *state, const OutCol *outs, uint32_t n
         break;
       case TSKV_AGG_FIRST: valid = state[oc.src_off + cell] != 0x7fffffffffffffffull; if (valid) v = state[oc.val_off + cell]; break;
       case TSKV_AGG_LAST: valid = state[oc.src_off + cell] != 0x8000000000000000ull; if (valid) v = state[oc.val_off + cell]; break;
+      case TSKV_AGG_M2:
+        valid = cnt > 0;
+        if (valid) {  // src = sum(d^2), val = sum(d): the corrected two-pass M2 (NaN stays NaN; rounding never goes below 0)
+          const double sd = __longlong_as_double((long long)state[oc.val_off + cell]);
+          const double m2 = __longlong_as_double((long long)state[oc.src_off + cell]) - sd * sd / (double)cnt;
+          v = (uint64_t)__double_as_longlong(m2 < 0.0 ? 0.0 : m2);
+        }
+        break;
       default: break;
     }
     values[(uint64_t)blockIdx.y * n_cells + cell] = v;

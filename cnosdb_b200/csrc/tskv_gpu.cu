@@ -243,6 +243,16 @@ struct tskv_scan {
   // explicit time-bucket edges (params.edges; tskvgpu_scan_prepare_edges / _labels), null otherwise; a labelled scan's
   // labels (uint32) follow its n + 1 edges
   async_ptr<int64_t> d_edges;
+  // TSKV_AGG_M2 (k_m2_prep, k_scan_m2): its columns, pass 2's parameters and column table, pass 2's bucket fills followed
+  // by its task counters, the bins pass 2 runs, the shift / sum(d) / sum(d^2) words at the end of the exchange region
+  uint32_t n_m2 = 0;
+  async_ptr<M2Col> d_m2;
+  async_ptr<ColState> d_cols2;
+  async_ptr<uint32_t> d_fill2;
+  ScanParams params2{};
+  bool m2_bin[N_BINS] = {false};
+  uint64_t m2_words = 0;
+  event_ptr ev_m2_fork, ev_m2_join[N_BINS];
 };
 
 namespace {
@@ -317,7 +327,17 @@ unsigned bits_for(uint64_t max_value) {  // bits needed to represent values in [
   return b;
 }
 
-unsigned popc8(unsigned x) { return (unsigned)__builtin_popcount(x & TSKV_AGG_ALL); }
+unsigned popc8(unsigned x) { return (unsigned)__builtin_popcount(x & 0xffu); }
+
+// The aggregates the pass-1 kernels compute for a column: its own, and for TSKV_AGG_M2 also the COUNT and the exact SUM
+// that MEAN keeps (pass 2 shifts by that mean). The M2 bit itself never reaches them.
+uint8_t kernel_mask(uint8_t m) { return (uint8_t)((m & TSKV_AGG_ALL) | ((m & TSKV_AGG_M2) ? TSKV_AGG_MEAN : 0)); }
+
+bool query_has_m2(const tskv_query *q) {
+  for (uint32_t c = 0; c < q->n_columns; c++)
+    if (q->columns[c].agg_mask & TSKV_AGG_M2) return true;
+  return false;
+}
 
 typedef void (*scan_kernel_t)(const ScanParams, int);
 // `narrow`: NARROW_* of the bin's pages (tskv_pages::h_bin_narrow); only the simple8b-value kernels without FIRST / LAST
@@ -346,6 +366,22 @@ template <bool SEL>
 scan_kernel_t scan_kernel_for(int bin, bool edges, int narrow = NARROW_NONE) {
   return edges ? scan_kernel_for<SEL, true>(bin, narrow) : scan_kernel_for<SEL, false>(bin, narrow);
 }
+// pass 2 of TSKV_AGG_M2 (k_scan_m2): one kernel per serial bin (narrow pages take the wide arithmetic)
+template <bool EDGES>
+scan_kernel_t m2_kernel_for(int bin) {
+  switch (bin) {
+    case TK_RLE * N_VK + VK_S8B: return k_scan_m2<TK_RLE, VK_S8B, EDGES>;
+    case TK_RLE * N_VK + VK_GOR: return k_scan_m2<TK_RLE, VK_GOR, EDGES>;
+    case TK_RLE * N_VK + VK_GEN: return k_scan_m2<TK_RLE, VK_GEN, EDGES>;
+    case TK_S8B * N_VK + VK_S8B: return k_scan_m2<TK_S8B, VK_S8B, EDGES>;
+    case TK_S8B * N_VK + VK_GOR: return k_scan_m2<TK_S8B, VK_GOR, EDGES>;
+    case TK_S8B * N_VK + VK_GEN: return k_scan_m2<TK_S8B, VK_GEN, EDGES>;
+    case TK_GEN * N_VK + VK_S8B: return k_scan_m2<TK_GEN, VK_S8B, EDGES>;
+    case TK_GEN * N_VK + VK_GOR: return k_scan_m2<TK_GEN, VK_GOR, EDGES>;
+    default: return k_scan_m2<TK_GEN, VK_GEN, EDGES>;
+  }
+}
+scan_kernel_t m2_kernel_for(int bin, bool edges) { return edges ? m2_kernel_for<true>(bin) : m2_kernel_for<false>(bin); }
 // the bin among 0-8 whose lane-per-page kernel also runs a short-page bin
 int serial_bin_of(int bin) {
   if (bin == BIN_SHORT_RLE_S8B) return TK_RLE * N_VK + VK_S8B;
@@ -502,6 +538,9 @@ struct StatePlan {
   std::vector<ColState> cols;
   std::vector<MeanExport> means;
   std::vector<uint64_t> msum_off;  // per column: the exported f64 exact integer sum of MEAN, or 0
+  std::vector<M2Col> m2;           // TSKV_AGG_M2 columns, in query order
+  std::vector<int> m2_of;          // per column: its index in m2, or -1
+  uint64_t m2_words = 0;           // their shift / sum(d) / sum(d^2) sections, which follow the values section
 };
 StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
   StatePlan plan;
@@ -518,10 +557,10 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
     cols[c] = ColState{};
     cols[c].column_id = qc.column_id;
     cols[c].phys_type = qc.phys_type;
-    cols[c].agg_mask = qc.agg_mask;
+    cols[c].agg_mask = kernel_mask(qc.agg_mask);
     cols[c].count_off = off;
     off += n_cells;
-    if ((qc.agg_mask & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) && qc.phys_type != TSKV_PT_F64) {
+    if ((kernel_mask(qc.agg_mask) & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) && qc.phys_type != TSKV_PT_F64) {
       cols[c].sum_off = off;
       off += n_cells;
     }
@@ -529,26 +568,26 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
   sl.sum_i64_len = off - sl.sum_i64_off;
   sl.sum_f64_off = off;
   for (uint32_t c = 0; c < q->n_columns; c++)
-    if ((q->columns[c].agg_mask & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) && q->columns[c].phys_type == TSKV_PT_F64) {
+    if ((kernel_mask(q->columns[c].agg_mask) & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) && q->columns[c].phys_type == TSKV_PT_F64) {
       cols[c].sum_off = off;
       off += n_cells;
     }
   for (uint32_t c = 0; c < q->n_columns; c++)
-    if ((q->columns[c].agg_mask & TSKV_AGG_MEAN) && q->columns[c].phys_type != TSKV_PT_F64) {
+    if ((kernel_mask(q->columns[c].agg_mask) & TSKV_AGG_MEAN) && q->columns[c].phys_type != TSKV_PT_F64) {
       msum_off[c] = off;  // exported exact integer sum as f64 (all-reducible)
       off += n_cells;
     }
   sl.sum_f64_len = off - sl.sum_f64_off;
   uint64_t n_first = 0, n_last = 0;
   for (uint32_t c = 0; c < q->n_columns; c++) {
-    if (q->columns[c].agg_mask & TSKV_AGG_FIRST) n_first += n_cells;
-    if (q->columns[c].agg_mask & TSKV_AGG_LAST) n_last += n_cells;
+    if (kernel_mask(q->columns[c].agg_mask) & TSKV_AGG_FIRST) n_first += n_cells;
+    if (kernel_mask(q->columns[c].agg_mask) & TSKV_AGG_LAST) n_last += n_cells;
   }
   sl.first_cells = n_first;
   sl.last_cells = n_last;
   sl.min_off = off;
   for (uint32_t c = 0; c < q->n_columns; c++)
-    if (q->columns[c].agg_mask & TSKV_AGG_MIN) {
+    if (kernel_mask(q->columns[c].agg_mask) & TSKV_AGG_MIN) {
       cols[c].min_off = off;
       off += n_cells;
     }
@@ -557,7 +596,7 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
   sl.min_len = off - sl.min_off;
   sl.max_off = off;
   for (uint32_t c = 0; c < q->n_columns; c++)
-    if (q->columns[c].agg_mask & TSKV_AGG_MAX) {
+    if (kernel_mask(q->columns[c].agg_mask) & TSKV_AGG_MAX) {
       cols[c].max_off = off;
       off += n_cells;
     }
@@ -567,12 +606,21 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
   sl.selval_off = off;
   off += n_first + n_last;
   sl.selval_len = n_first + n_last;
+  // TSKV_AGG_M2: the cells' shifts, sum(d) and sum(d^2), right after the values so that the exchange region holds them
+  plan.m2_of.assign(q->n_columns, -1);
+  for (uint32_t c = 0; c < q->n_columns; c++)
+    if (q->columns[c].agg_mask & TSKV_AGG_M2) {
+      plan.m2_of[c] = (int)plan.m2.size();
+      plan.m2.push_back(M2Col{cols[c].count_off, msum_off[c] ? msum_off[c] : cols[c].sum_off, off, off + n_cells, off + 2 * n_cells});
+      off += 3 * n_cells;
+    }
+  plan.m2_words = 3 * n_cells * plan.m2.size();
   off = (off + 1) & ~1ull;  // 16-byte alignment of the pair arrays
   sl.first_pairs_off = off;
   {
     uint64_t o = off;
     for (uint32_t c = 0; c < q->n_columns; c++)
-      if (q->columns[c].agg_mask & TSKV_AGG_FIRST) {
+      if (kernel_mask(q->columns[c].agg_mask) & TSKV_AGG_FIRST) {
         cols[c].first_off = o;
         o += 2 * n_cells;
       }
@@ -582,7 +630,7 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
   {
     uint64_t o = off;
     for (uint32_t c = 0; c < q->n_columns; c++)
-      if (q->columns[c].agg_mask & TSKV_AGG_LAST) {
+      if (kernel_mask(q->columns[c].agg_mask) & TSKV_AGG_LAST) {
         cols[c].last_off = o;
         o += 2 * n_cells;
       }
@@ -732,12 +780,12 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
     }
   for (uint32_t c = 0; c < q->n_columns; c++) {
     const tskv_agg_column &qc = q->columns[c];
-    if (qc.phys_type < TSKV_PT_I64 || qc.phys_type > TSKV_PT_BOOL || (qc.agg_mask & ~TSKV_AGG_ALL) || qc.agg_mask == 0) {
+    if (qc.phys_type < TSKV_PT_I64 || qc.phys_type > TSKV_PT_BOOL || (qc.agg_mask & ~(TSKV_AGG_ALL | TSKV_AGG_M2)) || qc.agg_mask == 0) {
       ctx->set_error("invalid query column (type or aggregate mask)");
       return TSKV_ERR_INVALID_ARG;
     }
-    if (qc.phys_type == TSKV_PT_BOOL && (qc.agg_mask & (TSKV_AGG_SUM | TSKV_AGG_MEAN))) {
-      ctx->set_error("sum / mean of a boolean column");
+    if (qc.phys_type == TSKV_PT_BOOL && (qc.agg_mask & (TSKV_AGG_SUM | TSKV_AGG_MEAN | TSKV_AGG_M2))) {
+      ctx->set_error("sum / mean / m2 of a boolean column");
       return TSKV_ERR_INVALID_ARG;
     }
     for (uint32_t c2 = 0; c2 < c; c2++)
@@ -762,6 +810,10 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
   }
   if (labels_first_last(q, E)) {
     ctx->set_error("bucket labels: first / last are not supported (the reference takes each batch's earliest row per label)");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  if (slide && query_has_m2(q)) {
+    ctx->set_error("sliding windows: M2 (variance) is not pushed down: folding panes would need a Chan merge of their second moments");
     return TSKV_ERR_UNSUPPORTED;
   }
   *win_k = 1;
@@ -818,6 +870,12 @@ struct ScanLayout {
   std::vector<MeanExport> means;
   std::vector<OutCol> outs;
   uint32_t use_smem = 0, smem_words = 0;  // the per-CTA shared-memory partial table (ScanParams)
+  // TSKV_AGG_M2: its columns, pass 2's column table (k_scan_m2) and shared-memory table, and the shift / sum(d) /
+  // sum(d^2) words that extend the exchange region
+  std::vector<M2Col> m2;
+  std::vector<ColState> cols2;
+  uint32_t use_smem2 = 0, smem_words2 = 0;
+  uint64_t m2_words = 0;
 };
 
 // n_cells: cells of the query's grid (a sliding scan: windows); kern_cells: cells of the fused kernels' grid (panes).
@@ -829,6 +887,8 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
   out.kern_sl = sliding ? pane.sl : win.sl;
   out.cols = sliding ? pane.cols : win.cols;
   out.means = win.means;
+  out.m2 = win.m2;  // (sliding scans refuse M2)
+  out.m2_words = win.m2_words;
   if (sliding) {
     for (uint32_t c = 0; c < q->n_columns; c++) {
       const ColState &p = pane.cols[c], &w = win.cols[c];
@@ -847,7 +907,7 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
   uint64_t fk = out.sl.first_keys_off, lk = out.sl.last_keys_off, fv = out.sl.selval_off, lv = out.sl.selval_off + out.sl.first_cells;
   for (uint32_t c = 0; c < q->n_columns; c++) {
     const tskv_agg_column &qc = q->columns[c];
-    for (unsigned bit = 0; bit < 7; bit++) {
+    for (unsigned bit = 0; bit < 8; bit++) {
       unsigned agg = 1u << bit;
       if (!(qc.agg_mask & agg)) continue;
       OutCol oc{};
@@ -861,6 +921,7 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
         case TSKV_AGG_MAX: oc.src_off = win.cols[c].max_off; break;
         case TSKV_AGG_FIRST: oc.src_off = fk; oc.val_off = fv; break;
         case TSKV_AGG_LAST: oc.src_off = lk; oc.val_off = lv; break;
+        case TSKV_AGG_M2: oc.src_off = win.m2[win.m2_of[c]].sd2_off; oc.val_off = win.m2[win.m2_of[c]].sd_off; break;
         default: break;
       }
       out.outs.push_back(oc);
@@ -873,7 +934,7 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
   std::vector<ColState> &cols = out.cols;
   uint32_t words = 0;
   for (uint32_t c = 0; c < q->n_columns; c++) {
-    const uint8_t m = q->columns[c].agg_mask;
+    const uint8_t m = kernel_mask(q->columns[c].agg_mask);
     const bool is_int = q->columns[c].phys_type != TSKV_PT_F64;
     cols[c].s_count = words; words += (uint32_t)kern_cells;
     if (m & (TSKV_AGG_SUM | TSKV_AGG_MEAN)) { cols[c].s_sum = words; words += (uint32_t)kern_cells; }
@@ -888,6 +949,26 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
   const uint64_t limit = (lim_env ? (uint64_t)atoi(lim_env) : 32) * 1024;
   out.use_smem = (!q->group_by_series && (uint64_t)words * 8 <= limit) ? 1u : 0u;
   out.smem_words = out.use_smem ? words : 0;
+  // pass 2: count_off = the shifts, sum_off / sumhi_off = sum(d) / sum(d^2); s_sum / s_hi in its own table
+  uint64_t words2 = 0;
+  for (uint32_t c = 0; c < q->n_columns && !out.m2.empty(); c++) {
+    ColState cs{};
+    cs.column_id = q->columns[c].column_id;
+    cs.phys_type = q->columns[c].phys_type;
+    if (win.m2_of[c] >= 0) {
+      const M2Col &mc = win.m2[win.m2_of[c]];
+      cs.agg_mask = TSKV_AGG_M2;
+      cs.count_off = mc.shift_off;
+      cs.sum_off = mc.sd_off;
+      cs.sumhi_off = mc.sd2_off;
+      cs.s_sum = (uint32_t)std::min<uint64_t>(words2, UINT32_MAX);
+      cs.s_hi = (uint32_t)std::min<uint64_t>(words2 + kern_cells, UINT32_MAX);
+      words2 += 2 * kern_cells;
+    }
+    out.cols2.push_back(cs);
+  }
+  out.use_smem2 = (!out.m2.empty() && !q->group_by_series && words2 * 8 <= limit) ? 1u : 0u;
+  out.smem_words2 = out.use_smem2 ? (uint32_t)words2 : 0;
   return out;
 }
 
@@ -1105,6 +1186,21 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
   for (uint32_t k = 0; k < q->n_predicates; k++) s->preds.p[k] = q->predicates[k];
   if (q->n_predicates) ensure_page_stats(ctx, pages);  // value-statistics pruning (filter_column_groups, reader/chunk.rs:12-50)
   if (e == cudaSuccess && q->n_predicates) e = stream_alloc(s->d_row_keep, (size_t)pages->keep_words, st);
+  s->n_m2 = (uint32_t)lay.m2.size();
+  s->m2_words = lay.m2_words;
+  if (s->n_m2) {
+    s->ev_m2_fork = new_event(cudaEventDisableTiming);
+    for (int b = 0; b < N_BINS; b++) s->ev_m2_join[b] = new_event(cudaEventDisableTiming);
+    if (e == cudaSuccess) e = upload(s->d_m2, lay.m2.data(), lay.m2.size(), st);
+    if (e == cudaSuccess) e = upload(s->d_cols2, lay.cols2.data(), lay.cols2.size(), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_fill2, (size_t)n_buckets + N_BINS, st);
+    *h2d += lay.m2.size() * sizeof(M2Col) + lay.cols2.size() * sizeof(ColState);
+    for (uint32_t c = 0; c < q->n_columns; c++) {  // the bins holding pages of an M2 column
+      const auto it = pages->col_bucket_pages.find(q->columns[c].column_id);
+      if (!(q->columns[c].agg_mask & TSKV_AGG_M2) || it == pages->col_bucket_pages.end()) continue;
+      for (int b = 0; b < N_BINS; b++) s->m2_bin[b] |= (it->second[b * WL_SUB] + it->second[b * WL_SUB + 1]) != 0;
+    }
+  }
   if (e == cudaSuccess) e = stream_alloc(s->d_aux, AUX_WORDS, st);
   if (e == cudaSuccess) e = stream_alloc(s->d_values, s->layout.n_out * s->layout.n_cells, st);
   if (e == cudaSuccess) e = stream_alloc(s->d_validity, s->layout.validity_bytes + 8, st);
@@ -1269,6 +1365,7 @@ tskv_status tskvgpu_ctx_create(int32_t device_id, tskv_ctx **out_ctx) {
       for (const bool edges : {false, true}) {
         for (int nm = NARROW_NONE; nm <= NARROW_ALL; nm++) raise((const void *)scan_kernel_for<false>(b, edges, nm));
         raise((const void *)scan_kernel_for<true>(b, edges));
+        raise((const void *)m2_kernel_for(b, edges));
       }
     }
     cudaGetLastError();
@@ -1950,6 +2047,15 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   P.n_tomb_global = pages->tomb.n_global;
   s->tomb_epoch = pages->tomb_epoch;
   plan_grids(ctx, pages, q, has_sel, P.edges != nullptr, P.smem_words, P.has_tomb, s->grid, s->occ, P.bin_parts, P.bin_part_rows);
+  if (s->n_m2) {  // pass 2: the same scan over the M2 columns' regions, with its own fills, task counters and tables
+    ScanParams &P2 = s->params2;
+    P2 = P;
+    P2.cols = s->d_cols2.get();
+    P2.region_fill = s->d_fill2.get();
+    P2.task_counter = s->d_fill2.get() + N_BINS * q->n_columns * WL_SUB;
+    P2.use_smem = lay.use_smem2;
+    P2.smem_words = lay.smem_words2;
+  }
   s->chunk_epoch = pages->chunk_epoch;
   if (pages->overlap.merge_rows && (st = prepare_merge(ctx, pages, q, s, &h2d)) != TSKV_OK) {
     delete s;
@@ -2090,7 +2196,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
                                                               s->n_merge_pages, s->d_mrow_off.get(), s->d_mbm_off.get(), s->d_mvals.get(),
                                                               reinterpret_cast<uint8_t *>(s->d_mvalid.get()), s->d_status, s->d_err_page, s->d_stats);
     const uint32_t mblocks = (uint32_t)((s->merge.n_rows + 127) / 128);
-    k_merge_chunks<<<mblocks, 128, 0, ctx->stream.get()>>>(s->params, s->merge);
+    k_merge_chunks<false><<<mblocks, 128, 0, ctx->stream.get()>>>(s->params, s->merge);
     launches += 2;
   }
   cudaEvent_t ev_fork = capturing ? s->ev_cfork.get() : s->ev_bin[0].get();
@@ -2146,7 +2252,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     cudaStreamWaitEvent(ctx->stream.get(), ev_done, 0);  // join
     launches++;
   }
-  if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
+  if (!capturing && !s->n_m2) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
   if (s->n_combine) {  // sliding windows: every window folds its panes (it writes every array the kernels fill)
     const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
     k_window_combine<<<dim3(std::max(1u, bx), s->n_combine), 256, 0, ctx->stream.get()>>>(
@@ -2158,6 +2264,33 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     uint32_t b = (uint32_t)std::min<uint64_t>((work + 255) / 256, 4096);
     k_export_pairs<<<std::max(1u, b), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->sl, s->d_means.get(), s->n_means, s->layout.n_cells);
     launches++;
+  }
+  if (s->n_m2) {  // TSKV_AGG_M2, pass 2: every cell's shift (pass-1 mean), then the M2 columns' rows once more
+    const uint32_t nb = N_BINS * s->n_cols * WL_SUB;
+    const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
+    k_m2_prep<<<dim3(std::max(1u, bx), s->n_m2), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_m2.get(), s->layout.n_cells,
+                                                                          s->d_bucket.get(), s->d_fill2.get(), nb, s->d_cols2.get(),
+                                                                          s->n_cols, s->params2.task_counter);
+    launches++;
+    if (s->merge.n_rows && s->n_merge_pages) {
+      k_merge_chunks<true><<<(uint32_t)((s->merge.n_rows + 127) / 128), 128, 0, ctx->stream.get()>>>(s->params2, s->merge);
+      launches++;
+    }
+    cudaEventRecord(s->ev_m2_fork.get(), ctx->stream.get());
+    const bool edges = s->params.edges != nullptr;
+    for (int b = 0; b < N_BINS; b++) {
+      if (!s->grid[b] || !s->m2_bin[b]) continue;
+      cudaStreamWaitEvent(ctx->bin_stream[b].get(), s->ev_m2_fork.get(), 0);
+      int bin = b;
+      const int sb = serial_bin_of(b);
+      void *args[] = {(void *)&s->params2, (void *)&bin};
+      CU_TRY(ctx, cudaLaunchKernel((const void *)m2_kernel_for(sb, edges), dim3(s->grid[b]), dim3(SCAN_THREADS), args,
+                                   serial_smem_bytes(sb, s->params2.smem_words, s->params2.has_tomb), ctx->bin_stream[b].get()));
+      cudaEventRecord(s->ev_m2_join[b].get(), ctx->bin_stream[b].get());
+      cudaStreamWaitEvent(ctx->stream.get(), s->ev_m2_join[b].get(), 0);
+      launches++;
+    }
+    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes pass 2)
   }
   if (!capturing) cudaEventRecord(s->ev1.get(), ctx->stream.get());
   CU_TRY(ctx, cudaGetLastError());
@@ -2296,6 +2429,11 @@ tskv_status tskvgpu_scan_work_list(tskv_ctx *ctx, tskv_scan *s, uint32_t *n_buck
 
 tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_view *out) {
   if (!ctx || !s || !out) return TSKV_ERR_INVALID_ARG;
+  if (s->n_m2) {
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    ctx->set_error("scan_partials: second moments (TSKV_AGG_M2) do not all-reduce element-wise; use tskvgpu_scan_exchange");
+    return TSKV_ERR_UNSUPPORTED;
+  }
   const StateLayout &L = s->sl;
   uint64_t base = (uint64_t)(uintptr_t)s->d_state.get();
   out->sum_i64_ptr = base + L.sum_i64_off * 8;
@@ -2313,10 +2451,18 @@ tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_vie
   return TSKV_OK;
 }
 
+// The M2 columns of gathered partials: Chan's merge of every rank's (count, sum, M2) (k_merge_m2).
+static void merge_m2(tskv_ctx *ctx, tskv_scan *s, const uint64_t *gathered, uint32_t n_ranks, uint64_t words) {
+  if (!s->n_m2) return;
+  const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
+  k_merge_m2<<<dim3(std::max(1u, bx), s->n_m2), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_m2.get(), s->layout.n_cells, gathered,
+                                                                         n_ranks, words);
+}
+
 tskv_status tskvgpu_scan_exchange_view(tskv_ctx *ctx, tskv_scan *s, uint64_t *out_dptr, uint64_t *out_words) {
   if (!ctx || !s || !out_dptr || !out_words) return TSKV_ERR_INVALID_ARG;
   *out_dptr = (uint64_t)(uintptr_t)s->d_state.get();
-  *out_words = s->sl.selval_off + s->sl.selval_len;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values
+  *out_words = s->sl.selval_off + s->sl.selval_len + s->m2_words;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values | M2
   return TSKV_OK;
 }
 
@@ -2324,10 +2470,11 @@ tskv_status tskvgpu_scan_merge_gathered(tskv_ctx *ctx, tskv_scan *s, uint64_t ga
   if (!ctx || !s || !gathered_dptr || n_ranks == 0) return TSKV_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(ctx->mu);
   cudaSetDevice(ctx->device);
-  const uint64_t words = s->sl.selval_off + s->sl.selval_len;
+  const uint64_t words = s->sl.selval_off + s->sl.selval_len + s->m2_words;
   uint32_t blocks = (uint32_t)std::min<uint64_t>((words + 255) / 256, 2048);
   k_merge_gathered<<<std::max(1u, blocks), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->sl, reinterpret_cast<const uint64_t *>((uintptr_t)gathered_dptr),
                                                                    n_ranks, words);
+  merge_m2(ctx, s, reinterpret_cast<const uint64_t *>((uintptr_t)gathered_dptr), n_ranks, words);
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;
 }
@@ -2341,7 +2488,7 @@ tskv_status tskvgpu_scan_exchange(tskv_ctx *ctx, tskv_scan *s) {
     return TSKV_ERR_NCCL;
   }
   const NcclApi &N = nccl_api();
-  const uint64_t words = s->sl.selval_off + s->sl.selval_len;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values
+  const uint64_t words = s->sl.selval_off + s->sl.selval_len + s->m2_words;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values | M2
   if (!s->d_gathered) CU_TRY(ctx, stream_alloc(s->d_gathered, (size_t)ctx->n_ranks * words, ctx->stream.get()));
   const ncclResult_t r = N.AllGather(s->d_state.get(), s->d_gathered.get(), words, ncclUint64, ctx->comm, ctx->stream.get());
   if (r != ncclSuccess) {
@@ -2350,6 +2497,7 @@ tskv_status tskvgpu_scan_exchange(tskv_ctx *ctx, tskv_scan *s) {
   }
   uint32_t blocks = (uint32_t)std::min<uint64_t>((words + 255) / 256, 2048);
   k_merge_gathered<<<std::max(1u, blocks), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->sl, s->d_gathered.get(), (uint32_t)ctx->n_ranks, words);
+  merge_m2(ctx, s, s->d_gathered.get(), (uint32_t)ctx->n_ranks, words);
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;
 }

@@ -12,11 +12,31 @@ import ctypes as C
 import numpy as np
 
 from . import cabi
-from .cabi import (TSKV_AGG_COUNT, TSKV_AGG_FIRST, TSKV_AGG_LAST, TSKV_AGG_MAX, TSKV_AGG_MEAN,
+from .cabi import (TSKV_AGG_COUNT, TSKV_AGG_FIRST, TSKV_AGG_LAST, TSKV_AGG_M2, TSKV_AGG_MAX, TSKV_AGG_MEAN,
                    TSKV_AGG_MIN, TSKV_AGG_SUM, TSKV_PT_F64, TSKV_PT_I64, TSKV_PT_TIME, TSKV_PT_U64)
 
 AGG_BITS = {"count": TSKV_AGG_COUNT, "sum": TSKV_AGG_SUM, "min": TSKV_AGG_MIN, "max": TSKV_AGG_MAX,
-            "mean": TSKV_AGG_MEAN, "avg": TSKV_AGG_MEAN, "first": TSKV_AGG_FIRST, "last": TSKV_AGG_LAST}
+            "mean": TSKV_AGG_MEAN, "avg": TSKV_AGG_MEAN, "first": TSKV_AGG_FIRST, "last": TSKV_AGG_LAST,
+            "m2": TSKV_AGG_M2}
+# DataFusion's statistical aggregates, computed on the host from the scan's COUNT and M2 (sum of squared deviations):
+# name -> (divisor n - ddof, sqrt?). stddev / var are the sample forms.
+STAT_AGGS = {"var": (1, False), "var_samp": (1, False), "var_pop": (0, False),
+             "stddev": (1, True), "stddev_samp": (1, True), "stddev_pop": (0, True)}
+
+
+def stat_from_m2(name, count, m2, valid):
+    """DataFusion's final formula of a STAT_AGGS aggregate from COUNT and M2 cells (numpy arrays): var_pop = m2 / n,
+    var_samp = m2 / (n - 1), stddev* = sqrt(var*). Returns (values f64, validity): NULL where n <= ddof (an empty cell; a
+    one-value cell for the sample forms)."""
+    ddof, root = STAT_AGGS[name]
+    n = np.asarray(count, dtype=np.uint64).astype(np.float64)
+    ok = np.asarray(valid, dtype=bool) & (n > ddof)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        v = np.where(ok, np.asarray(m2, dtype=np.float64) / np.where(ok, n - ddof, 1.0), 0.0)
+    if root:
+        with np.errstate(invalid="ignore"):
+            v = np.sqrt(v)
+    return v, ok
 
 
 def _wrap64(x):
@@ -185,10 +205,11 @@ class PushedAggregate:
         else:
             self.agg_mask = 0
             for a in aggs:
-                self.agg_mask |= AGG_BITS[a]
+                # var* / stddev* ask the scan for COUNT | M2; ScanResult.column derives them
+                self.agg_mask |= (TSKV_AGG_COUNT | TSKV_AGG_M2) if a in STAT_AGGS else AGG_BITS[a]
 
     def agg_list(self):
-        return [b for b in (1, 2, 4, 8, 16, 32, 64) if self.agg_mask & b]
+        return [b for b in (1, 2, 4, 8, 16, 32, 64, 128) if self.agg_mask & b]
 
 
 class QueryOption:
@@ -259,13 +280,18 @@ class ScanResult:
         self.phys = {(c.column_id): c.phys_type for c in query.columns}
 
     def column(self, column_id, agg):
-        """(typed values, validity) of one output column, shaped [n_groups, n_buckets]."""
+        """(typed values, validity) of one output column, shaped [n_groups, n_buckets]. agg may also name one of STAT_AGGS
+        (var, var_samp, var_pop, stddev, stddev_samp, stddev_pop), derived from the column's count and m2."""
+        if agg in STAT_AGGS:
+            n, _ = self.column(column_id, "count")
+            m2, ok = self.column(column_id, "m2")
+            return stat_from_m2(agg, n, m2, ok)
         j = self.names.index((column_id, agg))
         raw = self.values[j]
         pt = self.phys[column_id]
         if agg == "count":
             v = raw.view(np.uint64)
-        elif agg == "mean" or pt == TSKV_PT_F64:
+        elif agg in ("mean", "m2") or pt == TSKV_PT_F64:
             v = raw.view(np.float64)
         elif pt == TSKV_PT_I64:
             v = raw.view(np.int64)
@@ -507,6 +533,11 @@ class Engine:
         return (None if ids is None else ids.ctypes.data), int(n_groups), ids
 
     @staticmethod
+    def _no_m2_with_slide(query, slide):
+        if slide is not None and any(c.agg_mask & TSKV_AGG_M2 for c in query.columns):
+            raise ValueError("m2 / var* / stddev* and slide: sliding windows do not push the variance state down")
+
+    @staticmethod
     def _edges(edges, slide):
         """Explicit time-bucket edges as a contiguous int64 array (kept alive by the caller), or None."""
         if edges is None:
@@ -558,6 +589,7 @@ class Engine:
         origin and first_bucket_start 0; calendar_edges makes them for date_trunc). Not with slide.
         labels: with edges, labels[b] < query.n_buckets is the output bucket of edge bucket b (one per edge bucket;
         calendar_parts makes them for date_part). query.n_buckets is then the number of output buckets."""
+        self._no_m2_with_slide(query, slide)
         e = self._edges(edges, slide)
         lab = self._labels(labels, e)
         L = self.output_layout(pages, query, group_ids, n_groups, e, lab)
@@ -587,6 +619,7 @@ class Engine:
     def prepare(self, pages, query, slide=None, group_ids=None, n_groups=None, edges=None, labels=None):
         """Device-resident scan (run / enqueue / partials / exchange / finalize); slide, group_ids, edges, labels: as in
         scan_aggregate."""
+        self._no_m2_with_slide(query, slide)
         e = self._edges(edges, slide)
         lab = self._labels(labels, e)
         L = self.output_layout(pages, query, group_ids, n_groups, e, lab)

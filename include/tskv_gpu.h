@@ -105,7 +105,17 @@ enum {
   TSKV_AGG_MEAN = 1u << 4,  /* f64 = sum / count */
   TSKV_AGG_FIRST = 1u << 5, /* value at the smallest timestamp */
   TSKV_AGG_LAST = 1u << 6,  /* value at the largest timestamp */
-  TSKV_AGG_ALL = 0x7f
+  TSKV_AGG_ALL = 0x7f,      /* the seven aggregates above (not M2) */
+  /* f64 M2 = sum over the cell's valid, selected values of (x - mean)^2, x converted to f64 first (DataFusion's variance
+   * state, with count: var_pop = M2 / n, var_samp = M2 / (n - 1), stddev* = sqrt(var*)). Valid iff the cell holds at least
+   * one value; a one-value cell reads 0.0; NaN or +-inf among the values gives NaN. I64 / U64 / F64 columns; a BOOL column
+   * is refused like SUM (TSKV_ERR_INVALID_ARG). Computed in two passes over the column's pages: pass 1 (the scan as
+   * without M2, which also keeps the column's COUNT and exact SUM) gives every cell's mean m, pass 2 decodes the same rows
+   * again and sums d = x - m and d^2; M2 = sum(d^2) - sum(d)^2 / n (corrected two-pass algorithm). Refused before any
+   * launch with TSKV_ERR_UNSUPPORTED: sliding windows (slide != width). tskvgpu_scan_partials refuses a scan with M2.
+   * Counters: page_read_count, page_read_bytes, points_decoded and rows_in_range are those of the same query without M2
+   * (the reference reads each page once); kernel_launches and elapsed_fused_ms include pass 2. */
+  TSKV_AGG_M2 = 1u << 7
 };
 
 /* One projected value column and the aggregates wanted for it. Extends
@@ -341,6 +351,9 @@ typedef struct tskv_partials_view {
   uint64_t sel_first_len;            /* number of FIRST cells (prefix of sel_val / suffix of min) */
   uint64_t sel_last_len;             /* number of LAST cells */
 } tskv_partials_view;
+/* A scan with TSKV_AGG_M2 has no partials view (TSKV_ERR_UNSUPPORTED): second moments taken around each rank's own means
+ * do not all-reduce element-wise. Its ranks merge with tskvgpu_scan_exchange / _merge_gathered, which combine the ranks'
+ * (count, sum, M2) with Chan's formula M2 = sum M2_r + sum n_r (m_r - m)^2. */
 
 tskv_status tskvgpu_scan_prepare(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q,
                                  tskv_scan **out_scan);

@@ -30,6 +30,8 @@ pub const TSKV_AGG_MAX: u8 = 1 << 3;
 pub const TSKV_AGG_MEAN: u8 = 1 << 4;
 pub const TSKV_AGG_FIRST: u8 = 1 << 5;
 pub const TSKV_AGG_LAST: u8 = 1 << 6;
+/// f64 sum of squared deviations from the cell mean (the variance state; two passes, see tskv_gpu.h).
+pub const TSKV_AGG_M2: u8 = 1 << 7;
 
 pub const TSKV_UPLOAD_VERIFY_CRC: u32 = 1;
 pub const TSKV_UPLOAD_HOST_RESIDENT: u32 = 2;
