@@ -4,7 +4,6 @@ Gorilla, raw and boolean value pages; NULLs at runs' first / last rows, equal ti
 a run's first row, several column groups per series, the 62-bit key budget at 61 / 62 / 63 bits; tombstone edges on,
 one before and one after rows at bucket edges, restart-point cuts, page ends and the i64 limits. Every query runs with
 pages whole and cut into 3 parts, by bucket, by series, by tags and unbucketed; one per arena as a two-shard exchange."""
-import copy
 import functools
 
 import numpy as np
@@ -14,6 +13,7 @@ from cnosdb_b200 import cabi
 from cnosdb_b200.engine import TskvError
 from tests import exact_arenas as ea
 from tests.helpers import assert_matches_exact, exact_aggregate
+from tests.ranks import sharded_scans, with_series
 
 pytestmark = pytest.mark.gpu
 
@@ -35,46 +35,6 @@ def _scan(engine, pages, q, extra):
     return engine.scan_aggregate(pages, q, group_ids=extra.get("group_ids"), n_groups=extra.get("n_groups"))
 
 
-def with_series(q, ids):
-    q = copy.copy(q)
-    q.series_ids = np.asarray(ids, dtype=np.uint32)
-    q._keep = None
-    return q
-
-
-def two_shard_exchange(engine, arena, descs, q, shard_ids, files=None, tombstones=None):
-    """Scan the series shards of one arena separately (their page sets: the shards' descriptors) with the global
-    selection of `q`, gather the exchange regions like an all-gather on one device and merge them
-    (tskvgpu_scan_merge_gathered): -> every rank's finalized result. (An integer MEAN adds the ranks' f64 sums: compare
-    it with int_mean=False.)"""
-    import torch
-    from cnosdb_b200.parallel import device_tensor
-    dev = torch.device("cuda", engine.device)
-    cg_series = descs["series_id"][descs["phys_type"] == cabi.TSKV_PT_TIME]
-    scans, regions, keep, out = [], [], [], []
-    for ids in shard_ids:
-        pages = engine.upload_pages(arena, descs[np.isin(descs["series_id"], ids)])
-        if files is not None:
-            pages.set_chunk_files(np.asarray(files)[np.isin(cg_series, ids)])
-        if tombstones is not None:
-            pages.set_tombstones(tombstones)
-        s = engine.prepare(pages, q)
-        s.run()
-        ptr, words = s.exchange_view()
-        regions.append(device_tensor(ptr, words, torch.int64, dev).clone())
-        scans.append(s)
-        keep.append(pages)
-    gathered = torch.cat(regions)
-    torch.cuda.synchronize()
-    for s in scans:
-        s.merge_gathered(gathered.data_ptr(), len(scans))
-        out.append(s.finalize())
-        s.close()
-    for pages in keep:
-        pages.close()
-    return out
-
-
 @pytest.mark.parametrize("kind", ea.FL_KINDS)
 def test_first_last_runs(engine, kind, monkeypatch):
     arena, descs, truth = fl_arena(kind)
@@ -92,7 +52,7 @@ def test_first_last_runs(engine, kind, monkeypatch):
             continue
         q = q if q.series_ids is not None else with_series(q, ids)
         exp = exact_aggregate(truth, q)
-        for got in two_shard_exchange(engine, arena, descs, q, (ids[ids % 2 == 0], ids[ids % 2 == 1])):
+        for got in sharded_scans(engine, arena, descs, q, (ids[ids % 2 == 0], ids[ids % 2 == 1])):
             assert_matches_exact(got, exp, what="%s %s 2-shard exchange" % (kind, name), int_mean=False)
 
 
@@ -132,5 +92,5 @@ def test_tombstone_edges(engine, step, kind, monkeypatch):
     q = ea.tombstone_queries(truth, step)[0][1]
     ids = q.series_ids
     exp = exact_aggregate(truth, q, tombstones=tombs)
-    for got in two_shard_exchange(engine, arena, descs, q, (ids[:5], ids[5:]), tombstones=tombs):
+    for got in sharded_scans(engine, arena, descs, q, (ids[:5], ids[5:]), tombstones=tombs):
         assert_matches_exact(got, exp, what="step %d %s 2-shard exchange" % (step, kind), int_mean=False)

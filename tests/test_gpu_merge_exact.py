@@ -9,7 +9,7 @@ import pytest
 from oracle import pyoracle as orc
 from tests import exact_arenas as ea
 from tests.helpers import assert_matches_exact
-from tests.test_gpu_first_last_tombstones import two_shard_exchange
+from tests.ranks import sharded_scans
 
 pytestmark = pytest.mark.gpu
 
@@ -55,7 +55,7 @@ def test_merge_through_a_two_shard_exchange(engine, merge_set):
         ids = q.series_ids
         for tb in (None, tombs):
             exp = ea.expected(truth, q, {}, tombstones=tb, files=files)
-            for got in two_shard_exchange(engine, arena, descs, q, (ids[ids % 2 == 0], ids[ids % 2 == 1]), files=files,
-                                          tombstones=tb):
+            for got in sharded_scans(engine, arena, descs, q, (ids[ids % 2 == 0], ids[ids % 2 == 1]), files=files,
+                                     tombstones=tb):
                 assert_matches_exact(got, exp, what="%s tombstones=%s 2-shard exchange" % (name, tb is not None),
                                      int_mean=False)

@@ -25,7 +25,7 @@ from tests.labels_reference import exact_aggregate_labels
 from tests.test_gpu_bucket_edges import edge_query, random_edges, span
 from tests.test_gpu_bucket_labels import label_query
 from tests.test_gpu_parity import random_tombstones
-from tests.variance_reference import exact_m2, with_m2
+from tests.variance_reference import check_m2, exact_m2, with_m2
 
 pytestmark = pytest.mark.gpu
 
@@ -44,28 +44,6 @@ def without_m2(q):
     out.columns = [PushedAggregate(c.column_id, c.phys_type, c.agg_mask & ~cabi.TSKV_AGG_M2) for c in q.columns]
     out._keep = None
     return out
-
-
-def check_m2(got, exp, what, rtol=1e-9):
-    """got's m2 outputs against the exact ones: validity equal, NaN where NaN, else within rtol relative (plus the
-    rounding of a shift that is not exactly the mean, for cells whose M2 is 0)."""
-    n_m2 = 0
-    for j, (col, agg) in enumerate(got.names):
-        if agg != "m2":
-            continue
-        n_m2 += 1
-        gv, ev = got.validity[j], exp.validity[j]
-        assert (gv == ev).all(), "%s col %s: m2 validity differs at %s" % (what, col, np.nonzero(gv != ev)[0][:5])
-        g = got.values[j].view(np.float64)[ev]
-        e = exp.values[j].view(np.float64)[ev]
-        nan = np.isnan(e)
-        assert (np.isnan(g) == nan).all(), "%s col %s: NaN cells differ" % (what, col)
-        with np.errstate(invalid="ignore"):
-            bad = np.nonzero(~nan & ~(np.abs(g - e) <= rtol * np.abs(e) + 1e-300))[0]
-        assert bad.size == 0, "%s col %s m2 at cells %s: got %s exact %s" % (
-            what, col, np.nonzero(ev)[0][bad[:3]], g[bad[:3]], e[bad[:3]])
-        assert (got.values[j][~gv] == 0).all()
-    assert n_m2
 
 
 def check_rest_unchanged(engine, pages, q, got, counters, what, **kw):
@@ -184,11 +162,13 @@ def test_bins(engine, kind, n_points, monkeypatch):
     arena, descs, truth = bins_arena(kind, n_points)
     fbs, nb = grid(truth, 37_000)
     lo, hi = span(truth)
-    for parts in ("1", "3"):
+    for parts, smem_kb in (("1", None), ("3", None), ("1", "0")):  # TSKV_SMEM_TABLE_KB=0: the global-memory table
         monkeypatch.setenv("TSKV_PARTS", parts)
+        if smem_kb is not None:
+            monkeypatch.setenv("TSKV_SMEM_TABLE_KB", smem_kb)
         pages = engine.upload_pages(arena, descs)
         q = m2_query(width=37_000, first_bucket_start=fbs, n_buckets=nb)
-        scan_and_check(engine, pages, truth, q, "%s/%d parts %s" % (kind, n_points, parts),
+        scan_and_check(engine, pages, truth, q, "%s/%d parts %s smem_kb %s" % (kind, n_points, parts, smem_kb),
                        lambda: with_m2(lambda: exact_aggregate(truth, q), q))
         q = m2_query(width=37_000, first_bucket_start=fbs, n_buckets=nb, time_ranges=[(lo + 5_000, hi - 7_000)],
                      predicates=[(1, cabi.TSKV_PT_I64, ">", -40)])

@@ -101,3 +101,25 @@ def with_m2(run, query, n_groups=None):
             out[k], ok[k] = exact_m2(xs), True
         res.values[j], res.validity[j] = out.view(np.uint64), ok
     return res
+
+
+def check_m2(got, exp, what, rtol=1e-9):
+    """got's m2 outputs against the exact ones: validity equal, NaN where NaN, else within rtol relative (plus the
+    rounding of a shift that is not exactly the mean, for cells whose M2 is 0)."""
+    n_m2 = 0
+    for j, (col, agg) in enumerate(got.names):
+        if agg != "m2":
+            continue
+        n_m2 += 1
+        gv, ev = got.validity[j], exp.validity[j]
+        assert (gv == ev).all(), "%s col %s: m2 validity differs at %s" % (what, col, np.nonzero(gv != ev)[0][:5])
+        g = got.values[j].view(np.float64)[ev]
+        e = exp.values[j].view(np.float64)[ev]
+        nan = np.isnan(e)
+        assert (np.isnan(g) == nan).all(), "%s col %s: NaN cells differ" % (what, col)
+        with np.errstate(invalid="ignore"):
+            bad = np.nonzero(~nan & ~(np.abs(g - e) <= rtol * np.abs(e) + 1e-300))[0]
+        assert bad.size == 0, "%s col %s m2 at cells %s: got %s exact %s" % (
+            what, col, np.nonzero(ev)[0][bad[:3]], g[bad[:3]], e[bad[:3]])
+        assert (got.values[j][~gv] == 0).all()
+    assert n_m2
