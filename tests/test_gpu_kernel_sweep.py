@@ -1,0 +1,191 @@
+"""Every instantiation of the fused scan's kernels, and random combinations of query features, against the exact reference.
+
+1. test_every_instantiation: one case aimed at each key of sweep_reference.INSTANTIATIONS (k_scan_aggregate<TK, VK, SEL,
+   NARROW, EDGES> and k_scan_m2<TK, VK, EDGES>) through its long bin, and through its short bin too where it runs one
+   (bins 9-12). The arena holds field pages of that one bin only; the work list read back after the pass proves the bin
+   held them with the intended narrow flag, so a change of the generator cannot move a case to another kernel unseen. The
+   result is held to the exact reference (M2 to the exact M2), and the keys reached must be the whole list.
+2. test_random_combinations: N_RANDOM seeded cases (tests/sweep_reference.py: random_case) that draw the arena's codecs,
+   page lengths, NULLs, column groups and overlapping chunk files, the grouping (bucket, series, tags, edges, labels,
+   sliding window, unbucketed), aggregates with FIRST / LAST and M2, predicates, time ranges, tombstones, a host-resident
+   page set, CRC on read, TSKV_PARTS and TSKV_SMEM_TABLE_KB. Each is checked against its expected result or status, and
+   scanned twice (a prepared scan, then an end-to-end call): every output that does not depend on the order of f64
+   additions must be byte-identical. TSKV_SWEEP_CASE=<index> reruns one case."""
+import os
+
+import numpy as np
+import pytest
+
+from cnosdb_b200 import cabi
+from cnosdb_b200.engine import TskvError
+from tests import sweep_reference as sw
+from tests.helpers import assert_matches_exact
+from tests.variance_reference import check_m2
+
+pytestmark = pytest.mark.gpu
+
+BASE_SEED = 20261017
+N_RANDOM = 300
+ONE_CASE = os.environ.get("TSKV_SWEEP_CASE")  # rerun one index of test_random_combinations
+
+
+class _Picked:
+    """The outputs `keep` of a ScanResult / ExactResult (assert_matches_exact reads names, values, validity, phys and,
+    for ExactResult, center / bound by output index)."""
+
+    def __init__(self, res, keep):
+        self.names = [res.names[j] for j in keep]
+        self.values, self.validity, self.phys = res.values[keep], res.validity[keep], res.phys
+        if hasattr(res, "center"):
+            self.center = {i: res.center[j] for i, j in enumerate(keep) if j in res.center}
+            self.bound = {i: res.bound[j] for i, j in enumerate(keep) if j in res.bound}
+
+
+def check_exact(got, exp, what):
+    """Every output against the exact reference: M2 by check_m2, the rest by assert_matches_exact."""
+    rest = [j for j, (_, a) in enumerate(got.names) if a != "m2"]
+    if len(rest) < len(got.names):
+        check_m2(got, exp, what)
+    assert_matches_exact(_Picked(got, rest), _Picked(exp, rest), what=what)
+
+
+def deterministic_outputs(res):
+    """Indices of the outputs that do not depend on the order of f64 additions: counts, integer sums and means, MIN /
+    MAX and FIRST / LAST of every type."""
+    return [j for j, (c, a) in enumerate(res.names)
+            if not (a == "m2" or (a in ("sum", "mean") and res.phys[c] == cabi.TSKV_PT_F64))]
+
+
+def assert_same_bytes(a, b, what):
+    keep = deterministic_outputs(a)
+    assert a.names == b.names
+    assert (a.validity == b.validity).all(), "%s: validity differs between two runs" % what
+    bad = [a.names[j] for j in keep if (a.values[j] != b.values[j]).any()]
+    assert not bad, "%s: outputs %s differ between two runs" % (what, bad)
+
+
+def set_env(monkeypatch, env):
+    for k, v in env.items():
+        if v is None:
+            monkeypatch.delenv(k, raising=False)
+        else:
+            monkeypatch.setenv(k, v)
+
+
+def scan_kwargs(extra):
+    return {k: extra[k] for k in ("slide", "group_ids", "n_groups", "edges", "labels") if k in extra}
+
+
+def prepared_run(engine, pages, query, extra):
+    """-> (ScanResult, work list) of a prepared scan, or (status, None) when the library refuses it."""
+    try:
+        scan = engine.prepare(pages, query, **scan_kwargs(extra))
+    except TskvError as e:
+        return e.status, None
+    except ValueError:
+        return "ValueError", None
+    try:
+        scan.run()
+        return scan.finalize(), scan.work_list()
+    except TskvError as e:
+        return e.status, None
+    finally:
+        scan.close()
+
+
+# ---- 1. every instantiation --------------------------------------------------------------------------------------------
+def targets():
+    """(key, bin) of every targeted case: the key's serial bin, and the short bin that runs the same kernels."""
+    short_of = {s: b for b, s in sw.SHORT_BINS.items()}
+    out = []
+    for key in sw.INSTANTIATIONS:
+        sb = key[1] * sw.N_VK + key[2]
+        out.append((key, sb))
+        if sb in short_of:
+            out.append((key, short_of[sb]))
+    return out
+
+
+def arena_narrow(key):
+    """The narrow flag the case's bin must carry: the key's, for the narrow variants; wide pages otherwise."""
+    return key[4]
+
+
+def test_every_instantiation(engine, monkeypatch):
+    set_env(monkeypatch, {"TSKV_PARTS": None, "TSKV_SMEM_TABLE_KB": None})
+    reached, short_reached, arenas = {}, set(), {}
+    for i, (key, b) in enumerate(targets()):
+        what = "%s via bin %d" % (sw.key_name(key), b)
+        narrow = arena_narrow(key)
+        if (b, narrow) not in arenas:
+            arenas[(b, narrow)] = sw.bin_arena(b, narrow)
+        arena, descs, truth = arenas[(b, narrow)]
+        q, extra = sw.targeted_query(truth, key, seed=i)
+        exp = sw.expected(truth, q, extra)
+        assert not isinstance(exp, (int, str)), "%s: the reference refuses the case (%s)" % (what, exp)
+        pages = engine.upload_pages(arena, descs)
+        try:
+            got, wl = prepared_run(engine, pages, q, extra)
+        finally:
+            pages.close()
+        assert wl is not None, "%s: status %s" % (what, got)
+        field = (descs["phys_type"] != cabi.TSKV_PT_TIME) & np.isin(descs["series_id"], q.series_ids)
+        assert (wl["page_bin"][field] == b).all(), "%s: field pages in bins %s" % (what, sorted(set(wl["page_bin"][field])))
+        assert sw.bin_fill(wl, len(q.columns))[b].sum() == field.sum(), what
+        flags = sw.bin_narrow_flags(wl, descs)
+        assert flags[b] == narrow, "%s: narrow flag %d" % (what, flags[b])
+        if narrow != sw.NARROW_SOME and sw.serial_bin(b) in (0, 3):  # (HELPER_SERIES)
+            assert sw.NARROW_SOME in flags, "%s: the work list reports no narrow flags" % what
+        keys = sw.kernel_keys(wl, descs, q, "edges" in extra)
+        assert key in keys and all(bins == {b} for bins in keys.values()), "%s: ran %s" % (what, keys)
+        check_exact(got, exp, what)
+        for k in keys:
+            reached.setdefault(k, set()).add(b)
+        if b >= sw.N_SERIAL_BINS:
+            short_reached.add(b)
+    missed = [sw.key_name(k) for k in sw.INSTANTIATIONS if k not in reached]
+    assert not missed, "instantiations no targeted case reached: %s" % missed
+    assert short_reached == set(sw.SHORT_BINS), short_reached
+    print("\nkernel sweep: %d of %d instantiations reached, short bins %s" % (len(reached), len(sw.INSTANTIATIONS),
+                                                                           sorted(short_reached)))
+
+
+# ---- 2. random combinations --------------------------------------------------------------------------------------------
+def run_case(engine, case, exp, monkeypatch):
+    """-> the instantiation keys the case ran. Fails with the case's description."""
+    what = case.describe()
+    set_env(monkeypatch, case.env)
+    pages = engine.upload_pages(case.arena, case.descs, host_resident=case.host_resident,
+                                verify_on_read=case.verify_on_read)
+    try:
+        if case.tombstones is not None:
+            pages.set_tombstones(case.tombstones)
+        if case.files is not None:
+            pages.set_chunk_files(case.files)
+        got, wl = prepared_run(engine, pages, case.query, case.extra)
+        if isinstance(exp, (int, str)):
+            assert got == exp, "%s\nstatus %s, expected %s" % (what, got, exp)
+            return {}
+        assert wl is not None, "%s\nstatus %s, expected a result" % (what, got)
+        check_exact(got, exp, what)
+        again = engine.scan_aggregate(pages, case.query, **scan_kwargs(case.extra))
+        assert_same_bytes(got, again, what)
+        return sw.kernel_keys(wl, case.descs, case.query, "edges" in case.extra)
+    finally:
+        pages.close()
+
+
+def test_random_combinations(engine, monkeypatch):
+    indices = [int(ONE_CASE)] if ONE_CASE is not None else range(N_RANDOM)
+    reached, statuses = {}, {}
+    for i in indices:
+        case = sw.random_case(i, BASE_SEED)
+        exp = sw.case_expected(case)
+        outcome = exp if isinstance(exp, (int, str)) else "result"
+        statuses[outcome] = statuses.get(outcome, 0) + 1
+        for k, bins in run_case(engine, case, exp, monkeypatch).items():
+            reached.setdefault(k, set()).update(bins)
+    short = sorted({b for bins in reached.values() for b in bins if b >= sw.N_SERIAL_BINS})
+    print("\nrandom combinations: %d cases, outcomes %s, %d of %d instantiations reached, short bins %s; not reached: %s" % (
+        len(indices), statuses, len(reached), len(sw.INSTANTIATIONS), short,
+        [sw.key_name(k) for k in sw.INSTANTIATIONS if k not in reached]))
