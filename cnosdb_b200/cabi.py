@@ -35,6 +35,8 @@ TSKV_AGG_MEAN, TSKV_AGG_FIRST, TSKV_AGG_LAST, TSKV_AGG_ALL = 16, 32, 64, 0x7F
 # f64 sum of squared deviations from the cell mean (the variance state; engine.py derives var* / stddev* from it)
 TSKV_AGG_M2 = 0x80
 AGG_NAMES = {1: "count", 2: "sum", 4: "min", 8: "max", 16: "mean", 32: "first", 64: "last", 128: "m2"}
+# column pairs of tskv_query.n_pairs (covariance / correlation state; engine.py derives covar* / corr from it)
+TSKV_MAX_PAIRS = 8
 TSKV_UPLOAD_VERIFY_CRC = 1
 TSKV_UPLOAD_HOST_RESIDENT = 2
 TSKV_UPLOAD_VERIFY_ON_READ = 4
@@ -89,7 +91,7 @@ class Query(C.Structure):
                 ("origin", C.c_int64), ("width", C.c_int64), ("first_bucket_start", C.c_int64),
                 ("n_buckets", C.c_uint32), ("group_by_series", C.c_uint32),
                 ("columns", C.POINTER(AggColumn)), ("n_columns", C.c_uint32), ("reserved", C.c_uint32),
-                ("predicates", C.POINTER(FieldPredicate)), ("n_predicates", C.c_uint32), ("reserved2", C.c_uint32)]
+                ("predicates", C.POINTER(FieldPredicate)), ("n_predicates", C.c_uint32), ("n_pairs", C.c_uint32)]
 
 
 class OutputLayout(C.Structure):

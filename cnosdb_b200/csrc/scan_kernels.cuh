@@ -2218,6 +2218,253 @@ __global__ void k_merge_m2(uint64_t *state, const M2Col *m2, uint64_t n_cells, c
   }
 }
 
+// ---- column pairs (tskv_query.n_pairs): covariance / correlation state ---------------------------------------------
+// One pair's state is PAIR_WORDS sections of n_cells words from `off` on (PairSec), right after the M2 sections so that
+// the exchange region holds them. Pass 1 (k_scan_pair<false>) sums the paired rows' n, x and y and keeps the order keys
+// of their smallest and largest f64 x and y (pair_ukey; a min is kept as ~key so that every section starts at 0 and
+// grows with atomicMax); k_pair_prep writes the shifts sum / n; pass 2 sums dx, dy, dx dy, dx^2 and dy^2 around them.
+enum PairSec { PS_N = 0, PS_SX, PS_SY, PS_XMIN, PS_XMAX, PS_YMIN, PS_YMAX, PS_SHX, PS_SHY, PS_DX, PS_DY, PS_DXY, PS_DX2,
+               PS_DY2, PAIR_WORDS };
+struct PairCol {
+  uint64_t off;          // first word of the pair's sections
+  uint32_t qx, qy;       // the operands' columns in the scan's column table (work-list buckets: x's)
+  uint16_t x_id, y_id;
+  uint8_t x_pt, y_pt;
+  uint8_t pad[2];
+};
+
+__device__ __forceinline__ double pair_f64(uint64_t v, uint8_t pt) {  // the operand as f64, as DataFusion converts it
+  return pt == TSKV_PT_F64 ? __longlong_as_double((long long)v) : pt == TSKV_PT_I64 ? (double)(int64_t)v : (double)v;
+}
+__device__ __forceinline__ unsigned long long pair_ukey(double d) {  // unsigned order key of an f64 value
+  return (unsigned long long)okey((uint64_t)__double_as_longlong(d), TSKV_PT_F64) ^ 0x8000000000000000ull;
+}
+
+// The sums of one run of paired rows (one cell) of one lane, flushed with one atomic per quantity.
+struct PairAcc {
+  uint64_t n;
+  double a, b, c, d, e;                      // pass 1: sum x, sum y; pass 2: sum dx, sum dy, sum dx dy, sum dx^2, sum dy^2
+  unsigned long long xmin, xmax, ymin, ymax;  // pass 1: ~key / key of the extreme x and y
+  double shx, shy;                           // pass 2: the cell's shifts
+};
+template <bool PASS2>
+__device__ __forceinline__ void pair_start(const ScanParams &P, const PairCol &pc, uint64_t cell, PairAcc &r) {
+  r.n = 0; r.a = r.b = r.c = r.d = r.e = 0.0;
+  r.xmin = r.xmax = r.ymin = r.ymax = 0;
+  if (PASS2) {
+    r.shx = __longlong_as_double((long long)P.state[pc.off + PS_SHX * P.n_cells + cell]);
+    r.shy = __longlong_as_double((long long)P.state[pc.off + PS_SHY * P.n_cells + cell]);
+  }
+}
+template <bool PASS2>
+__device__ __forceinline__ void pair_add(PairAcc &r, double x, double y) {
+  r.n++;
+  if (PASS2) {
+    const double dx = x - r.shx, dy = y - r.shy;
+    r.a += dx; r.b += dy; r.c += dx * dy; r.d += dx * dx; r.e += dy * dy;
+  } else {
+    r.a += x; r.b += y;
+    const unsigned long long kx = pair_ukey(x), ky = pair_ukey(y);
+    r.xmin = max(r.xmin, ~kx); r.xmax = max(r.xmax, kx);
+    r.ymin = max(r.ymin, ~ky); r.ymax = max(r.ymax, ky);
+  }
+}
+template <bool PASS2>
+__device__ __forceinline__ void pair_flush(const ScanParams &P, const PairCol &pc, uint64_t cell, const PairAcc &r) {
+  if (!r.n) return;
+  uint64_t *s = P.state + pc.off + cell;
+  auto f = [&](int sec, double v) { atomicAdd(reinterpret_cast<double *>(s + sec * P.n_cells), v); };
+  auto m = [&](int sec, unsigned long long v) { atomicMax(reinterpret_cast<unsigned long long *>(s + sec * P.n_cells), v); };
+  if (PASS2) {
+    f(PS_DX, r.a); f(PS_DY, r.b); f(PS_DXY, r.c); f(PS_DX2, r.d); f(PS_DY2, r.e);
+  } else {
+    atomicAdd(reinterpret_cast<unsigned long long *>(s + PS_N * P.n_cells), (unsigned long long)r.n);
+    f(PS_SX, r.a); f(PS_SY, r.b);
+    m(PS_XMIN, r.xmin); m(PS_XMAX, r.xmax); m(PS_YMIN, r.ymin); m(PS_YMAX, r.ymax);
+  }
+}
+
+// One x page of a pair (work item `item` of x's buckets) and the y page of the same column group, decoded in lock-step
+// with the group's time page row by row; a row counts when scan_chunk_seg would select it (valid timestamp, keep bit,
+// time ranges, row-drop tombstones) and both x and y hold a value that no column tombstone masks. The y page is found
+// once per item in the group's descriptors. Decode errors of the three pages are pass 1's to report (every operand is a
+// column of the scan): the lane stops at the first.
+template <bool PASS2, bool EDGES>
+__device__ __forceinline__ void pair_page(const ScanParams &P, const PairCol &pc, uint64_t n_descs, uint32_t item) {
+  const uint32_t page = P.work_page[item], slot = P.work_slot[item];
+  const tskv_page_desc xd = P.descs[page];
+  const uint32_t tpage = P.time_page_of[page];
+  const tskv_page_desc td = P.descs[tpage];
+  uint32_t ypage = FULL;
+  for (uint64_t p = tpage + 1; p < n_descs && P.descs[p].phys_type != TSKV_PT_TIME; p++)
+    if (P.descs[p].column_id == pc.y_id) { ypage = (uint32_t)p; break; }
+  if (ypage == FULL) return;  // the group holds no y: NULL for every row (the reference null-fills it)
+  const tskv_page_desc yd = P.descs[ypage];
+  if (yd.phys_type != pc.y_pt || kind_status(xd.reserved) != TSKV_OK || kind_status(yd.reserved) != TSKV_OK ||
+      kind_status(td.reserved) != TSKV_OK || td.reserved == DK_ALLNULL || xd.reserved == DK_ALLNULL || yd.reserved == DK_ALLNULL)
+    return;
+  PageView tpv, xpv, ypv;
+  tpv.open(P.arena, td);
+  xpv.open(P.arena, xd);
+  ypv.open(P.arena, yd);
+  BitCursor tb, xb, yb;
+  tb.init(tpv.bitset);
+  xb.init(xpv.bitset);
+  yb.init(ypv.bitset);
+  DeltaCursor<-1> tc;
+  AnyCursor<> xc, yc;
+  if (tc.open(tpv, td.reserved) != TSKV_OK || xc.open(xpv, xd.reserved) != TSKV_OK || yc.open(ypv, yd.reserved) != TSKV_OK) return;
+  uint4 tx = make_uint4(0, 0, 0, 0), ty = tx;
+  if (P.has_tomb) {
+    tx = tomb_lookup(P, xd.series_id, pc.x_id);
+    ty = tomb_lookup(P, xd.series_id, pc.y_id);
+  }
+  const uint32_t *keepw = P.row_keep ? P.row_keep + P.keep_off[tpage] : nullptr;
+  const uint64_t group_base = group_cell_base<EDGES>(P, slot);
+  BucketState bk; bk.valid = false; bk.floor_regime = false; bk.lo = 0; bk.hi = 0; bk.idx = 0;
+  PairAcc acc;
+  uint64_t run_cell = 0;
+  bool have_run = false;
+  int64_t t = 0;
+  const uint32_t n_rows = xd.num_values;
+  for (uint32_t r = 0; r < n_rows; r++) {
+    const bool tv = tb.next(r), xv = xb.next(r), yv = yb.next(r);
+    uint64_t xr = 0, yr = 0;
+    if (tv) { t = (int64_t)tc.next(); if (tc.exhausted) break; }
+    else if (r == 0) tc.skip_first_if_s8b_sc();
+    if (xv) { xr = xc.next(); if (xc.failed()) break; }
+    else if (r == 0 && !xc.is_gorilla) xc.d.skip_first_if_s8b_sc();
+    if (yv) { yr = yc.next(); if (yc.failed()) break; }
+    else if (r == 0 && !yc.is_gorilla) yc.d.skip_first_if_s8b_sc();
+    if (!(tv && xv && yv)) continue;
+    if (keepw && !((__ldg(keepw + (r >> 5)) >> (r & 31)) & 1)) continue;
+    int64_t lo, hi;
+    if (!range_span(P, t, lo, hi)) continue;
+    if (P.has_tomb && (tomb_span(P.tomb_ranges, P.n_tomb_global, t, lo, hi) | tomb_span(P.tomb_ranges + tx.x, tx.y, t, lo, hi) |
+                       tomb_span(P.tomb_ranges + tx.z, tx.w, t, lo, hi) | tomb_span(P.tomb_ranges + ty.z, ty.w, t, lo, hi)))
+      continue;
+    if (!(bk.valid && t >= bk.lo && t <= bk.hi) && !locate_bucket<EDGES>(P, t, bk)) { bk.valid = false; continue; }  // (pass 1 reports it)
+    const uint64_t cell = group_base + bucket_cell<EDGES>(P, bk.idx);
+    if (!have_run || cell != run_cell) {
+      if (have_run) pair_flush<PASS2>(P, pc, run_cell, acc);
+      pair_start<PASS2>(P, pc, cell, acc);
+      run_cell = cell;
+      have_run = true;
+    }
+    pair_add<PASS2>(acc, pair_f64(xr, pc.x_pt), pair_f64(yr, pc.y_pt));
+  }
+  if (have_run) pair_flush<PASS2>(P, pc, run_cell, acc);
+}
+
+// Pass 1 / pass 2 of the column pairs (blockIdx.y: the pair): one lane per work item of the x operand's buckets (every
+// bin, wide and narrow), the same items pass 1 of the column scan read. Own kernels with their own arguments, so that the
+// fused kernels and ScanParams stay as they are.
+template <bool PASS2, bool EDGES>
+__global__ void __launch_bounds__(128) k_scan_pair(const __grid_constant__ ScanParams P, const PairCol *pairs, uint64_t n_descs) {
+  const PairCol pc = pairs[blockIdx.y];
+  const uint32_t stride = gridDim.x * blockDim.x, t0 = blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t k = pc.qx * WL_SUB; k < N_BINS * P.n_cols * WL_SUB; k += P.n_cols * WL_SUB)
+    for (uint32_t sub = 0; sub < WL_SUB; sub++) {
+      const uint32_t start = __ldg(P.region_start + k + sub), fill = __ldg(P.region_fill + k + sub);
+      for (uint32_t i = t0; i < fill; i += stride) pair_page<PASS2, EDGES>(P, pc, n_descs, start + i);
+    }
+}
+
+// Between the pair passes: the shifts sum x / n and sum y / n of every cell (0 for an empty cell).
+__global__ void k_pair_prep(uint64_t *state, const PairCol *pairs, uint64_t n_cells) {
+  const PairCol pc = pairs[blockIdx.y];
+  uint64_t *s = state + pc.off;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_cells; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t n = s[PS_N * n_cells + i];
+    const double sx = __longlong_as_double((long long)s[PS_SX * n_cells + i]), sy = __longlong_as_double((long long)s[PS_SY * n_cells + i]);
+    s[PS_SHX * n_cells + i] = (uint64_t)__double_as_longlong(n ? sx / (double)n : 0.0);
+    s[PS_SHY * n_cells + i] = (uint64_t)__double_as_longlong(n ? sy / (double)n : 0.0);
+  }
+}
+
+// Multi-GPU, after k_merge_gathered: every pair's cells from the gathered ranks' sections. Each rank's co-moments are
+// taken around its own shifts; its means relative to the shifts of the first rank holding the cell (as k_merge_m2) enter
+// Chan's formulas C = sum C_r + sum n_r (mx_r - mx)(my_r - my), M2 = sum M2_r + sum n_r (m_r - m)^2. Writes n, the extreme
+// keys, sum dx = sum dy = 0 and sum dx dy = C, sum dx^2 = M2x, sum dy^2 = M2y, which k_finalize_pairs reads unchanged.
+__global__ void k_merge_pairs(uint64_t *state, const PairCol *pairs, uint64_t n_cells, const uint64_t *gathered, uint32_t n_ranks,
+                              uint64_t exch_words) {
+  const PairCol pc = pairs[blockIdx.y];
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_cells; i += (uint64_t)gridDim.x * blockDim.x) {
+    auto at = [&](uint32_t r, int sec) { return gathered[r * exch_words + pc.off + sec * n_cells + i]; };
+    auto f64 = [&](uint32_t r, int sec) { return __longlong_as_double((long long)at(r, sec)); };
+    uint64_t n = 0;
+    unsigned long long km[4] = {0, 0, 0, 0};
+    double cx = 0.0, cy = 0.0, mx_sum = 0.0, my_sum = 0.0;
+    bool have_c = false;
+    for (uint32_t r = 0; r < n_ranks; r++) {
+      for (int q = 0; q < 4; q++) km[q] = max(km[q], (unsigned long long)at(r, PS_XMIN + q));
+      const uint64_t nr = at(r, PS_N);
+      if (!nr) continue;
+      if (!have_c) { cx = f64(r, PS_SHX); cy = f64(r, PS_SHY); have_c = true; }
+      n += nr;
+      mx_sum += (f64(r, PS_SHX) - cx) * (double)nr + f64(r, PS_DX);
+      my_sum += (f64(r, PS_SHY) - cy) * (double)nr + f64(r, PS_DY);
+    }
+    double c = 0.0, m2x = 0.0, m2y = 0.0;
+    if (n) {
+      const double mx = mx_sum / (double)n, my = my_sum / (double)n;
+      for (uint32_t r = 0; r < n_ranks; r++) {
+        const uint64_t nr = at(r, PS_N);
+        if (!nr) continue;
+        const double sdx = f64(r, PS_DX), sdy = f64(r, PS_DY), inv = 1.0 / (double)nr;
+        const double dmx = (f64(r, PS_SHX) - cx) + sdx * inv - mx, dmy = (f64(r, PS_SHY) - cy) + sdy * inv - my;
+        c += (f64(r, PS_DXY) - sdx * sdy * inv) + (double)nr * dmx * dmy;
+        m2x += (f64(r, PS_DX2) - sdx * sdx * inv) + (double)nr * dmx * dmx;
+        m2y += (f64(r, PS_DY2) - sdy * sdy * inv) + (double)nr * dmy * dmy;
+      }
+    }
+    uint64_t *s = state + pc.off + i;
+    s[PS_N * n_cells] = n;
+    for (int q = 0; q < 4; q++) s[(PS_XMIN + q) * n_cells] = km[q];
+    s[PS_DX * n_cells] = s[PS_DY * n_cells] = 0;
+    s[PS_DXY * n_cells] = (uint64_t)__double_as_longlong(c);
+    s[PS_DX2 * n_cells] = (uint64_t)__double_as_longlong(m2x);
+    s[PS_DY2 * n_cells] = (uint64_t)__double_as_longlong(m2y);
+  }
+}
+
+// M2 of one operand from its pass-2 sums: the corrected two-pass formula clamped at 0, and exactly 0 when every paired
+// value is the same finite number (the shift's rounding residue would otherwise make corr of a constant column noise).
+__device__ __forceinline__ double pair_m2(double sd, double sd2, uint64_t n, unsigned long long nkmin, unsigned long long kmax) {
+  if (~nkmin == kmax) {
+    const uint64_t bits = (uint64_t)okey_inv((int64_t)(kmax ^ 0x8000000000000000ull), TSKV_PT_F64);
+    if (isfinite(__longlong_as_double((long long)bits))) return 0.0;
+  }
+  const double m2 = sd2 - sd * sd / (double)n;
+  return m2 < 0.0 ? 0.0 : m2;
+}
+
+// The four outputs of every pair (blockIdx.y = 4 * pair + j; output column out0 + blockIdx.y): j = 0 n (always valid),
+// 1 C, 2 M2x, 3 M2y (valid iff n >= 1).
+__global__ void k_finalize_pairs(const uint64_t *state, const PairCol *pairs, uint32_t out0, uint64_t n_cells, uint64_t bitmap_stride,
+                                 uint64_t *values, uint8_t *validity) {
+  const PairCol pc = pairs[blockIdx.y >> 2];
+  const uint32_t j = blockIdx.y & 3;
+  const uint64_t cell = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  bool valid = false;
+  if (cell < n_cells) {
+    const uint64_t *s = state + pc.off + cell;
+    auto f64 = [&](int sec) { return __longlong_as_double((long long)s[sec * n_cells]); };
+    const uint64_t n = s[PS_N * n_cells];
+    double v = 0.0;
+    valid = j == 0 || n > 0;
+    if (j != 0 && n) {
+      if (j == 1) v = f64(PS_DXY) - f64(PS_DX) * f64(PS_DY) / (double)n;
+      else if (j == 2) v = pair_m2(f64(PS_DX), f64(PS_DX2), n, s[PS_XMIN * n_cells], s[PS_XMAX * n_cells]);
+      else v = pair_m2(f64(PS_DY), f64(PS_DY2), n, s[PS_YMIN * n_cells], s[PS_YMAX * n_cells]);
+    }
+    values[(uint64_t)(out0 + blockIdx.y) * n_cells + cell] = j == 0 ? n : (uint64_t)__double_as_longlong(v);
+  }
+  const uint32_t bits = __ballot_sync(FULL, valid);
+  if ((threadIdx.x & 31) == 0 && (cell >> 3) < bitmap_stride)
+    *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
+}
+
 // Per output column: which state arrays feed it.
 struct OutCol {
   uint64_t count_off;  // counts of the source column

@@ -253,6 +253,10 @@ struct tskv_scan {
   bool m2_bin[N_BINS] = {false};
   uint64_t m2_words = 0;
   event_ptr ev_m2_fork, ev_m2_join[N_BINS];
+  // column pairs (tskv_query.n_pairs; k_scan_pair): their state sections, which follow the M2 ones in the exchange region
+  uint32_t n_pairs = 0;
+  async_ptr<PairCol> d_pairs;
+  uint64_t pair_words = 0;
 };
 
 namespace {
@@ -337,6 +341,40 @@ bool query_has_m2(const tskv_query *q) {
   for (uint32_t c = 0; c < q->n_columns; c++)
     if (q->columns[c].agg_mask & TSKV_AGG_M2) return true;
   return false;
+}
+
+// The query the scan runs for a query with column pairs: its projected columns, then every pair operand that is not one
+// of them as a COUNT column without output (so that the work list, the page gathers, CRC checks, pass 1 and the reader
+// counters treat the operands' pages as they treat a COUNT column's), and per pair the operands' places in that table.
+struct PairQuery {
+  tskv_query q{};
+  std::vector<tskv_agg_column> cols;
+  std::vector<PairCol> pairs;  // (off is set by plan_state)
+};
+PairQuery plan_pair_query(const tskv_query *q) {
+  PairQuery pq;
+  pq.q = *q;
+  pq.cols.assign(q->columns, q->columns + q->n_columns);
+  auto place = [&](const tskv_agg_column &op) {
+    for (uint32_t c = 0; c < pq.cols.size(); c++)
+      if (pq.cols[c].column_id == op.column_id) return c;
+    pq.cols.push_back(tskv_agg_column{op.column_id, op.phys_type, (uint8_t)TSKV_AGG_COUNT});
+    return (uint32_t)pq.cols.size() - 1;
+  };
+  for (uint32_t p = 0; p < q->n_pairs; p++) {
+    const tskv_agg_column &x = q->columns[q->n_columns + 2 * p], &y = q->columns[q->n_columns + 2 * p + 1];
+    PairCol pc{};
+    pc.qx = place(x);
+    pc.qy = place(y);
+    pc.x_id = x.column_id;
+    pc.y_id = y.column_id;
+    pc.x_pt = x.phys_type;
+    pc.y_pt = y.phys_type;
+    pq.pairs.push_back(pc);
+  }
+  pq.q.columns = pq.cols.data();
+  pq.q.n_columns = (uint32_t)pq.cols.size();
+  return pq;
 }
 
 typedef void (*scan_kernel_t)(const ScanParams, int);
@@ -501,7 +539,7 @@ bool labels_first_last(const tskv_query *q, const BucketEdges &E) {
 
 // (an edge scan's buckets come from its edge table, width = 0)
 bool query_shape_ok(const tskv_query *q, bool edges = false) {
-  return q->n_buckets != 0 && q->n_columns != 0 && q->columns && (q->width > 0 || q->n_buckets == 1 || edges);
+  return q->n_buckets != 0 && (q->n_columns != 0 || q->n_pairs != 0) && q->columns && (q->width > 0 || q->n_buckets == 1 || edges);
 }
 
 // Output layout of a query that passed query_shape_ok and tag_groups_refusal.
@@ -509,6 +547,7 @@ tskv_output_layout output_layout(const tskv_pages *pages, const tskv_query *q, c
   tskv_output_layout out;
   uint64_t n_out = 0;
   for (uint32_t c = 0; c < q->n_columns; c++) n_out += popc8(q->columns[c].agg_mask);
+  if (q->n_pairs <= TSKV_MAX_PAIRS) n_out += 4ull * q->n_pairs;  // n, C, M2x, M2y per pair
   uint64_t n_groups = 1;
   if (q->group_by_series) n_groups = selected_slots(pages, q);
   if (tg.on) n_groups = tg.n;
@@ -541,6 +580,7 @@ struct StatePlan {
   std::vector<M2Col> m2;           // TSKV_AGG_M2 columns, in query order
   std::vector<int> m2_of;          // per column: its index in m2, or -1
   uint64_t m2_words = 0;           // their shift / sum(d) / sum(d^2) sections, which follow the values section
+  uint64_t pair_off = 0, pair_words = 0;  // the column pairs' sections (PAIR_WORDS per pair), after the M2 ones
 };
 StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
   StatePlan plan;
@@ -615,6 +655,9 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
       off += 3 * n_cells;
     }
   plan.m2_words = 3 * n_cells * plan.m2.size();
+  plan.pair_off = off;
+  plan.pair_words = (uint64_t)PAIR_WORDS * n_cells * q->n_pairs;
+  off += plan.pair_words;
   off = (off + 1) & ~1ull;  // 16-byte alignment of the pair arrays
   sl.first_pairs_off = off;
   {
@@ -769,6 +812,22 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
     ctx->set_error("invalid query: at most 126 columns and 8 time ranges");
     return TSKV_ERR_INVALID_ARG;
   }
+  if (q->n_pairs > TSKV_MAX_PAIRS || (uint64_t)q->n_columns + 2ull * q->n_pairs > 126) {
+    ctx->set_error("invalid query: at most 8 column pairs and 126 columns with the pairs' operands");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  for (uint32_t k = 0; k < 2 * q->n_pairs; k++) {
+    const tskv_agg_column &op = q->columns[q->n_columns + k];
+    if (op.agg_mask != 0 || op.phys_type < TSKV_PT_I64 || op.phys_type > TSKV_PT_F64) {
+      ctx->set_error("invalid pair operand: an I64 / U64 / F64 column with agg_mask 0");
+      return TSKV_ERR_INVALID_ARG;
+    }
+    for (uint32_t c = 0; c < q->n_columns + k; c++)
+      if (q->columns[c].column_id == op.column_id && q->columns[c].phys_type != op.phys_type) {
+        ctx->set_error("pair operand: one column id with two types");
+        return TSKV_ERR_INVALID_ARG;
+      }
+  }
   if (q->n_predicates > TSKV_MAX_PREDICATES || (q->n_predicates && !q->predicates)) {
     ctx->set_error("invalid query: at most 8 field predicates");
     return TSKV_ERR_INVALID_ARG;
@@ -814,6 +873,10 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
   }
   if (slide && query_has_m2(q)) {
     ctx->set_error("sliding windows: M2 (variance) is not pushed down: folding panes would need a Chan merge of their second moments");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  if (slide && q->n_pairs) {
+    ctx->set_error("sliding windows: column pairs (covariance / correlation) are not pushed down");
     return TSKV_ERR_UNSUPPORTED;
   }
   *win_k = 1;
@@ -876,10 +939,14 @@ struct ScanLayout {
   std::vector<ColState> cols2;
   uint32_t use_smem2 = 0, smem_words2 = 0;
   uint64_t m2_words = 0;
+  std::vector<PairCol> pairs;  // column pairs, with their state offsets
+  uint64_t pair_words = 0;
 };
 
 // n_cells: cells of the query's grid (a sliding scan: windows); kern_cells: cells of the fused kernels' grid (panes).
-ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint64_t kern_cells) {
+// n_user: the columns with outputs (the rest are pair operands read as COUNT columns); pairs: plan_pair_query's.
+ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint64_t kern_cells, uint32_t n_user,
+                       const std::vector<PairCol> &pairs) {
   ScanLayout out;
   const StatePlan win = plan_state(q, n_cells);
   const StatePlan pane = sliding ? plan_state(q, kern_cells) : StatePlan{};
@@ -889,6 +956,9 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
   out.means = win.means;
   out.m2 = win.m2;  // (sliding scans refuse M2)
   out.m2_words = win.m2_words;
+  out.pairs = pairs;  // (sliding scans refuse pairs)
+  for (size_t p = 0; p < out.pairs.size(); p++) out.pairs[p].off = win.pair_off + (uint64_t)PAIR_WORDS * n_cells * p;
+  out.pair_words = win.pair_words;
   if (sliding) {
     for (uint32_t c = 0; c < q->n_columns; c++) {
       const ColState &p = pane.cols[c], &w = win.cols[c];
@@ -905,7 +975,7 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
 
   // output column table
   uint64_t fk = out.sl.first_keys_off, lk = out.sl.last_keys_off, fv = out.sl.selval_off, lv = out.sl.selval_off + out.sl.first_cells;
-  for (uint32_t c = 0; c < q->n_columns; c++) {
+  for (uint32_t c = 0; c < n_user; c++) {
     const tskv_agg_column &qc = q->columns[c];
     for (unsigned bit = 0; bit < 8; bit++) {
       unsigned agg = 1u << bit;
@@ -1201,6 +1271,10 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
       for (int b = 0; b < N_BINS; b++) s->m2_bin[b] |= (it->second[b * WL_SUB] + it->second[b * WL_SUB + 1]) != 0;
     }
   }
+  s->n_pairs = (uint32_t)lay.pairs.size();
+  s->pair_words = lay.pair_words;
+  if (e == cudaSuccess && s->n_pairs) e = upload(s->d_pairs, lay.pairs.data(), lay.pairs.size(), st);
+  *h2d += lay.pairs.size() * sizeof(PairCol);
   if (e == cudaSuccess) e = stream_alloc(s->d_aux, AUX_WORDS, st);
   if (e == cudaSuccess) e = stream_alloc(s->d_values, s->layout.n_out * s->layout.n_cells, st);
   if (e == cudaSuccess) e = stream_alloc(s->d_validity, s->layout.validity_bytes + 8, st);
@@ -1964,6 +2038,11 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   tskv_status st = validate_query(ctx, pages, q, slide, tg, E, &win_k);
   if (st != TSKV_OK) return st;
   const tskv_output_layout L = output_layout(pages, q, tg);
+  // column pairs: from here on the scan runs the query with the operands as columns (plan_pair_query)
+  const uint32_t n_user = q->n_columns;
+  PairQuery pq = plan_pair_query(q);
+  pq.q.columns = pq.cols.data();
+  q = &pq.q;
   cudaSetDevice(ctx->device);
   bool has_sel = false;  // any FIRST / LAST
   for (uint32_t c = 0; c < q->n_columns; c++) has_sel |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
@@ -1983,7 +2062,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   s->win_k = win_k;
   s->n_windows = q->n_buckets;
   s->n_panes = q->n_buckets - win_k + 1;
-  const ScanLayout lay = plan_layout(q, slide != 0, L.n_cells, L.n_groups * s->n_panes);
+  const ScanLayout lay = plan_layout(q, slide != 0, L.n_cells, L.n_groups * s->n_panes, n_user, pq.pairs);
+  s->n_out = (uint32_t)lay.outs.size();  // (the pairs' outputs follow, k_finalize_pairs)
   s->sl = lay.sl;
   s->kern_sl = lay.kern_sl;
   uint64_t h2d = 0;
@@ -2252,7 +2332,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     cudaStreamWaitEvent(ctx->stream.get(), ev_done, 0);  // join
     launches++;
   }
-  if (!capturing && !s->n_m2) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
+  if (!capturing && !s->n_m2 && !s->n_pairs) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
   if (s->n_combine) {  // sliding windows: every window folds its panes (it writes every array the kernels fill)
     const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
     k_window_combine<<<dim3(std::max(1u, bx), s->n_combine), 256, 0, ctx->stream.get()>>>(
@@ -2290,7 +2370,33 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       cudaStreamWaitEvent(ctx->stream.get(), s->ev_m2_join[b].get(), 0);
       launches++;
     }
-    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes pass 2)
+    if (!capturing && !s->n_pairs) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes pass 2)
+  }
+  if (s->n_pairs) {  // column pairs: pass 1 (n, sums, extremes), the shifts, pass 2 (co-moments); overlap merge rows first
+    const bool edges = s->params.edges != nullptr;
+    const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
+    const uint32_t px = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)pages->n_descs + 127) / 128, (uint64_t)ctx->sm_count * 16));
+    const bool merge = s->merge.n_rows && s->n_merge_pages;
+    for (int pass = 0; pass < 2; pass++) {
+      if (pass == 1) {
+        k_pair_prep<<<dim3(std::max(1u, bx), s->n_pairs), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_pairs.get(), s->layout.n_cells);
+        launches++;
+      }
+      if (merge) {
+        const uint32_t mb = (uint32_t)((s->merge.n_rows + 127) / 128);
+        if (pass) k_merge_pairs_rows<true><<<mb, 128, 0, ctx->stream.get()>>>(s->params, s->merge, s->d_pairs.get(), s->n_pairs);
+        else k_merge_pairs_rows<false><<<mb, 128, 0, ctx->stream.get()>>>(s->params, s->merge, s->d_pairs.get(), s->n_pairs);
+        launches++;
+      }
+      const void *fn = pass ? (edges ? (const void *)k_scan_pair<true, true> : (const void *)k_scan_pair<true, false>)
+                            : (edges ? (const void *)k_scan_pair<false, true> : (const void *)k_scan_pair<false, false>);
+      const PairCol *pp = s->d_pairs.get();
+      uint64_t nd = pages->n_descs;
+      void *args[] = {(void *)&s->params, (void *)&pp, (void *)&nd};
+      CU_TRY(ctx, cudaLaunchKernel(fn, dim3(px, s->n_pairs), dim3(128), args, 0, ctx->stream.get()));
+      launches++;
+    }
+    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the pair passes)
   }
   if (!capturing) cudaEventRecord(s->ev1.get(), ctx->stream.get());
   CU_TRY(ctx, cudaGetLastError());
@@ -2429,9 +2535,9 @@ tskv_status tskvgpu_scan_work_list(tskv_ctx *ctx, tskv_scan *s, uint32_t *n_buck
 
 tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_view *out) {
   if (!ctx || !s || !out) return TSKV_ERR_INVALID_ARG;
-  if (s->n_m2) {
+  if (s->n_m2 || s->n_pairs) {
     std::lock_guard<std::mutex> lock(ctx->mu);
-    ctx->set_error("scan_partials: second moments (TSKV_AGG_M2) do not all-reduce element-wise; use tskvgpu_scan_exchange");
+    ctx->set_error("scan_partials: second moments (TSKV_AGG_M2, column pairs) do not all-reduce element-wise; use tskvgpu_scan_exchange");
     return TSKV_ERR_UNSUPPORTED;
   }
   const StateLayout &L = s->sl;
@@ -2452,17 +2558,21 @@ tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_vie
 }
 
 // The M2 columns of gathered partials: Chan's merge of every rank's (count, sum, M2) (k_merge_m2).
+// (and the column pairs: Chan's merge of every rank's n, means and co-moments, k_merge_pairs)
 static void merge_m2(tskv_ctx *ctx, tskv_scan *s, const uint64_t *gathered, uint32_t n_ranks, uint64_t words) {
-  if (!s->n_m2) return;
   const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
-  k_merge_m2<<<dim3(std::max(1u, bx), s->n_m2), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_m2.get(), s->layout.n_cells, gathered,
-                                                                         n_ranks, words);
+  if (s->n_m2)
+    k_merge_m2<<<dim3(std::max(1u, bx), s->n_m2), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_m2.get(), s->layout.n_cells, gathered,
+                                                                           n_ranks, words);
+  if (s->n_pairs)
+    k_merge_pairs<<<dim3(std::max(1u, bx), s->n_pairs), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_pairs.get(), s->layout.n_cells,
+                                                                                 gathered, n_ranks, words);
 }
 
 tskv_status tskvgpu_scan_exchange_view(tskv_ctx *ctx, tskv_scan *s, uint64_t *out_dptr, uint64_t *out_words) {
   if (!ctx || !s || !out_dptr || !out_words) return TSKV_ERR_INVALID_ARG;
   *out_dptr = (uint64_t)(uintptr_t)s->d_state.get();
-  *out_words = s->sl.selval_off + s->sl.selval_len + s->m2_words;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values | M2
+  *out_words = s->sl.selval_off + s->sl.selval_len + s->m2_words + s->pair_words;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values | M2 | pairs
   return TSKV_OK;
 }
 
@@ -2470,7 +2580,7 @@ tskv_status tskvgpu_scan_merge_gathered(tskv_ctx *ctx, tskv_scan *s, uint64_t ga
   if (!ctx || !s || !gathered_dptr || n_ranks == 0) return TSKV_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(ctx->mu);
   cudaSetDevice(ctx->device);
-  const uint64_t words = s->sl.selval_off + s->sl.selval_len + s->m2_words;
+  const uint64_t words = s->sl.selval_off + s->sl.selval_len + s->m2_words + s->pair_words;
   uint32_t blocks = (uint32_t)std::min<uint64_t>((words + 255) / 256, 2048);
   k_merge_gathered<<<std::max(1u, blocks), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->sl, reinterpret_cast<const uint64_t *>((uintptr_t)gathered_dptr),
                                                                    n_ranks, words);
@@ -2488,7 +2598,7 @@ tskv_status tskvgpu_scan_exchange(tskv_ctx *ctx, tskv_scan *s) {
     return TSKV_ERR_NCCL;
   }
   const NcclApi &N = nccl_api();
-  const uint64_t words = s->sl.selval_off + s->sl.selval_len + s->m2_words;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values | M2
+  const uint64_t words = s->sl.selval_off + s->sl.selval_len + s->m2_words + s->pair_words;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values | M2
   if (!s->d_gathered) CU_TRY(ctx, stream_alloc(s->d_gathered, (size_t)ctx->n_ranks * words, ctx->stream.get()));
   const ncclResult_t r = N.AllGather(s->d_state.get(), s->d_gathered.get(), words, ncclUint64, ctx->comm, ctx->stream.get());
   if (r != ncclSuccess) {
@@ -2526,9 +2636,14 @@ tskv_status tskvgpu_scan_mask_values(tskv_ctx *ctx, tskv_scan *s) {
 
 static tskv_status finalize_device(tskv_ctx *ctx, tskv_scan *s) {
   const tskv_output_layout &L = s->layout;
-  dim3 grid((uint32_t)((L.n_cells + 255) / 256), s->n_out);
-  k_finalize<<<grid, 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_outs.get(), s->n_out, L.n_cells, L.bitmap_stride, s->d_values.get(),
-                                            s->d_validity.get());
+  if (s->n_out) {
+    dim3 grid((uint32_t)((L.n_cells + 255) / 256), s->n_out);
+    k_finalize<<<grid, 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_outs.get(), s->n_out, L.n_cells, L.bitmap_stride, s->d_values.get(),
+                                              s->d_validity.get());
+  }
+  if (s->n_pairs)
+    k_finalize_pairs<<<dim3((uint32_t)((L.n_cells + 255) / 256), 4 * s->n_pairs), 256, 0, ctx->stream.get()>>>(
+        s->d_state.get(), s->d_pairs.get(), s->n_out, L.n_cells, L.bitmap_stride, s->d_values.get(), s->d_validity.get());
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;
 }

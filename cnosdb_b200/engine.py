@@ -39,6 +39,30 @@ def stat_from_m2(name, count, m2, valid):
     return v, ok
 
 
+# DataFusion's covariance / correlation, computed on the host from a column pair's n and co-moments (QueryOption.pairs).
+PAIR_AGGS = ("covar", "covar_samp", "covar_pop", "corr")
+PAIR_RAW = ("n", "c", "m2x", "m2y")
+
+
+def pair_stat(name, n, c, m2x, m2y, valid):
+    """DataFusion's final formula of a PAIR_AGGS aggregate from a pair's cells (numpy arrays): covar = covar_samp =
+    C / (n - 1), covar_pop = C / n, corr = (C / n) / sqrt(M2x / n) / sqrt(M2y / n) in that order, 0.0 when either root is
+    0. Returns (values f64, validity): NULL where n == 0, and for the sample form where n == 1."""
+    n = np.asarray(n, dtype=np.uint64).astype(np.float64)
+    ok = np.asarray(valid, dtype=bool) & (n > (1 if name in ("covar", "covar_samp") else 0))
+    c, m2x, m2y = (np.asarray(a, dtype=np.float64) for a in (c, m2x, m2y))
+    d = np.where(ok, n, 1.0)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        if name in ("covar", "covar_samp"):
+            v = c / np.where(ok, n - 1.0, 1.0)
+        elif name == "covar_pop":
+            v = c / d
+        else:
+            s1, s2 = np.sqrt(m2x / d), np.sqrt(m2y / d)
+            v = np.where((s1 == 0.0) | (s2 == 0.0), 0.0, (c / d) / s1 / s2)
+    return np.where(ok, v, 0.0), ok
+
+
 def _wrap64(x):
     x &= (1 << 64) - 1
     return x - (1 << 64) if x >> 63 else x
@@ -216,8 +240,10 @@ class QueryOption:
     """The pushed-down scan: series selection, closed time ranges, bucket expression, aggregates."""
 
     def __init__(self, columns, series_ids=None, time_ranges=(), origin=0, width=0,
-                 first_bucket_start=0, n_buckets=1, group_by_series=False, multi_rank=False, predicates=()):
+                 first_bucket_start=0, n_buckets=1, group_by_series=False, multi_rank=False, predicates=(), pairs=()):
         self.columns = list(columns)
+        # column pairs (covar* / corr): (x_id, x_phys_type, y_id, y_phys_type); ScanResult.pair reads them
+        self.pairs = [(int(a), int(b), int(c), int(d)) for a, b, c, d in pairs]
         self.series_ids = None if series_ids is None else np.ascontiguousarray(series_ids, dtype=np.uint32)
         self.time_ranges = [(int(a), int(b)) for a, b in time_ranges]
         self.origin = int(origin)
@@ -244,11 +270,15 @@ class QueryOption:
         q.first_bucket_start, q.n_buckets = self.first_bucket_start, self.n_buckets
         q.group_by_series = 1 if self.group_by_series else 0
         q.reserved = cabi.TSKV_QUERY_MULTI_RANK if self.multi_rank else 0
-        cols = (cabi.AggColumn * len(self.columns))()
+        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))]
+        cols = (cabi.AggColumn * max(1, len(self.columns) + len(ops)))()
         for i, c in enumerate(self.columns):
             cols[i].column_id, cols[i].phys_type, cols[i].agg_mask = c.column_id, c.phys_type, c.agg_mask
+        for i, (cid, pt) in enumerate(ops):  # the pairs' operands follow the projected columns, agg_mask 0
+            cols[len(self.columns) + i].column_id, cols[len(self.columns) + i].phys_type = cid, pt
         q.columns = cols
         q.n_columns = len(self.columns)
+        q.n_pairs = len(self.pairs)
         preds = (cabi.FieldPredicate * max(1, len(self.predicates)))()
         for i, (c, pt, op, v) in enumerate(self.predicates):
             preds[i].column_id, preds[i].phys_type, preds[i].op = c, pt, op
@@ -263,7 +293,8 @@ class QueryOption:
         return q
 
     def output_names(self):
-        return [(c.column_id, cabi.AGG_NAMES[a]) for c in self.columns for a in c.agg_list()]
+        return ([(c.column_id, cabi.AGG_NAMES[a]) for c in self.columns for a in c.agg_list()] +
+                [(("pair", k), r) for k in range(len(self.pairs)) for r in PAIR_RAW])
 
 
 class ScanResult:
@@ -278,6 +309,20 @@ class ScanResult:
                              bitorder="little")
         self.validity = bits[:, : int(layout.n_cells)].astype(bool)
         self.phys = {(c.column_id): c.phys_type for c in query.columns}
+
+    def pair(self, k, name):
+        """(values f64 / u64 for n, validity) of column pair k, shaped [n_groups, n_buckets]: one of PAIR_AGGS (covar,
+        covar_samp, covar_pop, corr), derived on the host by pair_stat, or the raw n / c / m2x / m2y."""
+        def raw(r):
+            j = self.names.index((("pair", k), r))
+            v = self.values[j].view(np.uint64 if r == "n" else np.float64)
+            shape = (self.n_groups, self.n_buckets)
+            return v.reshape(shape), self.validity[j].reshape(shape)
+        if name in PAIR_RAW:
+            return raw(name)
+        n, _ = raw("n")
+        (c, ok), (m2x, _), (m2y, _) = raw("c"), raw("m2x"), raw("m2y")
+        return pair_stat(name, n, c, m2x, m2y, ok)
 
     def column(self, column_id, agg):
         """(typed values, validity) of one output column, shaped [n_groups, n_buckets]. agg may also name one of STAT_AGGS
@@ -536,6 +581,8 @@ class Engine:
     def _no_m2_with_slide(query, slide):
         if slide is not None and any(c.agg_mask & TSKV_AGG_M2 for c in query.columns):
             raise ValueError("m2 / var* / stddev* and slide: sliding windows do not push the variance state down")
+        if slide is not None and getattr(query, "pairs", None):
+            raise ValueError("pairs (covar* / corr) and slide: sliding windows do not push the covariance state down")
 
     @staticmethod
     def _edges(edges, slide):

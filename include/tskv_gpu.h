@@ -170,8 +170,29 @@ typedef struct tskv_query {
   uint32_t reserved;          /* TSKV_QUERY_* flags (0 for a plain single-device scan) */
   const tskv_field_predicate *predicates; /* AND-ed field comparisons, or NULL */
   uint32_t n_predicates;      /* 0..TSKV_MAX_PREDICATES */
-  uint32_t reserved2;
+  uint32_t n_pairs;           /* 0..TSKV_MAX_PAIRS column pairs (covariance / correlation state, below); 0: none */
 } tskv_query;
+/* Column pairs: covar / covar_samp / covar_pop / corr (DataFusion's Covariance / Correlation). The 2 * n_pairs entries of
+ * `columns` after the n_columns projected ones are the pairs' operands x0, y0, x1, y1, ...: column_id and phys_type
+ * (I64 / U64 / F64) of each, agg_mask 0. n_columns may be 0 when n_pairs >= 1; n_columns + 2 * n_pairs <= 126; x may equal
+ * y. Both operands convert to f64. A row counts for a pair when it is selected (time ranges, series, the row filter of
+ * the predicates, row-drop tombstones) and both x and y are valid (non-NULL after column tombstones); a column group
+ * without a page of x or of y has no paired row. Per cell each pair adds four outputs after every column output, in pair
+ * order: n (u64, the paired rows, valid like COUNT), then f64 C = sum (x - mx)(y - my), M2x = sum (x - mx)^2 and
+ * M2y = sum (y - my)^2 over the paired rows (mx, my: their paired means), valid iff n >= 1. M2x is exactly 0.0 when the
+ * paired x values are all equal and finite (M2y alike); NaN or +-inf among them gives NaN. The host derives
+ * covar = covar_samp = C / (n - 1), covar_pop = C / n, corr = (C / n) / sqrt(M2x / n) / sqrt(M2y / n) (0.0 when either
+ * root is 0). Computed in two passes over the rows of x's pages paired with the same column group's y page: pass 1 sums
+ * n, x and y per cell, pass 2 sums dx = x - sum x / n, dy, dx dy, dx^2 and dy^2; C = sum dx dy - sum dx sum dy / n,
+ * M2 = sum d^2 - (sum d)^2 / n (corrected two-pass algorithm). An operand that is not a projected column is read like a
+ * COUNT column that has no output. Refused before any launch: TSKV_ERR_INVALID_ARG for n_pairs > TSKV_MAX_PAIRS, an
+ * operand with a non-zero agg_mask or a BOOL / TIME / unknown type, an operand id projected with another type, or more
+ * than 126 columns; TSKV_ERR_UNSUPPORTED for sliding windows (slide != width). tskvgpu_scan_partials refuses a scan with
+ * pairs (use tskvgpu_scan_exchange / _merge_gathered, which merge the ranks' co-moments with Chan's formula). Pages of
+ * another type under an operand's id are an error. Counters: page_read_count, page_read_bytes, points_decoded,
+ * rows_in_range and pruned_page_count equal those of the same query with every operand that is not projected added as a
+ * COUNT column; kernel_launches and elapsed_fused_ms include the pair passes. */
+#define TSKV_MAX_PAIRS 8
 /* The partial state of this scan will be merged with other ranks' (tskvgpu_scan_partials / _exchange_view): every
  * exchanged key is then derived from the query alone, never from this rank's own arena (its time bounds, its local
  * series ranks), so that all ranks build comparable first/last tie-break keys. Requires series_ids != NULL when the

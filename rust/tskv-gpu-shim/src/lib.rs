@@ -273,7 +273,7 @@ impl Query {
             reserved: if self.multi_rank { sys::TSKV_QUERY_MULTI_RANK } else { 0 },
             predicates: if self.predicates.is_empty() { std::ptr::null() } else { self.predicates.as_ptr() },
             n_predicates: self.predicates.len() as u32,
-            reserved2: 0,
+            n_pairs: 0,
         }
     }
 }

@@ -32,6 +32,8 @@ pub const TSKV_AGG_FIRST: u8 = 1 << 5;
 pub const TSKV_AGG_LAST: u8 = 1 << 6;
 /// f64 sum of squared deviations from the cell mean (the variance state; two passes, see tskv_gpu.h).
 pub const TSKV_AGG_M2: u8 = 1 << 7;
+/// At most this many column pairs (tskv_query.n_pairs; covariance / correlation, see tskv_gpu.h).
+pub const TSKV_MAX_PAIRS: u32 = 8;
 
 pub const TSKV_UPLOAD_VERIFY_CRC: u32 = 1;
 pub const TSKV_UPLOAD_HOST_RESIDENT: u32 = 2;
@@ -137,7 +139,8 @@ pub struct tskv_query {
     pub reserved: u32,
     pub predicates: *const tskv_field_predicate,
     pub n_predicates: u32,
-    pub reserved2: u32,
+    /// column pairs (covariance / correlation), operands after the projected columns; 0: none
+    pub n_pairs: u32,
 }
 
 #[repr(C)]
