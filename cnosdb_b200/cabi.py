@@ -37,6 +37,21 @@ TSKV_AGG_M2 = 0x80
 AGG_NAMES = {1: "count", 2: "sum", 4: "min", 8: "max", 16: "mean", 32: "first", 64: "last", 128: "m2"}
 # column pairs of tskv_query.n_pairs (covariance / correlation state; engine.py derives covar* / corr from it)
 TSKV_MAX_PAIRS = 8
+# medians: n_medians in bits 8..15 of tskv_query.reserved, operands after the pairs' (see include/tskv_gpu.h)
+TSKV_MAX_MEDIANS = 8
+TSKV_MAX_MEDIAN_CELLS = 1 << 22
+
+
+def query_medians(n):
+    """TSKV_QUERY_MEDIANS(n): the flags-word bits of n medians."""
+    return (int(n) & 0xFF) << 8
+
+
+def query_n_medians(flags):
+    """TSKV_QUERY_N_MEDIANS(flags)."""
+    return (int(flags) >> 8) & 0xFF
+
+
 TSKV_UPLOAD_VERIFY_CRC = 1
 TSKV_UPLOAD_HOST_RESIDENT = 2
 TSKV_UPLOAD_VERIFY_ON_READ = 4

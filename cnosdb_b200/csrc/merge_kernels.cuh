@@ -86,8 +86,8 @@ __device__ __forceinline__ bool merge_row_kept_in_stream(const ScanParams &P, co
   return merge_row_kept(P, M, i, k);
 }
 
-// (k_merge_pairs_rows below restates this kernel's leader test, row-level filters and take_last_and_merge rule for the
-// column pairs, in merge_value: a change to either rule must be made in both.)
+// (merged_row and merge_value below restate this kernel's leader test, row-level filters and take_last_and_merge rule
+// for the column pairs and the medians: a change to either rule must be made in both.)
 // M2: pass 2 of TSKV_AGG_M2 over the merged rows, with the pass-2 column table (k_scan_m2): the same merged rows and cells,
 // each M2 column's value adds d = (double)x - (its cell's shift) and d^2 to sum(d) / sum(d^2); other columns are skipped.
 template <bool M2>
@@ -219,8 +219,8 @@ __global__ void __launch_bounds__(128) k_merge_chunks(const ScanParams P, const 
 // The column pairs over the merged rows (pass 1 / pass 2 of k_scan_pair): one thread per merge row; the leader of a merged
 // row that survives the row-level filters takes, for each pair, the merged x and y values as k_merge_chunks takes them
 // for its columns (column tombstones, then the newest surviving non-null value with this timestamp) and adds the pair
-// when both exist. The leader test, the row-level filters and the take_last_and_merge rule (merge_value) restate
-// k_merge_chunks' so that the existing kernel's code stays as it is: a change to either must be made in both.
+// when both exist. The leader test, the row-level filters (merged_row) and the take_last_and_merge rule (merge_value)
+// restate k_merge_chunks' so that the existing kernel's code stays as it is: a change to either must be made in both.
 __device__ __forceinline__ bool merge_value(const ScanParams &P, const MergeParams &M, uint32_t c, uint32_t series, int64_t t,
                                             uint32_t s0, uint32_t s1, uint64_t &v) {
   if (P.has_tomb) {
@@ -247,45 +247,83 @@ __device__ __forceinline__ bool merge_value(const ScanParams &P, const MergePara
   return false;
 }
 
-template <bool PASS2>
-__global__ void __launch_bounds__(128) k_merge_pairs_rows(const ScanParams P, const MergeParams M, const PairCol *pairs, uint32_t n_pairs) {
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= M.n_rows) return;
+// A merged row of the column pairs and the medians: the leader of its timestamp and group, as k_merge_chunks leads one
+// (merge row i is kept and no earlier kept row of its stream, and no kept row of an older stream, has its timestamp),
+// past the row-level filters (time ranges, row-drop tombstones, its bucket). Sets the row's cell, timestamp and series
+// and its group's streams [s0, s1) (merge_value's arguments).
+struct MergedRow {
+  uint64_t cell;
+  int64_t t;
+  uint32_t series, s0, s1;
+};
+__device__ __forceinline__ bool merged_row(const ScanParams &P, const MergeParams &M, uint64_t i, MergedRow &mr) {
   const uint32_t k = merge_mcg_of(M, i);
-  if (!merge_row_kept(P, M, i, k)) return;
+  if (!merge_row_kept(P, M, i, k)) return false;
   const uint32_t s = M.mcg_stream[k], g = M.stream_group[s];
   const uint32_t cg = M.mcg_cg[k];
   const int32_t slot_i = M.cg_slot[cg];
-  if (slot_i < 0) return;
+  if (slot_i < 0) return false;
   const int64_t t = M.ts[i];
   const uint32_t s0 = M.group_first_stream[g], s1 = M.group_first_stream[g + 1];
   const uint32_t series = P.descs[M.cg_time_page[cg]].series_id;
   const uint64_t own0 = M.mcg_row0[M.stream_first_mcg[s]];
   for (uint64_t j = merge_lower_bound(M.ts, own0, i, t); j < i; j++)
-    if (merge_row_kept_in_stream(P, M, j, s)) return;
+    if (merge_row_kept_in_stream(P, M, j, s)) return false;
   for (uint32_t s2 = s0; s2 < s; s2++) {
     const uint64_t a = M.mcg_row0[M.stream_first_mcg[s2]], b = M.mcg_row0[M.stream_first_mcg[s2 + 1]];
     for (uint64_t j = merge_lower_bound(M.ts, a, b, t); j < b && M.ts[j] == t; j++)
-      if (merge_row_kept_in_stream(P, M, j, s2)) return;
+      if (merge_row_kept_in_stream(P, M, j, s2)) return false;
   }
   int64_t lo, hi;
-  if (!range_span(P, t, lo, hi)) return;
+  if (!range_span(P, t, lo, hi)) return false;
   if (P.has_tomb) {
     const uint4 tl = tomb_lookup(P, series, TSKV_TOMB_ALL);
-    if (tomb_span(P.tomb_ranges, P.n_tomb_global, t, lo, hi) | tomb_span(P.tomb_ranges + tl.x, tl.y, t, lo, hi)) return;
+    if (tomb_span(P.tomb_ranges, P.n_tomb_global, t, lo, hi) | tomb_span(P.tomb_ranges + tl.x, tl.y, t, lo, hi)) return false;
   }
   BucketState bk;
   bk.valid = false; bk.floor_regime = false; bk.lo = 0; bk.hi = 0; bk.idx = 0;
-  if (!(P.edges ? locate_bucket<true>(P, t, bk) : locate_bucket<false>(P, t, bk))) return;  // (k_merge_chunks reports it)
-  const uint64_t cell = group_cell_base<true>(P, (uint32_t)slot_i) + bucket_cell<true>(P, bk.idx);
+  if (!(P.edges ? locate_bucket<true>(P, t, bk) : locate_bucket<false>(P, t, bk))) return false;  // (k_merge_chunks reports it)
+  mr.cell = group_cell_base<true>(P, (uint32_t)slot_i) + bucket_cell<true>(P, bk.idx);
+  mr.t = t;
+  mr.series = series;
+  mr.s0 = s0;
+  mr.s1 = s1;
+  return true;
+}
+
+template <bool PASS2>
+__global__ void __launch_bounds__(128) k_merge_pairs_rows(const ScanParams P, const MergeParams M, const PairCol *pairs, uint32_t n_pairs) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  MergedRow mr;
+  if (i >= M.n_rows || !merged_row(P, M, i, mr)) return;
   for (uint32_t p = 0; p < n_pairs; p++) {
     const PairCol pc = pairs[p];
     uint64_t xv, yv;
-    if (!merge_value(P, M, pc.qx, series, t, s0, s1, xv) || !merge_value(P, M, pc.qy, series, t, s0, s1, yv)) continue;
+    if (!merge_value(P, M, pc.qx, mr.series, mr.t, mr.s0, mr.s1, xv) || !merge_value(P, M, pc.qy, mr.series, mr.t, mr.s0, mr.s1, yv))
+      continue;
     PairAcc acc;
-    pair_start<PASS2>(P, pc, cell, acc);
+    pair_start<PASS2>(P, pc, mr.cell, acc);
     pair_add<PASS2>(acc, pair_f64(xv, pc.x_pt), pair_f64(yv, pc.y_pt));
-    pair_flush<PASS2>(P, pc, cell, acc);
+    pair_flush<PASS2>(P, pc, mr.cell, acc);
+  }
+}
+
+// One selection pass of the medians over the merged rows (k_scan_median's pass): one thread per merge row; the leader of
+// a merged row adds, for each median, the operand's merged value (merge_value) to its cell.
+__global__ void __launch_bounds__(128) k_merge_median_rows(const ScanParams P, const MergeParams M, const MedianCol *meds, uint32_t n_meds,
+                                                           const MedianArgs A) {
+  if (*(volatile unsigned long long *)A.unresolved == 0) return;
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  MergedRow mr;
+  if (i >= M.n_rows || !merged_row(P, M, i, mr)) return;
+  for (uint32_t m = 0; m < n_meds; m++) {
+    const MedianCol mc = meds[m];
+    uint64_t v;
+    if (!merge_value(P, M, mc.qcol, mr.series, mr.t, mr.s0, mr.s1, v)) continue;
+    MedianRun run;
+    median_open(mc, A, P.n_cells, mr.cell, run);
+    median_add(mc, A, P.n_cells, run, median_ukey(v, mc.phys_type));
+    median_flush(mc, A, P.n_cells, run);
   }
 }
 

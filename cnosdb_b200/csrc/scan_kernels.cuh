@@ -2284,6 +2284,23 @@ __device__ __forceinline__ void pair_flush(const ScanParams &P, const PairCol &p
   }
 }
 
+// The row selection of the column pairs and the medians, as scan_chunk_seg selects: the keep bit of row r, the time
+// ranges, the row-drop tombstones (global, and the series' in ta.x / ta.y) and the operands' column tombstones (ta.z /
+// ta.w, tb.z / tb.w), then the bucket of timestamp t (bk caches the last one). Sets the row's cell when it is selected.
+template <bool EDGES>
+__device__ __forceinline__ bool select_row(const ScanParams &P, const uint32_t *keepw, uint32_t r, int64_t t, const uint4 &ta,
+                                           const uint4 &tb, uint64_t group_base, BucketState &bk, uint64_t &cell) {
+  if (keepw && !((__ldg(keepw + (r >> 5)) >> (r & 31)) & 1)) return false;
+  int64_t lo, hi;
+  if (!range_span(P, t, lo, hi)) return false;
+  if (P.has_tomb && (tomb_span(P.tomb_ranges, P.n_tomb_global, t, lo, hi) | tomb_span(P.tomb_ranges + ta.x, ta.y, t, lo, hi) |
+                     tomb_span(P.tomb_ranges + ta.z, ta.w, t, lo, hi) | tomb_span(P.tomb_ranges + tb.z, tb.w, t, lo, hi)))
+    return false;
+  if (!(bk.valid && t >= bk.lo && t <= bk.hi) && !locate_bucket<EDGES>(P, t, bk)) { bk.valid = false; return false; }  // (pass 1 reports it)
+  cell = group_base + bucket_cell<EDGES>(P, bk.idx);
+  return true;
+}
+
 // One x page of a pair (work item `item` of x's buckets) and the y page of the same column group, decoded in lock-step
 // with the group's time page row by row; a row counts when scan_chunk_seg would select it (valid timestamp, keep bit,
 // time ranges, row-drop tombstones) and both x and y hold a value that no column tombstone masks. The y page is found
@@ -2336,15 +2353,8 @@ __device__ __forceinline__ void pair_page(const ScanParams &P, const PairCol &pc
     else if (r == 0 && !xc.is_gorilla) xc.d.skip_first_if_s8b_sc();
     if (yv) { yr = yc.next(); if (yc.failed()) break; }
     else if (r == 0 && !yc.is_gorilla) yc.d.skip_first_if_s8b_sc();
-    if (!(tv && xv && yv)) continue;
-    if (keepw && !((__ldg(keepw + (r >> 5)) >> (r & 31)) & 1)) continue;
-    int64_t lo, hi;
-    if (!range_span(P, t, lo, hi)) continue;
-    if (P.has_tomb && (tomb_span(P.tomb_ranges, P.n_tomb_global, t, lo, hi) | tomb_span(P.tomb_ranges + tx.x, tx.y, t, lo, hi) |
-                       tomb_span(P.tomb_ranges + tx.z, tx.w, t, lo, hi) | tomb_span(P.tomb_ranges + ty.z, ty.w, t, lo, hi)))
-      continue;
-    if (!(bk.valid && t >= bk.lo && t <= bk.hi) && !locate_bucket<EDGES>(P, t, bk)) { bk.valid = false; continue; }  // (pass 1 reports it)
-    const uint64_t cell = group_base + bucket_cell<EDGES>(P, bk.idx);
+    uint64_t cell;
+    if (!(tv && xv && yv) || !select_row<EDGES>(P, keepw, r, t, tx, ty, group_base, bk, cell)) continue;
     if (!have_run || cell != run_cell) {
       if (have_run) pair_flush<PASS2>(P, pc, run_cell, acc);
       pair_start<PASS2>(P, pc, cell, acc);
@@ -2459,6 +2469,284 @@ __global__ void k_finalize_pairs(const uint64_t *state, const PairCol *pairs, ui
       else v = pair_m2(f64(PS_DY), f64(PS_DY2), n, s[PS_YMIN * n_cells], s[PS_YMAX * n_cells]);
     }
     values[(uint64_t)(out0 + blockIdx.y) * n_cells + cell] = j == 0 ? n : (uint64_t)__double_as_longlong(v);
+  }
+  const uint32_t bits = __ballot_sync(FULL, valid);
+  if ((threadIdx.x & 31) == 0 && (cell >> 3) < bitmap_stride)
+    *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
+}
+
+// ---- medians (TSKV_QUERY_N_MEDIANS): exact selection over the cells' unsigned order keys ------------------------------
+// Pass 1 (the fused scan) leaves every cell's n, smallest and largest key in the operand's COUNT / MIN / MAX sections.
+// k_median_prep sets each cell's targets, ranks (n - 1) / 2 and n / 2, under the common leading bits of its two
+// extremes. Every selection pass (k_scan_median, k_merge_median_rows for merged rows) counts the keys under a cell's
+// prefix by their next 8-bit digit; k_median_step finds the digits that hold the ranks and extends the prefix. Once the
+// two ranks of an even cell part, the lower one is the largest key under its prefix and the upper one the smallest
+// under its own: one more pass takes both with atomicMax / atomicMin. 8 passes resolve any cell.
+// A median's state is MEDIAN_WORDS sections of n_cells words from `off` on (MedianSec) and its histograms are
+// MEDIAN_BINS u32 per cell from hist_off on; the count of unresolved cells follows every median's sections.
+enum MedianSec { MS_MODE = 0, MS_BITS, MS_PLO, MS_PHI, MS_RLO, MS_RHI, MS_LO, MS_HI, MEDIAN_WORDS };
+enum MedianMode { MM_DONE = 0, MM_HIST, MM_EXTREME };
+constexpr uint32_t MEDIAN_BINS = 256;
+constexpr int MEDIAN_PASSES = 8;  // 64 key bits / 8 per pass (a pass that parts the ranks leaves the extremes pass a digit)
+struct MedianCol {
+  uint64_t count_off, min_off, max_off;  // the operand's COUNT and MIN / MAX key sections in the scan state
+  uint64_t off, hist_off;                // the median's sections in the median state, its histograms
+  uint32_t qcol;                         // the operand's column in the scan's column table (its work-list buckets)
+  uint16_t column_id;
+  uint8_t phys_type;
+  uint8_t pad;
+};
+// The pointers every median kernel takes: the median state, the histograms and the count of unresolved cells.
+struct MedianArgs {
+  uint64_t *state;
+  uint32_t *hist;
+  unsigned long long *unresolved;
+};
+
+__device__ __forceinline__ uint64_t median_ukey(uint64_t v, uint8_t pt) { return (uint64_t)okey(v, pt) ^ 0x8000000000000000ull; }
+__device__ __forceinline__ bool median_under(uint64_t u, uint64_t prefix, uint32_t bits) {  // u has the prefix's leading bits
+  return bits == 0 || ((u ^ prefix) >> (64 - bits)) == 0;
+}
+__device__ __forceinline__ uint32_t median_digit_shift(uint32_t bits) { return 64 - bits > 8 ? 56 - bits : 0; }
+__device__ __forceinline__ uint32_t median_digit(uint64_t u, uint32_t bits) {  // the (up to) 8 bits after the prefix
+  return (uint32_t)(u >> median_digit_shift(bits)) & ((1u << (64 - bits > 8 ? 8 : 64 - bits)) - 1);
+}
+
+// One lane's run of rows in one cell: the cell's selection state, and the pending histogram run of equal digits or the
+// extremes under the two prefixes.
+struct MedianRun {
+  uint64_t cell, plo, phi, xlo, xhi;
+  uint32_t mode, bits, digit, n;
+  bool have_lo, have_hi;
+};
+__device__ __forceinline__ void median_flush(const MedianCol &mc, const MedianArgs &A, uint64_t n_cells, MedianRun &r) {
+  if (r.mode == MM_HIST && r.n) atomicAdd(A.hist + mc.hist_off + r.cell * MEDIAN_BINS + r.digit, r.n);
+  if (r.have_lo) atomicMax(reinterpret_cast<unsigned long long *>(A.state + mc.off + MS_LO * n_cells + r.cell), (unsigned long long)r.xlo);
+  if (r.have_hi) atomicMin(reinterpret_cast<unsigned long long *>(A.state + mc.off + MS_HI * n_cells + r.cell), (unsigned long long)r.xhi);
+  r.n = 0;
+  r.have_lo = r.have_hi = false;
+}
+__device__ __forceinline__ void median_open(const MedianCol &mc, const MedianArgs &A, uint64_t n_cells, uint64_t cell, MedianRun &r) {
+  const uint64_t *s = A.state + mc.off + cell;
+  r.cell = cell;
+  r.mode = (uint32_t)s[MS_MODE * n_cells];
+  r.bits = (uint32_t)s[MS_BITS * n_cells];
+  r.plo = s[MS_PLO * n_cells];
+  r.phi = s[MS_PHI * n_cells];
+  r.n = 0;
+  r.have_lo = r.have_hi = false;
+}
+__device__ __forceinline__ void median_add(const MedianCol &mc, const MedianArgs &A, uint64_t n_cells, MedianRun &r, uint64_t u) {
+  if (r.mode == MM_HIST) {
+    if (!median_under(u, r.plo, r.bits)) return;
+    const uint32_t d = median_digit(u, r.bits);
+    if (r.n && d != r.digit) median_flush(mc, A, n_cells, r);
+    r.digit = d;
+    r.n++;
+  } else if (r.mode == MM_EXTREME) {
+    if (median_under(u, r.plo, r.bits)) { r.xlo = r.have_lo ? max(r.xlo, u) : u; r.have_lo = true; }
+    if (median_under(u, r.phi, r.bits)) { r.xhi = r.have_hi ? min(r.xhi, u) : u; r.have_hi = true; }
+  }
+}
+
+// One page of a median's operand (work item `item` of its buckets), decoded with its group's time page row by row and
+// selected as the column pairs select (select_row). Decode errors are pass 1's to report: the lane stops at the first.
+template <bool EDGES>
+__device__ __forceinline__ void median_page(const ScanParams &P, const MedianCol &mc, const MedianArgs &A, uint32_t item) {
+  const uint32_t page = P.work_page[item], slot = P.work_slot[item];
+  const tskv_page_desc vd = P.descs[page];
+  const uint32_t tpage = P.time_page_of[page];
+  const tskv_page_desc td = P.descs[tpage];
+  if (vd.phys_type != mc.phys_type || kind_status(vd.reserved) != TSKV_OK || kind_status(td.reserved) != TSKV_OK ||
+      td.reserved == DK_ALLNULL || vd.reserved == DK_ALLNULL)
+    return;
+  PageView tpv, vpv;
+  tpv.open(P.arena, td);
+  vpv.open(P.arena, vd);
+  BitCursor tb, vb;
+  tb.init(tpv.bitset);
+  vb.init(vpv.bitset);
+  DeltaCursor<-1> tc;
+  AnyCursor<> vc;
+  if (tc.open(tpv, td.reserved) != TSKV_OK || vc.open(vpv, vd.reserved) != TSKV_OK) return;
+  const uint4 none = make_uint4(0, 0, 0, 0);
+  const uint4 tv4 = P.has_tomb ? tomb_lookup(P, vd.series_id, mc.column_id) : none;
+  const uint32_t *keepw = P.row_keep ? P.row_keep + P.keep_off[tpage] : nullptr;
+  const uint64_t group_base = group_cell_base<EDGES>(P, slot);
+  BucketState bk; bk.valid = false; bk.floor_regime = false; bk.lo = 0; bk.hi = 0; bk.idx = 0;
+  MedianRun run;
+  run.mode = MM_DONE;
+  run.cell = ~0ull;
+  run.n = 0;
+  run.have_lo = run.have_hi = false;
+  int64_t t = 0;
+  const uint32_t n_rows = vd.num_values;
+  for (uint32_t r = 0; r < n_rows; r++) {
+    const bool tv = tb.next(r), vv = vb.next(r);
+    uint64_t v = 0;
+    if (tv) { t = (int64_t)tc.next(); if (tc.exhausted) break; }
+    else if (r == 0) tc.skip_first_if_s8b_sc();
+    if (vv) { v = vc.next(); if (vc.failed()) break; }
+    else if (r == 0 && !vc.is_gorilla) vc.d.skip_first_if_s8b_sc();
+    uint64_t cell;
+    if (!(tv && vv) || !select_row<EDGES>(P, keepw, r, t, tv4, none, group_base, bk, cell)) continue;
+    if (cell != run.cell) {
+      median_flush(mc, A, P.n_cells, run);
+      median_open(mc, A, P.n_cells, cell, run);
+    }
+    median_add(mc, A, P.n_cells, run, median_ukey(v, mc.phys_type));
+  }
+  median_flush(mc, A, P.n_cells, run);
+}
+
+// One selection pass of the medians (blockIdx.y: the median): one lane per work item of the operand's buckets (every
+// bin, wide and narrow), the items pass 1 read. Returns at once when every cell is resolved.
+template <bool EDGES>
+__global__ void __launch_bounds__(128) k_scan_median(const __grid_constant__ ScanParams P, const MedianCol *meds, const MedianArgs A) {
+  if (*(volatile unsigned long long *)A.unresolved == 0) return;
+  const MedianCol mc = meds[blockIdx.y];
+  const uint32_t stride = gridDim.x * blockDim.x, t0 = blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t k = mc.qcol * WL_SUB; k < N_BINS * P.n_cols * WL_SUB; k += P.n_cols * WL_SUB)
+    for (uint32_t sub = 0; sub < WL_SUB; sub++) {
+      const uint32_t start = __ldg(P.region_start + k + sub), fill = __ldg(P.region_fill + k + sub);
+      for (uint32_t i = t0; i < fill; i += stride) median_page<EDGES>(P, mc, A, start + i);
+    }
+}
+
+// After pass 1: every cell's targets. A cell with no value is done (NULL); one whose extremes are equal is done with
+// that key; any other starts its histogram passes under the common leading bits of its extremes.
+__global__ void k_median_prep(const uint64_t *state, const MedianCol *meds, const MedianArgs A, uint64_t n_cells) {
+  const MedianCol mc = meds[blockIdx.y];
+  uint64_t *s = A.state + mc.off;
+  unsigned open = 0;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_cells; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t n = state[mc.count_off + i];
+    const uint64_t kmin = state[mc.min_off + i] ^ 0x8000000000000000ull, kmax = state[mc.max_off + i] ^ 0x8000000000000000ull;
+    const bool hist = n > 1 && kmin != kmax;
+    const uint32_t bits = hist ? (uint32_t)__clzll((long long)(kmin ^ kmax)) : 64;
+    const uint64_t prefix = bits == 0 ? 0 : kmin & (~0ull << (64 - bits));
+    s[MS_MODE * n_cells + i] = hist ? MM_HIST : MM_DONE;
+    s[MS_BITS * n_cells + i] = bits;
+    s[MS_PLO * n_cells + i] = s[MS_PHI * n_cells + i] = prefix;
+    s[MS_RLO * n_cells + i] = n ? (n - 1) / 2 : 0;
+    s[MS_RHI * n_cells + i] = n / 2;
+    s[MS_LO * n_cells + i] = s[MS_HI * n_cells + i] = kmin;
+    open += hist;
+  }
+  open = __reduce_add_sync(FULL, open);
+  if ((threadIdx.x & 31) == 0 && open) atomicAdd(A.unresolved, (unsigned long long)open);
+}
+
+// After a selection pass: a warp per cell. A histogram cell (lane l holds bins 8 l .. 8 l + 7) finds the digits that
+// hold its two ranks, clears its bins and extends its prefixes; it is done when the key is complete, and goes to the
+// extremes pass when the ranks part. An extremes cell is done (the pass left its keys in MS_LO / MS_HI).
+__global__ void __launch_bounds__(256) k_median_step(const MedianCol *meds, const MedianArgs A, uint64_t n_cells) {
+  if (*(volatile unsigned long long *)A.unresolved == 0) return;
+  const MedianCol mc = meds[blockIdx.y];
+  uint64_t *s = A.state + mc.off;
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+  for (uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n_cells; i += warps) {
+    const uint64_t mode = s[MS_MODE * n_cells + i];
+    if (mode == MM_DONE) continue;
+    if (mode == MM_EXTREME) {
+      if (lane == 0) {
+        s[MS_MODE * n_cells + i] = MM_DONE;
+        atomicAdd(A.unresolved, ~0ull);
+      }
+      continue;
+    }
+    uint4 *h = reinterpret_cast<uint4 *>(A.hist + mc.hist_off + i * MEDIAN_BINS) + 2 * lane;
+    const uint4 a = h[0], b = h[1];
+    h[0] = h[1] = make_uint4(0, 0, 0, 0);
+    const uint32_t c[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    uint64_t sum = 0;
+#pragma unroll
+    for (int k = 0; k < 8; k++) sum += c[k];
+    uint64_t incl = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint64_t v = ((uint64_t)__shfl_up_sync(FULL, (uint32_t)(incl >> 32), o) << 32) | __shfl_up_sync(FULL, (uint32_t)incl, o);
+      if (lane >= (uint32_t)o) incl += v;
+    }
+    const uint64_t excl = incl - sum;
+    // the digit holding rank r and r's rank among the keys of that digit (found = false: the pass counted fewer keys
+    // than pass 1, which only a decode error that pass 1 reports can cause)
+    auto find = [&](uint64_t r, uint32_t &d, uint64_t &rest) {
+      const uint32_t owner = __ballot_sync(FULL, excl <= r && r < incl);
+      if (!owner) return false;
+      const int src = __ffs(owner) - 1;
+      uint32_t dd = 0;
+      uint64_t rr = r - excl;
+      if ((int)lane == src)
+        for (int k = 0; k < 8; k++) {
+          if (rr < c[k]) { dd = 8 * lane + k; break; }
+          rr -= c[k];
+        }
+      d = __shfl_sync(FULL, dd, src);
+      rest = shfl_u64(rr, src);
+      return true;
+    };
+    uint32_t dlo = 0, dhi = 0;
+    uint64_t qlo = 0, qhi = 0;
+    const bool found_lo = find(s[MS_RLO * n_cells + i], dlo, qlo);
+    const bool found_hi = find(s[MS_RHI * n_cells + i], dhi, qhi);
+    if (lane == 0) {
+      const uint32_t bits = (uint32_t)s[MS_BITS * n_cells + i];
+      const uint32_t sh = median_digit_shift(bits), nb = 64 - sh;
+      const uint64_t plo = s[MS_PLO * n_cells + i] | ((uint64_t)dlo << sh), phi = s[MS_PLO * n_cells + i] | ((uint64_t)dhi << sh);
+      s[MS_BITS * n_cells + i] = nb;
+      s[MS_PLO * n_cells + i] = plo;
+      s[MS_PHI * n_cells + i] = phi;
+      s[MS_RLO * n_cells + i] = qlo;
+      s[MS_RHI * n_cells + i] = qhi;
+      if (nb == 64 || !found_lo || !found_hi) {
+        s[MS_LO * n_cells + i] = plo;
+        s[MS_HI * n_cells + i] = phi;
+        s[MS_MODE * n_cells + i] = MM_DONE;
+        atomicAdd(A.unresolved, ~0ull);
+      } else if (dlo != dhi) {
+        s[MS_LO * n_cells + i] = 0;
+        s[MS_HI * n_cells + i] = ~0ull;
+        s[MS_MODE * n_cells + i] = MM_EXTREME;
+      }
+    }
+  }
+}
+
+// The median outputs (blockIdx.y: the median; output column out0 + blockIdx.y), in the operand's type, valid iff n >= 1:
+// the key at rank n / 2 for odd n, else lo.add_wrapping(hi).div_wrapping(2) of the keys at ranks n / 2 - 1 and n / 2.
+// f64 NaN results are those of x86-64 SSE arithmetic, on which DataFusion runs: a NaN operand's bits, quieted, the
+// first one first; -inf + inf gives the negative default NaN.
+__global__ void k_finalize_medians(const uint64_t *state, const MedianCol *meds, const MedianArgs A, uint32_t out0, uint64_t n_cells,
+                                   uint64_t bitmap_stride, uint64_t *values, uint8_t *validity) {
+  const MedianCol mc = meds[blockIdx.y];
+  const uint64_t cell = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  bool valid = false;
+  if (cell < n_cells) {
+    const uint64_t n = state[mc.count_off + cell];
+    const uint64_t *s = A.state + mc.off + cell;
+    const uint64_t lo = okey_inv((int64_t)(s[MS_LO * n_cells] ^ 0x8000000000000000ull), mc.phys_type);
+    const uint64_t hi = okey_inv((int64_t)(s[MS_HI * n_cells] ^ 0x8000000000000000ull), mc.phys_type);
+    uint64_t v = 0;
+    valid = n > 0;
+    if (n & 1) {
+      v = lo;
+    } else if (n) {
+      if (mc.phys_type == TSKV_PT_I64) {
+        v = (uint64_t)((int64_t)(lo + hi) / 2);
+      } else if (mc.phys_type == TSKV_PT_U64) {
+        v = (lo + hi) / 2;
+      } else {
+        const double x = __longlong_as_double((long long)lo), y = __longlong_as_double((long long)hi);
+        const double sum = x + y;
+        if (isnan(x)) v = lo | 0x0008000000000000ull;
+        else if (isnan(y)) v = hi | 0x0008000000000000ull;
+        else if (isnan(sum)) v = 0xfff8000000000000ull;
+        else v = (uint64_t)__double_as_longlong(sum / 2.0);
+      }
+    }
+    values[(uint64_t)(out0 + blockIdx.y) * n_cells + cell] = v;
   }
   const uint32_t bits = __ballot_sync(FULL, valid);
   if ((threadIdx.x & 31) == 0 && (cell >> 3) < bitmap_stride)

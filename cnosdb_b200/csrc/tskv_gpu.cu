@@ -257,6 +257,13 @@ struct tskv_scan {
   uint32_t n_pairs = 0;
   async_ptr<PairCol> d_pairs;
   uint64_t pair_words = 0;
+  // medians (TSKV_QUERY_N_MEDIANS; k_scan_median): their operands, selection state (MedianSec sections, then the count of
+  // unresolved cells) and histograms
+  uint32_t n_medians = 0;
+  async_ptr<MedianCol> d_medians;
+  async_ptr<uint64_t> d_med_state;
+  async_ptr<uint32_t> d_med_hist;
+  MedianArgs med{};
 };
 
 namespace {
@@ -343,16 +350,20 @@ bool query_has_m2(const tskv_query *q) {
   return false;
 }
 
-// The query the scan runs for a query with column pairs: its projected columns, then every pair operand that is not one
-// of them as a COUNT column without output (so that the work list, the page gathers, CRC checks, pass 1 and the reader
-// counters treat the operands' pages as they treat a COUNT column's), and per pair the operands' places in that table.
-struct PairQuery {
+uint32_t query_n_medians(const tskv_query *q) { return TSKV_QUERY_N_MEDIANS(q->reserved); }
+
+// The query the scan runs for a query with column pairs or medians: its projected columns, then every operand that is
+// not one of them as a COUNT column without output (so that the work list, the page gathers, CRC checks, pass 1 and the
+// reader counters treat the operands' pages as they treat a COUNT column's), and per pair and median the operands'
+// places in that table. A median's operand column also computes MIN and MAX in pass 1 (its extreme keys).
+struct OperandQuery {
   tskv_query q{};
   std::vector<tskv_agg_column> cols;
-  std::vector<PairCol> pairs;  // (off is set by plan_state)
+  std::vector<PairCol> pairs;      // (off is set by plan_layout)
+  std::vector<MedianCol> medians;  // (the offsets are set by plan_layout)
 };
-PairQuery plan_pair_query(const tskv_query *q) {
-  PairQuery pq;
+OperandQuery plan_operand_query(const tskv_query *q) {
+  OperandQuery pq;
   pq.q = *q;
   pq.cols.assign(q->columns, q->columns + q->n_columns);
   auto place = [&](const tskv_agg_column &op) {
@@ -371,6 +382,15 @@ PairQuery plan_pair_query(const tskv_query *q) {
     pc.x_pt = x.phys_type;
     pc.y_pt = y.phys_type;
     pq.pairs.push_back(pc);
+  }
+  for (uint32_t m = 0; m < query_n_medians(q); m++) {
+    const tskv_agg_column &op = q->columns[q->n_columns + 2 * q->n_pairs + m];
+    MedianCol mc{};
+    mc.qcol = place(op);
+    pq.cols[mc.qcol].agg_mask |= TSKV_AGG_MIN | TSKV_AGG_MAX;
+    mc.column_id = op.column_id;
+    mc.phys_type = op.phys_type;
+    pq.medians.push_back(mc);
   }
   pq.q.columns = pq.cols.data();
   pq.q.n_columns = (uint32_t)pq.cols.size();
@@ -539,7 +559,8 @@ bool labels_first_last(const tskv_query *q, const BucketEdges &E) {
 
 // (an edge scan's buckets come from its edge table, width = 0)
 bool query_shape_ok(const tskv_query *q, bool edges = false) {
-  return q->n_buckets != 0 && (q->n_columns != 0 || q->n_pairs != 0) && q->columns && (q->width > 0 || q->n_buckets == 1 || edges);
+  return q->n_buckets != 0 && (q->n_columns != 0 || q->n_pairs != 0 || query_n_medians(q) != 0) && q->columns &&
+         (q->width > 0 || q->n_buckets == 1 || edges);
 }
 
 // Output layout of a query that passed query_shape_ok and tag_groups_refusal.
@@ -548,6 +569,7 @@ tskv_output_layout output_layout(const tskv_pages *pages, const tskv_query *q, c
   uint64_t n_out = 0;
   for (uint32_t c = 0; c < q->n_columns; c++) n_out += popc8(q->columns[c].agg_mask);
   if (q->n_pairs <= TSKV_MAX_PAIRS) n_out += 4ull * q->n_pairs;  // n, C, M2x, M2y per pair
+  if (query_n_medians(q) <= TSKV_MAX_MEDIANS) n_out += query_n_medians(q);
   uint64_t n_groups = 1;
   if (q->group_by_series) n_groups = selected_slots(pages, q);
   if (tg.on) n_groups = tg.n;
@@ -828,6 +850,23 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
         return TSKV_ERR_INVALID_ARG;
       }
   }
+  const uint32_t n_med = query_n_medians(q);
+  if (n_med > TSKV_MAX_MEDIANS || (uint64_t)q->n_columns + 2ull * q->n_pairs + n_med > 126) {
+    ctx->set_error("invalid query: at most 8 medians and 126 columns with the pairs' and medians' operands");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  for (uint32_t k = 2 * q->n_pairs; k < 2 * q->n_pairs + n_med; k++) {
+    const tskv_agg_column &op = q->columns[q->n_columns + k];
+    if (op.agg_mask != 0 || op.phys_type < TSKV_PT_I64 || op.phys_type > TSKV_PT_F64) {
+      ctx->set_error("invalid median operand: an I64 / U64 / F64 column with agg_mask 0");
+      return TSKV_ERR_INVALID_ARG;
+    }
+    for (uint32_t c = 0; c < q->n_columns + k; c++)
+      if (q->columns[c].column_id == op.column_id && q->columns[c].phys_type != op.phys_type) {
+        ctx->set_error("median operand: one column id with two types");
+        return TSKV_ERR_INVALID_ARG;
+      }
+  }
   if (q->n_predicates > TSKV_MAX_PREDICATES || (q->n_predicates && !q->predicates)) {
     ctx->set_error("invalid query: at most 8 field predicates");
     return TSKV_ERR_INVALID_ARG;
@@ -878,6 +917,24 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
   if (slide && q->n_pairs) {
     ctx->set_error("sliding windows: column pairs (covariance / correlation) are not pushed down");
     return TSKV_ERR_UNSUPPORTED;
+  }
+  if (n_med && slide) {
+    ctx->set_error("sliding windows: medians are not pushed down");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  if (n_med && (q->reserved & TSKV_QUERY_MULTI_RANK)) {
+    ctx->set_error("multi-rank scan: medians are not pushed down (their selection state does not merge across ranks)");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  for (uint32_t m = 0; m < n_med; m++) {  // the histograms count a cell's keys in 32 bits
+    const uint16_t id = q->columns[q->n_columns + 2 * q->n_pairs + m].column_id;
+    uint64_t rows = 0;
+    for (const tskv_page_desc &d : pages->h_descs)
+      if (d.phys_type != TSKV_PT_TIME && d.column_id == id) rows += d.num_values;
+    if (rows >> 32) {
+      ctx->set_error("median: the operand's pages hold 2^32 rows or more");
+      return TSKV_ERR_UNSUPPORTED;
+    }
   }
   *win_k = 1;
   return slide ? check_sliding(ctx, pages, q, slide, win_k) : TSKV_OK;
@@ -941,12 +998,14 @@ struct ScanLayout {
   uint64_t m2_words = 0;
   std::vector<PairCol> pairs;  // column pairs, with their state offsets
   uint64_t pair_words = 0;
+  std::vector<MedianCol> medians;  // medians, with their operands' pass-1 sections and their selection state's offsets
 };
 
 // n_cells: cells of the query's grid (a sliding scan: windows); kern_cells: cells of the fused kernels' grid (panes).
-// n_user: the columns with outputs (the rest are pair operands read as COUNT columns); pairs: plan_pair_query's.
-ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint64_t kern_cells, uint32_t n_user,
-                       const std::vector<PairCol> &pairs) {
+// user_cols[0, n_user): the columns with outputs, as the caller asked for them (the rest of q's are operands read as
+// COUNT columns, and a median's operand has MIN | MAX added); oq: plan_operand_query's.
+ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint64_t kern_cells, const tskv_agg_column *user_cols,
+                       uint32_t n_user, const OperandQuery &oq) {
   ScanLayout out;
   const StatePlan win = plan_state(q, n_cells);
   const StatePlan pane = sliding ? plan_state(q, kern_cells) : StatePlan{};
@@ -956,9 +1015,18 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
   out.means = win.means;
   out.m2 = win.m2;  // (sliding scans refuse M2)
   out.m2_words = win.m2_words;
-  out.pairs = pairs;  // (sliding scans refuse pairs)
+  out.pairs = oq.pairs;  // (sliding scans refuse pairs and medians)
   for (size_t p = 0; p < out.pairs.size(); p++) out.pairs[p].off = win.pair_off + (uint64_t)PAIR_WORDS * n_cells * p;
   out.pair_words = win.pair_words;
+  out.medians = oq.medians;
+  for (size_t m = 0; m < out.medians.size(); m++) {
+    MedianCol &mc = out.medians[m];
+    mc.count_off = win.cols[mc.qcol].count_off;
+    mc.min_off = win.cols[mc.qcol].min_off;
+    mc.max_off = win.cols[mc.qcol].max_off;
+    mc.off = (uint64_t)MEDIAN_WORDS * n_cells * m;
+    mc.hist_off = (uint64_t)MEDIAN_BINS * n_cells * m;
+  }
   if (sliding) {
     for (uint32_t c = 0; c < q->n_columns; c++) {
       const ColState &p = pane.cols[c], &w = win.cols[c];
@@ -976,7 +1044,7 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
   // output column table
   uint64_t fk = out.sl.first_keys_off, lk = out.sl.last_keys_off, fv = out.sl.selval_off, lv = out.sl.selval_off + out.sl.first_cells;
   for (uint32_t c = 0; c < n_user; c++) {
-    const tskv_agg_column &qc = q->columns[c];
+    const tskv_agg_column &qc = user_cols[c];
     for (unsigned bit = 0; bit < 8; bit++) {
       unsigned agg = 1u << bit;
       if (!(qc.agg_mask & agg)) continue;
@@ -1275,6 +1343,18 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
   s->pair_words = lay.pair_words;
   if (e == cudaSuccess && s->n_pairs) e = upload(s->d_pairs, lay.pairs.data(), lay.pairs.size(), st);
   *h2d += lay.pairs.size() * sizeof(PairCol);
+  s->n_medians = (uint32_t)lay.medians.size();
+  if (s->n_medians) {  // (the histograms start cleared; every selection step clears the bins it read)
+    const uint64_t n_cells = s->layout.n_cells;
+    if (e == cudaSuccess) e = upload(s->d_medians, lay.medians.data(), lay.medians.size(), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_med_state, (size_t)MEDIAN_WORDS * n_cells * s->n_medians + 1, st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_med_hist, (size_t)MEDIAN_BINS * n_cells * s->n_medians, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(s->d_med_hist.get(), 0, (size_t)MEDIAN_BINS * n_cells * s->n_medians * 4, st);
+    s->med.state = s->d_med_state.get();
+    s->med.hist = s->d_med_hist.get();
+    s->med.unresolved = reinterpret_cast<unsigned long long *>(s->d_med_state.get() + (size_t)MEDIAN_WORDS * n_cells * s->n_medians);
+    *h2d += lay.medians.size() * sizeof(MedianCol);
+  }
   if (e == cudaSuccess) e = stream_alloc(s->d_aux, AUX_WORDS, st);
   if (e == cudaSuccess) e = stream_alloc(s->d_values, s->layout.n_out * s->layout.n_cells, st);
   if (e == cudaSuccess) e = stream_alloc(s->d_validity, s->layout.validity_bytes + 8, st);
@@ -2038,9 +2118,14 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   tskv_status st = validate_query(ctx, pages, q, slide, tg, E, &win_k);
   if (st != TSKV_OK) return st;
   const tskv_output_layout L = output_layout(pages, q, tg);
-  // column pairs: from here on the scan runs the query with the operands as columns (plan_pair_query)
+  if (query_n_medians(q) && (uint64_t)query_n_medians(q) * L.n_cells > TSKV_MAX_MEDIAN_CELLS) {
+    ctx->set_error("median: more than 2^22 cells times medians (1 KiB of histogram per cell and median)");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  // column pairs and medians: from here on the scan runs the query with the operands as columns (plan_operand_query)
+  const tskv_agg_column *user_cols = q->columns;
   const uint32_t n_user = q->n_columns;
-  PairQuery pq = plan_pair_query(q);
+  OperandQuery pq = plan_operand_query(q);
   pq.q.columns = pq.cols.data();
   q = &pq.q;
   cudaSetDevice(ctx->device);
@@ -2062,8 +2147,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   s->win_k = win_k;
   s->n_windows = q->n_buckets;
   s->n_panes = q->n_buckets - win_k + 1;
-  const ScanLayout lay = plan_layout(q, slide != 0, L.n_cells, L.n_groups * s->n_panes, n_user, pq.pairs);
-  s->n_out = (uint32_t)lay.outs.size();  // (the pairs' outputs follow, k_finalize_pairs)
+  const ScanLayout lay = plan_layout(q, slide != 0, L.n_cells, L.n_groups * s->n_panes, user_cols, n_user, pq);
+  s->n_out = (uint32_t)lay.outs.size();  // (the pairs' outputs follow, k_finalize_pairs, then the medians')
   s->sl = lay.sl;
   s->kern_sl = lay.kern_sl;
   uint64_t h2d = 0;
@@ -2332,7 +2417,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     cudaStreamWaitEvent(ctx->stream.get(), ev_done, 0);  // join
     launches++;
   }
-  if (!capturing && !s->n_m2 && !s->n_pairs) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
+  if (!capturing && !s->n_m2 && !s->n_pairs && !s->n_medians) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
   if (s->n_combine) {  // sliding windows: every window folds its panes (it writes every array the kernels fill)
     const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
     k_window_combine<<<dim3(std::max(1u, bx), s->n_combine), 256, 0, ctx->stream.get()>>>(
@@ -2370,7 +2455,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       cudaStreamWaitEvent(ctx->stream.get(), s->ev_m2_join[b].get(), 0);
       launches++;
     }
-    if (!capturing && !s->n_pairs) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes pass 2)
+    if (!capturing && !s->n_pairs && !s->n_medians) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes pass 2)
   }
   if (s->n_pairs) {  // column pairs: pass 1 (n, sums, extremes), the shifts, pass 2 (co-moments); overlap merge rows first
     const bool edges = s->params.edges != nullptr;
@@ -2396,7 +2481,31 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       CU_TRY(ctx, cudaLaunchKernel(fn, dim3(px, s->n_pairs), dim3(128), args, 0, ctx->stream.get()));
       launches++;
     }
-    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the pair passes)
+    if (!capturing && !s->n_medians) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the pair passes)
+  }
+  if (s->n_medians) {  // medians: the targets from pass 1, then MEDIAN_PASSES fixed selection passes (merged rows first)
+    const bool edges = s->params.edges != nullptr;
+    const uint64_t n_cells = s->layout.n_cells;
+    const uint32_t bx = (uint32_t)std::min<uint64_t>((n_cells + 255) / 256, 1024);
+    const uint32_t wx = (uint32_t)std::min<uint64_t>((n_cells + 7) / 8, 4096);  // k_median_step: a warp per cell
+    const uint32_t px = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)pages->n_descs + 127) / 128, (uint64_t)ctx->sm_count * 16));
+    const bool merge = s->merge.n_rows && s->n_merge_pages;
+    CU_TRY(ctx, cudaMemsetAsync(s->med.unresolved, 0, sizeof(unsigned long long), ctx->stream.get()));
+    k_median_prep<<<dim3(std::max(1u, bx), s->n_medians), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_medians.get(), s->med, n_cells);
+    launches++;
+    const void *fn = edges ? (const void *)k_scan_median<true> : (const void *)k_scan_median<false>;
+    const MedianCol *mp = s->d_medians.get();
+    void *args[] = {(void *)&s->params, (void *)&mp, (void *)&s->med};
+    for (int pass = 0; pass < MEDIAN_PASSES; pass++) {
+      if (merge) {
+        k_merge_median_rows<<<(uint32_t)((s->merge.n_rows + 127) / 128), 128, 0, ctx->stream.get()>>>(s->params, s->merge, mp, s->n_medians, s->med);
+        launches++;
+      }
+      CU_TRY(ctx, cudaLaunchKernel(fn, dim3(px, s->n_medians), dim3(128), args, 0, ctx->stream.get()));
+      k_median_step<<<dim3(std::max(1u, wx), s->n_medians), 256, 0, ctx->stream.get()>>>(mp, s->med, n_cells);
+      launches += 2;
+    }
+    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the selection passes)
   }
   if (!capturing) cudaEventRecord(s->ev1.get(), ctx->stream.get());
   CU_TRY(ctx, cudaGetLastError());
@@ -2533,8 +2642,17 @@ tskv_status tskvgpu_scan_work_list(tskv_ctx *ctx, tskv_scan *s, uint32_t *n_buck
   return TSKV_OK;
 }
 
+// Medians keep no mergeable partial state: the exchange calls refuse a scan with medians.
+static tskv_status refuse_medians(tskv_ctx *ctx, const tskv_scan *s, const char *call) {
+  if (!s->n_medians) return TSKV_OK;
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  ctx->set_error(std::string(call) + ": a scan with medians has no mergeable partial state");
+  return TSKV_ERR_UNSUPPORTED;
+}
+
 tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_view *out) {
   if (!ctx || !s || !out) return TSKV_ERR_INVALID_ARG;
+  if (tskv_status st = refuse_medians(ctx, s, "scan_partials")) return st;
   if (s->n_m2 || s->n_pairs) {
     std::lock_guard<std::mutex> lock(ctx->mu);
     ctx->set_error("scan_partials: second moments (TSKV_AGG_M2, column pairs) do not all-reduce element-wise; use tskvgpu_scan_exchange");
@@ -2571,6 +2689,7 @@ static void merge_m2(tskv_ctx *ctx, tskv_scan *s, const uint64_t *gathered, uint
 
 tskv_status tskvgpu_scan_exchange_view(tskv_ctx *ctx, tskv_scan *s, uint64_t *out_dptr, uint64_t *out_words) {
   if (!ctx || !s || !out_dptr || !out_words) return TSKV_ERR_INVALID_ARG;
+  if (tskv_status st = refuse_medians(ctx, s, "scan_exchange_view")) return st;
   *out_dptr = (uint64_t)(uintptr_t)s->d_state.get();
   *out_words = s->sl.selval_off + s->sl.selval_len + s->m2_words + s->pair_words;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values | M2 | pairs
   return TSKV_OK;
@@ -2578,6 +2697,7 @@ tskv_status tskvgpu_scan_exchange_view(tskv_ctx *ctx, tskv_scan *s, uint64_t *ou
 
 tskv_status tskvgpu_scan_merge_gathered(tskv_ctx *ctx, tskv_scan *s, uint64_t gathered_dptr, uint32_t n_ranks) {
   if (!ctx || !s || !gathered_dptr || n_ranks == 0) return TSKV_ERR_INVALID_ARG;
+  if (tskv_status st = refuse_medians(ctx, s, "scan_merge_gathered")) return st;
   std::lock_guard<std::mutex> lock(ctx->mu);
   cudaSetDevice(ctx->device);
   const uint64_t words = s->sl.selval_off + s->sl.selval_len + s->m2_words + s->pair_words;
@@ -2591,6 +2711,7 @@ tskv_status tskvgpu_scan_merge_gathered(tskv_ctx *ctx, tskv_scan *s, uint64_t ga
 
 tskv_status tskvgpu_scan_exchange(tskv_ctx *ctx, tskv_scan *s) {
   if (!ctx || !s) return TSKV_ERR_INVALID_ARG;
+  if (tskv_status st = refuse_medians(ctx, s, "scan_exchange")) return st;
   std::lock_guard<std::mutex> lock(ctx->mu);
   cudaSetDevice(ctx->device);
   if (!ctx->comm) {
@@ -2644,6 +2765,10 @@ static tskv_status finalize_device(tskv_ctx *ctx, tskv_scan *s) {
   if (s->n_pairs)
     k_finalize_pairs<<<dim3((uint32_t)((L.n_cells + 255) / 256), 4 * s->n_pairs), 256, 0, ctx->stream.get()>>>(
         s->d_state.get(), s->d_pairs.get(), s->n_out, L.n_cells, L.bitmap_stride, s->d_values.get(), s->d_validity.get());
+  if (s->n_medians)
+    k_finalize_medians<<<dim3((uint32_t)((L.n_cells + 255) / 256), s->n_medians), 256, 0, ctx->stream.get()>>>(
+        s->d_state.get(), s->d_medians.get(), s->med, s->n_out + 4 * s->n_pairs, L.n_cells, L.bitmap_stride, s->d_values.get(),
+        s->d_validity.get());
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;
 }

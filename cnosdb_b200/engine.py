@@ -219,16 +219,22 @@ class TskvError(RuntimeError):
 
 
 class PushedAggregate:
-    """One projected value column with its aggregate set (extends PushedAggregateFunction::Count)."""
+    """One projected value column with its aggregate set (extends PushedAggregateFunction::Count). "median" has no mask
+    bit: it makes the column a median operand (after the pairs' operands, agg_mask 0), and a column that asks for nothing
+    else has no projected entry."""
 
     def __init__(self, column_id, phys_type, aggs):
         self.column_id = int(column_id)
         self.phys_type = int(phys_type)
+        self.median = False
         if isinstance(aggs, int):
             self.agg_mask = aggs
         else:
             self.agg_mask = 0
             for a in aggs:
+                if a == "median":
+                    self.median = True
+                    continue
                 # var* / stddev* ask the scan for COUNT | M2; ScanResult.column derives them
                 self.agg_mask |= (TSKV_AGG_COUNT | TSKV_AGG_M2) if a in STAT_AGGS else AGG_BITS[a]
 
@@ -269,15 +275,17 @@ class QueryOption:
         q.origin, q.width = self.origin, self.width
         q.first_bucket_start, q.n_buckets = self.first_bucket_start, self.n_buckets
         q.group_by_series = 1 if self.group_by_series else 0
-        q.reserved = cabi.TSKV_QUERY_MULTI_RANK if self.multi_rank else 0
-        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))]
-        cols = (cabi.AggColumn * max(1, len(self.columns) + len(ops)))()
-        for i, c in enumerate(self.columns):
+        proj = self.projected()
+        meds = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "median", False)]
+        q.reserved = (cabi.TSKV_QUERY_MULTI_RANK if self.multi_rank else 0) | cabi.query_medians(len(meds))
+        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))] + meds
+        cols = (cabi.AggColumn * max(1, len(proj) + len(ops)))()
+        for i, c in enumerate(proj):
             cols[i].column_id, cols[i].phys_type, cols[i].agg_mask = c.column_id, c.phys_type, c.agg_mask
-        for i, (cid, pt) in enumerate(ops):  # the pairs' operands follow the projected columns, agg_mask 0
-            cols[len(self.columns) + i].column_id, cols[len(self.columns) + i].phys_type = cid, pt
+        for i, (cid, pt) in enumerate(ops):  # the pairs' operands, then the medians', follow the projected columns
+            cols[len(proj) + i].column_id, cols[len(proj) + i].phys_type = cid, pt
         q.columns = cols
-        q.n_columns = len(self.columns)
+        q.n_columns = len(proj)
         q.n_pairs = len(self.pairs)
         preds = (cabi.FieldPredicate * max(1, len(self.predicates)))()
         for i, (c, pt, op, v) in enumerate(self.predicates):
@@ -292,9 +300,14 @@ class QueryOption:
         self._keep = (tr, cols, preds)  # keep the ctypes arrays alive as long as the query
         return q
 
+    def projected(self):
+        """The columns with a projected entry (an aggregate other than median)."""
+        return [c for c in self.columns if c.agg_mask or not getattr(c, "median", False)]
+
     def output_names(self):
-        return ([(c.column_id, cabi.AGG_NAMES[a]) for c in self.columns for a in c.agg_list()] +
-                [(("pair", k), r) for k in range(len(self.pairs)) for r in PAIR_RAW])
+        return ([(c.column_id, cabi.AGG_NAMES[a]) for c in self.projected() for a in c.agg_list()] +
+                [(("pair", k), r) for k in range(len(self.pairs)) for r in PAIR_RAW] +
+                [(c.column_id, "median") for c in self.columns if getattr(c, "median", False)])
 
 
 class ScanResult:
@@ -326,7 +339,8 @@ class ScanResult:
 
     def column(self, column_id, agg):
         """(typed values, validity) of one output column, shaped [n_groups, n_buckets]. agg may also name one of STAT_AGGS
-        (var, var_samp, var_pop, stddev, stddev_samp, stddev_pop), derived from the column's count and m2."""
+        (var, var_samp, var_pop, stddev, stddev_samp, stddev_pop), derived from the column's count and m2, or "median"
+        (the operand's type)."""
         if agg in STAT_AGGS:
             n, _ = self.column(column_id, "count")
             m2, ok = self.column(column_id, "m2")
@@ -583,6 +597,11 @@ class Engine:
             raise ValueError("m2 / var* / stddev* and slide: sliding windows do not push the variance state down")
         if slide is not None and getattr(query, "pairs", None):
             raise ValueError("pairs (covar* / corr) and slide: sliding windows do not push the covariance state down")
+        if any(getattr(c, "median", False) for c in query.columns):
+            if slide is not None:
+                raise ValueError("median and slide: sliding windows do not push medians down")
+            if getattr(query, "multi_rank", False):
+                raise ValueError("median and multi_rank: medians have no mergeable partial state")
 
     @staticmethod
     def _edges(edges, slide):

@@ -198,6 +198,32 @@ typedef struct tskv_query {
  * series ranks), so that all ranks build comparable first/last tie-break keys. Requires series_ids != NULL when the
  * query groups by series or asks for first/last; unbucketed first/last across series need bounded time ranges. */
 #define TSKV_QUERY_MULTI_RANK 1u
+/* Medians: median(x) (DataFusion's MedianAccumulator), exact. Bits 8..15 of the flags word (`reserved`) hold n_medians:
+ * TSKV_QUERY_MEDIANS(n) sets them, TSKV_QUERY_N_MEDIANS(flags) reads them. The n_medians entries of `columns` after the
+ * pairs' 2 * n_pairs operands are the medians' operands: column_id and phys_type (I64 / U64 / F64) of each, agg_mask 0;
+ * n_columns may be 0; n_columns + 2 * n_pairs + n_medians <= 126. A median takes the operand's values in the selected rows
+ * (time ranges, series, the row filter of the predicates, row-drop and column tombstones), NULLs left out, ordered by the
+ * type's order (f64: IEEE totalOrder; NaN is a value). Per cell each median adds one output after the pairs' outputs, in
+ * the operand's type, valid iff the cell holds a value: for odd n the value at rank n / 2 (from 0), for even n
+ * (lo + hi) / 2 of the values lo, hi at ranks n / 2 - 1 and n / 2 in the operand's type: i64 wrapping add, then division
+ * truncating toward zero; u64 wrapping add, then / 2; f64 (lo + hi) / 2.0 with x86-64 NaN results (a NaN operand's bits,
+ * quieted, lo first; -inf + inf gives 0xfff8000000000000). Computed by radix selection on the order keys: pass 1 gives
+ * every cell's n and extreme keys (the operand's kernel mask gains COUNT | MIN | MAX; an operand that is not a projected
+ * column is read like such a column with no output), then 8 selection passes over the operand's pages each narrow the
+ * keys at the two ranks by an 8-bit digit (histograms of 1 KiB per cell and median) until a cell is resolved; passes
+ * that no cell needs decode nothing. Refused before any launch: TSKV_ERR_INVALID_ARG for n_medians > TSKV_MAX_MEDIANS, an
+ * operand with a non-zero agg_mask or a BOOL / TIME / unknown type, an operand id projected with another type, or more
+ * than 126 columns; TSKV_ERR_UNSUPPORTED for sliding windows (slide != width), TSKV_QUERY_MULTI_RANK, more than
+ * TSKV_MAX_MEDIAN_CELLS cells times medians (the histogram budget, 4 GiB; GROUP BY series over 100 000 series x 168
+ * buckets exceeds it), and an operand whose pages hold 2^32 rows or more (the histograms count in 32 bits).
+ * tskvgpu_scan_partials, _exchange_view, _exchange and _merge_gathered refuse a scan with medians. Pages of another type
+ * under an operand's id are an error. Counters: page_read_count, page_read_bytes, points_decoded, rows_in_range and
+ * pruned_page_count equal those of the same query with every operand that is not projected added as a COUNT column;
+ * kernel_launches and elapsed_fused_ms include the selection passes. */
+#define TSKV_MAX_MEDIANS 8
+#define TSKV_MAX_MEDIAN_CELLS (1u << 22)
+#define TSKV_QUERY_MEDIANS(n) (((uint32_t)(n) & 0xffu) << 8)
+#define TSKV_QUERY_N_MEDIANS(flags) (((uint32_t)(flags) >> 8) & 0xffu)
 
 /* Result layout. Outputs are dense: for output column j (query columns in order, and inside a
  * column the set agg bits in ascending bit order) and cell c = group * n_buckets + bucket:

@@ -34,6 +34,18 @@ pub const TSKV_AGG_LAST: u8 = 1 << 6;
 pub const TSKV_AGG_M2: u8 = 1 << 7;
 /// At most this many column pairs (tskv_query.n_pairs; covariance / correlation, see tskv_gpu.h).
 pub const TSKV_MAX_PAIRS: u32 = 8;
+/// At most this many medians; their count sits in bits 8..15 of tskv_query.reserved (see tskv_gpu.h).
+pub const TSKV_MAX_MEDIANS: u32 = 8;
+/// A scan with medians holds at most this many cells times medians (1 KiB of histogram each).
+pub const TSKV_MAX_MEDIAN_CELLS: u64 = 1 << 22;
+/// TSKV_QUERY_MEDIANS(n): the flags-word bits of n medians.
+pub const fn tskv_query_medians(n: u32) -> u32 {
+    (n & 0xff) << 8
+}
+/// TSKV_QUERY_N_MEDIANS(flags): the medians of a flags word.
+pub const fn tskv_query_n_medians(flags: u32) -> u32 {
+    (flags >> 8) & 0xff
+}
 
 pub const TSKV_UPLOAD_VERIFY_CRC: u32 = 1;
 pub const TSKV_UPLOAD_HOST_RESIDENT: u32 = 2;

@@ -1,0 +1,44 @@
+"""The median kernels of libtskv_gpu.so's sm_90a cubin (read with cuobjdump, demangled with cu++filt) are exactly the
+instantiations tests/test_gpu_median.py runs: k_scan_median<EDGES> for the selection passes of tumbling and edge scans,
+k_merge_median_rows for the merged rows of overlapping chunk files, and the three helpers between and after the
+passes."""
+import re
+import subprocess
+
+import pytest
+
+from cnosdb_b200 import cabi
+from tests.test_kernel_list import cuda_tool
+
+EXPECTED = {"k_scan_median<false>", "k_scan_median<true>", "k_merge_median_rows", "k_median_prep", "k_median_step",
+            "k_finalize_medians"}
+
+
+def normalise(demangled):
+    """'void tskv::k_scan_median<(bool)1>(tskv::ScanParams, ...)' -> 'k_scan_median<true>'."""
+    m = re.search(r"\b(k_scan_median|k_merge_median_rows|k_median_prep|k_median_step|k_finalize_medians)(<[^>]*>)?\(", demangled)
+    if not m:
+        return None
+    if not m.group(2):
+        return m.group(1)
+    args = [{"(bool)0": "false", "(bool)1": "true"}.get(a.strip(), a.strip()) for a in m.group(2)[1:-1].split(",")]
+    return "%s<%s>" % (m.group(1), ", ".join(args))
+
+
+def test_normalise():
+    assert normalise("void tskv::k_scan_median<(bool)1>(tskv::ScanParams, const tskv::MedianCol *, tskv::MedianArgs)") == \
+        "k_scan_median<true>"
+    assert normalise("tskv::k_median_step(const tskv::MedianCol *, tskv::MedianArgs, unsigned long)") == "k_median_step"
+    assert normalise("void tskv::k_scan_m2<(int)0, (int)0, (bool)0>(tskv::ScanParams, int)") is None
+
+
+def test_median_kernels_match_the_library():
+    cuobjdump, cufilt = cuda_tool("cuobjdump"), cuda_tool("cu++filt")
+    if cuobjdump is None or cufilt is None:
+        pytest.skip("cuobjdump / cu++filt (CUDA toolkit) not found: the kernel list cannot be read from the library")
+    out = subprocess.run([cuobjdump, "-ltext", cabi.gpu_library_path()], check=True, capture_output=True, text=True).stdout
+    mangled = [m for m in re.findall(r"SASS text section \d+ : \S*?-(_Z\w+)\.sm_90a\.", out) if "median" in m.lower()]
+    names = subprocess.run([cufilt], input="\n".join(mangled), check=True, capture_output=True, text=True).stdout.split("\n")
+    found = [k for k in (normalise(n) for n in names) if k]
+    assert len(found) == len(set(found)), found
+    assert set(found) == EXPECTED, (sorted(set(found) - EXPECTED), sorted(EXPECTED - set(found)))
