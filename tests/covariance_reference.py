@@ -4,14 +4,17 @@ random_arena's: truth[series] = [(ts, {column: (values, valid)}), ...] per colum
 The row selection is restated row by row, so that x and y stay paired: a row counts when its series is selected, its
 timestamp lies in the query's time ranges and in a bucket of the grid (or of the edges), the AND-ed predicates hold, no
 row-drop tombstone covers it, and both x and y are valid and not masked by a column tombstone. A column group without x
-or y has no paired row. Per cell: n, C = sum (x - mx)(y - my), M2x and M2y over the paired rows, computed with
-fractions.Fraction over the values converted to f64 and rounded once (NaN with a NaN or infinite value)."""
+or y has no paired row. Overlapping chunk files (`files=`) are merged as helpers.exact_aggregate merges them, with x and
+y as the merge's columns: predicates and row drops before the merge, the time ranges, column tombstones and buckets on
+the merged rows. Per cell: n, C = sum (x - mx)(y - my), M2x and M2y over the paired rows, computed exactly over the
+values converted to f64 and rounded once (NaN with a NaN or infinite value)."""
+import copy
 import math
 import os
-from fractions import Fraction
 
 import numpy as np
 
+from cnosdb_b200.engine import PushedAggregate
 from tests import helpers
 
 
@@ -24,46 +27,69 @@ def exact_comoments(xs, ys):
     if not all(math.isfinite(v) for v in xs + ys):
         bad_x = not all(math.isfinite(v) for v in xs)
         bad_y = not all(math.isfinite(v) for v in ys)
-        m2 = lambda vs: math.nan if not all(math.isfinite(v) for v in vs) else _m2(vs)
-        return n, math.nan, (math.nan if bad_x else m2(xs)), (math.nan if bad_y else m2(ys))
-    fx, fy = [Fraction(v) for v in xs], [Fraction(v) for v in ys]
-    mx, my = sum(fx) / n, sum(fy) / n
-    c = sum((a - mx) * (b - my) for a, b in zip(fx, fy))
-    return n, _round(c), _round(sum((a - mx) ** 2 for a in fx)), _round(sum((b - my) ** 2 for b in fy))
+        return n, math.nan, (math.nan if bad_x else _m2(xs)), (math.nan if bad_y else _m2(ys))
+    (kx, qx), (ky, qy) = _scaled(xs), _scaled(ys)
+    return n, _co(kx, qx, ky, qy), _co(kx, qx, kx, qx), _co(ky, qy, ky, qy)
 
 
 def _m2(vs):
-    f = [Fraction(v) for v in vs]
-    m = sum(f) / len(f)
-    return _round(sum((a - m) ** 2 for a in f))
+    k, q = _scaled(vs)
+    return _co(k, q, k, q)
 
 
-def _round(fr):
+def _scaled(vs):
+    """f64 values as integers k over one common power-of-two denominator q: v = k / q exactly."""
+    ratios = [v.as_integer_ratio() for v in vs]
+    q = max(d for _, d in ratios)
+    return [p * (q // d) for p, d in ratios], q
+
+
+def _co(ka, qa, kb, qb):
+    """sum (a - ma)(b - mb) = (n sum ka kb - sum ka sum kb) / (n qa qb), rounded once (int / int rounds correctly)."""
+    n = len(ka)
+    num = n * sum(a * b for a, b in zip(ka, kb)) - sum(ka) * sum(kb)
     try:
-        return float(fr)
+        return num / (n * qa * qb)
     except OverflowError:
-        return math.inf if fr > 0 else -math.inf
+        return math.inf if num > 0 else -math.inf
 
 
-def paired_rows(truth, query, pair, tombstones=None, group_ids=None, edges=None, labels=None):
+def paired_rows(truth, query, pair, tombstones=None, group_ids=None, edges=None, labels=None, files=None):
     """{cell: ([x], [y])} of the pair (x_id, x_pt, y_id, y_pt) under `query` (a QueryOption); cell = group * n_buckets +
-    bucket, group = series slot (group_by_series), group_ids[slot] (GROUP BY tags) or 0."""
+    bucket, group = series slot (group_by_series), group_ids[slot] (GROUP BY tags) or 0. files: the file id of every
+    column group in truth's order (helpers.exact_aggregate's `files`)."""
     x_id, x_pt, y_id, y_pt = pair
     glob, rows_t, cols_t = helpers.tombstone_lists(tombstones)
+    file_of = helpers.files_by_series(truth, files)
+    mq = copy.copy(query)  # the merge's query columns: the operands
+    mq.columns = [PushedAggregate(x_id, x_pt, 0), PushedAggregate(y_id, y_pt, 0)]
+    ops = list(dict.fromkeys((x_id, y_id)))
     sel = list(query.series_ids) if query.series_ids is not None else sorted(truth)
-    out = {}
+    cells, xs, ys = [], [], []
     for slot, sid in enumerate(sel):
         sid = int(sid)
         if sid not in truth:
             continue
+        cgs = truth[sid]
         group = slot if query.group_by_series else (int(group_ids[slot]) if group_ids is not None else 0)
-        for ts, cols in truth[sid]:
-            if x_id not in cols or y_id not in cols:
+        row_drop = glob + rows_t.get(sid, [])
+        units = []  # (timestamps, columns, rows that pass the predicates and row drops)
+        for streams in helpers.overlap_groups(cgs, file_of.get(sid)):
+            if len(streams) >= 2:
+                ts, cols = helpers._merged_rows(cgs, streams, mq, ops, row_drop)
+                cols = {c: (v.view(helpers._typed(pt, []).dtype), ok) for (c, pt), (v, ok) in
+                        zip(((x_id, x_pt), (y_id, y_pt)), (cols[x_id], cols[y_id]))}
+                units.append((ts, cols, np.ones(ts.size, dtype=bool)))
                 continue
-            ts = np.asarray(ts, dtype=np.int64)
-            keep = np.ones(ts.size, dtype=bool) if not query.time_ranges else helpers._in_ranges(ts, query.time_ranges)
-            keep &= helpers._predicates_hold(query, ts, cols)
-            keep &= ~helpers._in_ranges(ts, glob + rows_t.get(sid, []))
+            for k in streams[0]:
+                ts, cols = cgs[k]
+                if x_id not in cols or y_id not in cols:
+                    continue
+                ts = np.asarray(ts, dtype=np.int64)
+                units.append((ts, cols, helpers._predicates_hold(query, ts, cols) & ~helpers._in_ranges(ts, row_drop)))
+        for ts, cols, keep in units:
+            if query.time_ranges:
+                keep = keep & helpers._in_ranges(ts, query.time_ranges)
             (xv, xok), (yv, yok) = cols[x_id], cols[y_id]
             keep &= np.asarray(xok, dtype=bool) & np.asarray(yok, dtype=bool)
             keep &= ~helpers._in_ranges(ts, cols_t.get((sid, x_id), []))
@@ -77,14 +103,18 @@ def paired_rows(truth, query, pair, tombstones=None, group_ids=None, edges=None,
             else:
                 b, inb = helpers.bucket_index(ts, query)
             keep &= inb
+            cells.append(group * query.n_buckets + np.asarray(b, dtype=np.int64)[keep])
             # (int64 / uint64 / float64 arrays: astype is (double)x, round to nearest)
-            fx, fy = np.asarray(xv).astype(np.float64), np.asarray(yv).astype(np.float64)
-            for r in np.nonzero(keep)[0]:
-                cell = group * query.n_buckets + int(b[r])
-                xs, ys = out.setdefault(cell, ([], []))
-                xs.append(float(fx[r]))
-                ys.append(float(fy[r]))
-    return out
+            xs.append(np.asarray(xv).astype(np.float64)[keep])
+            ys.append(np.asarray(yv).astype(np.float64)[keep])
+    if not cells:
+        return {}
+    cl = np.concatenate(cells)
+    order = np.argsort(cl, kind="stable")  # (a cell's rows keep their order)
+    cl, fx, fy = cl[order], np.concatenate(xs)[order], np.concatenate(ys)[order]
+    heads = np.flatnonzero(np.concatenate([[True], cl[1:] != cl[:-1]])) if cl.size else cl
+    bounds = list(heads) + [cl.size]
+    return {int(cl[a]): (fx[a:z].tolist(), fy[a:z].tolist()) for a, z in zip(bounds[:-1], bounds[1:])}
 
 
 def exact_pair_cells(truth, query, pair, n_cells, **kw):

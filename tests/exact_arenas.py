@@ -436,3 +436,37 @@ def expected(truth, query, extra, tombstones=None, files=None):
         from tests.sliding_reference import expand_aggregate
         return expand_aggregate(merge_truth(truth, files, query) if files is not None else truth, query, extra["slide"])
     return exact_aggregate(truth, query, tombstones=tombstones, files=files)
+
+
+def two_file_arena(t0, step, seed=11):
+    """Six series of two chunk files of 120 rows each on the grid t0 + k * step; file 2 starts 50 rows later, so rows
+    50-119 of file 1 share file 2's times. An i64 column 1 and an f64 column 2 hold NULLs apart. -> (arena, descs,
+    truth, files, merged): merged is the truth of the merged rows, built by hand (the later file wins per column when it
+    holds a value: take_last_and_merge)."""
+    rng = np.random.default_rng(seed)
+    b = datagen.ArenaBuilder()
+    truth, files, rows = {}, [], {}
+    for sid in range(6):
+        for f in range(2):
+            n = 120
+            ts = t0 + (np.arange(n, dtype=np.int64) + 50 * f) * step
+            x = rng.integers(-100, 100, n).astype(np.int64)
+            y = rng.random(n) * 10
+            xv, yv = rng.random(n) > 0.2, rng.random(n) > 0.2
+            b.add_column_group(sid, ts, [(1, cabi.TSKV_PT_I64, x, xv), (2, cabi.TSKV_PT_F64, y, yv)])
+            truth.setdefault(sid, []).append((ts, {1: (x, xv), 2: (y, yv)}))
+            files.append(f + 1)
+            for i in range(n):
+                row = rows.setdefault((sid, int(ts[i])), {})
+                if xv[i]:
+                    row[1] = x[i]
+                if yv[i]:
+                    row[2] = y[i]
+    arena, descs = b.finish()
+    merged = {}
+    for sid in range(6):
+        tss = sorted(t for s, t in rows if s == sid)
+        cols = {c: (np.array([rows[(sid, t)].get(c, 0) for t in tss], dtype=dt),
+                    np.array([c in rows[(sid, t)] for t in tss])) for c, dt in ((1, np.int64), (2, np.float64))}
+        merged[sid] = [(np.array(tss, dtype=np.int64), cols)]
+    return arena, descs, truth, np.array(files, dtype=np.uint64), merged

@@ -307,6 +307,17 @@ def overlap_groups(cgs, files):
     return [[sorted(chunks[f], key=lambda k: int(np.min(cgs[k][0]))) for f in sorted(g)] for g in groups]
 
 
+def files_by_series(truth, files):
+    """{series: [file id of each of its column groups]} from `files` in truth's order ({} for None)."""
+    file_of, k = {}, 0
+    if files is not None:
+        for sid, cgs in truth.items():
+            file_of[sid] = list(files[k:k + len(cgs)])
+            k += len(cgs)
+        assert k == len(files)
+    return file_of
+
+
 def _merged_rows(cgs, streams, query, qcols, row_drop):
     """The merged rows of one overlap group of two or more chunks: rows of the column groups this scan reads that pass
     the predicates (on their own column group) and no row tombstone; equal times collapse, every query column takes the
@@ -383,17 +394,12 @@ def exact_aggregate(truth, query, tombstones=None, files=None, key_slots=None):
     if want_sel and slot_bits and first_last_rel_bits(truth, query) + slot_bits > 62:
         raise ReferenceError(cabi.TSKV_ERR_UNSUPPORTED)
     glob, row_tomb, col_tomb = tombstone_lists(tombstones)
-    file_of, k = {}, 0
-    if files is not None:
-        for sid, cgs in truth.items():
-            file_of[sid] = list(files[k:k + len(cgs)])
-            k += len(cgs)
-        assert k == len(files)
+    file_of = files_by_series(truth, files)
     units = []  # (slot, times, selected rows, {column: (u64 values, validity)}): one FIRST / LAST run per bucket
     for slot, sid in enumerate(slots):
         cgs = truth.get(sid, [])
         row_drop = glob + row_tomb.get(sid, [])
-        for streams in overlap_groups(cgs, file_of.get(sid) if files is not None else None):
+        for streams in overlap_groups(cgs, file_of.get(sid)):
             if len(streams) >= 2:
                 ts, cols = _merged_rows(cgs, streams, query, qcols, row_drop)
                 units.append((slot, ts, np.ones(ts.size, dtype=bool), cols))

@@ -97,3 +97,12 @@ def exact_median_cells(truth, query, col, pt, n_cells, **kw):
         if m is not None:
             v[cell], ok[cell] = m, True
     return v, ok
+
+
+def check_median(res, j, exact, what=""):
+    """Output j of a ScanResult, a median, against exact_median_cells: validity equal, values bit for bit."""
+    v_e, ok_e = exact
+    v, ok = res.values[j], res.validity[j]
+    np.testing.assert_array_equal(ok, ok_e, err_msg=what + " median validity")
+    bad = np.nonzero(ok_e & (v != v_e))[0]
+    assert bad.size == 0, (what, [(int(i), hex(int(v[i])), hex(int(v_e[i]))) for i in bad[:5]])

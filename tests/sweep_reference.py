@@ -12,7 +12,15 @@ A case's expected outcome is the exact reference of tests/helpers.py composed fo
 tags, sliding windows, M2, tombstones, the overlap merge), or the status the scan must refuse it with: the reference's own
 ReferenceError, or a refusal this module states: SUM or M2 on a BOOL column (TSKV_ERR_INVALID_ARG), FIRST / LAST with a
 sliding window (TSKV_ERR_UNSUPPORTED, sliding_reference.sliding_status), M2 with a sliding window (the engine's
-ValueError, before the library is called)."""
+ValueError, before the library is called).
+
+random_operand_case adds column pairs (covar / corr) and medians to a random case. Their outcome adds the exact
+co-moments (covariance_reference) and medians (median_reference) of every pair and median, or one more refusal this
+module states: a pair or a median with a sliding window (the engine's ValueError), a BOOL operand
+(TSKV_ERR_INVALID_ARG). The scan runs such a query with every operand that is not projected as a COUNT column without
+output (scan_query): the other outputs' reference is that query's."""
+import copy
+
 import numpy as np
 
 from cnosdb_b200 import cabi, datagen
@@ -20,9 +28,11 @@ from cnosdb_b200.engine import PushedAggregate, QueryOption, sliding_window_grid
 from tests.edges_reference import exact_aggregate_edges, exact_aggregate_grouped_edges
 from tests.exact_arenas import add_column_group, merge_truth
 from tests.group_reference import exact_aggregate_grouped
-from tests.helpers import ReferenceError, bucket_spec, exact_aggregate
+from tests.helpers import ReferenceError, bucket_spec, exact_aggregate, files_by_series, overlap_groups
 from tests.labels_reference import exact_aggregate_grouped_labels, exact_aggregate_labels
 from tests.sliding_reference import expand_aggregate, sliding_status
+from tests.covariance_reference import exact_pair_cells
+from tests.median_reference import exact_median_cells
 from tests.variance_reference import with_m2
 
 # ---- the kernels -------------------------------------------------------------------------------------------------------
@@ -478,8 +488,25 @@ def random_case(index, base_seed):
 
 
 def expected(truth, query, extra, tombstones=None, files=None):
-    """The composed exact reference of one scan -> ExactResult (M2 filled in), or the status int the scan must refuse it
-    with, or "ValueError" (the engine refuses M2 with a sliding window before calling the library)."""
+    """The composed exact reference of one scan -> ExactResult (M2 filled in; with pairs or medians, `pairs` holds
+    exact_pair_cells of every pair and `medians` exact_median_cells of every median), or the status int the scan must
+    refuse it with, or "ValueError" (the engine refuses M2, pairs and medians with a sliding window before calling the
+    library)."""
+    medians = [c for c in query.columns if c.median]
+    if query.pairs or medians:
+        if extra.get("slide") is not None:
+            return "ValueError"
+        if BOOL in [pt for _, pt in operands(query)]:
+            return cabi.TSKV_ERR_INVALID_ARG
+        res = expected(truth, scan_query(query), extra, tombstones, files)
+        if isinstance(res, (int, str)):
+            return res
+        kw = dict(tombstones=tombstones, files=files, group_ids=extra.get("group_ids"), edges=extra.get("edges"),
+                  labels=extra.get("labels"))
+        n_cells = res.values.shape[1]
+        res.pairs = [exact_pair_cells(truth, query, p, n_cells, **kw) for p in query.pairs]
+        res.medians = [exact_median_cells(truth, query, c.column_id, c.phys_type, n_cells, **kw) for c in medians]
+        return res
     has_m2 = any(c.agg_mask & cabi.TSKV_AGG_M2 for c in query.columns)
     has_sel = any(c.agg_mask & (cabi.TSKV_AGG_FIRST | cabi.TSKV_AGG_LAST) for c in query.columns)
     slide = extra.get("slide")
@@ -515,3 +542,123 @@ def expected(truth, query, extra, tombstones=None, files=None):
 
 def case_expected(case):
     return expected(case.truth, case.query, case.extra, tombstones=case.tombstones, files=case.files)
+
+
+# ---- random cases with column pairs and medians ----------------------------------------------------------------------
+def operands(query):
+    """(column id, type) of the pairs' operands (x0, y0, x1, ...), then the medians'."""
+    return [o for x, xt, y, yt in query.pairs for o in ((x, xt), (y, yt))] + \
+        [(c.column_id, c.phys_type) for c in query.columns if c.median]
+
+
+def scan_query(query):
+    """The query the scan runs for one with pairs or medians (plan_operand_query): the projected columns, then every
+    operand that is not one of them as a COUNT column without output."""
+    cols = [PushedAggregate(c.column_id, c.phys_type, c.agg_mask) for c in query.projected()]
+    for cid, pt in operands(query):
+        if cid not in [c.column_id for c in cols]:
+            cols.append(PushedAggregate(cid, pt, ["count"]))
+    q = copy.copy(query)
+    q.columns, q.pairs, q._keep = cols, [], None
+    return q
+
+
+def operand_columns(query):
+    """-> ([(qx, qy) of every pair], [qcol of every median]): the operands' places in scan_query's columns."""
+    ids = [c.column_id for c in scan_query(query).columns]
+    return [(ids.index(x), ids.index(y)) for x, _, y, _ in query.pairs], \
+        [ids.index(c.column_id) for c in query.columns if c.median]
+
+
+# the kernels of the pairs' and medians' row-by-row passes: the scan and merged-row kernels of the EXPECTED sets of
+# tests/test_pair_kernel_list.py and tests/test_median_kernel_list.py, which hold those sets to the library
+# (tests/test_pair_median_sweep_reference.py checks that this list is that subset)
+OPERAND_KERNELS = ("k_scan_pair<false, false>", "k_scan_pair<false, true>", "k_scan_pair<true, false>",
+                   "k_scan_pair<true, true>", "k_merge_pairs_rows<false>", "k_merge_pairs_rows<true>",
+                   "k_scan_median<false>", "k_scan_median<true>", "k_merge_median_rows")
+
+
+def merged_operands(truth, query, files, ops):
+    """Whether an overlap group of two or more chunks of a selected series holds every column of `ops` (merged rows of
+    those operands, which the k_merge_*_rows kernels read)."""
+    if files is None:
+        return False
+    file_of = files_by_series(truth, files)
+    for sid in (query.series_ids if query.series_ids is not None else sorted(truth)):
+        cgs = truth.get(int(sid), [])
+        for streams in overlap_groups(cgs, file_of.get(int(sid))):
+            held = {c for st in streams for k in st for c in cgs[k][1]}
+            if len(streams) >= 2 and set(ops) <= held:
+                return True
+    return False
+
+
+def operand_kernels(wl, query, edges, truth=None, files=None):
+    """The operand kernels a pass launched with work: both passes of k_scan_pair<PASS2, EDGES> when a pair's x operand
+    has work-list items, k_scan_median<EDGES> when a median's operand has, k_merge_pairs_rows<PASS2> when a pair's x and
+    y have merged rows, and k_merge_median_rows when a median's operand has (merged_operands over `files`)."""
+    qpairs, qmeds = operand_columns(query)
+    fill = bin_fill(wl, len(scan_query(query).columns))
+    e = "true" if edges else "false"
+    out = set()
+    if any(fill[:, qx].sum() for qx, _ in qpairs):
+        out |= {"k_scan_pair<false, %s>" % e, "k_scan_pair<true, %s>" % e}
+    if any(fill[:, qc].sum() for qc in qmeds):
+        out.add("k_scan_median<%s>" % e)
+    if any(merged_operands(truth, query, files, (x, y)) for x, _, y, _ in query.pairs):
+        out |= {"k_merge_pairs_rows<false>", "k_merge_pairs_rows<true>"}
+    if any(merged_operands(truth, query, files, (c.column_id,)) for c in query.columns if c.median):
+        out.add("k_merge_median_rows")
+    return out
+
+
+def random_operand_case(index, base_seed):
+    """random_case(index, base_seed) with 0-3 column pairs and 0-3 medians drawn from a stream of their own (the case's
+    other draws are random_case's): pairs over the arena's numeric columns, x == y among them; medians on one column
+    twice, on a projected column (the column's entry asks for it too) or on an unprojected one. At most one refusal per
+    case: a case that random_case makes a refusal gets no operand; a sliding-window case gets operands only as the
+    refusal "pair_sliding" / "median_sliding"; others may be "bool_pair" / "bool_median" (a BOOL operand)."""
+    case = random_case(index, base_seed)
+    rng = np.random.default_rng([base_seed, index, 1])
+    q = case.query
+    have = columns_of(case.truth)
+    num = [c for c in have if COLUMNS[c] != BOOL]
+    refusal = "none"
+    if "slide" in case.extra:
+        refusal = str(rng.choice(["pair_sliding", "median_sliding", "none"]))
+    elif BOOL in [COLUMNS[c] for c in have] and rng.random() < 0.06:
+        refusal = str(rng.choice(["bool_pair", "bool_median"]))
+    if case.desc["refusal"] != "none" or not num or (refusal == "none" and "slide" in case.extra):
+        case.desc.update(pairs=[], medians=[], operand_refusal="none")
+        return case
+    pick = lambda: int(rng.choice(num))  # noqa: E731
+    pairs = []
+    for _ in range(int(rng.integers(0, 4))):
+        x = pick()
+        y = x if rng.random() < 0.3 else pick()
+        pairs.append((x, COLUMNS[x], y, COLUMNS[y]))
+    meds = []
+    for _ in range(int(rng.integers(0, 4))):
+        c = meds[-1] if meds and rng.random() < 0.25 else pick()
+        meds.append(c)
+    if refusal in ("pair_sliding", "bool_pair") and not pairs:
+        x = pick()
+        pairs.append((x, COLUMNS[x], x, COLUMNS[x]))
+    if refusal in ("median_sliding", "bool_median") and not meds:
+        meds.append(pick())
+    if refusal == "bool_pair":
+        k = int(rng.integers(0, len(pairs)))
+        x, xt, y, yt = pairs[k]
+        pairs[k] = (4, BOOL, y, yt) if rng.random() < 0.5 else (x, xt, 4, BOOL)
+    if refusal == "bool_median":
+        meds[int(rng.integers(0, len(meds)))] = 4
+    q.pairs = pairs
+    for c in meds:
+        entry = [e for e in q.columns if e.column_id == c and e.agg_mask and not e.median]
+        if entry and rng.random() < 0.5:
+            entry[0].median = True  # the projected entry asks for the median as well
+        else:
+            q.columns.append(PushedAggregate(c, COLUMNS[c], ["median"]))
+    case.desc.update(pairs=[(x, y) for x, _, y, _ in pairs], medians=[c.column_id for c in q.columns if c.median],
+                     operand_refusal=refusal)
+    return case

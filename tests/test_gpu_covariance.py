@@ -1,8 +1,8 @@
 """Column pairs (tskv_query.n_pairs: covar / covar_samp / covar_pop / corr) through the scan, against the exact per-cell
 co-moments of tests/covariance_reference.py: every grouping, NULL patterns that differ between x and y, column groups
 without y, predicates, tombstones on one operand, time ranges, host-resident pages with CRC on read, overlapping chunk
-files, special values, constant columns, C(x, x) against TSKV_AGG_M2, counters, refusals, a three-rank exchange and
-graph replay."""
+files, special values, constant columns, C(x, x) against TSKV_AGG_M2, counters, refusals and graph replay (the
+multi-rank merge of pairs: tests/test_gpu_multi_rank.py)."""
 
 import ctypes as C
 
@@ -11,9 +11,8 @@ import pytest
 
 from cnosdb_b200 import cabi, datagen
 from cnosdb_b200.engine import Engine, PushedAggregate, QueryOption, TskvError
-from tests import ranks
 from tests.covariance_reference import check_pair, exact_pair_cells, load_golden, tb2_column
-from tests.exact_arenas import add_column_group
+from tests.exact_arenas import add_column_group, two_file_arena
 from tests.helpers import bucket_spec, random_arena
 
 pytestmark = pytest.mark.gpu
@@ -204,40 +203,12 @@ def test_extremes_special_values_constant(eng):
 
 def test_overlapping_chunk_files(eng):
     """Two overlapping chunk files per series: the pair passes run over the merged rows."""
-    rng = np.random.default_rng(11)
-    b = datagen.ArenaBuilder()
-    files, merged = [], {}
-    for sid in range(6):
-        for f in range(2):
-            n = 120
-            ts = T0 + (np.arange(n, dtype=np.int64) + 50 * f) * STEP  # rows 50-119 of file 1 share file 2's times
-            x = rng.integers(-100, 100, n).astype(np.int64)
-            y = rng.random(n) * 10
-            xv = rng.random(n) > 0.2
-            yv = rng.random(n) > 0.2
-            b.add_column_group(sid, ts, [(1, I64, x, xv), (2, F64, y, yv)])
-            files.append(f + 1)
-            for i in range(n):  # the later file wins per column when it holds a value (take_last_and_merge)
-                row = merged.setdefault((sid, int(ts[i])), {})
-                if xv[i]:
-                    row[1] = x[i]
-                if yv[i]:
-                    row[2] = y[i]
-    a, d = b.finish()
-    truth = {}
-    for sid in range(6):
-        tss = sorted(t for s, t in merged if s == sid)
-        cols = {}
-        for c, dt in ((1, np.int64), (2, np.float64)):
-            vals = np.array([merged[(sid, t)].get(c, 0) for t in tss], dtype=dt)
-            ok = np.array([c in merged[(sid, t)] for t in tss])
-            cols[c] = (vals, ok)
-        truth[sid] = [(np.array(tss, dtype=np.int64), cols)]
+    a, d, truth, files, _ = two_file_arena(T0, STEP)
     pages = eng.upload_pages(a, d)
     try:
-        pages.set_chunk_files(np.array(files, dtype=np.uint64))
+        pages.set_chunk_files(files)
         q = grid_query(truth, pairs=[(1, I64, 2, F64)], group_by_series=True)
-        check_all(eng.scan_aggregate(pages, q), truth, q, "overlap")
+        check_all(eng.scan_aggregate(pages, q), truth, q, "overlap", files=files)
     finally:
         pages.close()
 
@@ -292,17 +263,6 @@ def test_refusals(eng):
             s.close()
     finally:
         pages.close()
-
-
-def test_three_ranks(eng):
-    a, d, truth = arena(6)
-    q = grid_query(truth, pairs=[(1, I64, 2, F64), (4, F64, 3, U64)], series_ids=np.arange(24, dtype=np.uint32))
-    ids = list(range(24))
-    for n_ranks in (1, 3):
-        shards = [ids[r::n_ranks] for r in range(n_ranks)]
-        outs = ranks.sharded_scans(eng, a, d, q, shards)
-        for r, res in enumerate(outs):
-            check_all(res, truth, q, "%d ranks, rank %d" % (n_ranks, r))
 
 
 def test_graph_replay(eng, monkeypatch, capfd):

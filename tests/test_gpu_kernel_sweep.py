@@ -10,23 +10,37 @@
    sliding window, unbucketed), aggregates with FIRST / LAST and M2, predicates, time ranges, tombstones, a host-resident
    page set, CRC on read, TSKV_PARTS and TSKV_SMEM_TABLE_KB. Each is checked against its expected result or status, and
    scanned twice (a prepared scan, then an end-to-end call): every output that does not depend on the order of f64
-   additions must be byte-identical. TSKV_SWEEP_CASE=<index> reruns one case."""
+   additions must be byte-identical. TSKV_SWEEP_CASE=<index> reruns one case.
+3. test_random_operand_combinations: N_OPERAND random cases with column pairs and medians (sweep_reference:
+   random_operand_case). Where the query projects COUNT(c), the pair (c, c)'s n and the median of c's validity must
+   equal it first (the pairs' and medians' row selection against pass 1's); then the pairs by check_pair, the medians
+   bit for bit and every other output against the exact reference, and medians and pair n byte-identical between two
+   runs.
+   TSKV_SWEEP_CASE=<index> reruns one case here too.
+4. test_operands_in_every_bin: pairs over every numeric column pair and a median per numeric column over the arena of
+   each bin (simple8b-value bins: wide, mixed and narrow pages), tumbling and edge scans; the work list read back proves
+   the operands' pages sat in that bin's intended bucket.
+5. test_every_operand_kernel_reached: tests 3 and 4 together launched every operand kernel
+   (sweep_reference.OPERAND_KERNELS) on work (skipped unless both ran to the end, test 3 over every case)."""
 import os
 
 import numpy as np
 import pytest
 
 from cnosdb_b200 import cabi
-from cnosdb_b200.engine import TskvError
+from cnosdb_b200.engine import PushedAggregate, TskvError
 from tests import sweep_reference as sw
+from tests.covariance_reference import check_pair
 from tests.helpers import assert_matches_exact
+from tests.median_reference import check_median
 from tests.variance_reference import check_m2
 
 pytestmark = pytest.mark.gpu
 
 BASE_SEED = 20261017
 N_RANDOM = 300
-ONE_CASE = os.environ.get("TSKV_SWEEP_CASE")  # rerun one index of test_random_combinations
+N_OPERAND = 200
+ONE_CASE = os.environ.get("TSKV_SWEEP_CASE")  # rerun one index of test_random_combinations / _operand_combinations
 
 
 class _Picked:
@@ -51,9 +65,9 @@ def check_exact(got, exp, what):
 
 def deterministic_outputs(res):
     """Indices of the outputs that do not depend on the order of f64 additions: counts, integer sums and means, MIN /
-    MAX and FIRST / LAST of every type."""
+    MAX and FIRST / LAST of every type, pair n and medians."""
     return [j for j, (c, a) in enumerate(res.names)
-            if not (a == "m2" or (a in ("sum", "mean") and res.phys[c] == cabi.TSKV_PT_F64))]
+            if not (a in ("m2", "c", "m2x", "m2y") or (a in ("sum", "mean") and res.phys[c] == cabi.TSKV_PT_F64))]
 
 
 def assert_same_bytes(a, b, what):
@@ -150,9 +164,38 @@ def test_every_instantiation(engine, monkeypatch):
                                                                            sorted(short_reached)))
 
 
+def check_operands(got, exp, query, what):
+    """The pairs and medians of `got` against exp.pairs / exp.medians (sweep_reference.expected), and every other output
+    against the rest of exp. First, where the query projects COUNT(c): the pair (c, c)'s n equals it and the median of c
+    is valid where it is > 0."""
+    meds = [c for c in query.columns if c.median]
+    m0 = len(got.names) - len(meds)  # (the median outputs come last, in column order)
+    for k, (x, _, y, _) in enumerate(query.pairs):
+        if x == y and (x, "count") in got.names:
+            n, _ = got.pair(k, "n")
+            count = got.values[got.names.index((x, "count"))]
+            bad = np.nonzero(n.ravel() != count)[0]
+            assert bad.size == 0, "%s: pair %d (%d, %d): n differs from COUNT at cells %s: the selection passes " \
+                "disagree with pass 1" % (what, k, x, x, bad[:5])
+    for k, c in enumerate(meds):
+        if (c.column_id, "count") in got.names:
+            count = got.values[got.names.index((c.column_id, "count"))]
+            bad = np.nonzero(got.validity[m0 + k] != (count > 0))[0]
+            assert bad.size == 0, "%s: median %d of %d: validity differs from COUNT > 0 at cells %s: the selection " \
+                "passes disagree with pass 1" % (what, k, c.column_id, bad[:5])
+    for k in range(len(query.pairs)):
+        check_pair(got, k, exp.pairs[k], what="%s pair %d" % (what, k))
+    for k in range(len(meds)):
+        check_median(got, m0 + k, exp.medians[k], what="%s median %d" % (what, k))
+    rest = list(range(m0 - 4 * len(query.pairs)))
+    assert got.names[:len(rest)] == exp.names[:len(rest)], what
+    check_exact(_Picked(got, rest), _Picked(exp, rest), what)
+
+
 # ---- 2. random combinations --------------------------------------------------------------------------------------------
-def run_case(engine, case, exp, monkeypatch):
-    """-> the instantiation keys the case ran. Fails with the case's description."""
+def run_case(engine, case, exp, monkeypatch, reached_operands=None):
+    """-> the instantiation keys the case ran; adds the operand kernels it launched on work to reached_operands. Fails
+    with the case's description."""
     what = case.describe()
     set_env(monkeypatch, case.env)
     pages = engine.upload_pages(case.arena, case.descs, host_resident=case.host_resident,
@@ -167,10 +210,14 @@ def run_case(engine, case, exp, monkeypatch):
             assert got == exp, "%s\nstatus %s, expected %s" % (what, got, exp)
             return {}
         assert wl is not None, "%s\nstatus %s, expected a result" % (what, got)
-        check_exact(got, exp, what)
+        if hasattr(exp, "pairs"):
+            check_operands(got, exp, case.query, what)
+            reached_operands |= sw.operand_kernels(wl, case.query, "edges" in case.extra, case.truth, case.files)
+        else:
+            check_exact(got, exp, what)
         again = engine.scan_aggregate(pages, case.query, **scan_kwargs(case.extra))
         assert_same_bytes(got, again, what)
-        return sw.kernel_keys(wl, case.descs, case.query, "edges" in case.extra)
+        return sw.kernel_keys(wl, case.descs, sw.scan_query(case.query), "edges" in case.extra)
     finally:
         pages.close()
 
@@ -189,3 +236,88 @@ def test_random_combinations(engine, monkeypatch):
     print("\nrandom combinations: %d cases, outcomes %s, %d of %d instantiations reached, short bins %s; not reached: %s" % (
         len(indices), statuses, len(reached), len(sw.INSTANTIATIONS), short,
         [sw.key_name(k) for k in sw.INSTANTIATIONS if k not in reached]))
+
+
+# ---- 3. random combinations with pairs and medians -------------------------------------------------------------------
+OPERANDS_REACHED = set()  # the operand kernels tests 3 and 4 launched on work
+OPERAND_TESTS_RUN = set()  # tests 3 (every case) and 4 when they ran to the end in this session
+
+
+def test_random_operand_combinations(engine, monkeypatch):
+    indices = [int(ONE_CASE)] if ONE_CASE is not None else range(N_OPERAND)
+    statuses, n_pairs, n_meds = {}, 0, 0
+    for i in indices:
+        case = sw.random_operand_case(i, BASE_SEED)
+        exp = sw.case_expected(case)
+        outcome = exp if isinstance(exp, (int, str)) else "result"
+        statuses[outcome] = statuses.get(outcome, 0) + 1
+        n_pairs += len(case.query.pairs)
+        n_meds += len([c for c in case.query.columns if c.median])
+        run_case(engine, case, exp, monkeypatch, OPERANDS_REACHED)
+    if ONE_CASE is None:
+        OPERAND_TESTS_RUN.add("random")
+    print("\nrandom operand combinations: %d cases, %d pairs, %d medians, outcomes %s; operand kernels reached: %s" % (
+        len(indices), n_pairs, n_meds, statuses, sorted(OPERANDS_REACHED)))
+
+
+# ---- 4. operands in every bin ----------------------------------------------------------------------------------------
+def operand_query(truth, b, narrow, edges):
+    """targeted_query's tumbling or edge query of bin b's arena, plus a pair of every two numeric columns (x == y too)
+    and a median of every numeric column."""
+    tk, vk = divmod(sw.serial_bin(b), sw.N_VK)
+    q, extra = sw.targeted_query(truth, (sw.SCAN, tk, vk, False, narrow, edges), seed=b)
+    num = [c for c in sw.columns_of(truth) if sw.COLUMNS[c] != sw.BOOL]
+    q.pairs = [(x, sw.COLUMNS[x], y, sw.COLUMNS[y]) for i, x in enumerate(num) for y in num[i:]]
+    q.columns += [PushedAggregate(c, sw.COLUMNS[c], ["median"]) for c in num]
+    return q, extra, num
+
+
+def test_operands_in_every_bin(engine, monkeypatch):
+    set_env(monkeypatch, {"TSKV_PARTS": None, "TSKV_SMEM_TABLE_KB": None})
+    reached, buckets = set(), set()
+    for b in range(sw.N_BINS):
+        tk, vk = divmod(sw.serial_bin(b), sw.N_VK)
+        s8b = vk == sw.VK_S8B and tk != sw.TK_GEN  # (the bins whose pages the scan keeps in a narrow bucket)
+        for narrow in ((sw.NARROW_NONE, sw.NARROW_SOME, sw.NARROW_ALL) if s8b else (sw.NARROW_NONE,)):
+            arena, descs, truth = sw.bin_arena(b, narrow)
+            for edges in (False, True):
+                q, extra, num = operand_query(truth, b, narrow, edges)
+                what = "operands in bin %d narrow %d edges %s" % (b, narrow, edges)
+                exp = sw.expected(truth, q, extra)
+                assert not isinstance(exp, (int, str)), "%s: the reference refuses the case (%s)" % (what, exp)
+                pages = engine.upload_pages(arena, descs)
+                try:
+                    got, wl = prepared_run(engine, pages, q, extra)
+                finally:
+                    pages.close()
+                assert wl is not None, "%s: status %s" % (what, got)
+                # every page of every operand in bin b, in the wide or the narrow bucket as its narrow flag says
+                ids = [c.column_id for c in sw.scan_query(q).columns]
+                fill = wl["fill"].astype(np.int64).reshape(sw.N_BINS, len(ids), 2)
+                field = (descs["phys_type"] != cabi.TSKV_PT_TIME) & np.isin(descs["series_id"], q.series_ids)
+                for c in num:
+                    mine = field & (descs["column_id"] == c)
+                    nar = int(wl["page_narrow"][mine].astype(bool).sum())
+                    qc = ids.index(c)
+                    assert (wl["page_bin"][mine] == b).all() and fill[:, qc].sum() == fill[b, qc].sum(), what
+                    assert (fill[b, qc, 0], fill[b, qc, 1]) == (int(mine.sum()) - nar, nar), (what, c, fill[b, qc])
+                    if narrow == sw.NARROW_ALL:
+                        assert fill[b, qc, 0] == 0 and fill[b, qc, 1] > 0, (what, c, fill[b, qc])
+                    buckets |= {k for k in (0, 1) if fill[b, qc, k]}
+                check_operands(got, exp, q, what)
+                reached |= sw.operand_kernels(wl, q, edges)
+    assert buckets == {0, 1}, buckets
+    OPERANDS_REACHED.update(reached)
+    OPERAND_TESTS_RUN.add("bins")
+    print("\noperands in every bin: operand kernels reached: %s" % sorted(reached))
+
+
+def test_every_operand_kernel_reached():
+    """Tests 3 and 4 together launched every operand kernel on work. It reads what they recorded, so it needs both to
+    have run to the end in this session, test 3 over every case; otherwise it is skipped and says so."""
+    if OPERAND_TESTS_RUN != {"random", "bins"}:
+        pytest.skip("needs test_random_operand_combinations (every case) and test_operands_in_every_bin to run first "
+                    "in this session; ran: %s" % sorted(OPERAND_TESTS_RUN))
+    missed = [k for k in sw.OPERAND_KERNELS if k not in OPERANDS_REACHED]
+    assert not missed, "operand kernels neither operand test launched on work: %s" % missed
+    print("\noperand kernels reached: %s" % sorted(OPERANDS_REACHED))

@@ -10,8 +10,9 @@ import pytest
 
 from cnosdb_b200 import cabi, datagen
 from cnosdb_b200.engine import Engine, PushedAggregate, QueryOption, TskvError
+from tests.exact_arenas import two_file_arena
 from tests.helpers import bucket_spec, random_arena
-from tests.median_reference import exact_median_cells
+from tests.median_reference import check_median, exact_median_cells
 from tests.test_median_reference import golden_column, load_golden
 
 pytestmark = pytest.mark.gpu
@@ -49,13 +50,10 @@ def check_medians(res, truth, q, what, **kw):
     meds = [c for c in q.columns if c.median]
     assert meds
     for k, c in enumerate(meds):
-        v_e, ok_e = exact_median_cells(truth, q, c.column_id, c.phys_type, n_cells, **kw)
+        exact = exact_median_cells(truth, q, c.column_id, c.phys_type, n_cells, **kw)
         j = len(res.names) - len(meds) + k  # (the median outputs come last, in column order)
-        v, ok = res.values[j], res.validity[j]
-        np.testing.assert_array_equal(ok, ok_e, err_msg="%s median %d validity" % (what, k))
-        bad = np.nonzero(ok_e & (v != v_e))[0]
-        assert bad.size == 0, (what, k, [(int(i), hex(int(v[i])), hex(int(v_e[i]))) for i in bad[:5]])
-        assert ok_e.sum() > 0, what
+        check_median(res, j, exact, what="%s median %d" % (what, k))
+        assert exact[1].sum() > 0, what
 
 
 @pytest.mark.parametrize("kind", ["rle", "jitter", "raw"])
@@ -102,37 +100,13 @@ def test_filters_tombstones_host_resident(eng):
 
 def test_overlapping_chunk_files(eng):
     """Two overlapping chunk files per series: the selection passes run over the merged rows too."""
-    rng = np.random.default_rng(11)
-    b = datagen.ArenaBuilder()
-    files, merged = [], {}
-    for sid in range(6):
-        for f in range(2):
-            n = 120
-            ts = T0 + (np.arange(n, dtype=np.int64) + 50 * f) * STEP  # rows 50-119 of file 1 share file 2's times
-            x = rng.integers(-100, 100, n).astype(np.int64)
-            y = rng.random(n) * 10
-            xv, yv = rng.random(n) > 0.2, rng.random(n) > 0.2
-            b.add_column_group(sid, ts, [(1, I64, x, xv), (2, F64, y, yv)])
-            files.append(f + 1)
-            for i in range(n):  # the later file wins per column when it holds a value (take_last_and_merge)
-                row = merged.setdefault((sid, int(ts[i])), {})
-                if xv[i]:
-                    row[1] = x[i]
-                if yv[i]:
-                    row[2] = y[i]
-    a, d = b.finish()
-    truth = {}
-    for sid in range(6):
-        tss = sorted(t for s, t in merged if s == sid)
-        cols = {c: (np.array([merged[(sid, t)].get(c, 0) for t in tss], dtype=dt), np.array([c in merged[(sid, t)] for t in tss]))
-                for c, dt in ((1, np.int64), (2, np.float64))}
-        truth[sid] = [(np.array(tss, dtype=np.int64), cols)]
+    a, d, truth, files, _ = two_file_arena(T0, STEP)
     pages = eng.upload_pages(a, d)
     try:
-        pages.set_chunk_files(np.array(files, dtype=np.uint64))
+        pages.set_chunk_files(files)
         for gbs in (True, False):
             q = grid_query(truth, columns=MEDIANS[:2], group_by_series=gbs)
-            check_medians(eng.scan_aggregate(pages, q), truth, q, "overlap gbs=%s" % gbs)
+            check_medians(eng.scan_aggregate(pages, q), truth, q, "overlap gbs=%s" % gbs, files=files)
     finally:
         pages.close()
 

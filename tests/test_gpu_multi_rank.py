@@ -14,8 +14,12 @@ unselected series, a rank with no page, reversed gather order) at N = 1, 3, 4 an
 Families: tumbling ALL aggregates on i64 / u64 / f64 / bool with NULLs, ungrouped and by series; unbucketed FIRST /
 LAST over clipped ranges on ranks whose time minima differ; ranges, predicates, tombstones and the overlap merge;
 edges with FIRST / LAST, labels, GROUP BY tags; sliding windows; M2 with COUNT and MEAN; TSKV_PARTS=3 and
-TSKV_SMEM_TABLE_KB=0. M2 arenas of their own put the between-rank term, means near 2^63, ill-conditioned cells and
-special values through k_merge_m2 at the rank count that splits their cells."""
+TSKV_SMEM_TABLE_KB=0; column pairs (covar / corr) with COUNT and MEAN. M2 arenas of their own put the between-rank term,
+means near 2^63, ill-conditioned cells and special values through k_merge_m2 at the rank count that splits their cells,
+and the same arenas put the first three through k_merge_pairs.
+M2 and pair scans refuse tskvgpu_scan_partials; their moments are held to the exact ones within a tolerance, and the
+one-rank merge of a pair's moments (Chan's formulas around the rank's own means) to them, not to the plain finalize's
+bytes."""
 import copy
 import functools
 import math
@@ -28,6 +32,7 @@ from cnosdb_b200.engine import PushedAggregate, QueryOption, TskvError
 from tests import exact_arenas as ea
 from tests.edges_reference import exact_aggregate_edges
 from tests.group_reference import exact_aggregate_grouped
+from tests.covariance_reference import check_pair, exact_pair_cells
 from tests.helpers import assert_matches_exact, bucket_spec, exact_aggregate
 from tests.labels_reference import exact_aggregate_labels
 from tests.ranks import RankScans, layouts, rank_order_mean
@@ -55,15 +60,18 @@ UNSELECTED = ALL_IDS[ALL_IDS % 6 == 5]
 # ---- families ----------------------------------------------------------------------------------------------------------
 class Family:
     """One query over one arena: ref(truth, files) is the exact reference of the query over (a shard of) the arena; with
-    m2_rtol the query holds M2 and the expected result gets its exact M2 (variance_reference.with_m2)."""
+    m2_rtol the query holds M2 and the expected result gets its exact M2 (variance_reference.with_m2); with pair_rtol it
+    holds column pairs, held to their exact co-moments (covariance_reference.exact_pair_cells)."""
 
     def __init__(self, name, arena, descs, truth, q, ref, prep=None, files=None, tombstones=None, env=None,
-                 m2_rtol=None, unselected=(), all_ids=None, n_groups=None):
+                 m2_rtol=None, unselected=(), all_ids=None, n_groups=None, pair_rtol=None):
         self.name, self.arena, self.descs, self.truth, self.ref = name, arena, descs, truth, ref
         self.q = q
         self.q.multi_rank = True
         self.prep = prep or {}
         self.files, self.tombstones, self.env, self.m2_rtol = files, tombstones, env or {}, m2_rtol
+        self.pair_rtol = pair_rtol
+        self._pairs = None
         self.unselected = unselected
         self.all_ids = np.asarray(sorted(truth) if all_ids is None else all_ids, dtype=np.uint32)
         self.n_groups = n_groups
@@ -76,6 +84,14 @@ class Family:
             run = lambda: self.ref(self.truth, self.files)  # noqa: E731
             self._exp = with_m2(run, self.q, n_groups=self.n_groups) if self.m2_rtol else run()
         return self._exp
+
+    def pairs(self):
+        """exact_pair_cells of every pair of the query."""
+        if self._pairs is None:
+            n_cells = self.expected().values.shape[1]
+            kw = dict(tombstones=self.tombstones, files=self.files)
+            self._pairs = [exact_pair_cells(self.truth, self.q, p, n_cells, **kw) for p in self.q.pairs]
+        return self._pairs
 
     def shard_ref(self, ids):
         """The exact reference over one shard's series (for its exact integer sums)."""
@@ -140,7 +156,8 @@ def _plain_ref(q):
 
 
 FAMILIES = ("tumbling", "tumbling_by_series", "unbucketed_first_last", "filters", "edges", "labels", "tags", "sliding",
-            "m2", "m2_by_series", "parts3", "smem0", "smem0_m2")
+            "m2", "m2_by_series", "parts3", "smem0", "smem0_m2", "pairs")
+PAIRS = [(1, I64, 2, F64), (2, F64, 3, U64), (3, U64, 3, U64), (2, F64, 1, I64)]
 
 
 @functools.lru_cache(maxsize=None)
@@ -159,6 +176,11 @@ def family(name):
         unselected = np.setdiff1d(np.array(sorted(truth), dtype=np.uint32), sub)
         return Family(name, arena, descs, truth, q, lambda t, f: exact_aggregate(t, q, tombstones=tombs, files=f),
                       files=files, tombstones=tombs, unselected=unselected)
+    if name == "pairs":
+        arena, descs, truth = m2_arena()
+        q = QueryOption([PushedAggregate(c, pt, ("count", "mean")) for c, pt in NUM], series_ids=SELECTED, pairs=PAIRS,
+                        **_grid(truth, 23_000))
+        return Family(name, arena, descs, truth, q, _plain_ref(q), unselected=UNSELECTED, pair_rtol=1e-9)
     if name.startswith("m2") or name == "smem0_m2":
         arena, descs, truth = m2_arena()
         gbs = name == "m2_by_series"
@@ -208,11 +230,18 @@ def _m2_col(res, j):
     return res.names[j][1] == "m2"
 
 
-def assert_identical(a, b, what, nan_equal=False):
-    """Byte for byte (nan_equal: an M2 cell that is NaN in both matches whatever its payload)."""
+def _pair_moment(res, j):
+    return res.names[j][1] in ("c", "m2x", "m2y")
+
+
+def assert_identical(a, b, what, nan_equal=False, pair_moments=True):
+    """Byte for byte (nan_equal: an M2 cell that is NaN in both matches whatever its payload; pair_moments=False leaves
+    out the pairs' C, M2x and M2y)."""
     assert a.names == b.names
     assert (a.validity == b.validity).all(), "%s: validity differs" % what
     for j, name in enumerate(a.names):
+        if not pair_moments and _pair_moment(a, j):
+            continue
         x, y = a.values[j], b.values[j]
         same = x == y
         if nan_equal and _m2_col(a, j):
@@ -222,7 +251,7 @@ def assert_identical(a, b, what, nan_equal=False):
 
 def _added_in_f64(res, j):
     col, agg = res.names[j]
-    return agg in ("mean", "m2") or (agg == "sum" and res.phys[col] == F64)
+    return agg in ("mean", "m2", "c", "m2x", "m2y") or (agg == "sum" and res.phys[col] == F64)
 
 
 def assert_same_but_f64_sums(a, b, what):
@@ -232,10 +261,10 @@ def assert_same_but_f64_sums(a, b, what):
             assert (a.values[j] == b.values[j]).all(), "%s: %s differs" % (what, name)
 
 
-def without_m2(res):
-    """res without its M2 outputs (assert_matches_exact compares every output it does not know bit for bit; check_m2
-    holds M2 to its tolerance)."""
-    keep = [j for j, (_, agg) in enumerate(res.names) if agg != "m2"]
+def without_moments(res):
+    """res without its M2 and pair outputs (assert_matches_exact compares every output it does not know bit for bit;
+    check_m2 holds M2 to its tolerance, check_pair the pairs)."""
+    keep = [j for j, (_, agg) in enumerate(res.names) if agg not in ("m2", "n", "c", "m2x", "m2y")]
     out = copy.copy(res)
     out.names = [res.names[j] for j in keep]
     out.values, out.validity = res.values[keep], res.validity[keep]
@@ -275,15 +304,19 @@ def check_case(engine, fam, n, layout, shards, order):
         for r, res in enumerate(ranks[1:], 1):
             assert_identical(res, ranks[0], "%s: rank %d against rank 0" % (what, r))
         got = ranks[0]
-        if fam.m2_rtol:
-            check_m2(got, exp, what, rtol=fam.m2_rtol)
-            assert_matches_exact(without_m2(got), without_m2(exp), what=what, int_mean=False)
+        if fam.m2_rtol or fam.pair_rtol:
+            if fam.m2_rtol:
+                check_m2(got, exp, what, rtol=fam.m2_rtol)
+            for k, ex in enumerate(fam.pairs() if fam.pair_rtol else []):
+                check_pair(got, k, ex, rtol=fam.pair_rtol, what="%s pair %d" % (what, k))
+            assert_matches_exact(without_moments(got), without_moments(exp), what=what, int_mean=False)
         else:
             assert_matches_exact(got, exp, what=what, int_mean=False)
         check_int_mean_pin(got, exp, [fam.shard_ref(shards[r]) for r in order], what)
         if plain is not None:
-            assert_identical(got, plain, what + ": one rank against the plain finalize", nan_equal=True)
-        if fam.m2_rtol:
+            assert_identical(got, plain, what + ": one rank against the plain finalize", nan_equal=True,
+                             pair_moments=not fam.pair_rtol)
+        if fam.m2_rtol or fam.pair_rtol:
             with pytest.raises(TskvError) as e:
                 rs.scans[0].partials()
             assert e.value.status == cabi.TSKV_ERR_UNSUPPORTED
@@ -446,3 +479,58 @@ def test_m2_special_values_and_small_cells(engine, monkeypatch):
             v, ok = got.column(col, "var_samp")
             x = [float(truth[s][0][1][col][0][-1]) for s in range(8)]
             assert ok[0, 4] and abs(v[0, 4] - exact_m2(x) / 7) <= 1e-9 * exact_m2(x) / 7, (col, v[0, 4])
+
+
+# ---- column pairs through k_merge_pairs on the M2 arenas -------------------------------------------------------------
+def pair_family(name, arena, descs, truth, width, fields, pairs, rtol, gbs=False):
+    q = QueryOption([PushedAggregate(c, pt, ("count",)) for c, pt in fields],
+                    series_ids=np.array(sorted(truth), np.uint32), group_by_series=gbs, pairs=pairs,
+                    **_grid(truth, width))
+    return Family(name, arena, descs, truth, q, _plain_ref(q), pair_rtol=rtol)
+
+
+@pytest.mark.parametrize("kind,n,layout", [("steps", 8, "contiguous"), ("alternating", 4, "mod")])
+def test_pairs_far_apart_means(engine, kind, n, layout, monkeypatch):
+    """The between-rank terms n_r (mx_r - mx)(my_r - my) dominate C, M2x and M2y."""
+    fields = ((1, I64), (2, F64))
+
+    def values(rng, r, sid, m, pt):
+        x = far_apart_values(rng, r if kind == "steps" else sid % 2, m, kind)
+        return np.round(x).astype(np.int64) if pt == I64 else x
+    arena, descs, truth = rank_arena(8, 3, 120, values, fields)
+    pairs = [(1, I64, 2, F64), (2, F64, 2, F64), (2, F64, 1, I64)]
+    for gbs in (False, True):
+        fam = pair_family("pairs far apart %s gbs=%s" % (kind, gbs), arena, descs, truth, 30_000, fields, pairs, 1e-9,
+                          gbs)
+        run_family(engine, fam, n, monkeypatch, only=(layout,))
+        run_family(engine, fam, 1, monkeypatch)
+        if not gbs:  # the spread between ranks is what C holds
+            n_e, c_e, _, _ = fam.pairs()[0]
+            assert (n_e > 0).any() and np.abs(c_e[n_e > 0]).max() > 1e12
+
+
+@pytest.mark.parametrize("gbs", [False, True])
+def test_pairs_means_near_2_63(engine, gbs, monkeypatch):
+    """u64 2^63 + 2048 k against i64 -2^63 + 1024 k (exact in f64); rank 0's series stop half way, so the later cells
+    take their shifts from rank 1 (and, with the "empty" layout, rank 0 holds no page)."""
+    fields = ((1, I64), (3, U64))
+    arena, descs, truth = rank_arena(4, 4, 200, lambda rng, r, sid, m, pt: near_2_63_values(rng, r, m, pt), fields,
+                                     first_half=(0,))
+    pairs = [(1, I64, 3, U64), (3, U64, 3, U64), (1, I64, 1, I64)]
+    fam = pair_family("pairs near 2^63 gbs=%s" % gbs, arena, descs, truth, 25_000, fields, pairs, 1e-9, gbs)
+    run_family(engine, fam, 4, monkeypatch, only=("contiguous", "empty"))
+    run_family(engine, fam, 1, monkeypatch)
+    n_e = fam.pairs()[0][0]
+    late = np.arange(n_e.size) % fam.q.n_buckets >= fam.q.n_buckets * 3 // 4
+    assert (n_e[late] > 0).any()  # later cells hold pairs, none from rank 0
+
+
+def test_pairs_ill_conditioned(engine, monkeypatch):
+    """1e9 + N(0, 1e-3) in both operands, one series per rank with 1-3 rows of each cell."""
+    fields = ((2, F64), (4, F64))
+    arena, descs, truth = rank_arena(8, 1, 400, lambda rng, r, sid, m, pt: ill_conditioned_values(rng, m), fields)
+    fam = pair_family("pairs ill-conditioned", arena, descs, truth, 2_500, fields, [(2, F64, 4, F64), (4, F64, 4, F64)],
+                      1e-6)
+    run_family(engine, fam, 8, monkeypatch, only=("contiguous", "mod", "reversed"))
+    run_family(engine, fam, 1, monkeypatch)
+

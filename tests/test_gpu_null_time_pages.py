@@ -4,7 +4,9 @@ timestamp (timestamp.rs:273-279), an all-NULL time page holds no row. Time pages
 and raw, with NULLs at row 0, across the 31 / 32 / 33 bitmap-word edges, at the last row, everywhere and at random;
 zig-zag simple8b i64 / u64, Gorilla f64, raw i64 and boolean values with NULLs on and next to the NULL-time rows.
 Every query runs GROUP BY bucket, series, tags and unbucketed, with and without FIRST / LAST; the scan's
-points_decoded and rows_in_range are checked against counts restated from the generated arrays."""
+points_decoded and rows_in_range are checked against counts restated from the generated arrays. Column pairs and
+medians, whose passes decode the same pages row by row with their own NULL-time handling, are held to their exact
+references over the rows with a valid timestamp."""
 import functools
 from types import SimpleNamespace
 
@@ -12,9 +14,11 @@ import numpy as np
 import pytest
 
 from cnosdb_b200 import cabi, datagen
-from cnosdb_b200.engine import QueryOption, TskvError
+from cnosdb_b200.engine import PushedAggregate, QueryOption, TskvError
 from oracle import pyoracle as orc
+from tests.covariance_reference import check_pair, exact_pair_cells
 from tests.helpers import assert_results_equal, bucket_spec, make_query
+from tests.median_reference import check_median, exact_median_cells
 
 pytestmark = pytest.mark.gpu
 
@@ -71,7 +75,7 @@ def null_time_arena():
     The valid rows carry the timestamps (the grid, or the grid with jitter), so an RLE page stays RLE. "all" time
     pages are empty (DK_ALLNULL: no rows), "zero" ones hold timestamps behind an all-zero bitmap (rows that all fail
     is_not_null(time), whose values are still decoded). Returns (arena, descs, truth) with truth[sid] = (timestamps,
-    time validity, {column: value validity}, whether the time page is empty)."""
+    time validity, {column: value validity}, whether the time page is empty, {column: values})."""
     rng = np.random.default_rng(31)
     b = datagen.ArenaBuilder()
     truth = {}
@@ -82,7 +86,7 @@ def null_time_arena():
         k = np.cumsum(tv) - 1  # index of each valid row among the valid rows
         ts = T0 + (sid % 5) * 300 + k * STEP + (rng.integers(-300, 301, n) if kind == "s8b" else 0)
         ts = np.where(tv, ts, 0).astype(np.int64)
-        fl, cols = [], {}
+        fl, cols, values = [], {}, {}
         for col, pt in FIELDS:
             valid = rng.random(n) >= 0.15
             valid[~tv] = rng.random(int((~tv).sum())) < 0.5  # values on NULL-time rows, and NULLs next to them
@@ -97,9 +101,10 @@ def null_time_arena():
                 v = np.cumsum(rng.integers(-50, 51, n)).astype(np.int64)
             fl.append((col, pt, v, valid) + ((datagen.encode_raw,) if col == 4 else ()))
             cols[col] = valid
+            values[col] = v
         tvals = T0 + np.arange(n, dtype=np.int64) * STEP if pattern == "zero" else None
         add_group(b, sid, kind, ts, tv, fl, tvals)
-        truth[sid] = (ts, tv, cols, pattern == "all")
+        truth[sid] = (ts, tv, cols, pattern == "all", values)
     arena, descs = b.finish()
     return arena, descs, truth
 
@@ -120,7 +125,7 @@ def expected_counts(truth, q, sel):
     """(points_decoded, rows_in_range) restated from the arrays; queries without predicates or tombstones."""
     points = rows = 0
     for sid in sel:
-        ts, tv, cols, empty = truth[int(sid)]
+        ts, tv, cols, empty, _ = truth[int(sid)]
         if empty:  # an empty (DK_ALLNULL) time page holds no row: nothing is decoded
             continue
         inr = tv.copy()
@@ -191,6 +196,33 @@ def test_null_time_rows_match_the_oracle(engine):
     for by, q in queries(sids):
         check(engine, pages, arena, descs, q, by, tombs, "tombstones " + by)
     pages.close()
+
+
+def test_null_time_rows_pairs_and_medians(engine):
+    """Pairs and medians over every series of the arena, by series and bucket: their passes must drop the NULL-time
+    rows (and, behind a simple8b time page with a NULL row 0, the swallowed first timestamp) as the fused scan does. The
+    exact references read the rows with a valid timestamp."""
+    arena, descs, truth = null_time_arena()
+    rows = {sid: [(ts[tv], {c: (values[c][tv], cols[c][tv]) for c, _ in FIELDS})]
+            for sid, (ts, tv, cols, _, values) in truth.items()}
+    num = [(c, pt) for c, pt in FIELDS if pt != cabi.TSKV_PT_BOOL]
+    # every numeric column is x once with the next one and once with itself (the pair passes walk x's pages)
+    pairs = [x + num[(i + 1) % len(num)] for i, x in enumerate(num)] + [x + x for x in num]
+    fbs, nb = bucket_spec(T0 - 1000, T0 + 140 * STEP, W)
+    q = QueryOption([PushedAggregate(c, pt, ["median"]) for c, pt in num],
+                    series_ids=np.array(sorted(truth), dtype=np.uint32), width=W, first_bucket_start=fbs, n_buckets=nb,
+                    group_by_series=True, pairs=pairs)
+    pages = engine.upload_pages(arena, descs)
+    try:
+        got = engine.scan_aggregate(pages, q)
+    finally:
+        pages.close()
+    n_cells = got.n_groups * got.n_buckets
+    for k, p in enumerate(pairs):
+        check_pair(got, k, exact_pair_cells(rows, q, p, n_cells), what="NULL-time rows pair %s" % (p,))
+    for k, (c, pt) in enumerate(num):
+        check_median(got, len(got.names) - len(num) + k, exact_median_cells(rows, q, c, pt, n_cells),
+                     what="NULL-time rows median of %d" % c)
 
 
 @pytest.mark.parametrize("kind", ["raw", "s8b", "s8b_row0"])
