@@ -52,6 +52,20 @@ def query_n_medians(flags):
     return (int(flags) >> 8) & 0xFF
 
 
+# increases: n_increases in bits 16..23 of tskv_query.reserved, operands after the medians' (see include/tskv_gpu.h)
+TSKV_MAX_INCREASES = 8
+
+
+def query_increases(n):
+    """TSKV_QUERY_INCREASES(n): the flags-word bits of n increases."""
+    return (int(n) & 0xFF) << 16
+
+
+def query_n_increases(flags):
+    """TSKV_QUERY_N_INCREASES(flags)."""
+    return (int(flags) >> 16) & 0xFF
+
+
 TSKV_UPLOAD_VERIFY_CRC = 1
 TSKV_UPLOAD_HOST_RESIDENT = 2
 TSKV_UPLOAD_VERIFY_ON_READ = 4

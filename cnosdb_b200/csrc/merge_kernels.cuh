@@ -87,7 +87,7 @@ __device__ __forceinline__ bool merge_row_kept_in_stream(const ScanParams &P, co
 }
 
 // (merged_row and merge_value below restate this kernel's leader test, row-level filters and take_last_and_merge rule
-// for the column pairs and the medians: a change to either rule must be made in both.)
+// for the column pairs, the medians and the increases: a change to either rule must be made in both.)
 // M2: pass 2 of TSKV_AGG_M2 over the merged rows, with the pass-2 column table (k_scan_m2): the same merged rows and cells,
 // each M2 column's value adds d = (double)x - (its cell's shift) and d^2 to sum(d) / sum(d^2); other columns are skipped.
 template <bool M2>
@@ -325,6 +325,24 @@ __global__ void __launch_bounds__(128) k_merge_median_rows(const ScanParams P, c
     median_add(mc, A, P.n_cells, run, median_ukey(v, mc.phys_type));
     median_flush(mc, A, P.n_cells, run);
   }
+}
+
+// The increases over the merged rows (k_scan_increase's pages): one thread per (merge row, increase = blockIdx.y); the
+// leader of a merged row that survives the row-level filters (merged_row) and holds a merged value of the operand
+// (merge_value) writes record rec0 + i, one point: k_increase_stitch pairs it with the point before it in its series,
+// as it pairs the pages' boundary points, so a large merge group runs one thread per row, not one per group.
+__global__ void __launch_bounds__(128) k_merge_increase(const ScanParams P, const MergeParams M, const IncreaseCol *incs, const IncreaseArgs A,
+                                                        uint32_t rec0) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  MergedRow mr;
+  if (i >= M.n_rows || !merged_row(P, M, i, mr)) return;
+  const IncreaseCol ic = incs[blockIdx.y];
+  uint64_t v;
+  if (!merge_value(P, M, ic.qcol, mr.series, mr.t, mr.s0, mr.s1, v)) return;
+  IncreaseRun run;
+  increase_begin(run);
+  increase_add(P.state, ic, run, mr.cell, mr.t, v);
+  increase_end(P.state, ic, A, blockIdx.y, rec0 + i, (uint32_t)M.cg_slot[M.mcg_cg[merge_mcg_of(M, i)]], run);
 }
 
 }  // namespace tskv

@@ -2753,6 +2753,193 @@ __global__ void k_finalize_medians(const uint64_t *state, const MedianCol *meds,
     *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
 }
 
+// ---- counter increases (TSKV_QUERY_N_INCREASES): increase(time, x) over each cell's rows in time order --------------
+// A cell holds rows of one series (prepare refuses the rest), and along a series the cells are monotone in time. Pass 1
+// (the fused scan) gives every cell's n. k_scan_increase pairs the consecutive selected rows of each page (a lane per
+// work item), adds its pairs to the cells' sums and leaves one record: its first and last selected point;
+// k_merge_increase leaves one record per merged row of the overlap merge groups. The records of a series do not overlap
+// in time: sorted by (increase, slot, first time), k_increase_stitch adds the pair across each boundary whose two points
+// share a cell. The sums are sections of the exchange region's integer / f64 sum sections.
+struct IncreaseCol {
+  uint64_t count_off;  // the operand's COUNT section (validity)
+  uint64_t off;        // the increase's sum section
+  uint32_t qcol;       // the operand's column in the scan's column table (its work-list buckets, its merged values)
+  uint16_t column_id;
+  uint8_t phys_type;
+  uint8_t pad;
+};
+// The records of every increase: [n_increases][n_rec] (the operand's work items, bucket by bucket from rec0, then the
+// merge rows). A record's sort keys are (increase << slot_bits | slot), ~0 when it holds no point, and its first
+// point's time - t_base, clamped to t_mask (the page set's time span: the time sort reads only its bits).
+struct IncreaseArgs {
+  ulonglong4 *rec;        // first cell, last cell, first value, last value
+  uint64_t *slot_key;
+  uint64_t *time_key;
+  const uint32_t *rec0;   // [n_increases][N_BINS * WL_SUB]: the record of the first item of each of the operand's buckets
+  int64_t t_base;
+  uint64_t t_mask;
+  uint32_t n_rec, slot_bits;
+};
+
+// The contribution of value v after prev: v > prev adds v - prev, v < prev adds v (a reset), equal adds nothing, in the
+// type's order (f64: totalOrder); integers wrap
+__device__ __forceinline__ uint64_t increase_step(uint64_t prev, uint64_t v, uint8_t pt) {
+  const int64_t kp = okey(prev, pt), kv = okey(v, pt);
+  if (kv == kp) return 0;  // (+0.0 for f64)
+  if (pt != TSKV_PT_F64) return kv > kp ? v - prev : v;
+  const double x = __longlong_as_double((long long)v), y = __longlong_as_double((long long)prev);
+  return (uint64_t)__double_as_longlong(kv > kp ? x - y : x);
+}
+__device__ __forceinline__ void increase_flush(uint64_t *state, const IncreaseCol &ic, uint64_t cell, uint64_t acc) {
+  if (ic.phys_type == TSKV_PT_F64) atomicAdd(reinterpret_cast<double *>(state + ic.off + cell), __longlong_as_double((long long)acc));
+  else atomicAdd(reinterpret_cast<unsigned long long *>(state + ic.off + cell), (unsigned long long)acc);
+}
+
+// One lane's walk over selected points in time order: the run of pairs in the current cell, and the record's points.
+struct IncreaseRun {
+  uint64_t first_cell, first_v, cell, v, acc;
+  int64_t first_t;
+  bool have, pairs;
+};
+__device__ __forceinline__ void increase_begin(IncreaseRun &r) {
+  r.have = r.pairs = false;
+  r.first_cell = r.first_v = r.cell = r.v = r.acc = 0;
+  r.first_t = 0;
+}
+__device__ __forceinline__ void increase_add(uint64_t *state, const IncreaseCol &ic, IncreaseRun &r, uint64_t cell, int64_t t, uint64_t v) {
+  if (!r.have) {
+    r.first_cell = cell;
+    r.first_v = v;
+    r.first_t = t;
+    r.have = true;
+  } else if (cell == r.cell) {
+    const uint64_t d = increase_step(r.v, v, ic.phys_type);
+    r.acc = ic.phys_type == TSKV_PT_F64 ? (uint64_t)__double_as_longlong(__longlong_as_double((long long)r.acc) + __longlong_as_double((long long)d))
+                                        : r.acc + d;
+    r.pairs = true;
+  } else {
+    if (r.pairs) increase_flush(state, ic, r.cell, r.acc);
+    r.acc = 0;
+    r.pairs = false;
+  }
+  r.cell = cell;
+  r.v = v;
+}
+// Flushes the last run and writes record `k` of increase `inc` (slot: the points' series slot).
+__device__ __forceinline__ void increase_end(uint64_t *state, const IncreaseCol &ic, const IncreaseArgs &A, uint32_t inc, uint64_t k,
+                                             uint32_t slot, const IncreaseRun &r) {
+  if (r.pairs) increase_flush(state, ic, r.cell, r.acc);
+  const uint64_t i = (uint64_t)inc * A.n_rec + k;
+  if (!r.have) return;  // (the slot keys start at ~0)
+  A.rec[i] = make_ulonglong4(r.first_cell, r.cell, r.first_v, r.v);
+  A.slot_key[i] = ((uint64_t)inc << A.slot_bits) | slot;
+  const uint64_t dt = (uint64_t)r.first_t - (uint64_t)A.t_base;
+  A.time_key[i] = r.first_t < A.t_base ? 0 : min(dt, A.t_mask);
+}
+
+// One page of an increase's operand (work item `item` of its buckets), decoded with its group's time page row by row and
+// selected as the medians select (select_row). Decode errors are pass 1's to report: the lane stops at the first.
+template <bool EDGES>
+__device__ __forceinline__ void increase_page(const ScanParams &P, const IncreaseCol &ic, const IncreaseArgs &A, uint32_t inc,
+                                              uint32_t item, uint32_t rec) {
+  const uint32_t page = P.work_page[item], slot = P.work_slot[item];
+  const tskv_page_desc vd = P.descs[page];
+  const uint32_t tpage = P.time_page_of[page];
+  const tskv_page_desc td = P.descs[tpage];
+  IncreaseRun run;
+  increase_begin(run);
+  if (vd.phys_type != ic.phys_type || kind_status(vd.reserved) != TSKV_OK || kind_status(td.reserved) != TSKV_OK ||
+      td.reserved == DK_ALLNULL || vd.reserved == DK_ALLNULL)
+    return;
+  PageView tpv, vpv;
+  tpv.open(P.arena, td);
+  vpv.open(P.arena, vd);
+  BitCursor tb, vb;
+  tb.init(tpv.bitset);
+  vb.init(vpv.bitset);
+  DeltaCursor<-1> tc;
+  AnyCursor<> vc;
+  if (tc.open(tpv, td.reserved) != TSKV_OK || vc.open(vpv, vd.reserved) != TSKV_OK) return;
+  const uint4 none = make_uint4(0, 0, 0, 0);
+  const uint4 tv4 = P.has_tomb ? tomb_lookup(P, vd.series_id, ic.column_id) : none;
+  const uint32_t *keepw = P.row_keep ? P.row_keep + P.keep_off[tpage] : nullptr;
+  const uint64_t group_base = group_cell_base<EDGES>(P, slot);
+  BucketState bk; bk.valid = false; bk.floor_regime = false; bk.lo = 0; bk.hi = 0; bk.idx = 0;
+  int64_t t = 0;
+  const uint32_t n_rows = vd.num_values;
+  for (uint32_t r = 0; r < n_rows; r++) {
+    const bool tv = tb.next(r), vv = vb.next(r);
+    uint64_t v = 0;
+    if (tv) { t = (int64_t)tc.next(); if (tc.exhausted) break; }
+    else if (r == 0) tc.skip_first_if_s8b_sc();
+    if (vv) { v = vc.next(); if (vc.failed()) break; }
+    else if (r == 0 && !vc.is_gorilla) vc.d.skip_first_if_s8b_sc();
+    uint64_t cell;
+    if (!(tv && vv) || !select_row<EDGES>(P, keepw, r, t, tv4, none, group_base, bk, cell)) continue;
+    increase_add(P.state, ic, run, cell, t, v);
+  }
+  increase_end(P.state, ic, A, inc, rec, slot, run);
+}
+
+// The pages of the increases (blockIdx.y: the increase): one lane per work item of the operand's buckets (every bin,
+// wide and narrow), the items pass 1 read; item i of a bucket is record rec0 + i.
+template <bool EDGES>
+__global__ void __launch_bounds__(128) k_scan_increase(const __grid_constant__ ScanParams P, const IncreaseCol *incs, const IncreaseArgs A) {
+  const IncreaseCol ic = incs[blockIdx.y];
+  const uint32_t stride = gridDim.x * blockDim.x, t0 = blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t b = 0; b < N_BINS; b++)
+    for (uint32_t sub = 0; sub < WL_SUB; sub++) {
+      const uint32_t k = (b * P.n_cols + ic.qcol) * WL_SUB + sub;
+      const uint32_t start = __ldg(P.region_start + k), fill = __ldg(P.region_fill + k);
+      const uint32_t r0 = __ldg(A.rec0 + (blockIdx.y * N_BINS + b) * WL_SUB + sub);
+      for (uint32_t i = t0; i < fill; i += stride) increase_page<EDGES>(P, ic, A, blockIdx.y, start + i, r0 + i);
+    }
+}
+
+// Before the record kernels: every record empty, and the identity permutation the sorts start from.
+__global__ void k_increase_init(const IncreaseArgs A, uint64_t n, uint32_t *idx) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    A.slot_key[i] = ~0ull;
+    A.time_key[i] = 0;
+    idx[i] = (uint32_t)i;
+  }
+}
+
+// Between the two sorts: the slot keys in time order (out[j] = key[idx[j]]).
+__global__ void k_increase_gather(const uint64_t *key, const uint32_t *idx, uint64_t n, uint64_t *out) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) out[j] = key[idx[j]];
+}
+
+// After the sorts (records in (increase, slot, first time) order, empty ones last): each record whose predecessor holds
+// the same increase and slot, and whose first point lies in the predecessor's last cell, adds that pair to the cell.
+__global__ void k_increase_stitch(uint64_t *state, const IncreaseCol *incs, const IncreaseArgs A, const uint64_t *slot_sorted,
+                                  const uint32_t *idx, uint64_t n) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x + 1; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t key = slot_sorted[j];
+    if (key == ~0ull || slot_sorted[j - 1] != key) continue;
+    const ulonglong4 a = A.rec[idx[j - 1]], b = A.rec[idx[j]];
+    if (a.y != b.x) continue;
+    const IncreaseCol ic = incs[key >> A.slot_bits];
+    increase_flush(state, ic, b.x, increase_step(a.w, b.z, ic.phys_type));
+  }
+}
+
+// The increase outputs (blockIdx.y: the increase; output column out0 + blockIdx.y), in the operand's type, valid iff the
+// cell holds a value of the operand.
+__global__ void k_finalize_increases(const uint64_t *state, const IncreaseCol *incs, uint32_t out0, uint64_t n_cells, uint64_t bitmap_stride,
+                                     uint64_t *values, uint8_t *validity) {
+  const IncreaseCol ic = incs[blockIdx.y];
+  const uint64_t cell = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  bool valid = false;
+  if (cell < n_cells) {
+    valid = state[ic.count_off + cell] > 0;
+    values[(uint64_t)(out0 + blockIdx.y) * n_cells + cell] = valid ? state[ic.off + cell] : 0;
+  }
+  const uint32_t bits = __ballot_sync(FULL, valid);
+  if ((threadIdx.x & 31) == 0 && (cell >> 3) < bitmap_stride)
+    *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
+}
+
 // Per output column: which state arrays feed it.
 struct OutCol {
   uint64_t count_off;  // counts of the source column

@@ -15,6 +15,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include <cub/device/device_radix_sort.cuh>
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <nccl.h>  // types and enums only: the library is loaded with dlopen on first use
@@ -264,6 +265,19 @@ struct tskv_scan {
   async_ptr<uint64_t> d_med_state;
   async_ptr<uint32_t> d_med_hist;
   MedianArgs med{};
+  // increases (TSKV_QUERY_N_INCREASES; k_scan_increase): their operands, records (IncreaseArgs: n_rec per increase, the
+  // operand's work items then the merge rows), the sorts' key and index buffers and scratch
+  uint32_t n_increases = 0;
+  uint64_t n_inc_merge_rows = 0;
+  int inc_time_sort_bits = 64, inc_slot_sort_bits = 64;  // the key bits each sort reads
+  async_ptr<IncreaseCol> d_increases;
+  async_ptr<uint32_t> d_inc_rec0;      // IncreaseArgs::rec0
+  async_ptr<ulonglong4> d_inc_rec;
+  async_ptr<uint64_t> d_inc_keys;  // slot keys, time keys, sorted time keys, slot keys in time order, sorted slot keys
+  async_ptr<uint32_t> d_inc_idx;   // identity, after the time sort, after the slot sort
+  async_ptr<uint8_t> d_inc_tmp;
+  size_t inc_tmp_bytes = 0;
+  IncreaseArgs inc{};
 };
 
 namespace {
@@ -351,16 +365,19 @@ bool query_has_m2(const tskv_query *q) {
 }
 
 uint32_t query_n_medians(const tskv_query *q) { return TSKV_QUERY_N_MEDIANS(q->reserved); }
+uint32_t query_n_increases(const tskv_query *q) { return TSKV_QUERY_N_INCREASES(q->reserved); }
 
-// The query the scan runs for a query with column pairs or medians: its projected columns, then every operand that is
+// The query the scan runs for a query with column pairs, medians or increases: its projected columns, then every operand that is
 // not one of them as a COUNT column without output (so that the work list, the page gathers, CRC checks, pass 1 and the
-// reader counters treat the operands' pages as they treat a COUNT column's), and per pair and median the operands'
-// places in that table. A median's operand column also computes MIN and MAX in pass 1 (its extreme keys).
+// reader counters treat the operands' pages as they treat a COUNT column's), and per pair, median and increase the
+// operands' places in that table. A median's operand column also computes MIN and MAX in pass 1 (its extreme keys); an increase's
+// operand column computes COUNT (its validity).
 struct OperandQuery {
   tskv_query q{};
   std::vector<tskv_agg_column> cols;
-  std::vector<PairCol> pairs;      // (off is set by plan_layout)
-  std::vector<MedianCol> medians;  // (the offsets are set by plan_layout)
+  std::vector<PairCol> pairs;          // (off is set by plan_layout)
+  std::vector<MedianCol> medians;      // (the offsets are set by plan_layout)
+  std::vector<IncreaseCol> increases;  // (the offsets are set by plan_layout)
 };
 OperandQuery plan_operand_query(const tskv_query *q) {
   OperandQuery pq;
@@ -391,6 +408,15 @@ OperandQuery plan_operand_query(const tskv_query *q) {
     mc.column_id = op.column_id;
     mc.phys_type = op.phys_type;
     pq.medians.push_back(mc);
+  }
+  for (uint32_t k = 0; k < query_n_increases(q); k++) {
+    const tskv_agg_column &op = q->columns[q->n_columns + 2 * q->n_pairs + query_n_medians(q) + k];
+    IncreaseCol ic{};
+    ic.qcol = place(op);
+    pq.cols[ic.qcol].agg_mask |= TSKV_AGG_COUNT;
+    ic.column_id = op.column_id;
+    ic.phys_type = op.phys_type;
+    pq.increases.push_back(ic);
   }
   pq.q.columns = pq.cols.data();
   pq.q.n_columns = (uint32_t)pq.cols.size();
@@ -559,7 +585,8 @@ bool labels_first_last(const tskv_query *q, const BucketEdges &E) {
 
 // (an edge scan's buckets come from its edge table, width = 0)
 bool query_shape_ok(const tskv_query *q, bool edges = false) {
-  return q->n_buckets != 0 && (q->n_columns != 0 || q->n_pairs != 0 || query_n_medians(q) != 0) && q->columns &&
+  return q->n_buckets != 0 &&
+         (q->n_columns != 0 || q->n_pairs != 0 || query_n_medians(q) != 0 || query_n_increases(q) != 0) && q->columns &&
          (q->width > 0 || q->n_buckets == 1 || edges);
 }
 
@@ -570,6 +597,7 @@ tskv_output_layout output_layout(const tskv_pages *pages, const tskv_query *q, c
   for (uint32_t c = 0; c < q->n_columns; c++) n_out += popc8(q->columns[c].agg_mask);
   if (q->n_pairs <= TSKV_MAX_PAIRS) n_out += 4ull * q->n_pairs;  // n, C, M2x, M2y per pair
   if (query_n_medians(q) <= TSKV_MAX_MEDIANS) n_out += query_n_medians(q);
+  if (query_n_increases(q) <= TSKV_MAX_INCREASES) n_out += query_n_increases(q);
   uint64_t n_groups = 1;
   if (q->group_by_series) n_groups = selected_slots(pages, q);
   if (tg.on) n_groups = tg.n;
@@ -603,8 +631,10 @@ struct StatePlan {
   std::vector<int> m2_of;          // per column: its index in m2, or -1
   uint64_t m2_words = 0;           // their shift / sum(d) / sum(d^2) sections, which follow the values section
   uint64_t pair_off = 0, pair_words = 0;  // the column pairs' sections (PAIR_WORDS per pair), after the M2 ones
+  std::vector<uint64_t> inc_off;          // per increase: its sum section, after the integer / the f64 sums
 };
-StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
+// incs: the increases (plan_operand_query's), whose sums the exchange region's sum sections hold
+StatePlan plan_state(const tskv_query *q, uint64_t n_cells, const std::vector<IncreaseCol> &incs = {}) {
   StatePlan plan;
   plan.cols.resize(q->n_columns);
   plan.msum_off.assign(q->n_columns, 0);
@@ -627,6 +657,12 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
       off += n_cells;
     }
   }
+  plan.inc_off.assign(incs.size(), 0);
+  for (size_t k = 0; k < incs.size(); k++)
+    if (incs[k].phys_type != TSKV_PT_F64) {
+      plan.inc_off[k] = off;
+      off += n_cells;
+    }
   sl.sum_i64_len = off - sl.sum_i64_off;
   sl.sum_f64_off = off;
   for (uint32_t c = 0; c < q->n_columns; c++)
@@ -637,6 +673,11 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells) {
   for (uint32_t c = 0; c < q->n_columns; c++)
     if ((kernel_mask(q->columns[c].agg_mask) & TSKV_AGG_MEAN) && q->columns[c].phys_type != TSKV_PT_F64) {
       msum_off[c] = off;  // exported exact integer sum as f64 (all-reducible)
+      off += n_cells;
+    }
+  for (size_t k = 0; k < incs.size(); k++)
+    if (incs[k].phys_type == TSKV_PT_F64) {
+      plan.inc_off[k] = off;
       off += n_cells;
     }
   sl.sum_f64_len = off - sl.sum_f64_off;
@@ -867,6 +908,23 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
         return TSKV_ERR_INVALID_ARG;
       }
   }
+  const uint32_t n_inc = query_n_increases(q);
+  if (n_inc > TSKV_MAX_INCREASES || (uint64_t)q->n_columns + 2ull * q->n_pairs + n_med + n_inc > 126) {
+    ctx->set_error("invalid query: at most 8 increases and 126 columns with the pairs', medians' and increases' operands");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  for (uint32_t k = 2 * q->n_pairs + n_med; k < 2 * q->n_pairs + n_med + n_inc; k++) {
+    const tskv_agg_column &op = q->columns[q->n_columns + k];
+    if (op.agg_mask != 0 || op.phys_type < TSKV_PT_I64 || op.phys_type > TSKV_PT_F64) {
+      ctx->set_error("invalid increase operand: an I64 / U64 / F64 column with agg_mask 0");
+      return TSKV_ERR_INVALID_ARG;
+    }
+    for (uint32_t c = 0; c < q->n_columns + k; c++)
+      if (q->columns[c].column_id == op.column_id && q->columns[c].phys_type != op.phys_type) {
+        ctx->set_error("increase operand: one column id with two types");
+        return TSKV_ERR_INVALID_ARG;
+      }
+  }
   if (q->n_predicates > TSKV_MAX_PREDICATES || (q->n_predicates && !q->predicates)) {
     ctx->set_error("invalid query: at most 8 field predicates");
     return TSKV_ERR_INVALID_ARG;
@@ -925,6 +983,27 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
   if (n_med && (q->reserved & TSKV_QUERY_MULTI_RANK)) {
     ctx->set_error("multi-rank scan: medians are not pushed down (their selection state does not merge across ranks)");
     return TSKV_ERR_UNSUPPORTED;
+  }
+  if (n_inc) {  // increases pair consecutive rows of one series: a cell must never hold two selected series
+    const char *why = nullptr;
+    if (slide) why = "sliding windows: increases are not pushed down";
+    else if (E.labelled) why = "bucket labels: increases are not pushed down (date_part cells are not monotone in time)";
+    else if (tg.on) {
+      std::vector<uint8_t> seen(tg.n, 0);
+      const uint64_t n_slots = selected_slots(pages, q);
+      for (uint64_t i = 0; i < n_slots && !why; i++)
+        if (seen[tg.ids[i]]++) why = "increase: a tag group holds two selected series (a cell must hold one series)";
+    } else if (!q->group_by_series) {
+      // (a multi-rank scan decides from the query alone, so that every rank agrees: without series_ids each rank would
+      // count only its own series, and the exchange would sum several series' increases into one cell)
+      if (q->series_ids ? q->n_series > 1 : (q->reserved & TSKV_QUERY_MULTI_RANK) || pages->series.size() > 1)
+        why = "increase: an ungrouped scan over more than one selected series, or a multi-rank one without series_ids "
+              "(a cell must hold one series)";
+    }
+    if (why) {
+      ctx->set_error(why);
+      return TSKV_ERR_UNSUPPORTED;
+    }
   }
   for (uint32_t m = 0; m < n_med; m++) {  // the histograms count a cell's keys in 32 bits
     const uint16_t id = q->columns[q->n_columns + 2 * q->n_pairs + m].column_id;
@@ -999,6 +1078,7 @@ struct ScanLayout {
   std::vector<PairCol> pairs;  // column pairs, with their state offsets
   uint64_t pair_words = 0;
   std::vector<MedianCol> medians;  // medians, with their operands' pass-1 sections and their selection state's offsets
+  std::vector<IncreaseCol> increases;  // increases, with their operands' COUNT sections and their sum sections
 };
 
 // n_cells: cells of the query's grid (a sliding scan: windows); kern_cells: cells of the fused kernels' grid (panes).
@@ -1007,7 +1087,7 @@ struct ScanLayout {
 ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint64_t kern_cells, const tskv_agg_column *user_cols,
                        uint32_t n_user, const OperandQuery &oq) {
   ScanLayout out;
-  const StatePlan win = plan_state(q, n_cells);
+  const StatePlan win = plan_state(q, n_cells, oq.increases);
   const StatePlan pane = sliding ? plan_state(q, kern_cells) : StatePlan{};
   out.sl = win.sl;
   out.kern_sl = sliding ? pane.sl : win.sl;
@@ -1026,6 +1106,11 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
     mc.max_off = win.cols[mc.qcol].max_off;
     mc.off = (uint64_t)MEDIAN_WORDS * n_cells * m;
     mc.hist_off = (uint64_t)MEDIAN_BINS * n_cells * m;
+  }
+  out.increases = oq.increases;  // (sliding scans refuse increases)
+  for (size_t k = 0; k < out.increases.size(); k++) {
+    out.increases[k].count_off = win.cols[out.increases[k].qcol].count_off;
+    out.increases[k].off = win.inc_off[k];
   }
   if (sliding) {
     for (uint32_t c = 0; c < q->n_columns; c++) {
@@ -1354,6 +1439,61 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
     s->med.hist = s->d_med_hist.get();
     s->med.unresolved = reinterpret_cast<unsigned long long *>(s->d_med_state.get() + (size_t)MEDIAN_WORDS * n_cells * s->n_medians);
     *h2d += lay.medians.size() * sizeof(MedianCol);
+  }
+  s->n_increases = (uint32_t)lay.increases.size();
+  if (s->n_increases) {
+    s->n_inc_merge_rows = pages->overlap.merge_rows;
+    // records: each increase's operand items, bucket by bucket (rec0), then the merge rows
+    std::vector<uint32_t> rec0((size_t)s->n_increases * N_BINS * WL_SUB);
+    uint64_t n_items_max = 0;
+    for (uint32_t m = 0; m < s->n_increases; m++) {
+      uint64_t acc = 0;
+      for (int b = 0; b < N_BINS; b++)
+        for (uint32_t sub = 0; sub < WL_SUB; sub++) {
+          rec0[((size_t)m * N_BINS + b) * WL_SUB + sub] = (uint32_t)acc;
+          acc += capacity[(b * q->n_columns + lay.increases[m].qcol) * WL_SUB + sub];
+        }
+      n_items_max = std::max(n_items_max, acc);
+    }
+    const uint64_t n_rec = n_items_max + s->n_inc_merge_rows, n = n_rec * s->n_increases;
+    if (n >> 31) {
+      ctx->set_error("increase: more than 2^31 page and merge-row records");
+      return TSKV_ERR_UNSUPPORTED;
+    }
+    // sort keys: the slot sort reads (increase, slot) bits, and the slot field of a record never has all of its bits set,
+    // so an empty record's ~0 sorts after every other; the time sort reads the bits of the page set's time span
+    const uint64_t n_slots = selected_slots(pages, q);
+    s->inc.slot_bits = 64 - __builtin_clzll(std::max<uint64_t>(n_slots, 1));
+    s->inc_slot_sort_bits = (int)s->inc.slot_bits + (s->n_increases > 1 ? 32 - __builtin_clz(s->n_increases - 1) : 0);
+    ensure_time_bounds(ctx, pages);
+    s->inc.t_base = INT64_MIN;
+    s->inc.t_mask = ~0ull;
+    s->inc_time_sort_bits = 64;
+    if (pages->ts_min <= pages->ts_max && !(pages->ts_min == INT64_MIN && pages->ts_max == INT64_MAX)) {
+      const uint64_t span = (uint64_t)pages->ts_max - (uint64_t)pages->ts_min;
+      s->inc.t_base = pages->ts_min;
+      s->inc_time_sort_bits = span ? 64 - __builtin_clzll(span) : 1;
+      s->inc.t_mask = s->inc_time_sort_bits == 64 ? ~0ull : (1ull << s->inc_time_sort_bits) - 1;
+    }
+    size_t t1 = 0, t2 = 0;
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, t1, (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                                               (uint32_t *)nullptr, (int)n, 0, s->inc_time_sort_bits, st);
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, t2, (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                                               (uint32_t *)nullptr, (int)n, 0, s->inc_slot_sort_bits, st);
+    s->inc_tmp_bytes = std::max<size_t>(std::max(t1, t2), 1);
+    if (e == cudaSuccess) e = upload(s->d_increases, lay.increases.data(), lay.increases.size(), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_inc_rec, (size_t)std::max<uint64_t>(n, 1), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_inc_keys, (size_t)std::max<uint64_t>(5 * n, 1), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_inc_idx, (size_t)std::max<uint64_t>(3 * n, 1), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_inc_tmp, s->inc_tmp_bytes, st);
+    if (e == cudaSuccess) e = upload(s->d_inc_rec0, rec0.data(), rec0.size(), st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);  // (rec0 goes out of scope)
+    s->inc.rec = s->d_inc_rec.get();
+    s->inc.rec0 = s->d_inc_rec0.get();
+    s->inc.slot_key = s->d_inc_keys.get();
+    s->inc.time_key = s->d_inc_keys.get() + n;
+    s->inc.n_rec = (uint32_t)n_rec;
+    *h2d += lay.increases.size() * sizeof(IncreaseCol) + rec0.size() * 4;
   }
   if (e == cudaSuccess) e = stream_alloc(s->d_aux, AUX_WORDS, st);
   if (e == cudaSuccess) e = stream_alloc(s->d_values, s->layout.n_out * s->layout.n_cells, st);
@@ -2122,7 +2262,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
     ctx->set_error("median: more than 2^22 cells times medians (1 KiB of histogram per cell and median)");
     return TSKV_ERR_UNSUPPORTED;
   }
-  // column pairs and medians: from here on the scan runs the query with the operands as columns (plan_operand_query)
+  // column pairs, medians and increases: from here on the scan runs the query with the operands as columns
+  // (plan_operand_query)
   const tskv_agg_column *user_cols = q->columns;
   const uint32_t n_user = q->n_columns;
   OperandQuery pq = plan_operand_query(q);
@@ -2417,7 +2558,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     cudaStreamWaitEvent(ctx->stream.get(), ev_done, 0);  // join
     launches++;
   }
-  if (!capturing && !s->n_m2 && !s->n_pairs && !s->n_medians) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
+  if (!capturing && !s->n_m2 && !s->n_pairs && !s->n_medians && !s->n_increases) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
   if (s->n_combine) {  // sliding windows: every window folds its panes (it writes every array the kernels fill)
     const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
     k_window_combine<<<dim3(std::max(1u, bx), s->n_combine), 256, 0, ctx->stream.get()>>>(
@@ -2455,7 +2596,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       cudaStreamWaitEvent(ctx->stream.get(), s->ev_m2_join[b].get(), 0);
       launches++;
     }
-    if (!capturing && !s->n_pairs && !s->n_medians) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes pass 2)
+    if (!capturing && !s->n_pairs && !s->n_medians && !s->n_increases) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes pass 2)
   }
   if (s->n_pairs) {  // column pairs: pass 1 (n, sums, extremes), the shifts, pass 2 (co-moments); overlap merge rows first
     const bool edges = s->params.edges != nullptr;
@@ -2481,7 +2622,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       CU_TRY(ctx, cudaLaunchKernel(fn, dim3(px, s->n_pairs), dim3(128), args, 0, ctx->stream.get()));
       launches++;
     }
-    if (!capturing && !s->n_medians) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the pair passes)
+    if (!capturing && !s->n_medians && !s->n_increases) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the pair passes)
   }
   if (s->n_medians) {  // medians: the targets from pass 1, then MEDIAN_PASSES fixed selection passes (merged rows first)
     const bool edges = s->params.edges != nullptr;
@@ -2505,7 +2646,38 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       k_median_step<<<dim3(std::max(1u, wx), s->n_medians), 256, 0, ctx->stream.get()>>>(mp, s->med, n_cells);
       launches += 2;
     }
-    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the selection passes)
+    if (!capturing && !s->n_increases) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the selection passes)
+  }
+  if (s->n_increases) {  // increases: the pages' pairs and records and the merged rows' records, then the boundaries
+    const bool edges = s->params.edges != nullptr;
+    const uint64_t n = (uint64_t)s->inc.n_rec * s->n_increases;
+    const uint32_t nb = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + 255) / 256, 4096));
+    const uint32_t px = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)pages->n_descs + 127) / 128, (uint64_t)ctx->sm_count * 16));
+    uint64_t *keys = s->d_inc_keys.get();
+    uint32_t *idx = s->d_inc_idx.get();
+    const IncreaseCol *ip = s->d_increases.get();
+    k_increase_init<<<nb, 256, 0, ctx->stream.get()>>>(s->inc, n, idx);
+    const void *fn = edges ? (const void *)k_scan_increase<true> : (const void *)k_scan_increase<false>;
+    void *args[] = {(void *)&s->params, (void *)&ip, (void *)&s->inc};
+    CU_TRY(ctx, cudaLaunchKernel(fn, dim3(px, s->n_increases), dim3(128), args, 0, ctx->stream.get()));
+    launches += 2;
+    if (s->merge.n_rows && s->n_merge_pages) {
+      k_merge_increase<<<dim3((uint32_t)((s->merge.n_rows + 127) / 128), s->n_increases), 128, 0, ctx->stream.get()>>>(
+          s->params, s->merge, ip, s->inc, (uint32_t)(s->inc.n_rec - s->n_inc_merge_rows));
+      launches++;
+    }
+    // records by first time, then (stably) by (increase, slot): keys [slot | time | time sorted | slot in time order |
+    // slot sorted], indices [identity | time order | final order]; each sort reads only its keys' bits (alloc_scan)
+    size_t tmp = s->inc_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_inc_tmp.get(), tmp, keys + n, keys + 2 * n, idx, idx + n, (int)n, 0,
+                                                s->inc_time_sort_bits, ctx->stream.get()));
+    k_increase_gather<<<nb, 256, 0, ctx->stream.get()>>>(keys, idx + n, n, keys + 3 * n);
+    tmp = s->inc_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_inc_tmp.get(), tmp, keys + 3 * n, keys + 4 * n, idx + n, idx + 2 * n, (int)n, 0,
+                                                s->inc_slot_sort_bits, ctx->stream.get()));
+    k_increase_stitch<<<nb, 256, 0, ctx->stream.get()>>>(s->d_state.get(), ip, s->inc, keys + 4 * n, idx + 2 * n, n);
+    launches += 4;  // (a sort counts as one launch)
+    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the increase kernels)
   }
   if (!capturing) cudaEventRecord(s->ev1.get(), ctx->stream.get());
   CU_TRY(ctx, cudaGetLastError());
@@ -2768,6 +2940,10 @@ static tskv_status finalize_device(tskv_ctx *ctx, tskv_scan *s) {
   if (s->n_medians)
     k_finalize_medians<<<dim3((uint32_t)((L.n_cells + 255) / 256), s->n_medians), 256, 0, ctx->stream.get()>>>(
         s->d_state.get(), s->d_medians.get(), s->med, s->n_out + 4 * s->n_pairs, L.n_cells, L.bitmap_stride, s->d_values.get(),
+        s->d_validity.get());
+  if (s->n_increases)
+    k_finalize_increases<<<dim3((uint32_t)((L.n_cells + 255) / 256), s->n_increases), 256, 0, ctx->stream.get()>>>(
+        s->d_state.get(), s->d_increases.get(), s->n_out + 4 * s->n_pairs + s->n_medians, L.n_cells, L.bitmap_stride, s->d_values.get(),
         s->d_validity.get());
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;

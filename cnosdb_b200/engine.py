@@ -221,12 +221,14 @@ class TskvError(RuntimeError):
 class PushedAggregate:
     """One projected value column with its aggregate set (extends PushedAggregateFunction::Count). "median" has no mask
     bit: it makes the column a median operand (after the pairs' operands, agg_mask 0), and a column that asks for nothing
-    else has no projected entry."""
+    else has no projected entry. "increase" (increase(time, x ORDER BY time)) likewise makes it an increase operand, after
+    the medians' operands."""
 
     def __init__(self, column_id, phys_type, aggs):
         self.column_id = int(column_id)
         self.phys_type = int(phys_type)
         self.median = False
+        self.increase = False
         if isinstance(aggs, int):
             self.agg_mask = aggs
         else:
@@ -234,6 +236,9 @@ class PushedAggregate:
             for a in aggs:
                 if a == "median":
                     self.median = True
+                    continue
+                if a == "increase":
+                    self.increase = True
                     continue
                 # var* / stddev* ask the scan for COUNT | M2; ScanResult.column derives them
                 self.agg_mask |= (TSKV_AGG_COUNT | TSKV_AGG_M2) if a in STAT_AGGS else AGG_BITS[a]
@@ -277,12 +282,14 @@ class QueryOption:
         q.group_by_series = 1 if self.group_by_series else 0
         proj = self.projected()
         meds = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "median", False)]
-        q.reserved = (cabi.TSKV_QUERY_MULTI_RANK if self.multi_rank else 0) | cabi.query_medians(len(meds))
-        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))] + meds
+        incs = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "increase", False)]
+        q.reserved = ((cabi.TSKV_QUERY_MULTI_RANK if self.multi_rank else 0) | cabi.query_medians(len(meds)) |
+                      cabi.query_increases(len(incs)))
+        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))] + meds + incs
         cols = (cabi.AggColumn * max(1, len(proj) + len(ops)))()
         for i, c in enumerate(proj):
             cols[i].column_id, cols[i].phys_type, cols[i].agg_mask = c.column_id, c.phys_type, c.agg_mask
-        for i, (cid, pt) in enumerate(ops):  # the pairs' operands, then the medians', follow the projected columns
+        for i, (cid, pt) in enumerate(ops):  # the pairs', medians' and increases' operands follow the projected columns
             cols[len(proj) + i].column_id, cols[len(proj) + i].phys_type = cid, pt
         q.columns = cols
         q.n_columns = len(proj)
@@ -301,13 +308,14 @@ class QueryOption:
         return q
 
     def projected(self):
-        """The columns with a projected entry (an aggregate other than median)."""
-        return [c for c in self.columns if c.agg_mask or not getattr(c, "median", False)]
+        """The columns with a projected entry (an aggregate other than median and increase)."""
+        return [c for c in self.columns if c.agg_mask or not (getattr(c, "median", False) or getattr(c, "increase", False))]
 
     def output_names(self):
         return ([(c.column_id, cabi.AGG_NAMES[a]) for c in self.projected() for a in c.agg_list()] +
                 [(("pair", k), r) for k in range(len(self.pairs)) for r in PAIR_RAW] +
-                [(c.column_id, "median") for c in self.columns if getattr(c, "median", False)])
+                [(c.column_id, "median") for c in self.columns if getattr(c, "median", False)] +
+                [(c.column_id, "increase") for c in self.columns if getattr(c, "increase", False)])
 
 
 class ScanResult:
@@ -339,8 +347,8 @@ class ScanResult:
 
     def column(self, column_id, agg):
         """(typed values, validity) of one output column, shaped [n_groups, n_buckets]. agg may also name one of STAT_AGGS
-        (var, var_samp, var_pop, stddev, stddev_samp, stddev_pop), derived from the column's count and m2, or "median"
-        (the operand's type)."""
+        (var, var_samp, var_pop, stddev, stddev_samp, stddev_pop), derived from the column's count and m2, or "median" /
+        "increase" (the operand's type)."""
         if agg in STAT_AGGS:
             n, _ = self.column(column_id, "count")
             m2, ok = self.column(column_id, "m2")
@@ -602,6 +610,8 @@ class Engine:
                 raise ValueError("median and slide: sliding windows do not push medians down")
             if getattr(query, "multi_rank", False):
                 raise ValueError("median and multi_rank: medians have no mergeable partial state")
+        if slide is not None and any(getattr(c, "increase", False) for c in query.columns):
+            raise ValueError("increase and slide: sliding windows do not push increases down")
 
     @staticmethod
     def _edges(edges, slide):

@@ -224,6 +224,29 @@ typedef struct tskv_query {
 #define TSKV_MAX_MEDIAN_CELLS (1u << 22)
 #define TSKV_QUERY_MEDIANS(n) (((uint32_t)(n) & 0xffu) << 8)
 #define TSKV_QUERY_N_MEDIANS(flags) (((uint32_t)(flags) >> 8) & 0xffu)
+/* Counter increases: increase(time, x ORDER BY time) (CnosDB's IncreaseAccumulator). Bits 16..23 of the flags word hold
+ * n_increases: TSKV_QUERY_INCREASES(n) sets them, TSKV_QUERY_N_INCREASES(flags) reads them. The n_increases entries of
+ * `columns` after the medians' operands are the increases' operands: column_id and phys_type (I64 / U64 / F64) of each,
+ * agg_mask 0; n_columns + 2 * n_pairs + n_medians + n_increases <= 126. An increase walks a cell's selected rows (time
+ * ranges, series, the row filter of the predicates, row-drop and column tombstones, non-NULL time) in time order, NULL
+ * operand values left out; each value v after the previous one `last` adds v - last when v > last, v when v < last (a
+ * counter reset) and nothing when they are equal; the sum starts at 0. Integers subtract and sum wrapping (i64 compares
+ * signed, u64 unsigned); f64 compares by IEEE totalOrder and sums in atomic order. Per cell each increase adds one output
+ * after the medians' outputs, in the operand's type, valid iff the cell holds a value of the operand (the reference
+ * prints 0 for a group whose operand is NULL in every row). A cell must hold rows of one series only: the scan runs the
+ * operand as a COUNT column in pass 1, then one lane per page pairs consecutive rows and records the page's first and
+ * last selected points, every merged row of the overlap merge groups is a record of its own, and the records of every
+ * series, sorted by time, add the pairs across their boundaries. The increases sit in the exchange
+ * region's integer / f64 sum sections: tskvgpu_scan_partials, _exchange and _merge_gathered sum them across ranks.
+ * Refused before any launch: TSKV_ERR_INVALID_ARG for n_increases > TSKV_MAX_INCREASES, an operand with a non-zero agg_mask
+ * or a BOOL / TIME / unknown type, an operand id projected with another type, or more than 126 columns;
+ * TSKV_ERR_UNSUPPORTED for a cell that could hold rows of two selected series (an ungrouped scan over more than one
+ * selected series - series_ids NULL: the page set holds more than one; with TSKV_QUERY_MULTI_RANK, series_ids NULL at
+ * all, so that every rank decides from the query alone - or a group map with two selected slots in one group), sliding windows (slide != width) and tskvgpu_scan_prepare_labels. Counters: as for medians; kernel_launches and
+ * elapsed_fused_ms include the increase kernels. */
+#define TSKV_MAX_INCREASES 8
+#define TSKV_QUERY_INCREASES(n) (((uint32_t)(n) & 0xffu) << 16)
+#define TSKV_QUERY_N_INCREASES(flags) (((uint32_t)(flags) >> 16) & 0xffu)
 
 /* Result layout. Outputs are dense: for output column j (query columns in order, and inside a
  * column the set agg bits in ascending bit order) and cell c = group * n_buckets + bucket:

@@ -46,6 +46,16 @@ pub const fn tskv_query_medians(n: u32) -> u32 {
 pub const fn tskv_query_n_medians(flags: u32) -> u32 {
     (flags >> 8) & 0xff
 }
+/// At most this many increases; their count sits in bits 16..23 of tskv_query.reserved (see tskv_gpu.h).
+pub const TSKV_MAX_INCREASES: u32 = 8;
+/// TSKV_QUERY_INCREASES(n): the flags-word bits of n increases.
+pub const fn tskv_query_increases(n: u32) -> u32 {
+    (n & 0xff) << 16
+}
+/// TSKV_QUERY_N_INCREASES(flags): the increases of a flags word.
+pub const fn tskv_query_n_increases(flags: u32) -> u32 {
+    (flags >> 16) & 0xff
+}
 
 pub const TSKV_UPLOAD_VERIFY_CRC: u32 = 1;
 pub const TSKV_UPLOAD_HOST_RESIDENT: u32 = 2;
