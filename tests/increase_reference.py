@@ -88,6 +88,41 @@ def exact_increase_cells(truth, query, col, pt, n_cells, **kw):
     return v, ok, mag
 
 
+def increase_cells_np(cells, times, bits, pt, n_cells):
+    """The increase of every cell over selected rows given as arrays (cell index, time, u64 bit pattern per row; a cell
+    holds rows of one series, at distinct times), vectorized for page sets too large for exact_increase_cells -> the
+    same (bit patterns u64 [n_cells], validity bool [n_cells], f64 magnitudes [n_cells]). Integers sum in uint64
+    (wrapping); f64 contributions sum in row order, which check_increase's tolerance covers."""
+    cells = np.asarray(cells, dtype=np.int64)
+    bits = np.asarray(bits, dtype=np.uint64)
+    order = np.lexsort((np.asarray(times, dtype=np.int64), cells))
+    c, b = cells[order], bits[order]
+    ok = np.zeros(n_cells, dtype=bool)
+    ok[c] = True
+    v = np.zeros(n_cells, dtype=np.uint64)
+    mag = np.zeros(n_cells, dtype=np.float64)
+    pair = c[1:] == c[:-1]
+    last, cur, pc = b[:-1][pair], b[1:][pair], c[1:][pair]
+    if pt == cabi.TSKV_PT_F64:
+        neg = (1 << 63)
+        key = lambda u: np.where(u >> np.uint64(63), ~u, u | np.uint64(neg))  # noqa: E731  (totalOrder, unsigned)
+        kl, kv = key(last), key(cur)
+        x, y = cur.view(np.float64), last.view(np.float64)
+        with np.errstate(invalid="ignore", over="ignore"):
+            d = np.where(kv == kl, 0.0, np.where(kv > kl, x - y, x))
+            acc = np.zeros(n_cells, dtype=np.float64)
+            np.add.at(acc, pc, d)
+            np.add.at(mag, pc, np.abs(d))
+        return acc.view(np.uint64), ok, mag
+    if pt == cabi.TSKV_PT_I64:
+        kl, kv = last.view(np.int64), cur.view(np.int64)
+    else:
+        kl, kv = last, cur
+    d = np.where(kv == kl, np.uint64(0), np.where(kv > kl, cur - last, cur))
+    np.add.at(v, pc, d)
+    return v, ok, mag
+
+
 def check_increase(res, j, exact, pt, what=""):
     """Output j of a ScanResult, an increase, against exact_increase_cells: validity equal; integers bit for bit; f64
     NaN where the reference has NaN, +-inf equal, finite values within 1e-12 of the contributions' magnitude (the sum's

@@ -71,7 +71,8 @@ def rank_order_mean(rank_sums, n):
 
 
 class RankScans:
-    """One prepared scan per shard of `shards` (lists of series ids): the shard's descriptors uploaded as its own page set
+    """One prepared scan per shard of `shards` (lists of series ids, or boolean masks over the descriptors that keep
+    whole column groups: a series split over ranks by time): the shard's descriptors uploaded as its own page set
     (none for an empty shard), the column groups' chunk files (`files`, one per column group in descriptor order) and
     the tombstones set as on the whole arena, and `q` prepared with multi_rank=True and the same group map, edges,
     labels and slide on every rank (`prep`: Engine.prepare's keyword arguments)."""
@@ -80,13 +81,15 @@ class RankScans:
         self.engine = engine
         self.query = multi_rank(q)
         self.pages, self.scans = [], []
-        cg_series = descs["series_id"][descs["phys_type"] == cabi.TSKV_PT_TIME]
+        time_page = descs["phys_type"] == cabi.TSKV_PT_TIME
         try:
             for ids in shards:
-                pages = engine.upload_pages(arena, descs[np.isin(descs["series_id"], ids)])
+                ids = np.asarray(ids)
+                mine = ids if ids.dtype == bool else np.isin(descs["series_id"], ids)
+                pages = engine.upload_pages(arena, descs[mine])
                 self.pages.append(pages)
                 if files is not None:
-                    pages.set_chunk_files(np.asarray(files)[np.isin(cg_series, ids)])
+                    pages.set_chunk_files(np.asarray(files)[mine[time_page]])
                 if tombstones is not None:
                     pages.set_tombstones(tombstones)
                 self.scans.append(engine.prepare(pages, self.query, **prep))

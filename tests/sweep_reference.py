@@ -18,7 +18,11 @@ random_operand_case adds column pairs (covar / corr) and medians to a random cas
 co-moments (covariance_reference) and medians (median_reference) of every pair and median, or one more refusal this
 module states: a pair or a median with a sliding window (the engine's ValueError), a BOOL operand
 (TSKV_ERR_INVALID_ARG). The scan runs such a query with every operand that is not projected as a COUNT column without
-output (scan_query): the other outputs' reference is that query's."""
+output (scan_query): the other outputs' reference is that query's.
+
+random_increase_case adds counter increases (increase(time, x)) to a random case, and regroups most cases into a shape
+whose cells hold one series. Their outcome adds the exact increase of every increase (increase_reference), or the
+status of increase_status: the refusals of validate_query (cnosdb_b200/csrc/tskv_gpu.cu) in the order it checks them."""
 import copy
 
 import numpy as np
@@ -32,6 +36,7 @@ from tests.helpers import ReferenceError, bucket_spec, exact_aggregate, files_by
 from tests.labels_reference import exact_aggregate_grouped_labels, exact_aggregate_labels
 from tests.sliding_reference import expand_aggregate, sliding_status
 from tests.covariance_reference import exact_pair_cells
+from tests.increase_reference import exact_increase_cells
 from tests.median_reference import exact_median_cells
 from tests.variance_reference import with_m2
 
@@ -488,16 +493,20 @@ def random_case(index, base_seed):
 
 
 def expected(truth, query, extra, tombstones=None, files=None):
-    """The composed exact reference of one scan -> ExactResult (M2 filled in; with pairs or medians, `pairs` holds
-    exact_pair_cells of every pair and `medians` exact_median_cells of every median), or the status int the scan must
-    refuse it with, or "ValueError" (the engine refuses M2, pairs and medians with a sliding window before calling the
-    library)."""
+    """The composed exact reference of one scan -> ExactResult (M2 filled in; with pairs, medians or increases, `pairs`
+    holds exact_pair_cells of every pair, `medians` exact_median_cells of every median and `increases`
+    exact_increase_cells of every increase), or the status int the scan must refuse it with, or "ValueError" (the
+    engine refuses M2, pairs, medians and increases with a sliding window before calling the library)."""
     medians = [c for c in query.columns if c.median]
-    if query.pairs or medians:
+    incs = [c for c in query.columns if c.increase]
+    if query.pairs or medians or incs:
         if extra.get("slide") is not None:
             return "ValueError"
         if BOOL in [pt for _, pt in operands(query)]:
             return cabi.TSKV_ERR_INVALID_ARG
+        st = increase_status(truth, query, extra) if incs else None
+        if st is not None:
+            return st
         res = expected(truth, scan_query(query), extra, tombstones, files)
         if isinstance(res, (int, str)):
             return res
@@ -506,6 +515,8 @@ def expected(truth, query, extra, tombstones=None, files=None):
         n_cells = res.values.shape[1]
         res.pairs = [exact_pair_cells(truth, query, p, n_cells, **kw) for p in query.pairs]
         res.medians = [exact_median_cells(truth, query, c.column_id, c.phys_type, n_cells, **kw) for c in medians]
+        kw.pop("labels")  # (labels refuse increases)
+        res.increases = [exact_increase_cells(truth, query, c.column_id, c.phys_type, n_cells, **kw) for c in incs]
         return res
     has_m2 = any(c.agg_mask & cabi.TSKV_AGG_M2 for c in query.columns)
     has_sel = any(c.agg_mask & (cabi.TSKV_AGG_FIRST | cabi.TSKV_AGG_LAST) for c in query.columns)
@@ -546,9 +557,10 @@ def case_expected(case):
 
 # ---- random cases with column pairs and medians ----------------------------------------------------------------------
 def operands(query):
-    """(column id, type) of the pairs' operands (x0, y0, x1, ...), then the medians'."""
+    """(column id, type) of the pairs' operands (x0, y0, x1, ...), then the medians', then the increases'."""
     return [o for x, xt, y, yt in query.pairs for o in ((x, xt), (y, yt))] + \
-        [(c.column_id, c.phys_type) for c in query.columns if c.median]
+        [(c.column_id, c.phys_type) for c in query.columns if c.median] + \
+        [(c.column_id, c.phys_type) for c in query.columns if c.increase]
 
 
 def scan_query(query):
@@ -570,12 +582,13 @@ def operand_columns(query):
         [ids.index(c.column_id) for c in query.columns if c.median]
 
 
-# the kernels of the pairs' and medians' row-by-row passes: the scan and merged-row kernels of the EXPECTED sets of
-# tests/test_pair_kernel_list.py and tests/test_median_kernel_list.py, which hold those sets to the library
-# (tests/test_pair_median_sweep_reference.py checks that this list is that subset)
+# the kernels of the pairs', medians' and increases' row-by-row passes: the scan and merged-row kernels of the EXPECTED
+# sets of tests/test_pair_kernel_list.py, tests/test_median_kernel_list.py and tests/test_increase_kernel_list.py, which
+# hold those sets to the library (tests/test_pair_median_sweep_reference.py checks that this list is that subset)
 OPERAND_KERNELS = ("k_scan_pair<false, false>", "k_scan_pair<false, true>", "k_scan_pair<true, false>",
                    "k_scan_pair<true, true>", "k_merge_pairs_rows<false>", "k_merge_pairs_rows<true>",
-                   "k_scan_median<false>", "k_scan_median<true>", "k_merge_median_rows")
+                   "k_scan_median<false>", "k_scan_median<true>", "k_merge_median_rows",
+                   "k_scan_increase<false>", "k_scan_increase<true>", "k_merge_increase")
 
 
 def merged_operands(truth, query, files, ops):
@@ -595,10 +608,12 @@ def merged_operands(truth, query, files, ops):
 
 def operand_kernels(wl, query, edges, truth=None, files=None):
     """The operand kernels a pass launched with work: both passes of k_scan_pair<PASS2, EDGES> when a pair's x operand
-    has work-list items, k_scan_median<EDGES> when a median's operand has, k_merge_pairs_rows<PASS2> when a pair's x and
-    y have merged rows, and k_merge_median_rows when a median's operand has (merged_operands over `files`)."""
+    has work-list items, k_scan_median<EDGES> when a median's operand has, k_scan_increase<EDGES> when an increase's
+    operand has, k_merge_pairs_rows<PASS2> when a pair's x and y have merged rows, and k_merge_median_rows /
+    k_merge_increase when a median's / an increase's operand has (merged_operands over `files`)."""
     qpairs, qmeds = operand_columns(query)
-    fill = bin_fill(wl, len(scan_query(query).columns))
+    ids = [c.column_id for c in scan_query(query).columns]
+    fill = bin_fill(wl, len(ids))
     e = "true" if edges else "false"
     out = set()
     if any(fill[:, qx].sum() for qx, _ in qpairs):
@@ -609,6 +624,11 @@ def operand_kernels(wl, query, edges, truth=None, files=None):
         out |= {"k_merge_pairs_rows<false>", "k_merge_pairs_rows<true>"}
     if any(merged_operands(truth, query, files, (c.column_id,)) for c in query.columns if c.median):
         out.add("k_merge_median_rows")
+    incs = [c.column_id for c in query.columns if c.increase]
+    if any(fill[:, ids.index(c)].sum() for c in incs):
+        out.add("k_scan_increase<%s>" % e)
+    if any(merged_operands(truth, query, files, (c,)) for c in incs):
+        out.add("k_merge_increase")
     return out
 
 
@@ -661,4 +681,108 @@ def random_operand_case(index, base_seed):
             q.columns.append(PushedAggregate(c, COLUMNS[c], ["median"]))
     case.desc.update(pairs=[(x, y) for x, _, y, _ in pairs], medians=[c.column_id for c in q.columns if c.median],
                      operand_refusal=refusal)
+    return case
+
+
+# ---- random cases with counter increases -------------------------------------------------------------------------------
+def selected_slots(truth, query):
+    """The series a scan selects: series_ids, or else every series of the page set."""
+    return list(query.series_ids) if query.series_ids is not None else sorted(truth)
+
+
+def increase_status(truth, query, extra):
+    """The status the scan refuses a query with increases with (None: accepted), in the order the engine and
+    validate_query check (cnosdb_b200/csrc/tskv_gpu.cu, the increase checks at the end of validate_query):
+      1. a sliding window: the engine's ValueError, before the library is called;
+      2. an operand of type BOOL (a pair's, a median's or an increase's): TSKV_ERR_INVALID_ARG (the operand checks
+         come before every grouping check);
+      3. bucket labels: TSKV_ERR_UNSUPPORTED (date_part cells are not monotone in time);
+      4. a tag group map under which two selected slots share a group: TSKV_ERR_UNSUPPORTED;
+      5. no group map and no GROUP BY series over more than one selected slot ("selected": series_ids, or else every
+         series of the page set): TSKV_ERR_UNSUPPORTED.
+    A cell of an accepted query holds rows of one series."""
+    if extra.get("slide") is not None:
+        return "ValueError"
+    if BOOL in [pt for _, pt in operands(query)]:
+        return cabi.TSKV_ERR_INVALID_ARG
+    if extra.get("labels") is not None:
+        return cabi.TSKV_ERR_UNSUPPORTED
+    gids = extra.get("group_ids")
+    n_slots = len(selected_slots(truth, query))
+    if gids is not None:
+        if len(set(int(g) for g in gids[:n_slots])) < n_slots:
+            return cabi.TSKV_ERR_UNSUPPORTED
+    elif not query.group_by_series and n_slots > 1:
+        return cabi.TSKV_ERR_UNSUPPORTED
+    return None
+
+
+INC_SHAPES = ("series", "tags", "edges", "one")
+
+
+def random_increase_case(index, base_seed):
+    """random_case(index, base_seed) with 1-4 increases drawn from a stream of their own (random_case's draws are
+    unchanged): increases of numeric columns, duplicates and unprojected columns among them, sometimes with a pair or a
+    median. With probability 0.7 the case is regrouped into a shape whose cells hold one series (INC_SHAPES: GROUP BY
+    series; a tag map of one selected series per group; edges with GROUP BY series; one selected series, bucketed or
+    not); otherwise it keeps random_case's grouping and increase_status says whether the scan refuses it. A case that
+    random_case makes a refusal gets no increase; a few cases turn one increase into a BOOL operand (refused)."""
+    case = random_case(index, base_seed)
+    rng = np.random.default_rng([base_seed, index, 2])
+    q = case.query
+    have = columns_of(case.truth)
+    num = [c for c in have if COLUMNS[c] != BOOL]
+    if case.desc["refusal"] != "none" or not num:
+        case.desc.update(increases=[], shape="kept", increase_refusal="none")
+        return case
+    incs = [int(rng.choice(num)) for _ in range(int(rng.integers(1, 5)))]
+    if len(incs) > 1 and rng.random() < 0.3:
+        incs[-1] = incs[0]  # (a duplicate)
+    bool_op = BOOL in [COLUMNS[c] for c in have] and rng.random() < 0.05
+    if bool_op:
+        incs[int(rng.integers(0, len(incs)))] = 4
+    if rng.random() < 0.25:
+        x, y = int(rng.choice(num)), int(rng.choice(num))
+        q.pairs = [(x, COLUMNS[x], y, COLUMNS[y])]
+    if rng.random() < 0.25:
+        c = int(rng.choice(num))
+        q.columns.append(PushedAggregate(c, COLUMNS[c], ["median"]))
+    for c in incs:
+        entry = [e for e in q.columns if e.column_id == c and e.agg_mask and not e.increase]
+        if entry and rng.random() < 0.5:
+            entry[0].increase = True  # the projected entry asks for the increase as well
+        else:
+            q.columns.append(PushedAggregate(c, COLUMNS[c], ["increase"]))
+    shape = str(rng.choice(INC_SHAPES)) if rng.random() < 0.7 else "kept"
+    if shape != "kept":
+        lo, hi = span(case.truth)
+        step = case.desc["step"]
+        for k in ("slide", "edges", "labels", "group_ids", "n_groups"):
+            case.extra.pop(k, None)
+        w = int(rng.choice([37, 100, 1000])) * step
+        origin = int(rng.integers(-w, w))
+        fbs, nb = bucket_spec(lo, hi, w, origin)
+        q.width, q.origin, q.first_bucket_start, q.n_buckets, q.group_by_series = w, origin, fbs, nb, False
+        sids = sorted(case.truth)
+        if shape == "series":
+            q.group_by_series = True
+        elif shape == "tags":
+            n_slots = len(selected_slots(case.truth, q))
+            n_groups = n_slots + int(rng.integers(0, 3))
+            case.extra["n_groups"] = n_groups
+            case.extra["group_ids"] = rng.permutation(n_groups)[:n_slots].astype(np.uint32)
+        elif shape == "edges":
+            e = random_edges(rng, lo, hi, int(rng.integers(1, 60)))
+            case.extra["edges"] = e
+            q.width, q.origin, q.first_bucket_start, q.n_buckets, q.group_by_series = 0, 0, 0, e.size - 1, True
+        else:
+            q.series_ids = np.array([sids[int(rng.integers(0, len(sids)))]], dtype=np.uint32)
+            if rng.random() < 0.5:
+                q.width, q.origin, q.first_bucket_start, q.n_buckets = 0, 0, 0, 1
+        q._keep = None
+    case.desc.update(increases=incs, shape=shape, increase_refusal="bool_increase" if bool_op else "none",
+                     pairs=[(x, y) for x, _, y, _ in q.pairs], medians=[c.column_id for c in q.columns if c.median],
+                     inc_width=q.width, inc_n_buckets=q.n_buckets, inc_group_by_series=q.group_by_series,
+                     inc_series_ids=None if q.series_ids is None else q.series_ids.tolist(),
+                     inc_n_groups=case.extra.get("n_groups"))
     return case

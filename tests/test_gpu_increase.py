@@ -3,8 +3,8 @@ f64 within the SUM rules. Every grouping a cell of one series allows (GROUP BY s
 explicit edges, the unbucketed scan of one series) over RLE, jittered and raw time pages with several column groups per
 series written out of time order; simple8b, gorilla and raw values; buckets straddling pages; empty, all-NULL and
 filtered pages inside a chain; time-range gaps; predicates, tombstones, NULL-time pages, host-resident pages with CRC on read; merge groups at the
-start, middle and end of a series; every refusal; 1 / 3 / 4 / 8 ranks; random queries scanned twice; the reference's
-increase.slt answers."""
+start, middle and end of a series; every refusal; 1 / 3 / 4 / 8 ranks, with chunk files, tombstones and unselected
+series, and one series split over ranks by time; random queries scanned twice; the reference's increase.slt answers."""
 import ctypes as C
 
 import numpy as np
@@ -392,20 +392,104 @@ def test_refusals(eng):
         pages.close()
 
 
-@pytest.mark.parametrize("n", [1, 3, 4, 8])
-def test_ranks(eng, n):
+RANK_INPUTS = [pytest.param(n, "plain", id=str(n)) for n in (1, 3, 4, 8)] + \
+    [pytest.param(n, kind, id="%d-%s" % (n, kind)) for kind in ("files", "tombstones", "unselected") for n in (3, 4)]
+
+
+@pytest.mark.parametrize("n, kind", RANK_INPUTS)
+def test_ranks(eng, n, kind):
     """Series shards on n ranks, GROUP BY series: the all-gather merge and the all-reduce partials path sum every rank's
-    increases; each cell is one rank's, so the result is the whole scan's."""
-    a, d, truth = arena(7, n_series=10, n_points=300)
-    ids = np.array(sorted(truth), dtype=np.uint32)
+    increases; each cell is one rank's, so the result is the whole scan's. Page sets: plain; merge_arena's chunk files
+    (merge groups at the start, middle and end of a series); tombstones of rows and of columns; series the query does
+    not select, which the "unselected" layout puts alone on rank 0."""
+    kw, scan_kw, unselected = {}, {}, ()
+    if kind == "files":
+        a, d, truth, files = merge_arena(4)
+        kw = scan_kw = {"files": files}
+    else:
+        a, d, truth = arena(7, n_series=10, n_points=300)
+    if kind == "tombstones":
+        tombs = cabi.tombstones([(3, 2, T0 + 50 * STEP, T0 + 120 * STEP), (5, 1, T0, T0 + 200 * STEP),
+                                 (7, None, T0 + 10 * STEP, T0 + 40 * STEP), (None, None, T0 + 250 * STEP, T0 + 260 * STEP)])
+        kw, scan_kw = {"tombstones": tombs}, {"tombstones": tombs}
+    every = np.array(sorted(truth), dtype=np.uint32)
+    if kind == "unselected":
+        unselected = every[[0, 5]]
+    ids = np.setdiff1d(every, unselected).astype(np.uint32)
     q = grid_query(truth, group_by_series=True, series_ids=ids)
-    for name, (shards, order) in layouts(ids, n).items():
-        with RankScans(eng, a, d, q, shards) as rs:
+    outs = layouts(every, n, unselected=unselected)
+    assert kind != "unselected" or "unselected" in outs
+    for name, (shards, order) in outs.items():
+        with RankScans(eng, a, d, q, shards, **scan_kw) as rs:
             rs.run()
             for r, res in enumerate(rs.gather(order)):
-                check_increases(res, truth, q, "N=%d %s gather rank %d" % (n, name, r))
+                check_increases(res, truth, q, "N=%d %s %s gather rank %d" % (n, kind, name, r), **kw)
             for r, res in enumerate(rs.allreduce(order)):
-                check_increases(res, truth, q, "N=%d %s all-reduce rank %d" % (n, name, r))
+                check_increases(res, truth, q, "N=%d %s %s all-reduce rank %d" % (n, kind, name, r), **kw)
+
+
+def time_partitions(seed, n_ranks=4, n_series=8, n_rows=600):
+    """Every series one run of n_rows rows STEP apart, cut at 1-3 rows inside buckets of W (never on a bucket edge)
+    into 2-4 partitions on distinct ranks, each partition one or two column groups. -> (arena, descs, whole truth,
+    per-rank truths, per-rank descriptor masks)."""
+    rng = np.random.default_rng(seed)
+    b = datagen.ArenaBuilder()
+    truth, ranks, cg_rank = {}, [dict() for _ in range(n_ranks)], []
+    per_bucket = W // STEP
+    for sid in range(n_series):
+        ts = T0 + np.arange(n_rows, dtype=np.int64) * STEP
+        p = int(rng.integers(2, n_ranks + 1))
+        cuts = np.sort(rng.choice([k for k in range(20, n_rows - 20) if k % per_bucket], p - 1, replace=False))
+        owners = np.sort(rng.choice(n_ranks, p, replace=False))
+        cols = {}
+        for cid, pt in FIELDS:
+            v = np.cumsum(rng.integers(-2, 6, n_rows)).astype(DT[pt]) if pt != U64 else np.cumsum(rng.integers(0, 6, n_rows)).astype(np.uint64)
+            cols[cid] = (v + rng.random(n_rows) if pt == F64 else v, rng.random(n_rows) > 0.1)
+        bounds = [0] + list(cuts) + [n_rows]
+        for k in range(p):
+            lo, hi = int(bounds[k]), int(bounds[k + 1])
+            split = [lo, (lo + hi) // 2, hi] if rng.random() < 0.5 else [lo, hi]
+            for g0, g1 in zip(split, split[1:]):
+                part = {cid: (v[g0:g1], ok[g0:g1]) for cid, (v, ok) in cols.items()}
+                b.add_column_group(sid, ts[g0:g1], [(cid, pt, part[cid][0], part[cid][1]) for cid, pt in FIELDS])
+                ranks[owners[k]].setdefault(sid, []).append((ts[g0:g1], part))
+                cg_rank.append(int(owners[k]))
+        truth[sid] = [(ts, cols)]
+    a, d = b.finish()
+    cg_of_desc = np.cumsum(d["phys_type"] == cabi.TSKV_PT_TIME) - 1
+    masks = [np.asarray(cg_rank)[cg_of_desc] == r for r in range(n_ranks)]
+    return a, d, truth, ranks, masks
+
+
+def test_ranks_time_partitions(eng):
+    """One series split over ranks by time, as time-partitioned vnodes hold it. The reference's increase merges partial
+    states by adding them (IncreaseAccumulator::merge_inner, query_server/query/src/extension/expr/aggregate_function/
+    increase.rs:109-114), so the pair across a partition boundary is never counted: the expected cell is the wrapping
+    sum over ranks of each rank's exact increase (f64: the sum, within the magnitudes' tolerance), valid where any rank's
+    is. The scan's all-gather merge and all-reduce partials path sum the increase sections the same way. GROUP BY
+    series, and one selected series ungrouped; at least one cell differs from the whole series' increase."""
+    a, d, truth, ranks, masks = time_partitions(11)
+    ids = np.array(sorted(truth), dtype=np.uint32)
+    for what, q in (("series", grid_query(truth, group_by_series=True, series_ids=ids)),
+                    ("one series", grid_query(truth, series_ids=ids[3:4]))):
+        n_cells = (len(ids) if q.group_by_series else 1) * q.n_buckets
+        with RankScans(eng, a, d, q, masks) as rs:
+            rs.run()
+            results = [("gather", res) for res in rs.gather()] + [("all-reduce", res) for res in rs.allreduce()]
+        for k, c in enumerate(INCS):
+            parts = [exact_increase_cells(rt, q, c.column_id, c.phys_type, n_cells) for rt in ranks]
+            if c.phys_type == F64:
+                v = np.sum([p[0].view(np.float64) for p in parts], axis=0).view(np.uint64)
+            else:
+                v = np.sum([p[0] for p in parts], axis=0, dtype=np.uint64)
+            merged = (v, np.any([p[1] for p in parts], axis=0), np.sum([p[2] for p in parts], axis=0))
+            whole = exact_increase_cells(truth, q, c.column_id, c.phys_type, n_cells)
+            np.testing.assert_array_equal(whole[1], merged[1])
+            if c.phys_type != F64:
+                assert (whole[0] != merged[0])[merged[1]].any(), (what, k)
+            for path, res in results:
+                check_increase(res, len(res.names) - len(INCS) + k, merged, c.phys_type,
+                               what="time partitions %s %s increase %d" % (what, path, k))
 
 
 def test_ranks_ungrouped(eng):

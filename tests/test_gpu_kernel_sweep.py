@@ -20,8 +20,16 @@
 4. test_operands_in_every_bin: pairs over every numeric column pair and a median per numeric column over the arena of
    each bin (simple8b-value bins: wide, mixed and narrow pages), tumbling and edge scans; the work list read back proves
    the operands' pages sat in that bin's intended bucket.
-5. test_every_operand_kernel_reached: tests 3 and 4 together launched every operand kernel
-   (sweep_reference.OPERAND_KERNELS) on work (skipped unless both ran to the end, test 3 over every case)."""
+   Each bin also runs a GROUP BY series copy of the query with an increase of every numeric column and one duplicate.
+5. test_random_increase_combinations: N_INCREASE random cases with counter increases (sweep_reference:
+   random_increase_case), most regrouped into a shape whose cells hold one series, the rest kept and held to the
+   refusal rule of sweep_reference.increase_status. Where the query projects COUNT(c), each increase of c must be valid
+   exactly where COUNT(c) > 0; then the increases by check_increase, and integer increases byte-identical between two
+   runs. TSKV_SWEEP_CASE=<index> reruns one case here too.
+6. test_every_operand_kernel_reached: tests 3, 4 and 5 together launched every operand kernel
+   (sweep_reference.OPERAND_KERNELS) on work (skipped unless all three ran to the end, tests 3 and 5 over every
+   case)."""
+import copy
 import os
 
 import numpy as np
@@ -32,6 +40,7 @@ from cnosdb_b200.engine import PushedAggregate, TskvError
 from tests import sweep_reference as sw
 from tests.covariance_reference import check_pair
 from tests.helpers import assert_matches_exact
+from tests.increase_reference import check_increase
 from tests.median_reference import check_median
 from tests.variance_reference import check_m2
 
@@ -40,6 +49,7 @@ pytestmark = pytest.mark.gpu
 BASE_SEED = 20261017
 N_RANDOM = 300
 N_OPERAND = 200
+N_INCREASE = 150
 ONE_CASE = os.environ.get("TSKV_SWEEP_CASE")  # rerun one index of test_random_combinations / _operand_combinations
 
 
@@ -65,9 +75,10 @@ def check_exact(got, exp, what):
 
 def deterministic_outputs(res):
     """Indices of the outputs that do not depend on the order of f64 additions: counts, integer sums and means, MIN /
-    MAX and FIRST / LAST of every type, pair n and medians."""
+    MAX and FIRST / LAST of every type, pair n, medians and integer increases."""
     return [j for j, (c, a) in enumerate(res.names)
-            if not (a in ("m2", "c", "m2x", "m2y") or (a in ("sum", "mean") and res.phys[c] == cabi.TSKV_PT_F64))]
+            if not (a in ("m2", "c", "m2x", "m2y") or
+                    (a in ("sum", "mean", "increase") and res.phys[c] == cabi.TSKV_PT_F64))]
 
 
 def assert_same_bytes(a, b, what):
@@ -165,11 +176,14 @@ def test_every_instantiation(engine, monkeypatch):
 
 
 def check_operands(got, exp, query, what):
-    """The pairs and medians of `got` against exp.pairs / exp.medians (sweep_reference.expected), and every other output
-    against the rest of exp. First, where the query projects COUNT(c): the pair (c, c)'s n equals it and the median of c
-    is valid where it is > 0."""
+    """The pairs, medians and increases of `got` against exp.pairs / exp.medians / exp.increases
+    (sweep_reference.expected), and every other output against the rest of exp. First, where the query projects
+    COUNT(c): the pair (c, c)'s n equals it, and the median of c and every increase of c are valid where it is > 0."""
     meds = [c for c in query.columns if c.median]
-    m0 = len(got.names) - len(meds)  # (the median outputs come last, in column order)
+    incs = [c for c in query.columns if c.increase]
+    i0 = len(got.names) - len(incs)  # (the increase outputs come last, in column order)
+    m0 = i0 - len(meds)  # (the median outputs come before them, in column order)
+    assert got.names[m0:] == [(c.column_id, "median") for c in meds] + [(c.column_id, "increase") for c in incs], what
     for k, (x, _, y, _) in enumerate(query.pairs):
         if x == y and (x, "count") in got.names:
             n, _ = got.pair(k, "n")
@@ -183,10 +197,18 @@ def check_operands(got, exp, query, what):
             bad = np.nonzero(got.validity[m0 + k] != (count > 0))[0]
             assert bad.size == 0, "%s: median %d of %d: validity differs from COUNT > 0 at cells %s: the selection " \
                 "passes disagree with pass 1" % (what, k, c.column_id, bad[:5])
+    for k, c in enumerate(incs):
+        if (c.column_id, "count") in got.names:
+            count = got.values[got.names.index((c.column_id, "count"))]
+            bad = np.nonzero(got.validity[i0 + k] != (count > 0))[0]
+            assert bad.size == 0, "%s: increase %d of %d: validity differs from COUNT > 0 at cells %s: the increase " \
+                "pass disagrees with pass 1" % (what, k, c.column_id, bad[:5])
     for k in range(len(query.pairs)):
         check_pair(got, k, exp.pairs[k], what="%s pair %d" % (what, k))
     for k in range(len(meds)):
         check_median(got, m0 + k, exp.medians[k], what="%s median %d" % (what, k))
+    for k, c in enumerate(incs):
+        check_increase(got, i0 + k, exp.increases[k], c.phys_type, what="%s increase %d of %d" % (what, k, c.column_id))
     rest = list(range(m0 - 4 * len(query.pairs)))
     assert got.names[:len(rest)] == exp.names[:len(rest)], what
     check_exact(_Picked(got, rest), _Picked(exp, rest), what)
@@ -239,8 +261,8 @@ def test_random_combinations(engine, monkeypatch):
 
 
 # ---- 3. random combinations with pairs and medians -------------------------------------------------------------------
-OPERANDS_REACHED = set()  # the operand kernels tests 3 and 4 launched on work
-OPERAND_TESTS_RUN = set()  # tests 3 (every case) and 4 when they ran to the end in this session
+OPERANDS_REACHED = set()  # the operand kernels tests 3, 4 and 5 launched on work
+OPERAND_TESTS_RUN = set()  # tests 3 (every case), 4 and 5 (every case) when they ran to the end in this session
 
 
 def test_random_operand_combinations(engine, monkeypatch):
@@ -272,6 +294,44 @@ def operand_query(truth, b, narrow, edges):
     return q, extra, num
 
 
+def increase_query(q, num):
+    """A GROUP BY series copy of operand_query's query without its pairs and medians, plus an increase of every numeric
+    column and a second increase of the first."""
+    qi = copy.copy(q)
+    qi.pairs, qi._keep, qi.group_by_series = [], None, True
+    qi.columns = [c for c in q.columns if not c.median] + \
+        [PushedAggregate(c, sw.COLUMNS[c], ["increase"]) for c in num + num[:1]]
+    return qi
+
+
+def operand_bin_case(engine, arena, descs, truth, q, extra, b, narrow, num, what):
+    """Runs one query of test_operands_in_every_bin -> (work list, the buckets its operands' items sat in)."""
+    exp = sw.expected(truth, q, extra)
+    assert not isinstance(exp, (int, str)), "%s: the reference refuses the case (%s)" % (what, exp)
+    pages = engine.upload_pages(arena, descs)
+    try:
+        got, wl = prepared_run(engine, pages, q, extra)
+    finally:
+        pages.close()
+    assert wl is not None, "%s: status %s" % (what, got)
+    # every page of every operand in bin b, in the wide or the narrow bucket as its narrow flag says
+    ids = [c.column_id for c in sw.scan_query(q).columns]
+    fill = wl["fill"].astype(np.int64).reshape(sw.N_BINS, len(ids), 2)
+    field = (descs["phys_type"] != cabi.TSKV_PT_TIME) & np.isin(descs["series_id"], q.series_ids)
+    buckets = set()
+    for c in num:
+        mine = field & (descs["column_id"] == c)
+        nar = int(wl["page_narrow"][mine].astype(bool).sum())
+        qc = ids.index(c)
+        assert (wl["page_bin"][mine] == b).all() and fill[:, qc].sum() == fill[b, qc].sum(), what
+        assert (fill[b, qc, 0], fill[b, qc, 1]) == (int(mine.sum()) - nar, nar), (what, c, fill[b, qc])
+        if narrow == sw.NARROW_ALL:
+            assert fill[b, qc, 0] == 0 and fill[b, qc, 1] > 0, (what, c, fill[b, qc])
+        buckets |= {k for k in (0, 1) if fill[b, qc, k]}
+    check_operands(got, exp, q, what)
+    return wl, buckets
+
+
 def test_operands_in_every_bin(engine, monkeypatch):
     set_env(monkeypatch, {"TSKV_PARTS": None, "TSKV_SMEM_TABLE_KB": None})
     reached, buckets = set(), set()
@@ -283,41 +343,45 @@ def test_operands_in_every_bin(engine, monkeypatch):
             for edges in (False, True):
                 q, extra, num = operand_query(truth, b, narrow, edges)
                 what = "operands in bin %d narrow %d edges %s" % (b, narrow, edges)
-                exp = sw.expected(truth, q, extra)
-                assert not isinstance(exp, (int, str)), "%s: the reference refuses the case (%s)" % (what, exp)
-                pages = engine.upload_pages(arena, descs)
-                try:
-                    got, wl = prepared_run(engine, pages, q, extra)
-                finally:
-                    pages.close()
-                assert wl is not None, "%s: status %s" % (what, got)
-                # every page of every operand in bin b, in the wide or the narrow bucket as its narrow flag says
-                ids = [c.column_id for c in sw.scan_query(q).columns]
-                fill = wl["fill"].astype(np.int64).reshape(sw.N_BINS, len(ids), 2)
-                field = (descs["phys_type"] != cabi.TSKV_PT_TIME) & np.isin(descs["series_id"], q.series_ids)
-                for c in num:
-                    mine = field & (descs["column_id"] == c)
-                    nar = int(wl["page_narrow"][mine].astype(bool).sum())
-                    qc = ids.index(c)
-                    assert (wl["page_bin"][mine] == b).all() and fill[:, qc].sum() == fill[b, qc].sum(), what
-                    assert (fill[b, qc, 0], fill[b, qc, 1]) == (int(mine.sum()) - nar, nar), (what, c, fill[b, qc])
-                    if narrow == sw.NARROW_ALL:
-                        assert fill[b, qc, 0] == 0 and fill[b, qc, 1] > 0, (what, c, fill[b, qc])
-                    buckets |= {k for k in (0, 1) if fill[b, qc, k]}
-                check_operands(got, exp, q, what)
+                wl, bk = operand_bin_case(engine, arena, descs, truth, q, extra, b, narrow, num, what)
+                buckets |= bk
                 reached |= sw.operand_kernels(wl, q, edges)
+                qi = increase_query(q, num)
+                wl, bk = operand_bin_case(engine, arena, descs, truth, qi, extra, b, narrow, num, what + " increases")
+                buckets |= bk
+                reached |= sw.operand_kernels(wl, qi, edges)
     assert buckets == {0, 1}, buckets
     OPERANDS_REACHED.update(reached)
     OPERAND_TESTS_RUN.add("bins")
     print("\noperands in every bin: operand kernels reached: %s" % sorted(reached))
 
 
+# ---- 5. random combinations with increases ---------------------------------------------------------------------------
+def test_random_increase_combinations(engine, monkeypatch):
+    indices = [int(ONE_CASE)] if ONE_CASE is not None else range(N_INCREASE)
+    statuses, shapes, n_incs = {}, {}, 0
+    for i in indices:
+        case = sw.random_increase_case(i, BASE_SEED)
+        exp = sw.case_expected(case)
+        outcome = exp if isinstance(exp, (int, str)) else "result"
+        statuses[outcome] = statuses.get(outcome, 0) + 1
+        shape = "%s -> %s" % (case.desc["shape"], outcome)
+        shapes[shape] = shapes.get(shape, 0) + 1
+        n_incs += len([c for c in case.query.columns if c.increase])
+        run_case(engine, case, exp, monkeypatch, OPERANDS_REACHED)
+    if ONE_CASE is None:
+        OPERAND_TESTS_RUN.add("increases")
+    print("\nrandom increase combinations: %d cases, %d increases, outcomes %s, shapes %s; operand kernels reached: %s"
+          % (len(indices), n_incs, statuses, shapes, sorted(OPERANDS_REACHED)))
+
+
 def test_every_operand_kernel_reached():
-    """Tests 3 and 4 together launched every operand kernel on work. It reads what they recorded, so it needs both to
-    have run to the end in this session, test 3 over every case; otherwise it is skipped and says so."""
-    if OPERAND_TESTS_RUN != {"random", "bins"}:
-        pytest.skip("needs test_random_operand_combinations (every case) and test_operands_in_every_bin to run first "
-                    "in this session; ran: %s" % sorted(OPERAND_TESTS_RUN))
+    """Tests 3, 4 and 5 together launched every operand kernel on work. It reads what they recorded, so it needs all
+    three to have run to the end in this session, tests 3 and 5 over every case; otherwise it is skipped and says so."""
+    if OPERAND_TESTS_RUN != {"random", "bins", "increases"}:
+        pytest.skip("needs test_random_operand_combinations (every case), test_operands_in_every_bin and "
+                    "test_random_increase_combinations (every case) to run first in this session; ran: %s"
+                    % sorted(OPERAND_TESTS_RUN))
     missed = [k for k in sw.OPERAND_KERNELS if k not in OPERANDS_REACHED]
-    assert not missed, "operand kernels neither operand test launched on work: %s" % missed
+    assert not missed, "operand kernels no operand test launched on work: %s" % missed
     print("\noperand kernels reached: %s" % sorted(OPERANDS_REACHED))

@@ -1,6 +1,6 @@
 """The exact increase reference (tests/increase_reference.py) against the reference's increase.slt answers and hand
 cases: resets, equal runs, one value, NULLs, i64 / u64 wrapping at the extremes, NaN / +-inf / +-0.0 under totalOrder,
-time order against row order, and buckets."""
+time order against row order, and buckets; and the vectorized reference of the scale test against the exact one."""
 import math
 
 import numpy as np
@@ -8,7 +8,8 @@ import numpy as np
 from cnosdb_b200 import cabi
 from cnosdb_b200.engine import PushedAggregate, QueryOption
 from tests.covariance_reference import TB2_TYPES
-from tests.increase_reference import exact_increase_cells, increase_bits, load_golden
+from tests.helpers import bucket_index
+from tests.increase_reference import exact_increase_cells, increase_bits, increase_cells_np, load_golden
 
 I64, U64, F64 = cabi.TSKV_PT_I64, cabi.TSKV_PT_U64, cabi.TSKV_PT_F64
 PT = {"u64": U64, "i64": I64, "f64": F64}
@@ -108,3 +109,78 @@ def test_f64_special_values():
     assert np.float64(f([0.0, -0.0])).view(np.uint64) == np.float64(0.0).view(np.uint64)  # -0.0 < +0.0: a reset adds -0.0
     assert f([-0.0, 0.0]) == 0.0
     assert f([2.0, 2.0]) == 0.0
+
+
+def flat_rows(truth, col, pt, nb, bucket):
+    """(cells, times, bit patterns) of every valid row of `col`, cell = series slot * nb + bucket(times) (rows without a
+    bucket, bucket < 0, left out): the vectorized reference's input."""
+    cells, times, bits = [], [], []
+    for slot, sid in enumerate(sorted(truth)):
+        for ts, cols in truth[sid]:
+            if col not in cols:
+                continue
+            v, ok = cols[col]
+            b = bucket(np.asarray(ts, dtype=np.int64))
+            keep = np.asarray(ok, dtype=bool) & (b >= 0)
+            cells.append(slot * nb + b[keep])
+            times.append(np.asarray(ts, dtype=np.int64)[keep])
+            bits.append(np.asarray(v, dtype=DT[pt])[keep].view(np.uint64))
+    return np.concatenate(cells), np.concatenate(times), np.concatenate(bits)
+
+
+def random_truth(rng, pt, n_series=6):
+    """Series of 1-4 column groups, written out of time order, with NULLs, counter resets, runs of equal values and
+    (integers) values near the type's extremes that wrap the sum; f64 with NaN, +-inf and +-0.0."""
+    truth = {}
+    for sid in range(n_series):
+        cgs, t = [], int(rng.integers(-10**6, 10**6))
+        for _ in range(int(rng.integers(1, 5))):
+            n = int(rng.integers(1, 60))
+            ts = t + np.cumsum(rng.integers(1, 1000, n)).astype(np.int64)
+            t = int(ts[-1]) + 1
+            walk = np.cumsum(rng.integers(-3, 6, n))
+            walk[rng.random(n) < 0.1] = 0  # resets
+            if pt == F64:
+                v = walk.astype(np.float64) + np.round(rng.random(n), 2)
+                sp = rng.random(n) < 0.05
+                v[sp] = rng.choice([np.nan, np.inf, -np.inf, 0.0, -0.0], int(sp.sum()))
+            elif pt == I64:
+                v = walk.astype(np.int64) + (0, 2**63 - 50, -2**63 + 50)[int(rng.integers(0, 3))]
+            else:
+                v = walk.astype(np.int64).view(np.uint64) + np.uint64((0, 2**64 - 50, 2**63)[int(rng.integers(0, 3))])
+            cgs.append((ts, {1: (v, rng.random(n) > 0.2)}))
+        truth[sid] = [cgs[k] for k in rng.permutation(len(cgs))]
+    return truth
+
+
+def test_vectorized_reference_matches_the_exact_one():
+    """increase_cells_np (the reference of the scale test) equals exact_increase_cells on random truths, GROUP BY series
+    over tumbling buckets and over edges (rows outside the edges dropped): integers bit for bit, f64 bit for bit too
+    (both add in time order per cell) and the same magnitudes."""
+    rng = np.random.default_rng(77)
+    for trial in range(24):
+        pt = (I64, U64, F64)[trial % 3]
+        truth = random_truth(rng, pt)
+        lo = min(int(ts.min()) for cgs in truth.values() for ts, _ in cgs)
+        hi = max(int(ts.max()) for cgs in truth.values() for ts, _ in cgs)
+        if trial % 2:
+            e = np.unique(np.concatenate([[lo + 5], rng.integers(lo, hi, 6), [hi - 5]])).astype(np.int64)
+            q = QueryOption([PushedAggregate(1, pt, ["increase"])], n_buckets=e.size - 1, group_by_series=True)
+            kw = dict(edges=e)
+            bucket = lambda t: np.where((t >= e[0]) & (t < e[-1]), np.searchsorted(e, t, side="right") - 1, -1)  # noqa: E731
+        else:
+            w = int(rng.integers(500, 20000))
+            fbs = lo - lo % w
+            nb = (hi - fbs) // w + 1
+            q = QueryOption([PushedAggregate(1, pt, ["increase"])], width=w, first_bucket_start=fbs, n_buckets=nb,
+                            group_by_series=True)
+            kw = {}
+            bucket = lambda t: np.where(bucket_index(t, q)[1], bucket_index(t, q)[0], -1)  # noqa: E731
+        nb = q.n_buckets
+        n_cells = len(truth) * nb
+        v_e, ok_e, mag_e = exact_increase_cells(truth, q, 1, pt, n_cells, **kw)
+        v, ok, mag = increase_cells_np(*flat_rows(truth, 1, pt, nb, bucket), pt, n_cells)
+        np.testing.assert_array_equal(ok, ok_e, err_msg=str(trial))
+        np.testing.assert_array_equal(v[ok_e], v_e[ok_e], err_msg=str(trial))
+        np.testing.assert_array_equal(mag[ok_e], mag_e[ok_e], err_msg=str(trial))
+        assert ok_e.sum() >= 3, trial

@@ -11,11 +11,13 @@ import pytest
 from cnosdb_b200 import cabi
 from cnosdb_b200.engine import PushedAggregate, QueryOption
 from tests import sweep_reference as sw
+from tests import test_increase_kernel_list as increase_kernels
 from tests import test_median_kernel_list as median_kernels
 from tests import test_pair_kernel_list as pair_kernels
 from tests.covariance_reference import exact_pair_cells, paired_rows
 from tests.exact_arenas import two_file_arena
 from tests.helpers import bucket_spec
+from tests.increase_reference import exact_increase_cells
 from tests.median_reference import exact_median_cells
 
 I64, F64 = cabi.TSKV_PT_I64, cabi.TSKV_PT_F64
@@ -139,16 +141,95 @@ def test_operand_cases_cover_the_features():
 
 
 def test_operand_kernels_are_the_librarys():
-    """sweep_reference.OPERAND_KERNELS is exactly the scan and merged-row subset of the pair and median kernels the
-    kernel-list tests hold to the library."""
-    both = pair_kernels.EXPECTED | median_kernels.EXPECTED
-    prefixes = ("k_scan_pair<", "k_merge_pairs_rows<", "k_scan_median<", "k_merge_median_rows")
+    """sweep_reference.OPERAND_KERNELS is exactly the scan and merged-row subset of the pair, median and increase
+    kernels the kernel-list tests hold to the library."""
+    both = pair_kernels.EXPECTED | median_kernels.EXPECTED | increase_kernels.EXPECTED
+    prefixes = ("k_scan_pair<", "k_merge_pairs_rows<", "k_scan_median<", "k_merge_median_rows", "k_scan_increase<",
+                "k_merge_increase")
     want = {k for k in both if k.startswith(prefixes)}
     assert set(sw.OPERAND_KERNELS) == want and len(sw.OPERAND_KERNELS) == len(want)
 
 
 def test_first_cases_unchanged_by_the_operand_draw():
-    """random_operand_case draws its operands from a stream of its own: the case underneath is random_case's."""
+    """random_operand_case and random_increase_case draw their operands from streams of their own: the case underneath
+    is random_case's (its arena and every draw), and random_operand_case's cases do not change."""
     for i in range(20):
-        a, b = sw.random_case(i, BASE_SEED), sw.random_operand_case(i, BASE_SEED)
+        a, b, c = sw.random_case(i, BASE_SEED), sw.random_operand_case(i, BASE_SEED), sw.random_increase_case(i, BASE_SEED)
         assert {k: b.desc[k] for k in a.desc} == a.desc, i
+        assert {k: c.desc[k] for k in a.desc} == a.desc, i
+        assert (c.arena == a.arena).all() and (c.descs == a.descs).all(), i
+        assert not any(x.increase for x in b.query.columns), i
+
+
+N_INC_CASES = 150  # tests/test_gpu_kernel_sweep.py's N_INCREASE
+
+
+def test_increase_cases_cover_the_shapes_and_refusals():
+    """The random increase cases hold every accepted shape, kept groupings that are accepted and refused, every
+    refusal of increase_status, duplicates, unprojected operands, a pair or a median beside increases, and files."""
+    seen = set()
+    for i in range(N_INC_CASES):
+        case = sw.random_increase_case(i, BASE_SEED)
+        q = case.query
+        incs = [c.column_id for c in q.columns if c.increase]
+        if not incs:
+            continue
+        exp = sw.increase_status(case.truth, q, case.extra)
+        seen.add("%s %s" % (case.desc["shape"], "accepted" if exp is None else "refused"))
+        if exp is not None:
+            seen.add("refusal %s" % exp)
+            if exp == cabi.TSKV_ERR_UNSUPPORTED:
+                seen.add("unsupported: " + ("labels" if "labels" in case.extra else "tags" if "group_ids" in case.extra
+                                            else "ungrouped"))
+        if len(incs) > len(set(incs)):
+            seen.add("duplicate")
+        if any(c not in [p.column_id for p in q.projected()] for c in incs):
+            seen.add("unprojected")
+        if q.pairs or any(c.median for c in q.columns):
+            seen.add("pair or median")
+        if case.files is not None and exp is None:
+            seen.add("files")
+    want = {"series accepted", "tags accepted", "edges accepted", "one accepted", "kept accepted", "kept refused",
+            "refusal ValueError", "refusal %d" % cabi.TSKV_ERR_INVALID_ARG, "refusal %d" % cabi.TSKV_ERR_UNSUPPORTED,
+            "unsupported: labels", "unsupported: tags", "unsupported: ungrouped", "duplicate", "unprojected",
+            "pair or median", "files"}
+    assert want <= seen, want - seen
+
+
+def test_increase_status_order():
+    """increase_status gives the first refusal in the library's order when several apply: the engine's ValueError for a
+    sliding window, then a BOOL operand, then labels, a shared tag group, an ungrouped scan over several series."""
+    truth = {0: [], 1: []}
+    inc = lambda c, pt: PushedAggregate(c, pt, ["increase"])  # noqa: E731
+    q = QueryOption([inc(4, sw.BOOL)])
+    lab = {"edges": np.array([0, 5, 9]), "labels": np.zeros(2, dtype=np.uint32)}
+    assert sw.increase_status(truth, q, dict(lab, slide=5)) == "ValueError"
+    assert sw.increase_status(truth, q, lab) == cabi.TSKV_ERR_INVALID_ARG
+    q = QueryOption([inc(1, I64)])
+    assert sw.increase_status(truth, q, dict(lab, group_ids=np.zeros(2, dtype=np.uint32))) == cabi.TSKV_ERR_UNSUPPORTED
+    assert sw.increase_status(truth, q, {"group_ids": np.array([1, 0], dtype=np.uint32)}) is None
+    assert sw.increase_status(truth, q, {"group_ids": np.array([1, 1], dtype=np.uint32)}) == cabi.TSKV_ERR_UNSUPPORTED
+    assert sw.increase_status(truth, q, {}) == cabi.TSKV_ERR_UNSUPPORTED
+    assert sw.increase_status({0: []}, q, {}) is None
+    assert sw.increase_status(truth, QueryOption([inc(1, I64)], series_ids=[1]), {}) is None
+    assert sw.increase_status(truth, QueryOption([inc(1, I64)], group_by_series=True), {}) is None
+    # a group map decides alone: one selected series per group is accepted without GROUP BY series
+    q1 = QueryOption([inc(1, I64)], series_ids=[0, 1])
+    assert sw.increase_status(truth, q1, {"group_ids": np.array([0, 1], dtype=np.uint32)}) is None
+
+
+@pytest.mark.parametrize("index", range(0, N_INC_CASES, 5))
+def test_increase_validity_is_count(index):
+    """Every increase of an accepted random increase case is valid exactly where COUNT(c) > 0 of the independent exact
+    reference."""
+    case = sw.random_increase_case(index, BASE_SEED)
+    if sw.increase_status(case.truth, case.query, case.extra) is not None:
+        return
+    kw = dict(tombstones=case.tombstones, files=case.files, group_ids=case.extra.get("group_ids"),
+              edges=case.extra.get("edges"))
+    for col in sorted({c.column_id for c in case.query.columns if c.increase}):
+        count = count_result(case, col)
+        if count is None:
+            return
+        _, ok, _ = exact_increase_cells(case.truth, case.query, col, sw.COLUMNS[col], count.size, **kw)
+        np.testing.assert_array_equal(ok, count > 0, err_msg="%s column %d" % (case.describe(), col))
