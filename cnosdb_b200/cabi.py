@@ -66,6 +66,33 @@ def query_n_increases(flags):
     return (int(flags) >> 16) & 0xFF
 
 
+# modes / distincts: n_modes in bits 24..27, n_distincts in bits 28..31 of tskv_query.reserved, operands after the
+# increases' (see include/tskv_gpu.h)
+TSKV_MAX_MODES = 8
+TSKV_MAX_DISTINCTS = 8
+TSKV_MAX_SORTED_ROWS = 0x7FFFFFFF
+
+
+def query_modes(n):
+    """TSKV_QUERY_MODES(n): the flags-word bits of n modes."""
+    return (int(n) & 0xF) << 24
+
+
+def query_n_modes(flags):
+    """TSKV_QUERY_N_MODES(flags)."""
+    return (int(flags) >> 24) & 0xF
+
+
+def query_distincts(n):
+    """TSKV_QUERY_DISTINCTS(n): the flags-word bits of n distinct counts."""
+    return (int(n) & 0xF) << 28
+
+
+def query_n_distincts(flags):
+    """TSKV_QUERY_N_DISTINCTS(flags)."""
+    return (int(flags) >> 28) & 0xF
+
+
 TSKV_UPLOAD_VERIFY_CRC = 1
 TSKV_UPLOAD_HOST_RESIDENT = 2
 TSKV_UPLOAD_VERIFY_ON_READ = 4

@@ -345,4 +345,21 @@ __global__ void __launch_bounds__(128) k_merge_increase(const ScanParams P, cons
   increase_end(P.state, ic, A, blockIdx.y, rec0 + i, (uint32_t)M.cg_slot[M.mcg_cg[merge_mcg_of(M, i)]], run);
 }
 
+// The gathers over the merged rows (k_scan_mode's pages): one thread per (merge row, gather = blockIdx.y); the leader of a
+// merged row that survives the row-level filters (merged_row) and holds a merged value of the operand (merge_value)
+// writes its order key into its cell's slice.
+__global__ void __launch_bounds__(128) k_merge_mode_rows(const ScanParams P, const MergeParams M, const ModeGather *gathers, const ModeArgs A) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  MergedRow mr;
+  if (i >= M.n_rows || !merged_row(P, M, i, mr)) return;
+  const ModeGather mg = gathers[blockIdx.y];
+  uint64_t v;
+  if (!merge_value(P, M, mg.qcol, mr.series, mr.t, mr.s0, mr.s1, v)) return;
+  const uint64_t seg = (uint64_t)blockIdx.y * A.n_cells + mr.cell;
+  uint32_t pos;
+  if (!mode_reserve(A, seg, 1, pos)) return;
+  A.keys[pos] = median_ukey(v, mg.phys_type);
+  A.segs[pos] = (uint32_t)seg;
+}
+
 }  // namespace tskv

@@ -2940,6 +2940,225 @@ __global__ void k_finalize_increases(const uint64_t *state, const IncreaseCol *i
     *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
 }
 
+// ---- modes and distinct counts (TSKV_QUERY_N_MODES / _N_DISTINCTS): every cell's selected order keys, sorted ---------
+// One gather per distinct operand column id. Pass 1 (the fused scan) gives every cell's n; an exclusive sum of the n over
+// the (gather, cell) segments gives segment s the slice [off[s], off[s + 1]) of one key buffer (off[n_segs]: the keys of
+// all). k_scan_mode (a lane per page) and k_merge_mode_rows (a thread per merge row) write each selected value's order
+// key (median_ukey: one to one on bit patterns, so equal keys are equal values) and its segment into the slice through
+// the segment's cursor. Two radix sorts order the buffer by (segment, key); the slots past off[n_segs] hold segment ~0
+// and sort last. A run is a stretch of equal (segment, key): k_mode_heads marks each run's first position, a max-scan
+// carries it to the run's every position, and k_mode_runs counts each segment's runs (its distinct values) and keeps its
+// longest run, of tied lengths the first (the smallest key).
+struct ModeGather {
+  uint64_t count_off;  // the operand's COUNT section (its pass-1 n)
+  uint32_t qcol;       // the operand's column in the scan's column table (its work-list buckets, its merged values)
+  uint16_t column_id;
+  uint8_t phys_type;
+  uint8_t pad;
+};
+// One mode or distinct output: its gather, and whether it is a distinct count (else a mode).
+struct ModeOut {
+  uint32_t gather;
+  uint32_t distinct;
+};
+struct ModeArgs {
+  uint64_t *keys;            // [bound] the slices k_scan_mode fills; after the sorts, the sorted keys
+  uint32_t *segs;            // [bound] their segments (~0: no key); after the sorts, the sorted segments
+  int32_t *off;              // [n_segs + 1]
+  int32_t *cursor;           // [n_segs] the next free slot of each slice
+  unsigned long long *best;  // [n_segs] the longest run: length << 32 | ~(its first position)
+  unsigned long long *runs;  // [n_segs] the number of runs
+  int32_t *status;           // the scan's status slot and error page
+  unsigned long long *err_page;
+  uint64_t n_cells, n_segs, bound;
+};
+struct ModeMax {  // the run starts' max-scan
+  __device__ __forceinline__ uint32_t operator()(uint32_t a, uint32_t b) const { return a > b ? a : b; }
+};
+constexpr uint32_t MODE_STAGE = 16;  // keys a lane stages per slot reservation
+constexpr uint32_t MODE_ITEMS = 16;  // sorted positions per lane in k_mode_runs
+
+// A slice that receives more keys than its pass-1 n, or ends with fewer (only a decode error pass 1 reports first can
+// cause either): TSKV_ERR_BITSET_MISMATCH, page ~0.
+__device__ __forceinline__ void mode_mismatch(const ModeArgs &A) {
+  if (atomicCAS(A.status, 0, (int)TSKV_ERR_BITSET_MISMATCH) == 0) *A.err_page = ~0ull;
+}
+// Reserves n slots of segment seg's slice; false (and the error) when they do not fit it.
+__device__ __forceinline__ bool mode_reserve(const ModeArgs &A, uint64_t seg, uint32_t n, uint32_t &pos) {
+  pos = (uint32_t)atomicAdd(A.cursor + seg, (int)n);
+  const uint32_t end = (uint32_t)A.off[seg + 1];
+  if (pos + (uint64_t)n > end || end > A.bound) {
+    mode_mismatch(A);
+    return false;
+  }
+  return true;
+}
+
+// One lane's staged keys of one segment (stage: the CTA's [MODE_STAGE][128] buffer, column threadIdx.x).
+struct ModeRun {
+  uint64_t seg;
+  uint32_t n;
+};
+__device__ __forceinline__ void mode_flush(const ModeArgs &A, uint64_t (*stage)[128], ModeRun &r) {
+  uint32_t pos;
+  if (r.n && mode_reserve(A, r.seg, r.n, pos))
+    for (uint32_t k = 0; k < r.n; k++) {
+      A.keys[pos + k] = stage[k][threadIdx.x];
+      A.segs[pos + k] = (uint32_t)r.seg;
+    }
+  r.n = 0;
+}
+
+// One page of a gather's operand (work item `item` of its buckets), decoded with its group's time page row by row and
+// selected as the medians select (select_row). Decode errors are pass 1's to report: the lane stops at the first.
+template <bool EDGES>
+__device__ __forceinline__ void mode_page(const ScanParams &P, const ModeGather &mg, const ModeArgs &A, uint64_t seg0,
+                                          uint64_t (*stage)[128], uint32_t item) {
+  const uint32_t page = P.work_page[item], slot = P.work_slot[item];
+  const tskv_page_desc vd = P.descs[page];
+  const uint32_t tpage = P.time_page_of[page];
+  const tskv_page_desc td = P.descs[tpage];
+  if (vd.phys_type != mg.phys_type || kind_status(vd.reserved) != TSKV_OK || kind_status(td.reserved) != TSKV_OK ||
+      td.reserved == DK_ALLNULL || vd.reserved == DK_ALLNULL)
+    return;
+  PageView tpv, vpv;
+  tpv.open(P.arena, td);
+  vpv.open(P.arena, vd);
+  BitCursor tb, vb;
+  tb.init(tpv.bitset);
+  vb.init(vpv.bitset);
+  DeltaCursor<-1> tc;
+  AnyCursor<> vc;
+  if (tc.open(tpv, td.reserved) != TSKV_OK || vc.open(vpv, vd.reserved) != TSKV_OK) return;
+  const uint4 none = make_uint4(0, 0, 0, 0);
+  const uint4 tv4 = P.has_tomb ? tomb_lookup(P, vd.series_id, mg.column_id) : none;
+  const uint32_t *keepw = P.row_keep ? P.row_keep + P.keep_off[tpage] : nullptr;
+  const uint64_t group_base = group_cell_base<EDGES>(P, slot);
+  BucketState bk; bk.valid = false; bk.floor_regime = false; bk.lo = 0; bk.hi = 0; bk.idx = 0;
+  ModeRun run;
+  run.seg = ~0ull;
+  run.n = 0;
+  int64_t t = 0;
+  const uint32_t n_rows = vd.num_values;
+  for (uint32_t r = 0; r < n_rows; r++) {
+    const bool tv = tb.next(r), vv = vb.next(r);
+    uint64_t v = 0;
+    if (tv) { t = (int64_t)tc.next(); if (tc.exhausted) break; }
+    else if (r == 0) tc.skip_first_if_s8b_sc();
+    if (vv) { v = vc.next(); if (vc.failed()) break; }
+    else if (r == 0 && !vc.is_gorilla) vc.d.skip_first_if_s8b_sc();
+    uint64_t cell;
+    if (!(tv && vv) || !select_row<EDGES>(P, keepw, r, t, tv4, none, group_base, bk, cell)) continue;
+    if (seg0 + cell != run.seg || run.n == MODE_STAGE) {
+      mode_flush(A, stage, run);
+      run.seg = seg0 + cell;
+    }
+    stage[run.n++][threadIdx.x] = median_ukey(v, mg.phys_type);
+  }
+  mode_flush(A, stage, run);
+}
+
+// The gathers' pages (blockIdx.y: the gather): one lane per work item of the operand's buckets (every bin, wide and
+// narrow), the items pass 1 read.
+template <bool EDGES>
+__global__ void __launch_bounds__(128) k_scan_mode(const __grid_constant__ ScanParams P, const ModeGather *gathers, const ModeArgs A) {
+  __shared__ uint64_t stage[MODE_STAGE][128];
+  const ModeGather mg = gathers[blockIdx.y];
+  const uint64_t seg0 = (uint64_t)blockIdx.y * A.n_cells;
+  const uint32_t stride = gridDim.x * blockDim.x, t0 = blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t k = mg.qcol * WL_SUB; k < N_BINS * P.n_cols * WL_SUB; k += P.n_cols * WL_SUB)
+    for (uint32_t sub = 0; sub < WL_SUB; sub++) {
+      const uint32_t start = __ldg(P.region_start + k + sub), fill = __ldg(P.region_fill + k + sub);
+      for (uint32_t i = t0; i < fill; i += stride) mode_page<EDGES>(P, mg, A, seg0, stage, start + i);
+    }
+}
+
+// After pass 1: every segment's n (off, summed in place into the slices' starts next), off[n_segs] = 0, and the run
+// results cleared.
+__global__ void k_mode_counts(const uint64_t *state, const ModeGather *gathers, const ModeArgs A) {
+  for (uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; s <= A.n_segs; s += (uint64_t)gridDim.x * blockDim.x) {
+    if (s == A.n_segs) { A.off[s] = 0; continue; }
+    const uint64_t n = state[gathers[s / A.n_cells].count_off + s % A.n_cells];
+    A.off[s] = (int32_t)min(n, (uint64_t)TSKV_MAX_SORTED_ROWS);
+    A.best[s] = A.runs[s] = 0;
+  }
+}
+
+// After the sorts: start[i] = i at the first position of a run, else 0 (a max-scan then gives every position its run's
+// first); and every slice whose cursor did not end at its end is an error.
+__global__ void k_mode_heads(const ModeArgs A, uint32_t *start) {
+  const uint64_t total = min((uint64_t)(uint32_t)A.off[A.n_segs], A.bound), stride = (uint64_t)gridDim.x * blockDim.x;
+  const uint64_t t0 = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint64_t i = t0; i < A.bound; i += stride)
+    start[i] = i < total && (i == 0 || A.segs[i] != A.segs[i - 1] || A.keys[i] != A.keys[i - 1]) ? (uint32_t)i : 0;
+  for (uint64_t s = t0; s < A.n_segs; s += stride)
+    if (A.cursor[s] != A.off[s + 1]) mode_mismatch(A);
+}
+
+// After the max-scan: a lane per MODE_ITEMS sorted positions adds, at each run's last position, one run and the run's
+// (length, first position) to its segment; a warp combines its lanes' last segments before the atomics.
+__global__ void __launch_bounds__(256) k_mode_runs(const ModeArgs A, const uint32_t *start) {
+  const uint64_t total = min((uint64_t)(uint32_t)A.off[A.n_segs], A.bound);
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+  for (uint64_t base = (((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 32 * MODE_ITEMS; base < total;
+       base += warps * 32 * MODE_ITEMS) {
+    uint32_t seg = ~0u, runs = 0;
+    unsigned long long best = 0;
+    const uint64_t i0 = base + (uint64_t)lane * MODE_ITEMS, i1 = min(i0 + MODE_ITEMS, total);
+    for (uint64_t i = i0; i < i1; i++) {
+      const uint32_t s = A.segs[i];
+      if (i + 1 < total && A.segs[i + 1] == s && A.keys[i + 1] == A.keys[i]) continue;  // not a run's last position
+      if (s != seg) {
+        if (runs) {
+          atomicAdd(A.runs + seg, (unsigned long long)runs);
+          atomicMax(A.best + seg, best);
+        }
+        seg = s;
+        runs = 0;
+        best = 0;
+      }
+      const uint32_t first = start[i];
+      runs++;
+      best = max(best, ((unsigned long long)(i - first + 1) << 32) | (uint32_t)~first);
+    }
+    const uint32_t group = __match_any_sync(FULL, seg);
+    const uint32_t hi = __reduce_max_sync(group, (uint32_t)(best >> 32));
+    const uint32_t lo = __reduce_max_sync(group, (uint32_t)(best >> 32) == hi ? (uint32_t)best : 0u);
+    const uint32_t n = __reduce_add_sync(group, runs);
+    if (seg != ~0u && n && lane == (uint32_t)(__ffs(group) - 1)) {
+      atomicAdd(A.runs + seg, (unsigned long long)n);
+      atomicMax(A.best + seg, ((unsigned long long)hi << 32) | lo);
+    }
+  }
+}
+
+// The mode and distinct outputs (blockIdx.y: the output; output column out0 + blockIdx.y). A mode is in the operand's
+// type, valid iff its cell holds a value: the key of the cell's longest run. A distinct is the cell's number of runs, a
+// u64, always valid.
+__global__ void k_finalize_modes(const ModeArgs A, const ModeGather *gathers, const ModeOut *outs, uint32_t out0, uint64_t bitmap_stride,
+                                 uint64_t *values, uint8_t *validity) {
+  const ModeOut mo = outs[blockIdx.y];
+  const uint64_t cell = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  bool valid = false;
+  if (cell < A.n_cells) {
+    const uint64_t s = (uint64_t)mo.gather * A.n_cells + cell;
+    uint64_t v = 0;
+    if (mo.distinct) {
+      v = A.runs[s];
+      valid = true;
+    } else {
+      const uint32_t first = ~(uint32_t)A.best[s];
+      valid = A.off[s + 1] > A.off[s] && first < A.bound;
+      if (valid) v = okey_inv((int64_t)(A.keys[first] ^ 0x8000000000000000ull), gathers[mo.gather].phys_type);
+    }
+    values[(uint64_t)(out0 + blockIdx.y) * A.n_cells + cell] = v;
+  }
+  const uint32_t bits = __ballot_sync(FULL, valid);
+  if ((threadIdx.x & 31) == 0 && (cell >> 3) < bitmap_stride)
+    *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
+}
+
 // Per output column: which state arrays feed it.
 struct OutCol {
   uint64_t count_off;  // counts of the source column

@@ -16,6 +16,7 @@
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <nccl.h>  // types and enums only: the library is loaded with dlopen on first use
@@ -278,6 +279,19 @@ struct tskv_scan {
   async_ptr<uint8_t> d_inc_tmp;
   size_t inc_tmp_bytes = 0;
   IncreaseArgs inc{};
+  // modes and distincts (TSKV_QUERY_N_MODES / _N_DISTINCTS; k_scan_mode): their gathers and outputs, the key and segment
+  // buffers (slices, then sorted: ModeArgs), the slices' offsets and cursors, the run results and the run starts
+  uint32_t n_gathers = 0, n_mode_outs = 0;
+  int mode_seg_bits = 1;  // the segment bits the second sort reads (n_segs < 2^mode_seg_bits: segment ~0 sorts last)
+  async_ptr<ModeGather> d_gathers;
+  async_ptr<ModeOut> d_mode_outs;
+  async_ptr<uint64_t> d_mode_keys;  // [2 * bound]
+  async_ptr<uint32_t> d_mode_segs;  // [2 * bound]: segments, sorted segments, then the run starts
+  async_ptr<int32_t> d_mode_off;    // [2 * n_segs + 1]: offsets, cursors
+  async_ptr<unsigned long long> d_mode_res;  // [2 * n_segs]: best, runs
+  async_ptr<uint8_t> d_mode_tmp;
+  size_t mode_tmp_bytes = 0;
+  ModeArgs mode{};
 };
 
 namespace {
@@ -366,18 +380,23 @@ bool query_has_m2(const tskv_query *q) {
 
 uint32_t query_n_medians(const tskv_query *q) { return TSKV_QUERY_N_MEDIANS(q->reserved); }
 uint32_t query_n_increases(const tskv_query *q) { return TSKV_QUERY_N_INCREASES(q->reserved); }
+uint32_t query_n_modes(const tskv_query *q) { return TSKV_QUERY_N_MODES(q->reserved); }
+uint32_t query_n_distincts(const tskv_query *q) { return TSKV_QUERY_N_DISTINCTS(q->reserved); }
 
 // The query the scan runs for a query with column pairs, medians or increases: its projected columns, then every operand that is
 // not one of them as a COUNT column without output (so that the work list, the page gathers, CRC checks, pass 1 and the
 // reader counters treat the operands' pages as they treat a COUNT column's), and per pair, median and increase the
 // operands' places in that table. A median's operand column also computes MIN and MAX in pass 1 (its extreme keys); an increase's
-// operand column computes COUNT (its validity).
+// operand column computes COUNT (its validity), and so does a mode's or distinct's (its n). Modes and distincts share
+// one gather per operand column id.
 struct OperandQuery {
   tskv_query q{};
   std::vector<tskv_agg_column> cols;
   std::vector<PairCol> pairs;          // (off is set by plan_layout)
   std::vector<MedianCol> medians;      // (the offsets are set by plan_layout)
   std::vector<IncreaseCol> increases;  // (the offsets are set by plan_layout)
+  std::vector<ModeGather> gathers;     // (count_off is set by plan_layout)
+  std::vector<ModeOut> mode_outs;      // the modes', then the distincts' outputs
 };
 OperandQuery plan_operand_query(const tskv_query *q) {
   OperandQuery pq;
@@ -417,6 +436,21 @@ OperandQuery plan_operand_query(const tskv_query *q) {
     ic.column_id = op.column_id;
     ic.phys_type = op.phys_type;
     pq.increases.push_back(ic);
+  }
+  const uint32_t n_modes = query_n_modes(q), n_sorted = n_modes + query_n_distincts(q);
+  for (uint32_t k = 0; k < n_sorted; k++) {
+    const tskv_agg_column &op = q->columns[q->n_columns + 2 * q->n_pairs + query_n_medians(q) + query_n_increases(q) + k];
+    uint32_t g = 0;
+    while (g < pq.gathers.size() && pq.gathers[g].column_id != op.column_id) g++;
+    if (g == pq.gathers.size()) {
+      ModeGather mg{};
+      mg.qcol = place(op);
+      pq.cols[mg.qcol].agg_mask |= TSKV_AGG_COUNT;
+      mg.column_id = op.column_id;
+      mg.phys_type = op.phys_type;
+      pq.gathers.push_back(mg);
+    }
+    pq.mode_outs.push_back(ModeOut{g, k >= n_modes ? 1u : 0u});
   }
   pq.q.columns = pq.cols.data();
   pq.q.n_columns = (uint32_t)pq.cols.size();
@@ -586,7 +620,8 @@ bool labels_first_last(const tskv_query *q, const BucketEdges &E) {
 // (an edge scan's buckets come from its edge table, width = 0)
 bool query_shape_ok(const tskv_query *q, bool edges = false) {
   return q->n_buckets != 0 &&
-         (q->n_columns != 0 || q->n_pairs != 0 || query_n_medians(q) != 0 || query_n_increases(q) != 0) && q->columns &&
+         (q->n_columns != 0 || q->n_pairs != 0 || query_n_medians(q) != 0 || query_n_increases(q) != 0 ||
+          query_n_modes(q) != 0 || query_n_distincts(q) != 0) && q->columns &&
          (q->width > 0 || q->n_buckets == 1 || edges);
 }
 
@@ -598,6 +633,8 @@ tskv_output_layout output_layout(const tskv_pages *pages, const tskv_query *q, c
   if (q->n_pairs <= TSKV_MAX_PAIRS) n_out += 4ull * q->n_pairs;  // n, C, M2x, M2y per pair
   if (query_n_medians(q) <= TSKV_MAX_MEDIANS) n_out += query_n_medians(q);
   if (query_n_increases(q) <= TSKV_MAX_INCREASES) n_out += query_n_increases(q);
+  if (query_n_modes(q) <= TSKV_MAX_MODES) n_out += query_n_modes(q);
+  if (query_n_distincts(q) <= TSKV_MAX_DISTINCTS) n_out += query_n_distincts(q);
   uint64_t n_groups = 1;
   if (q->group_by_series) n_groups = selected_slots(pages, q);
   if (tg.on) n_groups = tg.n;
@@ -925,6 +962,23 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
         return TSKV_ERR_INVALID_ARG;
       }
   }
+  const uint32_t n_mode = query_n_modes(q), n_dist = query_n_distincts(q), k0 = 2 * q->n_pairs + n_med + n_inc;
+  if (n_mode > TSKV_MAX_MODES || n_dist > TSKV_MAX_DISTINCTS || (uint64_t)q->n_columns + k0 + n_mode + n_dist > 126) {
+    ctx->set_error("invalid query: at most 8 modes, 8 distincts and 126 columns with every operand");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  for (uint32_t k = k0; k < k0 + n_mode + n_dist; k++) {
+    const tskv_agg_column &op = q->columns[q->n_columns + k];
+    if (op.agg_mask != 0 || op.phys_type < TSKV_PT_I64 || op.phys_type > TSKV_PT_F64) {
+      ctx->set_error("invalid mode / distinct operand: an I64 / U64 / F64 column with agg_mask 0");
+      return TSKV_ERR_INVALID_ARG;
+    }
+    for (uint32_t c = 0; c < q->n_columns + k; c++)
+      if (q->columns[c].column_id == op.column_id && q->columns[c].phys_type != op.phys_type) {
+        ctx->set_error("mode / distinct operand: one column id with two types");
+        return TSKV_ERR_INVALID_ARG;
+      }
+  }
   if (q->n_predicates > TSKV_MAX_PREDICATES || (q->n_predicates && !q->predicates)) {
     ctx->set_error("invalid query: at most 8 field predicates");
     return TSKV_ERR_INVALID_ARG;
@@ -982,6 +1036,14 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
   }
   if (n_med && (q->reserved & TSKV_QUERY_MULTI_RANK)) {
     ctx->set_error("multi-rank scan: medians are not pushed down (their selection state does not merge across ranks)");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  if ((n_mode || n_dist) && slide) {
+    ctx->set_error("sliding windows: modes and distincts are not pushed down");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  if ((n_mode || n_dist) && (q->reserved & TSKV_QUERY_MULTI_RANK)) {
+    ctx->set_error("multi-rank scan: modes and distincts are not pushed down (their state is the values themselves)");
     return TSKV_ERR_UNSUPPORTED;
   }
   if (n_inc) {  // increases pair consecutive rows of one series: a cell must never hold two selected series
@@ -1079,6 +1141,8 @@ struct ScanLayout {
   uint64_t pair_words = 0;
   std::vector<MedianCol> medians;  // medians, with their operands' pass-1 sections and their selection state's offsets
   std::vector<IncreaseCol> increases;  // increases, with their operands' COUNT sections and their sum sections
+  std::vector<ModeGather> gathers;     // the modes' and distincts' gathers, with their operands' COUNT sections
+  std::vector<ModeOut> mode_outs;
 };
 
 // n_cells: cells of the query's grid (a sliding scan: windows); kern_cells: cells of the fused kernels' grid (panes).
@@ -1112,6 +1176,9 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
     out.increases[k].count_off = win.cols[out.increases[k].qcol].count_off;
     out.increases[k].off = win.inc_off[k];
   }
+  out.gathers = oq.gathers;  // (sliding scans refuse modes and distincts)
+  for (ModeGather &mg : out.gathers) mg.count_off = win.cols[mg.qcol].count_off;
+  out.mode_outs = oq.mode_outs;
   if (sliding) {
     for (uint32_t c = 0; c < q->n_columns; c++) {
       const ColState &p = pane.cols[c], &w = win.cols[c];
@@ -1277,6 +1344,17 @@ struct MergePages {
   std::vector<uint64_t> row_off, bm_off;
   uint64_t bytes = 0, read_pages = 0;
 };
+// Whether column group cg can hold selected rows: its series is selected and its time bounds (cg_bounds, needed with time
+// ranges) overlap a time range (filter_column_groups, reader/chunk.rs:12-50).
+bool cg_selected(const tskv_pages *pages, const tskv_query *q, const tskv_time_range *cg_bounds, uint32_t cg) {
+  const tskv_page_desc &td = pages->h_descs[pages->h_cg_time_page[cg]];
+  if (q->series_ids && !std::binary_search(q->series_ids, q->series_ids + q->n_series, td.series_id)) return false;
+  if (!q->n_time_ranges) return true;
+  for (uint32_t r = 0; r < q->n_time_ranges; r++)
+    if (cg_bounds[cg].min_ts <= q->time_ranges[r].max_ts && cg_bounds[cg].max_ts >= q->time_ranges[r].min_ts) return true;
+  return false;
+}
+
 // Refuses (TSKV_ERR_INVALID_ARG, with the page) a page whose type does not match its query column.
 tskv_status plan_merge_pages(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query *q, MergePages *m) {
   const OverlapTables &ov = pages->overlap;
@@ -1285,13 +1363,7 @@ tskv_status plan_merge_pages(tskv_ctx *ctx, const tskv_pages *pages, const tskv_
   for (size_t k = 0; k < op.mcg_cg.size(); k++) {
     const uint32_t cg = op.mcg_cg[k], tp = pages->h_cg_time_page[cg];
     const tskv_page_desc &td = pages->h_descs[tp];
-    if (q->series_ids && !std::binary_search(q->series_ids, q->series_ids + q->n_series, td.series_id)) continue;
-    if (q->n_time_ranges) {  // filter_column_groups (reader/chunk.rs:12-50)
-      bool overlaps = false;
-      for (uint32_t r = 0; r < q->n_time_ranges; r++)
-        overlaps = overlaps || (pages->h_cg_bounds[cg].min_ts <= q->time_ranges[r].max_ts && pages->h_cg_bounds[cg].max_ts >= q->time_ranges[r].min_ts);
-      if (!overlaps) continue;
-    }
+    if (!cg_selected(pages, q, pages->h_cg_bounds.data(), cg)) continue;
     bool any = false;
     for (uint64_t p = (uint64_t)tp + 1; p < pages->n_descs && pages->h_descs[p].phys_type != TSKV_PT_TIME; p++)
       for (uint32_t c = 0; c < q->n_columns; c++)
@@ -1494,6 +1566,37 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
     s->inc.time_key = s->d_inc_keys.get() + n;
     s->inc.n_rec = (uint32_t)n_rec;
     *h2d += lay.increases.size() * sizeof(IncreaseCol) + rec0.size() * 4;
+  }
+  s->n_gathers = (uint32_t)lay.gathers.size();
+  s->n_mode_outs = (uint32_t)lay.mode_outs.size();
+  if (s->n_gathers) {  // (prepare_scan has bounded the keys: s->mode.bound)
+    ModeArgs &A = s->mode;
+    A.n_cells = s->layout.n_cells;
+    A.n_segs = (uint64_t)s->n_gathers * A.n_cells;
+    A.bound = std::max<uint64_t>(A.bound, 1);
+    s->mode_seg_bits = 64 - __builtin_clzll(A.n_segs);
+    size_t t[4] = {0, 0, 0, 0};
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, t[0], (int32_t *)nullptr, (int64_t)(A.n_segs + 1), st);
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, t[1], (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                                               (uint32_t *)nullptr, (int)A.bound, 0, 64, st);
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, t[2], (const uint32_t *)nullptr, (uint32_t *)nullptr, (const uint64_t *)nullptr,
+                                                               (uint64_t *)nullptr, (int)A.bound, 0, s->mode_seg_bits, st);
+    if (e == cudaSuccess) e = cub::DeviceScan::InclusiveScan(nullptr, t[3], (const uint32_t *)nullptr, (uint32_t *)nullptr, ModeMax{}, (int)A.bound, st);
+    s->mode_tmp_bytes = std::max<size_t>(*std::max_element(t, t + 4), 1);
+    if (e == cudaSuccess) e = upload(s->d_gathers, lay.gathers.data(), lay.gathers.size(), st);
+    if (e == cudaSuccess) e = upload(s->d_mode_outs, lay.mode_outs.data(), lay.mode_outs.size(), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_mode_keys, (size_t)(2 * A.bound), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_mode_segs, (size_t)(2 * A.bound), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_mode_off, (size_t)(2 * A.n_segs + 1), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_mode_res, (size_t)(2 * A.n_segs), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_mode_tmp, s->mode_tmp_bytes, st);
+    A.keys = s->d_mode_keys.get();
+    A.segs = s->d_mode_segs.get();
+    A.off = s->d_mode_off.get();
+    A.cursor = s->d_mode_off.get() + A.n_segs + 1;
+    A.best = s->d_mode_res.get();
+    A.runs = s->d_mode_res.get() + A.n_segs;
+    *h2d += lay.gathers.size() * sizeof(ModeGather) + lay.mode_outs.size() * sizeof(ModeOut);
   }
   if (e == cudaSuccess) e = stream_alloc(s->d_aux, AUX_WORDS, st);
   if (e == cudaSuccess) e = stream_alloc(s->d_values, s->layout.n_out * s->layout.n_cells, st);
@@ -2268,8 +2371,40 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   const uint32_t n_user = q->n_columns;
   OperandQuery pq = plan_operand_query(q);
   pq.q.columns = pq.cols.data();
+  cudaSetDevice(ctx->device);  // (before the sizing below, which may compute the page set's time bounds)
+  // modes and distincts: the key buffer holds every row of each gather's operand pages in the column groups that can hold
+  // selected rows, sized here so that run and enqueue neither allocate nor synchronise
+  uint64_t mode_bound = 0;
+  if (!pq.gathers.empty()) {
+    if (((uint64_t)pq.gathers.size() * L.n_cells) >> 31) {
+      ctx->set_error("mode / distinct: 2^31 or more gathered columns times cells (the sorts count segments in int)");
+      return TSKV_ERR_UNSUPPORTED;
+    }
+    std::vector<tskv_time_range> cg_bounds;  // (the page set keeps them on the host only with chunk files)
+    if (q->n_time_ranges && pages->n_cg) {
+      ensure_time_bounds(ctx, pages);
+      cg_bounds.resize(pages->n_cg);
+      if (!pages->d_cg_bounds || cudaMemcpy(cg_bounds.data(), pages->d_cg_bounds.get(), pages->n_cg * sizeof(tskv_time_range),
+                                            cudaMemcpyDeviceToHost) != cudaSuccess) {
+        ctx->set_error(std::string("mode / distinct: column-group time bounds: ") + cudaGetErrorString(cudaGetLastError()));
+        return TSKV_ERR_CUDA;
+      }
+    }
+    for (const ModeGather &mg : pq.gathers) {
+      uint64_t rows = 0;
+      for (uint32_t cg = 0; cg < pages->n_cg; cg++) {
+        if (!cg_selected(pages, q, cg_bounds.data(), cg)) continue;
+        for (uint64_t p = (uint64_t)pages->h_cg_time_page[cg] + 1; p < pages->n_descs && pages->h_descs[p].phys_type != TSKV_PT_TIME; p++)
+          if (pages->h_descs[p].column_id == mg.column_id) rows += pages->h_descs[p].num_values;
+      }
+      mode_bound += rows;
+    }
+    if (mode_bound >= TSKV_MAX_SORTED_ROWS) {
+      ctx->set_error("mode / distinct: the operands' selectable rows reach TSKV_MAX_SORTED_ROWS (the sorts count items in int)");
+      return TSKV_ERR_UNSUPPORTED;
+    }
+  }
   q = &pq.q;
-  cudaSetDevice(ctx->device);
   bool has_sel = false;  // any FIRST / LAST
   for (uint32_t c = 0; c < q->n_columns; c++) has_sel |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
   uint32_t slot_bits = 0;
@@ -2293,6 +2428,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   s->sl = lay.sl;
   s->kern_sl = lay.kern_sl;
   uint64_t h2d = 0;
+  s->mode.bound = mode_bound;
   if ((st = alloc_scan(ctx, pages, q, tg, slide != 0, E, lay, s, &h2d)) != TSKV_OK) {
     delete s;
     return st;
@@ -2311,6 +2447,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   P.task_counter = reinterpret_cast<uint32_t *>(s->d_aux.get());
   P.status = s->d_status;
   P.err_page = s->d_err_page;
+  s->mode.status = s->d_status;
+  s->mode.err_page = s->d_err_page;
   P.stats = s->d_stats;
   P.n_ranges = q->n_time_ranges;
   for (uint32_t k = 0; k < q->n_time_ranges; k++) P.ranges[k] = q->time_ranges[k];
@@ -2558,7 +2696,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     cudaStreamWaitEvent(ctx->stream.get(), ev_done, 0);  // join
     launches++;
   }
-  if (!capturing && !s->n_m2 && !s->n_pairs && !s->n_medians && !s->n_increases) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
+  if (!capturing && !s->n_m2 && !s->n_pairs && !s->n_medians && !s->n_increases && !s->n_gathers) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());
   if (s->n_combine) {  // sliding windows: every window folds its panes (it writes every array the kernels fill)
     const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
     k_window_combine<<<dim3(std::max(1u, bx), s->n_combine), 256, 0, ctx->stream.get()>>>(
@@ -2596,7 +2734,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       cudaStreamWaitEvent(ctx->stream.get(), s->ev_m2_join[b].get(), 0);
       launches++;
     }
-    if (!capturing && !s->n_pairs && !s->n_medians && !s->n_increases) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes pass 2)
+    if (!capturing && !s->n_pairs && !s->n_medians && !s->n_increases && !s->n_gathers) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes pass 2)
   }
   if (s->n_pairs) {  // column pairs: pass 1 (n, sums, extremes), the shifts, pass 2 (co-moments); overlap merge rows first
     const bool edges = s->params.edges != nullptr;
@@ -2622,7 +2760,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       CU_TRY(ctx, cudaLaunchKernel(fn, dim3(px, s->n_pairs), dim3(128), args, 0, ctx->stream.get()));
       launches++;
     }
-    if (!capturing && !s->n_medians && !s->n_increases) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the pair passes)
+    if (!capturing && !s->n_medians && !s->n_increases && !s->n_gathers) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the pair passes)
   }
   if (s->n_medians) {  // medians: the targets from pass 1, then MEDIAN_PASSES fixed selection passes (merged rows first)
     const bool edges = s->params.edges != nullptr;
@@ -2646,7 +2784,7 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
       k_median_step<<<dim3(std::max(1u, wx), s->n_medians), 256, 0, ctx->stream.get()>>>(mp, s->med, n_cells);
       launches += 2;
     }
-    if (!capturing && !s->n_increases) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the selection passes)
+    if (!capturing && !s->n_increases && !s->n_gathers) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the selection passes)
   }
   if (s->n_increases) {  // increases: the pages' pairs and records and the merged rows' records, then the boundaries
     const bool edges = s->params.edges != nullptr;
@@ -2677,7 +2815,43 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
                                                 s->inc_slot_sort_bits, ctx->stream.get()));
     k_increase_stitch<<<nb, 256, 0, ctx->stream.get()>>>(s->d_state.get(), ip, s->inc, keys + 4 * n, idx + 2 * n, n);
     launches += 4;  // (a sort counts as one launch)
-    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the increase kernels)
+    if (!capturing && !s->n_gathers) cudaEventRecord(s->ev_bin[N_BINS].get(), ctx->stream.get());  // (the fused time includes the increase kernels)
+  }
+  if (s->n_gathers) {  // modes and distincts: the slices from pass 1's n, the keys (merged rows too), the sorts, the runs
+    const ModeArgs &A = s->mode;
+    cudaStream_t stream = ctx->stream.get();
+    const uint32_t sx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((A.n_segs + 256) / 256, 4096));
+    const uint32_t kx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((A.bound + 255) / 256, 4096));
+    const uint32_t rx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((A.bound + 8 * 32 * MODE_ITEMS - 1) / (8 * 32 * MODE_ITEMS), 4096));
+    const uint32_t px = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)pages->n_descs + 127) / 128, (uint64_t)ctx->sm_count * 16));
+    // keys [slices, then sorted | after the key sort], segments [slices, then sorted | after the key sort, then the run
+    // starts]; the max-scan writes the runs' first positions over the second half of the keys
+    uint64_t *k2 = A.keys + A.bound;
+    uint32_t *s2 = A.segs + A.bound, *first = reinterpret_cast<uint32_t *>(k2);
+    const ModeGather *gp = s->d_gathers.get();
+    k_mode_counts<<<sx, 256, 0, stream>>>(s->d_state.get(), gp, A);
+    size_t tmp = s->mode_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceScan::ExclusiveSum(s->d_mode_tmp.get(), tmp, A.off, (int64_t)(A.n_segs + 1), stream));
+    CU_TRY(ctx, cudaMemcpyAsync(A.cursor, A.off, A.n_segs * sizeof(int32_t), cudaMemcpyDeviceToDevice, stream));
+    CU_TRY(ctx, cudaMemsetAsync(A.segs, 0xff, A.bound * sizeof(uint32_t), stream));
+    const void *fn = s->params.edges ? (const void *)k_scan_mode<true> : (const void *)k_scan_mode<false>;
+    void *args[] = {(void *)&s->params, (void *)&gp, (void *)&s->mode};
+    CU_TRY(ctx, cudaLaunchKernel(fn, dim3(px, s->n_gathers), dim3(128), args, 0, stream));
+    launches += 3;
+    if (s->merge.n_rows && s->n_merge_pages) {
+      k_merge_mode_rows<<<dim3((uint32_t)((s->merge.n_rows + 127) / 128), s->n_gathers), 128, 0, stream>>>(s->params, s->merge, gp, A);
+      launches++;
+    }
+    tmp = s->mode_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_mode_tmp.get(), tmp, A.keys, k2, A.segs, s2, (int)A.bound, 0, 64, stream));
+    tmp = s->mode_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_mode_tmp.get(), tmp, s2, A.segs, k2, A.keys, (int)A.bound, 0, s->mode_seg_bits, stream));
+    k_mode_heads<<<kx, 256, 0, stream>>>(A, s2);
+    tmp = s->mode_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceScan::InclusiveScan(s->d_mode_tmp.get(), tmp, (const uint32_t *)s2, first, ModeMax{}, (int)A.bound, stream));
+    k_mode_runs<<<rx, 256, 0, stream>>>(A, first);
+    launches += 5;  // (a sort or scan counts as one launch)
+    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), stream);  // (the fused time includes the mode kernels)
   }
   if (!capturing) cudaEventRecord(s->ev1.get(), ctx->stream.get());
   CU_TRY(ctx, cudaGetLastError());
@@ -2814,11 +2988,11 @@ tskv_status tskvgpu_scan_work_list(tskv_ctx *ctx, tskv_scan *s, uint32_t *n_buck
   return TSKV_OK;
 }
 
-// Medians keep no mergeable partial state: the exchange calls refuse a scan with medians.
+// Medians, modes and distincts keep no mergeable partial state: the exchange calls refuse a scan with any of them.
 static tskv_status refuse_medians(tskv_ctx *ctx, const tskv_scan *s, const char *call) {
-  if (!s->n_medians) return TSKV_OK;
+  if (!s->n_medians && !s->n_gathers) return TSKV_OK;
   std::lock_guard<std::mutex> lock(ctx->mu);
-  ctx->set_error(std::string(call) + ": a scan with medians has no mergeable partial state");
+  ctx->set_error(std::string(call) + ": a scan with medians, modes or distincts has no mergeable partial state");
   return TSKV_ERR_UNSUPPORTED;
 }
 
@@ -2945,6 +3119,10 @@ static tskv_status finalize_device(tskv_ctx *ctx, tskv_scan *s) {
     k_finalize_increases<<<dim3((uint32_t)((L.n_cells + 255) / 256), s->n_increases), 256, 0, ctx->stream.get()>>>(
         s->d_state.get(), s->d_increases.get(), s->n_out + 4 * s->n_pairs + s->n_medians, L.n_cells, L.bitmap_stride, s->d_values.get(),
         s->d_validity.get());
+  if (s->n_mode_outs)
+    k_finalize_modes<<<dim3((uint32_t)((L.n_cells + 255) / 256), s->n_mode_outs), 256, 0, ctx->stream.get()>>>(
+        s->mode, s->d_gathers.get(), s->d_mode_outs.get(), s->n_out + 4 * s->n_pairs + s->n_medians + s->n_increases, L.bitmap_stride,
+        s->d_values.get(), s->d_validity.get());
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;
 }

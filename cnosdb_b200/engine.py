@@ -218,17 +218,24 @@ class TskvError(RuntimeError):
         self.page = page
 
 
+# the aggregates without a mask bit: each makes its column an operand of its own kind
+PSEUDO_AGGS = ("median", "increase", "mode", "count_distinct")
+
+
 class PushedAggregate:
     """One projected value column with its aggregate set (extends PushedAggregateFunction::Count). "median" has no mask
     bit: it makes the column a median operand (after the pairs' operands, agg_mask 0), and a column that asks for nothing
     else has no projected entry. "increase" (increase(time, x ORDER BY time)) likewise makes it an increase operand, after
-    the medians' operands."""
+    the medians' operands; "mode" (mode(x)) a mode operand, after the increases' operands; and "count_distinct"
+    (COUNT(DISTINCT x)) a distinct operand, after the modes' operands."""
 
     def __init__(self, column_id, phys_type, aggs):
         self.column_id = int(column_id)
         self.phys_type = int(phys_type)
         self.median = False
         self.increase = False
+        self.mode = False
+        self.count_distinct = False
         if isinstance(aggs, int):
             self.agg_mask = aggs
         else:
@@ -237,8 +244,8 @@ class PushedAggregate:
                 if a == "median":
                     self.median = True
                     continue
-                if a == "increase":
-                    self.increase = True
+                if a in ("increase", "mode", "count_distinct"):
+                    setattr(self, a, True)
                     continue
                 # var* / stddev* ask the scan for COUNT | M2; ScanResult.column derives them
                 self.agg_mask |= (TSKV_AGG_COUNT | TSKV_AGG_M2) if a in STAT_AGGS else AGG_BITS[a]
@@ -283,13 +290,15 @@ class QueryOption:
         proj = self.projected()
         meds = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "median", False)]
         incs = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "increase", False)]
+        modes = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "mode", False)]
+        dists = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "count_distinct", False)]
         q.reserved = ((cabi.TSKV_QUERY_MULTI_RANK if self.multi_rank else 0) | cabi.query_medians(len(meds)) |
-                      cabi.query_increases(len(incs)))
-        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))] + meds + incs
+                      cabi.query_increases(len(incs)) | cabi.query_modes(len(modes)) | cabi.query_distincts(len(dists)))
+        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))] + meds + incs + modes + dists
         cols = (cabi.AggColumn * max(1, len(proj) + len(ops)))()
         for i, c in enumerate(proj):
             cols[i].column_id, cols[i].phys_type, cols[i].agg_mask = c.column_id, c.phys_type, c.agg_mask
-        for i, (cid, pt) in enumerate(ops):  # the pairs', medians' and increases' operands follow the projected columns
+        for i, (cid, pt) in enumerate(ops):  # the pairs', medians', increases', modes' and distincts' operands follow
             cols[len(proj) + i].column_id, cols[len(proj) + i].phys_type = cid, pt
         q.columns = cols
         q.n_columns = len(proj)
@@ -308,14 +317,16 @@ class QueryOption:
         return q
 
     def projected(self):
-        """The columns with a projected entry (an aggregate other than median and increase)."""
-        return [c for c in self.columns if c.agg_mask or not (getattr(c, "median", False) or getattr(c, "increase", False))]
+        """The columns with a projected entry (an aggregate other than median, increase, mode and count_distinct)."""
+        return [c for c in self.columns if c.agg_mask or not any(getattr(c, a, False) for a in PSEUDO_AGGS)]
 
     def output_names(self):
         return ([(c.column_id, cabi.AGG_NAMES[a]) for c in self.projected() for a in c.agg_list()] +
                 [(("pair", k), r) for k in range(len(self.pairs)) for r in PAIR_RAW] +
                 [(c.column_id, "median") for c in self.columns if getattr(c, "median", False)] +
-                [(c.column_id, "increase") for c in self.columns if getattr(c, "increase", False)])
+                [(c.column_id, "increase") for c in self.columns if getattr(c, "increase", False)] +
+                [(c.column_id, "mode") for c in self.columns if getattr(c, "mode", False)] +
+                [(c.column_id, "count_distinct") for c in self.columns if getattr(c, "count_distinct", False)])
 
 
 class ScanResult:
@@ -347,8 +358,8 @@ class ScanResult:
 
     def column(self, column_id, agg):
         """(typed values, validity) of one output column, shaped [n_groups, n_buckets]. agg may also name one of STAT_AGGS
-        (var, var_samp, var_pop, stddev, stddev_samp, stddev_pop), derived from the column's count and m2, or "median" /
-        "increase" (the operand's type)."""
+        (var, var_samp, var_pop, stddev, stddev_samp, stddev_pop), derived from the column's count and m2, "median" /
+        "increase" / "mode" (the operand's type) or "count_distinct" (u64)."""
         if agg in STAT_AGGS:
             n, _ = self.column(column_id, "count")
             m2, ok = self.column(column_id, "m2")
@@ -356,7 +367,7 @@ class ScanResult:
         j = self.names.index((column_id, agg))
         raw = self.values[j]
         pt = self.phys[column_id]
-        if agg == "count":
+        if agg in ("count", "count_distinct"):
             v = raw.view(np.uint64)
         elif agg in ("mean", "m2") or pt == TSKV_PT_F64:
             v = raw.view(np.float64)
@@ -612,6 +623,11 @@ class Engine:
                 raise ValueError("median and multi_rank: medians have no mergeable partial state")
         if slide is not None and any(getattr(c, "increase", False) for c in query.columns):
             raise ValueError("increase and slide: sliding windows do not push increases down")
+        if any(getattr(c, "mode", False) or getattr(c, "count_distinct", False) for c in query.columns):
+            if slide is not None:
+                raise ValueError("mode / count_distinct and slide: sliding windows do not push them down")
+            if getattr(query, "multi_rank", False):
+                raise ValueError("mode / count_distinct and multi_rank: their state is the values themselves")
 
     @staticmethod
     def _edges(edges, slide):

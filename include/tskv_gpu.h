@@ -247,6 +247,40 @@ typedef struct tskv_query {
 #define TSKV_MAX_INCREASES 8
 #define TSKV_QUERY_INCREASES(n) (((uint32_t)(n) & 0xffu) << 16)
 #define TSKV_QUERY_N_INCREASES(flags) (((uint32_t)(flags) >> 16) & 0xffu)
+/* Modes and distinct counts: mode(x) (CnosDB's ModeAccumulator) and COUNT(DISTINCT x), exact. Bits 24..27 of the flags
+ * word hold n_modes (TSKV_QUERY_MODES(n) / TSKV_QUERY_N_MODES(flags)), bits 28..31 n_distincts (TSKV_QUERY_DISTINCTS(n)
+ * / TSKV_QUERY_N_DISTINCTS(flags)). The n_modes entries of `columns` after the increases' operands are the modes'
+ * operands, and the n_distincts entries after those the distincts' operands: column_id and phys_type (I64 / U64 / F64) of
+ * each, agg_mask 0; n_columns + 2 * n_pairs + n_medians + n_increases + n_modes + n_distincts <= 126. Both take the
+ * operand's values in the rows a median selects, NULLs left out. Two values are equal iff their bit patterns are: f64
+ * -0.0 and +0.0 differ, and two NaNs are equal only with equal bits (ModeAccumulator counts in a HashMap keyed by
+ * DataFusion's ScalarValue, whose Eq / Hash compare an f64 by to_bits(); that part is upstream DataFusion's and not in the
+ * CnosDB tree). Per cell each mode adds one output after the increases' outputs, in the operand's type, valid iff the cell
+ * holds a value: the value that occurs most often, and of tied values the smallest in the type's order (f64: IEEE
+ * totalOrder; the reference picks any tied value). Each distinct adds one u64 output after the modes' outputs: the number
+ * of distinct values in the cell, always valid (0 in a cell without a value). Computed per distinct operand column id
+ * (a gather): pass 1 gives every cell's n (the operand's kernel mask gains COUNT; an operand that is not a projected
+ * column is read like a COUNT column with no output), an exclusive sum of the n gives each cell a slice of one key buffer,
+ * one lane per operand page writes each selected value's order key into its cell's slice (the merged rows of the overlap
+ * merge groups one thread per row), two radix sorts order the buffer by (slice, key), and a pass over the sorted keys
+ * counts each slice's runs of equal keys and keeps its longest. A cell whose gathered keys do not number its pass-1 n is reported as
+ * TSKV_ERR_BITSET_MISMATCH with page ~0 (only a decode error pass 1 reports first can cause it). Buffers grow with the
+ * selected rows, not with the cells: the keys take 24 bytes per row of the operand pages whose column group is selected
+ * and overlaps the time ranges. Refused before any launch: TSKV_ERR_INVALID_ARG for n_modes > TSKV_MAX_MODES,
+ * n_distincts > TSKV_MAX_DISTINCTS, an operand with a non-zero agg_mask or a BOOL / TIME / unknown type, an operand id
+ * projected with another type, or more than 126 columns; TSKV_ERR_UNSUPPORTED for sliding windows (slide != width),
+ * TSKV_QUERY_MULTI_RANK (the state is the values themselves), operands whose selectable rows, summed over the gathers
+ * (they share one buffer), could reach TSKV_MAX_SORTED_ROWS, and gathers times cells of 2^31 or more (the sorts and
+ * scans count in int).
+ * tskvgpu_scan_partials, _exchange_view, _exchange and _merge_gathered refuse a scan with modes or distincts. Counters:
+ * as for medians; kernel_launches and elapsed_fused_ms include the gather, sort and run kernels. */
+#define TSKV_MAX_MODES 8
+#define TSKV_MAX_DISTINCTS 8
+#define TSKV_MAX_SORTED_ROWS 0x7fffffffu
+#define TSKV_QUERY_MODES(n) (((uint32_t)(n) & 0xfu) << 24)
+#define TSKV_QUERY_N_MODES(flags) (((uint32_t)(flags) >> 24) & 0xfu)
+#define TSKV_QUERY_DISTINCTS(n) (((uint32_t)(n) & 0xfu) << 28)
+#define TSKV_QUERY_N_DISTINCTS(flags) (((uint32_t)(flags) >> 28) & 0xfu)
 
 /* Result layout. Outputs are dense: for output column j (query columns in order, and inside a
  * column the set agg bits in ascending bit order) and cell c = group * n_buckets + bucket:

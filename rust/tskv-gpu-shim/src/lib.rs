@@ -26,6 +26,8 @@ use std::sync::Arc;
 pub use sys::{tskv_agg_column, tskv_field_predicate, tskv_page_desc, tskv_time_range, tskv_tombstone};
 pub use sys::{tskv_query_medians, tskv_query_n_medians, TSKV_MAX_MEDIANS, TSKV_MAX_MEDIAN_CELLS};
 pub use sys::{tskv_query_increases, tskv_query_n_increases, TSKV_MAX_INCREASES};
+pub use sys::{tskv_query_distincts, tskv_query_modes, tskv_query_n_distincts, tskv_query_n_modes};
+pub use sys::{TSKV_MAX_DISTINCTS, TSKV_MAX_MODES, TSKV_MAX_SORTED_ROWS};
 
 /// What a failed call reports; maps onto `TskvError` as INTEGRATION.md section 2 lists.
 #[derive(Debug, Clone)]

@@ -56,6 +56,28 @@ pub const fn tskv_query_increases(n: u32) -> u32 {
 pub const fn tskv_query_n_increases(flags: u32) -> u32 {
     (flags >> 16) & 0xff
 }
+/// At most this many modes; their count sits in bits 24..27 of tskv_query.reserved (see tskv_gpu.h).
+pub const TSKV_MAX_MODES: u32 = 8;
+/// At most this many distinct counts; their count sits in bits 28..31 of tskv_query.reserved.
+pub const TSKV_MAX_DISTINCTS: u32 = 8;
+/// Modes and distincts are refused when their operands' selectable rows could reach this many.
+pub const TSKV_MAX_SORTED_ROWS: u32 = 0x7fff_ffff;
+/// TSKV_QUERY_MODES(n): the flags-word bits of n modes.
+pub const fn tskv_query_modes(n: u32) -> u32 {
+    (n & 0xf) << 24
+}
+/// TSKV_QUERY_N_MODES(flags): the modes of a flags word.
+pub const fn tskv_query_n_modes(flags: u32) -> u32 {
+    (flags >> 24) & 0xf
+}
+/// TSKV_QUERY_DISTINCTS(n): the flags-word bits of n distinct counts.
+pub const fn tskv_query_distincts(n: u32) -> u32 {
+    (n & 0xf) << 28
+}
+/// TSKV_QUERY_N_DISTINCTS(flags): the distinct counts of a flags word.
+pub const fn tskv_query_n_distincts(flags: u32) -> u32 {
+    (flags >> 28) & 0xf
+}
 
 pub const TSKV_UPLOAD_VERIFY_CRC: u32 = 1;
 pub const TSKV_UPLOAD_HOST_RESIDENT: u32 = 2;
