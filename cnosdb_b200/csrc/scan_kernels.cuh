@@ -864,6 +864,16 @@ __device__ __forceinline__ bool locate_bucket(const ScanParams &P, int64_t t, Bu
   return true;
 }
 
+// Upper bound of bucket idx + 1, for a floor-regime bucket idx that ends at hi: locate_bucket's next-bucket step (the
+// next edge, or hi + width cut at floor_cap). hi itself when no bucket follows in that regime.
+template <bool EDGES>
+__device__ __forceinline__ int64_t next_bucket_hi(const ScanParams &P, uint32_t idx, int64_t hi) {
+  if (idx + 1 >= P.n_buckets) return hi;
+  if constexpr (EDGES) return __ldg(P.edges + idx + 2) - 1;
+  const uint64_t room = (uint64_t)P.floor_cap - (uint64_t)hi;
+  return (int64_t)((uint64_t)hi + (room < (uint64_t)P.width ? room : (uint64_t)P.width));
+}
+
 // Closed time ranges (TimeRange::contains, predicate/domain.rs:95-98): is t selected, and over which
 // inclusive interval [lo, hi] around t does that answer stay the same?
 __device__ __forceinline__ bool range_span(const ScanParams &P, int64_t t, int64_t &lo, int64_t &hi) {
@@ -1120,11 +1130,9 @@ __device__ __forceinline__ void reduce_staged(const ScanParams &P, uint64_t *sta
   __syncwarp();
 }
 
-// Every lane parks its partial (identities unless `live`) in staging slot `seq`, the lane `meta_lane` records the slot's
-// (query column << 32) | cell, and every NS slots the warp reduces them. Called by all 32 lanes.
-template <int VK, int NS, bool M2 = false>
-__device__ __forceinline__ void stage_partial(const ScanParams &P, uint64_t *stab, uint64_t *stage, uint32_t &seq, bool live,
-                                              const ValueAcc<VK> &va, bool meta_lane, uint64_t gcell) {
+// This lane's partial (identities unless `live`) into its column of staging slot `seq`.
+template <int VK, bool M2 = false>
+__device__ __forceinline__ void stage_lane(uint64_t *stage, uint32_t seq, bool live, const ValueAcc<VK> &va) {
   uint64_t *q = stage + (size_t)seq * FLUSH_Q * 32 + (threadIdx.x & 31);
   q[0] = live ? va.count : 0;
   q[32] = live ? va.sum : 0;  // 0 bits == +0.0
@@ -1133,6 +1141,14 @@ __device__ __forceinline__ void stage_partial(const ScanParams &P, uint64_t *sta
     q[96] = live ? (uint64_t)va.kmin : (uint64_t)INT64_MAX;
     q[128] = live ? (uint64_t)va.kmax : (uint64_t)INT64_MIN;
   }
+}
+
+// Every lane parks its partial (identities unless `live`) in staging slot `seq`, the lane `meta_lane` records the slot's
+// (query column << 32) | cell, and every NS slots the warp reduces them. Called by all 32 lanes.
+template <int VK, int NS, bool M2 = false>
+__device__ __forceinline__ void stage_partial(const ScanParams &P, uint64_t *stab, uint64_t *stage, uint32_t &seq, bool live,
+                                              const ValueAcc<VK> &va, bool meta_lane, uint64_t gcell) {
+  stage_lane<VK, M2>(stage, seq, live, va);
   if (meta_lane) stage[NS * FLUSH_Q * 32 + seq] = gcell;
   if (++seq == NS) {
     reduce_staged<VK, NS, M2>(P, stab, stage, seq);
@@ -1574,6 +1590,112 @@ __device__ __forceinline__ void scan_chunk_seg(const ScanParams &P, uint32_t ite
         row = r;
       }
       row = n_rows;  // nothing is left for the segment loop below
+    }
+  }
+
+  // ---- Lockstep schedule (simple8b timestamps, GROUP BY bucket / tags / edges / labels, no FIRST / LAST, at most one time
+  // range, no tombstones). When all 32 lanes hold rows, start and end at the same row, have the same query column and
+  // group, and their first rows lie in one bucket or the next (pages cut into equal parts: C4's jittered pages), the warp
+  // walks the rows one at a time in all lanes together and keeps ONE bucket schedule: bucket bidx = [blo, bhi] and the
+  // bound bhi2 of the next one. Every lane still decodes and compares its own timestamps. A lane whose row first passes
+  // bhi parks its partial of bidx in its column of staging slot `staged` and goes on accumulating bidx + 1 in the same
+  // registers; once every lane has crossed, the slot is committed and the schedule steps. This takes the segment head,
+  // the alignment reduction and the flush vote off every bucket, and no lane runs a row trip another lane does not need.
+  // The lanes' runs and the order of the staged slots are the ones the segment loop makes for such a warp. A row outside
+  // [blo, bhi2] (a gap, an empty bucket, the last bucket, time going backwards) or outside the time range, or a decode
+  // error at a lane's bucket end, hands the warp to the segment loop at that row, before it is consumed. On C4 the step
+  // follows the instructions per row, not the cycles the segment head kept a warp waiting (DESIGN.md §5), so the row is
+  // kept lean: one reduction decides the warp's step, every row the walk takes is inside the range (the range's bounds
+  // clip the lane's window instead of being tested per row), and a chunk with lanes that hold no rows keeps the segment
+  // loop rather than predicating every row on them.
+  if constexpr (TK == TK_S8B && VK != VK_GEN && !SEL && !M2) {
+    const int64_t tr_lo = P.n_ranges ? P.ranges[0].min_ts : INT64_MIN, tr_hi = P.n_ranges ? P.ranges[0].max_ts : INT64_MAX;
+    if ((P.width > 0 || EDGES) && !P.group_by_series && P.n_ranges <= 1 && tr_lo <= tr_hi && !P.has_tomb &&
+        __all_sync(FULL, row < n_rows)) {
+      const bool located = locate_bucket<EDGES>(P, pend_t, bk) && bk.floor_regime;
+      // the first bucket: the earliest of the lanes' (a part that starts on a bucket edge has lanes in the next one too)
+      const uint32_t b0 = __reduce_min_sync(FULL, located ? bk.idx : 0xffffffffu);
+      const bool agree = located & (pend_t >= tr_lo) & (pend_t <= tr_hi) &
+                         (__shfl_sync(FULL, row, 0) == row) & (__shfl_sync(FULL, n_rows, 0) == n_rows) &
+                         (__shfl_sync(FULL, qcol, 0) == qcol) &
+                         (__shfl_sync(FULL, (uint32_t)group_base, 0) == (uint32_t)group_base) & (bk.idx - b0 <= 1u);
+      if (__all_sync(FULL, agree)) {
+        const int src = __ffs(__ballot_sync(FULL, bk.idx == b0)) - 1;
+        uint32_t bidx = b0;
+        int64_t blo = (int64_t)shfl_u64((uint64_t)bk.lo, src), bhi = (int64_t)shfl_u64((uint64_t)bk.hi, src);
+        int64_t bhi2 = next_bucket_hi<EDGES>(P, bidx, bhi);
+        const uint64_t col = ((uint64_t)qcol << 32) | (uint32_t)group_base;
+        int64_t t = pend_t;
+        bool crossed = bk.idx != b0;  // this lane's rows have reached bucket bidx + 1
+        if (crossed) stage_lane<VK>(stage, staged, false, va);  // (it has no row in bucket bidx)
+        // this lane's next row must lie in [wlo, wlo + wspan]: in its bucket or the next one, and inside the range
+        int64_t wlo = 0;
+        uint64_t wspan = 0;
+        auto window = [&]() {
+          const int64_t lo = crossed ? bhi + 1 : blo, hi = bhi2 < tr_hi ? bhi2 : tr_hi;
+          wlo = lo > tr_lo ? lo : tr_lo;
+          wspan = (uint64_t)hi - (uint64_t)wlo;  // (t lies in the window when it is set: never empty)
+        };
+        window();
+        // slot `staged` of bucket bidx is complete: the lanes that have not filled their column there hold identities
+        auto commit = [&](bool filled) {
+          if (!filled) stage_lane<VK>(stage, staged, false, va);
+          if (lane == 0) stage[NS * FLUSH_Q * 32 + staged] = col + bucket_cell<EDGES>(P, bidx);
+          if (++staged == NS) {
+            reduce_staged<VK, NS>(P, stab, stage, staged);
+            staged = 0;
+          }
+        };
+#pragma unroll 1
+        while (row < n_rows) {
+          const bool up = t > bhi;  // row `row` lies past bucket bidx
+          const bool cross = up && !crossed;
+          // (the segment loop checks the cursors where a lane's segment ends: here, where the lane crosses)
+          const bool bad = (uint64_t)t - (uint64_t)wlo > wspan ||
+                           (cross && (cursor_exhausted(tcur) || (VK == VK_GOR ? vcur_g.failed() : cursor_exhausted(vcur_d))));
+          // one reduction for the warp's next step: 0 = a lane leaves the schedule, 2 = every lane is past bucket bidx
+          const uint32_t step = __reduce_min_sync(FULL, bad ? 0u : up ? 2u : 1u);
+          if (step == 0) break;
+          if (cross) {
+            va.fold(pt, NARROW);
+            stage_lane<VK>(stage, staged, va.count != 0, va);
+            va.reset(NARROW);
+            crossed = true;
+            window();
+          }
+          if (step == 2) {
+            commit(true);
+            bidx++;
+            blo = bhi + 1;
+            bhi = bhi2;
+            bhi2 = next_bucket_hi<EDGES>(P, bidx, bhi);
+            crossed = false;
+            window();
+          }
+          // the next row's timestamp first: its chain runs beside the value's (past the last row this runs one value too
+          // far - harmless)
+          const int64_t tn = (int64_t)tcur.next();
+          bool vv, kept;
+          row_value(true, vv, kept);
+          if (kept) n_inrange++;
+          t = tn;
+          row++;
+        }
+        // At the end of the rows every lane closes bucket bidx; at a handoff only the lanes already in bidx + 1 have closed
+        // it (their partials are committed, the other lanes keep their run of bidx for the segment loop).
+        const bool done = row >= n_rows;
+        if (done && !crossed) {
+          va.fold(pt, NARROW);
+          stage_lane<VK>(stage, staged, va.count != 0, va);
+        }
+        const bool filled = crossed || done;
+        if (__any_sync(FULL, filled)) commit(filled);
+        have_run = crossed || !done;
+        run_idx = crossed ? bidx + 1 : bidx;
+        pend_t = t;
+        bk.valid = false;
+        if (done) check_values();
+      }
     }
   }
 
