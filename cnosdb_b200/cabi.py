@@ -93,6 +93,21 @@ def query_n_distincts(flags):
     return (int(flags) >> 28) & 0xF
 
 
+# gauges (gauge_agg(time, x)): n_gauges in bits 1..4 of tskv_query.reserved, operands after the distincts', 9 outputs each
+# (see include/tskv_gpu.h)
+TSKV_MAX_GAUGES = 8
+
+
+def query_gauges(n):
+    """TSKV_QUERY_GAUGES(n): the flags-word bits of n gauges."""
+    return (int(n) & 0xF) << 1
+
+
+def query_n_gauges(flags):
+    """TSKV_QUERY_N_GAUGES(flags)."""
+    return (int(flags) >> 1) & 0xF
+
+
 TSKV_UPLOAD_VERIFY_CRC = 1
 TSKV_UPLOAD_HOST_RESIDENT = 2
 TSKV_UPLOAD_VERIFY_ON_READ = 4

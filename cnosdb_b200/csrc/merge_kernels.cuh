@@ -362,4 +362,18 @@ __global__ void __launch_bounds__(128) k_merge_mode_rows(const ScanParams P, con
   A.segs[pos] = (uint32_t)seg;
 }
 
+// The gauges over the merged rows (k_gauge_scan's pages): one thread per (merge row, gauge = blockIdx.y); the leader of a
+// merged row that survives the row-level filters (merged_row) and holds a merged value of the operand (merge_value)
+// appends a record of its one point.
+__global__ void __launch_bounds__(128) k_gauge_merge_rows(const ScanParams P, const MergeParams M, const GaugeCol *gcols, const GaugeArgs A) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  MergedRow mr;
+  if (i >= M.n_rows || !merged_row(P, M, i, mr)) return;
+  const GaugeCol gc = gcols[blockIdx.y];
+  uint64_t v;
+  if (!merge_value(P, M, gc.qcol, mr.series, mr.t, mr.s0, mr.s1, v)) return;
+  const uint32_t slot = (uint32_t)M.cg_slot[M.mcg_cg[merge_mcg_of(M, i)]];
+  gauge_emit(A, (uint64_t)blockIdx.y * A.kern_cells + mr.cell, gauge_point(mr.t, slot, v));
+}
+
 }  // namespace tskv

@@ -3281,6 +3281,272 @@ __global__ void k_finalize_modes(const ModeArgs A, const ModeGather *gathers, co
     *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
 }
 
+// ---- gauges (TSKV_QUERY_N_GAUGES): gauge_agg(time, x), each cell's first two and last two points ----------------------
+// Pass 1 (the fused scan) gives every cell's n. k_gauge_scan (a lane per work item of the operand's buckets) and
+// k_gauge_merge_rows (a thread per merged row) append one record per (page, cell) run: the run's points as a GaugeAcc.
+// A radix sort orders the records by key (gauge, kernel cell), a reduce by key joins each key's records with gauge_join,
+// and k_gauge_scatter writes the states of the kernel's grid. A sliding scan's panes fold into windows (k_gauge_fold),
+// and the ranks' states join in k_merge_gauges. The order of points is (t, slot): ties of time across series go to the
+// lower slot. gauge_join is associative and commutative on disjoint point sets, so the result does not depend on the
+// order the records were appended in.
+struct GaugeCol {
+  uint64_t count_off;  // the operand's COUNT section (n)
+  uint32_t qcol;       // the operand's column in the scan's column table (its work-list buckets, its merged values)
+  uint16_t column_id;
+  uint8_t phys_type;
+  uint8_t pad;
+};
+// A set of points: cnt = min(points, 2); p[0], p[1] its two smallest under (t, slot), p[2], p[3] its two largest. One
+// point fills all four places, two points give p0, p1, p0, p1 (the reference's second is then the last point and its
+// penultimate the first). v holds the operand's bit pattern.
+struct GaugeAcc {
+  int64_t t[4];
+  uint64_t v[4];
+  uint32_t s[4];
+  uint64_t cnt;
+};
+static_assert(sizeof(GaugeAcc) == 88, "a gauge state is 11 words of the exchange region");
+constexpr uint32_t GAUGE_WORDS = sizeof(GaugeAcc) / 8;
+constexpr uint32_t GAUGE_OUTS = 9;  // n, then (t, v) of first, second, penultimate, last
+
+__host__ __device__ __forceinline__ bool gauge_before(const GaugeAcc &a, int i, const GaugeAcc &b, int j) {
+  return a.t[i] < b.t[j] || (a.t[i] == b.t[j] && a.s[i] < b.s[j]);
+}
+__host__ __device__ __forceinline__ void gauge_put(GaugeAcc &r, int i, const GaugeAcc &a, int j) {
+  r.t[i] = a.t[j];
+  r.v[i] = a.v[j];
+  r.s[i] = a.s[j];
+}
+// The points of a and b (disjoint sets). The smallest is the smaller of the two first points; the second smallest the
+// smaller of the other first point and the winner's second (the loser's second is past its own first). The same for the
+// two largest.
+__host__ __device__ __forceinline__ GaugeAcc gauge_join(const GaugeAcc &a, const GaugeAcc &b) {
+  if (!b.cnt) return a;
+  if (!a.cnt) return b;
+  GaugeAcc r;
+  r.cnt = 2;
+  if (gauge_before(a, 0, b, 0)) {
+    gauge_put(r, 0, a, 0);
+    if (a.cnt >= 2 && gauge_before(a, 1, b, 0)) gauge_put(r, 1, a, 1);
+    else gauge_put(r, 1, b, 0);
+  } else {
+    gauge_put(r, 0, b, 0);
+    if (b.cnt >= 2 && gauge_before(b, 1, a, 0)) gauge_put(r, 1, b, 1);
+    else gauge_put(r, 1, a, 0);
+  }
+  if (gauge_before(b, 3, a, 3)) {
+    gauge_put(r, 3, a, 3);
+    if (a.cnt >= 2 && gauge_before(b, 3, a, 2)) gauge_put(r, 2, a, 2);
+    else gauge_put(r, 2, b, 3);
+  } else {
+    gauge_put(r, 3, b, 3);
+    if (b.cnt >= 2 && gauge_before(a, 3, b, 2)) gauge_put(r, 2, b, 2);
+    else gauge_put(r, 2, a, 3);
+  }
+  return r;
+}
+struct GaugeJoin {
+  __host__ __device__ __forceinline__ GaugeAcc operator()(const GaugeAcc &a, const GaugeAcc &b) const { return gauge_join(a, b); }
+};
+__device__ __forceinline__ GaugeAcc gauge_point(int64_t t, uint32_t slot, uint64_t v) {
+  GaugeAcc r;
+  for (int i = 0; i < 4; i++) {
+    r.t[i] = t;
+    r.v[i] = v;
+    r.s[i] = slot;
+  }
+  r.cnt = 1;
+  return r;
+}
+
+// The records and the buffers of the sort and the reduce, all sized at prepare (bound records).
+struct GaugeArgs {
+  GaugeAcc *rec;        // [bound] appended records
+  GaugeAcc *sorted;     // [bound] the records in key order (empty past the last key)
+  GaugeAcc *agg;        // [bound] the reduce's joined states, one per key
+  uint64_t *key;        // [2 * bound] the records' keys (~0: no record), then the sorted keys
+  uint32_t *idx;        // [2 * bound] the records' positions, then in key order
+  uint64_t *uniq;       // [bound] the reduce's keys
+  int32_t *n_runs;      // the reduce's number of keys
+  unsigned int *n_rec;  // the append counter
+  GaugeAcc *dst;        // [n_segs] the states of the kernels' grid (a sliding scan: its panes)
+  int32_t *status;      // the scan's status slot and error page
+  unsigned long long *err_page;
+  uint64_t kern_cells, n_segs, bound;
+};
+
+// A cell whose records disagree with its pass-1 n, or records past the bound (only a decode error pass 1 reports first
+// can cause either): TSKV_ERR_BITSET_MISMATCH, page ~0.
+__device__ __forceinline__ void gauge_mismatch(int32_t *status, unsigned long long *err_page) {
+  if (atomicCAS(status, 0, (int)TSKV_ERR_BITSET_MISMATCH) == 0) *err_page = ~0ull;
+}
+// Appends record r of key `key`: the converged lanes of the warp take their places with one atomic.
+__device__ __forceinline__ void gauge_emit(const GaugeArgs &A, uint64_t key, const GaugeAcc &r) {
+  const uint32_t m = __activemask(), lane = threadIdx.x & 31, leader = __ffs(m) - 1;
+  const uint32_t rank = __popc(m & ((1u << lane) - 1));
+  uint32_t base = 0;
+  if (lane == leader) base = atomicAdd(A.n_rec, (unsigned int)__popc(m));
+  const uint32_t pos = __shfl_sync(m, base, leader) + rank;
+  if (pos >= A.bound) {
+    gauge_mismatch(A.status, A.err_page);
+    return;
+  }
+  A.key[pos] = key;
+  A.idx[pos] = pos;
+  A.rec[pos] = r;
+}
+
+// One page of a gauge's operand (work item `item` of its buckets), decoded with its group's time page row by row and
+// selected as the medians select (select_row): one record per run of selected rows in one cell. Decode errors are pass
+// 1's to report: the lane stops at the first.
+template <bool EDGES>
+__device__ __forceinline__ void gauge_page(const ScanParams &P, const GaugeCol &gc, const GaugeArgs &A, uint64_t key0, uint32_t item) {
+  const uint32_t page = P.work_page[item], slot = P.work_slot[item];
+  const tskv_page_desc vd = P.descs[page];
+  const uint32_t tpage = P.time_page_of[page];
+  const tskv_page_desc td = P.descs[tpage];
+  if (vd.phys_type != gc.phys_type || kind_status(vd.reserved) != TSKV_OK || kind_status(td.reserved) != TSKV_OK ||
+      td.reserved == DK_ALLNULL || vd.reserved == DK_ALLNULL)
+    return;
+  PageView tpv, vpv;
+  tpv.open(P.arena, td);
+  vpv.open(P.arena, vd);
+  BitCursor tb, vb;
+  tb.init(tpv.bitset);
+  vb.init(vpv.bitset);
+  DeltaCursor<-1> tc;
+  AnyCursor<> vc;
+  if (tc.open(tpv, td.reserved) != TSKV_OK || vc.open(vpv, vd.reserved) != TSKV_OK) return;
+  const uint4 none = make_uint4(0, 0, 0, 0);
+  const uint4 tv4 = P.has_tomb ? tomb_lookup(P, vd.series_id, gc.column_id) : none;
+  const uint32_t *keepw = P.row_keep ? P.row_keep + P.keep_off[tpage] : nullptr;
+  const uint64_t group_base = group_cell_base<EDGES>(P, slot);
+  BucketState bk; bk.valid = false; bk.floor_regime = false; bk.lo = 0; bk.hi = 0; bk.idx = 0;
+  GaugeAcc run;
+  run.cnt = 0;
+  uint64_t run_cell = 0;
+  int64_t t = 0;
+  const uint32_t n_rows = vd.num_values;
+  for (uint32_t r = 0; r < n_rows; r++) {
+    const bool tv = tb.next(r), vv = vb.next(r);
+    uint64_t v = 0;
+    if (tv) { t = (int64_t)tc.next(); if (tc.exhausted) break; }
+    else if (r == 0) tc.skip_first_if_s8b_sc();
+    if (vv) { v = vc.next(); if (vc.failed()) break; }
+    else if (r == 0 && !vc.is_gorilla) vc.d.skip_first_if_s8b_sc();
+    uint64_t cell;
+    if (!(tv && vv) || !select_row<EDGES>(P, keepw, r, t, tv4, none, group_base, bk, cell)) continue;
+    if (run.cnt && cell != run_cell) {
+      gauge_emit(A, key0 + run_cell, run);
+      run.cnt = 0;
+    }
+    run_cell = cell;
+    run = gauge_join(run, gauge_point(t, slot, v));
+  }
+  if (run.cnt) gauge_emit(A, key0 + run_cell, run);
+}
+
+// The gauges' pages (blockIdx.y: the gauge): one lane per work item of the operand's buckets (every bin, wide and
+// narrow), the items pass 1 read.
+template <bool EDGES>
+__global__ void __launch_bounds__(128) k_gauge_scan(const __grid_constant__ ScanParams P, const GaugeCol *gcols, const GaugeArgs A) {
+  const GaugeCol gc = gcols[blockIdx.y];
+  const uint64_t key0 = (uint64_t)blockIdx.y * A.kern_cells;
+  const uint32_t stride = gridDim.x * blockDim.x, t0 = blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t k = gc.qcol * WL_SUB; k < N_BINS * P.n_cols * WL_SUB; k += P.n_cols * WL_SUB)
+    for (uint32_t sub = 0; sub < WL_SUB; sub++) {
+      const uint32_t start = __ldg(P.region_start + k + sub), fill = __ldg(P.region_fill + k + sub);
+      for (uint32_t i = t0; i < fill; i += stride) gauge_page<EDGES>(P, gc, A, key0, start + i);
+    }
+}
+
+// After the sort: the records in key order; positions past the last record (key ~0) hold an empty state.
+__global__ void k_gauge_gather(const GaugeArgs A) {
+  const uint64_t *skey = A.key + A.bound;
+  const uint32_t *sidx = A.idx + A.bound;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < A.bound; j += (uint64_t)gridDim.x * blockDim.x) {
+    if (skey[j] < A.n_segs) {
+      A.sorted[j] = A.rec[sidx[j]];
+    } else {
+      GaugeAcc e{};
+      A.sorted[j] = e;
+    }
+  }
+}
+
+// After the reduce: every key's joined state into the grid's states (cleared before).
+__global__ void k_gauge_scatter(const GaugeArgs A) {
+  const uint64_t n = (uint64_t)max(*A.n_runs, 0);
+  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (uint64_t)gridDim.x * blockDim.x)
+    if (A.uniq[r] < A.n_segs) A.dst[A.uniq[r]] = A.agg[r];
+}
+
+// Sliding windows: window j of a group joins its panes j - k + 1 .. j (those that exist), as k_window_combine folds.
+__global__ void k_gauge_fold(const GaugeAcc *pane, GaugeAcc *win, uint32_t n_gauges, uint32_t n_groups, uint32_t n_windows,
+                             uint32_t n_panes, uint32_t k) {
+  const uint64_t n = (uint64_t)n_gauges * n_groups * n_windows;
+  for (uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; c < n; c += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t g = c / n_windows;  // (gauge, group)
+    const uint32_t j = (uint32_t)(c - g * n_windows);
+    const uint32_t p0 = j + 1 >= k ? j + 1 - k : 0, p1 = j < n_panes - 1 ? j : n_panes - 1;
+    GaugeAcc acc;
+    acc.cnt = 0;
+    for (uint32_t p = p0; p <= p1; p++) acc = gauge_join(acc, pane[g * n_panes + p]);
+    win[c] = acc;
+  }
+}
+
+// Every cell of every gauge (the query's grid): a state without a pass-1 n, or an n without a state, is an error.
+__global__ void k_gauge_check(const uint64_t *state, const GaugeCol *gcols, const GaugeAcc *gs, uint32_t n_gauges, uint64_t n_cells,
+                              int32_t *status, unsigned long long *err_page) {
+  const uint64_t n = (uint64_t)n_gauges * n_cells;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t g = i / n_cells, cell = i - g * n_cells;
+    if ((gs[i].cnt != 0) != (state[gcols[g].count_off + cell] != 0)) gauge_mismatch(status, err_page);
+  }
+}
+
+// Multi-GPU, after k_merge_gathered: every gauge state joins the ranks' states (the gauge section at off, n states).
+__global__ void k_merge_gauges(uint64_t *state, uint64_t off, uint64_t n, const uint64_t *gathered, uint32_t n_ranks, uint64_t exch_words) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    GaugeAcc acc;
+    acc.cnt = 0;
+    for (uint32_t r = 0; r < n_ranks; r++)
+      acc = gauge_join(acc, reinterpret_cast<const GaugeAcc *>(gathered + r * exch_words + off)[i]);
+    reinterpret_cast<GaugeAcc *>(state + off)[i] = acc;
+  }
+}
+
+// The gauge outputs (blockIdx.y: gauge * GAUGE_OUTS + output; output column out0 + blockIdx.y): n (u64, always valid),
+// then t (i64) and v (f64: integers rounded to nearest) of the first, second, penultimate and last point, valid iff n >= 1.
+__global__ void k_finalize_gauges(const uint64_t *state, const GaugeCol *gcols, uint64_t off, uint32_t out0, uint64_t n_cells,
+                                  uint64_t bitmap_stride, uint64_t *values, uint8_t *validity) {
+  const uint32_t g = blockIdx.y / GAUGE_OUTS, f = blockIdx.y % GAUGE_OUTS;
+  const GaugeCol gc = gcols[g];
+  const uint64_t cell = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  bool valid = false;
+  if (cell < n_cells) {
+    const uint64_t n = state[gc.count_off + cell];
+    uint64_t v = n;
+    valid = f == 0 || n != 0;
+    if (f && valid) {
+      const GaugeAcc &a = reinterpret_cast<const GaugeAcc *>(state + off)[(uint64_t)g * n_cells + cell];
+      const uint32_t p = (f - 1) >> 1;
+      if (((f - 1) & 1) == 0) {
+        v = (uint64_t)a.t[p];
+      } else {
+        v = a.v[p];
+        if (gc.phys_type == TSKV_PT_I64) v = (uint64_t)__double_as_longlong(__ll2double_rn((long long)v));
+        else if (gc.phys_type == TSKV_PT_U64) v = (uint64_t)__double_as_longlong(__ull2double_rn((unsigned long long)v));
+      }
+    }
+    values[(uint64_t)(out0 + blockIdx.y) * n_cells + cell] = valid ? v : 0;
+  }
+  const uint32_t bits = __ballot_sync(FULL, valid);
+  if ((threadIdx.x & 31) == 0 && (cell >> 3) < bitmap_stride)
+    *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
+}
+
 // Per output column: which state arrays feed it.
 struct OutCol {
   uint64_t count_off;  // counts of the source column

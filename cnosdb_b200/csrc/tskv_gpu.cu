@@ -16,6 +16,7 @@
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -292,6 +293,18 @@ struct tskv_scan {
   async_ptr<uint8_t> d_mode_tmp;
   size_t mode_tmp_bytes = 0;
   ModeArgs mode{};
+  // gauges (TSKV_QUERY_N_GAUGES; k_gauge_scan): their operands, their states in the exchange region (gauge_off: GaugeAcc
+  // [n_gauges][n_cells]), a sliding scan's pane states, and the records with the sort's and the reduce's buffers (GaugeArgs)
+  uint32_t n_gauges = 0;
+  uint64_t gauge_off = 0, gauge_words = 0;
+  int gauge_key_bits = 1;  // the key bits the sort reads (n_segs < 2^gauge_key_bits: key ~0 sorts last)
+  async_ptr<GaugeCol> d_gauges;
+  async_ptr<GaugeAcc> d_gauge_acc;  // [3 * bound] records, sorted records, joined states; then the panes' states
+  async_ptr<uint64_t> d_gauge_key;  // [3 * bound] keys, sorted keys, the reduce's keys
+  async_ptr<uint32_t> d_gauge_idx;  // [2 * bound + 2] positions, sorted positions, the counter and the number of keys
+  async_ptr<uint8_t> d_gauge_tmp;
+  size_t gauge_tmp_bytes = 0;
+  GaugeArgs gauge{};
 };
 
 namespace {
@@ -382,13 +395,18 @@ uint32_t query_n_medians(const tskv_query *q) { return TSKV_QUERY_N_MEDIANS(q->r
 uint32_t query_n_increases(const tskv_query *q) { return TSKV_QUERY_N_INCREASES(q->reserved); }
 uint32_t query_n_modes(const tskv_query *q) { return TSKV_QUERY_N_MODES(q->reserved); }
 uint32_t query_n_distincts(const tskv_query *q) { return TSKV_QUERY_N_DISTINCTS(q->reserved); }
+uint32_t query_n_gauges(const tskv_query *q) { return TSKV_QUERY_N_GAUGES(q->reserved); }
+// the columns before the gauges' operands
+uint64_t query_gauge_col0(const tskv_query *q) {
+  return (uint64_t)q->n_columns + 2ull * q->n_pairs + query_n_medians(q) + query_n_increases(q) + query_n_modes(q) + query_n_distincts(q);
+}
 
 // The query the scan runs for a query with column pairs, medians or increases: its projected columns, then every operand that is
 // not one of them as a COUNT column without output (so that the work list, the page gathers, CRC checks, pass 1 and the
 // reader counters treat the operands' pages as they treat a COUNT column's), and per pair, median and increase the
 // operands' places in that table. A median's operand column also computes MIN and MAX in pass 1 (its extreme keys); an increase's
-// operand column computes COUNT (its validity), and so does a mode's or distinct's (its n). Modes and distincts share
-// one gather per operand column id.
+// operand column computes COUNT (its validity), and so does a mode's or distinct's (its n) and a gauge's (its n). Modes
+// and distincts share one gather per operand column id.
 struct OperandQuery {
   tskv_query q{};
   std::vector<tskv_agg_column> cols;
@@ -397,6 +415,7 @@ struct OperandQuery {
   std::vector<IncreaseCol> increases;  // (the offsets are set by plan_layout)
   std::vector<ModeGather> gathers;     // (count_off is set by plan_layout)
   std::vector<ModeOut> mode_outs;      // the modes', then the distincts' outputs
+  std::vector<GaugeCol> gauges;        // (count_off is set by plan_layout)
 };
 OperandQuery plan_operand_query(const tskv_query *q) {
   OperandQuery pq;
@@ -451,6 +470,15 @@ OperandQuery plan_operand_query(const tskv_query *q) {
       pq.gathers.push_back(mg);
     }
     pq.mode_outs.push_back(ModeOut{g, k >= n_modes ? 1u : 0u});
+  }
+  for (uint32_t k = 0; k < query_n_gauges(q); k++) {
+    const tskv_agg_column &op = q->columns[query_gauge_col0(q) + k];
+    GaugeCol gc{};
+    gc.qcol = place(op);
+    pq.cols[gc.qcol].agg_mask |= TSKV_AGG_COUNT;
+    gc.column_id = op.column_id;
+    gc.phys_type = op.phys_type;
+    pq.gauges.push_back(gc);
   }
   pq.q.columns = pq.cols.data();
   pq.q.n_columns = (uint32_t)pq.cols.size();
@@ -621,7 +649,7 @@ bool labels_first_last(const tskv_query *q, const BucketEdges &E) {
 bool query_shape_ok(const tskv_query *q, bool edges = false) {
   return q->n_buckets != 0 &&
          (q->n_columns != 0 || q->n_pairs != 0 || query_n_medians(q) != 0 || query_n_increases(q) != 0 ||
-          query_n_modes(q) != 0 || query_n_distincts(q) != 0) && q->columns &&
+          query_n_modes(q) != 0 || query_n_distincts(q) != 0 || query_n_gauges(q) != 0) && q->columns &&
          (q->width > 0 || q->n_buckets == 1 || edges);
 }
 
@@ -635,6 +663,7 @@ tskv_output_layout output_layout(const tskv_pages *pages, const tskv_query *q, c
   if (query_n_increases(q) <= TSKV_MAX_INCREASES) n_out += query_n_increases(q);
   if (query_n_modes(q) <= TSKV_MAX_MODES) n_out += query_n_modes(q);
   if (query_n_distincts(q) <= TSKV_MAX_DISTINCTS) n_out += query_n_distincts(q);
+  if (query_n_gauges(q) <= TSKV_MAX_GAUGES) n_out += (uint64_t)GAUGE_OUTS * query_n_gauges(q);
   uint64_t n_groups = 1;
   if (q->group_by_series) n_groups = selected_slots(pages, q);
   if (tg.on) n_groups = tg.n;
@@ -669,9 +698,11 @@ struct StatePlan {
   uint64_t m2_words = 0;           // their shift / sum(d) / sum(d^2) sections, which follow the values section
   uint64_t pair_off = 0, pair_words = 0;  // the column pairs' sections (PAIR_WORDS per pair), after the M2 ones
   std::vector<uint64_t> inc_off;          // per increase: its sum section, after the integer / the f64 sums
+  uint64_t gauge_off = 0, gauge_words = 0;  // the gauges' states (GaugeAcc [n_gauges][n_cells]), after the pairs' sections
 };
-// incs: the increases (plan_operand_query's), whose sums the exchange region's sum sections hold
-StatePlan plan_state(const tskv_query *q, uint64_t n_cells, const std::vector<IncreaseCol> &incs = {}) {
+// incs: the increases (plan_operand_query's), whose sums the exchange region's sum sections hold; n_gauges: the gauges,
+// whose states the exchange region holds last
+StatePlan plan_state(const tskv_query *q, uint64_t n_cells, const std::vector<IncreaseCol> &incs = {}, uint32_t n_gauges = 0) {
   StatePlan plan;
   plan.cols.resize(q->n_columns);
   plan.msum_off.assign(q->n_columns, 0);
@@ -758,6 +789,9 @@ StatePlan plan_state(const tskv_query *q, uint64_t n_cells, const std::vector<In
   plan.pair_off = off;
   plan.pair_words = (uint64_t)PAIR_WORDS * n_cells * q->n_pairs;
   off += plan.pair_words;
+  plan.gauge_off = off;
+  plan.gauge_words = (uint64_t)GAUGE_WORDS * n_cells * n_gauges;
+  off += plan.gauge_words;
   off = (off + 1) & ~1ull;  // 16-byte alignment of the pair arrays
   sl.first_pairs_off = off;
   {
@@ -979,6 +1013,23 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
         return TSKV_ERR_INVALID_ARG;
       }
   }
+  const uint32_t n_gauge = query_n_gauges(q);
+  if (n_gauge > TSKV_MAX_GAUGES || query_gauge_col0(q) + n_gauge > 126) {
+    ctx->set_error("invalid query: at most 8 gauges and 126 columns with every operand");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  for (uint64_t k = query_gauge_col0(q); k < query_gauge_col0(q) + n_gauge; k++) {
+    const tskv_agg_column &op = q->columns[k];
+    if (op.agg_mask != 0 || op.phys_type < TSKV_PT_I64 || op.phys_type > TSKV_PT_F64) {
+      ctx->set_error("invalid gauge operand: an I64 / U64 / F64 column with agg_mask 0");
+      return TSKV_ERR_INVALID_ARG;
+    }
+    for (uint64_t c = 0; c < k; c++)
+      if (q->columns[c].column_id == op.column_id && q->columns[c].phys_type != op.phys_type) {
+        ctx->set_error("gauge operand: one column id with two types");
+        return TSKV_ERR_INVALID_ARG;
+      }
+  }
   if (q->n_predicates > TSKV_MAX_PREDICATES || (q->n_predicates && !q->predicates)) {
     ctx->set_error("invalid query: at most 8 field predicates");
     return TSKV_ERR_INVALID_ARG;
@@ -1011,10 +1062,10 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
         return TSKV_ERR_INVALID_ARG;
       }
   if ((q->reserved & TSKV_QUERY_MULTI_RANK) && !q->series_ids) {
-    bool needs_slots = q->group_by_series != 0 || tg.on;
+    bool needs_slots = q->group_by_series != 0 || tg.on || n_gauge != 0;  // (gauges order tied points by slot)
     for (uint32_t c = 0; c < q->n_columns; c++) needs_slots |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
     if (needs_slots) {
-      ctx->set_error("multi-rank scan: GROUP BY series / tags and first/last need the global series_ids list (slots are positions in it)");
+      ctx->set_error("multi-rank scan: GROUP BY series / tags, first/last and gauges need the global series_ids list (slots are positions in it)");
       return TSKV_ERR_INVALID_ARG;
     }
   }
@@ -1143,6 +1194,8 @@ struct ScanLayout {
   std::vector<IncreaseCol> increases;  // increases, with their operands' COUNT sections and their sum sections
   std::vector<ModeGather> gathers;     // the modes' and distincts' gathers, with their operands' COUNT sections
   std::vector<ModeOut> mode_outs;
+  std::vector<GaugeCol> gauges;        // the gauges, with their operands' COUNT sections
+  uint64_t gauge_off = 0, gauge_words = 0;
 };
 
 // n_cells: cells of the query's grid (a sliding scan: windows); kern_cells: cells of the fused kernels' grid (panes).
@@ -1151,7 +1204,7 @@ struct ScanLayout {
 ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint64_t kern_cells, const tskv_agg_column *user_cols,
                        uint32_t n_user, const OperandQuery &oq) {
   ScanLayout out;
-  const StatePlan win = plan_state(q, n_cells, oq.increases);
+  const StatePlan win = plan_state(q, n_cells, oq.increases, (uint32_t)oq.gauges.size());
   const StatePlan pane = sliding ? plan_state(q, kern_cells) : StatePlan{};
   out.sl = win.sl;
   out.kern_sl = sliding ? pane.sl : win.sl;
@@ -1179,6 +1232,10 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
   out.gathers = oq.gathers;  // (sliding scans refuse modes and distincts)
   for (ModeGather &mg : out.gathers) mg.count_off = win.cols[mg.qcol].count_off;
   out.mode_outs = oq.mode_outs;
+  out.gauges = oq.gauges;
+  for (GaugeCol &gc : out.gauges) gc.count_off = win.cols[gc.qcol].count_off;
+  out.gauge_off = win.gauge_off;
+  out.gauge_words = win.gauge_words;
   if (sliding) {
     for (uint32_t c = 0; c < q->n_columns; c++) {
       const ColState &p = pane.cols[c], &w = win.cols[c];
@@ -1597,6 +1654,38 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
     A.best = s->d_mode_res.get();
     A.runs = s->d_mode_res.get() + A.n_segs;
     *h2d += lay.gathers.size() * sizeof(ModeGather) + lay.mode_outs.size() * sizeof(ModeOut);
+  }
+  s->n_gauges = (uint32_t)lay.gauges.size();
+  s->gauge_off = lay.gauge_off;
+  s->gauge_words = lay.gauge_words;
+  if (s->n_gauges) {  // (prepare_scan has bounded the records: s->gauge.bound)
+    GaugeArgs &A = s->gauge;
+    A.kern_cells = (uint64_t)s->layout.n_groups * s->n_panes;
+    A.n_segs = (uint64_t)s->n_gauges * A.kern_cells;
+    A.bound = std::max<uint64_t>(A.bound, 1);
+    s->gauge_key_bits = 64 - __builtin_clzll(A.n_segs);
+    size_t t[2] = {0, 0};
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, t[0], (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                                               (uint32_t *)nullptr, (int)A.bound, 0, s->gauge_key_bits, st);
+    if (e == cudaSuccess) e = cub::DeviceReduce::ReduceByKey(nullptr, t[1], (const uint64_t *)nullptr, (uint64_t *)nullptr, (const GaugeAcc *)nullptr,
+                                                              (GaugeAcc *)nullptr, (int32_t *)nullptr, GaugeJoin{}, (int)A.bound, st);
+    s->gauge_tmp_bytes = std::max<size_t>(std::max(t[0], t[1]), 1);
+    const uint64_t panes = sliding ? A.n_segs : 0;  // a sliding scan's pane states follow the joined states
+    if (e == cudaSuccess) e = upload(s->d_gauges, lay.gauges.data(), lay.gauges.size(), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_gauge_acc, (size_t)(3 * A.bound + panes), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_gauge_key, (size_t)(3 * A.bound), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_gauge_idx, (size_t)(2 * A.bound + 2), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_gauge_tmp, s->gauge_tmp_bytes, st);
+    A.rec = s->d_gauge_acc.get();
+    A.sorted = A.rec + A.bound;
+    A.agg = A.rec + 2 * A.bound;
+    A.key = s->d_gauge_key.get();
+    A.uniq = A.key + 2 * A.bound;
+    A.idx = s->d_gauge_idx.get();
+    A.n_rec = reinterpret_cast<unsigned int *>(A.idx + 2 * A.bound);
+    A.n_runs = reinterpret_cast<int32_t *>(A.idx + 2 * A.bound + 1);
+    A.dst = sliding ? A.rec + 3 * A.bound : reinterpret_cast<GaugeAcc *>(s->d_state.get() + s->gauge_off);
+    *h2d += lay.gauges.size() * sizeof(GaugeCol);
   }
   if (e == cudaSuccess) e = stream_alloc(s->d_aux, AUX_WORDS, st);
   if (e == cudaSuccess) e = stream_alloc(s->d_values, s->layout.n_out * s->layout.n_cells, st);
@@ -2404,6 +2493,59 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
       return TSKV_ERR_UNSUPPORTED;
     }
   }
+  // gauges: one record per (operand page, cell) run at most: per page of a column group that can hold selected rows, the
+  // fewer of its rows and the grid buckets its time span can touch (edge buckets of a labelled scan, panes of a sliding
+  // one), and one per merge row; sized here so that run and enqueue neither allocate nor synchronise
+  uint64_t gauge_bound = 0;
+  if (!pq.gauges.empty()) {
+    std::vector<tskv_time_range> cg_bounds;
+    if (pages->n_cg) {
+      ensure_time_bounds(ctx, pages);
+      cg_bounds.resize(pages->n_cg);
+      if (!pages->d_cg_bounds || cudaMemcpy(cg_bounds.data(), pages->d_cg_bounds.get(), pages->n_cg * sizeof(tskv_time_range),
+                                            cudaMemcpyDeviceToHost) != cudaSuccess) {
+        ctx->set_error(std::string("gauge: column-group time bounds: ") + cudaGetErrorString(cudaGetLastError()));
+        return TSKV_ERR_CUDA;
+      }
+    }
+    // (a page's time span is its column group's: every page of a group shares the group's time page) The span is first
+    // clipped to the query's time ranges and to the kernels' grid: rows outside them make no record.
+    const int64_t kern_width = slide ? slide : q->width;
+    __int128 grid_lo = INT64_MIN, grid_hi = INT64_MAX;
+    if (E.on) {
+      grid_lo = E.edges[0];
+      grid_hi = (__int128)E.edges[E.n] - 1;
+    } else if (kern_width > 0) {
+      grid_lo = (__int128)q->first_bucket_start + (__int128)(win_k - 1) * kern_width;
+      grid_hi = grid_lo + (__int128)(q->n_buckets - win_k + 1) * kern_width - 1;
+    }
+    auto buckets = [&](const tskv_time_range &b) -> uint64_t {
+      int64_t lo = b.min_ts, hi = b.max_ts;
+      clip_to_query_ranges(q, lo, hi);
+      lo = (int64_t)std::max<__int128>(lo, grid_lo);
+      hi = (int64_t)std::min<__int128>(hi, grid_hi);
+      if (lo > hi) return b.min_ts > b.max_ts ? 1 : 0;  // (a group without time bounds: one run at most per page)
+      if (E.on) {
+        const int64_t *e0 = E.edges, *e1 = E.edges + E.n + 1;
+        return (uint64_t)(std::upper_bound(e0, e1, hi) - std::upper_bound(e0, e1, lo)) + 1;
+      }
+      if (kern_width > 0) return ((uint64_t)hi - (uint64_t)lo) / (uint64_t)kern_width + 2;
+      return 1;
+    };
+    for (const GaugeCol &gc : pq.gauges) {
+      for (uint32_t cg = 0; cg < pages->n_cg; cg++) {
+        if (!cg_selected(pages, q, cg_bounds.data(), cg)) continue;
+        const uint64_t touch = buckets(cg_bounds[cg]);
+        for (uint64_t p = (uint64_t)pages->h_cg_time_page[cg] + 1; p < pages->n_descs && pages->h_descs[p].phys_type != TSKV_PT_TIME; p++)
+          if (pages->h_descs[p].column_id == gc.column_id) gauge_bound += std::min<uint64_t>(pages->h_descs[p].num_values, touch);
+      }
+      gauge_bound += pages->overlap.merge_rows;
+    }
+    if (gauge_bound >> 31) {
+      ctx->set_error("gauge: the record bound reaches 2^31 (the sort and the reduce count items in int)");
+      return TSKV_ERR_UNSUPPORTED;
+    }
+  }
   q = &pq.q;
   bool has_sel = false;  // any FIRST / LAST
   for (uint32_t c = 0; c < q->n_columns; c++) has_sel |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
@@ -2429,6 +2571,7 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   s->kern_sl = lay.kern_sl;
   uint64_t h2d = 0;
   s->mode.bound = mode_bound;
+  s->gauge.bound = gauge_bound;
   if ((st = alloc_scan(ctx, pages, q, tg, slide != 0, E, lay, s, &h2d)) != TSKV_OK) {
     delete s;
     return st;
@@ -2449,6 +2592,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   P.err_page = s->d_err_page;
   s->mode.status = s->d_status;
   s->mode.err_page = s->d_err_page;
+  s->gauge.status = s->d_status;
+  s->gauge.err_page = s->d_err_page;
   P.stats = s->d_stats;
   P.n_ranges = q->n_time_ranges;
   for (uint32_t k = 0; k < q->n_time_ranges; k++) P.ranges[k] = q->time_ranges[k];
@@ -2853,6 +2998,43 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     launches += 5;  // (a sort or scan counts as one launch)
     if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), stream);  // (the fused time includes the mode kernels)
   }
+  if (s->n_gauges) {  // gauges: the records (merged rows too), the sort, the reduce by key, the states, the check
+    const GaugeArgs &A = s->gauge;
+    cudaStream_t stream = ctx->stream.get();
+    const uint32_t kx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((A.bound + 255) / 256, 4096));
+    const uint32_t cx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)s->n_gauges * s->layout.n_cells + 255) / 256, 4096));
+    const uint32_t px = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)pages->n_descs + 127) / 128, (uint64_t)ctx->sm_count * 16));
+    const GaugeCol *gp = s->d_gauges.get();
+    CU_TRY(ctx, cudaMemsetAsync(A.key, 0xff, A.bound * sizeof(uint64_t), stream));
+    CU_TRY(ctx, cudaMemsetAsync(A.n_rec, 0, sizeof(unsigned int), stream));
+    CU_TRY(ctx, cudaMemsetAsync(A.dst, 0, A.n_segs * sizeof(GaugeAcc), stream));
+    const void *fn = s->params.edges ? (const void *)k_gauge_scan<true> : (const void *)k_gauge_scan<false>;
+    void *args[] = {(void *)&s->params, (void *)&gp, (void *)&s->gauge};
+    CU_TRY(ctx, cudaLaunchKernel(fn, dim3(px, s->n_gauges), dim3(128), args, 0, stream));
+    launches++;
+    if (s->merge.n_rows && s->n_merge_pages) {
+      k_gauge_merge_rows<<<dim3((uint32_t)((s->merge.n_rows + 127) / 128), s->n_gauges), 128, 0, stream>>>(s->params, s->merge, gp, A);
+      launches++;
+    }
+    size_t tmp = s->gauge_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_gauge_tmp.get(), tmp, A.key, A.key + A.bound, A.idx, A.idx + A.bound, (int)A.bound, 0,
+                                                s->gauge_key_bits, stream));
+    k_gauge_gather<<<kx, 256, 0, stream>>>(A);
+    tmp = s->gauge_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceReduce::ReduceByKey(s->d_gauge_tmp.get(), tmp, (const uint64_t *)(A.key + A.bound), A.uniq,
+                                               (const GaugeAcc *)A.sorted, A.agg, A.n_runs, GaugeJoin{},
+                                               (int)A.bound, stream));
+    k_gauge_scatter<<<kx, 256, 0, stream>>>(A);
+    launches += 4;  // (a sort or reduce counts as one launch)
+    GaugeAcc *win = reinterpret_cast<GaugeAcc *>(s->d_state.get() + s->gauge_off);
+    if (A.dst != win) {  // a sliding scan
+      k_gauge_fold<<<cx, 256, 0, stream>>>(A.dst, win, s->n_gauges, (uint32_t)s->layout.n_groups, s->n_windows, s->n_panes, s->win_k);
+      launches++;
+    }
+    k_gauge_check<<<cx, 256, 0, stream>>>(s->d_state.get(), gp, win, s->n_gauges, s->layout.n_cells, A.status, A.err_page);
+    launches++;
+    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), stream);  // (the fused time includes the gauge kernels)
+  }
   if (!capturing) cudaEventRecord(s->ev1.get(), ctx->stream.get());
   CU_TRY(ctx, cudaGetLastError());
   ctx->counters.kernel_launches = launches;
@@ -2999,9 +3181,10 @@ static tskv_status refuse_medians(tskv_ctx *ctx, const tskv_scan *s, const char 
 tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_view *out) {
   if (!ctx || !s || !out) return TSKV_ERR_INVALID_ARG;
   if (tskv_status st = refuse_medians(ctx, s, "scan_partials")) return st;
-  if (s->n_m2 || s->n_pairs) {
+  if (s->n_m2 || s->n_pairs || s->n_gauges) {
     std::lock_guard<std::mutex> lock(ctx->mu);
-    ctx->set_error("scan_partials: second moments (TSKV_AGG_M2, column pairs) do not all-reduce element-wise; use tskvgpu_scan_exchange");
+    ctx->set_error("scan_partials: second moments (TSKV_AGG_M2, column pairs) and gauge points do not all-reduce element-wise; use "
+                   "tskvgpu_scan_exchange");
     return TSKV_ERR_UNSUPPORTED;
   }
   const StateLayout &L = s->sl;
@@ -3021,8 +3204,14 @@ tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_vie
   return TSKV_OK;
 }
 
+// The words of the exchange region: sum_i64 | sum_f64 | min+first keys | max+last keys | values | M2 | pairs | gauges
+static uint64_t exchange_words(const tskv_scan *s) {
+  return s->sl.selval_off + s->sl.selval_len + s->m2_words + s->pair_words + s->gauge_words;
+}
+
 // The M2 columns of gathered partials: Chan's merge of every rank's (count, sum, M2) (k_merge_m2).
-// (and the column pairs: Chan's merge of every rank's n, means and co-moments, k_merge_pairs)
+// (and the column pairs: Chan's merge of every rank's n, means and co-moments, k_merge_pairs; and the gauges' points,
+// k_merge_gauges)
 static void merge_m2(tskv_ctx *ctx, tskv_scan *s, const uint64_t *gathered, uint32_t n_ranks, uint64_t words) {
   const uint32_t bx = (uint32_t)std::min<uint64_t>((s->layout.n_cells + 255) / 256, 1024);
   if (s->n_m2)
@@ -3031,13 +3220,18 @@ static void merge_m2(tskv_ctx *ctx, tskv_scan *s, const uint64_t *gathered, uint
   if (s->n_pairs)
     k_merge_pairs<<<dim3(std::max(1u, bx), s->n_pairs), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->d_pairs.get(), s->layout.n_cells,
                                                                                  gathered, n_ranks, words);
+  if (s->n_gauges) {
+    const uint64_t n = (uint64_t)s->n_gauges * s->layout.n_cells;
+    const uint32_t gx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + 255) / 256, 4096));
+    k_merge_gauges<<<gx, 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->gauge_off, n, gathered, n_ranks, words);
+  }
 }
 
 tskv_status tskvgpu_scan_exchange_view(tskv_ctx *ctx, tskv_scan *s, uint64_t *out_dptr, uint64_t *out_words) {
   if (!ctx || !s || !out_dptr || !out_words) return TSKV_ERR_INVALID_ARG;
   if (tskv_status st = refuse_medians(ctx, s, "scan_exchange_view")) return st;
   *out_dptr = (uint64_t)(uintptr_t)s->d_state.get();
-  *out_words = s->sl.selval_off + s->sl.selval_len + s->m2_words + s->pair_words;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values | M2 | pairs
+  *out_words = exchange_words(s);
   return TSKV_OK;
 }
 
@@ -3046,7 +3240,7 @@ tskv_status tskvgpu_scan_merge_gathered(tskv_ctx *ctx, tskv_scan *s, uint64_t ga
   if (tskv_status st = refuse_medians(ctx, s, "scan_merge_gathered")) return st;
   std::lock_guard<std::mutex> lock(ctx->mu);
   cudaSetDevice(ctx->device);
-  const uint64_t words = s->sl.selval_off + s->sl.selval_len + s->m2_words + s->pair_words;
+  const uint64_t words = exchange_words(s);
   uint32_t blocks = (uint32_t)std::min<uint64_t>((words + 255) / 256, 2048);
   k_merge_gathered<<<std::max(1u, blocks), 256, 0, ctx->stream.get()>>>(s->d_state.get(), s->sl, reinterpret_cast<const uint64_t *>((uintptr_t)gathered_dptr),
                                                                    n_ranks, words);
@@ -3065,7 +3259,7 @@ tskv_status tskvgpu_scan_exchange(tskv_ctx *ctx, tskv_scan *s) {
     return TSKV_ERR_NCCL;
   }
   const NcclApi &N = nccl_api();
-  const uint64_t words = s->sl.selval_off + s->sl.selval_len + s->m2_words + s->pair_words;  // sum_i64 | sum_f64 | min+first keys | max+last keys | values | M2
+  const uint64_t words = exchange_words(s);
   if (!s->d_gathered) CU_TRY(ctx, stream_alloc(s->d_gathered, (size_t)ctx->n_ranks * words, ctx->stream.get()));
   const ncclResult_t r = N.AllGather(s->d_state.get(), s->d_gathered.get(), words, ncclUint64, ctx->comm, ctx->stream.get());
   if (r != ncclSuccess) {
@@ -3123,6 +3317,10 @@ static tskv_status finalize_device(tskv_ctx *ctx, tskv_scan *s) {
     k_finalize_modes<<<dim3((uint32_t)((L.n_cells + 255) / 256), s->n_mode_outs), 256, 0, ctx->stream.get()>>>(
         s->mode, s->d_gathers.get(), s->d_mode_outs.get(), s->n_out + 4 * s->n_pairs + s->n_medians + s->n_increases, L.bitmap_stride,
         s->d_values.get(), s->d_validity.get());
+  if (s->n_gauges)
+    k_finalize_gauges<<<dim3((uint32_t)((L.n_cells + 255) / 256), GAUGE_OUTS * s->n_gauges), 256, 0, ctx->stream.get()>>>(
+        s->d_state.get(), s->d_gauges.get(), s->gauge_off, s->n_out + 4 * s->n_pairs + s->n_medians + s->n_increases + s->n_mode_outs,
+        L.n_cells, L.bitmap_stride, s->d_values.get(), s->d_validity.get());
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;
 }

@@ -219,15 +219,57 @@ class TskvError(RuntimeError):
 
 
 # the aggregates without a mask bit: each makes its column an operand of its own kind
-PSEUDO_AGGS = ("median", "increase", "mode", "count_distinct")
+PSEUDO_AGGS = ("median", "increase", "mode", "count_distinct", "gauge_agg")
+# the outputs of one gauge_agg(time, x): the points, then (time, value) of its first, second, penultimate and last point
+GAUGE_OUTS = ("n", "first_t", "first_v", "second_t", "second_v", "penultimate_t", "penultimate_v", "last_t", "last_v")
+# the accessors of CnosDB's GaugeData (gauge/mod.rs) that gauge_stat derives from the nine outputs
+GAUGE_STATS = ("delta", "time_delta", "rate", "idelta_left", "idelta_right", "first_time", "first_val", "last_time", "last_val",
+               "num_elements")
+
+
+def gauge_stat(name, n, first_t, first_v, second_t, second_v, penultimate_t, penultimate_v, last_t, last_v):
+    """(values, validity) of one GaugeData accessor (gauge/mod.rs), elementwise over cells, from a gauge's nine outputs
+    (n u64, *_t i64, *_v f64). Every accessor is NULL where n == 0 (a NULL GaugeData). delta = last_v - first_v,
+    idelta_left = second_v - first_v, idelta_right = last_v - penultimate_v; time_delta = last_t - first_t, NULL when the
+    subtraction overflows i64; rate = delta / (time_delta as f64), NULL when time_delta is 0 (the reference fails the query
+    when time_delta overflows; here it is NULL too)."""
+    n = np.asarray(n, dtype=np.uint64)
+    ok = n > 0
+    ft, lt = np.asarray(first_t, dtype=np.int64), np.asarray(last_t, dtype=np.int64)
+    fv, sv = np.asarray(first_v, dtype=np.float64), np.asarray(second_v, dtype=np.float64)
+    pv, lv = np.asarray(penultimate_v, dtype=np.float64), np.asarray(last_v, dtype=np.float64)
+    if name == "num_elements":
+        return n.copy(), ok
+    if name in ("first_time", "last_time"):
+        return (ft if name == "first_time" else lt).copy(), ok
+    if name in ("first_val", "last_val"):
+        return (fv if name == "first_val" else lv).copy(), ok
+    with np.errstate(all="ignore"):
+        if name == "delta":
+            return lv - fv, ok
+        if name == "idelta_left":
+            return sv - fv, ok
+        if name == "idelta_right":
+            return lv - pv, ok
+        dt = lt.astype(object) - ft.astype(object) if lt.ndim else int(lt) - int(ft)
+        dt = np.asarray(dt, dtype=object)
+        fits = np.vectorize(lambda d: -(1 << 63) <= d < (1 << 63), otypes=[bool])(dt) if dt.size else np.zeros(dt.shape, bool)
+        td = np.where(fits, dt, 0).astype(np.int64)
+        if name == "time_delta":
+            return td, ok & fits
+        if name == "rate":
+            keep = ok & fits & (td != 0)
+            return (lv - fv) / np.where(keep, td, 1).astype(np.float64), keep
+    raise ValueError("unknown gauge accessor %r (one of %s)" % (name, ", ".join(GAUGE_STATS)))
 
 
 class PushedAggregate:
     """One projected value column with its aggregate set (extends PushedAggregateFunction::Count). "median" has no mask
     bit: it makes the column a median operand (after the pairs' operands, agg_mask 0), and a column that asks for nothing
     else has no projected entry. "increase" (increase(time, x ORDER BY time)) likewise makes it an increase operand, after
-    the medians' operands; "mode" (mode(x)) a mode operand, after the increases' operands; and "count_distinct"
-    (COUNT(DISTINCT x)) a distinct operand, after the modes' operands."""
+    the medians' operands; "mode" (mode(x)) a mode operand, after the increases' operands; "count_distinct"
+    (COUNT(DISTINCT x)) a distinct operand, after the modes' operands; and "gauge_agg" (gauge_agg(time, x)) a gauge
+    operand, after the distincts' operands."""
 
     def __init__(self, column_id, phys_type, aggs):
         self.column_id = int(column_id)
@@ -236,6 +278,7 @@ class PushedAggregate:
         self.increase = False
         self.mode = False
         self.count_distinct = False
+        self.gauge_agg = False
         if isinstance(aggs, int):
             self.agg_mask = aggs
         else:
@@ -244,7 +287,7 @@ class PushedAggregate:
                 if a == "median":
                     self.median = True
                     continue
-                if a in ("increase", "mode", "count_distinct"):
+                if a in ("increase", "mode", "count_distinct", "gauge_agg"):
                     setattr(self, a, True)
                     continue
                 # var* / stddev* ask the scan for COUNT | M2; ScanResult.column derives them
@@ -292,13 +335,15 @@ class QueryOption:
         incs = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "increase", False)]
         modes = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "mode", False)]
         dists = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "count_distinct", False)]
+        gauges = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "gauge_agg", False)]
         q.reserved = ((cabi.TSKV_QUERY_MULTI_RANK if self.multi_rank else 0) | cabi.query_medians(len(meds)) |
-                      cabi.query_increases(len(incs)) | cabi.query_modes(len(modes)) | cabi.query_distincts(len(dists)))
-        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))] + meds + incs + modes + dists
+                      cabi.query_increases(len(incs)) | cabi.query_modes(len(modes)) | cabi.query_distincts(len(dists)) |
+                      cabi.query_gauges(len(gauges)))
+        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))] + meds + incs + modes + dists + gauges
         cols = (cabi.AggColumn * max(1, len(proj) + len(ops)))()
         for i, c in enumerate(proj):
             cols[i].column_id, cols[i].phys_type, cols[i].agg_mask = c.column_id, c.phys_type, c.agg_mask
-        for i, (cid, pt) in enumerate(ops):  # the pairs', medians', increases', modes' and distincts' operands follow
+        for i, (cid, pt) in enumerate(ops):  # the pairs', medians', increases', modes', distincts' and gauges' operands follow
             cols[len(proj) + i].column_id, cols[len(proj) + i].phys_type = cid, pt
         q.columns = cols
         q.n_columns = len(proj)
@@ -317,7 +362,8 @@ class QueryOption:
         return q
 
     def projected(self):
-        """The columns with a projected entry (an aggregate other than median, increase, mode and count_distinct)."""
+        """The columns with a projected entry (an aggregate other than median, increase, mode, count_distinct and
+        gauge_agg)."""
         return [c for c in self.columns if c.agg_mask or not any(getattr(c, a, False) for a in PSEUDO_AGGS)]
 
     def output_names(self):
@@ -326,7 +372,8 @@ class QueryOption:
                 [(c.column_id, "median") for c in self.columns if getattr(c, "median", False)] +
                 [(c.column_id, "increase") for c in self.columns if getattr(c, "increase", False)] +
                 [(c.column_id, "mode") for c in self.columns if getattr(c, "mode", False)] +
-                [(c.column_id, "count_distinct") for c in self.columns if getattr(c, "count_distinct", False)])
+                [(c.column_id, "count_distinct") for c in self.columns if getattr(c, "count_distinct", False)] +
+                [(c.column_id, "gauge_" + g) for c in self.columns if getattr(c, "gauge_agg", False) for g in GAUGE_OUTS])
 
 
 class ScanResult:
@@ -355,6 +402,18 @@ class ScanResult:
         n, _ = raw("n")
         (c, ok), (m2x, _), (m2y, _) = raw("c"), raw("m2x"), raw("m2y")
         return pair_stat(name, n, c, m2x, m2y, ok)
+
+    def gauge(self, column_id, name):
+        """(values, validity) of the gauge_agg of column_id, shaped [n_groups, n_buckets]: one of GAUGE_OUTS (n u64, *_t
+        i64, *_v f64) or one of GAUGE_STATS, derived on the host by gauge_stat."""
+        def raw(g):
+            j = self.names.index((column_id, "gauge_" + g))
+            dt = np.uint64 if g == "n" else np.int64 if g.endswith("_t") else np.float64
+            shape = (self.n_groups, self.n_buckets)
+            return self.values[j].view(dt).reshape(shape), self.validity[j].reshape(shape)
+        if name in GAUGE_OUTS:
+            return raw(name)
+        return gauge_stat(name, *(raw(g)[0] for g in GAUGE_OUTS))
 
     def column(self, column_id, agg):
         """(typed values, validity) of one output column, shaped [n_groups, n_buckets]. agg may also name one of STAT_AGGS

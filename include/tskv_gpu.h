@@ -281,6 +281,37 @@ typedef struct tskv_query {
 #define TSKV_QUERY_N_MODES(flags) (((uint32_t)(flags) >> 24) & 0xfu)
 #define TSKV_QUERY_DISTINCTS(n) (((uint32_t)(n) & 0xfu) << 28)
 #define TSKV_QUERY_N_DISTINCTS(flags) (((uint32_t)(flags) >> 28) & 0xfu)
+/* Gauges: gauge_agg(time, x) (CnosDB's GaugeData: the cell's number of points and its first, second, penultimate and last
+ * point), for delta / rate / time_delta / idelta_left / idelta_right / first_* / last_*. Bits 1..4 of the flags word hold
+ * n_gauges: TSKV_QUERY_GAUGES(n) sets them, TSKV_QUERY_N_GAUGES(flags) reads them (bits 5..7 stay 0). The n_gauges entries
+ * of `columns` after the distincts' operands are the gauges' operands: column_id and phys_type (I64 / U64 / F64) of each,
+ * agg_mask 0; n_columns + 2 * n_pairs + n_medians + n_increases + n_modes + n_distincts + n_gauges <= 126. A gauge takes
+ * the rows a median or increase selects (time ranges, series, the row filter of the predicates, row-drop and column
+ * tombstones, non-NULL time; the merged rows of the overlap merge groups), NULL operand values left out, as points
+ * (t, v) ordered by (t, slot): of points with equal timestamps (several series in one cell) the lower slot comes first
+ * (the reference sorts with sort_unstable_by on the timestamp and leaves that order unspecified). Per cell each gauge adds
+ * 9 outputs after the distincts' outputs: n (u64, the points, always valid, 0 in an empty cell), then first_t, first_v,
+ * second_t, second_v, penultimate_t, penultimate_v, last_t, last_v, the points at positions 0, 1, n - 2 and n - 1 (one
+ * point: all four are it; two: second is the last point, penultimate the first), valid iff n >= 1. The *_t outputs are
+ * i64 in the time column's unit; the *_v outputs f64, integers converted to the nearest double (ties to even, Rust's
+ * `as f64`), f64 values bit for bit. Every grid is accepted, sliding windows included (a window's points are its panes').
+ * Computed in passes of their own: pass 1 gives every cell's n (the operand's kernel mask gains COUNT; an operand that is
+ * not a projected column is read like a COUNT column with no output), one lane per operand page (one thread per merged
+ * row) appends a record per (page, cell) run holding the run's first two and last two points, a radix sort by
+ * (gauge, cell) and a reduce by key join the records, and a sliding scan folds its panes. A cell whose records disagree
+ * with its n is reported as TSKV_ERR_BITSET_MISMATCH with page ~0 (only a decode error pass 1 reports first can cause
+ * it). The record buffers are sized at prepare: summed over the gauges and the operand pages whose column group is
+ * selected and overlaps the time ranges, min(num_values, the grid buckets the group's time span can touch: edge buckets
+ * for labels, panes for sliding scans), plus the merge rows; 88 bytes of state per record, 3 records' worth of buffers.
+ * Multi-rank: the gauge states sit in the exchange region after the pairs' sections; tskvgpu_scan_exchange and
+ * _merge_gathered join the ranks' states; tskvgpu_scan_partials refuses a scan with gauges (TSKV_ERR_UNSUPPORTED). A
+ * multi-rank gauge scan needs series_ids (TSKV_ERR_INVALID_ARG otherwise, as for FIRST / LAST). Refused before any
+ * launch: TSKV_ERR_INVALID_ARG for n_gauges > TSKV_MAX_GAUGES, an operand with a non-zero agg_mask or a BOOL / TIME /
+ * unknown type, an operand id projected with another type, or more than 126 columns; TSKV_ERR_UNSUPPORTED for a record
+ * bound of 2^31 or more. Counters: as for medians; kernel_launches and elapsed_fused_ms include the gauge kernels. */
+#define TSKV_MAX_GAUGES 8
+#define TSKV_QUERY_GAUGES(n) (((uint32_t)(n) & 0xfu) << 1)
+#define TSKV_QUERY_N_GAUGES(flags) (((uint32_t)(flags) >> 1) & 0xfu)
 
 /* Result layout. Outputs are dense: for output column j (query columns in order, and inside a
  * column the set agg bits in ascending bit order) and cell c = group * n_buckets + bucket:

@@ -28,6 +28,7 @@ pub use sys::{tskv_query_medians, tskv_query_n_medians, TSKV_MAX_MEDIANS, TSKV_M
 pub use sys::{tskv_query_increases, tskv_query_n_increases, TSKV_MAX_INCREASES};
 pub use sys::{tskv_query_distincts, tskv_query_modes, tskv_query_n_distincts, tskv_query_n_modes};
 pub use sys::{TSKV_MAX_DISTINCTS, TSKV_MAX_MODES, TSKV_MAX_SORTED_ROWS};
+pub use sys::{tskv_query_gauges, tskv_query_n_gauges, TSKV_MAX_GAUGES};
 
 /// What a failed call reports; maps onto `TskvError` as INTEGRATION.md section 2 lists.
 #[derive(Debug, Clone)]
@@ -114,7 +115,7 @@ impl GpuEngine {
 
     /// The end-to-end call a `BatchReader::process()` makes: query arguments H2D, fused scan, dense result D2H.
     pub fn scan_aggregate(&self, pages: &PageSet<'_>, q: &Query) -> GpuResult<AggregateResult> {
-        let raw = q.as_raw();
+        let raw = q.as_raw()?;
         let layout = self.output_layout(pages, q, &raw)?;
         let mut values = vec![0u64; (layout.n_out * layout.n_cells) as usize];
         let mut validity = vec![0u8; layout.validity_bytes as usize];
@@ -150,7 +151,7 @@ impl GpuEngine {
     /// Sharded scan: every rank scans its own pages with the GLOBAL series list (`Query::multi_rank`), exchanges the
     /// partial state with one ncclAllGather inside the library and finalises the merged result.
     pub fn scan_aggregate_sharded(&self, pages: &PageSet<'_>, q: &Query) -> GpuResult<AggregateResult> {
-        let raw = q.as_raw();
+        let raw = q.as_raw()?;
         let layout = self.output_layout(pages, q, &raw)?;
         let mut scan = std::ptr::null_mut();
         self.check(unsafe {
@@ -255,14 +256,28 @@ pub struct Query {
     /// GROUP BY tags: (group id of every selected series slot, number of groups); output cell = group * n_buckets +
     /// bucket. The shim derives dense ids from the `SeriesKey` tag values (INTEGRATION.md section 6).
     pub groups: Option<(Vec<u32>, u32)>,
+    /// the projected columns, then the `n_gauges` gauges' operands (agg_mask 0)
     pub columns: Vec<tskv_agg_column>,
     pub predicates: Vec<tskv_field_predicate>,
     pub multi_rank: bool,
+    /// gauge_agg(time, x): the last `n_gauges` entries of `columns` are the operands (at most TSKV_MAX_GAUGES); each adds
+    /// 9 outputs after the projected columns' (n, then t / v of the first, second, penultimate and last point), from
+    /// which the shim builds DataFusion's GaugeData struct column (INTEGRATION.md section 6)
+    pub n_gauges: u32,
 }
 
 impl Query {
-    fn as_raw(&self) -> sys::tskv_query {
-        sys::tskv_query {
+    /// The C view of the query; TSKV_ERR_INVALID_ARG when `n_gauges` exceeds TSKV_MAX_GAUGES or the entries of
+    /// `columns` (the library would read operands past the Vec).
+    fn as_raw(&self) -> GpuResult<sys::tskv_query> {
+        if self.n_gauges > sys::TSKV_MAX_GAUGES || self.n_gauges as usize > self.columns.len() {
+            return Err(GpuError {
+                status: sys::TSKV_ERR_INVALID_ARG,
+                message: format!("n_gauges {} exceeds TSKV_MAX_GAUGES or the {} column entries", self.n_gauges, self.columns.len()),
+                page: -1,
+            });
+        }
+        Ok(sys::tskv_query {
             series_ids: self.series_ids.as_ref().map_or(std::ptr::null(), |v| v.as_ptr()),
             n_series: self.series_ids.as_ref().map_or(0, |v| v.len() as u32),
             n_time_ranges: self.time_ranges.len() as u32,
@@ -273,12 +288,12 @@ impl Query {
             n_buckets: self.n_buckets.max(1),
             group_by_series: self.group_by_series as u32,
             columns: self.columns.as_ptr(),
-            n_columns: self.columns.len() as u32,
-            reserved: if self.multi_rank { sys::TSKV_QUERY_MULTI_RANK } else { 0 },
+            n_columns: self.columns.len() as u32 - self.n_gauges,
+            reserved: (if self.multi_rank { sys::TSKV_QUERY_MULTI_RANK } else { 0 }) | sys::tskv_query_gauges(self.n_gauges),
             predicates: if self.predicates.is_empty() { std::ptr::null() } else { self.predicates.as_ptr() },
             n_predicates: self.predicates.len() as u32,
             n_pairs: 0,
-        }
+        })
     }
 }
 

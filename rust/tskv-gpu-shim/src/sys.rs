@@ -78,6 +78,18 @@ pub const fn tskv_query_distincts(n: u32) -> u32 {
 pub const fn tskv_query_n_distincts(flags: u32) -> u32 {
     (flags >> 28) & 0xf
 }
+/// At most this many gauges (gauge_agg(time, x)); their count sits in bits 1..4 of tskv_query.reserved. Their operands
+/// follow the distincts' operands in `columns`; each adds 9 outputs: n, then (t, v) of the first, second, penultimate
+/// and last point.
+pub const TSKV_MAX_GAUGES: u32 = 8;
+/// TSKV_QUERY_GAUGES(n): the flags-word bits of n gauges.
+pub const fn tskv_query_gauges(n: u32) -> u32 {
+    (n & 0xf) << 1
+}
+/// TSKV_QUERY_N_GAUGES(flags): the gauges of a flags word.
+pub const fn tskv_query_n_gauges(flags: u32) -> u32 {
+    (flags >> 1) & 0xf
+}
 
 pub const TSKV_UPLOAD_VERIFY_CRC: u32 = 1;
 pub const TSKV_UPLOAD_HOST_RESIDENT: u32 = 2;
