@@ -376,4 +376,21 @@ __global__ void __launch_bounds__(128) k_gauge_merge_rows(const ScanParams P, co
   gauge_emit(A, (uint64_t)blockIdx.y * A.kern_cells + mr.cell, gauge_point(mr.t, slot, v));
 }
 
+// The state aggs over the merged rows (k_state_scan's pages): one thread per (merge row, state agg = blockIdx.y); the
+// leader of a merged row that survives the row-level filters (merged_row) is a piece of one point, its state the
+// operand's merged value (merge_value), NULL when there is none: k_state_stitch joins it to the points around it in its
+// series, as it joins the pages' pieces.
+__global__ void __launch_bounds__(128) k_state_merge_rows(const ScanParams P, const MergeParams M, const StateCol *scols, const StateArgs A) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  MergedRow mr;
+  if (i >= M.n_rows || !merged_row(P, M, i, mr)) return;
+  const StateCol sc = scols[blockIdx.y];
+  uint64_t v;
+  const bool null = !merge_value(P, M, sc.qcol, mr.series, mr.t, mr.s0, mr.s1, v);
+  StateRun run;
+  run.open = false;
+  state_add(A, blockIdx.y, (uint32_t)M.cg_slot[M.mcg_cg[merge_mcg_of(M, i)]], run, mr.cell, mr.t, null, null ? 0 : state_key(v, sc.phys_type));
+  state_close(A, blockIdx.y, (uint32_t)M.cg_slot[M.mcg_cg[merge_mcg_of(M, i)]], run);
+}
+
 }  // namespace tskv

@@ -3547,6 +3547,283 @@ __global__ void k_finalize_gauges(const uint64_t *state, const GaugeCol *gcols, 
     *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
 }
 
+// ---- state aggs (TSKV_QUERY_N_STATE_AGGS): compact_state_agg(time, x), the time each cell spends in every state ----------
+// A cell holds rows of one series (prepare refuses the rest), and along a series the cells are monotone in time. Every
+// selected row is a point (t, state), a NULL value (the page's bitmap, a column tombstone, a merged row without a value)
+// a state of its own. Each pair of consecutive points adds t' - t to the earlier point's state. Pass 1 (the fused scan)
+// counts each cell's non-NULL rows. k_state_scan (a lane per work item of the operand's buckets) walks a page's points:
+// a run of one state that ends at the next run's first point appends one duration record (segment, state key, t' - t0),
+// and at a cell change or at the page's end the open run appends its partial duration (last t - t0) and the (page, cell)
+// piece appends a boundary record (its first time, its last time and state). k_state_merge_rows does the same for every
+// merged row of the overlap merge groups. Sorted by first time, then stably by (agg, slot), consecutive boundary records
+// of one cell add the gap between them to the earlier one's last state (k_state_stitch). Since every piece already gave
+// its last state an entry, the reference's finalize (a 0 entry for the cell's final state) needs no record of its own.
+// Two radix sorts order the duration records by (segment, state key), a reduce by key sums each key's durations: its
+// unique keys are the cells' map entries in output order. A segment is (agg, cell) << 1 | non-NULL, so that the NULL
+// state comes first; the state key is the operand's order key (i64: sign bit flipped; u64: itself).
+struct StateCol {
+  uint64_t count_off;  // the operand's COUNT section (the cell's non-NULL rows)
+  uint32_t qcol;       // the operand's column in the scan's column table (its work-list buckets, its merged values)
+  uint16_t column_id;
+  uint8_t phys_type;
+  uint8_t pad;
+};
+// One map entry's key: the segment and the state key.
+struct StateKey {
+  uint64_t seg, key;
+  __host__ __device__ __forceinline__ bool operator==(const StateKey &o) const { return seg == o.seg && key == o.key; }
+};
+// One (page, cell) piece of a slot's points: its first time, its last time and its last state.
+struct StateBound {
+  int64_t first_t, last_t;
+  uint64_t seg, key;  // the last state's segment and key
+};
+// The records and the buffers of the sorts and the reduce, all sized at prepare: dbound duration records, bbound
+// boundary records.
+struct StateArgs {
+  uint64_t *seg;        // [2 * dbound] the duration records' segments (~0: no record; sorted after the sorts), then in key order
+  uint64_t *key;        // [2 * dbound] their state keys, then sorted
+  int64_t *dur;         // [dbound] their durations
+  uint32_t *idx;        // [2 * dbound] positions: identity (the (segment, key) order after the sorts), then key order
+  StateKey *skey;       // [dbound] the records' keys in (segment, key) order (segment ~0 past the last record)
+  int64_t *sdur;        // [dbound] their durations
+  StateKey *uniq;       // [dbound] the reduce's keys
+  int64_t *sum;         // [dbound] the reduce's sums
+  int32_t *n_runs;      // the reduce's number of keys
+  unsigned int *n_dur;  // the duration records' append counter
+  unsigned int *n_bnd;  // the boundary records' append counter
+  StateBound *bnd;      // [bbound] boundary records
+  uint64_t *bkey;       // [5 * bbound] slot keys | time keys | time keys sorted | slot keys in time order | slot keys sorted
+  uint32_t *bidx;       // [3 * bbound] identity | time order | (agg, slot, first time) order
+  uint64_t *rows;       // [n_segs] the non-NULL rows the records saw, per (agg, cell)
+  uint32_t *off;        // [n_segs + 1] the entries per (agg, cell), then their exclusive sum (the CSR offsets)
+  int32_t *status;      // the scan's status slot and error page
+  unsigned long long *err_page;
+  uint64_t n_cells, n_segs, dbound, bbound;
+  int64_t t_base;       // boundary time keys: first time - t_base, clamped to t_mask (the page set's time span)
+  uint64_t t_mask;
+  uint32_t slot_bits;   // boundary slot keys: agg << slot_bits | slot
+};
+
+struct StateSum {
+  __host__ __device__ __forceinline__ int64_t operator()(int64_t a, int64_t b) const { return a + b; }
+};
+
+__device__ __forceinline__ uint64_t state_key(uint64_t v, uint8_t pt) { return pt == TSKV_PT_I64 ? v ^ 0x8000000000000000ull : v; }
+__device__ __forceinline__ uint64_t state_seg(uint64_t agg_cell, bool null) { return (agg_cell << 1) | (null ? 0u : 1u); }
+
+// Appends a duration record: the converged lanes of the warp take their places with one atomic.
+__device__ __forceinline__ void state_emit(const StateArgs &A, uint64_t seg, uint64_t key, int64_t d) {
+  const uint32_t m = __activemask(), lane = threadIdx.x & 31, leader = __ffs(m) - 1;
+  uint32_t base = 0;
+  if (lane == leader) base = atomicAdd(A.n_dur, (unsigned int)__popc(m));
+  const uint32_t pos = __shfl_sync(m, base, leader) + __popc(m & ((1u << lane) - 1));
+  if (pos >= A.dbound) {
+    gauge_mismatch(A.status, A.err_page);
+    return;
+  }
+  A.seg[pos] = seg;
+  A.key[pos] = key;
+  A.dur[pos] = d;
+}
+// Appends a boundary record of slot `slot` (agg: the record's state agg) and the piece's non-NULL row count.
+__device__ __forceinline__ void state_bound(const StateArgs &A, uint32_t agg, uint32_t slot, const StateBound &b, uint64_t nn) {
+  const uint32_t m = __activemask(), lane = threadIdx.x & 31, leader = __ffs(m) - 1;
+  uint32_t base = 0;
+  if (lane == leader) base = atomicAdd(A.n_bnd, (unsigned int)__popc(m));
+  const uint32_t pos = __shfl_sync(m, base, leader) + __popc(m & ((1u << lane) - 1));
+  if (nn) atomicAdd(reinterpret_cast<unsigned long long *>(A.rows + (b.seg >> 1)), (unsigned long long)nn);
+  if (pos >= A.bbound) {
+    gauge_mismatch(A.status, A.err_page);
+    return;
+  }
+  A.bnd[pos] = b;
+  A.bkey[pos] = ((uint64_t)agg << A.slot_bits) | slot;
+  const uint64_t dt = (uint64_t)b.first_t - (uint64_t)A.t_base;
+  A.bkey[A.bbound + pos] = b.first_t < A.t_base ? 0 : min(dt, A.t_mask);
+}
+
+// One lane's walk over a piece of points in time order: the open run and the piece.
+struct StateRun {
+  StateBound b;    // the piece: first time, last time, the open run's state
+  int64_t run_t;   // the open run's first time
+  uint64_t nn;     // the piece's non-NULL rows
+  bool open;
+};
+__device__ __forceinline__ void state_close(const StateArgs &A, uint32_t agg, uint32_t slot, StateRun &r) {
+  if (!r.open) return;
+  state_emit(A, r.b.seg, r.b.key, r.b.last_t - r.run_t);
+  state_bound(A, agg, slot, r.b, r.nn);
+  r.open = false;
+}
+__device__ __forceinline__ void state_add(const StateArgs &A, uint32_t agg, uint32_t slot, StateRun &r, uint64_t cell, int64_t t,
+                                          bool null, uint64_t key) {
+  const uint64_t seg = state_seg((uint64_t)agg * A.n_cells + cell, null);
+  if (r.open && (r.b.seg >> 1) != (seg >> 1)) state_close(A, agg, slot, r);
+  if (!r.open) {
+    r.open = true;
+    r.b.first_t = t;
+    r.nn = 0;
+  } else if (r.b.seg != seg || r.b.key != key) {
+    state_emit(A, r.b.seg, r.b.key, t - r.run_t);
+  } else {
+    r.b.last_t = t;
+    r.nn += !null;
+    return;
+  }
+  r.b.seg = seg;
+  r.b.key = key;
+  r.run_t = t;
+  r.b.last_t = t;
+  r.nn += !null;
+}
+
+// One page of a state agg's operand (work item `item` of its buckets), decoded with its group's time page row by row and
+// selected as the medians select (select_row) except that the operand's column tombstones make NULL states instead of
+// dropping the row. Decode errors are pass 1's to report: the lane stops at the first.
+template <bool EDGES>
+__device__ __forceinline__ void state_page(const ScanParams &P, const StateCol &sc, const StateArgs &A, uint32_t agg, uint32_t item) {
+  const uint32_t page = P.work_page[item], slot = P.work_slot[item];
+  const tskv_page_desc vd = P.descs[page];
+  const uint32_t tpage = P.time_page_of[page];
+  const tskv_page_desc td = P.descs[tpage];
+  if (vd.phys_type != sc.phys_type || kind_status(vd.reserved) != TSKV_OK || kind_status(td.reserved) != TSKV_OK ||
+      td.reserved == DK_ALLNULL)
+    return;
+  PageView tpv, vpv;
+  tpv.open(P.arena, td);
+  vpv.open(P.arena, vd);
+  BitCursor tb, vb;
+  tb.init(tpv.bitset);
+  vb.init(vpv.bitset);
+  DeltaCursor<-1> tc;
+  AnyCursor<> vc;
+  if (tc.open(tpv, td.reserved) != TSKV_OK || vc.open(vpv, vd.reserved) != TSKV_OK) return;
+  const bool allnull = vd.reserved == DK_ALLNULL;
+  const uint4 none = make_uint4(0, 0, 0, 0);
+  const uint4 tv4 = P.has_tomb ? tomb_lookup(P, vd.series_id, sc.column_id) : none;
+  const uint4 rows4 = make_uint4(tv4.x, tv4.y, 0, 0);  // (row drops select; the column's ranges make NULL states)
+  const uint32_t *keepw = P.row_keep ? P.row_keep + P.keep_off[tpage] : nullptr;
+  const uint64_t group_base = group_cell_base<EDGES>(P, slot);
+  BucketState bk; bk.valid = false; bk.floor_regime = false; bk.lo = 0; bk.hi = 0; bk.idx = 0;
+  StateRun run;
+  run.open = false;
+  run.b.first_t = run.b.last_t = run.run_t = 0;
+  run.b.seg = run.b.key = run.nn = 0;
+  int64_t t = 0;
+  const uint32_t n_rows = vd.num_values;
+  for (uint32_t r = 0; r < n_rows; r++) {
+    const bool tv = tb.next(r), vv = vb.next(r) && !allnull;
+    uint64_t v = 0;
+    if (tv) { t = (int64_t)tc.next(); if (tc.exhausted) break; }
+    else if (r == 0) tc.skip_first_if_s8b_sc();
+    if (vv) { v = vc.next(); if (vc.failed()) break; }
+    else if (r == 0 && !vc.is_gorilla) vc.d.skip_first_if_s8b_sc();
+    uint64_t cell;
+    if (!tv || !select_row<EDGES>(P, keepw, r, t, rows4, none, group_base, bk, cell)) continue;
+    bool null = !vv;
+    if (!null && tv4.w) {
+      int64_t lo = INT64_MIN, hi = INT64_MAX;
+      null = tomb_span(P.tomb_ranges + tv4.z, tv4.w, t, lo, hi);
+    }
+    state_add(A, agg, slot, run, cell, t, null, null ? 0 : state_key(v, sc.phys_type));
+  }
+  state_close(A, agg, slot, run);
+}
+
+// The state aggs' pages (blockIdx.y: the state agg): one lane per work item of the operand's buckets (every bin, wide and
+// narrow), the items pass 1 read. (A minimum of one block per SM lets ptxas keep the walk in registers: with the
+// default it settles on 128 registers and spills.)
+template <bool EDGES>
+__global__ void __launch_bounds__(128, 1) k_state_scan(const __grid_constant__ ScanParams P, const StateCol *scols, const StateArgs A) {
+  const StateCol sc = scols[blockIdx.y];
+  const uint32_t stride = gridDim.x * blockDim.x, t0 = blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t k = sc.qcol * WL_SUB; k < N_BINS * P.n_cols * WL_SUB; k += P.n_cols * WL_SUB)
+    for (uint32_t sub = 0; sub < WL_SUB; sub++) {
+      const uint32_t start = __ldg(P.region_start + k + sub), fill = __ldg(P.region_fill + k + sub);
+      for (uint32_t i = t0; i < fill; i += stride) state_page<EDGES>(P, sc, A, blockIdx.y, start + i);
+    }
+}
+
+// Before the record kernels: no boundary record, the identity permutations the sorts start from.
+__global__ void k_state_init(const StateArgs A) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < A.bbound; i += (uint64_t)gridDim.x * blockDim.x) {
+    A.bkey[i] = ~0ull;
+    A.bkey[A.bbound + i] = 0;
+    A.bidx[i] = (uint32_t)i;
+  }
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < A.dbound; i += (uint64_t)gridDim.x * blockDim.x) {
+    A.seg[i] = ~0ull;
+    A.key[i] = ~0ull;
+    A.dur[i] = 0;
+    A.idx[i] = (uint32_t)i;
+  }
+}
+
+// After the boundary sorts (records in (agg, slot, first time) order, empty ones last): a record whose successor holds
+// the same agg and slot and starts in the same cell adds the gap to its last state.
+__global__ void k_state_stitch(const StateArgs A) {
+  const uint64_t *slot_sorted = A.bkey + 4 * A.bbound;
+  const uint32_t *order = A.bidx + 2 * A.bbound;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x + 1; j < A.bbound; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t key = slot_sorted[j];
+    if (key == ~0ull || slot_sorted[j - 1] != key) continue;
+    const StateBound a = A.bnd[order[j - 1]], b = A.bnd[order[j]];
+    if ((a.seg >> 1) != (b.seg >> 1)) continue;
+    state_emit(A, a.seg, a.key, b.first_t - a.last_t);
+  }
+}
+
+// Between the two sorts of the boundary records (out[j] = key[idx[j]]) and of the duration records (the segments in key
+// order): one gather.
+__global__ void k_state_gather(const uint64_t *key, const uint32_t *idx, uint64_t n, uint64_t *out) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) out[j] = key[idx[j]];
+}
+
+// After the duration sorts (the sorted segments and the final order over the records' own): the records' (segment, key)
+// and durations in that order.
+__global__ void k_state_order(const StateArgs A) {
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < A.dbound; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t i = A.idx[j];
+    StateKey k;
+    k.seg = A.seg[j];
+    k.key = A.key[i];
+    A.skey[j] = k;
+    A.sdur[j] = A.dur[i];
+  }
+}
+
+// After the reduce: each (agg, cell)'s entries (the unique keys past the last cell's, segment ~0, are not entries).
+__global__ void k_state_count(const StateArgs A) {
+  const uint64_t n = (uint64_t)max(*A.n_runs, 0);
+  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t s = A.uniq[r].seg >> 1;
+    if (s < A.n_segs) atomicAdd(A.off + s, 1u);
+  }
+}
+
+// Every cell of every state agg: a non-NULL row count that disagrees with pass 1's is an error.
+__global__ void k_state_check(const uint64_t *state, const StateCol *scols, const StateArgs A) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < A.n_segs; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t g = i / A.n_cells, cell = i - g * A.n_cells;
+    if (A.rows[i] != state[scols[g].count_off + cell]) gauge_mismatch(A.status, A.err_page);
+  }
+}
+
+// The state agg outputs (blockIdx.y: the state agg; output column out0 + blockIdx.y): the cell's map entries (u64,
+// always valid).
+__global__ void k_finalize_states(const StateArgs A, uint32_t out0, uint64_t bitmap_stride, uint64_t *values, uint8_t *validity) {
+  const uint64_t cell = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool valid = cell < A.n_cells;
+  if (valid) {
+    const uint64_t s = (uint64_t)blockIdx.y * A.n_cells + cell;
+    values[(uint64_t)(out0 + blockIdx.y) * A.n_cells + cell] = (uint64_t)(A.off[s + 1] - A.off[s]);
+  }
+  const uint32_t bits = __ballot_sync(FULL, valid);
+  if ((threadIdx.x & 31) == 0 && (cell >> 3) < bitmap_stride)
+    *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
+}
+
 // Per output column: which state arrays feed it.
 struct OutCol {
   uint64_t count_off;  // counts of the source column

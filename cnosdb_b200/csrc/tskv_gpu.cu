@@ -305,6 +305,22 @@ struct tskv_scan {
   async_ptr<uint8_t> d_gauge_tmp;
   size_t gauge_tmp_bytes = 0;
   GaugeArgs gauge{};
+  // state aggs (TSKV_QUERY_N_STATE_AGGS; k_state_scan): their operands (on the host too: the result call reads their
+  // types), the duration and boundary records with the sorts' and the reduce's buffers (StateArgs), and the CSR offsets
+  uint32_t n_states = 0;
+  std::vector<StateCol> h_states;
+  int state_seg_bits = 1;         // the segment bits the second duration sort reads (segment ~0 sorts last)
+  int state_time_sort_bits = 64;  // the boundary sorts' bits
+  int state_slot_sort_bits = 1;
+  bool state_time_span_known = true;  // false: a selected group has rows outside the page set's time span (alloc_scan)
+  async_ptr<StateCol> d_states;
+  async_ptr<uint64_t> d_state_u64;   // seg [2 * dbound] | key [2 * dbound] | dur [dbound] | sdur | sum | bkey [5 * bbound] | rows [n_segs]
+  async_ptr<StateKey> d_state_keys;  // skey [dbound] | uniq [dbound]
+  async_ptr<StateBound> d_state_bnd;
+  async_ptr<uint32_t> d_state_u32;   // idx [2 * dbound] | bidx [3 * bbound] | off [n_segs + 1] | n_dur | n_bnd | n_runs
+  async_ptr<uint8_t> d_state_tmp;
+  size_t state_tmp_bytes = 0;
+  StateArgs st{};
 };
 
 namespace {
@@ -400,13 +416,16 @@ uint32_t query_n_gauges(const tskv_query *q) { return TSKV_QUERY_N_GAUGES(q->res
 uint64_t query_gauge_col0(const tskv_query *q) {
   return (uint64_t)q->n_columns + 2ull * q->n_pairs + query_n_medians(q) + query_n_increases(q) + query_n_modes(q) + query_n_distincts(q);
 }
+uint32_t query_n_state_aggs(const tskv_query *q) { return TSKV_QUERY_N_STATE_AGGS(q->reserved); }
+// the columns before the state aggs' operands
+uint64_t query_state_col0(const tskv_query *q) { return query_gauge_col0(q) + query_n_gauges(q); }
 
 // The query the scan runs for a query with column pairs, medians or increases: its projected columns, then every operand that is
 // not one of them as a COUNT column without output (so that the work list, the page gathers, CRC checks, pass 1 and the
 // reader counters treat the operands' pages as they treat a COUNT column's), and per pair, median and increase the
 // operands' places in that table. A median's operand column also computes MIN and MAX in pass 1 (its extreme keys); an increase's
-// operand column computes COUNT (its validity), and so does a mode's or distinct's (its n) and a gauge's (its n). Modes
-// and distincts share one gather per operand column id.
+// operand column computes COUNT (its validity), and so does a mode's or distinct's (its n), a gauge's (its n) and a state
+// agg's (its non-NULL rows). Modes and distincts share one gather per operand column id.
 struct OperandQuery {
   tskv_query q{};
   std::vector<tskv_agg_column> cols;
@@ -416,6 +435,7 @@ struct OperandQuery {
   std::vector<ModeGather> gathers;     // (count_off is set by plan_layout)
   std::vector<ModeOut> mode_outs;      // the modes', then the distincts' outputs
   std::vector<GaugeCol> gauges;        // (count_off is set by plan_layout)
+  std::vector<StateCol> states;        // (count_off is set by plan_layout)
 };
 OperandQuery plan_operand_query(const tskv_query *q) {
   OperandQuery pq;
@@ -479,6 +499,15 @@ OperandQuery plan_operand_query(const tskv_query *q) {
     gc.column_id = op.column_id;
     gc.phys_type = op.phys_type;
     pq.gauges.push_back(gc);
+  }
+  for (uint32_t k = 0; k < query_n_state_aggs(q); k++) {
+    const tskv_agg_column &op = q->columns[query_state_col0(q) + k];
+    StateCol sc{};
+    sc.qcol = place(op);
+    pq.cols[sc.qcol].agg_mask |= TSKV_AGG_COUNT;
+    sc.column_id = op.column_id;
+    sc.phys_type = op.phys_type;
+    pq.states.push_back(sc);
   }
   pq.q.columns = pq.cols.data();
   pq.q.n_columns = (uint32_t)pq.cols.size();
@@ -649,7 +678,8 @@ bool labels_first_last(const tskv_query *q, const BucketEdges &E) {
 bool query_shape_ok(const tskv_query *q, bool edges = false) {
   return q->n_buckets != 0 &&
          (q->n_columns != 0 || q->n_pairs != 0 || query_n_medians(q) != 0 || query_n_increases(q) != 0 ||
-          query_n_modes(q) != 0 || query_n_distincts(q) != 0 || query_n_gauges(q) != 0) && q->columns &&
+          query_n_modes(q) != 0 || query_n_distincts(q) != 0 || query_n_gauges(q) != 0 || query_n_state_aggs(q) != 0) &&
+         q->columns &&
          (q->width > 0 || q->n_buckets == 1 || edges);
 }
 
@@ -664,6 +694,7 @@ tskv_output_layout output_layout(const tskv_pages *pages, const tskv_query *q, c
   if (query_n_modes(q) <= TSKV_MAX_MODES) n_out += query_n_modes(q);
   if (query_n_distincts(q) <= TSKV_MAX_DISTINCTS) n_out += query_n_distincts(q);
   if (query_n_gauges(q) <= TSKV_MAX_GAUGES) n_out += (uint64_t)GAUGE_OUTS * query_n_gauges(q);
+  n_out += query_n_state_aggs(q);  // (3 bits: at most TSKV_MAX_STATE_AGGS)
   uint64_t n_groups = 1;
   if (q->group_by_series) n_groups = selected_slots(pages, q);
   if (tg.on) n_groups = tg.n;
@@ -1030,6 +1061,23 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
         return TSKV_ERR_INVALID_ARG;
       }
   }
+  const uint32_t n_state = query_n_state_aggs(q);
+  if (query_state_col0(q) + n_state > 126) {
+    ctx->set_error("invalid query: at most 126 columns with every operand");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  for (uint64_t k = query_state_col0(q); k < query_state_col0(q) + n_state; k++) {
+    const tskv_agg_column &op = q->columns[k];
+    if (op.agg_mask != 0 || (op.phys_type != TSKV_PT_I64 && op.phys_type != TSKV_PT_U64)) {
+      ctx->set_error("invalid state agg operand: an I64 / U64 column with agg_mask 0");
+      return TSKV_ERR_INVALID_ARG;
+    }
+    for (uint64_t c = 0; c < k; c++)
+      if (q->columns[c].column_id == op.column_id && q->columns[c].phys_type != op.phys_type) {
+        ctx->set_error("state agg operand: one column id with two types");
+        return TSKV_ERR_INVALID_ARG;
+      }
+  }
   if (q->n_predicates > TSKV_MAX_PREDICATES || (q->n_predicates && !q->predicates)) {
     ctx->set_error("invalid query: at most 8 field predicates");
     return TSKV_ERR_INVALID_ARG;
@@ -1097,23 +1145,29 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
     ctx->set_error("multi-rank scan: modes and distincts are not pushed down (their state is the values themselves)");
     return TSKV_ERR_UNSUPPORTED;
   }
-  if (n_inc) {  // increases pair consecutive rows of one series: a cell must never hold two selected series
-    const char *why = nullptr;
-    if (slide) why = "sliding windows: increases are not pushed down";
-    else if (E.labelled) why = "bucket labels: increases are not pushed down (date_part cells are not monotone in time)";
+  if (n_state && (q->reserved & TSKV_QUERY_MULTI_RANK)) {
+    ctx->set_error("multi-rank scan: state aggs are not pushed down (a cell's map does not fit the fixed exchange region)");
+    return TSKV_ERR_UNSUPPORTED;
+  }
+  // increases and state aggs pair consecutive rows of one series: a cell must never hold two selected series
+  if (n_inc || n_state) {
+    const char *what = n_inc ? "increase" : "state agg";
+    std::string why;
+    if (slide) why = std::string("sliding windows: ") + what + "s are not pushed down";
+    else if (E.labelled) why = std::string("bucket labels: ") + what + "s are not pushed down (date_part cells are not monotone in time)";
     else if (tg.on) {
       std::vector<uint8_t> seen(tg.n, 0);
       const uint64_t n_slots = selected_slots(pages, q);
-      for (uint64_t i = 0; i < n_slots && !why; i++)
-        if (seen[tg.ids[i]]++) why = "increase: a tag group holds two selected series (a cell must hold one series)";
+      for (uint64_t i = 0; i < n_slots && why.empty(); i++)
+        if (seen[tg.ids[i]]++) why = std::string(what) + ": a tag group holds two selected series (a cell must hold one series)";
     } else if (!q->group_by_series) {
       // (a multi-rank scan decides from the query alone, so that every rank agrees: without series_ids each rank would
       // count only its own series, and the exchange would sum several series' increases into one cell)
       if (q->series_ids ? q->n_series > 1 : (q->reserved & TSKV_QUERY_MULTI_RANK) || pages->series.size() > 1)
-        why = "increase: an ungrouped scan over more than one selected series, or a multi-rank one without series_ids "
+        why = std::string(what) + ": an ungrouped scan over more than one selected series, or a multi-rank one without series_ids "
               "(a cell must hold one series)";
     }
-    if (why) {
+    if (!why.empty()) {
       ctx->set_error(why);
       return TSKV_ERR_UNSUPPORTED;
     }
@@ -1196,6 +1250,7 @@ struct ScanLayout {
   std::vector<ModeOut> mode_outs;
   std::vector<GaugeCol> gauges;        // the gauges, with their operands' COUNT sections
   uint64_t gauge_off = 0, gauge_words = 0;
+  std::vector<StateCol> states;        // the state aggs, with their operands' COUNT sections
 };
 
 // n_cells: cells of the query's grid (a sliding scan: windows); kern_cells: cells of the fused kernels' grid (panes).
@@ -1236,6 +1291,8 @@ ScanLayout plan_layout(const tskv_query *q, bool sliding, uint64_t n_cells, uint
   for (GaugeCol &gc : out.gauges) gc.count_off = win.cols[gc.qcol].count_off;
   out.gauge_off = win.gauge_off;
   out.gauge_words = win.gauge_words;
+  out.states = oq.states;  // (sliding scans refuse state aggs)
+  for (StateCol &sc : out.states) sc.count_off = win.cols[sc.qcol].count_off;
   if (sliding) {
     for (uint32_t c = 0; c < q->n_columns; c++) {
       const ColState &p = pane.cols[c], &w = win.cols[c];
@@ -1686,6 +1743,72 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
     A.n_runs = reinterpret_cast<int32_t *>(A.idx + 2 * A.bound + 1);
     A.dst = sliding ? A.rec + 3 * A.bound : reinterpret_cast<GaugeAcc *>(s->d_state.get() + s->gauge_off);
     *h2d += lay.gauges.size() * sizeof(GaugeCol);
+  }
+  s->n_states = (uint32_t)lay.states.size();
+  s->h_states = lay.states;
+  if (s->n_states) {  // (prepare_scan has bounded the records: s->st.dbound, s->st.bbound)
+    StateArgs &A = s->st;
+    A.n_cells = s->layout.n_cells;
+    A.n_segs = (uint64_t)s->n_states * A.n_cells;
+    A.dbound = std::max<uint64_t>(A.dbound, 1);
+    A.bbound = std::max<uint64_t>(A.bbound, 1);
+    const uint64_t D = A.dbound, B = A.bbound;
+    s->state_seg_bits = 64 - __builtin_clzll(2 * A.n_segs);
+    // boundary sort keys: the slot sort reads (agg, slot) bits, and the slot field of a record never has all of its bits
+    // set, so an empty record's ~0 sorts after every other; the time sort reads the bits of the page set's time span
+    const uint64_t n_slots = selected_slots(pages, q);
+    A.slot_bits = 64 - __builtin_clzll(std::max<uint64_t>(n_slots, 1));
+    s->state_slot_sort_bits = (int)A.slot_bits + (s->n_states > 1 ? 32 - __builtin_clz(s->n_states - 1) : 0);
+    ensure_time_bounds(ctx, pages);
+    A.t_base = INT64_MIN;
+    A.t_mask = ~0ull;
+    s->state_time_sort_bits = 64;
+    if (s->state_time_span_known && pages->ts_min <= pages->ts_max && !(pages->ts_min == INT64_MIN && pages->ts_max == INT64_MAX)) {
+      const uint64_t span = (uint64_t)pages->ts_max - (uint64_t)pages->ts_min;
+      A.t_base = pages->ts_min;
+      s->state_time_sort_bits = span ? 64 - __builtin_clzll(span) : 1;
+      A.t_mask = s->state_time_sort_bits == 64 ? ~0ull : (1ull << s->state_time_sort_bits) - 1;
+    }
+    size_t t[6] = {0, 0, 0, 0, 0, 0};
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, t[0], (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                                               (uint32_t *)nullptr, (int)B, 0, s->state_time_sort_bits, st);
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, t[1], (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                                               (uint32_t *)nullptr, (int)B, 0, s->state_slot_sort_bits, st);
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, t[2], (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                                               (uint32_t *)nullptr, (int)D, 0, 64, st);
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, t[3], (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                                               (uint32_t *)nullptr, (int)D, 0, s->state_seg_bits, st);
+    if (e == cudaSuccess) e = cub::DeviceReduce::ReduceByKey(nullptr, t[4], (const StateKey *)nullptr, (StateKey *)nullptr, (const int64_t *)nullptr,
+                                                              (int64_t *)nullptr, (int32_t *)nullptr, StateSum{}, (int)D, st);
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, t[5], (uint32_t *)nullptr, (int64_t)(A.n_segs + 1), st);
+    s->state_tmp_bytes = std::max<size_t>(*std::max_element(t, t + 6), 1);
+    if (e == cudaSuccess) e = upload(s->d_states, lay.states.data(), lay.states.size(), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_state_u64, (size_t)(7 * D + 5 * B + A.n_segs), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_state_keys, (size_t)(2 * D), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_state_bnd, (size_t)B, st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_state_u32, (size_t)(2 * D + 3 * B + A.n_segs + 4), st);
+    if (e == cudaSuccess) e = stream_alloc(s->d_state_tmp, s->state_tmp_bytes, st);
+    uint64_t *w = s->d_state_u64.get();
+    A.seg = w;
+    A.key = w + 2 * D;
+    A.dur = reinterpret_cast<int64_t *>(w + 4 * D);
+    A.sdur = reinterpret_cast<int64_t *>(w + 5 * D);
+    A.sum = reinterpret_cast<int64_t *>(w + 6 * D);
+    A.bkey = w + 7 * D;
+    A.rows = w + 7 * D + 5 * B;
+    A.skey = s->d_state_keys.get();
+    A.uniq = A.skey + D;
+    A.bnd = s->d_state_bnd.get();
+    uint32_t *u = s->d_state_u32.get();
+    A.idx = u;
+    A.bidx = u + 2 * D;
+    A.off = u + 2 * D + 3 * B;
+    A.n_dur = reinterpret_cast<unsigned int *>(A.off + A.n_segs + 1);
+    A.n_bnd = A.n_dur + 1;
+    A.n_runs = reinterpret_cast<int32_t *>(A.n_dur + 2);
+    // (a scan that has not run yet holds empty maps: tskvgpu_scan_state_durations reads the offsets)
+    if (e == cudaSuccess) e = cudaMemsetAsync(A.off, 0, (A.n_segs + 1) * sizeof(uint32_t), st);
+    *h2d += lay.states.size() * sizeof(StateCol);
   }
   if (e == cudaSuccess) e = stream_alloc(s->d_aux, AUX_WORDS, st);
   if (e == cudaSuccess) e = stream_alloc(s->d_values, s->layout.n_out * s->layout.n_cells, st);
@@ -2546,6 +2669,97 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
       return TSKV_ERR_UNSUPPORTED;
     }
   }
+  // state aggs: per operand page of a column group that can hold selected rows, one duration record per row (a run
+  // ends at most once per row) and one boundary record per (page, cell) piece (the gauges' bound), each piece adding
+  // its open run's record and a stitch record; every merge row is a piece of its own. Sized here so that run and enqueue
+  // neither allocate nor synchronise.
+  uint64_t state_dbound = 0, state_bbound = 0;
+  bool state_time_span_known = true;  // (the boundary records' time keys may be narrowed to the page set's span)
+  if (!pq.states.empty()) {
+    ensure_time_bounds(ctx, pages);
+    std::vector<tskv_time_range> cg_bounds(pages->n_cg);
+    if (pages->n_cg && (!pages->d_cg_bounds || cudaMemcpy(cg_bounds.data(), pages->d_cg_bounds.get(), pages->n_cg * sizeof(tskv_time_range),
+                                                          cudaMemcpyDeviceToHost) != cudaSuccess)) {
+      ctx->set_error(std::string("state agg: column-group time bounds: ") + cudaGetErrorString(cudaGetLastError()));
+      return TSKV_ERR_CUDA;
+    }
+    // A selected group whose bounds say min > max: bounds computed from its time page mean it has no timestamp, but
+    // bounds handed in by the caller may say so of a group with rows, whose times the page set's span then misses.
+    bool unbounded = false;
+    for (uint32_t cg = 0; cg < pages->n_cg && !unbounded; cg++) {
+      if (!cg_selected(pages, q, cg_bounds.data(), cg) || cg_bounds[cg].min_ts <= cg_bounds[cg].max_ts) continue;
+      for (uint64_t p = (uint64_t)pages->h_cg_time_page[cg] + 1; p < pages->n_descs && pages->h_descs[p].phys_type != TSKV_PT_TIME; p++)
+        unbounded |= pages->h_descs[p].num_values != 0;
+    }
+    // a cell's durations sum to at most its last time - its first time, which must fit i64: only a cell that can span
+    // 2^63 or more (an unbucketed scan, or an edge bucket that wide) can break that
+    state_time_span_known = !unbounded;
+    int64_t lo = unbounded ? INT64_MIN : pages->ts_min, hi = unbounded ? INT64_MAX : pages->ts_max;
+    clip_to_query_ranges(q, lo, hi);
+    bool too_wide = false;
+    if (lo <= hi) {
+      if (E.on) {
+        for (uint32_t b = 0; b < E.n && !too_wide; b++) {
+          const int64_t blo = std::max(E.edges[b], lo), bhi = std::min<int64_t>((int64_t)((uint64_t)E.edges[b + 1] - 1), hi);
+          too_wide = bhi >= blo && (((uint64_t)bhi - (uint64_t)blo) >> 63);
+        }
+      } else if (q->width <= 0) {
+        too_wide = ((uint64_t)hi - (uint64_t)lo) >> 63;
+      }
+    }
+    if (too_wide) {
+      ctx->set_error("state agg: a cell's selectable rows can span 2^63 or more (its durations would not fit i64)");
+      return TSKV_ERR_UNSUPPORTED;
+    }
+    __int128 grid_lo = INT64_MIN, grid_hi = INT64_MAX;
+    if (E.on) {
+      grid_lo = E.edges[0];
+      grid_hi = (__int128)E.edges[E.n] - 1;
+    } else if (q->width > 0) {
+      grid_lo = q->first_bucket_start;
+      grid_hi = grid_lo + (__int128)q->n_buckets * q->width - 1;
+    }
+    auto buckets = [&](const tskv_time_range &b) -> uint64_t {  // (as the gauges' bound)
+      int64_t blo = b.min_ts, bhi = b.max_ts;
+      clip_to_query_ranges(q, blo, bhi);
+      blo = (int64_t)std::max<__int128>(blo, grid_lo);
+      bhi = (int64_t)std::min<__int128>(bhi, grid_hi);
+      if (blo > bhi) return 0;
+      if (E.on) {
+        const int64_t *e0 = E.edges, *e1 = E.edges + E.n + 1;
+        return (uint64_t)(std::upper_bound(e0, e1, bhi) - std::upper_bound(e0, e1, blo)) + 1;
+      }
+      if (q->width > 0) return ((uint64_t)bhi - (uint64_t)blo) / (uint64_t)q->width + 2;
+      return 1;
+    };
+    for (const StateCol &sc : pq.states) {
+      for (uint32_t cg = 0; cg < pages->n_cg; cg++) {
+        if (!cg_selected(pages, q, cg_bounds.data(), cg)) continue;
+        // (a group without time bounds, min > max: bounds computed from its time page mean it has no timestamp, but
+        // bounds handed in by the caller may say so of a group with rows, so every row may be a piece of its own)
+        const bool unbounded = cg_bounds[cg].min_ts > cg_bounds[cg].max_ts;
+        const uint64_t touch = unbounded ? UINT64_MAX : buckets(cg_bounds[cg]);
+        bool has = false;
+        for (uint64_t p = (uint64_t)pages->h_cg_time_page[cg] + 1; p < pages->n_descs && pages->h_descs[p].phys_type != TSKV_PT_TIME; p++)
+          if (pages->h_descs[p].column_id == sc.column_id) {
+            const uint64_t n = pages->h_descs[p].num_values, pieces = std::min<uint64_t>(n, touch);
+            state_dbound += n + pieces;
+            state_bbound += pieces;
+            has = true;
+          }
+        if (!has) {
+          ctx->set_error("state agg: a selected column group has no page of the operand (its rows would be NULL states)");
+          return TSKV_ERR_UNSUPPORTED;
+        }
+      }
+      state_dbound += 2 * pages->overlap.merge_rows;
+      state_bbound += pages->overlap.merge_rows;
+    }
+    if (state_dbound >> 31) {
+      ctx->set_error("state agg: the record bound reaches 2^31 (the sorts and the reduce count items in int)");
+      return TSKV_ERR_UNSUPPORTED;
+    }
+  }
   q = &pq.q;
   bool has_sel = false;  // any FIRST / LAST
   for (uint32_t c = 0; c < q->n_columns; c++) has_sel |= (q->columns[c].agg_mask & (TSKV_AGG_FIRST | TSKV_AGG_LAST)) != 0;
@@ -2572,6 +2786,9 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   uint64_t h2d = 0;
   s->mode.bound = mode_bound;
   s->gauge.bound = gauge_bound;
+  s->st.dbound = state_dbound;
+  s->st.bbound = state_bbound;
+  s->state_time_span_known = state_time_span_known;
   if ((st = alloc_scan(ctx, pages, q, tg, slide != 0, E, lay, s, &h2d)) != TSKV_OK) {
     delete s;
     return st;
@@ -2594,6 +2811,8 @@ static tskv_status prepare_scan(tskv_ctx *ctx, const tskv_pages *pages, const ts
   s->mode.err_page = s->d_err_page;
   s->gauge.status = s->d_status;
   s->gauge.err_page = s->d_err_page;
+  s->st.status = s->d_status;
+  s->st.err_page = s->d_err_page;
   P.stats = s->d_stats;
   P.n_ranges = q->n_time_ranges;
   for (uint32_t k = 0; k < q->n_time_ranges; k++) P.ranges[k] = q->time_ranges[k];
@@ -3035,6 +3254,57 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     launches++;
     if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), stream);  // (the fused time includes the gauge kernels)
   }
+  if (s->n_states) {  // state aggs: the pieces' records (merged rows too), the stitch, the sorts, the reduce, the entries
+    const StateArgs &A = s->st;
+    cudaStream_t stream = ctx->stream.get();
+    const uint64_t D = A.dbound, B = A.bbound;
+    const uint32_t dx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((D + 255) / 256, 4096));
+    const uint32_t bx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((B + 255) / 256, 4096));
+    const uint32_t cx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((A.n_segs + 255) / 256, 4096));
+    const uint32_t px = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)pages->n_descs + 127) / 128, (uint64_t)ctx->sm_count * 16));
+    const StateCol *sp = s->d_states.get();
+    CU_TRY(ctx, cudaMemsetAsync(A.rows, 0, A.n_segs * sizeof(uint64_t), stream));
+    CU_TRY(ctx, cudaMemsetAsync(A.off, 0, (A.n_segs + 3) * sizeof(uint32_t), stream));  // (the offsets and the two counters)
+    k_state_init<<<std::max(dx, bx), 256, 0, stream>>>(A);
+    const void *fn = s->params.edges ? (const void *)k_state_scan<true> : (const void *)k_state_scan<false>;
+    void *args[] = {(void *)&s->params, (void *)&sp, (void *)&s->st};
+    CU_TRY(ctx, cudaLaunchKernel(fn, dim3(px, s->n_states), dim3(128), args, 0, stream));
+    launches += 2;
+    if (s->merge.n_rows && s->n_merge_pages) {
+      k_state_merge_rows<<<dim3((uint32_t)((s->merge.n_rows + 127) / 128), s->n_states), 128, 0, stream>>>(s->params, s->merge, sp, A);
+      launches++;
+    }
+    // boundary records by first time, then (stably) by (agg, slot): keys [slot | time | time sorted | slot in time order |
+    // slot sorted], indices [identity | time order | final order]; each sort reads only its keys' bits (alloc_scan)
+    uint64_t *bk = A.bkey;
+    uint32_t *bi = A.bidx;
+    size_t tmp = s->state_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_state_tmp.get(), tmp, bk + B, bk + 2 * B, bi, bi + B, (int)B, 0,
+                                                s->state_time_sort_bits, stream));
+    k_state_gather<<<bx, 256, 0, stream>>>(bk, bi + B, B, bk + 3 * B);
+    tmp = s->state_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_state_tmp.get(), tmp, bk + 3 * B, bk + 4 * B, bi + B, bi + 2 * B, (int)B, 0,
+                                                s->state_slot_sort_bits, stream));
+    k_state_stitch<<<bx, 256, 0, stream>>>(A);
+    // duration records by state key, then (stably) by segment: segments [records, then sorted | in key order], positions
+    // [identity, then final order | key order]; then the keys and durations in (segment, key) order for the reduce
+    tmp = s->state_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_state_tmp.get(), tmp, A.key, A.key + D, A.idx, A.idx + D, (int)D, 0, 64, stream));
+    k_state_gather<<<dx, 256, 0, stream>>>(A.seg, A.idx + D, D, A.seg + D);
+    tmp = s->state_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_state_tmp.get(), tmp, A.seg + D, A.seg, A.idx + D, A.idx, (int)D, 0,
+                                                s->state_seg_bits, stream));
+    k_state_order<<<dx, 256, 0, stream>>>(A);
+    tmp = s->state_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceReduce::ReduceByKey(s->d_state_tmp.get(), tmp, (const StateKey *)A.skey, A.uniq, (const int64_t *)A.sdur, A.sum,
+                                               A.n_runs, StateSum{}, (int)D, stream));
+    k_state_count<<<dx, 256, 0, stream>>>(A);
+    tmp = s->state_tmp_bytes;
+    CU_TRY(ctx, cub::DeviceScan::ExclusiveSum(s->d_state_tmp.get(), tmp, A.off, (int64_t)(A.n_segs + 1), stream));
+    k_state_check<<<cx, 256, 0, stream>>>(s->d_state.get(), sp, A);
+    launches += 12;  // (a sort, reduce or scan counts as one launch)
+    if (!capturing) cudaEventRecord(s->ev_bin[N_BINS].get(), stream);  // (the fused time includes the state agg kernels)
+  }
   if (!capturing) cudaEventRecord(s->ev1.get(), ctx->stream.get());
   CU_TRY(ctx, cudaGetLastError());
   ctx->counters.kernel_launches = launches;
@@ -3170,12 +3440,47 @@ tskv_status tskvgpu_scan_work_list(tskv_ctx *ctx, tskv_scan *s, uint32_t *n_buck
   return TSKV_OK;
 }
 
-// Medians, modes and distincts keep no mergeable partial state: the exchange calls refuse a scan with any of them.
+// Medians, modes, distincts and state aggs keep no mergeable partial state: the exchange calls refuse a scan with any of
+// them.
 static tskv_status refuse_medians(tskv_ctx *ctx, const tskv_scan *s, const char *call) {
-  if (!s->n_medians && !s->n_gathers) return TSKV_OK;
+  if (!s->n_medians && !s->n_gathers && !s->n_states) return TSKV_OK;
   std::lock_guard<std::mutex> lock(ctx->mu);
-  ctx->set_error(std::string(call) + ": a scan with medians, modes or distincts has no mergeable partial state");
+  ctx->set_error(std::string(call) + ": a scan with medians, modes, distincts or state aggs has no mergeable partial state");
   return TSKV_ERR_UNSUPPORTED;
+}
+
+tskv_status tskvgpu_scan_state_durations(tskv_ctx *ctx, tskv_scan *s, uint32_t k, uint64_t *offsets, uint64_t *states, uint8_t *state_valid,
+                                         int64_t *durations, uint64_t *n_entries) {
+  if (!ctx || !s || !n_entries) return TSKV_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  ctx->set_error("");
+  if (k >= s->n_states) {
+    ctx->set_error("scan_state_durations: k is not a state agg of the scan");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  const StateArgs &A = s->st;
+  const uint64_t n_cells = A.n_cells;
+  std::vector<uint32_t> off(n_cells + 1);
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream.get()));
+  CU_TRY(ctx, cudaMemcpy(off.data(), A.off + (uint64_t)k * n_cells, off.size() * 4, cudaMemcpyDeviceToHost));
+  const uint64_t base = off[0], n = off[n_cells] - base;
+  *n_entries = n;
+  if (offsets)
+    for (uint64_t c = 0; c <= n_cells; c++) offsets[c] = off[c] - base;
+  if (!n || !(states || state_valid || durations)) return TSKV_OK;
+  if (states || state_valid) {
+    std::vector<StateKey> keys(n);
+    CU_TRY(ctx, cudaMemcpy(keys.data(), A.uniq + base, n * sizeof(StateKey), cudaMemcpyDeviceToHost));
+    const bool i64 = s->h_states[k].phys_type == TSKV_PT_I64;
+    for (uint64_t i = 0; i < n; i++) {
+      const bool valid = keys[i].seg & 1;
+      if (state_valid) state_valid[i] = valid;
+      if (states) states[i] = !valid ? 0 : i64 ? keys[i].key ^ 0x8000000000000000ull : keys[i].key;
+    }
+  }
+  if (durations) CU_TRY(ctx, cudaMemcpy(durations, A.sum + base, n * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  return TSKV_OK;
 }
 
 tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *s, tskv_partials_view *out) {
@@ -3321,6 +3626,10 @@ static tskv_status finalize_device(tskv_ctx *ctx, tskv_scan *s) {
     k_finalize_gauges<<<dim3((uint32_t)((L.n_cells + 255) / 256), GAUGE_OUTS * s->n_gauges), 256, 0, ctx->stream.get()>>>(
         s->d_state.get(), s->d_gauges.get(), s->gauge_off, s->n_out + 4 * s->n_pairs + s->n_medians + s->n_increases + s->n_mode_outs,
         L.n_cells, L.bitmap_stride, s->d_values.get(), s->d_validity.get());
+  if (s->n_states)
+    k_finalize_states<<<dim3((uint32_t)((L.n_cells + 255) / 256), s->n_states), 256, 0, ctx->stream.get()>>>(
+        s->st, s->n_out + 4 * s->n_pairs + s->n_medians + s->n_increases + s->n_mode_outs + GAUGE_OUTS * s->n_gauges, L.bitmap_stride,
+        s->d_values.get(), s->d_validity.get());
   CU_TRY(ctx, cudaGetLastError());
   return TSKV_OK;
 }

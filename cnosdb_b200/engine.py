@@ -219,7 +219,7 @@ class TskvError(RuntimeError):
 
 
 # the aggregates without a mask bit: each makes its column an operand of its own kind
-PSEUDO_AGGS = ("median", "increase", "mode", "count_distinct", "gauge_agg")
+PSEUDO_AGGS = ("median", "increase", "mode", "count_distinct", "gauge_agg", "compact_state_agg")
 # the outputs of one gauge_agg(time, x): the points, then (time, value) of its first, second, penultimate and last point
 GAUGE_OUTS = ("n", "first_t", "first_v", "second_t", "second_v", "penultimate_t", "penultimate_v", "last_t", "last_v")
 # the accessors of CnosDB's GaugeData (gauge/mod.rs) that gauge_stat derives from the nine outputs
@@ -263,13 +263,20 @@ def gauge_stat(name, n, first_t, first_v, second_t, second_v, penultimate_t, pen
     raise ValueError("unknown gauge accessor %r (one of %s)" % (name, ", ".join(GAUGE_STATS)))
 
 
+def duration_in(state_map, state):
+    """duration_in(compact_state_agg(time, x), state) without a start time: the map's duration of `state` (None: the
+    NULL state), 0 when the map has no entry for it (StateAggData::duration_in)."""
+    return state_map.get(None if state is None else int(state), 0)
+
+
 class PushedAggregate:
     """One projected value column with its aggregate set (extends PushedAggregateFunction::Count). "median" has no mask
     bit: it makes the column a median operand (after the pairs' operands, agg_mask 0), and a column that asks for nothing
     else has no projected entry. "increase" (increase(time, x ORDER BY time)) likewise makes it an increase operand, after
     the medians' operands; "mode" (mode(x)) a mode operand, after the increases' operands; "count_distinct"
-    (COUNT(DISTINCT x)) a distinct operand, after the modes' operands; and "gauge_agg" (gauge_agg(time, x)) a gauge
-    operand, after the distincts' operands."""
+    (COUNT(DISTINCT x)) a distinct operand, after the modes' operands; "gauge_agg" (gauge_agg(time, x)) a gauge
+    operand, after the distincts' operands; and "compact_state_agg" (compact_state_agg(time, x)) a state agg operand,
+    after the gauges' operands."""
 
     def __init__(self, column_id, phys_type, aggs):
         self.column_id = int(column_id)
@@ -279,6 +286,7 @@ class PushedAggregate:
         self.mode = False
         self.count_distinct = False
         self.gauge_agg = False
+        self.compact_state_agg = False
         if isinstance(aggs, int):
             self.agg_mask = aggs
         else:
@@ -287,7 +295,7 @@ class PushedAggregate:
                 if a == "median":
                     self.median = True
                     continue
-                if a in ("increase", "mode", "count_distinct", "gauge_agg"):
+                if a in ("increase", "mode", "count_distinct", "gauge_agg", "compact_state_agg"):
                     setattr(self, a, True)
                     continue
                 # var* / stddev* ask the scan for COUNT | M2; ScanResult.column derives them
@@ -336,14 +344,15 @@ class QueryOption:
         modes = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "mode", False)]
         dists = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "count_distinct", False)]
         gauges = [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "gauge_agg", False)]
+        states = self.state_aggs()
         q.reserved = ((cabi.TSKV_QUERY_MULTI_RANK if self.multi_rank else 0) | cabi.query_medians(len(meds)) |
                       cabi.query_increases(len(incs)) | cabi.query_modes(len(modes)) | cabi.query_distincts(len(dists)) |
-                      cabi.query_gauges(len(gauges)))
-        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))] + meds + incs + modes + dists + gauges
+                      cabi.query_gauges(len(gauges)) | cabi.query_state_aggs(len(states)))
+        ops = [o for x, xt, y, yt in self.pairs for o in ((x, xt), (y, yt))] + meds + incs + modes + dists + gauges + states
         cols = (cabi.AggColumn * max(1, len(proj) + len(ops)))()
         for i, c in enumerate(proj):
             cols[i].column_id, cols[i].phys_type, cols[i].agg_mask = c.column_id, c.phys_type, c.agg_mask
-        for i, (cid, pt) in enumerate(ops):  # the pairs', medians', increases', modes', distincts' and gauges' operands follow
+        for i, (cid, pt) in enumerate(ops):  # the pairs', medians', increases', modes', distincts', gauges' and state aggs' operands follow
             cols[len(proj) + i].column_id, cols[len(proj) + i].phys_type = cid, pt
         q.columns = cols
         q.n_columns = len(proj)
@@ -361,9 +370,14 @@ class QueryOption:
         self._keep = (tr, cols, preds)  # keep the ctypes arrays alive as long as the query
         return q
 
+    def state_aggs(self):
+        """(column_id, phys_type) of the compact_state_agg operands, in the order of their outputs and of k in
+        PreparedScan.state_durations(k)."""
+        return [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "compact_state_agg", False)]
+
     def projected(self):
-        """The columns with a projected entry (an aggregate other than median, increase, mode, count_distinct and
-        gauge_agg)."""
+        """The columns with a projected entry (an aggregate other than median, increase, mode, count_distinct, gauge_agg
+        and compact_state_agg)."""
         return [c for c in self.columns if c.agg_mask or not any(getattr(c, a, False) for a in PSEUDO_AGGS)]
 
     def output_names(self):
@@ -373,7 +387,8 @@ class QueryOption:
                 [(c.column_id, "increase") for c in self.columns if getattr(c, "increase", False)] +
                 [(c.column_id, "mode") for c in self.columns if getattr(c, "mode", False)] +
                 [(c.column_id, "count_distinct") for c in self.columns if getattr(c, "count_distinct", False)] +
-                [(c.column_id, "gauge_" + g) for c in self.columns if getattr(c, "gauge_agg", False) for g in GAUGE_OUTS])
+                [(c.column_id, "gauge_" + g) for c in self.columns if getattr(c, "gauge_agg", False) for g in GAUGE_OUTS] +
+                [(cid, "state_entries") for cid, _ in self.state_aggs()])
 
 
 class ScanResult:
@@ -388,6 +403,9 @@ class ScanResult:
                              bitorder="little")
         self.validity = bits[:, : int(layout.n_cells)].astype(bool)
         self.phys = {(c.column_id): c.phys_type for c in query.columns}
+        # compact_state_agg: column_id -> (offsets, states, state_valid, durations), PreparedScan.state_durations's CSR
+        # (set by PreparedScan.finalize; the one-shot C calls return only the entry counts)
+        self.state_csr = {}
 
     def pair(self, k, name):
         """(values f64 / u64 for n, validity) of column pair k, shaped [n_groups, n_buckets]: one of PAIR_AGGS (covar,
@@ -415,10 +433,19 @@ class ScanResult:
             return raw(name)
         return gauge_stat(name, *(raw(g)[0] for g in GAUGE_OUTS))
 
+    def state_maps(self, column_id):
+        """The compact_state_agg maps of column_id, one {state: duration} dict per cell, shaped [n_groups][n_buckets]
+        (the NULL state is the key None; states are Python ints of the operand's type, durations i64 in the time
+        column's unit). duration_in(map, state) reads one."""
+        off, states, valid, durs = self.state_csr[column_id]
+        maps = [{(int(states[i]) if valid[i] else None): int(durs[i]) for i in range(off[c], off[c + 1])}
+                for c in range(len(off) - 1)]
+        return [maps[g * self.n_buckets:(g + 1) * self.n_buckets] for g in range(self.n_groups)]
+
     def column(self, column_id, agg):
         """(typed values, validity) of one output column, shaped [n_groups, n_buckets]. agg may also name one of STAT_AGGS
         (var, var_samp, var_pop, stddev, stddev_samp, stddev_pop), derived from the column's count and m2, "median" /
-        "increase" / "mode" (the operand's type) or "count_distinct" (u64)."""
+        "increase" / "mode" (the operand's type), "count_distinct" or "state_entries" (u64)."""
         if agg in STAT_AGGS:
             n, _ = self.column(column_id, "count")
             m2, ok = self.column(column_id, "m2")
@@ -426,7 +453,7 @@ class ScanResult:
         j = self.names.index((column_id, agg))
         raw = self.values[j]
         pt = self.phys[column_id]
-        if agg in ("count", "count_distinct"):
+        if agg in ("count", "count_distinct", "state_entries"):
             v = raw.view(np.uint64)
         elif agg in ("mean", "m2") or pt == TSKV_PT_F64:
             v = raw.view(np.float64)
@@ -521,6 +548,22 @@ class PreparedScan:
                                                       *[a.ctypes.data for a in out.values()]))
         return out
 
+    def state_durations(self, k):
+        """The maps of state agg k (query.state_aggs()[k]) after run / sync, tskvgpu_scan_state_durations's CSR:
+        (offsets u64 [n_cells + 1], states [n_entries] in the operand's type (0 for the NULL state), state_valid bool,
+        durations i64); cell c owns entries offsets[c] .. offsets[c + 1], the NULL state first, then the states in order."""
+        lib, ctx = self.engine.lib, self.engine.ctx
+        n = C.c_uint64(0)
+        self.engine._check(lib.tskvgpu_scan_state_durations(ctx, self.handle, int(k), None, None, None, None, C.byref(n)))
+        pt = self.query.state_aggs()[k][1] if k < len(self.query.state_aggs()) else TSKV_PT_I64
+        off = np.zeros(int(self.layout.n_cells) + 1, np.uint64)
+        states = np.zeros(n.value, np.int64 if pt == TSKV_PT_I64 else np.uint64)
+        valid = np.zeros(n.value, np.uint8)
+        durs = np.zeros(n.value, np.int64)
+        self.engine._check(lib.tskvgpu_scan_state_durations(ctx, self.handle, int(k), off.ctypes.data, states.ctypes.data,
+                                                            valid.ctypes.data, durs.ctypes.data, C.byref(n)))
+        return off, states, valid.astype(bool), durs
+
     def exchange_view(self):
         """(device pointer, length in 8-byte words) of the region a multi-GPU run all-gathers."""
         a, b = C.c_uint64(0), C.c_uint64(0)
@@ -547,7 +590,10 @@ class PreparedScan:
         bitmaps = np.empty(int(L.validity_bytes), dtype=np.uint8)
         self.engine._check(self.engine.lib.tskvgpu_scan_finalize(
             self.engine.ctx, self.handle, values.ctypes.data, bitmaps.ctypes.data))
-        return ScanResult(self.query, L, values, bitmaps)
+        res = ScanResult(self.query, L, values, bitmaps)
+        for k, (cid, _) in enumerate(self.query.state_aggs()):
+            res.state_csr[cid] = self.state_durations(k)
+        return res
 
     def finalize_device(self):
         a, b = C.c_uint64(0), C.c_uint64(0)
@@ -739,7 +785,15 @@ class Engine:
         edges: explicit time buckets [edges[b], edges[b + 1]) (query.n_buckets + 1 increasing timestamps, query.width,
         origin and first_bucket_start 0; calendar_edges makes them for date_trunc). Not with slide.
         labels: with edges, labels[b] < query.n_buckets is the output bucket of edge bucket b (one per edge bucket;
-        calendar_parts makes them for date_part). query.n_buckets is then the number of output buckets."""
+        calendar_parts makes them for date_part). query.n_buckets is then the number of output buckets.
+        A query with compact_state_agg runs prepare, run and finalize, so that its result holds the maps too."""
+        if query.state_aggs():
+            scan = self.prepare(pages, query, slide, group_ids, n_groups, edges, labels)
+            try:
+                scan.run()
+                return scan.finalize()
+            finally:
+                scan.close()
         self._no_m2_with_slide(query, slide)
         e = self._edges(edges, slide)
         lab = self._labels(labels, e)

@@ -283,7 +283,7 @@ typedef struct tskv_query {
 #define TSKV_QUERY_N_DISTINCTS(flags) (((uint32_t)(flags) >> 28) & 0xfu)
 /* Gauges: gauge_agg(time, x) (CnosDB's GaugeData: the cell's number of points and its first, second, penultimate and last
  * point), for delta / rate / time_delta / idelta_left / idelta_right / first_* / last_*. Bits 1..4 of the flags word hold
- * n_gauges: TSKV_QUERY_GAUGES(n) sets them, TSKV_QUERY_N_GAUGES(flags) reads them (bits 5..7 stay 0). The n_gauges entries
+ * n_gauges: TSKV_QUERY_GAUGES(n) sets them, TSKV_QUERY_N_GAUGES(flags) reads them. The n_gauges entries
  * of `columns` after the distincts' operands are the gauges' operands: column_id and phys_type (I64 / U64 / F64) of each,
  * agg_mask 0; n_columns + 2 * n_pairs + n_medians + n_increases + n_modes + n_distincts + n_gauges <= 126. A gauge takes
  * the rows a median or increase selects (time ranges, series, the row filter of the predicates, row-drop and column
@@ -312,6 +312,43 @@ typedef struct tskv_query {
 #define TSKV_MAX_GAUGES 8
 #define TSKV_QUERY_GAUGES(n) (((uint32_t)(n) & 0xfu) << 1)
 #define TSKV_QUERY_N_GAUGES(flags) (((uint32_t)(flags) >> 1) & 0xfu)
+/* State aggs: compact_state_agg(time, x) (CnosDB's DurationStates: the time a cell spends in every state of x), for
+ * duration_in(agg, state) and duration_in(state_agg(time, x), state) without a start time. Bits 5..7 of the flags word
+ * hold n_state_aggs: TSKV_QUERY_STATE_AGGS(n) sets them, TSKV_QUERY_N_STATE_AGGS(flags) reads them; with them every bit
+ * of the flags word is taken. The n_state_aggs entries of `columns` after the gauges' operands are the state aggs'
+ * operands: column_id and phys_type (I64 / U64) of each, agg_mask 0; n_columns + 2 * n_pairs + n_medians + n_increases +
+ * n_modes + n_distincts + n_gauges + n_state_aggs <= 126. A state agg walks a cell's selected rows (time ranges, series,
+ * the row filter of the predicates, row-drop tombstones, non-NULL time; the merged rows of the overlap merge groups) in
+ * time order as points (t, state). A NULL value - the page's bitmap, a column tombstone, a merged row without a value -
+ * is a state of its own (the reference keys its map by ScalarValue, and Int64(None) is a key). Each pair of consecutive
+ * points (t, s), (t', s') adds t' - t to the duration of s; the last point's state then gets a 0 entry if it has none
+ * (DurationStates::finalize). A cell without rows has an empty map. Durations are i64 in the time column's unit. Per
+ * cell each state agg adds one u64 output after the gauges' outputs: the number of the map's entries, the NULL state
+ * included, always valid (0 in an empty cell). The maps themselves come from tskvgpu_scan_state_durations (below); the
+ * one-shot tskvgpu_scan_aggregate* calls return only the counts. A cell must hold rows of one series only (the rule of
+ * the increases). Computed in passes of their own: pass 1 gives every cell's non-NULL rows (the operand's kernel mask
+ * gains COUNT; an operand that is not a projected column is read like a COUNT column with no output), one lane per
+ * operand page appends a duration record per run of one state and a boundary record per (page, cell) piece, every
+ * merged row is a piece of its own, the boundary records of every series, sorted by time, add the gaps between the
+ * pieces of a cell, and two radix sorts and a reduce by key sum the durations per (state agg, cell, NULL flag, state).
+ * A cell whose records saw another number of non-NULL rows than pass 1 counted is reported as TSKV_ERR_BITSET_MISMATCH
+ * with page ~0 (only a decode error pass 1 reports first can cause it). The record buffers are sized at prepare: summed
+ * over the state aggs and the operand pages whose column group is selected and overlaps the time ranges, num_values
+ * plus min(num_values, the grid buckets the group's time span can touch; num_values for a group whose bounds have
+ * min > max) duration records and as many boundary records, plus two duration records and one boundary record per merge
+ * row; about 90 bytes per record. Refused before any launch:
+ * TSKV_ERR_INVALID_ARG for an operand with a non-zero agg_mask or an F64 / BOOL / TIME / unknown type, an operand id
+ * projected with another type, or more than 126 columns; TSKV_ERR_UNSUPPORTED for a cell that could hold rows of two
+ * selected series (as for increases), sliding windows (slide != width), tskvgpu_scan_prepare_labels,
+ * TSKV_QUERY_MULTI_RANK (a map does not fit the fixed exchange region), a selected column group that overlaps the time
+ * ranges and has no page of the operand (its rows would be NULL states, and the scan reads no time page alone), a cell
+ * whose selectable rows can span 2^63 or more (an unbucketed scan, or an edge bucket that wide: its durations would not
+ * fit i64), and a duration record bound of 2^31 or more. tskvgpu_scan_partials, _exchange_view, _exchange and
+ * _merge_gathered refuse a scan with state aggs. Counters: as for medians; kernel_launches and elapsed_fused_ms include
+ * the state agg kernels. */
+#define TSKV_MAX_STATE_AGGS 7
+#define TSKV_QUERY_STATE_AGGS(n) (((uint32_t)(n) & 0x7u) << 5)
+#define TSKV_QUERY_N_STATE_AGGS(flags) (((uint32_t)(flags) >> 5) & 0x7u)
 
 /* Result layout. Outputs are dense: for output column j (query columns in order, and inside a
  * column the set agg bits in ascending bit order) and cell c = group * n_buckets + bucket:
@@ -508,6 +545,14 @@ tskv_status tskvgpu_scan_partials(tskv_ctx *ctx, tskv_scan *scan, tskv_partials_
 tskv_status tskvgpu_scan_work_list(tskv_ctx *ctx, tskv_scan *scan, uint32_t *n_buckets, uint32_t *n_items,
                                    uint32_t *region_start, uint32_t *fill, uint32_t *work_page, uint32_t *work_slot,
                                    uint8_t *work_qcol, uint8_t *page_bin, uint8_t *page_narrow);
+/* The maps of state agg k (< TSKV_QUERY_N_STATE_AGGS, TSKV_ERR_INVALID_ARG otherwise) after scan_run / scan_sync, in CSR
+ * form in host buffers: cell c owns entries [offsets[c], offsets[c + 1]) (offsets [n_cells + 1]); entry i is the state
+ * states[i] (the i64 / u64 bit pattern; 0 for the NULL state) with state_valid[i] (0: the NULL state, 1: a value) and its
+ * duration durations[i] (i64, the time column's unit). Within a cell the NULL state comes first, then the states in the
+ * type's order (i64 signed, u64 unsigned). Each array may be null; *n_entries (= offsets[n_cells]) is always written:
+ * call with null arrays first to size them. A scan that has not run yet has empty maps (*n_entries 0). */
+tskv_status tskvgpu_scan_state_durations(tskv_ctx *ctx, tskv_scan *scan, uint32_t k, uint64_t *offsets, uint64_t *states,
+                                         uint8_t *state_valid, int64_t *durations, uint64_t *n_entries);
 /* Alternative with a single collective: all-gather the exchange region (device pointer + length in
  * 8-byte words) of every rank into `gathered` (rank-major, n_ranks * words) and merge locally. */
 tskv_status tskvgpu_scan_exchange_view(tskv_ctx *ctx, tskv_scan *scan, uint64_t *out_dptr, uint64_t *out_words);

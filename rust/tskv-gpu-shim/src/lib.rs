@@ -29,6 +29,7 @@ pub use sys::{tskv_query_increases, tskv_query_n_increases, TSKV_MAX_INCREASES};
 pub use sys::{tskv_query_distincts, tskv_query_modes, tskv_query_n_distincts, tskv_query_n_modes};
 pub use sys::{TSKV_MAX_DISTINCTS, TSKV_MAX_MODES, TSKV_MAX_SORTED_ROWS};
 pub use sys::{tskv_query_gauges, tskv_query_n_gauges, TSKV_MAX_GAUGES};
+pub use sys::{tskv_query_n_state_aggs, tskv_query_state_aggs, TSKV_MAX_STATE_AGGS};
 
 /// What a failed call reports; maps onto `TskvError` as INTEGRATION.md section 2 lists.
 #[derive(Debug, Clone)]
@@ -132,6 +133,57 @@ impl GpuEngine {
         Ok(AggregateResult { layout, values, validity })
     }
 
+    /// `scan_aggregate` for a query with state aggs (`Query::n_state_aggs`): the dense result (each state agg's output is
+    /// the cell's number of map entries) and every state agg's maps, which the one-shot call does not return.
+    pub fn scan_aggregate_states(&self, pages: &PageSet<'_>, q: &Query) -> GpuResult<(AggregateResult, Vec<StateDurations>)> {
+        let raw = q.as_raw()?;
+        let layout = self.output_layout(pages, q, &raw)?;
+        let mut scan = std::ptr::null_mut();
+        self.check(unsafe {
+            match (&q.groups, q.slide) {
+                (Some((ids, n)), slide) => {
+                    sys::tskvgpu_scan_prepare_grouped(self.ctx, pages.pages, &raw, ids.as_ptr(), *n, slide.unwrap_or(0), &mut scan)
+                }
+                (None, None) => sys::tskvgpu_scan_prepare(self.ctx, pages.pages, &raw, &mut scan),
+                (None, Some(slide)) => sys::tskvgpu_scan_prepare_sliding(self.ctx, pages.pages, &raw, slide, &mut scan),
+            }
+        })?;
+        let mut values = vec![0u64; (layout.n_out * layout.n_cells) as usize];
+        let mut validity = vec![0u8; layout.validity_bytes as usize];
+        let mut maps = Vec::with_capacity(q.n_state_aggs as usize);
+        let mut run = || -> GpuResult<()> {
+            self.check(unsafe { sys::tskvgpu_scan_run(self.ctx, scan) })?;
+            self.check(unsafe { sys::tskvgpu_scan_finalize(self.ctx, scan, values.as_mut_ptr(), validity.as_mut_ptr()) })?;
+            for k in 0..q.n_state_aggs {
+                maps.push(self.state_durations(scan, k, layout.n_cells)?);
+            }
+            Ok(())
+        };
+        let r = run();
+        unsafe { sys::tskvgpu_scan_destroy(self.ctx, scan) };
+        r.map(|_| (AggregateResult { layout, values, validity }, maps))
+    }
+
+    /// The maps of state agg k of a scan that has run: sized by a first call with null arrays, then filled.
+    fn state_durations(&self, scan: *mut sys::tskv_scan, k: u32, n_cells: u64) -> GpuResult<StateDurations> {
+        let mut n = 0u64;
+        self.check(unsafe {
+            sys::tskvgpu_scan_state_durations(self.ctx, scan, k, std::ptr::null_mut(), std::ptr::null_mut(), std::ptr::null_mut(),
+                                              std::ptr::null_mut(), &mut n)
+        })?;
+        let mut m = StateDurations {
+            offsets: vec![0; n_cells as usize + 1],
+            states: vec![0; n as usize],
+            state_valid: vec![0; n as usize],
+            durations: vec![0; n as usize],
+        };
+        self.check(unsafe {
+            sys::tskvgpu_scan_state_durations(self.ctx, scan, k, m.offsets.as_mut_ptr(), m.states.as_mut_ptr(),
+                                              m.state_valid.as_mut_ptr(), m.durations.as_mut_ptr(), &mut n)
+        })?;
+        Ok(m)
+    }
+
     fn output_layout(&self, pages: &PageSet<'_>, q: &Query, raw: &sys::tskv_query) -> GpuResult<sys::tskv_output_layout> {
         let mut layout = sys::tskv_output_layout::default();
         self.check(unsafe {
@@ -165,7 +217,7 @@ impl GpuEngine {
         })?;
         let mut values = vec![0u64; (layout.n_out * layout.n_cells) as usize];
         let mut validity = vec![0u8; layout.validity_bytes as usize];
-        let run = || -> GpuResult<()> {
+        let mut run = || -> GpuResult<()> {
             self.check(unsafe { sys::tskvgpu_scan_enqueue(self.ctx, scan) })?;
             self.check(unsafe { sys::tskvgpu_scan_exchange(self.ctx, scan) })?;
             self.check(unsafe { sys::tskvgpu_scan_finalize(self.ctx, scan, values.as_mut_ptr(), validity.as_mut_ptr()) })?;
@@ -256,7 +308,8 @@ pub struct Query {
     /// GROUP BY tags: (group id of every selected series slot, number of groups); output cell = group * n_buckets +
     /// bucket. The shim derives dense ids from the `SeriesKey` tag values (INTEGRATION.md section 6).
     pub groups: Option<(Vec<u32>, u32)>,
-    /// the projected columns, then the `n_gauges` gauges' operands (agg_mask 0)
+    /// the projected columns, then the `n_gauges` gauges' operands, then the `n_state_aggs` state aggs' operands
+    /// (agg_mask 0)
     pub columns: Vec<tskv_agg_column>,
     pub predicates: Vec<tskv_field_predicate>,
     pub multi_rank: bool,
@@ -264,16 +317,34 @@ pub struct Query {
     /// 9 outputs after the projected columns' (n, then t / v of the first, second, penultimate and last point), from
     /// which the shim builds DataFusion's GaugeData struct column (INTEGRATION.md section 6)
     pub n_gauges: u32,
+    /// compact_state_agg(time, x): the last `n_state_aggs` entries of `columns` are the operands (I64 / U64, at most
+    /// TSKV_MAX_STATE_AGGS); each adds 1 output after the gauges' (the cell's map entries), and
+    /// `GpuEngine::scan_aggregate_states` returns the maps, from which the shim builds the DurationStates list column
+    /// (INTEGRATION.md section 6)
+    pub n_state_aggs: u32,
+}
+
+/// One state agg's maps in CSR form (tskvgpu_scan_state_durations): cell c owns entries `offsets[c]..offsets[c + 1]`,
+/// the NULL state (`state_valid` 0) first, then the states (i64 / u64 bit patterns) in the type's order; `durations` in
+/// the time column's unit.
+#[derive(Clone, Debug, Default)]
+pub struct StateDurations {
+    pub offsets: Vec<u64>,
+    pub states: Vec<u64>,
+    pub state_valid: Vec<u8>,
+    pub durations: Vec<i64>,
 }
 
 impl Query {
-    /// The C view of the query; TSKV_ERR_INVALID_ARG when `n_gauges` exceeds TSKV_MAX_GAUGES or the entries of
-    /// `columns` (the library would read operands past the Vec).
+    /// The C view of the query; TSKV_ERR_INVALID_ARG when `n_gauges` exceeds TSKV_MAX_GAUGES, `n_state_aggs`
+    /// TSKV_MAX_STATE_AGGS, or their sum the entries of `columns` (the library would read operands past the Vec).
     fn as_raw(&self) -> GpuResult<sys::tskv_query> {
-        if self.n_gauges > sys::TSKV_MAX_GAUGES || self.n_gauges as usize > self.columns.len() {
+        let n_ops = self.n_gauges as usize + self.n_state_aggs as usize;
+        if self.n_gauges > sys::TSKV_MAX_GAUGES || self.n_state_aggs > sys::TSKV_MAX_STATE_AGGS || n_ops > self.columns.len() {
             return Err(GpuError {
                 status: sys::TSKV_ERR_INVALID_ARG,
-                message: format!("n_gauges {} exceeds TSKV_MAX_GAUGES or the {} column entries", self.n_gauges, self.columns.len()),
+                message: format!("n_gauges {} / n_state_aggs {} exceed their maxima or the {} column entries", self.n_gauges,
+                                 self.n_state_aggs, self.columns.len()),
                 page: -1,
             });
         }
@@ -288,8 +359,10 @@ impl Query {
             n_buckets: self.n_buckets.max(1),
             group_by_series: self.group_by_series as u32,
             columns: self.columns.as_ptr(),
-            n_columns: self.columns.len() as u32 - self.n_gauges,
-            reserved: (if self.multi_rank { sys::TSKV_QUERY_MULTI_RANK } else { 0 }) | sys::tskv_query_gauges(self.n_gauges),
+            n_columns: (self.columns.len() - n_ops) as u32,
+            reserved: (if self.multi_rank { sys::TSKV_QUERY_MULTI_RANK } else { 0 })
+                | sys::tskv_query_gauges(self.n_gauges)
+                | sys::tskv_query_state_aggs(self.n_state_aggs),
             predicates: if self.predicates.is_empty() { std::ptr::null() } else { self.predicates.as_ptr() },
             n_predicates: self.predicates.len() as u32,
             n_pairs: 0,

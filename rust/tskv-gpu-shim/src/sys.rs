@@ -90,6 +90,18 @@ pub const fn tskv_query_gauges(n: u32) -> u32 {
 pub const fn tskv_query_n_gauges(flags: u32) -> u32 {
     (flags >> 1) & 0xf
 }
+/// At most this many state aggs (compact_state_agg(time, x)); their count sits in bits 5..7 of tskv_query.reserved (with
+/// them the flags word is full). Their operands follow the gauges' operands in `columns`; each adds 1 output (the cell's
+/// map entries), and tskvgpu_scan_state_durations returns the maps.
+pub const TSKV_MAX_STATE_AGGS: u32 = 7;
+/// TSKV_QUERY_STATE_AGGS(n): the flags-word bits of n state aggs.
+pub const fn tskv_query_state_aggs(n: u32) -> u32 {
+    (n & 0x7) << 5
+}
+/// TSKV_QUERY_N_STATE_AGGS(flags): the state aggs of a flags word.
+pub const fn tskv_query_n_state_aggs(flags: u32) -> u32 {
+    (flags >> 5) & 0x7
+}
 
 pub const TSKV_UPLOAD_VERIFY_CRC: u32 = 1;
 pub const TSKV_UPLOAD_HOST_RESIDENT: u32 = 2;
@@ -449,6 +461,16 @@ extern "C" {
         work_qcol: *mut u8,
         page_bin: *mut u8,
         page_narrow: *mut u8,
+    ) -> tskv_status;
+    pub fn tskvgpu_scan_state_durations(
+        ctx: *mut tskv_ctx,
+        scan: *mut tskv_scan,
+        k: u32,
+        offsets: *mut u64,
+        states: *mut u64,
+        state_valid: *mut u8,
+        durations: *mut i64,
+        n_entries: *mut u64,
     ) -> tskv_status;
     pub fn tskvgpu_scan_exchange_view(
         ctx: *mut tskv_ctx,
