@@ -111,6 +111,8 @@ def query_n_gauges(flags):
 # state aggs (compact_state_agg(time, x)): n_state_aggs in bits 5..7 of tskv_query.reserved, operands after the gauges',
 # one output each (the cell's map entries); the maps come from tskvgpu_scan_state_durations (see include/tskv_gpu.h)
 TSKV_MAX_STATE_AGGS = 7
+# a state agg operand's agg_mask: the agg computes state_agg(time, x)'s periods too (tskvgpu_scan_state_periods)
+TSKV_STATE_PERIODS = 1 << 7
 
 
 def query_state_aggs(n):
@@ -211,7 +213,7 @@ GPU_SYMBOLS = [
     "tskvgpu_pages_series_count", "tskvgpu_pages_set_time_bounds", "tskvgpu_pages_set_tombstones", "tskvgpu_pages_set_chunk_files", "tskvgpu_pages_set_value_stats", "tskvgpu_decode_pages",
     "tskvgpu_query_output_layout", "tskvgpu_comm_unique_id", "tskvgpu_comm_init", "tskvgpu_comm_destroy", "tskvgpu_scan_exchange",
     "tskvgpu_scan_aggregate", "tskvgpu_scan_prepare", "tskvgpu_scan_run", "tskvgpu_scan_enqueue",
-    "tskvgpu_scan_sync", "tskvgpu_scan_partials", "tskvgpu_scan_work_list", "tskvgpu_scan_state_durations", "tskvgpu_scan_exchange_view", "tskvgpu_scan_merge_gathered",
+    "tskvgpu_scan_sync", "tskvgpu_scan_partials", "tskvgpu_scan_work_list", "tskvgpu_scan_state_durations", "tskvgpu_scan_state_periods", "tskvgpu_scan_exchange_view", "tskvgpu_scan_merge_gathered",
     "tskvgpu_scan_snapshot_keys", "tskvgpu_scan_mask_values", "tskvgpu_scan_finalize",
     "tskvgpu_scan_finalize_device", "tskvgpu_scan_destroy", "tskvgpu_version",
     "tskvgpu_scan_prepare_sliding", "tskvgpu_scan_aggregate_sliding",
@@ -297,6 +299,7 @@ def load_gpu_library():
     lib.tskvgpu_scan_partials.argtypes = [vp, vp, C.POINTER(PartialsView)]
     lib.tskvgpu_scan_work_list.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.tskvgpu_scan_state_durations.argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp, u64p]
+    lib.tskvgpu_scan_state_periods.argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp, vp, u64p]
     lib.tskvgpu_scan_exchange_view.argtypes = [vp, vp, u64p, u64p]
     lib.tskvgpu_scan_merge_gathered.argtypes = [vp, vp, C.c_uint64, C.c_uint32]
     lib.tskvgpu_scan_snapshot_keys.argtypes = [vp, vp]

@@ -3566,7 +3566,7 @@ struct StateCol {
   uint32_t qcol;       // the operand's column in the scan's column table (its work-list buckets, its merged values)
   uint16_t column_id;
   uint8_t phys_type;
-  uint8_t pad;
+  uint8_t periods;     // the operand's agg_mask is TSKV_STATE_PERIODS: the agg returns its periods too
 };
 // One map entry's key: the segment and the state key.
 struct StateKey {
@@ -3584,6 +3584,7 @@ struct StateArgs {
   uint64_t *seg;        // [2 * dbound] the duration records' segments (~0: no record; sorted after the sorts), then in key order
   uint64_t *key;        // [2 * dbound] their state keys, then sorted
   int64_t *dur;         // [dbound] their durations
+  int64_t *start;       // [dbound] their start times (null: no operand has TSKV_STATE_PERIODS, nothing is written)
   uint32_t *idx;        // [2 * dbound] positions: identity (the (segment, key) order after the sorts), then key order
   StateKey *skey;       // [dbound] the records' keys in (segment, key) order (segment ~0 past the last record)
   int64_t *sdur;        // [dbound] their durations
@@ -3612,8 +3613,8 @@ struct StateSum {
 __device__ __forceinline__ uint64_t state_key(uint64_t v, uint8_t pt) { return pt == TSKV_PT_I64 ? v ^ 0x8000000000000000ull : v; }
 __device__ __forceinline__ uint64_t state_seg(uint64_t agg_cell, bool null) { return (agg_cell << 1) | (null ? 0u : 1u); }
 
-// Appends a duration record: the converged lanes of the warp take their places with one atomic.
-__device__ __forceinline__ void state_emit(const StateArgs &A, uint64_t seg, uint64_t key, int64_t d) {
+// Appends a duration record [t, t + d): the converged lanes of the warp take their places with one atomic.
+__device__ __forceinline__ void state_emit(const StateArgs &A, uint64_t seg, uint64_t key, int64_t t, int64_t d) {
   const uint32_t m = __activemask(), lane = threadIdx.x & 31, leader = __ffs(m) - 1;
   uint32_t base = 0;
   if (lane == leader) base = atomicAdd(A.n_dur, (unsigned int)__popc(m));
@@ -3625,6 +3626,7 @@ __device__ __forceinline__ void state_emit(const StateArgs &A, uint64_t seg, uin
   A.seg[pos] = seg;
   A.key[pos] = key;
   A.dur[pos] = d;
+  if (A.start) A.start[pos] = t;
 }
 // Appends a boundary record of slot `slot` (agg: the record's state agg) and the piece's non-NULL row count.
 __device__ __forceinline__ void state_bound(const StateArgs &A, uint32_t agg, uint32_t slot, const StateBound &b, uint64_t nn) {
@@ -3652,7 +3654,7 @@ struct StateRun {
 };
 __device__ __forceinline__ void state_close(const StateArgs &A, uint32_t agg, uint32_t slot, StateRun &r) {
   if (!r.open) return;
-  state_emit(A, r.b.seg, r.b.key, r.b.last_t - r.run_t);
+  state_emit(A, r.b.seg, r.b.key, r.run_t, r.b.last_t - r.run_t);
   state_bound(A, agg, slot, r.b, r.nn);
   r.open = false;
 }
@@ -3665,7 +3667,7 @@ __device__ __forceinline__ void state_add(const StateArgs &A, uint32_t agg, uint
     r.b.first_t = t;
     r.nn = 0;
   } else if (r.b.seg != seg || r.b.key != key) {
-    state_emit(A, r.b.seg, r.b.key, t - r.run_t);
+    state_emit(A, r.b.seg, r.b.key, r.run_t, t - r.run_t);
   } else {
     r.b.last_t = t;
     r.nn += !null;
@@ -3770,7 +3772,7 @@ __global__ void k_state_stitch(const StateArgs A) {
     if (key == ~0ull || slot_sorted[j - 1] != key) continue;
     const StateBound a = A.bnd[order[j - 1]], b = A.bnd[order[j]];
     if ((a.seg >> 1) != (b.seg >> 1)) continue;
-    state_emit(A, a.seg, a.key, b.first_t - a.last_t);
+    state_emit(A, a.seg, a.key, a.last_t, b.first_t - a.last_t);
   }
 }
 
@@ -3822,6 +3824,89 @@ __global__ void k_finalize_states(const StateArgs A, uint32_t out0, uint64_t bit
   const uint32_t bits = __ballot_sync(FULL, valid);
   if ((threadIdx.x & 31) == 0 && (cell >> 3) < bitmap_stride)
     *reinterpret_cast<uint32_t *>(validity + (uint64_t)(out0 + blockIdx.y) * bitmap_stride + (cell >> 3)) = bits;
+}
+
+// ---- state periods (TSKV_STATE_PERIODS): state_agg(time, x)'s periods, for state_at and duration_in with a start --------
+// The duration records tile every series' timeline from its first selected point to its last: a run record [t0, t'),
+// a piece's open run [t0, last t) and a stitch record [last t, next piece's first t), each of the state at its start.
+// After the stitch (before the duration sorts, which overwrite the segments), a stable sort by start time and the stable
+// sorts by state key and by segment order the records by (segment, key, start); a record of length 0, of an operand
+// without the flag or past the last record gets the segment ~0 and sorts last. A record whose predecessor has the same
+// segment and key and ends where it starts joins the predecessor's period (the reference's periods of one pair of points
+// each, joined where they touch); the others start a period. An exclusive sum over the period heads gives every record
+// its period, the heads write the starts and the last record of a period its end. The output order is the CSR order.
+struct PeriodArgs {
+  uint64_t *pkey;   // [2 * dbound] sort keys: start time keys | sorted, then state keys | sorted, then segments | sorted
+  uint32_t *idx;    // [2 * dbound] positions: identity | time order | (time, key) order | (segment, key, start) order
+  uint32_t *head;   // [dbound + 1] 1: the record in (segment, key, start) order starts a period
+  uint32_t *pos;    // [dbound + 1] the heads' exclusive sum (pos[dbound]: the periods)
+  StateKey *out_key;  // [dbound] each period's segment and state key
+  int64_t *out_start, *out_end;  // [dbound] each period's start and end
+  uint32_t *off;    // [n_segs + 1] the periods per (agg, cell), then their exclusive sum (the CSR offsets)
+  uint32_t agg_mask;  // bit g: state agg g has the flag
+};
+
+// The records' start time keys (as the boundary records' time keys: start - t_base, clamped to t_mask) and the identity.
+__global__ void k_period_keys(const StateArgs A, const PeriodArgs Q) {
+  const uint64_t n = min((uint64_t)*A.n_dur, A.dbound);
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < A.dbound; j += (uint64_t)gridDim.x * blockDim.x) {
+    uint64_t k = 0;
+    if (j < n) {
+      const int64_t t = A.start[j];
+      k = t < A.t_base ? 0 : min((uint64_t)t - (uint64_t)A.t_base, A.t_mask);
+    }
+    Q.pkey[j] = k;
+    Q.idx[j] = (uint32_t)j;
+  }
+}
+
+// In (time, key) order: the segment a record sorts by (~0: it is no period's part).
+__global__ void k_period_segs(const StateArgs A, const PeriodArgs Q) {
+  const uint64_t n = min((uint64_t)*A.n_dur, A.dbound);
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < A.dbound; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t i = Q.idx[j];
+    const uint64_t s = A.seg[i];
+    const bool keep = i < n && s != ~0ull && A.dur[i] > 0 && ((Q.agg_mask >> ((s >> 1) / A.n_cells)) & 1);
+    Q.pkey[j] = keep ? s : ~0ull;
+  }
+}
+
+// In (segment, key, start) order (segments Q.pkey + dbound, positions Q.idx + dbound): the period heads, counted per
+// (agg, cell).
+__global__ void k_period_mark(const StateArgs A, const PeriodArgs Q) {
+  const uint64_t *seg = Q.pkey + A.dbound;
+  const uint32_t *idx = Q.idx + A.dbound;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j <= A.dbound; j += (uint64_t)gridDim.x * blockDim.x) {
+    bool h = false;
+    if (j < A.dbound && seg[j] != ~0ull) {
+      const uint32_t i = idx[j];
+      h = true;
+      if (j && seg[j - 1] == seg[j]) {
+        const uint32_t p = idx[j - 1];
+        h = !(A.key[p] == A.key[i] && A.start[p] + A.dur[p] == A.start[i]);
+      }
+      if (h) atomicAdd(Q.off + (seg[j] >> 1), 1u);
+    }
+    Q.head[j] = h;
+  }
+}
+
+// After the heads' exclusive sum: the periods' states, starts and ends.
+__global__ void k_period_write(const StateArgs A, const PeriodArgs Q) {
+  const uint64_t *seg = Q.pkey + A.dbound;
+  const uint32_t *idx = Q.idx + A.dbound;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < A.dbound; j += (uint64_t)gridDim.x * blockDim.x) {
+    if (seg[j] == ~0ull) continue;
+    const uint32_t i = idx[j], g = Q.pos[j] + Q.head[j] - 1;
+    if (Q.head[j]) {
+      StateKey k;
+      k.seg = seg[j];
+      k.key = A.key[i];
+      Q.out_key[g] = k;
+      Q.out_start[g] = A.start[i];
+    }
+    if (j + 1 == A.dbound || Q.head[j + 1] || seg[j + 1] == ~0ull) Q.out_end[g] = A.start[i] + A.dur[i];
+  }
 }
 
 // Per output column: which state arrays feed it.

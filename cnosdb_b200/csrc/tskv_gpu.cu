@@ -321,6 +321,11 @@ struct tskv_scan {
   async_ptr<uint8_t> d_state_tmp;
   size_t state_tmp_bytes = 0;
   StateArgs st{};
+  // state periods (TSKV_STATE_PERIODS; k_period_*): only when an operand has the flag (per.agg_mask != 0)
+  async_ptr<uint64_t> d_period_u64;     // pkey [2 * dbound] | out_start [dbound] | out_end [dbound] | the records' starts [dbound]
+  async_ptr<uint32_t> d_period_u32;     // idx [2 * dbound] | head [dbound + 1] | pos [dbound + 1] | off [n_segs + 1]
+  async_ptr<StateKey> d_period_keys;    // out_key [dbound]
+  PeriodArgs per{};
 };
 
 namespace {
@@ -507,6 +512,7 @@ OperandQuery plan_operand_query(const tskv_query *q) {
     pq.cols[sc.qcol].agg_mask |= TSKV_AGG_COUNT;
     sc.column_id = op.column_id;
     sc.phys_type = op.phys_type;
+    sc.periods = op.agg_mask == TSKV_STATE_PERIODS;
     pq.states.push_back(sc);
   }
   pq.q.columns = pq.cols.data();
@@ -1068,8 +1074,8 @@ tskv_status validate_query(tskv_ctx *ctx, const tskv_pages *pages, const tskv_qu
   }
   for (uint64_t k = query_state_col0(q); k < query_state_col0(q) + n_state; k++) {
     const tskv_agg_column &op = q->columns[k];
-    if (op.agg_mask != 0 || (op.phys_type != TSKV_PT_I64 && op.phys_type != TSKV_PT_U64)) {
-      ctx->set_error("invalid state agg operand: an I64 / U64 column with agg_mask 0");
+    if ((op.agg_mask != 0 && op.agg_mask != TSKV_STATE_PERIODS) || (op.phys_type != TSKV_PT_I64 && op.phys_type != TSKV_PT_U64)) {
+      ctx->set_error("invalid state agg operand: an I64 / U64 column with agg_mask 0 or TSKV_STATE_PERIODS");
       return TSKV_ERR_INVALID_ARG;
     }
     for (uint64_t c = 0; c < k; c++)
@@ -1782,6 +1788,16 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
                                                               (int64_t *)nullptr, (int32_t *)nullptr, StateSum{}, (int)D, st);
     if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, t[5], (uint32_t *)nullptr, (int64_t)(A.n_segs + 1), st);
     s->state_tmp_bytes = std::max<size_t>(*std::max_element(t, t + 6), 1);
+    PeriodArgs &Q = s->per;
+    Q.agg_mask = 0;
+    for (uint32_t g = 0; g < s->n_states; g++) Q.agg_mask |= (uint32_t)lay.states[g].periods << g;
+    if (Q.agg_mask) {  // the period pass: the start time sort and the heads' exclusive sum (its other sorts are sized above)
+      size_t p[2] = {0, 0};
+      if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, p[0], (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                                                 (uint32_t *)nullptr, (int)D, 0, s->state_time_sort_bits, st);
+      if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, p[1], (uint32_t *)nullptr, (int64_t)(D + 1), st);
+      s->state_tmp_bytes = std::max(s->state_tmp_bytes, std::max(p[0], p[1]));
+    }
     if (e == cudaSuccess) e = upload(s->d_states, lay.states.data(), lay.states.size(), st);
     if (e == cudaSuccess) e = stream_alloc(s->d_state_u64, (size_t)(7 * D + 5 * B + A.n_segs), st);
     if (e == cudaSuccess) e = stream_alloc(s->d_state_keys, (size_t)(2 * D), st);
@@ -1808,6 +1824,25 @@ tskv_status alloc_scan(tskv_ctx *ctx, const tskv_pages *pages, const tskv_query 
     A.n_runs = reinterpret_cast<int32_t *>(A.n_dur + 2);
     // (a scan that has not run yet holds empty maps: tskvgpu_scan_state_durations reads the offsets)
     if (e == cudaSuccess) e = cudaMemsetAsync(A.off, 0, (A.n_segs + 1) * sizeof(uint32_t), st);
+    A.start = nullptr;
+    if (Q.agg_mask) {
+      if (e == cudaSuccess) e = stream_alloc(s->d_period_u64, (size_t)(5 * D), st);
+      if (e == cudaSuccess) e = stream_alloc(s->d_period_u32, (size_t)(4 * D + 2 + A.n_segs + 1), st);
+      if (e == cudaSuccess) e = stream_alloc(s->d_period_keys, (size_t)D, st);
+      uint64_t *pw = s->d_period_u64.get();
+      Q.pkey = pw;
+      Q.out_start = reinterpret_cast<int64_t *>(pw + 2 * D);
+      Q.out_end = reinterpret_cast<int64_t *>(pw + 3 * D);
+      A.start = reinterpret_cast<int64_t *>(pw + 4 * D);
+      uint32_t *pu = s->d_period_u32.get();
+      Q.idx = pu;
+      Q.head = pu + 2 * D;
+      Q.pos = pu + 3 * D + 1;
+      Q.off = pu + 4 * D + 2;
+      Q.out_key = s->d_period_keys.get();
+      // (a scan that has not run yet holds empty lists: tskvgpu_scan_state_periods reads the offsets)
+      if (e == cudaSuccess) e = cudaMemsetAsync(Q.off, 0, (A.n_segs + 1) * sizeof(uint32_t), st);
+    }
     *h2d += lay.states.size() * sizeof(StateCol);
   }
   if (e == cudaSuccess) e = stream_alloc(s->d_aux, AUX_WORDS, st);
@@ -3286,6 +3321,30 @@ static tskv_status enqueue_scan(tskv_ctx *ctx, tskv_scan *s, bool capturing = fa
     CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_state_tmp.get(), tmp, bk + 3 * B, bk + 4 * B, bi + B, bi + 2 * B, (int)B, 0,
                                                 s->state_slot_sort_bits, stream));
     k_state_stitch<<<bx, 256, 0, stream>>>(A);
+    if (s->per.agg_mask) {  // periods, before the duration sorts overwrite the records' segments
+      // by start time, then (stably) by state key and by segment: keys [start keys, then state keys, then segments |
+      // sorted], positions [identity | time order], then [(time, key) order | (segment, key, start) order]
+      const PeriodArgs &Q = s->per;
+      CU_TRY(ctx, cudaMemsetAsync(Q.off, 0, (A.n_segs + 1) * sizeof(uint32_t), stream));
+      k_period_keys<<<dx, 256, 0, stream>>>(A, Q);
+      tmp = s->state_tmp_bytes;
+      CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_state_tmp.get(), tmp, Q.pkey, Q.pkey + D, Q.idx, Q.idx + D, (int)D, 0,
+                                                  s->state_time_sort_bits, stream));
+      k_state_gather<<<dx, 256, 0, stream>>>(A.key, Q.idx + D, D, Q.pkey);
+      tmp = s->state_tmp_bytes;
+      CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_state_tmp.get(), tmp, Q.pkey, Q.pkey + D, Q.idx + D, Q.idx, (int)D, 0, 64, stream));
+      k_period_segs<<<dx, 256, 0, stream>>>(A, Q);
+      tmp = s->state_tmp_bytes;
+      CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(s->d_state_tmp.get(), tmp, Q.pkey, Q.pkey + D, Q.idx, Q.idx + D, (int)D, 0,
+                                                  s->state_seg_bits, stream));
+      k_period_mark<<<dx, 256, 0, stream>>>(A, Q);
+      tmp = s->state_tmp_bytes;
+      CU_TRY(ctx, cub::DeviceScan::ExclusiveSum(s->d_state_tmp.get(), tmp, Q.head, Q.pos, (int64_t)(D + 1), stream));
+      k_period_write<<<dx, 256, 0, stream>>>(A, Q);
+      tmp = s->state_tmp_bytes;
+      CU_TRY(ctx, cub::DeviceScan::ExclusiveSum(s->d_state_tmp.get(), tmp, Q.off, (int64_t)(A.n_segs + 1), stream));
+      launches += 10;  // (a sort or scan counts as one launch)
+    }
     // duration records by state key, then (stably) by segment: segments [records, then sorted | in key order], positions
     // [identity, then final order | key order]; then the keys and durations in (segment, key) order for the reduce
     tmp = s->state_tmp_bytes;
@@ -3480,6 +3539,41 @@ tskv_status tskvgpu_scan_state_durations(tskv_ctx *ctx, tskv_scan *s, uint32_t k
     }
   }
   if (durations) CU_TRY(ctx, cudaMemcpy(durations, A.sum + base, n * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  return TSKV_OK;
+}
+
+tskv_status tskvgpu_scan_state_periods(tskv_ctx *ctx, tskv_scan *s, uint32_t k, uint64_t *offsets, uint64_t *states, uint8_t *state_valid,
+                                       int64_t *starts, int64_t *ends, uint64_t *n_periods) {
+  if (!ctx || !s || !n_periods) return TSKV_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  ctx->set_error("");
+  if (k >= s->n_states || !((s->per.agg_mask >> k) & 1)) {
+    ctx->set_error("scan_state_periods: k is not a state agg of the scan with TSKV_STATE_PERIODS");
+    return TSKV_ERR_INVALID_ARG;
+  }
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  const PeriodArgs &Q = s->per;
+  const uint64_t n_cells = s->st.n_cells;
+  std::vector<uint32_t> off(n_cells + 1);
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream.get()));
+  CU_TRY(ctx, cudaMemcpy(off.data(), Q.off + (uint64_t)k * n_cells, off.size() * 4, cudaMemcpyDeviceToHost));
+  const uint64_t base = off[0], n = off[n_cells] - base;
+  *n_periods = n;
+  if (offsets)
+    for (uint64_t c = 0; c <= n_cells; c++) offsets[c] = off[c] - base;
+  if (!n) return TSKV_OK;
+  if (states || state_valid) {
+    std::vector<StateKey> keys(n);
+    CU_TRY(ctx, cudaMemcpy(keys.data(), Q.out_key + base, n * sizeof(StateKey), cudaMemcpyDeviceToHost));
+    const bool i64 = s->h_states[k].phys_type == TSKV_PT_I64;
+    for (uint64_t i = 0; i < n; i++) {
+      const bool valid = keys[i].seg & 1;
+      if (state_valid) state_valid[i] = valid;
+      if (states) states[i] = !valid ? 0 : i64 ? keys[i].key ^ 0x8000000000000000ull : keys[i].key;
+    }
+  }
+  if (starts) CU_TRY(ctx, cudaMemcpy(starts, Q.out_start + base, n * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  if (ends) CU_TRY(ctx, cudaMemcpy(ends, Q.out_end + base, n * sizeof(int64_t), cudaMemcpyDeviceToHost));
   return TSKV_OK;
 }
 

@@ -219,7 +219,7 @@ class TskvError(RuntimeError):
 
 
 # the aggregates without a mask bit: each makes its column an operand of its own kind
-PSEUDO_AGGS = ("median", "increase", "mode", "count_distinct", "gauge_agg", "compact_state_agg")
+PSEUDO_AGGS = ("median", "increase", "mode", "count_distinct", "gauge_agg", "compact_state_agg", "state_agg")
 # the outputs of one gauge_agg(time, x): the points, then (time, value) of its first, second, penultimate and last point
 GAUGE_OUTS = ("n", "first_t", "first_v", "second_t", "second_v", "penultimate_t", "penultimate_v", "last_t", "last_v")
 # the accessors of CnosDB's GaugeData (gauge/mod.rs) that gauge_stat derives from the nine outputs
@@ -263,10 +263,44 @@ def gauge_stat(name, n, first_t, first_v, second_t, second_v, penultimate_t, pen
     raise ValueError("unknown gauge accessor %r (one of %s)" % (name, ", ".join(GAUGE_STATS)))
 
 
-def duration_in(state_map, state):
-    """duration_in(compact_state_agg(time, x), state) without a start time: the map's duration of `state` (None: the
-    NULL state), 0 when the map has no entry for it (StateAggData::duration_in)."""
-    return state_map.get(None if state is None else int(state), 0)
+class CompactAggError(ValueError):
+    """state_at, or duration_in with a start time, over an aggregate with a duration map and no periods: the reference's
+    StateAggData::try_from takes it for a compact_state_agg and refuses it ("... doesn't support compact_agg"). A
+    state_agg over a cell of one row is one."""
+
+
+def _refuse_compact(state_map, periods, what):
+    if not periods and state_map:
+        raise CompactAggError("%s doesn't support compact_agg" % what)
+
+
+def duration_in(state_map, state, start=None, end=None, periods=None):
+    """duration_in(agg, state[, start[, interval]]) of one cell (StateAggData::duration_in). Without a start time: the
+    map's duration of `state` (None: the NULL state), 0 when the map has no entry for it. With one: the lengths of the
+    periods of `state` (`periods`, the cell's {state: [(start, end)]} from ScanResult.state_periods) that overlap
+    [start, end), each clipped to it; end None (a NULL interval) is +inf, and end = start + interval otherwise. Raises
+    CompactAggError where the reference does: the cell has map entries and no period."""
+    key = None if state is None else int(state)
+    if start is None:
+        return state_map.get(key, 0)
+    _refuse_compact(state_map, periods, "duration_in(state_agg, state, start_time%s)" % ("" if end is None else ", interval"))
+    total = 0
+    for a, b in periods.get(key, ()):
+        lo, hi = max(a, start), b if end is None else min(b, end)
+        if hi > lo:
+            total += hi - lo
+    return total
+
+
+def state_at(periods, ts, state_map):
+    """state_at(state_agg(time, x), ts) of one cell (StateAggData::state_at): the state of the period [start, end) that
+    holds ts, None when none does (or when it is the NULL state's). `periods` and `state_map` as for duration_in; raises
+    CompactAggError where the reference does, with the reference's message (which names duration_in)."""
+    _refuse_compact(state_map, periods, "duration_in(state_agg, state, start_time, interval)")  # (the reference's text)
+    for s, ps in periods.items():
+        if any(a <= ts < b for a, b in ps):
+            return s
+    return None
 
 
 class PushedAggregate:
@@ -276,7 +310,9 @@ class PushedAggregate:
     the medians' operands; "mode" (mode(x)) a mode operand, after the increases' operands; "count_distinct"
     (COUNT(DISTINCT x)) a distinct operand, after the modes' operands; "gauge_agg" (gauge_agg(time, x)) a gauge
     operand, after the distincts' operands; and "compact_state_agg" (compact_state_agg(time, x)) a state agg operand,
-    after the gauges' operands."""
+    after the gauges' operands. "state_agg" (state_agg(time, x), for state_at and duration_in with a start time) makes it
+    a state agg operand with agg_mask TSKV_STATE_PERIODS, which computes the periods as well as the map; asked together
+    with "compact_state_agg", both share that one operand."""
 
     def __init__(self, column_id, phys_type, aggs):
         self.column_id = int(column_id)
@@ -287,6 +323,7 @@ class PushedAggregate:
         self.count_distinct = False
         self.gauge_agg = False
         self.compact_state_agg = False
+        self.state_agg = False
         if isinstance(aggs, int):
             self.agg_mask = aggs
         else:
@@ -295,7 +332,7 @@ class PushedAggregate:
                 if a == "median":
                     self.median = True
                     continue
-                if a in ("increase", "mode", "count_distinct", "gauge_agg", "compact_state_agg"):
+                if a in ("increase", "mode", "count_distinct", "gauge_agg", "compact_state_agg", "state_agg"):
                     setattr(self, a, True)
                     continue
                 # var* / stddev* ask the scan for COUNT | M2; ScanResult.column derives them
@@ -354,6 +391,9 @@ class QueryOption:
             cols[i].column_id, cols[i].phys_type, cols[i].agg_mask = c.column_id, c.phys_type, c.agg_mask
         for i, (cid, pt) in enumerate(ops):  # the pairs', medians', increases', modes', distincts', gauges' and state aggs' operands follow
             cols[len(proj) + i].column_id, cols[len(proj) + i].phys_type = cid, pt
+        for k, periods in enumerate(self.state_periods()):
+            if periods:
+                cols[len(proj) + len(ops) - len(states) + k].agg_mask = cabi.TSKV_STATE_PERIODS
         q.columns = cols
         q.n_columns = len(proj)
         q.n_pairs = len(self.pairs)
@@ -371,13 +411,21 @@ class QueryOption:
         return q
 
     def state_aggs(self):
-        """(column_id, phys_type) of the compact_state_agg operands, in the order of their outputs and of k in
-        PreparedScan.state_durations(k)."""
-        return [(c.column_id, c.phys_type) for c in self.columns if getattr(c, "compact_state_agg", False)]
+        """(column_id, phys_type) of the compact_state_agg and state_agg operands, in the order of their outputs and of k
+        in PreparedScan.state_durations(k) / state_periods(k)."""
+        return [(c.column_id, c.phys_type) for c in self.columns if self._state(c)]
+
+    def state_periods(self):
+        """Per state agg operand (as state_aggs()): whether it computes its periods (state_agg)."""
+        return [bool(getattr(c, "state_agg", False)) for c in self.columns if self._state(c)]
+
+    @staticmethod
+    def _state(c):
+        return getattr(c, "compact_state_agg", False) or getattr(c, "state_agg", False)
 
     def projected(self):
-        """The columns with a projected entry (an aggregate other than median, increase, mode, count_distinct, gauge_agg
-        and compact_state_agg)."""
+        """The columns with a projected entry (an aggregate other than median, increase, mode, count_distinct, gauge_agg,
+        compact_state_agg and state_agg)."""
         return [c for c in self.columns if c.agg_mask or not any(getattr(c, a, False) for a in PSEUDO_AGGS)]
 
     def output_names(self):
@@ -406,6 +454,8 @@ class ScanResult:
         # compact_state_agg: column_id -> (offsets, states, state_valid, durations), PreparedScan.state_durations's CSR
         # (set by PreparedScan.finalize; the one-shot C calls return only the entry counts)
         self.state_csr = {}
+        # state_agg: column_id -> (offsets, states, state_valid, starts, ends), PreparedScan.state_periods's CSR
+        self.period_csr = {}
 
     def pair(self, k, name):
         """(values f64 / u64 for n, validity) of column pair k, shaped [n_groups, n_buckets]: one of PAIR_AGGS (covar,
@@ -441,6 +491,20 @@ class ScanResult:
         maps = [{(int(states[i]) if valid[i] else None): int(durs[i]) for i in range(off[c], off[c + 1])}
                 for c in range(len(off) - 1)]
         return [maps[g * self.n_buckets:(g + 1) * self.n_buckets] for g in range(self.n_groups)]
+
+    def state_periods(self, column_id):
+        """The state_agg periods of column_id, one {state: [(start, end), ...]} dict per cell, shaped
+        [n_groups][n_buckets] (keys as in state_maps, the NULL state first, then the states in order; each state's
+        maximal periods by start time, in the time column's unit). state_at and duration_in with a start read one, next
+        to the cell's state_maps entry."""
+        off, states, valid, starts, ends = self.period_csr[column_id]
+        cells = []
+        for c in range(len(off) - 1):
+            d = {}
+            for i in range(off[c], off[c + 1]):
+                d.setdefault(int(states[i]) if valid[i] else None, []).append((int(starts[i]), int(ends[i])))
+            cells.append(d)
+        return [cells[g * self.n_buckets:(g + 1) * self.n_buckets] for g in range(self.n_groups)]
 
     def column(self, column_id, agg):
         """(typed values, validity) of one output column, shaped [n_groups, n_buckets]. agg may also name one of STAT_AGGS
@@ -564,6 +628,24 @@ class PreparedScan:
                                                             valid.ctypes.data, durs.ctypes.data, C.byref(n)))
         return off, states, valid.astype(bool), durs
 
+    def state_periods(self, k):
+        """The periods of state agg k (a state_agg operand) after run / sync, tskvgpu_scan_state_periods's CSR: (offsets
+        u64 [n_cells + 1], states [n_periods] in the operand's type (0 for the NULL state), state_valid bool, starts i64,
+        ends i64); cell c owns periods offsets[c] .. offsets[c + 1], the NULL state first, then the states in order, each
+        state's periods by start."""
+        lib, ctx = self.engine.lib, self.engine.ctx
+        n = C.c_uint64(0)
+        self.engine._check(lib.tskvgpu_scan_state_periods(ctx, self.handle, int(k), None, None, None, None, None, C.byref(n)))
+        pt = self.query.state_aggs()[k][1] if k < len(self.query.state_aggs()) else TSKV_PT_I64
+        off = np.zeros(int(self.layout.n_cells) + 1, np.uint64)
+        states = np.zeros(n.value, np.int64 if pt == TSKV_PT_I64 else np.uint64)
+        valid = np.zeros(n.value, np.uint8)
+        starts = np.zeros(n.value, np.int64)
+        ends = np.zeros(n.value, np.int64)
+        self.engine._check(lib.tskvgpu_scan_state_periods(ctx, self.handle, int(k), off.ctypes.data, states.ctypes.data,
+                                                          valid.ctypes.data, starts.ctypes.data, ends.ctypes.data, C.byref(n)))
+        return off, states, valid.astype(bool), starts, ends
+
     def exchange_view(self):
         """(device pointer, length in 8-byte words) of the region a multi-GPU run all-gathers."""
         a, b = C.c_uint64(0), C.c_uint64(0)
@@ -591,8 +673,10 @@ class PreparedScan:
         self.engine._check(self.engine.lib.tskvgpu_scan_finalize(
             self.engine.ctx, self.handle, values.ctypes.data, bitmaps.ctypes.data))
         res = ScanResult(self.query, L, values, bitmaps)
-        for k, (cid, _) in enumerate(self.query.state_aggs()):
+        for k, ((cid, _), periods) in enumerate(zip(self.query.state_aggs(), self.query.state_periods())):
             res.state_csr[cid] = self.state_durations(k)
+            if periods:
+                res.period_csr[cid] = self.state_periods(k)
         return res
 
     def finalize_device(self):
@@ -786,7 +870,8 @@ class Engine:
         origin and first_bucket_start 0; calendar_edges makes them for date_trunc). Not with slide.
         labels: with edges, labels[b] < query.n_buckets is the output bucket of edge bucket b (one per edge bucket;
         calendar_parts makes them for date_part). query.n_buckets is then the number of output buckets.
-        A query with compact_state_agg runs prepare, run and finalize, so that its result holds the maps too."""
+        A query with compact_state_agg or state_agg runs prepare, run and finalize, so that its result holds the maps
+        (and the periods) too."""
         if query.state_aggs():
             scan = self.prepare(pages, query, slide, group_ids, n_groups, edges, labels)
             try:

@@ -337,7 +337,8 @@ typedef struct tskv_query {
  * plus min(num_values, the grid buckets the group's time span can touch; num_values for a group whose bounds have
  * min > max) duration records and as many boundary records, plus two duration records and one boundary record per merge
  * row; about 90 bytes per record. Refused before any launch:
- * TSKV_ERR_INVALID_ARG for an operand with a non-zero agg_mask or an F64 / BOOL / TIME / unknown type, an operand id
+ * TSKV_ERR_INVALID_ARG for an operand with an agg_mask other than 0 and TSKV_STATE_PERIODS (below) or an F64 / BOOL /
+ * TIME / unknown type, an operand id
  * projected with another type, or more than 126 columns; TSKV_ERR_UNSUPPORTED for a cell that could hold rows of two
  * selected series (as for increases), sliding windows (slide != width), tskvgpu_scan_prepare_labels,
  * TSKV_QUERY_MULTI_RANK (a map does not fit the fixed exchange region), a selected column group that overlaps the time
@@ -349,6 +350,21 @@ typedef struct tskv_query {
 #define TSKV_MAX_STATE_AGGS 7
 #define TSKV_QUERY_STATE_AGGS(n) (((uint32_t)(n) & 0x7u) << 5)
 #define TSKV_QUERY_N_STATE_AGGS(flags) (((uint32_t)(flags) >> 5) & 0x7u)
+/* State periods: state_agg(time, x)'s periods (CnosDB's StatePeriods), for state_at(agg, ts) and duration_in(agg, state,
+ * start[, interval]). A state agg operand whose agg_mask is TSKV_STATE_PERIODS (instead of 0) computes its periods as
+ * well as its duration map; any other non-zero mask of a state agg operand, and this value on any other operand, is
+ * TSKV_ERR_INVALID_ARG. Every other rule of the state aggs applies unchanged, and the output is the same (one u64 per
+ * cell: the map's entries). The reference lists one period [t, t') of state s per pair of consecutive points (t, s),
+ * (t', s'); the scan returns maximal periods instead: periods of one state that touch end to end are joined into one,
+ * and periods of length 0 are dropped, so that the output follows the state changes, not the rows. state_at and
+ * duration_in with a start time give the same answers on both (clipped lengths add up exactly, and an empty period
+ * neither holds a time nor adds a length). A query with the flag adds to the state agg pass, after the stitch: every
+ * duration record carries its start time; a stable radix sort by start time and the two sorts by state key and by
+ * segment order the records by (state agg, cell, NULL flag, state, start); records of length 0 and of operands without
+ * the flag are dropped, a record whose predecessor has the same segment and state and ends where it starts joins it,
+ * and an exclusive sum gives each period its place. Buffers, sized at prepare from the duration record bound: about 80
+ * bytes more per record. tskvgpu_scan_state_periods (below) returns the periods. */
+#define TSKV_STATE_PERIODS (1u << 7)
 
 /* Result layout. Outputs are dense: for output column j (query columns in order, and inside a
  * column the set agg bits in ascending bit order) and cell c = group * n_buckets + bucket:
@@ -553,6 +569,16 @@ tskv_status tskvgpu_scan_work_list(tskv_ctx *ctx, tskv_scan *scan, uint32_t *n_b
  * call with null arrays first to size them. A scan that has not run yet has empty maps (*n_entries 0). */
 tskv_status tskvgpu_scan_state_durations(tskv_ctx *ctx, tskv_scan *scan, uint32_t k, uint64_t *offsets, uint64_t *states,
                                          uint8_t *state_valid, int64_t *durations, uint64_t *n_entries);
+/* The periods of state agg k after scan_run / scan_sync, in CSR form in host buffers; k must be a state agg whose operand
+ * has agg_mask TSKV_STATE_PERIODS (TSKV_ERR_INVALID_ARG otherwise, and for k >= TSKV_QUERY_N_STATE_AGGS). Cell c owns
+ * periods [offsets[c], offsets[c + 1]) (offsets [n_cells + 1]); period i is [starts[i], ends[i]) (i64, the time column's
+ * unit) of the state states[i] (the i64 / u64 bit pattern; 0 for the NULL state) with state_valid[i] (0: the NULL state,
+ * 1: a value). Within a cell the NULL state comes first, then the states in the type's order, and each state's periods by
+ * start time. The periods are maximal: ends[i] < starts[i + 1] between two periods of one state, and starts[i] < ends[i]
+ * (see TSKV_STATE_PERIODS). Each array may be null; *n_periods (= offsets[n_cells]) is always written: call with null
+ * arrays first to size them. A scan that has not run yet has empty lists (*n_periods 0). */
+tskv_status tskvgpu_scan_state_periods(tskv_ctx *ctx, tskv_scan *scan, uint32_t k, uint64_t *offsets, uint64_t *states,
+                                       uint8_t *state_valid, int64_t *starts, int64_t *ends, uint64_t *n_periods);
 /* Alternative with a single collective: all-gather the exchange region (device pointer + length in
  * 8-byte words) of every rank into `gathered` (rank-major, n_ranks * words) and merge locally. */
 tskv_status tskvgpu_scan_exchange_view(tskv_ctx *ctx, tskv_scan *scan, uint64_t *out_dptr, uint64_t *out_words);

@@ -29,7 +29,7 @@ pub use sys::{tskv_query_increases, tskv_query_n_increases, TSKV_MAX_INCREASES};
 pub use sys::{tskv_query_distincts, tskv_query_modes, tskv_query_n_distincts, tskv_query_n_modes};
 pub use sys::{TSKV_MAX_DISTINCTS, TSKV_MAX_MODES, TSKV_MAX_SORTED_ROWS};
 pub use sys::{tskv_query_gauges, tskv_query_n_gauges, TSKV_MAX_GAUGES};
-pub use sys::{tskv_query_n_state_aggs, tskv_query_state_aggs, TSKV_MAX_STATE_AGGS};
+pub use sys::{tskv_query_n_state_aggs, tskv_query_state_aggs, TSKV_MAX_STATE_AGGS, TSKV_STATE_PERIODS};
 
 /// What a failed call reports; maps onto `TskvError` as INTEGRATION.md section 2 lists.
 #[derive(Debug, Clone)]
@@ -134,8 +134,13 @@ impl GpuEngine {
     }
 
     /// `scan_aggregate` for a query with state aggs (`Query::n_state_aggs`): the dense result (each state agg's output is
-    /// the cell's number of map entries) and every state agg's maps, which the one-shot call does not return.
-    pub fn scan_aggregate_states(&self, pages: &PageSet<'_>, q: &Query) -> GpuResult<(AggregateResult, Vec<StateDurations>)> {
+    /// the cell's number of map entries), every state agg's maps, which the one-shot call does not return, and the
+    /// periods of every state agg whose operand has agg_mask TSKV_STATE_PERIODS (None for the others).
+    pub fn scan_aggregate_states(
+        &self,
+        pages: &PageSet<'_>,
+        q: &Query,
+    ) -> GpuResult<(AggregateResult, Vec<StateDurations>, Vec<Option<StatePeriods>>)> {
         let raw = q.as_raw()?;
         let layout = self.output_layout(pages, q, &raw)?;
         let mut scan = std::ptr::null_mut();
@@ -151,17 +156,46 @@ impl GpuEngine {
         let mut values = vec![0u64; (layout.n_out * layout.n_cells) as usize];
         let mut validity = vec![0u8; layout.validity_bytes as usize];
         let mut maps = Vec::with_capacity(q.n_state_aggs as usize);
+        let mut periods = Vec::with_capacity(q.n_state_aggs as usize);
+        let ops = &q.columns[q.columns.len() - q.n_state_aggs as usize..];
         let mut run = || -> GpuResult<()> {
             self.check(unsafe { sys::tskvgpu_scan_run(self.ctx, scan) })?;
             self.check(unsafe { sys::tskvgpu_scan_finalize(self.ctx, scan, values.as_mut_ptr(), validity.as_mut_ptr()) })?;
             for k in 0..q.n_state_aggs {
                 maps.push(self.state_durations(scan, k, layout.n_cells)?);
+                periods.push(if ops[k as usize].agg_mask as u32 == sys::TSKV_STATE_PERIODS {
+                    Some(self.state_periods(scan, k, layout.n_cells)?)
+                } else {
+                    None
+                });
             }
             Ok(())
         };
         let r = run();
         unsafe { sys::tskvgpu_scan_destroy(self.ctx, scan) };
-        r.map(|_| (AggregateResult { layout, values, validity }, maps))
+        r.map(|_| (AggregateResult { layout, values, validity }, maps, periods))
+    }
+
+    /// The periods of state agg k (an operand with TSKV_STATE_PERIODS) of a scan that has run: sized by a first call
+    /// with null arrays, then filled.
+    fn state_periods(&self, scan: *mut sys::tskv_scan, k: u32, n_cells: u64) -> GpuResult<StatePeriods> {
+        let mut n = 0u64;
+        self.check(unsafe {
+            sys::tskvgpu_scan_state_periods(self.ctx, scan, k, std::ptr::null_mut(), std::ptr::null_mut(), std::ptr::null_mut(),
+                                            std::ptr::null_mut(), std::ptr::null_mut(), &mut n)
+        })?;
+        let mut p = StatePeriods {
+            offsets: vec![0; n_cells as usize + 1],
+            states: vec![0; n as usize],
+            state_valid: vec![0; n as usize],
+            starts: vec![0; n as usize],
+            ends: vec![0; n as usize],
+        };
+        self.check(unsafe {
+            sys::tskvgpu_scan_state_periods(self.ctx, scan, k, p.offsets.as_mut_ptr(), p.states.as_mut_ptr(), p.state_valid.as_mut_ptr(),
+                                            p.starts.as_mut_ptr(), p.ends.as_mut_ptr(), &mut n)
+        })?;
+        Ok(p)
     }
 
     /// The maps of state agg k of a scan that has run: sized by a first call with null arrays, then filled.
@@ -320,7 +354,8 @@ pub struct Query {
     /// compact_state_agg(time, x): the last `n_state_aggs` entries of `columns` are the operands (I64 / U64, at most
     /// TSKV_MAX_STATE_AGGS); each adds 1 output after the gauges' (the cell's map entries), and
     /// `GpuEngine::scan_aggregate_states` returns the maps, from which the shim builds the DurationStates list column
-    /// (INTEGRATION.md section 6)
+    /// (INTEGRATION.md section 6); an operand with agg_mask TSKV_STATE_PERIODS (state_agg(time, x)) returns its
+    /// periods too
     pub n_state_aggs: u32,
 }
 
@@ -333,6 +368,19 @@ pub struct StateDurations {
     pub states: Vec<u64>,
     pub state_valid: Vec<u8>,
     pub durations: Vec<i64>,
+}
+
+/// One state agg's periods in CSR form (tskvgpu_scan_state_periods): cell c owns periods `offsets[c]..offsets[c + 1]`,
+/// the NULL state (`state_valid` 0) first, then the states (i64 / u64 bit patterns) in the type's order, each state's
+/// maximal periods `[starts[i], ends[i])` by start, in the time column's unit. The shim builds state_agg's
+/// `state_periods` list column from them (INTEGRATION.md section 6).
+#[derive(Clone, Debug, Default)]
+pub struct StatePeriods {
+    pub offsets: Vec<u64>,
+    pub states: Vec<u64>,
+    pub state_valid: Vec<u8>,
+    pub starts: Vec<i64>,
+    pub ends: Vec<i64>,
 }
 
 impl Query {

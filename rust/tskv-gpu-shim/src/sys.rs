@@ -102,6 +102,9 @@ pub const fn tskv_query_state_aggs(n: u32) -> u32 {
 pub const fn tskv_query_n_state_aggs(flags: u32) -> u32 {
     (flags >> 5) & 0x7
 }
+/// A state agg operand's agg_mask (instead of 0): the agg computes state_agg(time, x)'s periods as well as its map, and
+/// tskvgpu_scan_state_periods returns them.
+pub const TSKV_STATE_PERIODS: u32 = 1 << 7;
 
 pub const TSKV_UPLOAD_VERIFY_CRC: u32 = 1;
 pub const TSKV_UPLOAD_HOST_RESIDENT: u32 = 2;
@@ -471,6 +474,17 @@ extern "C" {
         state_valid: *mut u8,
         durations: *mut i64,
         n_entries: *mut u64,
+    ) -> tskv_status;
+    pub fn tskvgpu_scan_state_periods(
+        ctx: *mut tskv_ctx,
+        scan: *mut tskv_scan,
+        k: u32,
+        offsets: *mut u64,
+        states: *mut u64,
+        state_valid: *mut u8,
+        starts: *mut i64,
+        ends: *mut i64,
+        n_periods: *mut u64,
     ) -> tskv_status;
     pub fn tskvgpu_scan_exchange_view(
         ctx: *mut tskv_ctx,

@@ -1,5 +1,7 @@
-"""The cost of compact_state_agg(time, x) in alternating runs on one GPU, MEAN only against MEAN plus the state agg of
-the i64 column (column 1), ms per step (one enqueue of the prepared scan followed by its sync):
+"""The cost of compact_state_agg(time, x) and of state_agg(time, x) in alternating runs on one GPU: MEAN only
+(`mean`), MEAN plus the i64 column's (column 1) compact state agg (`state_i64`: its duration map) and MEAN plus its state
+agg (`periods_i64`: the map and the periods, TSKV_STATE_PERIODS), ms per step (one enqueue of the prepared scan followed
+by its sync):
 
   c4/one_series     C4 (bench.py), its first selected series with an i64 column alone, unbucketed (a state agg cell
                     holds one series)
@@ -14,9 +16,9 @@ per row. The run-structured set makes about one per 100 rows.
   python tools/bench_state_agg.py [--series N] [--run-series S] [--run-rows R] [--steps K] [--warmup W] [--rounds R] [--out DIR]
 
 Prints one JSON line: ms per step of each variant (median, min, max over the rounds), the card's name and power limit,
-the counters, the map entries and selected rows of each state agg variant, and whether the MEAN outputs of the state
-agg variants equal the `mean` variant's (bit for bit; f64 within 1e-12 relative). Exits non-zero otherwise. Writes the
-JSON to DIR/bench_state_agg.json."""
+the counters, the map entries, periods and selected rows of each state agg variant, and whether the MEAN outputs of the
+state agg variants equal the `mean` variant's (bit for bit; f64 within 1e-12 relative) and the periods variant's map
+entries the compact variant's. Exits non-zero otherwise. Writes the JSON to DIR/bench_state_agg.json."""
 import argparse
 import json
 import os
@@ -37,8 +39,11 @@ from cnosdb_b200.engine import Engine, PushedAggregate, QueryOption  # noqa: E40
 MIN = 60_000_000_000
 
 
-def c4_variant(q, state, grid, with_i64):
-    cols = [PushedAggregate(c.column_id, c.phys_type, ["mean"] + (["compact_state_agg"] if state and c.column_id == 1 else []))
+VARIANTS = {"mean": [], "state_i64": ["compact_state_agg"], "periods_i64": ["state_agg"]}
+
+
+def c4_variant(q, variant, grid, with_i64):
+    cols = [PushedAggregate(c.column_id, c.phys_type, ["mean"] + (VARIANTS[variant] if c.column_id == 1 else []))
             for c in q.columns]
     kw = dict(series_ids=q.series_ids, time_ranges=q.time_ranges, origin=q.origin, width=q.width,
               first_bucket_start=q.first_bucket_start, n_buckets=q.n_buckets,
@@ -91,12 +96,12 @@ def main():
     rp = engine.upload_pages(ra, rd)
     queries = {}
     for grid in ("one_series", "series"):
-        for name, state in (("mean", False), ("state_i64", True)):
-            queries["c4/%s/%s" % (grid, name)] = (c4, c4_variant(base, state, grid, with_i64))
+        for name in VARIANTS:
+            queries["c4/%s/%s" % (grid, name)] = (c4, c4_variant(base, name, grid, with_i64))
     fbs = (r_lo // MIN) * MIN
     nb = (r_hi - fbs) // MIN + 1
-    for name, state in (("mean", False), ("state_i64", True)):
-        cols = [PushedAggregate(1, cabi.TSKV_PT_I64, ["mean"] + (["compact_state_agg"] if state else [])),
+    for name in VARIANTS:
+        cols = [PushedAggregate(1, cabi.TSKV_PT_I64, ["mean"] + VARIANTS[name]),
                 PushedAggregate(2, cabi.TSKV_PT_F64, ["mean"])]
         queries["runs/series/" + name] = (rp, QueryOption(cols, width=MIN, first_bucket_start=fbs, n_buckets=nb, group_by_series=True))
     scans = {n: engine.prepare(p, q) for n, (p, q) in queries.items()}
@@ -116,16 +121,21 @@ def main():
             runs[name].append(time_steps(s, args.steps))
     same, mean_check, states = True, {}, {}
     for prefix in ("c4/one_series", "c4/series", "runs/series"):
-        a, b = results[prefix + "/mean"], results[prefix + "/state_i64"]
-        for j, name in enumerate(a.names):
-            k = b.names.index(name)
-            bits = bool((a.values[j] == b.values[k]).all() and (a.validity[j] == b.validity[k]).all())
-            x, y = a.values[j].view(np.float64), b.values[k].view(np.float64)
-            rel = float(np.nanmax(np.abs(x - y) / np.maximum(np.abs(x), 1e-300))) if x.size else 0.0
-            mean_check["%s col %s" % (prefix, name[0])] = {"bit_identical": bits, "max_rel_diff": rel}
-            same &= bits or (rel <= 1e-12 and bool((a.validity[j] == b.validity[k]).all()))
+        a = results[prefix + "/mean"]
+        for variant in ("state_i64", "periods_i64"):
+            b = results[prefix + "/" + variant]
+            for j, name in enumerate(a.names):
+                k = b.names.index(name)
+                bits = bool((a.values[j] == b.values[k]).all() and (a.validity[j] == b.validity[k]).all())
+                x, y = a.values[j].view(np.float64), b.values[k].view(np.float64)
+                rel = float(np.nanmax(np.abs(x - y) / np.maximum(np.abs(x), 1e-300))) if x.size else 0.0
+                mean_check["%s/%s col %s" % (prefix, variant, name[0])] = {"bit_identical": bits, "max_rel_diff": rel}
+                same &= bits or (rel <= 1e-12 and bool((a.validity[j] == b.validity[k]).all()))
+        b, p = results[prefix + "/state_i64"], results[prefix + "/periods_i64"]
         n, _ = b.column(1, "state_entries")
-        states[prefix] = {"map_entries": int(n.sum()), "selected_rows": int(counters[prefix + "/state_i64"]["rows_in_range"])}
+        same &= bool((p.column(1, "state_entries")[0] == n).all())
+        states[prefix] = {"map_entries": int(n.sum()), "periods": int(p.period_csr[1][0][-1]),
+                          "selected_rows": int(counters[prefix + "/state_i64"]["rows_in_range"])}
     states["runs/series"]["state_runs"] = n_runs
     out = {"workload": bench.WORKLOADS["C4"].config(args.series)["workload"], "gpu": bench.gpu_identity(0),
            "run_set": {"series": args.run_series, "rows_per_series": args.run_rows, "mean_run_rows": 100},
